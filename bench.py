@@ -10,9 +10,9 @@ collective ("scaling": "weak"); the only collectives are the timing barrier and 
   value   captions/s with the step's inputs already resident in HBM (CUDA events, max over ranks)
   e2e     the same metric through the public model(...) call with HOST (pinned) inputs: H2D copy of the features and the
           D2H read of the caption ids are inside the timed region, every step
-  roofline the dominant kernel (the persistent tcgen05 GEMM: CTA-pair kernel for the LSTM-gate and logit call sites): algorithmic
-          FLOPs of all its launches / their CUDA-event time vs the measured bf16 tensor peak in MEASURED_PEAKS.json, the DRAM traffic
-          of the largest call site from the committed ncu capture, and the fraction of the 3-pass ceiling (DESIGN.md section 3)
+  roofline the dominant kernel (the persistent wgmma GEMM of every dense call site): algorithmic FLOPs of all its launches / their
+          CUDA-event time vs the bf16 tensor peak (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet figure), and the
+          fraction of the 3-pass ceiling (DESIGN.md section 3)
   cpu_baseline  the unmodified reference modules (oracle/_ref; "kind": "reference"), timed on this box's host cores on a bounded sample
   scst    the second half of BASELINE.json's metric in the SAME line: SCST samples/sec on configs[3] (AoANet, per-GPU batch 10 x 5
           samples, CIDEr-D reward, BPTT, NCCL gradient all-reduce, Adam), with per-rank times, the all-reduce time and its HBM roofline
@@ -20,6 +20,10 @@ collective ("scaling": "weak"); the only collectives are the timing barrier and 
 Other workloads (--workload): transformer_beam / aoa_beam (BASELINE configs[2] shape and AoANet decode), updown_scst / aoa_scst (SCST
 training step incl. H2D, the single NCCL gradient all-reduce and Adam; aoa_scst = BASELINE configs[3]).  The GPU arms build their
 seeded random-init model and features from imagecaptioning.pytorch_b200.synthetic; only cpu_reference_rate() / cpu_reference_scst_rate() touch oracle/.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB in all):
+decode workloads the caption ids and (a fixed, seeded sample of the rows of) the log-probabilities, SCST workloads the loss and a fixed,
+seeded sample of the parameters after the optimizer step.  Inputs and weights are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -49,6 +53,7 @@ def parse():
     p.add_argument('--mode', default='tc_f16x3', choices=['tc_f16x3', 'tc_f16x1', 'simt_fp32'])
     p.add_argument('--cpu-batch', type=int, default=32, help='images per CPU-baseline step (bounded sample)')
     p.add_argument('--no-cpu-baseline', action='store_true')
+    p.add_argument('--dump-outputs', default=None, metavar='DIR', help='write the outputs of the last timed step as DIR/<name>.npy')
     p.add_argument('--workload', default='updown_beam', choices=['updown_beam', 'transformer_beam', 'aoa_beam', 'updown_scst', 'aoa_scst', 'transformer_scst'],
                    help='updown_beam = BASELINE.json configs[1] (the headline); transformer_beam = configs[2] (use --batch 64); aoa_beam = AoANet decode')
     args = p.parse_args()
@@ -204,7 +209,34 @@ def _per_rank(ms, dev, world):
     return vals, max(vals)
 
 
-def bench_scst(args, rank, world, local_rank, dev, workload, batch):
+DUMP_BYTES = 64 * 10 ** 6
+
+
+def _seeded_sample(flat, budget_elems, seed=0):
+    """(values, indices) of a fixed, seeded sample of a 1-D tensor: all of it when it fits the budget."""
+    import numpy as np
+    import torch
+    n = flat.numel()
+    if n <= budget_elems:
+        return flat, None
+    idx = np.sort(np.random.default_rng(seed).choice(n, size=budget_elems, replace=False))
+    return flat[torch.from_numpy(idx).to(flat.device)], idx
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor / array; written as float64 (integers, small arrays) or float32, at most DUMP_BYTES in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, 'detach') else np.asarray(a)
+        a = a.astype(np.float64 if (a.dtype.kind in 'iub' or a.dtype == np.float64) else np.float32)
+        total += a.nbytes
+        assert total <= DUMP_BYTES, 'dump exceeds %d bytes' % DUMP_BYTES
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
+def bench_scst(args, rank, world, local_rank, dev, workload, batch, dump=False):
     """SCST samples/sec (the second half of BASELINE.json's metric): AoANet (configs[3]) or UpDown, per-GPU batch `batch` images,
     train_sample_n = 5, CIDEr-D reward, greedy baseline, BPTT, gradient all-reduce over NCCL (overlapped with the backward pass when the loss
     wrapper supports it), value clipping and Adam.  Every step starts from pinned HOST features (H2D inside the timed region) and ends with
@@ -275,12 +307,21 @@ def bench_scst(args, rank, world, local_rank, dev, workload, batch):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     step_ms = []
+    last_loss = None
     for i in range(args.steps):
         t_s = time.perf_counter()
-        step(args.warmup + i, timed=True)
+        last_loss = step(args.warmup + i, timed=True)
         step_ms.append((time.perf_counter() - t_s) * 1e3)
     e1.record()
     barrier()
+    if dump and args.dump_outputs and rank == 0:
+        import torch as _t
+        flat = _t.cat([p.detach().reshape(-1) for p in model.parameters()])
+        vals, idx = _seeded_sample(flat, 1 << 21)             # 8 MB of values + 16 MB of float64 indices
+        arrays = {'loss': [last_loss], 'params_sample': vals}
+        if idx is not None:
+            arrays['params_sample_index'] = idx
+        dump_outputs(args.dump_outputs, arrays)
     if os.environ.get('CAPB200_BENCH_STEP_TIMES'):
         print('rank %d per-step wall ms: %s' % (rank, ' '.join('%.1f' % v for v in step_ms)), file=sys.stderr, flush=True)
     sampler.stop_flag = True
@@ -291,7 +332,7 @@ def bench_scst(args, rank, world, local_rank, dev, workload, batch):
     else:
         allreduce_ms = statistics.mean(a.elapsed_time(b) for a, b in ar_events) if ar_events else 0.0
     peaks_path = os.path.join(REPO, 'MEASURED_PEAKS.json')
-    hbm = float(json.load(open(peaks_path))['hbm_gbs']) if os.path.exists(peaks_path) else 6650.0
+    hbm = float(json.load(open(peaks_path))['hbm_gbs']) if os.path.exists(peaks_path) else 3350.0     # H100 SXM data sheet
     step_s = ms / args.steps / 1e3
     # algorithmic HBM bytes of one step (SURVEY.md 8d, AoANet): the 110 MB of fp32 decoder weights are streamed once per time step by the
     # sampling forward and about twice by the backward (input gradients read W, weight gradients write dW): 3 x T x 110 MB = 6.6 GB
@@ -303,7 +344,7 @@ def bench_scst(args, rank, world, local_rank, dev, workload, batch):
            'launches': (model.launch_count - l0) // max(args.steps, 1), 'scaling': 'weak',
            'step_wall_ms': {'min': min(step_ms), 'median': statistics.median(step_ms), 'max': max(step_ms)},
            'config': {'workload': '%s SCST step (BASELINE configs[3]), per-GPU batch=%d images x %d samples, 36x2048 feats, seq_len=20, V=9487' % (fam_name, B, n),
-                      'numeric_mode': 'greedy baseline %s (tcgen05 kind::f16 x3); sampling, backward and weight gradients on 3xTF32 tensor-core GEMMs over the fp32 weights' % args.mode},
+                      'numeric_mode': 'greedy baseline %s (wgmma f16 x3); sampling, backward and weight gradients on 3xTF32 tensor-core GEMMs over the fp32 weights' % args.mode},
            'clocks': sampler.summary(),
            'roofline': None if alg_bytes is None else {'bound': 'hbm', 'bytes': alg_bytes, 'achieved': alg_bytes / step_s / 1e9, 'peak': hbm, 'unit': 'GB/s',
                                                        'frac': alg_bytes / step_s / 1e9 / hbm,
@@ -329,7 +370,7 @@ def main():
         # configured batch; rank 0 alone runs it.
         if rank != 0:
             return
-        steps = max(1, min(args.steps, 3))
+        steps = args.steps
         batch = args.batch if args.workload == 'updown_beam' else args.cpu_batch
         rate, dt, cores, kind = cpu_reference_rate(batch, args.beam, steps, 1)
         line = {'impl': 'reference', 'metric': 'captions/sec at beam=5 seq_len=20', 'value': rate, 'unit': 'captions/s', 'n_gpus': args.gpus,
@@ -346,12 +387,13 @@ def main():
         print(json.dumps(line))
         return
 
+    import numpy as np
     import torch
     import torch.distributed as dist
-    import __graft_entry__ as ge
-    if local_rank == 0:
-        ge.build()
+    import imagecaptioning.pytorch_b200 as b200pkg
+    b200pkg._lib.load()                     # built by __graft_entry__.build(); the benchmark writes nothing into the tree
     torch.cuda.set_device(local_rank)
+    torch.manual_seed(1234)                 # the sampling seeds of the SCST steps follow torch's generator
     try:        # bind this rank to the CPU cores next to its GPU (NUMA): the SCST step is ~1300 launches of host-side work per step
         if os.environ.get('CAPB200_BENCH_NO_AFFINITY'):
             raise RuntimeError('disabled')
@@ -366,7 +408,7 @@ def main():
     from imagecaptioning.pytorch_b200 import synthetic as syn      # seeded random-init weights / features: the GPU arm never touches oracle/
     dev = torch.device('cuda', local_rank)
     if args.workload in ('updown_scst', 'aoa_scst', 'transformer_scst'):
-        res = bench_scst(args, rank, world, local_rank, dev, args.workload, args.batch)
+        res = bench_scst(args, rank, world, local_rank, dev, args.workload, args.batch, dump=True)
         if rank == 0:
             line = dict(res, warmup=args.warmup, higher_is_better=True, vs_baseline=None, dtype='f32', data='synthetic', gpu_launches=res['launches'] * args.steps)
             print(json.dumps(line))
@@ -382,7 +424,7 @@ def main():
         model = syn.build_model('aoa', seed=1234, logit_scale=6.0, mode=args.mode, device=dev, heads=8, **dict(CFG, E=1024, H=1024, A=0))
     B, T = args.batch, CFG['T']
     opt = {'beam_size': args.beam, 'sample_n': 1}
-    n_rot = 3                                         # rotate input batches; per-step working set (features, weights, 1 GB slab) >> 126 MB L2
+    n_rot = 3                                         # rotate input batches; per-step working set (features, weights, 1 GB slab) >> 50 MB L2
     host = [syn.make_inputs(B, R, CFG['F_fc'], CFG['F_att'], seed=1234 + 17 * rank + i) for i in range(n_rot)]
     host = [(a.pin_memory(), b.pin_memory()) for a, b in host]
     devin = [(a.to(dev), b.to(dev)) for a, b in host]
@@ -442,18 +484,29 @@ def main():
         l0 = model.launch_count
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        out = None
         for i in range(steps):
-            fn(warmup + i)
+            out = fn(warmup + i)
         e1.record()
         barrier()
         sampler.stop_flag = True
         sampler.join()
         per_rank, mx = _per_rank(e0.elapsed_time(e1), dev, world)
-        return mx, sampler.summary(), model.launch_count - l0, per_rank
+        return mx, sampler.summary(), model.launch_count - l0, per_rank, out
 
-    ms, clocks, launches, per_rank = timed(step_resident, args.steps, max(3, args.warmup))
+    ms, clocks, launches, per_rank, last = timed(step_resident, args.steps, max(3, args.warmup))
+    if args.dump_outputs and rank == 0:
+        seq, lp = last
+        rows = lp.reshape(-1, lp.shape[-1])
+        per_row = rows.shape[1] * 4
+        keep = min(rows.shape[0], (DUMP_BYTES * 3 // 4) // per_row)          # 48 MB of log-prob rows
+        idx = None if keep >= rows.shape[0] else np.sort(np.random.default_rng(0).choice(rows.shape[0], size=keep, replace=False))
+        arrays = {'seq': seq, 'logprobs': rows if idx is None else rows[torch.from_numpy(idx).to(rows.device)]}
+        if idx is not None:
+            arrays['logprobs_row_index'] = idx
+        dump_outputs(args.dump_outputs, arrays)
     value = world * B * args.steps / (ms / 1e3)
-    ms_e2e, _, _, per_rank_e2e = timed(step_e2e, args.steps, max(3, args.warmup))
+    ms_e2e, _, _, per_rank_e2e, _ = timed(step_e2e, args.steps, max(3, args.warmup))
     pending.clear()
     e2e = world * B * args.steps / (ms_e2e / 1e3)
 
@@ -480,25 +533,18 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))['bf16_tflops_sustained']), 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)'
     else:
-        peak, peak_src = 1400.0, 'fallback 1.4 PFLOP/s sustained (of fallback)'
-    # The dominant kernel is the persistent tcgen05 GEMM (gemm_tc_kernel): every dense contraction of the step is a launch of it.
+        peak, peak_src = 989.0, 'H100 SXM data sheet: 989 TFLOP/s dense bf16 at 700 W (not reached on a power-limited card)'
+    # The dominant kernel is the persistent wgmma GEMM (gemm_tc_kernel): every dense contraction of the step is a launch of it.
     # achieved = algorithmic FLOPs (2*M*N*K of the contraction actually executed) of ALL its launches / their summed CUDA-event time;
     # the largest single call site (language-LSTM gates, M=B*beam, N=4000, K=3000) is listed beside it.
-    # DRAM bytes per launch of one of the three large call sites (the capture's own `kernel` field says which) from the committed
-    # `ncu --set full` capture, when present
-    traffic, traffic_src = None, None
-    tpath = os.path.join(REPO, 'profiles', 'roofline_traffic.json')
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj.get('dram_bytes_per_launch'), tj.get('source')
     all_ms = sum(v[0] for v in prof.values())
     all_fl = sum(v[1] for v in prof.values())
     all_calls = sum(v[2] for v in prof.values())
     achieved = all_fl / (all_ms / 1e3) / 1e12 if all_ms > 0 else 0.0
     big_ms, big_fl, big_calls = prof['lang_lstm']
     passes = 3 if args.mode == 'tc_f16x3' else 1
-    roofline = {'bound': 'tensor', 'kernel': 'gemm_tc_pair_kernel<144,%d> / gemm_tc_kernel<64,..> (persistent tcgen05 GEMM, cta_group::2 pairs for the large call sites; all call sites of the step)' % passes,
-                'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak, 'traffic': traffic, 'traffic_source': traffic_src, 'traffic_kernel': tj.get('kernel') if traffic is not None else None, 'peak_source': peak_src,
+    roofline = {'bound': 'tensor', 'kernel': 'gemm_tc_kernel<128|64,%d> (persistent wgmma GEMM; all call sites of the step)' % passes,
+                'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak, 'peak_source': peak_src,
                 'mma_passes': passes,
                 'frac_of_pass_ceiling': achieved / (peak / passes),       # fp32-grade results cost 3 MMA passes per product
                 'launches_timed': all_calls, 'avg_launch_ms': all_ms / max(all_calls, 1),
@@ -527,7 +573,7 @@ def main():
             'ms_per_step': ms / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
             'dtype': 'f32 (fp32-grade: split-fp16 x3 tensor-core passes, fp32 accumulate)' if args.mode == 'tc_f16x3' else args.mode, 'data': 'synthetic',
             'config': {'workload': workload, 'numeric_mode': args.mode, 'global_batch': B * world, 'parallelism': 'dp%d (independent images, no collective)' % world,
-                       'l2': 'inputs rotated over %d batches; per-step working set ~1.3 GB >> 126 MB L2' % n_rot},
+                       'l2': 'inputs rotated over %d batches; per-step working set ~1.3 GB >> 50 MB L2' % n_rot},
             'clocks': clocks, 'per_rank_ms_per_step': [v / args.steps for v in per_rank],
             'e2e': {'value': e2e, 'unit': 'captions/s', 'h2d_bytes_per_step': B * (CFG['F_fc'] + R * CFG['F_att']) * 4, 'd2h_bytes_per_step': B * T * 8,
                     'ms_per_step': ms_e2e / args.steps, 'per_rank_ms_per_step': [v / args.steps for v in per_rank_e2e]},

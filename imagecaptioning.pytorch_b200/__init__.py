@@ -1,6 +1,6 @@
-"""imagecaptioning.pytorch_b200 -- B200-native caption decoding + SCST engine behind the reference's Python surfaces.
+"""imagecaptioning.pytorch_b200 -- H100 caption decoding + SCST engine behind the reference's Python surfaces.
 
-Only what the hot path needs lives here: ``csrc/`` (hand-written sm_100a kernels + the C ABI of include/capb200.h) and the
+Only what the hot path needs lives here: ``csrc/`` (hand-written sm_90a kernels + the C ABI of include/capb200.h) and the
 host-side mirrors of the reference interfaces (``models``, ``loss_wrapper``, ``rewards``, ``eval_utils``) plus the data-parallel plumbing
 (``parallel``, ``grad_sync``).  See DESIGN.md.
 """

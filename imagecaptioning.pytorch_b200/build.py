@@ -1,8 +1,8 @@
-"""Builds libcapb200.so (the C-ABI shared library, include/capb200.h) in-tree with nvcc for sm_100a.
+"""Builds libcapb200.so (the C-ABI shared library, include/capb200.h) in-tree with nvcc for sm_90a (H100).
 
     python imagecaptioning.pytorch_b200/build.py [--force]
 
-nvcc cross-compiles without a GPU; the resulting .so is git-ignored but travels with the repo snapshot to the GPU box.
+nvcc cross-compiles without a GPU; the resulting .so and the object files are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(PKG, 'build')
 LIB = os.path.join(PKG, 'libcapb200.so')
 SOURCES = ['gemm_tc.cu', 'gemm_simt.cu', 'pointwise.cu', 'vocab.cu', 'beam.cu', 'reward.cu', 'transformer.cu', 'gemm_generic.cu', 'gemm_tf32.cu', 'scst_kernels.cu', 'aoa_train_kernels.cu', 'tfm_train_kernels.cu', 'optim.cu', 'engine.cu', 'tfm_engine.cu', 'aoa_engine.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
 
 
 def _nvcc() -> str:
@@ -55,7 +55,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
         results = list(ex.map(compile_one, SOURCES))
     objs = [o for o, _ in results]
     if force or any(c for _, c in results) or _stale(LIB, objs):
-        cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+        cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

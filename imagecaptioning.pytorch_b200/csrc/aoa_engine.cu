@@ -6,7 +6,7 @@
 //   AoA_Decoder_Core :163-186  att_lstm(cat[xt, mean + ctx_prev]) -> LayerNorm(h) -> Linear -> 8-head dot attention over the image's
 //                              K | V -> GLU(Linear(cat[att, h_att])) = the new context vector, which is also the output and is
 //                              carried in state[0][1]; state[1][1] is never touched
-// B200 specifics: the mean-feature term of the LSTM gates is contracted once per image (row bias), the word term comes from the
+// Engine specifics: the mean-feature term of the LSTM gates is contracted once per image (row bias), the word term comes from the
 // per-token gate table, the LSTM cell is applied in the GEMM epilogue (tensor-core modes), K | V are indexed per image.
 #include <vector>
 

@@ -164,7 +164,7 @@ __global__ void glu_backward_fused_kernel(int rows, int H, const float* __restri
 //   queries [q_lo, q_hi) of every sequence; keys [0, n_keys) (causal: key r is visible to query qi iff r <= qi)
 //   key_mask [b, ld_mask] (0 = masked) or nullptr;  dropout element index = ((b*heads + head)*idx_L + qi)*idx_L + r
 // Grid (sequences, heads, query chunks): the chunks split the query range (forward) or the output elements (backward) so that a
-// 10-image batch still fills the machine (80 CTAs of 148 SMs took 65-72 us per launch, profiles/r02c_scst_table_aoa.txt).
+// 10-image batch still fills the machine (80 CTAs, one per (sequence, head), leave most SMs idle and make every launch long).
 struct SeqAttn {
     int n_keys, dk, heads, q_lo, q_hi, causal, idx_L;
     long b_stride, p_stride, ld;
@@ -488,7 +488,7 @@ __global__ void cat_dropout_kernel(int rows, int c1, int c2, const float* __rest
 
 int blocks_for(long n) {
     long b = (n + 255) / 256;
-    return (int)(b < 1 ? 1 : (b > 148 * 16 ? 148 * 16 : b));
+    return (int)(b < 1 ? 1 : (b > sm_count() * 16 ? sm_count() * 16 : b));
 }
 
 }  // namespace
@@ -545,7 +545,7 @@ int seq_attn_backward_launch(int seqs, int n_keys, int heads, int dk, int causal
     a.ld = ld; a.scale = 1.0f / sqrtf((float)dk); a.p_drop = p; a.seed = seed; a.site = (uint32_t)site; a.key_mask = key_mask; a.ld_mask = ld_mask;
     // every chunk CTA rebuilds P and dS (half of the kernel's work) and owns a whole SM (up to 150 KB of shared memory): chunks only help while
     // the grid stays within one wave (measured: 4 chunks at 80 (image, head) pairs = 320 CTAs took 108 us, 1 chunk 72 us)
-    int z = 148 / (seqs * heads);
+    int z = sm_count() / (seqs * heads);
     z = z < 1 ? 1 : (z > 4 ? 4 : z);
     seq_attn_backward_kernel<<<dim3(seqs, heads, z), 256, smem, st>>>(a, q, k, v, d_out, ld_do, dq, dk_, dv, ld_d);
     LAUNCH_OK();

@@ -3,8 +3,8 @@
 // The rows are few (10 .. 1280) and every row-head pair is a chain of dependent global loads, so the kernel is built for loads in
 // flight rather than for arithmetic: scores -- each warp takes chunks of eight regions and issues all of a chunk's key loads (lanes
 // across the head's dk columns: coalesced 128-byte segments) before the first warp reduction; softmax -- warp 0; weighted sum --
-// thread c owns column c and walks the regions twelve independent value loads at a time.  The first version (one warp per pair,
-// one dependent load per step) took 50-60 us per launch at 50 rows x 8 heads; see profiles/r02b_scst_table_aoa.txt.
+// thread c owns column c and walks the regions twelve independent value loads at a time (one warp per pair with one dependent load
+// per step was latency-bound).
 #pragma once
 #include <cuda_runtime.h>
 

@@ -289,7 +289,7 @@ int beam_edit_launch(int rows, int k_in, int beam, int t, const DecodeEdits& ed,
 int scale_rows_launch(float* x, long ld, int rows, int cols, float factor, cudaStream_t stream) {
     if (rows <= 0 || cols <= 0) return 0;
     long blocks = ((long)rows * cols + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     scale_rows_kernel<<<(int)blocks, 256, 0, stream>>>(x, ld, rows, cols, factor);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;

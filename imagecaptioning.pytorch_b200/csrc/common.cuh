@@ -42,13 +42,26 @@ inline bool first_use_on_device(std::atomic<unsigned long long>& mask) {
     return (mask.fetch_or(bit) & bit) == 0;
 }
 
+// Streaming multiprocessors of the current device (132 on an H100 SXM): persistent and grid-stride grids are sized from it.
+inline int sm_count() {
+    static std::atomic<int> cache[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev > 63) dev = 0;
+    int n = cache[dev].load();
+    if (n == 0) {
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 132;
+        cache[dev].store(n);
+    }
+    return n;
+}
+
 // ---- split-fp16 representation of an fp32 value: x ~= hi + lo, |x - hi - lo| <= 2^-22 |x| + 2^-25
 __device__ __forceinline__ void split_f32(float x, __half& hi, __half& lo) {
     hi = __float2half_rn(x);
     lo = __float2half_rn(x - __half2float(hi));
 }
 
-// ---- GEMM problem description shared by the SIMT and the tcgen05 back ends ------------------------
+// ---- GEMM problem description shared by the SIMT and the wgmma back ends --------------------------
 // C[M,N] = sum_s A_s[M,K_s] * W_s[N,K_s]^T  (+ bias[N]) (+ row_bias[row / rows_per_group, N]) ; optional ReLU.
 // Each K-segment has its own activation and weight views so concatenated LSTM inputs are never materialised
 // (the reference builds torch.cat([prev_h, fc_feats, xt]) every step, AttModel.py:626).
@@ -58,7 +71,7 @@ struct GemmSeg {
     long lda = 0;
     const float* W = nullptr;      // fp32 weights [N, K], row pitch ldw       (SIMT path)
     long ldw = 0;
-    const __half* A_hi = nullptr;  // split planes of A, pitch lda_h (multiple of 8 elements)   (tcgen05 path)
+    const __half* A_hi = nullptr;  // split planes of A, pitch lda_h (multiple of 8 elements)   (wgmma path)
     const __half* A_lo = nullptr;
     long lda_h = 0;
     const __half* W_hi = nullptr;  // split planes of W, pitch ldw_h
@@ -96,7 +109,7 @@ struct GemmEpilogue {
     __half* h_hi = nullptr;
     __half* h_lo = nullptr;
     long ld_h = 0;
-    unsigned long long* trace = nullptr;    // optional phase time stamps of the pair kernel ([CTAs][16] %globaltimer values), tools/gemm_trace.py
+    unsigned long long* trace = nullptr;    // optional phase time stamps of the wgmma kernel ([CTAs][16] %globaltimer values), tools/gemm_trace.py
 };
 
 // SFU-based transcendental forms (ex2.approx + fast reciprocal): absolute error < 3e-7 on outputs in [-1, 1].
@@ -128,13 +141,13 @@ struct GemmProblem {
 
 enum NumericMode : int {
     kModeSimtFp32 = 0,   // plain fp32 FFMA on CUDA cores (exact reference arithmetic up to summation order)
-    kModeTcF16x3 = 1,    // tcgen05 kind::f16, split-fp16 operands, 3 MMA passes (hi*hi + hi*lo + lo*hi), fp32 accumulate
-    kModeTcF16x1 = 2,    // tcgen05 kind::f16, hi plane only (throughput mode; NOT parity grade)
+    kModeTcF16x3 = 1,    // wgmma f16, split-fp16 operands, 3 MMA passes (hi*hi + hi*lo + lo*hi), fp32 accumulate
+    kModeTcF16x1 = 2,    // wgmma f16, hi plane only (throughput mode; NOT parity grade)
 };
 
 int gemm_simt_launch(const GemmProblem& p, cudaStream_t stream);
 
-// tcgen05 path: a plan owns the encoded TMA tensor maps; build once per buffer set, launch many times.
+// wgmma path: a plan owns the encoded TMA tensor maps; build once per buffer set, launch many times.
 struct GemmTcPlan;
 GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes);   // nullptr on failure (see last_error)
 void gemm_tc_plan_destroy(GemmTcPlan* plan);

@@ -776,7 +776,7 @@ int capb200_linear(const float* x, long ldx, const float* w, long ldw, const flo
         return rc;
     }
     if (mode == CAPB200_MODE_TF32X3_TC || mode == CAPB200_MODE_TF32X3_TC_DGRAD || mode == CAPB200_MODE_TF32X3_TC_WGRAD) {
-        // the training steps' tcgen05 kind::tf32 kernel (gemm_tf32.cu) through the same helper the engines use:
+        // the training steps' wgmma tf32 kernel (gemm_tf32.cu) through the same helper the engines use:
         //   TF32X3_TC        y[M,N]  = x[M,K] w[N,K]^T + b                         (forward)
         //   TF32X3_TC_DGRAD  y[M,N]  = x[M,K] w'[K,N]       with w' passed as `w`  (input gradient: W stored [out = K, in = N], cached transpose)
         //   TF32X3_TC_WGRAD  y[M,N]  = x'[K,M]^T w'[K,N]    with x', w' row-major   (weight gradient: dY = x', X = w', transposed per call)
@@ -788,7 +788,7 @@ int capb200_linear(const float* x, long ldx, const float* w, long ldw, const flo
         if (mode == CAPB200_MODE_TF32X3_TC) rc = sk.lin(x, ldx, w, ldw, b, y, ldy, M, N, K, 0);
         else if (mode == CAPB200_MODE_TF32X3_TC_DGRAD) rc = sk.dgrad(M, N, K, x, ldx, w, ldw, y, ldy, 0);
         else rc = sk.wgrad(M, N, K, x, ldx, w, ldw, y, ldy, 0);
-        if (tf32_context_launches(ctx) == 0 && !rc) { set_error("capb200_linear: the operands are not TMA-compatible, the tcgen05 tf32 kernel did not run"); rc = 1; }
+        if (tf32_context_launches(ctx) == 0 && !rc) { set_error("capb200_linear: the operands are not TMA-compatible, the wgmma tf32 kernel did not run"); rc = 1; }
         cudaStreamSynchronize(st);
         tf32_context_destroy(ctx);
         return rc;
@@ -816,7 +816,7 @@ int capb200_bench_linear(const float* x, const float* w, const float* b, float* 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CAPB_REQUIRE(x && w && y && ms_per_launch && M > 0 && N > 0 && K > 0 && iters > 0, "bad argument");
     if (mode == CAPB200_MODE_TF32X3_TC || mode == CAPB200_MODE_SKINNY_TF32X3) {
-        // the training GEMMs: tcgen05 kind::tf32 kernel (gemm_tf32.cu) or the mma.sync split-K kernel it replaced, timed back to back
+        // the training GEMMs: wgmma tf32 kernel (gemm_tf32.cu) or the mma.sync split-K kernel it replaced, timed back to back
         Tf32Context* ctx = mode == CAPB200_MODE_TF32X3_TC ? tf32_context_create() : nullptr;
         float* scratch = nullptr;
         const size_t cap = (size_t)4 << 20;
@@ -878,7 +878,7 @@ int capb200_bench_linear(const float* x, const float* w, const float* b, float* 
 }
 
 int capb200_gemm_trace(const float* x, const float* w, float* y, int M, int N, int K, unsigned long long* trace_host, int n_slots, void* stream) {
-    // one traced launch of the decode GEMM (3-pass tcgen05, CTA pairs) after three warm launches: trace_host[296][16] %globaltimer stamps
+    // one traced launch of the decode GEMM (3-pass wgmma) after three warm launches: trace_host[296][16] %globaltimer stamps
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CAPB_REQUIRE(x && w && y && trace_host && n_slots >= 296 * 16, "bad argument");
     GemmProblem g;
@@ -1084,7 +1084,7 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
     tf32_context_new_step(e->tf32);                                          // the weights may have changed since the last step
     const long tf32_l0 = tf32_context_launches(e->tf32);
-    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};              // tcgen05 3xTF32 GEMMs unless the engine is in simt_fp32 mode
+    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};              // wgmma 3xTF32 GEMMs unless the engine is in simt_fp32 mode
     sk.ctx = e->tf32;
 
     // ---- (2) train-mode prologue: fc_embed / att_embed with dropout, ctx2att, per-image gate term
@@ -1262,7 +1262,7 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     rc |= relu_dropout_backward_launch((long)B * H, tp.fc_e, tp.d_fc_e, tp.dpre_fc, keep_scale, st);
     rc |= sk.wgrad(H, Ff, B, tp.dpre_fc, H, fc, Ff, G.fc_embed_w, Ff, 0);
     rc |= colsum_launch(B, H, tp.dpre_fc, H, G.fc_embed_b, 0, st);
-    e->launches += 30 + (tf32_context_launches(e->tf32) - tf32_l0);     // + transposes of the tcgen05 path
+    e->launches += 30 + (tf32_context_launches(e->tf32) - tf32_l0);     // + transposes of the wgmma path
     if (!rc && record_group_event(e->grad_events[1], st)) return 1;
     return rc;
 }

@@ -515,7 +515,7 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
     }
     p.ksteps_total = ksteps;
     const int tiles = cdiv(N, GT) * cdiv(M, GT);
-    int ksplit = ((v2 ? 3 : 2) * 148 + tiles - 1) / tiles;          // CTAs resident per SM: 3 (v2, 74 KB of shared memory each) or 2
+    int ksplit = ((v2 ? 3 : 2) * sm_count() + tiles - 1) / tiles;          // CTAs resident per SM: 3 (v2, 74 KB of shared memory each) or 2
     if (ksplit > ksteps / 4) ksplit = ksteps / 4;                  // at least 4 K-steps per CTA
     if (ksplit < 1) ksplit = 1;
     while (ksplit > 1 && (size_t)ksplit * M * N > scratch_floats) --ksplit;
@@ -538,7 +538,7 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
     CAPB_CHECK_CUDA(cudaGetLastError());
     if (ksplit > 1) {
         long blocks = ((long)M * N + 255) / 256;
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > sm_count() * 8) blocks = sm_count() * 8;
         skinny_reduce_kernel<<<(int)blocks, 256, 0, st>>>(M, N, ksplit, scratch, C, ldc, bias, row_bias, ld_rb, p.rpg, accumulate);
         CAPB_CHECK_CUDA(cudaGetLastError());
     }

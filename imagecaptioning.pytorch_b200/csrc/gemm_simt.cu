@@ -1,6 +1,6 @@
 // fp32 CUDA-core GEMM (exact-arithmetic mode) and the fp32 -> split-fp16 plane conversion.
 //
-// Same contract as the tcgen05 kernel in gemm_tc.cu:  C[M,N] = sum_s A_s[M,K_s] * W_s[N,K_s]^T + bias (+row bias, ReLU)
+// Same contract as the wgmma kernel in gemm_tc.cu:  C[M,N] = sum_s A_s[M,K_s] * W_s[N,K_s]^T + bias (+row bias, ReLU)
 // with K-segments so torch.cat'ed LSTM inputs (AttModel.py:626,632) are never materialised.  This mode keeps the
 // reference's fp32 FFMA arithmetic (only the summation order differs from cuBLAS / MKL) and serves as the on-device
 // cross-check of the tensor-core path and as the path for shapes the TMA layout rules exclude.
@@ -209,7 +209,7 @@ int split_planes_interleave_launch(const float* x, long ldx, int H, int cols, __
     const long total = (long)4 * H * cols;
     if (total <= 0) return 0;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     split_planes_interleave_kernel<<<blocks, 256, 0, stream>>>(x, ldx, H, cols, hi, lo, ldh, range_flag_ptr());
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -244,13 +244,13 @@ int split_planes_launch(const float* x, long ldx, int rows, int cols, __half* hi
                      (reinterpret_cast<uintptr_t>(hi) & 7) == 0 && (reinterpret_cast<uintptr_t>(lo) & 7) == 0;
     if (vec) {
         int vb = (int)((total / 4 + 255) / 256);
-        if (vb > 148 * 16) vb = 148 * 16;
+        if (vb > sm_count() * 16) vb = sm_count() * 16;
         split_planes_vec4_kernel<<<vb, 256, 0, stream>>>(x, ldx, rows, cols / 4, hi, lo, ldh, range_flag_ptr());
         CAPB_CHECK_CUDA(cudaGetLastError());
         return 0;
     }
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     split_planes_kernel<<<blocks, 256, 0, stream>>>(x, ldx, rows, cols, hi, lo, ldh, range_flag_ptr());
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;

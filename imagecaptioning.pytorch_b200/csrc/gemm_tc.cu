@@ -1,22 +1,21 @@
-// tcgen05 GEMM for the caption-decode path:  C[M,N] = sum_s A_s * W_s^T (+bias, +per-group row bias, ReLU)
+// wgmma GEMM for the caption-decode path:  C[M,N] = sum_s A_s * W_s^T (+bias, +per-group row bias, ReLU)
 //
 // Replaces the cuBLAS SGEMMs behind nn.Linear / nn.LSTMCell on the hot path (reference call sites:
 // captioning/models/AttModel.py:119 att_embed, :172 logit, :628/:635 LSTMCell, :733 h2att).
 //
 // Numerics.  The reference computes in fp32; parity demands log-probs within 1e-4 and bit-exact greedy ids, which
 // single-pass fp16/bf16/tf32 tensor-core products do not deliver.  Operands are therefore kept in HBM as two fp16
-// planes (hi = fp16(x), lo = fp16(x - hi): same bytes as fp32) and every K-block issues three kind::f16 MMAs into
-// one fp32 TMEM accumulator:  hi*lo + lo*hi + hi*hi  (the lo*lo term, <= 2^-22 relative, is dropped).
+// planes (hi = fp16(x), lo = fp16(x - hi): same bytes as fp32) and every K-block issues three f16 wgmmas into
+// one fp32 register accumulator:  hi*lo + lo*hi + hi*hi  (the lo*lo term, <= 2^-22 relative, is dropped).
 // PASSES == 1 is the throughput mode (hi plane only) and is never used for parity claims.
 //
-// Structure (one 128 x BN output tile per CTA, 384 threads):
-//   warp 0      TMA producer: cp.async.bulk.tensor 2-D boxes [64 k x 128 rows] (128B swizzle) for A_hi, A_lo, W_hi,
-//               W_lo of the current K-block into a STAGES-deep shared-memory ring, mbarrier complete_tx signalling.
-//   warp 1      MMA issuer: one thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16) straight from
-//               shared-memory descriptors; tcgen05.commit releases ring slots and finally signals the epilogue.
-//   warp 2      allocates / frees the TMEM accumulator columns.
-//   warps 4..11 epilogue (two warps per TMEM lane quadrant, half of the columns each): tcgen05.ld, fused bias / row-bias / ReLU, fp32 store and
-//               (optionally) a split-fp16 copy so the next GEMM can consume the result without a conversion pass.
+// Structure (persistent: one 128 x BN output tile at a time per CTA, 384 threads = three warpgroups):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2-D boxes [64 k x rows] (128B swizzle) for A_hi, A_lo, W_hi,
+//                   W_lo of the current K-block into a STAGES-deep shared-memory ring, mbarrier complete_tx signalling.  It runs ahead
+//                   into the next tile while the consumers are in their epilogue.
+//   warpgroups 1,2  consumers: each owns 64 rows of the tile, issues wgmma.m64nBNk16 straight from shared-memory descriptors, releases
+//                   the ring slot once its wgmmas retired, and runs the fused epilogue (bias / row-bias / ReLU, fp32 store, optional
+//                   split-fp16 copy for the next GEMM, or the fused LSTM cell) from the register accumulator.
 // K-segments (up to 3 activation/weight pairs) are walked back to back so concatenated LSTM inputs are never built.
 #include <cstdlib>
 
@@ -29,11 +28,8 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;   // fp16 elements: one 128-byte swizzle row
-// Two epilogue warps per TMEM lane quadrant (warps 4..7 drain the lower half of the accumulator columns, warps 8..11 the upper half): the
-// epilogue of the LAST tile of a CTA cannot overlap a main loop, and the fused LSTM-cell epilogue is LSU-bound (one row per thread), so
-// doubling the threads that drain it halves the exposed tail of every GEMM launch.
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 128 + 32 * kEpiWarps;
+constexpr int kConsumers = 2;                  // consumer warpgroups, 64 accumulator rows each
+constexpr int kThreads = 128 * (1 + kConsumers);
 
 struct TcParams {
     CUtensorMap a_hi[kMaxSeg];
@@ -55,7 +51,7 @@ struct TcParams {
     int relu;
     const float* residual;
     long ld_res;
-    int tiles_m, tiles_n;       // CTA tiles, padded to whole clusters
+    int tiles_m, tiles_n;
     // fused LSTM epilogue (see GemmEpilogue)
     int lstm, H;
     const float* c_prev;
@@ -70,7 +66,7 @@ struct TcParams {
     __half* h_hi;
     __half* h_lo;
     long ld_h;
-    unsigned long long* trace;  // optional [CTAs][16] %globaltimer stamps of the pair kernel's phases (tools/gemm_trace.py); nullptr = off
+    unsigned long long* trace;  // optional [CTAs][16] %globaltimer stamps of the kernel's phases (tools/gemm_trace.py); nullptr = off
 };
 
 __device__ __forceinline__ unsigned long long gtimer() {
@@ -78,7 +74,7 @@ __device__ __forceinline__ unsigned long long gtimer() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
-// compiled in only for the TRACE = true instantiation of the pair kernel (tools/gemm_trace.py): the production kernels carry no trace branches
+// compiled in only for the TRACE = true instantiation (tools/gemm_trace.py): the production kernels carry no trace branches
 #define CAPB_TRACE(slot) do { if (TRACE && p.trace != nullptr) p.trace[(long)blockIdx.x * 16 + (slot)] = gtimer(); } while (0)
 
 template <int BN, int PASSES>
@@ -87,189 +83,123 @@ struct TcCfg {
     static constexpr uint32_t kABytes = BM * BK * 2;
     static constexpr uint32_t kWBytes = BN * BK * 2;
     static constexpr uint32_t kStageBytes = kPlanes * (kABytes + kWBytes);
-    static constexpr int kStages = (206 * 1024) / kStageBytes >= 8 ? 8 : (206 * 1024) / kStageBytes;
+    static constexpr int kStages = (200 * 1024) / kStageBytes >= 8 ? 8 : (200 * 1024) / kStageBytes;
     static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr uint32_t kTmemCols = 2 * BN <= 64 ? 64 : 2 * BN <= 128 ? 128 : 2 * BN <= 256 ? 256 : 512;   // two accumulators
-    static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "UMMA N for M=128 must be a multiple of 16 in [16, 256]");
+    static_assert(BN == 64 || BN == 128, "wgmma wrappers exist for N = 64 and 128");
     static_assert(kWBytes % 1024 == 0, "operand tiles must keep the 1024-byte swizzle-atom alignment");
     static_assert(kStages >= 2, "need at least a double buffer");
+    static_assert(kSmemBytes <= 227 * 1024, "shared memory of one H100 block");
 };
 
-// Drains one 128 x BN accumulator (TMEM columns tmem_acc .. tmem_acc + BN) into global memory: thread (q, lane) owns tile row q*32 + lane.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t tmem_acc, int m0, int n0, int q, int lane, bool vec4, bool vec2h, bool lstm_vec,
-                                              int c_begin, int c_end) {
-    const int row = m0 + q * 32 + lane;
-    const bool row_ok = row < p.M;
-    const float* rb = (p.row_bias != nullptr && row_ok) ? p.row_bias + (long)(row / p.rows_per_group) * p.ld_row_bias : nullptr;
-    const float* gb = (p.gather_bias != nullptr && row_ok) ? p.gather_bias + (long)p.gather_idx[row] * p.ld_gb : nullptr;
-    int src = row;
-    if (p.lstm && row_ok && p.src_row != nullptr) src = p.src_row[row];
-    // 128-bit operand loads need 16-byte aligned rows of every additive term
-    const bool vec_in = (p.bias == nullptr || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) &&
-                        (p.row_bias == nullptr || ((reinterpret_cast<uintptr_t>(p.row_bias) & 15) == 0 && (p.ld_row_bias & 3) == 0)) &&
-                        (p.gather_bias == nullptr || ((reinterpret_cast<uintptr_t>(p.gather_bias) & 15) == 0 && (p.ld_gb & 3) == 0)) &&
-                        (p.residual == nullptr || ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0 && (p.ld_res & 3) == 0));
-#pragma unroll 1
-    for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-        uint32_t r[16];
-        __syncwarp();   // tcgen05.ld is .sync.aligned: reconverge after the guarded stores of the previous chunk
-        ptx::tmem_ld_32x32b_x16(tmem_acc + (static_cast<uint32_t>(q * 32) << 16) + c0, r);
-        ptx::tmem_ld_wait();
-        const int col0 = n0 + c0;
-        if (!row_ok || col0 >= p.N) continue;
-        float v[16];
+__device__ __forceinline__ void wgmma_f16(float* acc, uint64_t da, uint64_t db, int scale_d) {
+    if (BN == 128) ptx::wgmma_f16_n128(acc, da, db, scale_d);
+    else ptx::wgmma_f16_n64(acc, da, db, scale_d);
+}
+
+// Bias / row bias / gathered bias / residual / ReLU of one accumulator element (row < M, col < N checked by the caller).
+__device__ __forceinline__ float epi_add(const TcParams& p, const float* rb, const float* gb, int row, int col, float x) {
+    if (p.bias != nullptr) x += __ldg(p.bias + col);
+    if (rb != nullptr) x += __ldg(rb + col);
+    if (gb != nullptr) x += __ldg(gb + col);
+    if (p.residual != nullptr) x += p.residual[(long)row * p.ld_res + col];
+    if (p.relu) x = fmaxf(x, 0.0f);
+    return x;
+}
+
+// Drains this warpgroup's 64 x BN accumulator.  Thread (w, lane) owns rows r0 = 16w + lane/4 and r0 + 8, columns 8j + 2*(lane%4) (+1).
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const TcParams& p, float* acc, int m0, int n0, int tid) {
+    const int warp = tid >> 5, lane = tid & 31;
+    int rows[2];
+    rows[0] = m0 + warp * 16 + (lane >> 2);
+    rows[1] = rows[0] + 8;
+    const float* rb[2];
+    const float* gb[2];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (col0 + 16 <= p.N && vec_in) {
-            // each lane reads a different row: 128-bit loads keep the number of distinct-line wavefronts per chunk at 4 per operand
-            // (scalar loads cost 16 and made this epilogue, not the MMA main loop, the critical path of the LSTM GEMMs)
+    for (int h = 0; h < 2; ++h) {
+        const bool ok = rows[h] < p.M;
+        rb[h] = (p.row_bias != nullptr && ok) ? p.row_bias + (long)(rows[h] / p.rows_per_group) * p.ld_row_bias : nullptr;
+        gb[h] = (p.gather_bias != nullptr && ok) ? p.gather_bias + (long)p.gather_idx[rows[h]] * p.ld_gb : nullptr;
+    }
 #pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-                if (p.bias != nullptr) { const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + j)); v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w; }
-                if (rb != nullptr) { const float4 b = __ldg(reinterpret_cast<const float4*>(rb + col0 + j)); v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w; }
-                if (gb != nullptr) { const float4 b = __ldg(reinterpret_cast<const float4*>(gb + col0 + j)); v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w; }
-                if (p.residual != nullptr) {
-                    const float4 b = *reinterpret_cast<const float4*>(p.residual + (long)row * p.ld_res + col0 + j);
-                    v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
-                }
-            }
-            if (p.relu) {
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * (lane & 3);
+        float v[4];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.0f);
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const int col = col0 + j;
-                float x = v[j];
-                if (col < p.N) {
-                    if (p.bias != nullptr) x += __ldg(p.bias + col);
-                    if (rb != nullptr) x += __ldg(rb + col);
-                    if (gb != nullptr) x += __ldg(gb + col);
-                    if (p.residual != nullptr) x += p.residual[(long)row * p.ld_res + col];
-                    if (p.relu) x = fmaxf(x, 0.0f);
-                }
-                v[j] = x;
-            }
+        for (int e = 0; e < 4; ++e) {
+            const int row = rows[e >> 1], c = col + (e & 1);
+            v[e] = (row < p.M && c < p.N) ? epi_add(p, rb[e >> 1], gb[e >> 1], row, c, acc[4 * j + e]) : 0.0f;
         }
         if (p.lstm) {
-            // columns col0 .. col0+15 = hidden units u0 .. u0+3, gates (i,f,g,o) interleaved
-            const int u0 = col0 >> 2;
-            float cn[4], hn[4], cpv[4] = {0.f, 0.f, 0.f, 0.f};
-            if (src >= 0 && p.c_prev != nullptr) {
-                if (lstm_vec && (p.ld_cprev & 3) == 0 && u0 + 4 <= p.H) {
-                    const float4 c4 = *reinterpret_cast<const float4*>(p.c_prev + (long)src * p.ld_cprev + u0);
-                    cpv[0] = c4.x; cpv[1] = c4.y; cpv[2] = c4.z; cpv[3] = c4.w;
-                } else {
-                    for (int u = 0; u < 4; ++u) if (u0 + u < p.H) cpv[u] = p.c_prev[(long)src * p.ld_cprev + u0 + u];
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const float cp = cpv[u];
-                cn[u] = fast_sigmoid(v[4 * u + 1]) * cp + fast_sigmoid(v[4 * u]) * fast_tanh(v[4 * u + 2]);
-                hn[u] = fast_sigmoid(v[4 * u + 3]) * fast_tanh(cn[u]);
-            }
-            if (lstm_vec && u0 + 4 <= p.H) {
-                *reinterpret_cast<float4*>(p.c_out + (long)row * p.ld_cout + u0) = make_float4(cn[0], cn[1], cn[2], cn[3]);
-                *reinterpret_cast<float4*>(p.h_f + (long)row * p.ld_h + u0) = make_float4(hn[0], hn[1], hn[2], hn[3]);
+            // gates (i,f,g,o) of hidden unit col/4 sit in lanes 2k (i,f) and 2k+1 (g,o): the even lane finishes the unit for row r0,
+            // the odd lane for row r0 + 8, each taking the two gates it lacks from its neighbour
+            const bool odd = lane & 1;
+            const float s0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 1);
+            const float s1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 1);
+            const float gi = odd ? s0 : v[0], gf = odd ? s1 : v[1], gg = odd ? v[2] : s0, go = odd ? v[3] : s1;
+            const int row = rows[odd ? 1 : 0];
+            const int unit = (col & ~3) >> 2;
+            if (row < p.M && unit < p.H) {
+                int src = row;
+                if (p.src_row != nullptr) src = p.src_row[row];
+                const float cp = (src >= 0 && p.c_prev != nullptr) ? p.c_prev[(long)src * p.ld_cprev + unit] : 0.0f;
+                const float cn = fast_sigmoid(gf) * cp + fast_sigmoid(gi) * fast_tanh(gg);
+                const float hn = fast_sigmoid(go) * fast_tanh(cn);
+                p.c_out[(long)row * p.ld_cout + unit] = cn;
+                p.h_f[(long)row * p.ld_h + unit] = hn;
                 if (p.h_hi != nullptr) {
-                    __align__(8) __half h[4];
-                    __align__(8) __half l[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) split_f32(hn[u], h[u], l[u]);
-                    *reinterpret_cast<uint2*>(p.h_hi + (long)row * p.ld_h + u0) = *reinterpret_cast<const uint2*>(h);
-                    *reinterpret_cast<uint2*>(p.h_lo + (long)row * p.ld_h + u0) = *reinterpret_cast<const uint2*>(l);
-                }
-            } else {
-                for (int u = 0; u < 4; ++u) {
-                    const int unit = u0 + u;
-                    if (unit < p.H) {
-                        p.c_out[(long)row * p.ld_cout + unit] = cn[u];
-                        p.h_f[(long)row * p.ld_h + unit] = hn[u];
-                        if (p.h_hi != nullptr) {
-                            __half h, l;
-                            split_f32(hn[u], h, l);
-                            p.h_hi[(long)row * p.ld_h + unit] = h;
-                            p.h_lo[(long)row * p.ld_h + unit] = l;
-                        }
-                    }
+                    __half hh, hl;
+                    split_f32(hn, hh, hl);
+                    p.h_hi[(long)row * p.ld_h + unit] = hh;
+                    p.h_lo[(long)row * p.ld_h + unit] = hl;
                 }
             }
             continue;
         }
-        const bool full = col0 + 16 <= p.N;
-        if (p.C != nullptr) {
-            float* dst = p.C + (long)row * p.ldc + col0;
-            if (full && vec4) {
 #pragma unroll
-                for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            } else {
-                for (int j = 0; j < 16; ++j) if (col0 + j < p.N) dst[j] = v[j];
+        for (int h = 0; h < 2; ++h) {
+            const int row = rows[h];
+            if (row >= p.M || col >= p.N) continue;
+            const float x0 = v[2 * h], x1 = v[2 * h + 1];
+            const bool pair = col + 1 < p.N;
+            if (p.C != nullptr) {
+                float* dst = p.C + (long)row * p.ldc + col;
+                if (pair && ((reinterpret_cast<uintptr_t>(dst) & 7) == 0)) *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
+                else { dst[0] = x0; if (pair) dst[1] = x1; }
             }
-        }
-        if (p.C_hi != nullptr) {
-            __half* dh = p.C_hi + (long)row * p.ldcs + col0;
-            __half* dl = p.C_lo + (long)row * p.ldcs + col0;
-            if (full && vec2h) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 8) {
-                    __align__(16) __half h[8];
-                    __align__(16) __half l[8];
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) split_f32(v[j + u], h[u], l[u]);
-                    *reinterpret_cast<uint4*>(dh + j) = *reinterpret_cast<const uint4*>(h);
-                    *reinterpret_cast<uint4*>(dl + j) = *reinterpret_cast<const uint4*>(l);
-                }
-            } else {
-                for (int j = 0; j < 16; ++j) {
-                    if (col0 + j < p.N) {
-                        __half h, l;
-                        split_f32(v[j], h, l);
-                        dh[j] = h;
-                        dl[j] = l;
-                    }
+            if (p.C_hi != nullptr) {
+                __half h0, l0, h1, l1;
+                split_f32(x0, h0, l0);
+                split_f32(x1, h1, l1);
+                __half* dh = p.C_hi + (long)row * p.ldcs + col;
+                __half* dl = p.C_lo + (long)row * p.ldcs + col;
+                if (pair && ((reinterpret_cast<uintptr_t>(dh) & 3) == 0) && ((reinterpret_cast<uintptr_t>(dl) & 3) == 0)) {
+                    *reinterpret_cast<__half2*>(dh) = __halves2half2(h0, h1);
+                    *reinterpret_cast<__half2*>(dl) = __halves2half2(l0, l1);
+                } else {
+                    dh[0] = h0; dl[0] = l0;
+                    if (pair) { dh[1] = h1; dl[1] = l1; }
                 }
             }
         }
     }
 }
 
-// CX x CY thread-block cluster: the CX CTAs of a cluster row share their A row block, the CY CTAs of a cluster column share
-// their W column block.  Each CTA fetches 1/CX of its A tile and 1/CY of its W tile and TMA-multicasts it to the peers, so
-// L2->SM operand traffic per CTA drops to A/CX + W/CY (the r01 ncu capture shows that traffic is the limiter of the
-// single-CTA kernel).  Stage release is the mirror image: tcgen05.commit multicasts the "slot free" arrival to every CTA
-// that writes into this CTA's slot.
-template <int BN, int PASSES, int CX, int CY>
+// Persistent schedule: gridDim.x = min(tiles, SMs); CTA b walks tiles b, b + gridDim.x, ... in m-fastest order so that concurrently
+// running CTAs share the same weight columns (the W tile comes from HBM once, then from L2).
+template <int BN, int PASSES, bool TRACE = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
     using Cfg = TcCfg<BN, PASSES>;
-    constexpr bool kCluster = (CX * CY) > 1;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + Cfg::kStages;
-    uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;        // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;              // [2]
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    // Persistent schedule: gridDim = (CX * P, CY); cluster c walks cluster-tiles c, c + P, ... in n-major order so that
-    // concurrently running clusters share the same weight columns (W tile comes from HBM once, then from L2).
-    const uint32_t cx = blockIdx.x % CX;
-    const uint32_t cy = blockIdx.y;
-    const int cluster_id = blockIdx.x / CX;
-    const int num_clusters = gridDim.x / CX;
-    const int cl_m = p.tiles_m / CY;
-    const int n_ctiles = (p.tiles_n / CX) * cl_m;
-    uint16_t mask_a = 0, mask_w = 0;          // CTAs that receive my A slice / my W slice (cluster rank = x + CX * y)
-    if (kCluster) {
-        for (int x = 0; x < CX; ++x) mask_a |= static_cast<uint16_t>(1u << (x + CX * cy));
-        for (int y = 0; y < CY; ++y) mask_w |= static_cast<uint16_t>(1u << (cx + CX * y));
-    }
+    const int wg = threadIdx.x >> 7;
+    const int n_tiles = p.tiles_m * p.tiles_n;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int s = 0; s < p.nseg; ++s) {
             ptx::prefetch_tmap(&p.a_hi[s]);
             ptx::prefetch_tmap(&p.w_hi[s]);
@@ -278,223 +208,22 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 ptx::prefetch_tmap(&p.w_lo[s]);
             }
         }
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < Cfg::kStages; ++i) {
             ptx::mbar_init(&full_bar[i], 1);
-            ptx::mbar_init(&empty_bar[i], CX + CY - 1);      // one release per CTA that writes into this slot
-        }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&tmem_full_bar[i], 1);
-            ptx::mbar_init(&tmem_empty_bar[i], 32 * kEpiWarps);   // every epilogue thread releases the accumulator
+            ptx::mbar_init(&empty_bar[i], kConsumers);        // one release per consumer warpgroup
         }
         ptx::fence_mbar_init();
     }
-    if (warp == 2) {
-        ptx::tmem_alloc(tmem_holder, Cfg::kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before_sync();
     __syncthreads();
-    if (kCluster) ptx::cluster_sync_all();                   // every CTA's barriers are initialised before any remote arrive
-    ptx::tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_holder;
+    if (threadIdx.x == 0) CAPB_TRACE(0);                       // set-up done
 
-    constexpr uint32_t kASlice = Cfg::kABytes / CX;           // bytes of my share of an A plane tile
-    constexpr uint32_t kWSlice = Cfg::kWBytes / CY;
-    constexpr int kARows = BM / CX, kWRows = BN / CY;
-    static_assert(kASlice % 1024 == 0 && kWSlice % 1024 == 0, "slices must stay swizzle-atom aligned");
-
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int ct = cluster_id; ct < n_ctiles; ct += num_clusters) {
-                const int m0 = ((ct % cl_m) * CY + cy) * BM;
-                const int n0 = ((ct / cl_m) * CX + cx) * BN;
-                for (int s = 0; s < p.nseg; ++s) {
-                    for (int kb = 0; kb < p.kblocks[s]; ++kb) {
-                        ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-                        uint8_t* st = smem + stage * Cfg::kStageBytes;
-                        uint8_t* a_hi = st + cx * kASlice;
-                        uint8_t* a_lo = st + Cfg::kABytes + cx * kASlice;
-                        uint8_t* w_hi = st + Cfg::kABytes * Cfg::kPlanes + cy * kWSlice;
-                        uint8_t* w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes + cy * kWSlice;
-                        ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-                        if (kCluster) {
-                            ptx::tma_load_2d_mcast(a_hi, &p.a_hi[s], &full_bar[stage], kb * BK, m0 + cx * kARows, mask_a);
-                            ptx::tma_load_2d_mcast(w_hi, &p.w_hi[s], &full_bar[stage], kb * BK, n0 + cy * kWRows, mask_w);
-                            if (PASSES == 3) {
-                                ptx::tma_load_2d_mcast(a_lo, &p.a_lo[s], &full_bar[stage], kb * BK, m0 + cx * kARows, mask_a);
-                                ptx::tma_load_2d_mcast(w_lo, &p.w_lo[s], &full_bar[stage], kb * BK, n0 + cy * kWRows, mask_w);
-                            }
-                        } else {
-                            ptx::tma_load_2d(a_hi, &p.a_hi[s], &full_bar[stage], kb * BK, m0);
-                            ptx::tma_load_2d(w_hi, &p.w_hi[s], &full_bar[stage], kb * BK, n0);
-                            if (PASSES == 3) {
-                                ptx::tma_load_2d(a_lo, &p.a_lo[s], &full_bar[stage], kb * BK, m0);
-                                ptx::tma_load_2d(w_lo, &p.w_lo[s], &full_bar[stage], kb * BK, n0);
-                            }
-                        }
-                        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = ptx::make_idesc_f16_f32(BM, BN);
-            const uint16_t release_mask = static_cast<uint16_t>(mask_a | mask_w);
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int ct = cluster_id; ct < n_ctiles; ct += num_clusters, ++it) {
-                const int buf = it & 1;
-                ptx::mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1);       // epilogue drained this accumulator
-                ptx::tc_fence_after_sync();
-                const uint32_t tmem_d = tmem_base + buf * BN;
-                uint32_t accumulate = 0;
-                for (int s = 0; s < p.nseg; ++s) {
-                    for (int kb = 0; kb < p.kblocks[s]; ++kb) {
-                        ptx::mbar_wait(&full_bar[stage], phase);
-                        ptx::tc_fence_after_sync();
-                        const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-                        const uint32_t a_hi = st;
-                        const uint32_t a_lo = st + Cfg::kABytes;                          // only valid when PASSES == 3
-                        const uint32_t w_hi = st + Cfg::kABytes * Cfg::kPlanes;
-                        const uint32_t w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;       // only valid when PASSES == 3
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            const uint32_t koff = k * 32;   // 16 fp16 = 32 bytes inside the 128-byte swizzle row
-                            if (PASSES == 3) {
-                                ptx::umma_f16(tmem_d, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_lo + koff), idesc, accumulate);
-                                ptx::umma_f16(tmem_d, ptx::make_smem_desc_sw128(a_lo + koff), ptx::make_smem_desc_sw128(w_hi + koff), idesc, 1);
-                                ptx::umma_f16(tmem_d, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_hi + koff), idesc, 1);
-                            } else {
-                                ptx::umma_f16(tmem_d, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_hi + koff), idesc, accumulate);
-                            }
-                            accumulate = 1;
-                        }
-                        if (kCluster) ptx::umma_commit_mcast(&empty_bar[stage], release_mask);
-                        else ptx::umma_commit(&empty_bar[stage]);
-                        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-                    }
-                }
-                ptx::umma_commit(&tmem_full_bar[buf]);
-            }
-        }
-    } else if (warp >= 4) {
-        const int q = warp & 3;                 // TMEM lane quadrant this warp may read
-        const bool vec4 = p.C != nullptr && (p.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 15) == 0;
-        const bool vec2h = p.C_hi != nullptr && (p.ldcs & 7) == 0 && (reinterpret_cast<uintptr_t>(p.C_hi) & 15) == 0 &&
-                           (reinterpret_cast<uintptr_t>(p.C_lo) & 15) == 0;
-        const bool lstm_vec = p.lstm && (p.ld_cout & 3) == 0 && (p.ld_h & 3) == 0;
-        int it = 0;
-        for (int ct = cluster_id; ct < n_ctiles; ct += num_clusters, ++it) {
-            const int buf = it & 1;
-            const int m0 = ((ct % cl_m) * CY + cy) * BM;
-            const int n0 = ((ct / cl_m) * CX + cx) * BN;
-            ptx::mbar_wait(&tmem_full_bar[buf], (it >> 1) & 1);
-            ptx::tc_fence_after_sync();
-            // column split between the two warps of a lane quadrant, in 16-column chunks
-            constexpr int kChunks = BN / 16, kLow = (kChunks + 1) / 2;
-            const int grp = (warp - 4) >> 2;
-            const int c_begin = (kEpiWarps == 8 && grp == 1) ? kLow * 16 : 0;
-            const int c_end = (kEpiWarps == 8 && grp == 0) ? kLow * 16 : BN;
-            epilogue_tile<BN>(p, tmem_base + buf * BN, m0, n0, q, lane, vec4, vec2h, lstm_vec, c_begin, c_end);
-            __syncwarp();
-            ptx::tc_fence_before_sync();
-            ptx::mbar_arrive(&tmem_empty_bar[buf]);            // accumulator drained: the MMA warp may reuse it
-        }
-    }
-    ptx::tc_fence_before_sync();
-    __syncthreads();
-    if (kCluster) ptx::cluster_sync_all();                   // no CTA leaves while a peer may still write its slots / barriers
-    ptx::tc_fence_after_sync();
-    if (warp == 2) ptx::tmem_dealloc(tmem_base, Cfg::kTmemCols);
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): the two CTAs of a 2 x 1 cluster sit on the two SMs of one TPC and execute ONE
-// M = 256, N = BN MMA per instruction.  Each CTA stages its own 128 A rows and only HALF of the W tile (BN/2 rows), so the
-// operand bytes a CTA must pull through L2 -> shared memory per K-block drop from (128 + BN) to (128 + BN/2) rows, the stage
-// shrinks (one more pipeline stage fits) and the shared-memory read traffic of the MMA halves.  Both CTAs run a TMA producer
-// (complete_tx lands on the leader's "full" barrier) and an epilogue over their own 128 accumulator rows; only the leader
-// (cluster rank 0) issues MMAs, and its tcgen05.commit multicasts the "slot free" / "accumulator ready" arrivals to both CTAs.
-// ---------------------------------------------------------------------------------------------------------------------
-template <int BN, int PASSES>
-struct TcPairCfg {
-    static constexpr int kPlanes = (PASSES == 3) ? 2 : 1;
-    static constexpr uint32_t kABytes = BM * BK * 2;
-    static constexpr uint32_t kWBytes = (BN / 2) * BK * 2;            // this CTA's half of the W tile
-    static constexpr uint32_t kStageBytes = kPlanes * (kABytes + kWBytes);
-    static constexpr int kStages = (206 * 1024) / kStageBytes >= 8 ? 8 : (206 * 1024) / kStageBytes;
-    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + 256;
-    static constexpr uint32_t kTmemCols = 2 * BN <= 64 ? 64 : 2 * BN <= 128 ? 128 : 2 * BN <= 256 ? 256 : 512;
-    static_assert(BN % 16 == 0 && BN >= 32 && BN <= 256, "UMMA N for M=256 must be a multiple of 16 in [32, 256]");
-    static_assert(kWBytes % 1024 == 0, "the half W tile must keep the 1024-byte swizzle-atom alignment");
-    static_assert(kStages >= 2, "need at least a double buffer");
-};
-
-template <int BN, int PASSES, bool TRACE = false>
-__global__ void __launch_bounds__(kThreads, 1) gemm_tc_pair_kernel(const __grid_constant__ TcParams p) {
-    using Cfg = TcPairCfg<BN, PASSES>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-    uint64_t* empty_bar = full_bar + Cfg::kStages;
-    uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;        // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;              // [2]  (the leader's copy collects both CTAs' epilogue threads)
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t rank = blockIdx.x & 1;                      // cluster (2, 1, 1): rank in the pair; 0 = leader
-    const int pair_id = blockIdx.x >> 1;
-    const int num_pairs = gridDim.x >> 1;
-    const int cl_m = p.tiles_m / 2;
-    const int n_ptiles = p.tiles_n * cl_m;
-
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < p.nseg; ++s) {
-            ptx::prefetch_tmap(&p.a_hi[s]);
-            ptx::prefetch_tmap(&p.w_hi[s]);
-            if (PASSES == 3) {
-                ptx::prefetch_tmap(&p.a_lo[s]);
-                ptx::prefetch_tmap(&p.w_lo[s]);
-            }
-        }
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < Cfg::kStages; ++i) {
-            ptx::mbar_init(&full_bar[i], 1);                   // the leader's expect_tx arrive (+ the bytes of both CTAs)
-            ptx::mbar_init(&empty_bar[i], 1);                  // one multicast commit per use
-        }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&tmem_full_bar[i], 1);
-            ptx::mbar_init(&tmem_empty_bar[i], 2 * 32 * kEpiWarps);   // the epilogue threads of both CTAs
-        }
-        ptx::fence_mbar_init();
-    }
-    if (warp == 2) {
-        ptx::tmem_alloc_pair(tmem_holder, Cfg::kTmemCols);
-        ptx::tmem_relinquish_pair();
-    }
-    ptx::tc_fence_before_sync();
-    __syncthreads();
-    ptx::cluster_sync_all();
-    ptx::tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_holder;
-    if (threadIdx.x == 0) CAPB_TRACE(0);                 // set-up done (barriers, TMEM, cluster sync)
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int pt = pair_id; pt < n_ptiles; pt += num_pairs) {
-                const int m0 = ((pt % cl_m) * 2 + rank) * BM;
-                const int n0 = (pt / cl_m) * BN + rank * (BN / 2);
+            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+                const int m0 = (t % p.tiles_m) * BM;
+                const int n0 = (t / p.tiles_m) * BN;
                 for (int s = 0; s < p.nseg; ++s) {
                     for (int kb = 0; kb < p.kblocks[s]; ++kb) {
                         ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -503,92 +232,67 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_pair_kernel(const __grid_
                         uint8_t* a_lo = st + Cfg::kABytes;
                         uint8_t* w_hi = st + Cfg::kABytes * Cfg::kPlanes;
                         uint8_t* w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;
-                        if (rank == 0) ptx::mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-                        ptx::tma_load_2d_pair(a_hi, &p.a_hi[s], &full_bar[stage], kb * BK, m0);
-                        ptx::tma_load_2d_pair(w_hi, &p.w_hi[s], &full_bar[stage], kb * BK, n0);
+                        ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+                        ptx::tma_load_2d(a_hi, &p.a_hi[s], &full_bar[stage], kb * BK, m0);
+                        ptx::tma_load_2d(w_hi, &p.w_hi[s], &full_bar[stage], kb * BK, n0);
                         if (PASSES == 3) {
-                            ptx::tma_load_2d_pair(a_lo, &p.a_lo[s], &full_bar[stage], kb * BK, m0);
-                            ptx::tma_load_2d_pair(w_lo, &p.w_lo[s], &full_bar[stage], kb * BK, n0);
+                            ptx::tma_load_2d(a_lo, &p.a_lo[s], &full_bar[stage], kb * BK, m0);
+                            ptx::tma_load_2d(w_lo, &p.w_lo[s], &full_bar[stage], kb * BK, n0);
                         }
                         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {
-            constexpr uint32_t idesc = ptx::make_idesc_f16_f32(2 * BM, BN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int pt = pair_id; pt < n_ptiles; pt += num_pairs, ++it) {
-                const int buf = it & 1;
-                ptx::mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1);       // both CTAs drained this accumulator
-                ptx::tc_fence_after_sync();
-                const uint32_t tmem_d = tmem_base + buf * BN;
-                uint32_t accumulate = 0;
-                for (int s = 0; s < p.nseg; ++s) {
-                    for (int kb = 0; kb < p.kblocks[s]; ++kb) {
-                        ptx::mbar_wait(&full_bar[stage], phase);
-                        ptx::tc_fence_after_sync();
-                        if (it == 0 && s == 0 && kb == 0) CAPB_TRACE(1);      // first operands landed
-                        const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-                        const uint32_t a_hi = st;
-                        const uint32_t a_lo = st + Cfg::kABytes;
-                        const uint32_t w_hi = st + Cfg::kABytes * Cfg::kPlanes;
-                        const uint32_t w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            const uint32_t koff = k * 32;
-                            if (PASSES == 3) {
-                                ptx::umma_f16_pair(tmem_d, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_lo + koff), idesc, accumulate);
-                                ptx::umma_f16_pair(tmem_d, ptx::make_smem_desc_sw128(a_lo + koff), ptx::make_smem_desc_sw128(w_hi + koff), idesc, 1);
-                                ptx::umma_f16_pair(tmem_d, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_hi + koff), idesc, 1);
-                            } else {
-                                ptx::umma_f16_pair(tmem_d, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_hi + koff), idesc, accumulate);
-                            }
-                            accumulate = 1;
-                        }
-                        ptx::umma_commit_pair(&empty_bar[stage]);
-                        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-                    }
-                }
-                ptx::umma_commit_pair(&tmem_full_bar[buf]);
-                if (it < 2) CAPB_TRACE(2 + it);                   // all MMAs of tile `it` issued
-            }
-        }
-    } else if (warp >= 4) {
-        const int q = warp & 3;
-        const bool vec4 = p.C != nullptr && (p.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 15) == 0;
-        const bool vec2h = p.C_hi != nullptr && (p.ldcs & 7) == 0 && (reinterpret_cast<uintptr_t>(p.C_hi) & 15) == 0 &&
-                           (reinterpret_cast<uintptr_t>(p.C_lo) & 15) == 0;
-        const bool lstm_vec = p.lstm && (p.ld_cout & 3) == 0 && (p.ld_h & 3) == 0;
+    } else {
+        const int cw = wg - 1;                                  // rows [64 cw, 64 cw + 64) of every tile
+        const int tid = threadIdx.x & 127;
+        const uint32_t a_off = cw * 64 * 128;                   // 64 rows of 128 bytes: a whole number of swizzle atoms
+        int stage = 0;
+        uint32_t phase = 0;
         int it = 0;
-        for (int pt = pair_id; pt < n_ptiles; pt += num_pairs, ++it) {
-            const int buf = it & 1;
-            const int m0 = ((pt % cl_m) * 2 + rank) * BM;
-            const int n0 = (pt / cl_m) * BN;
-            ptx::mbar_wait(&tmem_full_bar[buf], (it >> 1) & 1);
-            ptx::tc_fence_after_sync();
-            if (threadIdx.x == 128 && it < 2) CAPB_TRACE(4 + it);       // accumulator of tile `it` complete: epilogue starts
-            // column split between the two warps of a lane quadrant, in 16-column chunks
-            constexpr int kChunks = BN / 16, kLow = (kChunks + 1) / 2;
-            const int grp = (warp - 4) >> 2;
-            const int c_begin = (kEpiWarps == 8 && grp == 1) ? kLow * 16 : 0;
-            const int c_end = (kEpiWarps == 8 && grp == 0) ? kLow * 16 : BN;
-            epilogue_tile<BN>(p, tmem_base + buf * BN, m0, n0, q, lane, vec4, vec2h, lstm_vec, c_begin, c_end);
-            __syncwarp();
-            if (threadIdx.x == 128 && it < 2) CAPB_TRACE(6 + it);       // this warp's share of the epilogue of tile `it` done
-            ptx::tc_fence_before_sync();
-            ptx::mbar_arrive_leader(&tmem_empty_bar[buf]);
+        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
+            const int m0 = (t % p.tiles_m) * BM;
+            const int n0 = (t / p.tiles_m) * BN;
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+            for (int s = 0; s < p.nseg; ++s) {
+                for (int kb = 0; kb < p.kblocks[s]; ++kb) {
+                    ptx::mbar_wait(&full_bar[stage], phase);
+                    if (TRACE && it == 0 && s == 0 && kb == 0 && tid == 0 && cw == 0) CAPB_TRACE(1);    // first operands landed
+                    const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
+                    const uint32_t a_hi = st + a_off;
+                    const uint32_t a_lo = st + Cfg::kABytes + a_off;                  // only valid when PASSES == 3
+                    const uint32_t w_hi = st + Cfg::kABytes * Cfg::kPlanes;
+                    const uint32_t w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;       // only valid when PASSES == 3
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) ptx::reg_fence(acc[i]);
+                    ptx::wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < BK / 16; ++k) {
+                        const uint32_t koff = k * 32;   // 16 fp16 = 32 bytes inside the 128-byte swizzle row
+                        if (PASSES == 3) {
+                            wgmma_f16<BN>(acc, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_lo + koff), 1);
+                            wgmma_f16<BN>(acc, ptx::make_smem_desc_sw128(a_lo + koff), ptx::make_smem_desc_sw128(w_hi + koff), 1);
+                        }
+                        wgmma_f16<BN>(acc, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_hi + koff), 1);
+                    }
+                    ptx::wgmma_commit();
+                    ptx::wgmma_wait<0>();
+#pragma unroll
+                    for (int i = 0; i < BN / 2; ++i) ptx::reg_fence(acc[i]);
+                    if (tid == 0) ptx::mbar_arrive(&empty_bar[stage]);                // this warpgroup no longer reads the slot
+                    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+                }
+            }
+            if (TRACE && it < 2 && tid == 0 && cw == 0) CAPB_TRACE(2 + it);          // main loop of tile `it` done
+            epilogue_tile<BN>(p, acc, m0 + cw * 64, n0, tid);
+            if (TRACE && it < 2 && tid == 0 && cw == 0) CAPB_TRACE(6 + it);          // epilogue of tile `it` done
         }
     }
-    ptx::tc_fence_before_sync();
     __syncthreads();
-    ptx::cluster_sync_all();
-    ptx::tc_fence_after_sync();
-    if (threadIdx.x == 0) CAPB_TRACE(8);                 // every role of the pair is done
-    if (warp == 2) ptx::tmem_dealloc_pair(tmem_base, Cfg::kTmemCols);
+    if (threadIdx.x == 0) CAPB_TRACE(8);                       // every role is done
 }
 
 // ---- host side ------------------------------------------------------------------------------------
@@ -624,77 +328,21 @@ bool encode_plane(CUtensorMap* map, const __half* base, long rows, long K, long 
     return true;
 }
 
-template <int BN, int PASSES, int CX, int CY>
+template <int BN, int PASSES, bool TRACE = false>
 int launch_cfg(const TcParams& prm, cudaStream_t stream) {
     using Cfg = TcCfg<BN, PASSES>;
     static std::atomic<unsigned long long> attr_set{0};
     if (first_use_on_device(attr_set)) {
-        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, CX, CY>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    }
-    // grid padded to whole clusters; CTAs outside the matrix still run the pipeline (their TMA boxes are zero-filled) so
-    // that their cluster peers receive the multicast slices they wait for
-    TcParams prm2 = prm;
-    prm2.tiles_n = (int)round_up(cdiv(prm.N, BN), CX);
-    prm2.tiles_m = (int)round_up(cdiv(prm.M, BM), CY);
-    const int n_ctiles = (prm2.tiles_n / CX) * (prm2.tiles_m / CY);
-    const int slots = (CX * CY == 4) ? 33 : 148 / (CX * CY);          // clusters resident at once
-    const int P = n_ctiles < slots ? n_ctiles : slots;
-    dim3 grid(CX * P, CY);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CX;
-    attr[0].val.clusterDim.y = CY;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = (CX * CY > 1) ? 1 : 0;
-    CAPB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, PASSES, CX, CY>, prm2));
-    return 0;
-}
-
-
-template <int BN, int PASSES, bool TRACE = false>
-int launch_pair(const TcParams& prm, cudaStream_t stream) {
-    using Cfg = TcPairCfg<BN, PASSES>;
-    static std::atomic<unsigned long long> attr_set{0};
-    if (first_use_on_device(attr_set)) {
-        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_pair_kernel<BN, PASSES, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     }
     TcParams prm2 = prm;
-    prm2.tiles_n = (int)cdiv(prm.N, BN);
-    prm2.tiles_m = (int)round_up(cdiv(prm.M, BM), 2);
-    const int n_ptiles = prm2.tiles_n * (prm2.tiles_m / 2);
-    const int P = n_ptiles < 74 ? n_ptiles : 74;                       // one pair per TPC
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * P, 1);                                      // the pair must be adjacent in x (clusterDim.x = 2)
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    CAPB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_pair_kernel<BN, PASSES, TRACE>, prm2));
+    prm2.tiles_n = cdiv(prm.N, BN);
+    prm2.tiles_m = cdiv(prm.M, BM);
+    const int n_tiles = prm2.tiles_n * prm2.tiles_m;
+    const int sms = sm_count();
+    gemm_tc_kernel<BN, PASSES, TRACE><<<n_tiles < sms ? n_tiles : sms, kThreads, Cfg::kSmemBytes, stream>>>(prm2);
+    CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
-}
-
-// Round count of a tiling on 148 SMs: clusters are placed whole, so only floor(148 / cluster size) of them run at once.
-double tiling_cost(int M, int N, int bn, int cx, int cy) {
-    const long tiles_n = round_up(cdiv(N, bn), cx), tiles_m = round_up(cdiv(M, BM), cy);
-    const long clusters = (tiles_n / cx) * (tiles_m / cy);
-    const long slots = (cx * cy == 4) ? 33 : 148 / (cx * cy);      // 4-CTA clusters strand SMs in GPCs of 18 (33 x 4 = 132 usable)
-    const long rounds = (clusters + slots - 1) / slots;
-    // per-round time ~ max(MMA time, operand delivery): operand bytes per CTA per K-block scale with BM/cx + bn/cy
-    const double mma = bn;                                         // cycles per k16 MMA ~ BM * bn / 256
-    const double bytes = (double)BM / cx + (double)bn / cy;        // rows fetched per K-block
-    return rounds * (mma > 0.75 * bytes ? mma : 0.75 * bytes);
 }
 
 }  // namespace
@@ -703,8 +351,6 @@ struct GemmTcPlan {
     TcParams prm;
     int passes;
     int bn;
-    int cx, cy;       // cluster shape (multicast of A across cx CTAs, of W across cy CTAs)
-    int pair;         // 1: cta_group::2 kernel (cx = 1, cy = 2; W box = bn / 2 rows)
 };
 
 static void fill_epilogue(TcParams& t, const GemmEpilogue& e) {
@@ -742,48 +388,8 @@ GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes) {
     GemmTcPlan* plan = new GemmTcPlan();
     memset(&plan->prm, 0, sizeof(TcParams));
     plan->passes = passes;
-    plan->pair = 0;
-    // pick the tile width / cluster shape with the lowest modelled cost; tiny problems stay on the plain kernel
-    {
-        const int cand_bn[2] = {128, 144};
-        const int cand_c[4][2] = {{1, 1}, {2, 1}, {1, 2}, {2, 2}};
-        double best = 1e30;
-        plan->bn = 128;
-        plan->cx = plan->cy = 1;
-        for (int c = 0; c < 4; ++c) {
-            for (int b = 0; b < 2; ++b) {
-                const int cx = cand_c[c][0], cy = cand_c[c][1];
-                if (cdiv(p.M, BM) < cy || cdiv(p.N, cand_bn[b]) < cx) continue;
-                const double cost = tiling_cost(p.M, p.N, cand_bn[b], cx, cy);
-                if (cost < best) { best = cost; plan->bn = cand_bn[b]; plan->cx = cx; plan->cy = cy; }
-            }
-        }
-        // small problems (fewer 128-wide tiles than half the SMs) are latency-bound: halve the tile width to double the CTAs
-        if (cdiv(p.M, BM) * cdiv(p.N, 128) < 74 && p.N > 64) { plan->bn = 64; plan->cx = plan->cy = 1; }
-        else if (cdiv(p.M, BM) >= 2 && getenv("CAPB200_GEMM_NO_PAIR") == nullptr) {
-            // large problems: CTA pairs (cta_group::2, M = 256 per MMA) stage only half a W tile per CTA -- 26 % fewer operand bytes through
-            // L2 -> shared memory per FLOP and a 4-deep ring; pick the tile width with the fewest rounds over the 74 TPCs
-            const int pb[2] = {144, 128};
-            double pbest = 1e30;
-            for (int b = 0; b < 2; ++b) {
-                const long ptiles = cdiv(p.N, pb[b]) * cdiv(cdiv(p.M, BM), 2);
-                const double cost = (double)((ptiles + 73) / 74) * pb[b];
-                if (cost < pbest) { pbest = cost; plan->bn = pb[b]; }
-            }
-            plan->cx = 1; plan->cy = 2; plan->pair = 1;
-        }
-        const char* force = getenv("CAPB200_GEMM_TILING");      // "<BN>x<CX>x<CY>", e.g. "144x2x1" (debug / sweeps)
-        if (force != nullptr) {
-            int fb = 0, fx = 0, fy = 0;
-            if (sscanf(force, "%dx%dx%d", &fb, &fx, &fy) == 3 && (fb == 32 || fb == 64 || fb == 128 || fb == 144) && (fx == 1 || fx == 2 || (fx == 4 && fy == 1 && fb <= 64)) &&
-                (fy == 1 || fy == 2)) {
-                plan->bn = fb; plan->cx = fx; plan->cy = fy; plan->pair = 0;
-            }
-            if (sscanf(force, "pair%d", &fb) == 1 && (fb == 128 || fb == 144 || fb == 192 || fb == 256) && cdiv(p.M, BM) >= 2) {
-                plan->bn = fb; plan->cx = 1; plan->cy = 2; plan->pair = 1;
-            }
-        }
-    }
+    // problems with fewer 128-wide tiles than half the SMs are latency-bound: halve the tile width to double the CTAs
+    plan->bn = (cdiv(p.M, BM) * cdiv(p.N, 128) < sm_count() / 2 && p.N > 64) ? 64 : 128;
     TcParams& t = plan->prm;
     t.nseg = p.nseg;
     t.M = p.M;
@@ -792,13 +398,12 @@ GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes) {
     for (int s = 0; s < p.nseg; ++s) {
         const GemmSeg& g = p.seg[s];
         t.kblocks[s] = cdiv(g.K, BK);
-        const int a_box = BM / plan->cx, w_box = plan->bn / plan->cy;     // each CTA fetches its slice of the tile
-        bool ok = encode_plane(&t.a_hi[s], g.A_hi, p.M, g.K, g.lda_h, a_box, &err) &&
-                  encode_plane(&t.w_hi[s], g.W_hi, p.N, g.K, g.ldw_h, w_box, &err);
+        bool ok = encode_plane(&t.a_hi[s], g.A_hi, p.M, g.K, g.lda_h, BM, &err) &&
+                  encode_plane(&t.w_hi[s], g.W_hi, p.N, g.K, g.ldw_h, plan->bn, &err);
         if (ok && passes == 3) {
             if (g.A_lo == nullptr || g.W_lo == nullptr) { err = "lo planes missing for 3-pass mode"; ok = false; }
-            ok = ok && encode_plane(&t.a_lo[s], g.A_lo, p.M, g.K, g.lda_h, a_box, &err) &&
-                 encode_plane(&t.w_lo[s], g.W_lo, p.N, g.K, g.ldw_h, w_box, &err);
+            ok = ok && encode_plane(&t.a_lo[s], g.A_lo, p.M, g.K, g.lda_h, BM, &err) &&
+                 encode_plane(&t.w_lo[s], g.W_lo, p.N, g.K, g.ldw_h, plan->bn, &err);
         }
         if (!ok) { set_error("gemm_tc: " + err); delete plan; return nullptr; }
     }
@@ -820,31 +425,12 @@ int gemm_tc_plan_launch(GemmTcPlan* plan, const GemmEpilogue* epi_override, int 
         return 1;
     }
     if (prm.M <= 0 || prm.N <= 0) return 0;
-    if (plan->pair) {
-        switch (plan->bn) {
-            case 128: return plan->passes == 3 ? launch_pair<128, 3>(prm, stream) : launch_pair<128, 1>(prm, stream);
-            case 144:
-                if (prm.trace != nullptr && plan->passes == 3) return launch_pair<144, 3, true>(prm, stream);      // capb200_gemm_trace only
-                return plan->passes == 3 ? launch_pair<144, 3>(prm, stream) : launch_pair<144, 1>(prm, stream);
-            case 192: return plan->passes == 3 ? launch_pair<192, 3>(prm, stream) : launch_pair<192, 1>(prm, stream);
-            case 256: return plan->passes == 3 ? launch_pair<256, 3>(prm, stream) : launch_pair<256, 1>(prm, stream);
-        }
-        set_error("gemm_tc: no pair kernel instance for the planned tile width");
-        return 1;
+    if (prm.trace != nullptr) {                                  // capb200_gemm_trace only
+        if (plan->passes != 3) { set_error("gemm_tc: the traced kernel is the 3-pass one"); return 1; }
+        return plan->bn == 128 ? launch_cfg<128, 3, true>(prm, stream) : launch_cfg<64, 3, true>(prm, stream);
     }
-    const int key = plan->bn * 100 + plan->cx * 10 + plan->cy;
-#define CAPB_TC_CASE(BN_, CX_, CY_)                                                      \
-    case BN_ * 100 + CX_ * 10 + CY_:                                                     \
-        return plan->passes == 3 ? launch_cfg<BN_, 3, CX_, CY_>(prm, stream) : launch_cfg<BN_, 1, CX_, CY_>(prm, stream);
-    switch (key) {
-        CAPB_TC_CASE(32, 1, 1) CAPB_TC_CASE(32, 2, 1) CAPB_TC_CASE(32, 4, 1) CAPB_TC_CASE(64, 4, 1)
-        CAPB_TC_CASE(64, 1, 1) CAPB_TC_CASE(64, 2, 1) CAPB_TC_CASE(64, 1, 2) CAPB_TC_CASE(64, 2, 2)
-        CAPB_TC_CASE(128, 1, 1) CAPB_TC_CASE(128, 2, 1) CAPB_TC_CASE(128, 1, 2) CAPB_TC_CASE(128, 2, 2)
-        CAPB_TC_CASE(144, 1, 1) CAPB_TC_CASE(144, 2, 1) CAPB_TC_CASE(144, 1, 2) CAPB_TC_CASE(144, 2, 2)
-    }
-#undef CAPB_TC_CASE
-    set_error("gemm_tc: no kernel instance for the planned tiling");
-    return 1;
+    if (plan->bn == 128) return plan->passes == 3 ? launch_cfg<128, 3>(prm, stream) : launch_cfg<128, 1>(prm, stream);
+    return plan->passes == 3 ? launch_cfg<64, 3>(prm, stream) : launch_cfg<64, 1>(prm, stream);
 }
 
 }  // namespace capb200

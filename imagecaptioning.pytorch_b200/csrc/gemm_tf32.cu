@@ -1,4 +1,4 @@
-// tcgen05 kind::tf32 GEMM for the training steps (SCST / XE):  C[M,N] (+)= sum_s X_s[M,K_s] * W_s[N,K_s]^T (+ bias + row bias)
+// wgmma tf32 GEMM for the training steps (SCST / XE):  C[M,N] (+)= sum_s X_s[M,K_s] * W_s[N,K_s]^T (+ bias + row bias)
 //
 // Replaces the mma.sync 3xTF32 kernels of gemm_generic.cu on the hot path of LossWrapper's sc branch (reference call sites:
 // captioning/modules/loss_wrapper.py:56-73 -> every nn.Linear / nn.LSTMCell of AoAModel.py / AttModel.py in train mode, and the
@@ -8,21 +8,18 @@
 // ~1e-7, which fp16 planes would flush to zero, so the operands stay fp32 in HBM and are split INSIDE the kernel into TF32 pairs:
 //   hi = cvt.rna.tf32(x)  (exactly representable: the tensor core's own fp32 -> tf32 conversion, whatever its rounding, is the identity)
 //   lo = x - hi           (exact in fp32; the tensor core keeps its top 11 bits: relative error <= 2^-21 of x)
-// and every K-block issues three kind::tf32 MMAs into one fp32 TMEM accumulator: hi*lo + lo*hi + hi*hi (3xTF32, dropped lo*lo <= 2^-22).
+// and every K-block issues three tf32 wgmmas into one fp32 register accumulator: hi*lo + lo*hi + hi*hi (3xTF32, dropped lo*lo <= 2^-22).
 //
-// Structure (one 128 x BN accumulator tile per CTA, 384 threads, split-K across a thread-block cluster):
-//   warp 0      TMA producer: cp.async.bulk.tensor 2-D boxes of RAW fp32 [32 k x 128 rows] (A side) and [32 k x BN rows] (B side), 128B swizzle,
-//               into a STAGES-deep ring (mbarrier complete_tx).
-//   warps 4..11 converters: read the raw tiles from shared memory, write hi in place and lo next to it (element-wise, so the swizzle
-//               pattern is preserved), fence.proxy.async, arrive on the stage's "converted" barrier.  Eight warps (the same warps drain
-//               the accumulator, two per TMEM lane quadrant); going from four to eight converter warps did not change the per-call times
-//               (profiles/r02c_tf32_sweep_trunc.txt vs r02f_tf32_sweep.txt): at the skinny shapes a launch is bound by its fixed costs and
-//               the depth of its K chain, not by the conversion (profiles/r02k_gemm_full.md).
-//   warp 1      MMA issuer: one thread, 12 tcgen05.mma.kind::tf32 (M = 128, N = BN, K = 8) per K-block, tcgen05.commit releases the slot.
-//   warp 2      TMEM allocation.
-//   epilogue    warps 4..11 (two per TMEM lane quadrant) drain the accumulator into a shared-memory staging tile laid out like the OUTPUT (so global stores are
-//               coalesced); with split-K the CTAs of the cluster (cluster dim = ksplit <= 8, K-ranges side by side) then add their tiles
-//               through distributed shared memory in rank order (deterministic, no atomics, no second kernel) and each stores a slice.
+// Structure (one 128 x BN accumulator tile per CTA, 384 threads = three warpgroups, split-K across a thread-block cluster):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2-D boxes of RAW fp32 [32 k x 128 rows] (A side) and [32 k x BN rows]
+//                   (B side), 128B swizzle, into a STAGES-deep ring (mbarrier complete_tx).
+//   warpgroups 1,2  converters and MMA issuers: read the raw tiles from shared memory, write hi in place and lo next to it (element-wise,
+//                   so the swizzle pattern is preserved), fence.proxy.async, meet at a named barrier, then each issues the wgmmas of its
+//                   64 accumulator rows (m64nNk8) and releases the slot once they retired.
+//   epilogue        the consumers drain the register accumulators into a shared-memory staging tile laid out like the OUTPUT (so global
+//                   stores are coalesced); with split-K the CTAs of the cluster (cluster dim = ksplit <= 8, K-ranges side by side) then
+//                   add their tiles through distributed shared memory in rank order (deterministic, no atomics, no second kernel) and
+//                   each stores a slice.
 // Operand roles: the A side always supplies 128 accumulator rows, the B side BN columns.  Skinny problems (M <= 256 activation rows:
 // the 50-row sampling steps) run SWAPPED -- weights on the A side, activations on the B side -- so no tensor-core row is padding and
 // the weights are streamed exactly once; problems with many rows (refiner: B*R rows; batched-over-time gradients: T*N rows) run normally.
@@ -42,7 +39,8 @@ namespace {
 constexpr int TM = 128;          // accumulator rows per CTA (A-side rows)
 constexpr int TK = 32;           // fp32 elements per K-block: one 128-byte swizzle row
 constexpr int kMaxSegT = 3;
-constexpr int kConvThreads = 256;   // warps 4..11
+constexpr int kConvThreads = 256;   // warpgroups 1 and 2
+constexpr int kConsumersT = 2;
 constexpr int kThreadsT = 128 + kConvThreads;
 
 struct Tf32Params {
@@ -80,26 +78,22 @@ struct Tf32Cfg {
     static constexpr uint32_t kStaging = kStagingSwapped > kStagingNormal ? kStagingSwapped : kStagingNormal;
     static constexpr uint32_t kBody = kRingBytes > kStaging ? kRingBytes : kStaging;
     static constexpr uint32_t kSmemBytes = kBody + 1024 /*align*/ + 512 /*barriers*/;
-    static constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
-    static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "UMMA N for M = 128");
+    static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "wgmma wrappers exist for N = 32, 64, 128 (256 = two halves)");
     static_assert(kStages >= 2, "need a double buffer");
     static_assert(kBBytes % 1024 == 0, "tiles must keep the 1024-byte swizzle-atom alignment");
+    static_assert(kSmemBytes <= 227 * 1024, "shared memory of one H100 block");
 };
 
-__host__ __device__ constexpr uint32_t make_idesc_tf32(uint32_t M, uint32_t N) {
-    // c_format [4,6) = 1 (F32); a_format [7,10) = 2 (TF32); b_format [10,13) = 2 (TF32); both K-major; n_dim [17,23) = N>>3; m_dim [24,29) = M>>4
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+// acc[BN / 2] (+)= A[64 rows] * B[BN rows]^T for one k8 step; N = 256 runs as two N = 128 halves (B rows 128.. start 16 KB further)
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float* acc, uint32_t a, uint32_t b) {
+    const uint64_t da = ptx::make_smem_desc_sw128(a);
+    if (BN == 32) ptx::wgmma_tf32_n32(acc, da, ptx::make_smem_desc_sw128(b), 1);
+    else if (BN == 64) ptx::wgmma_tf32_n64(acc, da, ptx::make_smem_desc_sw128(b), 1);
+    else {
+#pragma unroll
+        for (int h = 0; h < BN / 128; ++h) ptx::wgmma_tf32_n128(acc + 64 * h, da, ptx::make_smem_desc_sw128(b + h * 128 * 128), 1);
+    }
 }
 
 __device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
@@ -112,6 +106,8 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr) {
     asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
     return v;
 }
+// the 256 converter / consumer threads only (the producer warpgroup never joins)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConvThreads) : "memory"); }
 
 __device__ __forceinline__ void split_keep_tf32(float x, float& hi, float& lo) {
     uint32_t h;
@@ -120,25 +116,15 @@ __device__ __forceinline__ void split_keep_tf32(float x, float& hi, float& lo) {
     lo = x - hi;
 }
 
-// TRUNC = true: the raw fp32 tile is left in place as the hi operand (the tensor core reads its top 19 bits, i.e. truncates) and only
-// lo = x - trunc(x) is written: one third less shared-memory traffic in the converter.  Valid because the tensor core's fp32 -> tf32
-// operand conversion IS a truncation on sm_100a: the fp64 accuracy tests (tests/test_gpu_ops.py, same 4e-6 bar) pass with it, and they
-// could not if the hardware rounded (hi would then differ from trunc(x) by up to 2^-11 |x|).  10-20 % faster on every training shape
-// (profiles/r02c_tf32_sweep*.txt), so it is the default; CAPB200_TF32_RNA=1 selects the round-to-nearest split above.
-__device__ __forceinline__ void split_trunc_tf32(float x, float& lo) { lo = x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
-
-template <int BN, bool TRUNC>
+template <int BN>
 __global__ void __launch_bounds__(kThreadsT, 1) gemm_tf32x3_kernel(const __grid_constant__ Tf32Params p) {
     using Cfg = Tf32Cfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBody);
-    uint64_t* conv_bar = full_bar + Cfg::kStages;
-    uint64_t* empty_bar = conv_bar + Cfg::kStages;
-    uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+    uint64_t* empty_bar = full_bar + Cfg::kStages;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int ksplit = gridDim.x;                       // cluster = (ksplit, 1, 1): blockIdx.x is the K-rank
     const int krank = blockIdx.x;
     const int a_row0 = blockIdx.y * TM;                 // first A-side row of this tile
@@ -147,26 +133,15 @@ __global__ void __launch_bounds__(kThreadsT, 1) gemm_tf32x3_kernel(const __grid_
     const int ks1 = (int)(((long)p.ksteps_total * (krank + 1)) / ksplit);
     const int nk = ks1 - ks0;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int s = 0; s < p.nseg; ++s) { ptx::prefetch_tmap(&p.a_map[s]); ptx::prefetch_tmap(&p.b_map[s]); }
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < Cfg::kStages; ++i) {
             ptx::mbar_init(&full_bar[i], 1);
-            ptx::mbar_init(&conv_bar[i], kConvThreads);
-            ptx::mbar_init(&empty_bar[i], 1);
+            ptx::mbar_init(&empty_bar[i], kConsumersT);
         }
-        ptx::mbar_init(tmem_full_bar, 1);
         ptx::fence_mbar_init();
     }
-    if (warp == 2) {
-        ptx::tmem_alloc(tmem_holder, Cfg::kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before_sync();
     __syncthreads();
-    ptx::tc_fence_after_sync();
-    const uint32_t tmem_acc = *tmem_holder;
 
     // flattened K-step -> (segment, k-block inside the segment)
     auto locate = [&](int ks, int& seg, int& kb) {
@@ -176,8 +151,8 @@ __global__ void __launch_bounds__(kThreadsT, 1) gemm_tf32x3_kernel(const __grid_
         kb = ks - first;
     };
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int it = 0; it < nk; ++it) {
@@ -191,39 +166,19 @@ __global__ void __launch_bounds__(kThreadsT, 1) gemm_tf32x3_kernel(const __grid_
                 if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc_tf32(TM, BN);
-            int stage = 0;
-            uint32_t phase = 0;
-            uint32_t accumulate = 0;
-            for (int it = 0; it < nk; ++it) {
-                ptx::mbar_wait(&conv_bar[stage], phase);
-                ptx::tc_fence_after_sync();
-                const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-                const uint32_t a_hi = st, a_lo = st + Cfg::kABytes;
-                const uint32_t b_hi = st + 2 * Cfg::kABytes, b_lo = b_hi + Cfg::kBBytes;
+    } else {
+        const int ct = threadIdx.x - 128;               // 0 .. 255 over both consumer warpgroups
+        const int cw = wg - 1;                          // accumulator rows [64 cw, 64 cw + 64) of the tile
+        const int tid = threadIdx.x & 127;
+        float acc[BN / 2];
 #pragma unroll
-                for (int k = 0; k < TK / 8; ++k) {
-                    const uint32_t koff = k * 32;          // 8 tf32 = 32 bytes inside the 128-byte swizzle row
-                    umma_tf32(tmem_acc, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(b_lo + koff), idesc, accumulate);
-                    umma_tf32(tmem_acc, ptx::make_smem_desc_sw128(a_lo + koff), ptx::make_smem_desc_sw128(b_hi + koff), idesc, 1);
-                    umma_tf32(tmem_acc, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(b_hi + koff), idesc, 1);
-                    accumulate = 1;
-                }
-                ptx::umma_commit(&empty_bar[stage]);
-                if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-            }
-            ptx::umma_commit(tmem_full_bar);
-        }
-    } else if (warp >= 4) {
-        // ---- converters: raw fp32 -> (hi in place, lo beside it); purely element-wise, so the TMA swizzle is preserved
-        const int ct = threadIdx.x - 128;
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
         int stage = 0;
         uint32_t phase = 0;
         constexpr int kAVec = Cfg::kABytes / 16, kBVec = Cfg::kBBytes / 16;
         for (int it = 0; it < nk; ++it) {
             ptx::mbar_wait(&full_bar[stage], phase);
+            // ---- converters: raw fp32 -> (hi in place, lo beside it); purely element-wise, so the TMA swizzle is preserved
             uint8_t* st = smem + stage * Cfg::kStageBytes;
             float4* a_hi = reinterpret_cast<float4*>(st);
             float4* a_lo = reinterpret_cast<float4*>(st + Cfg::kABytes);
@@ -233,55 +188,56 @@ __global__ void __launch_bounds__(kThreadsT, 1) gemm_tf32x3_kernel(const __grid_
             for (int i = ct; i < kAVec; i += kConvThreads) {
                 const float4 x = a_hi[i];
                 float4 h, l;
-                if (TRUNC) { split_trunc_tf32(x.x, l.x); split_trunc_tf32(x.y, l.y); split_trunc_tf32(x.z, l.z); split_trunc_tf32(x.w, l.w); }
-                else {
-                    split_keep_tf32(x.x, h.x, l.x); split_keep_tf32(x.y, h.y, l.y); split_keep_tf32(x.z, h.z, l.z); split_keep_tf32(x.w, h.w, l.w);
-                    a_hi[i] = h;
-                }
+                split_keep_tf32(x.x, h.x, l.x); split_keep_tf32(x.y, h.y, l.y); split_keep_tf32(x.z, h.z, l.z); split_keep_tf32(x.w, h.w, l.w);
+                a_hi[i] = h;
                 a_lo[i] = l;
             }
 #pragma unroll 4
             for (int i = ct; i < kBVec; i += kConvThreads) {
                 const float4 x = b_hi[i];
                 float4 h, l;
-                if (TRUNC) { split_trunc_tf32(x.x, l.x); split_trunc_tf32(x.y, l.y); split_trunc_tf32(x.z, l.z); split_trunc_tf32(x.w, l.w); }
-                else {
-                    split_keep_tf32(x.x, h.x, l.x); split_keep_tf32(x.y, h.y, l.y); split_keep_tf32(x.z, h.z, l.z); split_keep_tf32(x.w, h.w, l.w);
-                    b_hi[i] = h;
-                }
+                split_keep_tf32(x.x, h.x, l.x); split_keep_tf32(x.y, h.y, l.y); split_keep_tf32(x.z, h.z, l.z); split_keep_tf32(x.w, h.w, l.w);
+                b_hi[i] = h;
                 b_lo[i] = l;
             }
             ptx::fence_proxy_async_smem();              // generic-proxy writes -> visible to the tensor core's async-proxy reads
-            ptx::mbar_arrive(&conv_bar[stage]);
+            consumers_sync();                           // both warpgroups' halves of the conversion are done
+            const uint32_t s0 = ptx::smem_u32(st);
+            const uint32_t ah = s0 + cw * 64 * 128, al = s0 + Cfg::kABytes + cw * 64 * 128;
+            const uint32_t bh = s0 + 2 * Cfg::kABytes, bl = bh + Cfg::kBBytes;
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) ptx::reg_fence(acc[i]);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TK / 8; ++k) {
+                const uint32_t koff = k * 32;          // 8 tf32 = 32 bytes inside the 128-byte swizzle row
+                wgmma_tf32<BN>(acc, ah + koff, bl + koff);
+                wgmma_tf32<BN>(acc, al + koff, bh + koff);
+                wgmma_tf32<BN>(acc, ah + koff, bh + koff);
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) ptx::reg_fence(acc[i]);
+            if (tid == 0) ptx::mbar_arrive(&empty_bar[stage]);
             if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
         }
-        // ---- drain the accumulator into the staging tile (output orientation); the ring is idle once tmem_full_bar fires
-        ptx::mbar_wait(tmem_full_bar, 0);
-        ptx::tc_fence_after_sync();
+        // ---- drain the accumulator into the staging tile (output orientation); it aliases the ring, so both warpgroups' wgmmas must
+        // have retired first (the producer's loads all landed: every one of them was waited for above)
+        consumers_sync();
         float* S = reinterpret_cast<float*>(smem);
-        const int q = warp & 3;
-        const int arow = q * 32 + lane;                 // accumulator row (A-side row inside the tile) owned by this thread
-        const int half = (warp - 4) >> 2;               // two warps share a lane quadrant and split its columns
-        constexpr int kColsPerWarp = BN >= 32 ? BN / 2 : BN;
-#pragma unroll 1
-        for (int c0 = (BN >= 32 ? half * kColsPerWarp : 0); c0 < (BN >= 32 ? (half + 1) * kColsPerWarp : (half == 0 ? BN : 0)); c0 += 16) {
-            uint32_t r[16];
-            __syncwarp();
-            ptx::tmem_ld_32x32b_x16(tmem_acc + (static_cast<uint32_t>(q * 32) << 16) + c0, r);
-            ptx::tmem_ld_wait();
-            if (p.swapped) {
-                // S[m = c0 + j][n = arow]: a warp writes 32 consecutive floats per j
+        const int warp = tid >> 5, lane = tid & 31;
+        const int arow0 = cw * 64 + warp * 16 + (lane >> 2);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) S[(c0 + j) * (TM + Cfg::kPad) + arow] = __uint_as_float(r[j]);
-            } else {
-                // S[m = arow][n = c0 .. c0 + 15]
-                float4* dst = reinterpret_cast<float4*>(S + (long)arow * (BN + Cfg::kPad) + c0);
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
+            for (int e = 0; e < 4; ++e) {
+                const int arow = arow0 + 8 * (e >> 1);
+                const int bcol = 8 * j + 2 * (lane & 3) + (e & 1);
+                if (p.swapped) S[bcol * (TM + Cfg::kPad) + arow] = acc[4 * j + e];
+                else S[arow * (BN + Cfg::kPad) + bcol] = acc[4 * j + e];
             }
         }
-        ptx::tc_fence_before_sync();
     }
     __syncthreads();
     const bool via_scratch = ksplit > 1 && p.scratch != nullptr;
@@ -360,11 +316,8 @@ __global__ void __launch_bounds__(kThreadsT, 1) gemm_tf32x3_kernel(const __grid_
             }
         }
     }
-    ptx::tc_fence_before_sync();
     __syncthreads();
     if (ksplit > 1 && !via_scratch) ptx::cluster_sync_all();            // nobody leaves while a peer may still read its staging tile
-    ptx::tc_fence_after_sync();
-    if (warp == 2) ptx::tmem_dealloc(tmem_acc, Cfg::kTmemCols);
 }
 
 // ---- transposes for operands that are not K-major in HBM (input gradients need W^T, weight gradients dY^T and X^T) -------------------
@@ -456,12 +409,12 @@ const CUtensorMap* get_map(Tf32Context* ctx, const float* base, long rows, long 
     return &(ctx->maps[key] = m);
 }
 
-template <int BN, bool TRUNC>
-int launch_tf32_v(const Tf32Params& prm, int ksplit, int tiles_a, int tiles_b, cudaStream_t st) {
+template <int BN>
+int launch_tf32(const Tf32Params& prm, int ksplit, int tiles_a, int tiles_b, cudaStream_t st) {
     using Cfg = Tf32Cfg<BN>;
     static std::atomic<unsigned long long> attr_set{0};
     if (first_use_on_device(attr_set)) {
-        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tf32x3_kernel<BN, TRUNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tf32x3_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(ksplit, tiles_a, tiles_b);
@@ -475,13 +428,8 @@ int launch_tf32_v(const Tf32Params& prm, int ksplit, int tiles_a, int tiles_b, c
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = (ksplit > 1 && prm.scratch == nullptr) ? 1 : 0;
-    CAPB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tf32x3_kernel<BN, TRUNC>, prm));
+    CAPB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tf32x3_kernel<BN>, prm));
     return 0;
-}
-template <int BN>
-int launch_tf32(const Tf32Params& prm, int ksplit, int tiles_a, int tiles_b, cudaStream_t st) {
-    static const bool trunc = !(getenv("CAPB200_TF32_RNA") != nullptr && atoi(getenv("CAPB200_TF32_RNA")) != 0);
-    return trunc ? launch_tf32_v<BN, true>(prm, ksplit, tiles_a, tiles_b, st) : launch_tf32_v<BN, false>(prm, ksplit, tiles_a, tiles_b, st);
 }
 
 bool tma_ok(const float* p, long pitch, int K) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0 && (pitch & 3) == 0 && K >= 1; }
@@ -528,22 +476,21 @@ int gemm_tf32_launch(Tf32Context* ctx, int M, int N, int nseg, const float* cons
     }
     p.ksteps_total = ksteps;
     const int tiles_a = (int)cdiv((int)a_rows, TM), tiles_b = (int)cdiv((int)b_rows, bn);
-    // split-K so that ~all 148 SMs stream disjoint K-slices.
-    //  * default: across a thread-block cluster with the DSMEM reduction (largest power of two <= 8 with tiles * ksplit <= 148), except
+    // split-K so that ~all SMs stream disjoint K-slices.
+    //  * default: across a thread-block cluster with the DSMEM reduction (largest power of two <= 8 with tiles * ksplit <= SMs), except
     //    for the shape class named below.
     //  * CAPB200_TF32_SCRATCH=1 (0 = never): finer splits (up to 24 K-ranks, >= 2 K-blocks each) with the partial tiles in a global scratch buffer and a
-    //    last-arriver reduction in rank order.  Measured (profiles/r02p_tf32_sweep*.txt): it helps where the cluster form tops out at 64 CTAs on a
-    //    large K (att2ctx 22.6 -> 18.5 us) but loses elsewhere (q-projection 10.3 -> 14.3 us: the last CTA re-reads 16 partial tiles; gates
-    //    22.8 -> 26.1 us) and on the whole step (AoANet SCST 10.8 -> 11.2 ms), so the cluster form stays the default.
+    //    last-arriver reduction in rank order.  It helps where the cluster form tops out on a large K and few tiles, and loses where the last
+    //    CTA re-reads many partial tiles, so the cluster form stays the default.
     static const int scratch_mode = getenv("CAPB200_TF32_SCRATCH") != nullptr ? atoi(getenv("CAPB200_TF32_SCRATCH")) : -1;     // 1 always, 0 never, unset: hybrid
     const long tiles = (long)tiles_a * tiles_b;
+    const int sms = sm_count();
     int ksplit = 1;
-    while (ksplit < 8 && tiles * (ksplit * 2) <= 148 && ksteps / (ksplit * 2) >= 2) ksplit *= 2;
-    // hybrid default: the one shape class where the cluster form loses is 16 clusters of 8 (att2ctx and its input gradient, 2048 x 2048:
-    // 22.6 us as clusters, 18.5 us with 9 independent K-ranks per tile)
+    while (ksplit < 8 && tiles * (ksplit * 2) <= sms && ksteps / (ksplit * 2) >= 2) ksplit *= 2;
+    // hybrid default: the shape class where the cluster form loses is 16 or more clusters of 8 (att2ctx and its input gradient, 2048 x 2048)
     bool use_scratch = scratch_mode == 1 || (scratch_mode != 0 && ksplit == 8 && tiles >= 16);
     if (use_scratch) {
-        ksplit = (int)(148 / tiles);
+        ksplit = (int)(sms / tiles);
         if (ksplit > ksteps / 2) ksplit = ksteps / 2;
         if (ksplit > 24) ksplit = 24;
         if (ksplit < 1) ksplit = 1;

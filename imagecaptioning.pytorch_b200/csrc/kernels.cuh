@@ -140,7 +140,7 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
 int gemm_wgrad_launch(int M, int N, int K, const float* dY, long ld_dy, const float* X, long ld_x, float* G, long ld_g, int accumulate, int mode,
                       cudaStream_t st);   // G[M,N] (+)= dY[K,M]^T X[K,N]; mode 1 = 3xTF32 tensor cores
 int colsum_launch(int rows, int cols, const float* x, long ld, float* out, int accumulate, cudaStream_t st);
-// ---- gemm_tf32.cu: tcgen05 kind::tf32 3-pass GEMM on fp32 operands (in-kernel hi/lo split), split-K over a cluster with a DSMEM reduction
+// ---- gemm_tf32.cu: wgmma tf32 3-pass GEMM on fp32 operands (in-kernel hi/lo split), split-K over a cluster with a DSMEM reduction
 struct Tf32Context;      // per-engine cache of encoded tensor maps and transposed operands
 Tf32Context* tf32_context_create();
 void tf32_context_destroy(Tf32Context* c);

@@ -2,8 +2,7 @@
 //
 // Reference: tools/train.py:193-196 -- utils.clip_gradient(optimizer, opt.grad_clip_value) (captioning/utils/misc.py:156-160: every
 // param.grad clamped to [-c, c] in place) followed by optimizer.step() with torch.optim.Adam built by build_optimizer (misc.py:186-205).
-// The stock path is ~125 launches and ~10 passes over the 85 M parameters of AoANet (2.0 ms of a 17 ms step on B200,
-// profiles/r02e_timeline_aoa.txt); here it is ONE launch and one pass: g, p, m, v read once, p, m, v (and the clamped g) written once.
+// The stock path is ~125 launches and ~10 passes over the 85 M parameters of AoANet; here it is ONE launch and one pass: g, p, m, v read once, p, m, v (and the clamped g) written once.
 // Arithmetic follows torch's single-tensor Adam term by term (lerp for exp_avg, mul + addcmul for exp_avg_sq, sqrt / bias2_sqrt + eps,
 // addcdiv with -lr / bias1), so the result matches torch.optim.Adam to fp32 rounding (tests/test_gpu_ops.py).
 #include "../../include/capb200.h"

@@ -14,7 +14,7 @@ namespace capb200 {
 
 static int pw_blocks(long total) {
     long b = (total + 255) / 256;
-    return (int)(b > 148 * 8 ? 148 * 8 : b);
+    return (int)(b > sm_count() * 8 ? sm_count() * 8 : b);
 }
 
 namespace {
@@ -173,7 +173,7 @@ constexpr int ATT_JB = 5;       // rows handled per pass (beam 5 = one pass)
 constexpr int ATT_SW = 8;       // warps (= regions) per CTA
 // grid = (ceil(R / 8), B): the CTA stages the image's att_h rows in shared memory once (coalesced), then each warp scores one region.
 // NA = ceil(A / 32) rounded up to a power of two is a template parameter so the inner loops are branch-free and the
-// independent tanh chains of different k overlap (the runtime-bound version serialised them: 61 us -> see profiles/).
+// independent tanh chains of different k overlap (the runtime-bound version serialised them).
 template <int NA>
 __global__ void __launch_bounds__(ATT_SW * 32, NA <= 16 ? 5 : 2) att_score_kernel(int rpi, int R, int A, const float* __restrict__ att_h, long ld_ah,
                                                                 const float* __restrict__ p_att, long ld_pa, const float* __restrict__ alpha_w,

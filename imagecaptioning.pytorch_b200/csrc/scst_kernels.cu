@@ -338,7 +338,7 @@ __global__ void embed_backward_kernel(int rows, int E, const int* __restrict__ t
 
 // out[img, c] (+)= sum over the image's rows and all steps of x[step][row, c]
 // grid (images, column slices of 256): one column per thread, the steps x rpi terms of a column four loads at a time
-// (the first version ran one CTA per image over all columns: 10 CTAs on 148 SMs, 196 us for [20 x 50 x 4096])
+// (the first version ran one CTA per image over all columns: 10 CTAs for the whole GPU, 196 us for [20 x 50 x 4096])
 __global__ void per_image_sum_kernel(int steps, int rows, int rpi, int cols, const float* __restrict__ x, float* __restrict__ out) {
     const int img = blockIdx.x;
     const int c = blockIdx.y * blockDim.x + threadIdx.x;
@@ -359,7 +359,7 @@ __global__ void add_strided_kernel(float* a, const float* b, long ld_b, int rows
 
 int nblocks(long n) {
     long b = (n + 255) / 256;
-    return (int)(b > 148 * 8 ? 148 * 8 : (b < 1 ? 1 : b));
+    return (int)(b > sm_count() * 8 ? sm_count() * 8 : (b < 1 ? 1 : b));
 }
 
 }  // namespace

@@ -397,7 +397,7 @@ int capb200_tfm_decode_sample(capb200_tfm_engine* e, const float* att, const flo
 // Shape of the implementation: decoder activations live on a TIME-major tape (row = t * N + n), so
 //   * the teacher-forced pass runs every kernel once over all L * N rows,
 //   * the sampling pass runs the same kernels on the N rows of one position per step (the tape's earlier K/V rows are its cache),
-//   * the backward pass is always batched over the L * N rows: every contraction is a tcgen05 kind::tf32 GEMM (gemm_tf32.cu).
+//   * the backward pass is always batched over the L * N rows: every contraction is a wgmma tf32 GEMM (gemm_tf32.cu).
 // Dropout masks are functions of (seed, site, position, element), so both forward forms draw the same masks.  Sites: 1 att_embed;
 // 2 target embedding + positional encoding; encoder layer l: 10+l attention probabilities, 20+l / 40+l the two SublayerConnections,
 // 30+l the feed-forward hidden layer; decoder layer l: 50+l self-attention probabilities, 60+l / 80+l / 100+l the three

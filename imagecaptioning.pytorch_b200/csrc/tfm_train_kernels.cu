@@ -15,7 +15,7 @@ namespace {
 
 inline int blocks_for(long n) {
     long b = (n + 255) / 256;
-    return (int)(b > 148 * 16 ? 148 * 16 : (b < 1 ? 1 : b));
+    return (int)(b > sm_count() * 16 ? sm_count() * 16 : (b < 1 ? 1 : b));
 }
 
 // x[r, :] = dropout(lut[tok[r]] * scale + pe[t0 + r / rps]);  Embeddings (TransformerModel.py:208-215) + PositionalEncoding (:217-235)

@@ -222,7 +222,7 @@ __global__ void masked_mean_kernel(int R, int H, const float* __restrict__ x, lo
 int glu_launch(int rows, int H, const float* t, long ld_t, const float* residual, long ld_res, ActView out, cudaStream_t st) {
     if (rows <= 0) return 0;
     long blocks = ((long)rows * H + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > sm_count() * 8) blocks = sm_count() * 8;
     glu_kernel<<<(int)blocks, 256, 0, st>>>(rows, H, t, ld_t, residual, ld_res, out);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -759,7 +759,7 @@ int vocab_step_launch(const VocabStepArgs& a, cudaStream_t stream) {
         CAPB_REQUIRE(a.select == 0 && a.topk > 0, "stats mode is the beam-search epilogue");
         const bool vec = ((a.V1 & 3) == 0) && ((a.ld & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.logits) & 15) == 0);
         const size_t stream_smem = sizeof(float) * 2 * (size_t)a.V1;
-        // default: single-pass online kernel; "stream" / "reg" / "plain" select the other variants for A/B timing (profiles/)
+        // default: single-pass online kernel; "stream" / "reg" / "plain" select the other variants for A/B timing
         static const char* variant = getenv("CAPB200_VOCAB_STATS");
         const char vsel = variant ? variant[0] : 'o';
         if (vec && vsel == 'o' && !(variant && variant[1] == '2')) {
@@ -771,7 +771,7 @@ int vocab_step_launch(const VocabStepArgs& a, cudaStream_t stream) {
             if (first_use_on_device(configured)) {
                 CAPB_CHECK_CUDA(cudaFuncSetAttribute(vocab_stats_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(100 * 1024)));
             }
-            const int grid = a.rows < 2 * 148 ? a.rows : 2 * 148;       // two resident CTAs per SM, each double-buffering one row
+            const int grid = a.rows < 2 * sm_count() ? a.rows : 2 * sm_count();       // two resident CTAs per SM, each double-buffering one row
             vocab_stats_stream_kernel<<<grid, VT, stream_smem, stream>>>(a);
         } else if (vec && vsel == 'r' && a.V1 <= VT * 4 * 10) {
             vocab_stats_reg_kernel<10><<<a.rows, VT, 0, stream>>>(a);
@@ -789,7 +789,7 @@ int vocab_step_launch(const VocabStepArgs& a, cudaStream_t stream) {
         CAPB_CHECK_CUDA(cudaFuncSetAttribute(vocab_step_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
         CAPB_CHECK_CUDA(cudaFuncSetAttribute(vocab_step_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
     }
-    if (a.topk <= 2 && a.select != 0 && a.rows <= 2 * 148) {
+    if (a.topk <= 2 && a.select != 0 && a.rows <= 2 * sm_count()) {
         static std::atomic<unsigned long long> configured2{0};
         if (first_use_on_device(configured2)) {
             CAPB_CHECK_CUDA(cudaFuncSetAttribute(vocab_step_kernel<2, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));

@@ -94,13 +94,13 @@ class StructureLosses(nn.Module):
         self.opt = opt
         self.loss_type = opt.structure_loss_type
         if self.loss_type != 'new_self_critical':
-            raise NotImplementedError("structure_loss_type %r: the B200 engine implements 'new_self_critical'" % self.loss_type)
+            raise NotImplementedError("structure_loss_type %r: the engine implements 'new_self_critical'" % self.loss_type)
 
     def forward(self, input, seq, data_gts, reduction='mean'):
         n = input.shape[0] // len(data_gts)
         assert n == self.opt.train_sample_n, n
         if getattr(self.opt, 'entropy_reward_weight', 0) > 0 or getattr(self.opt, 'self_cider_reward_weight', 0) > 0:
-            raise NotImplementedError('entropy / self-CIDEr rewards are out of scope of the B200 engine')
+            raise NotImplementedError('entropy / self-CIDEr rewards are out of scope of the engine')
         mask = _shifted_mask(seq)
         w = float(getattr(self.opt, 'cider_reward_weight', 1))
         scores = (cider_scores(data_gts, seq) * w).to(input).view(-1, n)
@@ -320,7 +320,7 @@ class B200LossWrapper(nn.Module):
                 why.append('train_sample_method / train_beam_size other than multinomial sampling')
             if opt.sc_sample_method != 'greedy' or opt.sc_beam_size != 1:
                 why.append('sc_sample_method / sc_beam_size other than a greedy baseline')
-            raise NotImplementedError('self-critical training step outside the fused B200 path: ' + '; '.join(why or ['unsupported configuration']))
+            raise NotImplementedError('self-critical training step outside the fused engine path: ' + '; '.join(why or ['unsupported configuration']))
         # no-grad evaluation of the sc branch (reward monitoring): host-level composition of the engine calls, dropout off
         self.model.eval()
         with torch.no_grad():

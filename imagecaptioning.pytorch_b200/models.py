@@ -11,7 +11,7 @@
     and ``self.done_beams`` after beam search                                      AttModel.py:218-352
 
 The parameters are ordinary ``nn.Parameter``s owned by PyTorch; every timestep of every decode runs in the hand-written
-sm_100a kernels behind the C ABI (include/capb200.h).  Nothing here computes on the CPU and nothing falls back to
+sm_90a kernels behind the C ABI (include/capb200.h).  Nothing here computes on the CPU and nothing falls back to
 PyTorch ops: unsupported decode options raise.
 """
 from __future__ import annotations
@@ -143,9 +143,9 @@ class B200CaptionModel(nn.Module):
         if (self.bos_idx, self.eos_idx, self.pad_idx) != (0, 0, 0):
             raise NotImplementedError('capb200 engine assumes bos = eos = pad = 0 (AttModel.py:65-67 defaults)')
         if getattr(opt, 'use_bn', 0):
-            raise NotImplementedError('use_bn is not on the B200 decode path')
+            raise NotImplementedError('use_bn is not on the engine decode path')
         if getattr(opt, 'logit_layers', 1) != 1:
-            raise NotImplementedError('logit_layers > 1 is not on the B200 decode path')
+            raise NotImplementedError('logit_layers > 1 is not on the engine decode path')
         self.ss_prob = 0.0
         self.vocab = opt.vocab
         self.bad_endings_ix = [int(k) for k, v in self.vocab.items() if v in BAD_ENDINGS]
@@ -292,9 +292,9 @@ class B200CaptionModel(nn.Module):
 
     def _check_opts(self, opt):
         if opt.get('group_size', 1) != 1:
-            raise NotImplementedError('diverse beam search (group_size > 1) is out of scope of the B200 engine (SURVEY.md section 8f)')
+            raise NotImplementedError('diverse beam search (group_size > 1) is out of scope of the engine (SURVEY.md section 8f)')
         if opt.get('output_logsoftmax', 1) != 1:
-            raise NotImplementedError('output_logsoftmax=0 is out of scope of the B200 engine')
+            raise NotImplementedError('output_logsoftmax=0 is out of scope of the engine')
 
     def _decode_edits(self, opt, device, beam, batch_size=0):
         """The reference's per-step log-prob edits as a capb200_decode_edits (CaptionModel.py:118-120,154-162; AttModel.py:265-332)."""
@@ -341,7 +341,7 @@ class B200CaptionModel(nn.Module):
                 raise ValueError('sample_method %r: top-k needs k >= 1, nucleus sampling 0 < p < 1' % sample_method)
             method = _lib.SAMPLE_TOPP if top < 1 else _lib.SAMPLE_TOPK
         else:
-            raise NotImplementedError("sample_method %r is out of scope of the B200 engine" % sample_method)
+            raise NotImplementedError("sample_method %r is out of scope of the engine" % sample_method)
         lib = self._ensure_engine(fc_feats.device)
         fc = self._f32(fc_feats)
         att, masks = self._clip(att_feats, att_masks)
@@ -389,7 +389,7 @@ class B200CaptionModel(nn.Module):
         n_kinds = int(bool(opt.get('decoding_constraint', 0))) + int(bool(opt.get('remove_bad_endings', 0)) and bool(self.bad_endings_ix)) + \
             int((bool(opt.get('suppress_UNK', 0)) and self.vocab.get(str(self.vocab_size)) == 'UNK') or self.unk_idx is not None)
         if beam_size + n_kinds > 16:
-            raise NotImplementedError('beam_size + number of active decode edits must be <= 16 on the B200 engine')
+            raise NotImplementedError('beam_size + number of active decode edits must be <= 16 on the engine')
         cfg = opt.get('length_penalty', '')
         kind, alpha = (cfg.split('_') + ['0'])[:2] if cfg else ('', '0')
         lib = self._ensure_engine(fc_feats.device)
@@ -935,7 +935,7 @@ class B200AoAModel(B200CaptionModel):
         need = dict(refine=1, refine_aoa=1, use_ff=0, decoder_type='AoA', use_multi_head=2, multi_head_scale=1)
         for k, v in need.items():
             if getattr(opt, k, v) != v:
-                raise NotImplementedError('AoA option %s=%r is outside the configs/aoa.yml configuration the B200 engine implements' % (k, getattr(opt, k)))
+                raise NotImplementedError('AoA option %s=%r is outside the configs/aoa.yml configuration the engine implements' % (k, getattr(opt, k)))
         if not getattr(opt, 'mean_feats', 1):
             raise NotImplementedError('mean_feats=0 is outside the configs/aoa.yml configuration')
         if getattr(opt, 'out_res', 0):
@@ -1147,7 +1147,7 @@ class B200AoAModel(B200CaptionModel):
 
 def setup(opt, numeric_mode=None):
     """Factory with the contract of captioning.models.setup (captioning/models/__init__.py:20-73) for the families on the
-    B200 hot path."""
+    engine hot path."""
     name = opt.caption_model
     if name in ('topdown', 'updown'):
         return B200UpDownModel(opt, numeric_mode)
@@ -1157,6 +1157,6 @@ def setup(opt, numeric_mode=None):
         return B200AoAModel(opt, numeric_mode)
     if name == 'transformer':
         if getattr(opt, 'cached_transformer', False):
-            raise NotImplementedError('cachedTransformer is a reference-side variant; the B200 engine always caches K/V')
+            raise NotImplementedError('cachedTransformer is a reference-side variant; the engine always caches K/V')
         return B200TransformerModel(opt, numeric_mode)
-    raise NotImplementedError('caption_model %r is not on the B200 decode path yet (SURVEY.md section 8)' % name)
+    raise NotImplementedError('caption_model %r is not on the engine decode path yet (SURVEY.md section 8)' % name)

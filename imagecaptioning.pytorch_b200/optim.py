@@ -1,8 +1,8 @@
-"""Optimizer step of the training loop on the B200 engine.
+"""Optimizer step of the training loop on the engine.
 
 The reference's loop (tools/train.py:193-196) clamps every gradient (``utils.clip_gradient``, captioning/utils/misc.py:156-160) and
 then calls ``torch.optim.Adam.step()`` (``build_optimizer``, misc.py:186-205).  On the stock path that is ~125 small launches and
-about ten passes over the parameters -- 2 ms of a 17 ms AoANet SCST step on B200.  ``FusedAdam`` is ``torch.optim.Adam`` with ``step()``
+about ten passes over the parameters.  ``FusedAdam`` is ``torch.optim.Adam`` with ``step()``
 replaced by one launch of ``capb200_adam_step`` (csrc/optim.cu): same constructor, same ``state_dict`` layout (``step`` / ``exp_avg`` /
 ``exp_avg_sq`` per parameter, so checkpoints written by either load into the other -- tools/train.py:74-77 resumes ``optimizer.pth``),
 same arithmetic term by term; ``clip_value`` folds ``clip_gradient`` into the same pass.

@@ -184,7 +184,7 @@ def get_self_critical_reward(greedy_res, data_gts, gen_result, opt):
     """reward[i*n+j, :] = CIDEr-D(sample j of image i) - CIDEr-D(greedy of image i), as a device fp32 tensor [S, T]
     (the reference returns the same values as a host float64 array that LossWrapper immediately moves back to the GPU)."""
     if getattr(opt, 'bleu_reward_weight', 0) > 0:
-        raise NotImplementedError('BLEU reward is out of scope of the B200 engine (bleu_reward_weight defaults to 0)')
+        raise NotImplementedError('BLEU reward is out of scope of the engine (bleu_reward_weight defaults to 0)')
     w = float(getattr(opt, 'cider_reward_weight', 1))
     _, reward = cider_scores_and_reward(greedy_res, data_gts, gen_result)
     return reward if w == 1.0 else reward * w
@@ -215,7 +215,7 @@ def get_scores(data_gts, gen_result, opt):
     """rewards.py:83-114 with the CIDEr-D term only: ``cider_reward_weight * CIDEr-D`` per sampled caption, float64 [S] on the device
     (the reference returns the same values as a host numpy array)."""
     if getattr(opt, 'bleu_reward_weight', 0) > 0:
-        raise NotImplementedError('BLEU reward is out of scope of the B200 engine (bleu_reward_weight defaults to 0)')
+        raise NotImplementedError('BLEU reward is out of scope of the engine (bleu_reward_weight defaults to 0)')
     w = float(getattr(opt, 'cider_reward_weight', 1))
     scores = cider_scores(data_gts, gen_result)
     return scores if w == 1.0 else scores * w

@@ -174,7 +174,7 @@ def model_opt(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int
 
 def build_model(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int, T: int, seed: int, logit_scale: float, mode: str,
                 device='cuda', heads: int = 8):
-    """B200 model of ``family`` with the seeded synthetic weights loaded, on ``device``, in eval mode."""
+    """Engine model of ``family`` with the seeded synthetic weights loaded, on ``device``, in eval mode."""
     from . import setup
     W = make_weights(family, V, E, H, A, F_fc, F_att, seed=seed, logit_scale=logit_scale)
     model = setup(model_opt(family, V, E, H, A, F_fc, F_att, T, heads), numeric_mode=mode)

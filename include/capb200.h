@@ -1,4 +1,4 @@
-/* capb200 -- C ABI of the B200-native caption-decoding / SCST engine.
+/* capb200 -- C ABI of the H100 (sm_90a) caption-decoding / SCST engine.
  *
  * Drop-in boundary.  The reference (ruotianluo/ImageCaptioning.pytorch) is pure Python and has no FFI layer; its boundary
  * for this path is two Python call surfaces (SURVEY.md section 8b):
@@ -24,11 +24,11 @@ extern "C" {
 
 /* numeric modes of the dense contractions */
 #define CAPB200_MODE_SIMT_FP32 0 /* fp32 FFMA on CUDA cores */
-#define CAPB200_MODE_TC_F16X3 1  /* tcgen05 kind::f16, split-fp16 operands, 3 MMA passes, fp32 accumulate (parity grade) */
-#define CAPB200_MODE_TC_F16X1 2  /* tcgen05 kind::f16, single pass (throughput mode, not parity grade) */
+#define CAPB200_MODE_TC_F16X3 1  /* wgmma f16, split-fp16 operands, 3 MMA passes, fp32 accumulate (parity grade) */
+#define CAPB200_MODE_TC_F16X1 2  /* wgmma f16, single pass (throughput mode, not parity grade) */
 #define CAPB200_MODE_SKINNY_TF32X3 3 /* capb200_linear only: the training step's split-K GEMM, 3xTF32 mma.sync on the fp32 weights */
 #define CAPB200_MODE_SKINNY_FP32 4   /* capb200_linear only: same split-K GEMM on CUDA cores */
-#define CAPB200_MODE_TF32X3_TC 5       /* capb200_linear only: the training steps' tcgen05 kind::tf32 3-pass GEMM on fp32 operands (gemm_tf32.cu) */
+#define CAPB200_MODE_TF32X3_TC 5       /* capb200_linear only: the training steps' wgmma tf32 3-pass GEMM on fp32 operands (gemm_tf32.cu) */
 #define CAPB200_MODE_TF32X3_TC_DGRAD 6 /* same kernel, input-gradient form: y[M,N] = x[M,K] * w[K,N]  (w row-major [K,N], transposed internally) */
 #define CAPB200_MODE_TF32X3_TC_WGRAD 7 /* same kernel, weight-gradient form: y[M,N] = x[K,M]^T * w[K,N] (both row-major, transposed internally) */
 

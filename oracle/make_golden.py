@@ -758,12 +758,41 @@ def gen_state_dict_keys(out_dir):
     print('state_dict_keys', {k: len(v) for k, v in res.items()})
 
 
+def gen_eval_split(out_dir, scratch):
+    """The reference's eval_split on the stub model / loader of tests/test_eval_cpu.py: loss, captions, perplexities and entropies, and for
+    sample_n = 3 the n-predictions it saves beside them (one entry per sample_n_method)."""
+    import json
+    sys.path.insert(0, os.path.join(REPO, 'tests'))
+    import test_eval_cpu as tec
+    import captioning.utils.eval_utils as REF
+    T, V1 = 6, 12
+    res = {}
+    kwargs = {'verbose': False, 'verbose_loss': 1, 'split': 'val', 'language_eval': 0, 'dataset': 'coco', 'beam_size': 1, 'sample_n': 1,
+              'device': 'cpu', 'id': 'stub', 'num_images': -1}
+    loss, preds, _ = REF.eval_split(tec._StubModel(T, V1), tec._crit, tec._StubLoader(10, 4, T, V1), dict(kwargs))
+    res['sample_n_1'] = {'loss': float(loss), 'caption': [p['caption'] for p in preds], 'perplexity': [float(p['perplexity']) for p in preds],
+                         'entropy': [float(p['entropy']) for p in preds]}
+    for method in ('sample', 'bs', 'top3'):
+        d = tempfile.mkdtemp(dir=scratch)
+        os.chdir(d)
+        kw = dict(kwargs, sample_n=3, sample_n_method=method, id='stubn')
+        loss, preds, _ = REF.eval_split(tec._StubModel(T, V1), tec._crit, tec._StubLoader(10, 4, T, V1), kw)
+        _, rn = torch.load(os.path.join('eval_results', '.saved_pred_stubn_val.pth'), weights_only=False)
+        res['sample_n_3_' + method] = {'loss': float(loss), 'caption': [p['caption'] for p in preds],
+                                       'n_image_id': [int(e['image_id']) for e in rn], 'n_caption': [e['caption'] for e in rn],
+                                       'n_perplexity': [float(e['perplexity']) for e in rn] if method != 'bs' else None}
+        os.chdir(scratch)
+    with open(os.path.join(out_dir, 'eval_split.json'), 'w') as f:
+        json.dump(res, f, indent=1, sort_keys=True)
+    print('eval_split', sorted(res))
+
+
 def main():
     out_dir = os.path.join(REPO, 'tests', 'golden')
     os.makedirs(out_dir, exist_ok=True)
     scratch = _enter_scratch()
     torch.set_num_threads(os.cpu_count())
-    which = sys.argv[1:] or ['small', 'newfc', 'full', 'ciderd', 'rc', 'keys', 'tfm', 'aoa', 'xe', 'dseq', 'pascal', 'penalty', 'b256', 'tfm64', 'aoafull', 'options', 'tfmtrain', 'tfmtrainfull']
+    which = sys.argv[1:] or ['small', 'newfc', 'full', 'ciderd', 'rc', 'keys', 'tfm', 'aoa', 'xe', 'dseq', 'pascal', 'penalty', 'b256', 'tfm64', 'aoafull', 'options', 'tfmtrain', 'tfmtrainfull', 'eval']
     if 'small' in which:
         gen_updown_small(out_dir)
     if 'newfc' in which:
@@ -800,6 +829,8 @@ def main():
         gen_transformer_train(out_dir, scratch)
     if 'tfmtrainfull' in which:
         gen_transformer_train_full(out_dir, scratch)
+    if 'eval' in which:
+        gen_eval_split(out_dir, scratch)
 
 
 if __name__ == '__main__':

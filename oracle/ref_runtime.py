@@ -16,17 +16,16 @@ from collections import defaultdict
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 _REF_COPY = os.path.join(HERE, '_ref')
-_LIVE = '/root/reference'
 _state = {'scratch': None, 'root': None}
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(_REF_COPY, 'captioning')) or os.path.isdir(os.path.join(_LIVE, 'captioning'))
+    return os.path.isdir(os.path.join(_REF_COPY, 'captioning'))
 
 
 def root() -> str:
-    """oracle/_ref when the copy exists (it is what travels to the GPU box), else the live tree of the build container."""
-    return _REF_COPY if os.path.isdir(os.path.join(_REF_COPY, 'captioning')) else _LIVE
+    """oracle/_ref, the copy oracle/build_ref.py makes."""
+    return _REF_COPY
 
 
 def enter() -> str:
@@ -35,7 +34,7 @@ def enter() -> str:
         os.chdir(_state['scratch'])
         return _state['scratch']
     if not available():
-        raise RuntimeError('the reference copy oracle/_ref/ is missing: run python oracle/build_ref.py in the build container')
+        raise RuntimeError('the reference copy oracle/_ref/ is missing: run python oracle/build_ref.py where the reference is checked out')
     r = root()
     d = tempfile.mkdtemp(prefix='refcwd_')
     os.symlink(os.path.join(r, 'cider'), os.path.join(d, 'cider'))

@@ -1,4 +1,4 @@
-"""Stand-alone first-contact script for a fresh B200 box: exercises the tcgen05 GEMM on a few shapes with a hard
+"""Stand-alone first-contact script for a fresh GPU machine: exercises the wgmma GEMM on a few shapes with a hard
 process-level timeout around each launch group, so a protocol bug becomes a log line rather than a hung box.
 Usage: python tests/gpu_first_contact.py   (writes to stdout)"""
 import os

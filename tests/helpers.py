@@ -29,7 +29,7 @@ def make_opt(family, V, E, H, A, F_fc, F_att, T):
 
 
 def build_pair(family, V, E, H, A, F_fc, F_att, T, seed, logit_scale, mode, device='cuda', heads=8):
-    """Returns (B200 model on the GPU, oracle Family on the CPU) sharing the same synthetic weights.
+    """Returns (engine model on the GPU, oracle Family on the CPU) sharing the same synthetic weights.
     For 'transformer': E = d_model, H = d_ff, A = layers per stack (the make_weights convention)."""
     import imagecaptioning.pytorch_b200 as b200
     W = co.make_weights(family, V, E, H, A, F_fc, F_att, seed=seed, logit_scale=logit_scale)

@@ -1,4 +1,4 @@
-"""GPU parity of the whole decode path (through the Python mirror -> C ABI -> sm_100a kernels) against the oracle and the
+"""GPU parity of the whole decode path (through the Python mirror -> C ABI -> sm_90a kernels) against the oracle and the
 golden vectors produced by the live reference.  Bar (BASELINE.json north_star): token ids bit-exact, log-probs within 1e-4."""
 import os
 

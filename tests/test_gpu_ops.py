@@ -37,7 +37,7 @@ def test_linear_matches_fp64(L, mode, shape):
     y = _linear(L, x.cuda(), w.cuda(), b.cuda(), False, mode).cpu().double()
     err = float((y - ref).abs().max())
     fp32_err = float(((x @ w.t() + b).double() - ref).abs().max())
-    # fp32-grade modes must stay within summation-order noise of an fp32 GEMM.  The tcgen05 accumulator truncates (round
+    # fp32-grade modes must stay within summation-order noise of an fp32 GEMM.  The tensor-core accumulator truncates (round
     # toward zero) once per MMA instruction, so the 3-pass mode gets an explicit budget of one fp32 ulp of the largest
     # output per accumulate (3 * K/16 of them); the single-pass mode is fp16-input grade.
     if mode == 'simt_fp32':
@@ -72,7 +72,7 @@ def test_skinny_linear_matches_fp64(L, mode, shape):
 @pytest.mark.parametrize('shape', [(50, 4096, 3072), (50, 9488, 1024), (50, 1000, 4000), (12, 41, 48), (64, 256, 96), (200, 520, 1000), (360, 3072, 1024),
                                    (1000, 1024, 9488), (257, 130, 36)])
 def test_tf32x3_tcgen05_linear_matches_fp64(L, shape):
-    """The training steps' tcgen05 kind::tf32 kernel (gemm_tf32.cu: raw fp32 tiles by TMA, hi/lo split in shared memory, 3 MMAs per K-block,
+    """The training steps' wgmma tf32 kernel (gemm_tf32.cu: raw fp32 tiles by TMA, hi/lo split in shared memory, 3 MMAs per K-block,
     split-K over a cluster with a DSMEM reduction), swapped (M <= 256) and normal orientation, ragged M / N / K, against float64.  Half of
     the rows are gradient-like (1e-7): they must not be flushed."""
     M, N, K = shape

@@ -1,4 +1,4 @@
-"""GPU: where the time of one decode GEMM launch goes.  Runs the CTA-pair tcgen05 kernel on a decode-step shape with the phase stamps on
+"""GPU: where the time of one decode GEMM launch goes.  Runs the 3-pass wgmma kernel on a decode-step shape with the phase stamps on
 (capb200_gemm_trace) and prints, relative to the earliest set-up stamp, when each phase happened (median / max over the CTAs).
 
     python tools/gemm_trace.py [M N K]        default: the language-LSTM gates of the headline shape, 1280 x 4000 x 3000
@@ -18,7 +18,7 @@ L.check(lib.capb200_gemm_trace(L.ptr(x), L.ptr(w), L.ptr(y), M, N, K, tr.ctypes.
 used = tr[:, 0] > 0
 t = tr[used].astype(np.float64)
 t0 = t[:, 0].min()
-names = ['set-up done', 'first operands landed', 'tile 0: all MMAs issued', 'tile 1: all MMAs issued', 'tile 0: accumulator complete', 'tile 1: accumulator complete',
+names = ['set-up done', 'first operands landed', 'tile 0: main loop done', 'tile 1: main loop done', '(unused)', '(unused)',
          'tile 0: epilogue done', 'tile 1: epilogue done', 'kernel end']
 print('decode GEMM %d x %d x %d, %d CTAs traced; times in us after the first CTA finished its set-up' % (M, N, K, int(used.sum())))
 for i, n in enumerate(names):
@@ -30,8 +30,8 @@ for i, n in enumerate(names):
 lead = t[(t[:, 2] > 0)]
 if lead.size:
     d01 = (lead[:, 2] - lead[:, 1]) / 1e3
-    print('leader CTAs: first operands -> tile 0 MMAs issued: median %.2f us (%d K-blocks => %.3f us per K-block)' % (np.median(d01), -(-K // 64), np.median(d01) / (-(-K // 64))))
+    print('first operands -> tile 0 main loop done: median %.2f us (%d K-blocks => %.3f us per K-block)' % (np.median(d01), -(-K // 64), np.median(d01) / (-(-K // 64))))
     two = lead[lead[:, 3] > 0]
     if two.size:
         d12 = (two[:, 3] - two[:, 2]) / 1e3
-        print('leader CTAs with two tiles: tile 0 issued -> tile 1 issued: median %.2f us' % np.median(d12))
+        print('CTAs with two tiles: tile 0 main loop -> tile 1 main loop: median %.2f us' % np.median(d12))

@@ -1,4 +1,4 @@
-"""GPU: time the training-step GEMM shapes of BASELINE configs[3] (AoANet, 10 images x 5 samples) on the tcgen05 kind::tf32 kernel and on the
+"""GPU: time the training-step GEMM shapes of BASELINE configs[3] (AoANet, 10 images x 5 samples) on the wgmma tf32 kernel and on the
 mma.sync kernel it replaced; reports microseconds per launch and the fraction of the HBM roofline (fp32 weight bytes / time).
 
     python tools/tf32_sweep.py [iters]
@@ -17,7 +17,7 @@ SHAPES = [('att_lstm gates (3 segments in the step)', 50, 4096, 3072), ('attenti
           ('logit', 50, 9488, 1024), ('d gates -> d x (W^T)', 50, 1024, 4096), ('refiner q|k|v', 360, 3072, 1024), ('refiner AoA', 360, 2048, 2048),
           ('logit input gradient, batched over time', 1000, 1024, 9488), ('weight gradient att_lstm (out x in over T*N rows)', 4096, 1024, 1000),
           ('weight gradient logit', 9488, 1024, 1000), ('greedy-sized rows', 10, 4096, 3072)]
-print('%-52s %6s %6s %6s  %10s %10s  %8s %8s' % ('call site', 'M', 'N', 'K', 'tcgen05 us', 'mma.sync us', 'GB/s', 'of HBM'))
+print('%-52s %6s %6s %6s  %10s %10s  %8s %8s' % ('call site', 'M', 'N', 'K', 'wgmma us', 'mma.sync us', 'GB/s', 'of HBM'))
 for name, M, N, K in SHAPES:
     x = torch.randn(M, K, device='cuda'); w = torch.randn(N, K, device='cuda') / K ** 0.5; b = torch.zeros(N, device='cuda'); y = torch.empty(M, N, device='cuda')
     out = []
