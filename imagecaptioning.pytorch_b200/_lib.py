@@ -49,6 +49,13 @@ class BeamOpts(Structure):
         super().__init__(beam_size, sample_n, penalty_kind, penalty_alpha, temperature, edits if edits is not None else DecodeEdits.none())
 
 
+class DiverseOpts(Structure):
+    _fields_ = [('base', BeamOpts), ('group_size', c_int), ('diversity_lambda', c_float)]
+
+    def __init__(self, base, group_size, diversity_lambda):
+        super().__init__(base, group_size, diversity_lambda)
+
+
 class SampleOpts(Structure):
     _fields_ = [('sample_n', c_int), ('method', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('steps', c_int), ('top', c_float),
                 ('edits', DecodeEdits)]
@@ -165,6 +172,8 @@ SIGNATURES = {
     'capb200_decode_beam': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
     'capb200_beam_record_logprobs': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    'capb200_decode_beam_diverse': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(DiverseOpts), c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p]),
     'capb200_decode_sample': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(SampleOpts), c_void_p, c_long, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),
     'capb200_engine_launch_count': (c_long, [c_void_p]),
@@ -185,6 +194,8 @@ SIGNATURES = {
     'capb200_aoa_decode_beam': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p]),
     'capb200_aoa_beam_record_logprobs': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    'capb200_aoa_decode_beam_diverse': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(DiverseOpts), c_void_p, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_void_p]),
     'capb200_aoa_decode_sample': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(SampleOpts), c_void_p, c_long, c_void_p, c_void_p, c_void_p,
                                           c_void_p]),
     'capb200_aoa_scst_step': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(AoaScstOpts), c_void_p, c_void_p, c_void_p, c_int, POINTER(AoaWeights),

@@ -327,8 +327,7 @@ void capb200_aoa_destroy(capb200_aoa_engine* e) {
     destroy_plans(e);
     cudaFree(e->wblock);
     cudaFree(e->ws);
-    if (e->d.loop_exec) cudaGraphExecDestroy(e->d.loop_exec);
-    cudaFree(e->d.slab);
+    e->d.release();
     cudaFree(e->tape);
     e->sg.destroy();
     tf32_context_destroy(e->tf32);
@@ -440,6 +439,25 @@ int capb200_aoa_decode_beam(capb200_aoa_engine* e, const float* att, const float
     };
     return beam_decode_driver(e->d, e->V1, e->T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
                               done_raw, core, &e->launches, st, loop_graph_key(e->ws, e->wblock, mask, R, 9), to_edits(opts->edits), opts->temperature);
+}
+
+int capb200_aoa_decode_beam_diverse(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
+                                    long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
+    if (check_ready(e)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CAPB_REQUIRE(opts != nullptr && att != nullptr && seq != nullptr && B >= 1 && R >= 1, "bad argument");
+    if (opts->group_size == 1) return capb200_aoa_decode_beam(e, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream);
+    const int beam = opts->base.beam_size;
+    CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= e->V1, "beam_size must be in 2..16 and <= V+1");
+    if (ensure_workspace(e, B, B * beam, R, beam, st)) return 1;
+    if (prepare(e, att, mask, B, R, st)) return 1;
+    e->core_cur = 0;
+    auto core = [&](int nrows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
+        return core_step(e, nrows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
+    };
+    return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
+                                      opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
+                                      loop_graph_key(e->ws, e->wblock, mask, R, 9), to_edits(opts->base.edits), opts->base.temperature);
 }
 
 int capb200_aoa_beam_record_logprobs(capb200_aoa_engine* e, int image, int rank, float* dst, void* stream) {

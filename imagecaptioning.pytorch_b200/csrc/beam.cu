@@ -1,4 +1,4 @@
-// Device-resident beam search bookkeeping (group_size == 1 path of CaptionModel.beam_search).
+// Device-resident beam search bookkeeping (CaptionModel.beam_search: the group_size == 1 path and diverse beam search).
 //
 // The reference (captioning/models/CaptionModel.py:60-110,148-207) sorts all b*(V+1) candidates per image, gathers and
 // re-concatenates the whole [B,b,t,V+1] log-prob history every step, runs three .all() host syncs and a Python loop with
@@ -25,14 +25,17 @@ __device__ __forceinline__ double apply_penalty(int kind, float alpha, int lengt
     return p;
 }
 
-// one warp per image
-__global__ void __launch_bounds__(32) beam_step_kernel(BeamState s, int t, int live, const float* __restrict__ top_val,
-                                                       const int* __restrict__ top_idx, int penalty_kind, float penalty_alpha,
-                                                       double* __restrict__ done_p) {
-    const int img = blockIdx.x;
+// One step of the search for one image (or one group of an image in diverse beam search), run by one warp.  `img` indexes the sums /
+// sequence tables / records (s.beam beams each); the `live` parent rows of this step are top-list rows row0 .. row0 + live - 1 with `kl`
+// candidates each.  The n_pen words at `pen` (shared memory) lower a candidate by lambda per occurrence (add_diversity,
+// CaptionModel.py:38-55).  Chosen words go to s.tokens / s.src_row[img * beam + j] with parent row row0 + parent; the log-prob slab row
+// of a record is hist0 + parent.
+__device__ __forceinline__ void select_step(const BeamState& s, int img, int t, int live, int kl, int row0, int hist0, const float* __restrict__ top_val,
+                                            const int* __restrict__ top_idx, const int* pen, int n_pen, float lambda, int penalty_kind,
+                                            float penalty_alpha, double* __restrict__ done_p) {
     const int lane = threadIdx.x;
     const int b = s.beam, T = s.T;
-    const int ncand = live * b;
+    const int ncand = live * kl;
     // each lane owns candidates lane, lane+32, ... (ncand <= 256)
     float cv[8];
     int cf[8];
@@ -42,10 +45,15 @@ __global__ void __launch_bounds__(32) beam_step_kernel(BeamState s, int t, int l
         cv[u] = -INFINITY;
         cf[u] = 0x7fffffff;
         if (c < ncand) {
-            const int pb = c / b, k = c % b;
-            const long row = (long)img * live + pb;
-            cv[u] = s.sums[(long)img * b + pb] + top_val[row * b + k];      // same fp32 add as CaptionModel.py:79
-            cf[u] = pb * s.V1 + top_idx[row * b + k];                       // flat index into the [live*(V+1)] candidate list
+            const int pb = c / kl, k = c % kl;
+            const long row = (long)row0 + pb;
+            const int w = top_idx[row * kl + k];
+            float v = top_val[row * kl + k];
+            int cnt = 0;
+            for (int q = 0; q < n_pen; ++q) cnt += (pen[q] == w);
+            if (cnt) v = __fsub_rn(v, __fmul_rn((float)cnt, lambda));     // logprobs - change * diversity_lambda
+            cv[u] = s.sums[(long)img * b + pb] + v;                          // same fp32 add as CaptionModel.py:79
+            cf[u] = pb * s.V1 + w;                                           // flat index into the [live*(V+1)] candidate list
         }
     }
     const int* seq_old = (t & 1) ? s.seq_b : s.seq_a;
@@ -100,13 +108,13 @@ __global__ void __launch_bounds__(32) beam_step_kernel(BeamState s, int t, int l
             if (sh_slot[j] < 0) continue;
             const long rec = ((long)img * b * T + sh_slot[j]) * T, src = ((long)img * b + sh_parent[j]) * T;
             s.done_seq[rec + q] = (q < t) ? seq_old[src + q] : sh_word[j];
-            s.done_hist[rec + q] = (q < t) ? hist_old[src + q] : img * live + sh_parent[j];
+            s.done_hist[rec + q] = (q < t) ? hist_old[src + q] : hist0 + sh_parent[j];
         }
     }
     if (has) {
         const long dst = ((long)img * b + lane) * T;
         seq_new[dst + t] = word;
-        hist_new[dst + t] = img * live + parent;
+        hist_new[dst + t] = hist0 + parent;
         float new_sum = my_v;
         if (ended) {
             const long rec = (long)img * b * T + slot;
@@ -117,9 +125,43 @@ __global__ void __launch_bounds__(32) beam_step_kernel(BeamState s, int t, int l
         }
         s.sums[(long)img * b + lane] = new_sum;
         s.tokens[(long)img * b + lane] = word;
-        s.src_row[(long)img * b + lane] = img * live + parent;
+        s.src_row[(long)img * b + lane] = row0 + parent;
     }
     if (lane == 0 && em != 0u) s.done_cnt[img] = cnt0 + __popc(em);
+}
+
+// one warp per image
+__global__ void __launch_bounds__(32) beam_step_kernel(BeamState s, int t, int live, const float* __restrict__ top_val,
+                                                       const int* __restrict__ top_idx, int penalty_kind, float penalty_alpha,
+                                                       double* __restrict__ done_p) {
+    const int img = blockIdx.x;
+    select_step(s, img, t, live, s.beam, img * live, img * live, top_val, top_idx, nullptr, 0, 0.f, penalty_kind, penalty_alpha, done_p);
+}
+
+// one warp per real image; its groups step in order, each seeing the words the earlier groups chose at this global step
+__global__ void __launch_bounds__(32) diverse_beam_step_kernel(BeamState s, int G, int t, int k, const float* __restrict__ top_val,
+                                                               const int* __restrict__ top_idx, float lambda, int rows_total, int penalty_kind,
+                                                               float penalty_alpha, double* __restrict__ done_p) {
+    const int i = blockIdx.x, lane = threadIdx.x;
+    const int b = s.beam, T = s.T;
+    __shared__ int sh_pen[MAXB];
+    for (int g = 0; g < G && g <= t; ++g) {
+        const int lt = t - g;              // the group's local time
+        if (lt >= T) continue;             // finished group
+        const int n_pen = g * b;
+        __syncwarp();                      // the previous group's table writes and shared-memory reads are complete
+        if (lane < n_pen) {
+            const int pg = lane / b, j = lane - pg * b;
+            const int last = min(t - pg, T - 1);       // the last local step of earlier group pg (taken at this t unless it has finished)
+            const int* seq_pg = (last & 1) ? s.seq_a : s.seq_b;
+            sh_pen[lane] = seq_pg[((long)(i * G + pg) * b + j) * T + lt];
+        }
+        __syncwarp();
+        const int vimg = i * G + g;
+        // the group's first step reads the one bos row of the group (its row j = 0), like the B-row first step of beam_step
+        select_step(s, vimg, lt, lt == 0 ? 1 : b, k, vimg * b, g * rows_total + vimg * b, top_val, top_idx, sh_pen, n_pen, lambda, penalty_kind,
+                    penalty_alpha, done_p);
+    }
 }
 
 // one warp per image: stable selection of the `keep` best records by penalised score (CaptionModel.py:207)
@@ -172,10 +214,13 @@ __global__ void __launch_bounds__(32) beam_finalize_kernel(BeamState s, int keep
 // Decode edits on a per-row candidate list (beam search): the vocabulary kernel delivered the k_in best raw candidates of every row;
 // drop / lower the edited ones exactly as the reference edits the log-prob row (CaptionModel.py:154-162) and keep the `beam` best.
 // k_in = beam + (number of active edit kinds) guarantees that `beam` unedited candidates remain.  One thread per row.
+// Rows with (r % first_beam) / first_group_rows == first_group (diverse beam search: the group starting at this step) are at their first step.
 __global__ void beam_edit_kernel(int rows, int k_in, int beam, int t, DecodeEdits ed, const int* __restrict__ prev_tokens,
-                                 const float* __restrict__ val_in, const int* __restrict__ idx_in, float* __restrict__ val_out, int* __restrict__ idx_out) {
+                                 const float* __restrict__ val_in, const int* __restrict__ idx_in, float* __restrict__ val_out, int* __restrict__ idx_out,
+                                 int first_beam, int first_group_rows, int first_group) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= rows) return;
+    if (first_beam > 0 && (r % first_beam) / first_group_rows == first_group) t = 0;
     float v[MAXB];
     int ix[MAXB];
     const int prev = (t > 0 && prev_tokens != nullptr) ? prev_tokens[r] : -1;
@@ -203,10 +248,11 @@ __global__ void beam_edit_kernel(int rows, int k_in, int beam, int t, DecodeEdit
     }
 }
 
-__global__ void scale_rows_kernel(float* __restrict__ x, long ld, int rows, int cols, float f) {
+__global__ void scale_rows_kernel(float* __restrict__ x, long ld, int rows, int cols, float f, int skip_beam, int skip_group_rows, int skip_group) {
     const long total = (long)rows * cols;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
         const long r = i / cols, c = i % cols;
+        if (skip_beam > 0 && (int)(r % skip_beam) / skip_group_rows == skip_group) continue;
         x[r * ld + c] *= f;
     }
 }
@@ -278,19 +324,20 @@ __global__ void gather_rows_kernel(const float* __restrict__ slab, long step_str
 }  // namespace
 
 int beam_edit_launch(int rows, int k_in, int beam, int t, const DecodeEdits& ed, const int* prev_tokens, const float* val_in, const int* idx_in,
-                     float* val_out, int* idx_out, cudaStream_t stream) {
+                     float* val_out, int* idx_out, cudaStream_t stream, int first_beam, int first_group_rows, int first_group) {
     CAPB_REQUIRE(k_in >= beam && k_in <= MAXB, "beam_size + number of active decode edits must be <= 16");
     if (rows <= 0) return 0;
-    beam_edit_kernel<<<cdiv(rows, 128), 128, 0, stream>>>(rows, k_in, beam, t, ed, prev_tokens, val_in, idx_in, val_out, idx_out);
+    beam_edit_kernel<<<cdiv(rows, 128), 128, 0, stream>>>(rows, k_in, beam, t, ed, prev_tokens, val_in, idx_in, val_out, idx_out, first_beam,
+                                                          first_group_rows, first_group);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-int scale_rows_launch(float* x, long ld, int rows, int cols, float factor, cudaStream_t stream) {
+int scale_rows_launch(float* x, long ld, int rows, int cols, float factor, cudaStream_t stream, int skip_beam, int skip_group_rows, int skip_group) {
     if (rows <= 0 || cols <= 0) return 0;
     long blocks = ((long)rows * cols + 255) / 256;
     if (blocks > sm_count() * 16) blocks = sm_count() * 16;
-    scale_rows_kernel<<<(int)blocks, 256, 0, stream>>>(x, ld, rows, cols, factor);
+    scale_rows_kernel<<<(int)blocks, 256, 0, stream>>>(x, ld, rows, cols, factor, skip_beam, skip_group_rows, skip_group);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -300,6 +347,17 @@ int beam_step_launch(const BeamState& s, int t, int live, const float* top_val, 
     CAPB_REQUIRE(s.beam >= 1 && s.beam <= MAXB, "beam size 1..16");
     CAPB_REQUIRE(s.beam * s.T <= MAXB * 64, "beam*T record capacity");
     beam_step_kernel<<<s.B, 32, 0, stream>>>(s, t, live, top_val, top_idx, penalty_kind, penalty_alpha, s.done_p);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int diverse_beam_step_launch(const BeamState& s, int G, int t, int k, const float* top_val, const int* top_idx, float lambda, int rows_total,
+                             int penalty_kind, float penalty_alpha, cudaStream_t stream) {
+    CAPB_REQUIRE(G >= 2 && s.beam >= 1 && G * s.beam <= MAXB, "group_size * beams per group must be in 2..16");
+    CAPB_REQUIRE(k >= s.beam && k <= MAXB && s.beam * k <= 256, "candidate list width");
+    CAPB_REQUIRE(s.beam * s.T <= MAXB * 64, "beam*T record capacity");
+    CAPB_REQUIRE(lambda >= 0.f, "diversity_lambda must be >= 0 (the candidate lists rely on the penalty only lowering values)");
+    diverse_beam_step_kernel<<<s.B / G, 32, 0, stream>>>(s, G, t, k, top_val, top_idx, lambda, rows_total, penalty_kind, penalty_alpha, s.done_p);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -535,8 +535,7 @@ void capb200_engine_destroy(capb200_engine* e) {
     for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
     cudaFree(e->wblock);
     cudaFree(e->ws);
-    if (e->d.loop_exec) cudaGraphExecDestroy(e->d.loop_exec);
-    cudaFree(e->d.slab);
+    e->d.release();
     cudaFree(e->tape);
     e->sg.destroy();
     tf32_context_destroy(e->tf32);
@@ -714,6 +713,31 @@ int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, co
     return beam_decode_driver(e->d, V1, T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
                               done_raw, core, &e->launches, st, e->profiling ? 0ull : loop_graph_key(e->ws, e->wblock, mask, R, (int)e->cfg.family),
                               to_edits(opts->edits), opts->temperature);
+}
+
+int capb200_decode_beam_diverse(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
+                                long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
+    if (check_ready(e)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CAPB_REQUIRE(opts != nullptr && fc != nullptr && seq != nullptr, "null argument");
+    // NewFC picks its fresh-state pass (the image embedding step) per core call, not per row, so its groups cannot start at different steps
+    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_UPDOWN, "diverse beam search runs on UpDown (NewFC's fresh-state pass is chosen per call, not per row)");
+    if (opts->group_size == 1) return capb200_decode_beam(e, fc, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream);
+    const int beam = opts->base.beam_size;
+    CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= e->V1, "beam_size must be in 2..16 and <= V+1");
+    CAPB_REQUIRE(B >= 1, "empty batch");
+    CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
+    const int rows = B * beam;
+    if (ensure_workspace(e, B, rows, R, beam, st)) return 1;
+    if (prepare(e, fc, att, mask, B, R, st)) return 1;
+    e->core_cur = 0;
+    auto core = [&](int nrows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
+        return core_step(e, nrows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
+    };
+    return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
+                                      opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
+                                      e->profiling ? 0ull : loop_graph_key(e->ws, e->wblock, mask, R, (int)e->cfg.family), to_edits(opts->base.edits),
+                                      opts->base.temperature);
 }
 
 int capb200_beam_record_logprobs(capb200_engine* e, int image, int rank, float* dst, void* stream) {

@@ -111,6 +111,12 @@ struct DecodeBuffers {
     float *rec_p = nullptr, *rec_raw = nullptr, *tmp_p = nullptr, *tmp_raw = nullptr;
     float* slab = nullptr;            // separately allocated: [T, rows, V1] raw logits of a beam search
     size_t slab_bytes = 0;
+    // diverse beam search: separately allocated, grown on demand: [T + G - 1, rows] row statistics and [B * G] record counts
+    float2* dbs_stats = nullptr;
+    size_t dbs_stats_bytes = 0;
+    int* dbs_done_cnt = nullptr;
+    size_t dbs_done_bytes = 0;
+    const float2* last_stats = nullptr;   // row statistics of the last beam decode (slab_stats or dbs_stats)
     long slab_step_stride = 0;
     int last_B = 0, last_beam = 0;
     DecodeEdits last_edits;           // edits of the last beam decode (re-applied when a finished beam's rows are materialised later)
@@ -120,6 +126,15 @@ struct DecodeBuffers {
     unsigned long long loop_key[8] = {0, 0, 0, 0, 0, 0, 0, 0}, seen_key[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     long loop_launches = 0;
     bool graph_broken = false;
+
+    void release() {
+        if (loop_exec) cudaGraphExecDestroy(loop_exec);
+        loop_exec = nullptr;
+        cudaFree(slab);
+        cudaFree(dbs_stats);
+        cudaFree(dbs_done_cnt);
+        slab = nullptr; dbs_stats = nullptr; dbs_done_cnt = nullptr;
+    }
 
     void carve(Arena& a, int B, int rows, int beam, int T) {
         tokens = a.take<int>(rows);
@@ -177,6 +192,58 @@ inline unsigned long long loop_graph_key(const void* ws, const void* wblock, con
     return h | 1ull;
 }
 
+// grows a separately allocated device buffer to at least `need` bytes (contents are not kept)
+inline int grow_buffer(void** p, size_t* bytes, size_t need, cudaStream_t st) {
+    if (need <= *bytes) return 0;
+    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
+    if (*p) CAPB_CHECK_CUDA(cudaFree(*p));
+    *p = nullptr;
+    *bytes = 0;
+    CAPB_CHECK_CUDA(cudaMalloc(p, need));
+    *bytes = need;
+    return 0;
+}
+
+// Runs a beam loop (`run_loop` enqueues every launch of it on `st`): eagerly the first time `key` is seen, captured into a CUDA graph the
+// second time, replayed from the graph afterwards.  `key` covers everything the captured launches depend on.
+template <class Loop>
+int run_beam_loop(DecodeBuffers& d, const unsigned long long (&key)[8], bool use_graph, long* launches, cudaStream_t st, Loop run_loop) {
+    static const bool graphs_off = getenv("CAPB200_NO_GRAPH") != nullptr;
+    const bool debug = getenv("CAPB200_GRAPH_DEBUG") != nullptr;
+    const bool try_graph = use_graph && !graphs_off && !d.graph_broken;
+    if (try_graph && d.loop_exec != nullptr && memcmp(key, d.loop_key, sizeof(key)) == 0) {
+        CAPB_CHECK_CUDA(cudaGraphLaunch(d.loop_exec, st));
+        *launches += d.loop_launches;
+        if (debug) fprintf(stderr, "capb200: beam loop replayed from its CUDA graph\n");
+    } else if (try_graph && memcmp(key, d.seen_key, sizeof(key)) == 0) {
+        // second decode with this configuration: every lazy initialisation has happened, capture the loop and replay it from now on
+        if (d.loop_exec != nullptr) { cudaGraphExecDestroy(d.loop_exec); d.loop_exec = nullptr; }
+        const long l0 = *launches;
+        cudaGraph_t graph = nullptr;
+        bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+        const int rc = ok ? run_loop() : 1;
+        if (ok) ok = cudaStreamEndCapture(st, &graph) == cudaSuccess && graph != nullptr && rc == 0;
+        if (ok) ok = cudaGraphInstantiate(&d.loop_exec, graph, 0) == cudaSuccess;
+        if (graph != nullptr) cudaGraphDestroy(graph);
+        if (!ok) {
+            (void)cudaGetLastError();
+            d.loop_exec = nullptr;
+            d.graph_broken = true;          // fall back to eager launches for good
+            *launches = l0;
+            if (run_loop()) return 1;
+        } else {
+            d.loop_launches = *launches - l0;
+            memcpy(d.loop_key, key, sizeof(key));
+            CAPB_CHECK_CUDA(cudaGraphLaunch(d.loop_exec, st));
+            if (debug) fprintf(stderr, "capb200: beam loop captured into a CUDA graph (%ld launches)\n", d.loop_launches);
+        }
+    } else {
+        memcpy(d.seen_key, key, sizeof(key));
+        if (run_loop()) return 1;
+    }
+    return 0;
+}
+
 template <class CoreFn>
 int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int keep, int penalty_kind, float penalty_alpha, long long* seq,
                        float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, CoreFn core, long* launches,
@@ -188,14 +255,7 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
     CAPB_REQUIRE(k_in <= 16, "beam_size + number of active decode edits (decoding_constraint, remove_bad_endings, UNK suppression) must be <= 16");
     if (temperature == 0.f) temperature = 1.0f;
     CAPB_REQUIRE(temperature > 0.f, "temperature must be positive");
-    const size_t slab_need = (size_t)T * rows * V1 * sizeof(float);
-    if (slab_need > d.slab_bytes) {
-        CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-        if (d.slab) CAPB_CHECK_CUDA(cudaFree(d.slab));
-        d.slab = nullptr;
-        CAPB_CHECK_CUDA(cudaMalloc(&d.slab, slab_need));
-        d.slab_bytes = slab_need;
-    }
+    if (grow_buffer(reinterpret_cast<void**>(&d.slab), &d.slab_bytes, (size_t)T * rows * V1 * sizeof(float), st)) return 1;
     d.slab_step_stride = (long)rows * V1;
     d.last_B = B;
     d.last_beam = beam;
@@ -242,36 +302,8 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
     key[5] ^= ((unsigned long long)(ed.constraint & 1) << 8) ^ ((unsigned long long)(unsigned)(ed.unk_col + 1) << 16) ^ ((unsigned long long)ed.n_bad << 48);
     key[0] ^= (unsigned long long)reinterpret_cast<uintptr_t>(ed.bad) * 0x9E3779B97F4A7C15ull;
     d.last_edits = ed;
-    static const bool graphs_off = getenv("CAPB200_NO_GRAPH") != nullptr;
-    const bool try_graph = graph_key != 0 && !graphs_off && !d.graph_broken;
-    if (try_graph && d.loop_exec != nullptr && memcmp(key, d.loop_key, sizeof(key)) == 0) {
-        CAPB_CHECK_CUDA(cudaGraphLaunch(d.loop_exec, st));
-        *launches += d.loop_launches;
-    } else if (try_graph && memcmp(key, d.seen_key, sizeof(key)) == 0) {
-        // second decode with this configuration: every lazy initialisation has happened, capture the loop and replay it from now on
-        if (d.loop_exec != nullptr) { cudaGraphExecDestroy(d.loop_exec); d.loop_exec = nullptr; }
-        const long l0 = *launches;
-        cudaGraph_t graph = nullptr;
-        bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-        const int rc = ok ? run_loop() : 1;
-        if (ok) ok = cudaStreamEndCapture(st, &graph) == cudaSuccess && graph != nullptr && rc == 0;
-        if (ok) ok = cudaGraphInstantiate(&d.loop_exec, graph, 0) == cudaSuccess;
-        if (graph != nullptr) cudaGraphDestroy(graph);
-        if (!ok) {
-            (void)cudaGetLastError();
-            d.loop_exec = nullptr;
-            d.graph_broken = true;          // fall back to eager launches for good
-            *launches = l0;
-            if (run_loop()) return 1;
-        } else {
-            d.loop_launches = *launches - l0;
-            memcpy(d.loop_key, key, sizeof(key));
-            CAPB_CHECK_CUDA(cudaGraphLaunch(d.loop_exec, st));
-        }
-    } else {
-        memcpy(d.seen_key, key, sizeof(key));
-        if (run_loop()) return 1;
-    }
+    d.last_stats = d.slab_stats;
+    if (run_beam_loop(d, key, graph_key != 0, launches, st, run_loop)) return 1;
     // all finished beams of every image, best first
     CAPB_NVTX("capb200 beam finalize + log-prob rows");
     if (beam_finalize_launch(s, beam, d.rec_seq, d.rec_len, d.rec_p, d.rec_raw, d.rec_hist, st)) return 1;
@@ -297,10 +329,113 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
     return 0;
 }
 
+// Diverse beam search (AttModel._sample_beam + CaptionModel.beam_search with group_size G > 1): G groups of bdash = beam / G beams, group g
+// running its own beam search staggered by g steps, lowered by lambda for every earlier group's beam that holds the same word at the same
+// position.  Rows are image-major, row = i*beam + g*bdash + j, and every global step t = 0 .. T+G-2 runs ONE core call over all B*beam rows:
+// the rows of groups g >= t are fed <bos> with a fresh state (src_row -1), so a group starting at t == g finds exactly the <bos> step's
+// logits in each of its rows, and the rows of groups g < t are fed their chosen word and parent.  Group g's position-p logits are slab step
+// p + g: its records' slab rows are g*rows + row, which gather_logprob_rows addresses as slab step p and row statistic p*rows + (g*rows + row).
+// The records of (image i, group g) form virtual image i*G + g, so the finalize over B*G virtual images of bdash beams writes done_* in the
+// reference's order: each group's records sorted by score, the groups concatenated (CaptionModel.py:207-208).
+template <class CoreFn>
+int diverse_beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int G, float lambda, int keep, int penalty_kind, float penalty_alpha,
+                               long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, CoreFn core,
+                               long* launches, cudaStream_t st, unsigned long long graph_key, const DecodeEdits& ed, float temperature) {
+    CAPB_REQUIRE(G >= 2 && beam % G == 0, "diverse beam search needs group_size >= 2 dividing beam_size");
+    CAPB_REQUIRE(lambda >= 0.f, "diversity_lambda must be >= 0");
+    const int bdash = beam / G, rows = B * beam, steps = T + G - 1;
+    CAPB_REQUIRE(keep == 1 || keep == bdash, "sample_n must be 1 or beam_size / group_size (AttModel.py:223)");
+    const bool edits = ed.any();
+    const int k_in = beam + ed.kinds();
+    CAPB_REQUIRE(!ed.trigrams, "block_trigrams applies to _sample only (AttModel.py:306)");
+    CAPB_REQUIRE(k_in <= 16, "beam_size + number of active decode edits (decoding_constraint, remove_bad_endings, UNK suppression) must be <= 16");
+    if (temperature == 0.f) temperature = 1.0f;
+    CAPB_REQUIRE(temperature > 0.f, "temperature must be positive");
+    if (grow_buffer(reinterpret_cast<void**>(&d.slab), &d.slab_bytes, (size_t)steps * rows * V1 * sizeof(float), st)) return 1;
+    if (grow_buffer(reinterpret_cast<void**>(&d.dbs_stats), &d.dbs_stats_bytes, (size_t)steps * rows * sizeof(float2), st)) return 1;
+    if (grow_buffer(reinterpret_cast<void**>(&d.dbs_done_cnt), &d.dbs_done_bytes, (size_t)B * G * sizeof(int), st)) return 1;
+    d.slab_step_stride = (long)rows * V1;
+    d.last_B = B;
+    d.last_beam = beam;
+    d.last_edits = ed;
+    d.last_stats = d.dbs_stats;
+    BeamState s = d.bs;              // B*G virtual images of bdash beams over the same [B*beam]-sized tables
+    s.B = B * G; s.beam = bdash; s.T = T; s.V1 = V1;
+    s.done_cnt = d.dbs_done_cnt;
+    auto run_loop = [&]() -> int {
+        CAPB_NVTX("capb200 diverse beam loop (T+G-1 steps: core, vocab stats, group steps)");
+        CAPB_CHECK_CUDA(cudaMemsetAsync(s.sums, 0, sizeof(float) * rows, st));
+        CAPB_CHECK_CUDA(cudaMemsetAsync(s.done_cnt, 0, sizeof(int) * B * G, st));
+        CAPB_CHECK_CUDA(cudaMemsetAsync(d.tokens, 0, sizeof(int) * rows, st));          // <bos> = 0
+        CAPB_CHECK_CUDA(cudaMemsetAsync(d.src_row, 0xff, sizeof(int) * rows, st));     // -1: fresh zero state until a group starts
+        for (int t = 0; t < steps; ++t) {
+            float* logits = d.slab + (long)t * d.slab_step_stride;
+            if (core(rows, beam, d.tokens, d.src_row, t, logits, (long)V1)) return 1;
+            // group t (if any) is at its first step: one log_softmax, no temperature; every other row as at t > 0 of the plain search
+            if (t > 0 && temperature != 1.0f) {
+                if (scale_rows_launch(logits, V1, rows, V1, 1.0f / temperature, st, beam, bdash, t)) return 1;
+                *launches += 1;
+            }
+            VocabStepArgs va;
+            va.rows = rows; va.V1 = V1; va.logits = logits; va.ld = V1;
+            va.twice = (t > 0) ? 1 : 0;
+            va.first_beam = beam; va.first_group_rows = bdash; va.first_group = t;
+            va.topk = edits ? k_in : beam; va.top_val = d.top_val; va.top_idx = d.top_idx;
+            va.stats = d.dbs_stats + (long)t * rows;
+            if (vocab_step_launch(va, st)) return 1;
+            const float* tv = d.top_val;
+            const int* ti = d.top_idx;
+            if (edits) {
+                if (beam_edit_launch(rows, k_in, beam, t, ed, d.tokens, d.top_val, d.top_idx, d.top_val_e, d.top_idx_e, st, beam, bdash, t)) return 1;
+                tv = d.top_val_e; ti = d.top_idx_e;
+                *launches += 1;
+            }
+            // the candidate lists hold each row's `beam` best: the penalty lowers at most (G-1)*bdash words, so they contain its bdash best
+            if (diverse_beam_step_launch(s, G, t, beam, tv, ti, lambda, rows, penalty_kind, penalty_alpha, st)) return 1;
+            *launches += 2;
+        }
+        return 0;
+    };
+    unsigned long long key[8] = {graph_key, (unsigned long long)B, (unsigned long long)beam, (unsigned long long)T, (unsigned long long)V1,
+                                 (unsigned long long)penalty_kind, 0ull, (unsigned long long)reinterpret_cast<uintptr_t>(d.slab)};
+    memcpy(&key[6], &penalty_alpha, sizeof(float));
+    memcpy(reinterpret_cast<char*>(&key[6]) + 4, &temperature, sizeof(float));
+    key[5] ^= ((unsigned long long)(ed.constraint & 1) << 8) ^ ((unsigned long long)(unsigned)(ed.unk_col + 1) << 16) ^ ((unsigned long long)ed.n_bad << 48);
+    key[0] ^= (unsigned long long)reinterpret_cast<uintptr_t>(ed.bad) * 0x9E3779B97F4A7C15ull;
+    // a diverse loop never replays a plain one (or one of another group count / lambda) with the same shapes
+    unsigned lambda_bits = 0;
+    memcpy(&lambda_bits, &lambda, sizeof(float));
+    key[3] ^= (1ull << 63) ^ ((unsigned long long)G << 40);
+    key[1] ^= (unsigned long long)lambda_bits << 32;
+    key[4] ^= (unsigned long long)reinterpret_cast<uintptr_t>(d.dbs_stats) * 0x9E3779B97F4A7C15ull;
+    key[2] ^= (unsigned long long)reinterpret_cast<uintptr_t>(d.dbs_done_cnt) << 8;
+    if (run_beam_loop(d, key, graph_key != 0, launches, st, run_loop)) return 1;
+
+    CAPB_NVTX("capb200 diverse beam finalize + log-prob rows");
+    if (beam_finalize_launch(s, bdash, d.rec_seq, d.rec_len, d.rec_p, d.rec_raw, d.rec_hist, st)) return 1;
+    *launches += 1;
+    // seq[k] = done_beams[k][0] (group 0's best) for k < B; with sample_n == bdash the rows B .. B*sample_n-1 stay pad with zero log-probs
+    // (AttModel.py:241-254 only fills all sample_n rows when sample_n == beam_size)
+    CAPB_CHECK_CUDA(cudaMemcpy2DAsync(seq, sizeof(long long) * T, d.rec_seq, sizeof(long long) * beam * T, sizeof(long long) * T, B,
+                                      cudaMemcpyDeviceToDevice, st));
+    if (keep > 1) CAPB_CHECK_CUDA(cudaMemsetAsync(seq + (long)B * T, 0, sizeof(long long) * (long)B * (keep - 1) * T, st));
+    if (seq_logprobs) {
+        CAPB_CHECK_CUDA(cudaMemcpy2DAsync(d.out_hist, sizeof(int) * T, d.rec_hist, sizeof(int) * beam * T, sizeof(int) * T, B, cudaMemcpyDeviceToDevice, st));
+        *launches += 1;
+        if (gather_logprob_rows_launch(d.slab, d.slab_step_stride, V1, d.out_hist, B, T, V1, seq_logprobs, d.dbs_stats, rows, st, seq, &ed)) return 1;
+        if (keep > 1) CAPB_CHECK_CUDA(cudaMemsetAsync(seq_logprobs + (long)B * T * V1, 0, sizeof(float) * (long)B * (keep - 1) * T * V1, st));
+    }
+    if (done_seq) CAPB_CHECK_CUDA(cudaMemcpyAsync(done_seq, d.rec_seq, sizeof(long long) * rows * T, cudaMemcpyDeviceToDevice, st));
+    if (done_len) CAPB_CHECK_CUDA(cudaMemcpyAsync(done_len, d.rec_len, sizeof(int) * rows, cudaMemcpyDeviceToDevice, st));
+    if (done_p) CAPB_CHECK_CUDA(cudaMemcpyAsync(done_p, d.rec_p, sizeof(float) * rows, cudaMemcpyDeviceToDevice, st));
+    if (done_raw) CAPB_CHECK_CUDA(cudaMemcpyAsync(done_raw, d.rec_raw, sizeof(float) * rows, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
 inline int beam_record_logprobs(DecodeBuffers& d, int V1, int T, int image, int rank, float* dst, cudaStream_t st) {
     CAPB_REQUIRE(d.slab != nullptr && image >= 0 && image < d.last_B && rank >= 0 && rank < d.last_beam, "no such finished beam");
     return gather_logprob_rows_launch(d.slab, d.slab_step_stride, V1, d.rec_hist + ((long)image * d.last_beam + rank) * T, 1, T, V1, dst,
-                                      d.slab_stats, (long)d.last_B * d.last_beam, st, d.rec_seq + ((long)image * d.last_beam + rank) * T, &d.last_edits);
+                                      d.last_stats, (long)d.last_B * d.last_beam, st, d.rec_seq + ((long)image * d.last_beam + rank) * T, &d.last_edits);
 }
 
 // AttModel._sample (greedy / multinomial / forced replay) and AttModel._forward (teacher forcing); method codes = CAPB200_SAMPLE_*

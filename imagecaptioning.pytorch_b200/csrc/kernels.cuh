@@ -80,12 +80,21 @@ struct VocabStepArgs {
     int t = 0;
     float* picked_lp = nullptr;   // optional: picked_lp[row * ld_picked] = log-prob of the chosen token
     long ld_picked = 1;
+    // diverse beam search (image-major rows, `first_beam` rows per image in groups of `first_group_rows`): the rows of group `first_group`
+    // are at their group's first step and get a single log_softmax (the shared init_logprobs, AttModel.py:239); off when first_beam == 0
+    int first_beam = 0, first_group_rows = 1, first_group = -1;
+    __host__ __device__ int row_twice(int r) const {
+        return twice && !(first_beam > 0 && (r % first_beam) / first_group_rows == first_group);
+    }
 };
 int vocab_step_launch(const VocabStepArgs& a, cudaStream_t stream);
-// beam search with decode edits: the per-row candidate list [rows, k_in] (k_in = beam + edits.kinds()) is edited and cut to [rows, beam]
+// beam search with decode edits: the per-row candidate list [rows, k_in] (k_in = beam + edits.kinds()) is edited and cut to [rows, beam];
+// first_* as in VocabStepArgs (those rows are edited as at step 0)
 int beam_edit_launch(int rows, int k_in, int beam, int t, const DecodeEdits& ed, const int* prev_tokens, const float* val_in, const int* idx_in,
-                     float* val_out, int* idx_out, cudaStream_t stream);
-int scale_rows_launch(float* x, long ld, int rows, int cols, float factor, cudaStream_t stream);
+                     float* val_out, int* idx_out, cudaStream_t stream, int first_beam = 0, int first_group_rows = 1, int first_group = -1);
+// x[r, :] *= factor; with skip_beam > 0 the rows r with (r % skip_beam) / skip_group_rows == skip_group are left alone (diverse beam search)
+int scale_rows_launch(float* x, long ld, int rows, int cols, float factor, cudaStream_t stream, int skip_beam = 0, int skip_group_rows = 1,
+                      int skip_group = -1);
 
 // ---- beam.cu
 struct BeamState {
@@ -106,6 +115,13 @@ struct BeamState {
 };
 int beam_step_launch(const BeamState& s, int t, int live, const float* top_val, const int* top_idx, int penalty_kind, float penalty_alpha,
                      cudaStream_t stream);
+// Diverse beam search, global step t (CaptionModel.py:35-209 with G = group_size groups of bdash = s.beam beams, staggered by one step per group).
+// `s` describes B*G virtual images of bdash beams (virtual image i*G + g = group g of image i, rows i*G*bdash + g*bdash + j); every group
+// active at t (0 <= t - g < T) takes one step in group order: its candidates [rows, k] (k = G*bdash per row) are lowered by lambda times the
+// number of earlier groups' beams of the same image holding that word at position t - g, then merged as in beam_step.  Slab rows are
+// recorded as g * rows_total + row (the step-(t - g) slab of group g is slab step t).
+int diverse_beam_step_launch(const BeamState& s, int G, int t, int k, const float* top_val, const int* top_idx, float lambda, int rows_total,
+                             int penalty_kind, float penalty_alpha, cudaStream_t stream);
 // sorts each image's finished beams by score, writes the best `keep` records:
 //   out_seq [B*keep, T] int64, out_len/out_p [B*keep], out_hist [B*keep, T] (slab rows, -1 beyond length)
 int beam_finalize_launch(const BeamState& s, int keep, long long* out_seq, int* out_len, float* out_p, float* out_raw, int* out_hist,

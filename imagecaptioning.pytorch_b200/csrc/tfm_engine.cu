@@ -281,8 +281,7 @@ void capb200_tfm_destroy(capb200_tfm_engine* e) {
     if (e->ev_fork) cudaEventDestroy(e->ev_fork);
     if (e->ev_join) cudaEventDestroy(e->ev_join);
     if (e->side) cudaStreamDestroy(e->side);
-    if (e->d.loop_exec) cudaGraphExecDestroy(e->d.loop_exec);
-    cudaFree(e->d.slab);
+    e->d.release();
     delete e;
 }
 

@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(NT) vocab_step_kernel(const VocabStepArgs a) {
     // Second log_softmax (beam search, CaptionModel.py:204): its max is m2 = -lsum, so exp(lp - m2) = exp(x - mx) term by term and
     // its normaliser is the first pass's `sum` again (up to one rounding, ~1e-7 on the log-prob); no second exp pass is needed.
     const float l2 = lsum;
-    if (a.twice) {
+    if (a.row_twice(r)) {
         for (int v = threadIdx.x; v < V1; v += NT) g[v] = (row[v] - m2) - l2;
     } else {
         for (int v = threadIdx.x; v < V1; v += NT) g[v] = row[v];
@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(NT) vocab_step_kernel(const VocabStepArgs a) {
         }
         if (k == 0) greedy_tok = oi;
         if (a.topk > 0 && threadIdx.x == 0) {
-            a.top_val[(long)r * a.topk + k] = a.twice ? (ov - m2) - l2 : ov;
+            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (ov - m2) - l2 : ov;
             a.top_idx[(long)r * a.topk + k] = oi;
         }
     }
@@ -339,7 +339,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_kernel(const VocabStepArgs a) 
         }
         if (threadIdx.x == 0) {
             const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.twice ? (lp - m2) - l2 : lp;
+            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
             a.top_idx[(long)r * a.topk + k] = oi;
         }
     }
@@ -414,7 +414,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_online_kernel(const VocabStepA
         }
         if (threadIdx.x == 0) {
             const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.twice ? (lp - m2) - l2 : lp;
+            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
             a.top_idx[(long)r * a.topk + k] = oi;
         }
     }
@@ -530,7 +530,7 @@ __global__ void __launch_bounds__(VT2) vocab_stats_online128_kernel(const VocabS
         }
         if (threadIdx.x == 0) {
             const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.twice ? (lp - m2) - l2 : lp;
+            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
             a.top_idx[(long)r * a.topk + k] = oi;
         }
     }
@@ -599,7 +599,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_reg_kernel(const VocabStepArgs
         }
         if (threadIdx.x == 0) {
             const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.twice ? (lp - m2) - l2 : lp;
+            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
             a.top_idx[(long)r * a.topk + k] = oi;
         }
     }
@@ -701,7 +701,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_stream_kernel(const VocabStepA
             }
             if (threadIdx.x == 0) {
                 const float lp = (ov - mx) - lsum;
-                a.top_val[(long)r * a.topk + k] = a.twice ? (lp - m2) - l2 : lp;
+                a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
                 a.top_idx[(long)r * a.topk + k] = oi;
             }
         }

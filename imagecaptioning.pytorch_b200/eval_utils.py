@@ -86,8 +86,9 @@ def caption_stats(seq: torch.Tensor, seq_logprobs: torch.Tensor):
 def eval_split_n(model, n_predictions, input_data, eval_kwargs: Dict[str, Any] = {}):
     """Contract of captioning/utils/eval_utils.py:230-283: ``sample_n`` captions per image, appended to ``n_predictions``.
     ``sample_n_method`` 'bs' (the sample_n best beams), 'sample' / 'gumbel' / 'top<k>' / 'top<p>' (sample_n draws, with their perplexity:
-    read back with ONE transfer for the batch instead of one .item() per caption).  'dbs' and the remaining branch are diverse beam
-    search (group_size > 1), which the engine refuses; the model's own NotImplementedError surfaces."""
+    read back with ONE transfer for the batch instead of one .item() per caption).  'dbs' is diverse beam search: sample_n groups of
+    beam_size beams, one caption per group (each group's best), on the engine for UpDown and AoANet.  The remaining branch is diverse
+    sampling (group_size > 1 with beam_size 1), which the engine refuses; the model's own NotImplementedError surfaces."""
     verbose = eval_kwargs.get('verbose', True)
     beam_size = eval_kwargs.get('beam_size', 1)
     sample_n = eval_kwargs.get('sample_n', 1)

@@ -290,9 +290,25 @@ class B200CaptionModel(nn.Module):
             att_masks = att_masks[:, :max_len]
         return self._f32(att_feats), self._f32(att_masks)
 
-    def _check_opts(self, opt):
-        if opt.get('group_size', 1) != 1:
-            raise NotImplementedError('diverse beam search (group_size > 1) is out of scope of the engine (SURVEY.md section 8f)')
+    # why a family has no diverse beam search (None: it has one)
+    _no_diverse = None
+
+    def _check_opts(self, opt, beam_size=None, sample_n=None):
+        """Refuses what the engine does not run, before any device work.  beam_size / sample_n: the values _sample_beam reads (None: the
+        call is not a beam search)."""
+        group_size = opt.get('group_size', 1)
+        if group_size != 1:
+            if beam_size is None or beam_size <= 1:
+                raise NotImplementedError('diverse sampling (group_size > 1 with beam_size 1, AttModel._diverse_sample) is out of scope of the engine')
+            if self._no_diverse is not None:
+                raise NotImplementedError('diverse beam search is not implemented for %s: %s' % (self.family_name, self._no_diverse))
+            if group_size < 1 or beam_size % group_size != 0:
+                raise NotImplementedError('diverse beam search needs group_size dividing beam_size (got %r, %r)' % (beam_size, group_size))
+            if sample_n not in (1, beam_size // group_size):
+                raise NotImplementedError('diverse beam search returns sample_n = 1 or beam_size // group_size captions per image (AttModel.py:223)')
+            if float(opt.get('diversity_lambda', 0.5)) < 0:
+                raise NotImplementedError('diverse beam search needs diversity_lambda >= 0 on the engine (its candidate lists rely on the '
+                                          'penalty only lowering log-probs)')
         if opt.get('output_logsoftmax', 1) != 1:
             raise NotImplementedError('output_logsoftmax=0 is out of scope of the engine')
 
@@ -322,9 +338,9 @@ class B200CaptionModel(nn.Module):
         beam_size = opt.get('beam_size', 1)
         temperature = float(opt.get('temperature', 1.0))
         sample_n = int(opt.get('sample_n', 1))
-        self._check_opts(opt)
         if beam_size > 1 and sample_method in ('greedy', 'beam_search'):
             return self._sample_beam(fc_feats, att_feats, att_masks, opt)
+        self._check_opts(opt)
         top = 0.0
         if forced_tokens is not None:
             method = _lib.SAMPLE_FORCED
@@ -371,6 +387,10 @@ class B200CaptionModel(nn.Module):
         return lib.capb200_decode_beam(self._engine, _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(bo), _lib.ptr(seq),
                                        _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
 
+    def _call_beam_diverse(self, lib, fc, att, masks, B, R, do, seq, logprobs, d_seq, d_len, d_p, d_raw):
+        return lib.capb200_decode_beam_diverse(self._engine, _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(do), _lib.ptr(seq),
+                                               _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
+
     def _call_record(self, lib, image, rank, dst):
         return lib.capb200_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
 
@@ -383,8 +403,10 @@ class B200CaptionModel(nn.Module):
     def _sample_beam(self, fc_feats, att_feats, att_masks=None, opt={}):
         beam_size = opt.get('beam_size', 10)
         sample_n = opt.get('sample_n', 10)
-        self._check_opts(opt)
-        assert sample_n == 1 or sample_n == beam_size, 'when beam search, sample_n == 1 or beam search'
+        group_size = opt.get('group_size', 1)
+        self._check_opts(opt, beam_size, sample_n)
+        if group_size == 1:
+            assert sample_n == 1 or sample_n == beam_size, 'when beam search, sample_n == 1 or beam search'
         assert beam_size <= self.vocab_size + 1
         n_kinds = int(bool(opt.get('decoding_constraint', 0))) + int(bool(opt.get('remove_bad_endings', 0)) and bool(self.bad_endings_ix)) + \
             int((bool(opt.get('suppress_UNK', 0)) and self.vocab.get(str(self.vocab_size)) == 'UNK') or self.unk_idx is not None)
@@ -408,7 +430,11 @@ class B200CaptionModel(nn.Module):
         d_raw = torch.empty(B, beam_size, dtype=torch.float32, device=dev)
         edits, keep_bad = self._decode_edits(opt, dev, beam=True)
         bo = _lib.BeamOpts(beam_size, sample_n, _PENALTY[kind], float(alpha), float(opt.get('temperature', 1.0)), edits)
-        _lib.check(self._call_beam(lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw), 'decode_beam')
+        if group_size == 1:
+            _lib.check(self._call_beam(lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw), 'decode_beam')
+        else:       # done_beams[i]: each group's bdash best in group order (CaptionModel.py:207-208)
+            do = _lib.DiverseOpts(bo, group_size, float(opt.get('diversity_lambda', 0.5)))
+            _lib.check(self._call_beam_diverse(lib, fc, att, masks, B, R, do, seq, logprobs, d_seq, d_len, d_p, d_raw), 'decode_beam_diverse')
         self._last_beam = (d_seq, d_len, d_p, d_raw)
         self.done_beams = _LazyDoneBeams(self, B, beam_size)
         return seq, logprobs
@@ -630,6 +656,8 @@ class B200NewFCModel(B200CaptionModel):
 
     family = _lib.FAMILY_NEWFC
     family_name = 'newfc'
+    _no_diverse = ("the engine chooses NewFC's fresh-state pass (the image-embedding step, AttModel.py:925-936) per core call, not per row, "
+                   "so its groups cannot start at different steps")
 
     def __init__(self, opt, numeric_mode=None):
         super().__init__(opt, numeric_mode)
@@ -682,6 +710,7 @@ class B200TransformerModel(B200CaptionModel):
     model.tgt_embed.1.pe buffer, model.generator.proj.*).  Decoding keeps a per-layer K/V cache on the device."""
 
     family_name = 'transformer'
+    _no_diverse = 'the decoder K/V cache and positional encoding take one position per launch, so its groups cannot be at different positions'
 
     def __init__(self, opt, numeric_mode=None):
         super().__init__(opt, numeric_mode)
@@ -1140,6 +1169,11 @@ class B200AoAModel(B200CaptionModel):
     def _call_beam(self, lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw):
         return lib.capb200_aoa_decode_beam(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(bo), _lib.ptr(seq), _lib.ptr(logprobs),
                                            _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
+
+    def _call_beam_diverse(self, lib, fc, att, masks, B, R, do, seq, logprobs, d_seq, d_len, d_p, d_raw):
+        return lib.capb200_aoa_decode_beam_diverse(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(do), _lib.ptr(seq),
+                                                   _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw),
+                                                   _lib.current_stream())
 
     def _call_record(self, lib, image, rank, dst):
         return lib.capb200_aoa_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())

@@ -145,6 +145,21 @@ int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, co
  * (done_beams[image][rank]['logps'], CaptionModel.py:192); dst must hold T*(V+1) floats, rows beyond the length are zeroed. */
 int capb200_beam_record_logprobs(capb200_engine* e, int image, int rank, float* dst, void* stream);
 
+typedef struct {
+    capb200_beam_opts base;   /* beam_size = group_size * bdash (bdash beams per group); sample_n 1 or bdash (AttModel.py:223) */
+    int group_size;           /* G >= 2, dividing beam_size */
+    float diversity_lambda;   /* >= 0: a candidate word loses lambda for every beam of an earlier group holding it at the same position */
+} capb200_diverse_opts;
+
+/* Diverse beam search: AttModel._sample_beam + CaptionModel.beam_search with group_size > 1 (CaptionModel.py:35-209), UpDown only.
+ * Same output contract as capb200_decode_beam, except:
+ *   done_*[B, beam]: for each group in order, its bdash best finished beams by score (the reference's group-concatenated done_beams);
+ *   seq / seq_logprobs rows k < B: done_beams[k][0] (group 0's best); with sample_n == bdash the rows B .. B*sample_n-1 are pad / zero
+ *   (AttModel.py:241-254 fills every sample_n row only when sample_n == beam_size).
+ * capb200_beam_record_logprobs reads the records of the last call (rank in 0..beam-1, group order). */
+int capb200_decode_beam_diverse(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
+                                long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream);
+
 #define CAPB200_SAMPLE_GREEDY 0
 #define CAPB200_SAMPLE_MULTINOMIAL 1
 #define CAPB200_SAMPLE_FORCED 2  /* replay given tokens (parity checks against another sampler's draw) */
@@ -253,6 +268,9 @@ int capb200_aoa_bind_weights(capb200_aoa_engine* e, const capb200_aoa_weights* w
 int capb200_aoa_decode_beam(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq,
                             float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream);
 int capb200_aoa_beam_record_logprobs(capb200_aoa_engine* e, int image, int rank, float* dst, void* stream);
+/* same contract as capb200_decode_beam_diverse */
+int capb200_aoa_decode_beam_diverse(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
+                                    long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream);
 int capb200_aoa_decode_sample(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_sample_opts* opts,
                               const long long* tokens_in, long ld_tok, long long* seq, float* seq_logprobs, float* picked, void* stream);
 long capb200_aoa_launch_count(const capb200_aoa_engine* e);
