@@ -14,7 +14,7 @@ MODE_SIMT_FP32, MODE_TC_F16X3, MODE_TC_F16X1 = 0, 1, 2
 MODES = {'simt_fp32': MODE_SIMT_FP32, 'tc_f16x3': MODE_TC_F16X3, 'tc_f16x1': MODE_TC_F16X1}
 # capb200_linear additionally exposes the training step's split-K GEMM variants
 OP_MODES = dict(MODES, skinny_tf32x3=3, skinny_fp32=4, tf32x3_tc=5, tf32x3_tc_dgrad=6, tf32x3_tc_wgrad=7)
-FAMILY_UPDOWN, FAMILY_NEWFC = 0, 1
+FAMILY_UPDOWN, FAMILY_NEWFC, FAMILY_ATT2IN2 = 0, 1, 2
 SAMPLE_GREEDY, SAMPLE_MULTINOMIAL, SAMPLE_FORCED, SAMPLE_TEACHER, SAMPLE_TOPK, SAMPLE_TOPP = 0, 1, 2, 3, 4, 5
 
 
@@ -25,7 +25,7 @@ class ModelCfg(Structure):
 
 WEIGHT_FIELDS = ['embed', 'fc_embed_w', 'fc_embed_b', 'att_embed_w', 'att_embed_b', 'ctx2att_w', 'ctx2att_b', 'logit_w', 'logit_b',
                  'att_lstm_w_ih', 'att_lstm_w_hh', 'att_lstm_b_ih', 'att_lstm_b_hh', 'lang_lstm_w_ih', 'lang_lstm_w_hh', 'lang_lstm_b_ih',
-                 'lang_lstm_b_hh', 'h2att_w', 'h2att_b', 'alpha_w', 'alpha_b', 'i2h_w', 'i2h_b', 'h2h_w', 'h2h_b']
+                 'lang_lstm_b_hh', 'h2att_w', 'h2att_b', 'alpha_w', 'alpha_b', 'i2h_w', 'i2h_b', 'h2h_w', 'h2h_b', 'a2c_w', 'a2c_b']
 
 
 class Weights(Structure):
@@ -96,6 +96,14 @@ GRAD_FIELDS = ['embed', 'fc_embed_w', 'fc_embed_b', 'att_embed_w', 'att_embed_b'
 
 class UpdownGrads(Structure):
     _fields_ = [(f, c_void_p) for f in GRAD_FIELDS]
+
+
+ATT2IN2_GRAD_FIELDS = ['embed', 'att_embed_w', 'att_embed_b', 'ctx2att_w', 'ctx2att_b', 'logit_w', 'logit_b', 'h2att_w', 'h2att_b', 'alpha_w', 'alpha_b',
+                       'i2h_w', 'i2h_b', 'h2h_w', 'h2h_b', 'a2c_w', 'a2c_b']
+
+
+class Att2in2Grads(Structure):
+    _fields_ = [(f, c_void_p) for f in ATT2IN2_GRAD_FIELDS]
 
 
 TFM_MAX_LAYERS = 8
@@ -205,6 +213,10 @@ SIGNATURES = {
     'capb200_aoa_launch_count': (c_long, [c_void_p]),
     'capb200_updown_scst_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), c_void_p, c_void_p, c_void_p, c_int,
                                          POINTER(UpdownGrads), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_att2in2_scst_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), c_void_p, c_void_p, c_void_p, c_int,
+                                          POINTER(Att2in2Grads), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_att2in2_xe_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), c_void_p, c_void_p, c_int, POINTER(Att2in2Grads),
+                                        c_void_p, c_void_p, c_void_p]),
     'capb200_dropout_mask': (c_int, [c_void_p, c_long, c_ulonglong, c_int, c_int, c_float, c_void_p]),
     'capb200_tfm_xe_step': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmXeOpts), c_void_p, c_void_p, c_int, POINTER(TfmWeights), c_void_p, c_void_p,
                                     c_void_p]),

@@ -74,8 +74,9 @@ __global__ void iota_div_kernel(int* p, int n, int div) {
 }
 
 
-enum GemmId { G_FC = 0, G_ATT, G_CTX, G_GFC, G_LSTM1, G_H2ATT, G_LSTM2, G_LOGIT, G_CORE, G_LSTM2A, G_LSTM2B, G_COUNT };
-constexpr int G_REPORTED = 9;      // ids exposed through capb200_engine_read_profile (the split language-LSTM launches are folded into G_LSTM2)
+enum GemmId { G_FC = 0, G_ATT, G_CTX, G_GFC, G_LSTM1, G_H2ATT, G_LSTM2, G_LOGIT, G_CORE, G_LSTM2A, G_LSTM2B, G_A2C, G_COUNT };
+constexpr int G_REPORTED = 9;      // ids exposed through capb200_engine_read_profile (the split language-LSTM launches are folded into G_LSTM2,
+                                   // Att2in2's a2c launch into G_CORE)
 
 }  // namespace
 }  // namespace capb200
@@ -100,7 +101,7 @@ struct capb200_engine {
     float* xgate = nullptr;          // [V+1, 4H] relu(embed) * W_ih[:, 2H:]^T: per-token gate contribution (eval-mode decode)
     long ld_xgate = 0;
     bool use_xgate = true;
-    Planes p_fc, p_attw, p_ctx, p_logit, p_a_ih_h, p_a_ih_fc, p_a_ih_x, p_a_hh, p_l_ih_a, p_l_ih_h, p_l_hh, p_h2att, p_i2h, p_h2h;
+    Planes p_fc, p_attw, p_ctx, p_logit, p_a_ih_h, p_a_ih_fc, p_a_ih_x, p_a_hh, p_l_ih_a, p_l_ih_h, p_l_hh, p_h2att, p_i2h, p_h2h, p_a2c;
 
     // workspace (owned)
     char* ws = nullptr;
@@ -172,12 +173,22 @@ void layout_weights(capb200_engine* e, Arena& a) {
         e->p_l_ih_h = carve_planes(a, 4 * H, H);
         e->p_l_hh = carve_planes(a, 4 * H, H);
         e->p_h2att = carve_planes(a, A, H);
+    } else if (e->cfg.family == CAPB200_FAMILY_ATT2IN2) {
+        e->p_attw = carve_planes(a, H, e->cfg.att_feat_size);
+        e->p_ctx = carve_planes(a, A, H);
+        e->p_h2att = carve_planes(a, A, H);
+        e->p_i2h = carve_planes(a, 5 * H, E);
+        e->p_h2h = carve_planes(a, 5 * H, H);
+        e->p_a2c = carve_planes(a, 2 * H, H);
     } else {
         e->p_fc = carve_planes(a, E, e->cfg.fc_feat_size);
         e->p_i2h = carve_planes(a, 5 * H, E);
         e->p_h2h = carve_planes(a, 5 * H, H);
     }
 }
+
+// the families that attend over the regions (UpDown, Att2in2); NewFC reads the fc features only
+bool attends(const capb200_engine* e) { return e->cfg.family != CAPB200_FAMILY_NEWFC; }
 
 int pack(capb200_engine* e, const float* w, long ldw, int rows, int cols, const Planes& p, cudaStream_t st) {
     e->launches++;
@@ -192,20 +203,23 @@ int pack_gates(capb200_engine* e, const float* w, long ldw, int H, int cols, con
 void layout_workspace(capb200_engine* e, Arena& a, int B, int rows, int R, int beam) {
     const int H = e->H, E = e->E, A = e->A, T = e->T;
     const bool updown = e->cfg.family == CAPB200_FAMILY_UPDOWN;
+    const bool attn = attends(e);
     const bool tc = e->tc;
     if (tc) {
         e->in_fc = carve_planes(a, B, e->cfg.fc_feat_size);
-        if (updown) e->in_att = carve_planes(a, (long)B * R, e->cfg.att_feat_size);
+        if (attn) e->in_att = carve_planes(a, (long)B * R, e->cfg.att_feat_size);
     }
     e->fc_e.carve(a, B, updown ? H : E, tc);
-    if (updown) {
+    if (attn) {
         e->att_e.carve(a, (long)B * R, H, tc);
         e->p_att.carve(a, (long)B * R, A, false);
+        e->att_res.carve(a, rows, H, tc);
+        e->att_h.carve(a, rows, A, false);
+    }
+    if (updown) {
         e->g_fc.carve(a, B, 4 * H, false);
         e->h1_in.carve(a, rows, H, tc);
         e->h1_out.carve(a, rows, H, tc);
-        e->att_res.carve(a, rows, H, tc);
-        e->att_h.carve(a, rows, A, false);
     }
     e->xt.carve(a, rows, E, tc);
     e->h0_in.carve(a, rows, H, tc);
@@ -283,11 +297,11 @@ int prepare(capb200_engine* e, const float* fc, const float* att, const float* m
     const bool updown = e->cfg.family == CAPB200_FAMILY_UPDOWN;
     const capb200_weights& w = e->w;
     ActView fc_in;  fc_in.f = const_cast<float*>(fc);  fc_in.ld = e->cfg.fc_feat_size;
-    if (e->tc) {
+    if (e->tc && e->cfg.family != CAPB200_FAMILY_ATT2IN2) {
         e->launches++;
         if (split_planes_launch(fc, e->cfg.fc_feat_size, B, e->cfg.fc_feat_size, e->in_fc.hi, e->in_fc.lo, e->in_fc.ld, st)) return 1;
     }
-    {   // fc_embed: Linear (+ReLU for the attention models; NewFC has a bare Linear, AttModel.py:907)
+    if (e->cfg.family != CAPB200_FAMILY_ATT2IN2) {   // fc_embed: Linear (+ReLU for UpDown; NewFC has a bare Linear, AttModel.py:907; Att2in2 has none, :858)
         GemmProblem g;
         g.M = B; g.N = updown ? H : E; g.nseg = 1;
         g.seg[0] = seg_of(fc_in, w.fc_embed_w, e->cfg.fc_feat_size, e->p_fc, e->cfg.fc_feat_size);
@@ -296,7 +310,7 @@ int prepare(capb200_engine* e, const float* fc, const float* att, const float* m
         g.epi.C = e->fc_e.v.f; g.epi.ldc = e->fc_e.v.ld; g.epi.C_hi = e->fc_e.v.hi; g.epi.C_lo = e->fc_e.v.lo; g.epi.ldcs = e->fc_e.v.ld;
         if (run_gemm(e, G_FC, g, e->capB, st)) return 1;
     }
-    if (!updown) return 0;
+    if (!attends(e)) return 0;
     ActView att_in; att_in.f = const_cast<float*>(att); att_in.ld = e->cfg.att_feat_size;
     if (e->tc) {
         e->launches++;
@@ -323,6 +337,7 @@ int prepare(capb200_engine* e, const float* fc, const float* att, const float* m
         g.epi.C = e->p_att.v.f; g.epi.ldc = e->p_att.v.ld;
         if (run_gemm(e, G_CTX, g, e->capB * e->capR, st)) return 1;
     }
+    if (!updown) return 0;
     {   // time-invariant part of the attention-LSTM gates: fc' * W_ih[:, H:2H]^T + b_ih + b_hh
         GemmProblem g;
         g.M = B; g.N = 4 * H; g.nseg = 1;
@@ -441,6 +456,52 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
         }
         return 0;
     }
+    if (e->cfg.family == CAPB200_FAMILY_ATT2IN2) {
+        // ---- Att2in2 (AttModel.py:770-790): attention on the PREVIOUS h, maxout cell whose candidate pair also gets a2c(att_res).
+        // A fresh row (src_row < 0) gathers h = 0, so its att_h is the h2att bias and the cell sees c = 0.
+        StateCopy s0, s1;
+        s0.src = e->h0_out.v.f; s0.ld_src = e->h0_out.v.ld; s0.dst = e->h0_in.v;
+        e->launches++;
+        if (state_gather_embed_launch(rows, tokens, src_row, w.embed, E, E, 1, e->xt.v, H, 1, s0, s1, st)) return 1;
+        const int cur = e->core_cur, nxt = cur ^ 1;
+        {   // h2att on h_prev
+            GemmProblem g;
+            g.M = rows; g.N = A; g.nseg = 1;
+            g.seg[0] = seg_of(e->h0_in.v, w.h2att_w, H, e->p_h2att, H);
+            g.epi.bias = w.h2att_b;
+            g.epi.C = e->att_h.v.f; g.epi.ldc = e->att_h.v.ld;
+            if (run_gemm(e, G_H2ATT, g, e->capRows, st)) return 1;
+        }
+        e->launches += 2;
+        if (additive_attention_launch(n_images, rpi, R, A, H, e->att_h.v.f, e->att_h.v.ld, e->p_att.v.f, e->p_att.v.ld, e->att_e.v.f, e->att_e.v.ld,
+                                      mask, R, w.alpha_w, w.alpha_b, e->att_score, e->att_res.v, st)) return 1;
+        {   // sums = [xt | h_prev] [i2h | h2h]^T + (i2h_b + h2h_b + [0 | a2c_b])
+            GemmProblem g;
+            g.M = rows; g.N = 5 * H; g.nseg = 2;
+            g.seg[0] = seg_of(e->xt.v, w.i2h_w, E, e->p_i2h, E);
+            g.seg[1] = seg_of(e->h0_in.v, w.h2h_w, H, e->p_h2h, H);
+            g.epi.bias = e->bsum_core;
+            g.epi.C = e->gates.v.f; g.epi.ldc = e->gates.v.ld;
+            if (run_gemm(e, G_CORE, g, e->capRows, st)) return 1;
+        }
+        {   // sums[:, 3H:5H] += att_res a2c^T  (in place through the residual epilogue)
+            GemmProblem g;
+            g.M = rows; g.N = 2 * H; g.nseg = 1;
+            g.seg[0] = seg_of(e->att_res.v, w.a2c_w, H, e->p_a2c, H);
+            g.epi.residual = e->gates.v.f + 3 * H; g.epi.ld_res = e->gates.v.ld;
+            g.epi.C = e->gates.v.f + 3 * H; g.epi.ldc = e->gates.v.ld;
+            if (run_gemm(e, G_A2C, g, e->capRows, st)) return 1;
+        }
+        e->launches++;
+        if (maxout_pointwise_launch(rows, H, e->gates.v.f, e->gates.v.ld, src_row, e->c0[cur], e->ld_c, e->c0[nxt], e->ld_c, e->h0_out.v, st)) return 1;
+        e->core_cur = nxt;
+        GemmProblem g;
+        g.M = rows; g.N = V1; g.nseg = 1;
+        g.seg[0] = seg_of(e->h0_out.v, w.logit_w, H, e->p_logit, H);
+        g.epi.bias = w.logit_b;
+        g.epi.C = logits; g.epi.ldc = ld_logits;
+        return run_gemm(e, G_LOGIT, g, e->capRows, st);
+    }
     // ---- NewFC: maxout LSTM; a fresh state first consumes the image embedding (AttModel.py:925-936)
     const bool fresh = (src_row == e->d.neg1);
     for (int pass = fresh ? 0 : 1; pass < 2; ++pass) {
@@ -503,7 +564,10 @@ int capb200_range_status(int reset) { return range_flag_read(reset); }
 
 capb200_engine* capb200_engine_create(const capb200_model_cfg* cfg) {
     if (cfg == nullptr) { set_error("null cfg"); return nullptr; }
-    if (cfg->family != CAPB200_FAMILY_UPDOWN && cfg->family != CAPB200_FAMILY_NEWFC) { set_error("unknown model family"); return nullptr; }
+    if (cfg->family != CAPB200_FAMILY_UPDOWN && cfg->family != CAPB200_FAMILY_NEWFC && cfg->family != CAPB200_FAMILY_ATT2IN2) {
+        set_error("unknown model family");
+        return nullptr;
+    }
     if (cfg->numeric_mode < 0 || cfg->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
     if (cfg->seq_length < 1 || cfg->seq_length > 64) { set_error("seq_length must be in 1..64"); return nullptr; }
     int ndev = 0;
@@ -568,8 +632,9 @@ int capb200_engine_read_profile(capb200_engine* e, int reset, double* ms, double
     e->ev_ids.clear();
     e->ev_flops.clear();
     e->ev_used = 0;
-    for (int i = G_LSTM2A; i <= G_LSTM2B; ++i) {       // the split language-LSTM launches report under the language-LSTM id
-        e->prof_ms[G_LSTM2] += e->prof_ms[i]; e->prof_flops[G_LSTM2] += e->prof_flops[i]; e->prof_calls[G_LSTM2] += e->prof_calls[i];
+    for (int i = G_LSTM2A; i <= G_A2C; ++i) {       // the split language-LSTM launches report under the language-LSTM id, a2c under the core id
+        const int to = i == G_A2C ? G_CORE : G_LSTM2;
+        e->prof_ms[to] += e->prof_ms[i]; e->prof_flops[to] += e->prof_flops[i]; e->prof_calls[to] += e->prof_calls[i];
         e->prof_ms[i] = 0; e->prof_flops[i] = 0; e->prof_calls[i] = 0;
     }
     for (int i = 0; i < G_REPORTED; ++i) {
@@ -585,8 +650,12 @@ int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, voi
     CAPB_REQUIRE(e != nullptr && w != nullptr, "null argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool updown = e->cfg.family == CAPB200_FAMILY_UPDOWN;
-    CAPB_REQUIRE(w->embed && w->fc_embed_w && w->fc_embed_b && w->logit_w && w->logit_b, "missing shared weights");
-    if (updown) {
+    const bool att2in2 = e->cfg.family == CAPB200_FAMILY_ATT2IN2;
+    CAPB_REQUIRE(w->embed && (att2in2 || (w->fc_embed_w && w->fc_embed_b)) && w->logit_w && w->logit_b, "missing shared weights");
+    if (att2in2) {
+        CAPB_REQUIRE(w->att_embed_w && w->att_embed_b && w->ctx2att_w && w->ctx2att_b && w->h2att_w && w->h2att_b && w->alpha_w && w->alpha_b &&
+                         w->i2h_w && w->i2h_b && w->h2h_w && w->h2h_b && w->a2c_w && w->a2c_b, "missing Att2in2 weights");
+    } else if (updown) {
         CAPB_REQUIRE(w->att_embed_w && w->att_embed_b && w->ctx2att_w && w->ctx2att_b && w->att_lstm_w_ih && w->att_lstm_w_hh && w->att_lstm_b_ih &&
                          w->att_lstm_b_hh && w->lang_lstm_w_ih && w->lang_lstm_w_hh && w->lang_lstm_b_ih && w->lang_lstm_b_hh && w->h2att_w &&
                          w->h2att_b && w->alpha_w && w->alpha_b, "missing UpDown weights");
@@ -614,6 +683,10 @@ int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, voi
     } else {
         add_vec_kernel<<<cdiv(5 * H, 256), 256, 0, st>>>(w->i2h_b, w->h2h_b, e->bsum_core, 5 * H);
         e->launches += 1;
+        if (att2in2) {     // the a2c bias joins the candidate columns' bias: the a2c GEMM then needs no bias of its own
+            add_vec_kernel<<<cdiv(2 * H, 256), 256, 0, st>>>(e->bsum_core + 3 * H, w->a2c_b, e->bsum_core + 3 * H, 2 * H);
+            e->launches += 1;
+        }
     }
     CAPB_CHECK_CUDA(cudaGetLastError());
     if (e->tc) {
@@ -630,6 +703,13 @@ int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, voi
             rc |= pack_gates(e, w->lang_lstm_w_ih + H, 2 * H, H, H, e->p_l_ih_h, st);
             rc |= pack_gates(e, w->lang_lstm_w_hh, H, H, H, e->p_l_hh, st);
             rc |= pack(e, w->h2att_w, H, A, H, e->p_h2att, st);
+        } else if (att2in2) {
+            rc |= pack(e, w->att_embed_w, e->cfg.att_feat_size, H, e->cfg.att_feat_size, e->p_attw, st);
+            rc |= pack(e, w->ctx2att_w, H, A, H, e->p_ctx, st);
+            rc |= pack(e, w->h2att_w, H, A, H, e->p_h2att, st);
+            rc |= pack(e, w->i2h_w, E, 5 * H, E, e->p_i2h, st);
+            rc |= pack(e, w->h2h_w, H, 5 * H, H, e->p_h2h, st);
+            rc |= pack(e, w->a2c_w, H, 2 * H, H, e->p_a2c, st);
         } else {
             rc |= pack(e, w->fc_embed_w, e->cfg.fc_feat_size, E, e->cfg.fc_feat_size, e->p_fc, st);
             rc |= pack(e, w->i2h_w, E, 5 * H, E, e->p_i2h, st);
@@ -693,18 +773,18 @@ int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, co
                         long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
     if (check_ready(e)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && fc != nullptr && seq != nullptr, "null argument");
+    CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq != nullptr, "null argument");
     const int beam = opts->beam_size, keep = opts->sample_n;
     CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= e->V1, "beam_size must be in 1..16 and <= V+1");
     CAPB_REQUIRE(keep == 1 || keep == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
     CAPB_REQUIRE(B >= 1, "empty batch");
-    const bool updown = e->cfg.family == CAPB200_FAMILY_UPDOWN;
-    if (updown) CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
-    if (!updown) R = 1;
+    const bool attn = attends(e);
+    if (attn) CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
+    if (!attn) R = 1;
     const int T = e->T, V1 = e->V1;
     const int rows = B * beam;
     if (ensure_workspace(e, B, rows, R, beam, st)) return 1;
-    if (!updown) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, 1); e->launches++; }
+    if (!attn) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, 1); e->launches++; }
     if (prepare(e, fc, att, mask, B, R, st)) return 1;
     e->core_cur = 0;
     auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
@@ -719,9 +799,9 @@ int capb200_decode_beam_diverse(capb200_engine* e, const float* fc, const float*
                                 long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
     if (check_ready(e)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && fc != nullptr && seq != nullptr, "null argument");
+    CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq != nullptr, "null argument");
     // NewFC picks its fresh-state pass (the image embedding step) per core call, not per row, so its groups cannot start at different steps
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_UPDOWN, "diverse beam search runs on UpDown (NewFC's fresh-state pass is chosen per call, not per row)");
+    CAPB_REQUIRE(attends(e), "diverse beam search runs on UpDown and Att2in2 (NewFC's fresh-state pass is chosen per call, not per row)");
     if (opts->group_size == 1) return capb200_decode_beam(e, fc, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream);
     const int beam = opts->base.beam_size;
     CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= e->V1, "beam_size must be in 2..16 and <= V+1");
@@ -749,12 +829,12 @@ int capb200_decode_sample(capb200_engine* e, const float* fc, const float* att, 
                           const long long* tokens_in, long ld_tok, long long* seq, float* seq_logprobs, float* picked, void* stream) {
     if (check_ready(e)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && fc != nullptr && seq_logprobs != nullptr, "null argument");
+    CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq_logprobs != nullptr, "null argument");
     const int n = opts->sample_n;
     CAPB_REQUIRE(n >= 1 && B >= 1, "empty batch");
-    const bool updown = e->cfg.family == CAPB200_FAMILY_UPDOWN;
-    if (updown) CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
-    if (!updown) R = 1;
+    const bool attn = attends(e);
+    if (attn) CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
+    if (!attn) R = 1;
     const int method = opts->method;
     CAPB_REQUIRE(method >= 0 && method <= 5, "unknown sampling method");
     if (method == CAPB200_SAMPLE_FORCED || method == CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(tokens_in != nullptr && ld_tok >= 1, "token matrix required");
@@ -766,7 +846,7 @@ int capb200_decode_sample(capb200_engine* e, const float* fc, const float* att, 
     const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : T;
     CAPB_REQUIRE(steps >= 0 && steps <= t_out, "steps out of range");
     if (ensure_workspace(e, B, rows, R, 1, st)) return 1;
-    if (!updown) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, n); e->launches++; }
+    if (!attn) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, n); e->launches++; }
     if (prepare(e, fc, att, mask, B, R, st)) return 1;
     e->core_cur = 0;
     auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
@@ -1056,6 +1136,70 @@ struct TrainArgs {
     float* logprobs = nullptr; float* loss = nullptr;
 };
 
+// Grows the engine's training tape to `need` bytes (synchronises only when it has to reallocate).
+int grow_tape(capb200_engine* e, size_t need, cudaStream_t st) {
+    if (need <= e->tape_bytes) return 0;
+    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
+    if (e->tape) CAPB_CHECK_CUDA(cudaFree(e->tape));
+    e->tape = nullptr;
+    CAPB_CHECK_CUDA(cudaMalloc(&e->tape, need));
+    e->tape_bytes = need;
+    return 0;
+}
+
+// (1) of an SCST step with the greedy baseline: the eval-mode greedy decode (no dropout) on the regular decode path.
+int start_greedy_baseline(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, float* glp, bool* on_side,
+                          cudaStream_t st) {
+    *on_side = false;
+    if (ta.xe || !ta.greedy_baseline) return 0;
+    // The eval-mode greedy baseline (B rows, the regular decode path with its own workspace) and the train-mode sampling forward (B*n rows,
+    // on the tape) are independent chains of small, latency-bound kernels: the baseline runs on a side stream and joins before the reward.
+    CAPB_NVTX("capb200 scst: greedy baseline (eval mode, side stream)");
+    const int T = ta.T;
+    capb200_sample_opts so; memset(&so, 0, sizeof(so)); so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.seed = 0; so.steps = T;
+    cudaStream_t gs = st;
+    static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
+    if (!serial && ensure_side(e)) {
+        CAPB_CHECK_CUDA(cudaEventRecord(e->ev_gfork, st));
+        CAPB_CHECK_CUDA(cudaStreamWaitEvent(e->side, e->ev_gfork, 0));
+        gs = e->side;
+        *on_side = true;
+    }
+    CAPB_CHECK_CUDA(cudaMemsetAsync(glp, 0, sizeof(float) * (size_t)B * T * e->V1, gs));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(ta.greedy_seq, 0, sizeof(long long) * (size_t)B * T, gs));
+    if (capb200_decode_sample(e, fc, att, ta.mask, B, R, &so, nullptr, 0, ta.greedy_seq, glp, nullptr, static_cast<void*>(gs))) return 1;
+    if (*on_side) CAPB_CHECK_CUDA(cudaEventRecord(e->ev_gjoin, e->side));
+    return 0;
+}
+
+// (4) + (5) of a training step: reward and loss (SCST) or the XE criterion, d logits, then the logit layer's backward batched over all (n, t):
+// dOUT [N, T, H] and the logit gradients (group 0, whose event is recorded here).  tp.out holds the dropped-out core outputs [N, T, H].
+int loss_and_logit_backward(capb200_engine* e, const TrainArgs& ta, const Skinny& sk, const Tape& tp, int B, int N, bool greedy_on_side, float* g_logit_w,
+                            float* g_logit_b, cudaStream_t st) {
+    const int T = ta.T, H = e->H, V1 = e->V1;
+    const long TN = (long)T * N;
+    const long ld_lp = (long)ta.Tl * V1;
+    const capb200_weights& w = e->w;
+    if (ta.xe) {
+        if (xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
+                                    tp.mask_sum, tp.item_loss, tp.DL, ta.loss, st, ta.keep, ta.row_loss ? ta.row_loss : tp.row_loss, tp.row_msum, tp.row_coef)) return 1;
+    } else {
+        if (greedy_on_side) CAPB_CHECK_CUDA(cudaStreamWaitEvent(st, e->ev_gjoin, 0));     // join: the reward needs the baseline captions
+        if (cider_reward_launch(ta.table->t, ta.sample_seq, N, ta.greedy_baseline ? ta.greedy_seq : nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores,
+                                ta.reward, T, T, st)) return 1;
+        float* rl = ta.keep > 0 ? (ta.row_loss ? ta.row_loss : tp.row_loss) : nullptr;
+        if (reward_criterion_fwd_launch(ta.logprobs, ld_lp, V1, ta.sample_seq, ta.reward, N, T, ta.loss, rl, tp.mask_sum, st)) return 1;
+        if (ta.keep > 0 && scst_drop_worst_launch(ta.sample_seq, rl, N, T, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, ta.loss, st)) return 1;
+        // ---- (5) backward: logit layer, batched over all (n, t)
+        if (scst_dlogits_launch(ta.logprobs, ld_lp, ta.sample_seq, ta.reward, tp.mask_sum, ta.upstream, N, T, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr)) return 1;
+    }
+    e->launches += 3;
+    if (sk.dgrad((int)TN, H, V1, tp.DL, V1, w.logit_w, H, tp.dOUT, H, 0)) return 1;          // dOUT = DL * W
+    if (sk.wgrad(V1, H, (int)TN, tp.DL, V1, tp.out, H, g_logit_w, H, 0)) return 1;            // dW = DL^T * OUT
+    if (colsum_launch((int)TN, V1, tp.DL, V1, g_logit_b, 0, st)) return 1;
+    return record_group_event(e->grad_events[0], st);                                         // group 0 (logit) is final
+}
+
 int updown_train_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const capb200_updown_grads* grads,
                       cudaStream_t st) {
     void* stream = static_cast<void*>(st);
@@ -1068,43 +1212,15 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     float* const sample_logprobs = ta.logprobs;
     const long ld_lp = (long)ta.Tl * V1;
     long long* const sample_seq = ta.sample_seq;
-    long long* const greedy_seq = ta.greedy_seq;
-    float* const reward = ta.reward;
-    float* const loss = ta.loss;
 
     // ---- (1) greedy baseline, eval mode (no dropout): the regular decode path
-    {
-        Arena dry; Tape t0; layout_tape(t0, dry, B, R, N, T, E, H, A, V1, Fa, Ff);
-        if (dry.off + 256 > e->tape_bytes) {
-            CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-            if (e->tape) CAPB_CHECK_CUDA(cudaFree(e->tape));
-            e->tape = nullptr;
-            CAPB_CHECK_CUDA(cudaMalloc(&e->tape, dry.off + 256));
-            e->tape_bytes = dry.off + 256;
-        }
-    }
+    Arena dry; Tape t0; layout_tape(t0, dry, B, R, N, T, E, H, A, V1, Fa, Ff);
+    if (grow_tape(e, dry.off + 256, st)) return 1;
     Arena ar; ar.base = e->tape;
     Tape tp; layout_tape(tp, ar, B, R, N, T, E, H, A, V1, Fa, Ff);
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;        // decode workspace sized before anything is in flight
     bool greedy_on_side = false;
-    if (!ta.xe && ta.greedy_baseline) {
-        // The eval-mode greedy baseline (B rows, the regular decode path with its own workspace) and the train-mode sampling forward (B*n rows,
-        // on the tape) are independent chains of small, latency-bound kernels: the baseline runs on a side stream and joins before the reward.
-        CAPB_NVTX("capb200 scst: greedy baseline (eval mode, side stream)");
-        capb200_sample_opts so; memset(&so, 0, sizeof(so)); so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.seed = 0; so.steps = T;
-        cudaStream_t gs = st;
-        static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
-        if (!serial && ensure_side(e)) {
-            CAPB_CHECK_CUDA(cudaEventRecord(e->ev_gfork, st));
-            CAPB_CHECK_CUDA(cudaStreamWaitEvent(e->side, e->ev_gfork, 0));
-            gs = e->side;
-            greedy_on_side = true;
-        }
-        CAPB_CHECK_CUDA(cudaMemsetAsync(tp.glp, 0, sizeof(float) * (size_t)B * T * V1, gs));
-        CAPB_CHECK_CUDA(cudaMemsetAsync(greedy_seq, 0, sizeof(long long) * (size_t)B * T, gs));
-        if (capb200_decode_sample(e, fc, att, ta.mask, B, R, &so, nullptr, 0, greedy_seq, tp.glp, nullptr, static_cast<void*>(gs))) return 1;
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaEventRecord(e->ev_gjoin, e->side));
-    }
+    if (start_greedy_baseline(e, fc, att, B, R, ta, tp.glp, &greedy_on_side, st)) return 1;
     if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
     tf32_context_new_step(e->tf32);                                          // the weights may have changed since the last step
     const long tf32_l0 = tf32_context_launches(e->tf32);
@@ -1203,24 +1319,7 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     CAPB_NVTX("capb200 train step: reward, loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_updown_grads& G = *grads;
-    if (ta.xe) {
-        if (xe_loss_backward_launch(sample_logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
-                                    tp.mask_sum, tp.item_loss, tp.DL, loss, st, ta.keep, ta.row_loss ? ta.row_loss : tp.row_loss, tp.row_msum, tp.row_coef)) return 1;
-    } else {
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaStreamWaitEvent(st, e->ev_gjoin, 0));     // join: the reward needs the baseline captions
-        if (cider_reward_launch(ta.table->t, sample_seq, N, ta.greedy_baseline ? greedy_seq : nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores, reward,
-                                T, T, st)) return 1;
-        float* rl = ta.keep > 0 ? (ta.row_loss ? ta.row_loss : tp.row_loss) : nullptr;
-        if (reward_criterion_fwd_launch(sample_logprobs, ld_lp, V1, sample_seq, reward, N, T, loss, rl, tp.mask_sum, st)) return 1;
-        if (ta.keep > 0 && scst_drop_worst_launch(sample_seq, rl, N, T, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, loss, st)) return 1;
-        // ---- (5) backward: logit layer, batched over all (n, t)
-        if (scst_dlogits_launch(sample_logprobs, ld_lp, sample_seq, reward, tp.mask_sum, ta.upstream, N, T, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr)) return 1;
-    }
-    e->launches += 3;
-    if (sk.dgrad((int)TN, H, V1, tp.DL, V1, w.logit_w, H, tp.dOUT, H, 0)) return 1;          // dOUT = DL * W
-    if (sk.wgrad(V1, H, (int)TN, tp.DL, V1, tp.out, H, G.logit_w, H, 0)) return 1;            // dW = DL^T * OUT
-    if (colsum_launch((int)TN, V1, tp.DL, V1, G.logit_b, 0, st)) return 1;
-    if (record_group_event(e->grad_events[0], st)) return 1;                                  // group 0 (logit) is final
+    if (loss_and_logit_backward(e, ta, sk, tp, B, N, greedy_on_side, G.logit_w, G.logit_b, st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh1, 0, sizeof(float) * NH, st));
@@ -1291,6 +1390,175 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     return rc;
 }
 
+// ---- Att2in2 (Att2in2Core, AttModel.py:770-790) ---------------------------------------------------------------------------------------
+// The Tape fields the Att2in2 step uses, sized for its core: g1 / DG1 hold the maxout sums (i, f, o, a, b) and their gradient [T][N][5H];
+// h0 / c0 hold T+1 slots (slot 0 = the zero initial state, slot t+1 = step t), so step t -- and the batched weight gradients of h2h and
+// h2att -- read the previous state from slot t.
+void layout_tape_att2in2(Tape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int A, int V1) {
+    const long TN = (long)T * N, BR = (long)B * R, NH = (long)N * H;
+    tp = Tape{};
+    tp.tok = a.take<int>(TN);
+    tp.xt = a.take<float>(TN * E); tp.g1 = a.take<float>(TN * 5 * H); tp.h0 = a.take<float>(TN * H + NH); tp.c0 = a.take<float>(TN * H + NH);
+    tp.atth = a.take<float>(TN * A); tp.alpha = a.take<float>(TN * R); tp.attres = a.take<float>(TN * H); tp.out = a.take<float>(TN * H);
+    tp.att_e = a.take<float>(BR * H); tp.p_att = a.take<float>(BR * A); tp.glp = a.take<float>((long)B * T * V1);
+    tp.DL = a.take<float>(TN * V1); tp.dOUT = a.take<float>(TN * H); tp.DG1 = a.take<float>(TN * 5 * H); tp.DATTH = a.take<float>(TN * A);
+    tp.dh0 = a.take<float>(NH); tp.dc0 = a.take<float>(NH); tp.tmpH = a.take<float>(NH); tp.dxt = a.take<float>((long)N * E);
+    tp.d_att_e = a.take<float>(BR * H); tp.d_p_att = a.take<float>(BR * A); tp.dpre_att = a.take<float>(BR * H); tp.mask_sum = a.take<float>(8);
+    tp.scores = a.take<double>((long)N + B);
+    tp.dalpha = a.take<float>((long)N * R);
+    tp.item_loss = a.take<float>(TN);
+    tp.skinny_floats = (size_t)4 << 20;
+    tp.skinny = a.take<float>((long)tp.skinny_floats);
+    tp.s_tokens = a.take<int>(N); tp.s_unfinished = a.take<int>(N); tp.s_forced = a.take<int>(N);
+    tp.s_att_score = a.take<float>((long)N * R);
+    tp.row_loss = a.take<float>(N); tp.row_msum = a.take<float>(N); tp.row_coef = a.take<float>(N);
+}
+
+// One Att2in2 training step: the train-mode forward on the tape (dropout sites 1 att_embed, 2 word embedding, 3 core output, as UpDown),
+// the loss, and back-propagation through time.  fc is only handed to the greedy baseline's decode call, which ignores it.
+int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const capb200_att2in2_grads* grads,
+                       cudaStream_t st) {
+    const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, A = e->A, V1 = e->V1, H5 = 5 * H;
+    const int Fa = e->cfg.att_feat_size;
+    const float p = ta.p;
+    const float keep_scale = 1.0f / (1.0f - p);
+    const unsigned long long seed = ta.seed;
+    const capb200_weights& w = e->w;
+    float* const sample_logprobs = ta.logprobs;
+    const long ld_lp = (long)ta.Tl * V1;
+
+    Arena dry; Tape t0; layout_tape_att2in2(t0, dry, B, R, N, T, E, H, A, V1);
+    if (grow_tape(e, dry.off + 256, st)) return 1;
+    Arena ar; ar.base = e->tape;
+    Tape tp; layout_tape_att2in2(tp, ar, B, R, N, T, E, H, A, V1);
+    if (ensure_workspace(e, B, N, R, 1, st)) return 1;
+    bool greedy_on_side = false;
+    if (start_greedy_baseline(e, fc, att, B, R, ta, tp.glp, &greedy_on_side, st)) return 1;
+    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
+    tf32_context_new_step(e->tf32);
+    const long tf32_l0 = tf32_context_launches(e->tf32);
+    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};
+    sk.ctx = e->tf32;
+
+    // ---- train-mode prologue: att_embed (ReLU, dropout site 1, region mask), ctx2att
+    nvtxRangePushA("capb200 att2in2 train step: forward on the tape");
+    const long BR = (long)B * R, NH = (long)N * H;
+    if (sk.lin(att, Fa, w.att_embed_w, Fa, w.att_embed_b, tp.att_e, H, (int)BR, H, Fa, 0)) return 1;
+    if (relu_copy_launch(tp.att_e, BR * H, ActView{tp.att_e, nullptr, nullptr, H}, st)) return 1;
+    if (dropout_apply_launch(tp.att_e, (int)BR, H, H, seed, 1, 0, p, st)) return 1;
+    if (ta.mask != nullptr) {
+        if (mask_rows_launch(ActView{tp.att_e, nullptr, nullptr, H}, B, R, H, ta.mask, R, st)) return 1;
+        e->launches++;
+    }
+    if (sk.lin(tp.att_e, H, w.ctx2att_w, H, w.ctx2att_b, tp.p_att, A, (int)BR, A, H, 0)) return 1;
+    e->launches += 4;
+
+    // ---- T steps with the tape
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.h0, 0, sizeof(float) * NH, st));     // slot 0: h = c = 0
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.c0, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
+    for (int t = 0; t < T; ++t) {
+        int* tok = tp.tok + (long)t * N;
+        if (ta.xe) {
+            if (t >= 1 && ta.ss_prob > 0.f) {      // scheduled sampling (AttModel.py:145-154)
+                if (ss_select_launch(N, V1, sample_logprobs + (long)(t - 1) * V1, ld_lp, ta.labels, ta.ld_labels, t, seed, ta.ss_prob, tok, st)) return 1;
+            } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
+            if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
+        }
+        else CAPB_CHECK_CUDA(cudaMemcpyAsync(tok, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        float* xt = tp.xt + (long)t * N * E;
+        float* sums = tp.g1 + (long)t * N * H5;
+        const float* hp = tp.h0 + (long)t * NH;
+        const float* cp = tp.c0 + (long)t * NH;
+        float *h = tp.h0 + (long)(t + 1) * NH, *c = tp.c0 + (long)(t + 1) * NH;
+        if (embed_relu_dropout_launch(N, E, tok, w.embed, xt, seed, (unsigned)t, p, st)) return 1;
+        // attention on the previous hidden state
+        float* atth = tp.atth + (long)t * N * A;
+        if (sk.lin(hp, H, w.h2att_w, H, w.h2att_b, atth, A, N, A, H, 0)) return 1;
+        float* attres = tp.attres + (long)t * NH;
+        if (additive_attention_launch(B, n, R, A, H, atth, A, tp.p_att, A, tp.att_e, H, ta.mask, R, w.alpha_w, w.alpha_b, tp.s_att_score,
+                                      ActView{attres, nullptr, nullptr, H}, st, tp.alpha + (long)t * N * R)) return 1;
+        {   // sums = xt i2h^T + h_prev h2h^T + (i2h_b + h2h_b + [0 | a2c_b]), then sums[:, 3H:] += att_res a2c^T
+            GemmProblem g; g.M = N; g.N = H5; g.nseg = 2;
+            g.seg[0].A = xt; g.seg[0].lda = E; g.seg[0].W = w.i2h_w; g.seg[0].ldw = E; g.seg[0].K = E;
+            g.seg[1].A = hp; g.seg[1].lda = H; g.seg[1].W = w.h2h_w; g.seg[1].ldw = H; g.seg[1].K = H;
+            g.epi.bias = e->bsum_core;
+            g.epi.C = sums; g.epi.ldc = H5;
+            if (sk.gates(g)) return 1;
+        }
+        if (sk.lin(attres, H, w.a2c_w, H, nullptr, sums + 3 * H, H5, N, 2 * H, H, 1)) return 1;
+        if (maxout_pointwise_launch(N, H, sums, H5, nullptr, cp, H, c, H, ActView{h, nullptr, nullptr, H}, st)) return 1;
+        // core output = dropout(h), stored in (n, t) order for the batched logit backward
+        float* out = tp.out + (long)t * H;
+        if (dropout_copy_launch(h, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
+        float* logits = sample_logprobs + (long)t * V1;
+        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, logits, ld_lp, N, V1, H, 0)) return 1;
+        VocabStepArgs va;
+        va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
+        if (!ta.xe) {
+            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
+            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
+            va.seq_out = ta.sample_seq; va.ld_seq = T; va.t = t;
+            if (ta.forced != nullptr) {
+                if (load_token_column_launch(ta.forced, T, t, N, tp.s_forced, st)) return 1;
+                va.select = 3; va.forced = tp.s_forced;
+            }
+        }
+        if (vocab_step_launch(va, st)) return 1;
+        e->launches += 11;
+    }
+
+    // ---- loss, logit backward, back-propagation through time
+    nvtxRangePop();
+    CAPB_NVTX("capb200 att2in2 train step: loss, backward through time, weight gradients");
+    const long TN = (long)T * N;
+    const capb200_att2in2_grads& G = *grads;
+    if (loss_and_logit_backward(e, ta, sk, tp, B, N, greedy_on_side, G.logit_w, G.logit_b, st)) return 1;
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.d_att_e, 0, sizeof(float) * BR * H, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.d_p_att, 0, sizeof(float) * BR * A, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(G.alpha_w, 0, sizeof(float) * A, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(G.alpha_b, 0, sizeof(float), st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(G.embed, 0, sizeof(float) * (size_t)V1 * E, st));
+    for (int t = T - 1; t >= 0; --t) {
+        const float* sums = tp.g1 + (long)t * N * H5;
+        float* ds = tp.DG1 + (long)t * N * H5;
+        // cell: dh = carried dh + dropout-masked dOUT[:, t]
+        if (maxout_cell_backward_launch(N, H, sums, tp.c0 + (long)t * NH, tp.c0 + (long)(t + 1) * NH, tp.dh0, tp.dOUT + (long)t * H, (long)T * H, 3,
+                                        (unsigned)t, seed, p, tp.dc0, ds, st)) return 1;
+        if (sk.dgrad(N, E, H5, ds, H5, w.i2h_w, E, tp.dxt, E, 0)) return 1;                     // d xt
+        if (sk.dgrad(N, H, H5, ds, H5, w.h2h_w, H, tp.dh0, H, 0)) return 1;                     // d h_prev through h2h (the carried dh is consumed)
+        if (sk.dgrad(N, H, 2 * H, ds + 3 * H, H5, w.a2c_w, H, tp.tmpH, H, 0)) return 1;         // d att_res: a2c only feeds the candidate pair
+        float* datth = tp.DATTH + (long)t * N * A;
+        if (attention_backward_launch(B, n, R, A, H, tp.tmpH, tp.alpha + (long)t * N * R, tp.atth + (long)t * N * A, tp.p_att, tp.att_e, w.alpha_w, datth,
+                                      tp.d_att_e, tp.d_p_att, G.alpha_w, G.alpha_b, tp.dalpha, st)) return 1;
+        if (sk.dgrad(N, H, A, datth, A, w.h2att_w, H, tp.dh0, H, 1)) return 1;                  // + d h_prev through h2att
+        if (embed_backward_launch(N, E, tp.tok + (long)t * N, tp.xt + (long)t * N * E, tp.dxt, E, keep_scale, G.embed, st)) return 1;
+        e->launches += 8;
+    }
+    // weight gradients, batched over time (K = T*N); h0 slots 0..T-1 are the previous states h2h and h2att read
+    int rc = 0;
+    rc |= sk.wgrad(H5, E, (int)TN, tp.DG1, H5, tp.xt, E, G.i2h_w, E, 0);
+    rc |= sk.wgrad(H5, H, (int)TN, tp.DG1, H5, tp.h0, H, G.h2h_w, H, 0);
+    rc |= sk.wgrad(2 * H, H, (int)TN, tp.DG1 + 3 * H, H5, tp.attres, H, G.a2c_w, H, 0);
+    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.i2h_b, 0, st);
+    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.h2h_b, 0, st);
+    rc |= colsum_launch((int)TN, 2 * H, tp.DG1 + 3 * H, H5, G.a2c_b, 0, st);
+    rc |= sk.wgrad(A, H, (int)TN, tp.DATTH, A, tp.h0, H, G.h2att_w, H, 0);
+    rc |= colsum_launch((int)TN, A, tp.DATTH, A, G.h2att_b, 0, st);
+    // prologue
+    rc |= sk.dgrad((int)BR, H, A, tp.d_p_att, A, w.ctx2att_w, H, tp.d_att_e, H, 1);
+    rc |= sk.wgrad(A, H, (int)BR, tp.d_p_att, A, tp.att_e, H, G.ctx2att_w, H, 0);
+    rc |= colsum_launch((int)BR, A, tp.d_p_att, A, G.ctx2att_b, 0, st);
+    rc |= relu_dropout_backward_launch(BR * H, tp.att_e, tp.d_att_e, tp.dpre_att, keep_scale, st);
+    rc |= sk.wgrad(H, Fa, (int)BR, tp.dpre_att, H, att, Fa, G.att_embed_w, Fa, 0);
+    rc |= colsum_launch((int)BR, H, tp.dpre_att, H, G.att_embed_b, 0, st);
+    e->launches += 14 + (tf32_context_launches(e->tf32) - tf32_l0);
+    if (!rc && record_group_event(e->grad_events[1], st)) return 1;
+    return rc;
+}
+
 }  // namespace
 
 extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
@@ -1340,8 +1608,76 @@ extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, cons
     return rc_graph;
 }
 
+extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                                         const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                                         const capb200_att2in2_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
+                                         float* reward, float* loss, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_ATT2IN2, "capb200_att2in2_scst_step needs an Att2in2 engine");
+    CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
+    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
+    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
+    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
+    CAPB_REQUIRE(greedy_baseline || opts->sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
+    CAPB_REQUIRE(opts->sample_n >= 1 && opts->sample_n <= 16 && B >= 1 && R >= 1, "sample_n must be in 1..16");
+    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
+    TrainArgs ta;
+    ta.n = opts->sample_n; ta.T = e->T; ta.Tl = e->T; ta.p = opts->drop_prob; ta.temperature = opts->temperature; ta.upstream = opts->upstream;
+    ta.seed = opts->seed; ta.greedy_baseline = greedy_baseline; ta.table = table; ta.refs = refs; ta.ref_offsets = ref_offsets; ta.L = L;
+    ta.sample_seq = sample_seq; ta.greedy_seq = greedy_seq; ta.reward = reward; ta.logprobs = sample_logprobs; ta.loss = loss;
+    ta.forced = opts->forced_tokens; ta.mask = opts->att_masks; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
+    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->sample_n, "keep_rows must be in 0..rows");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the whole step as one CUDA graph, as capb200_updown_scst_step (the fc features are not read: only att and the mask are staged)
+    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
+        if (dropout_salt_set_all(0ull, st)) return 1;
+        return att2in2_train_step(e, fc, att, B, R, ta, grads, st);
+    }
+    cudaStream_t gst = e->sg.enter(st);
+    const void* srcs[2] = {att, ta.mask};
+    const size_t bytes[2] = {sizeof(float) * (size_t)B * R * e->cfg.att_feat_size, ta.mask ? sizeof(float) * (size_t)B * R : 0};
+    size_t off[2];
+    if (e->sg.stage_inputs(2, srcs, bytes, off, gst)) return 1;
+    const float* att_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
+    if (ta.mask) ta.mask = reinterpret_cast<const float*>(e->sg.stage + off[1]);
+    unsigned long long key = 1469598103934665603ull;
+    capb200_scst_opts o2 = *opts; o2.seed = 0; o2.att_masks = ta.mask;
+    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
+    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
+    StepGraph::mix(key, ptrs, sizeof(ptrs));
+    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
+    const int dims[] = {B, R, L};
+    StepGraph::mix(key, dims, sizeof(dims));
+    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return att2in2_train_step(e, nullptr, att_s, B, R, ta, grads, gst); });
+    if (e->sg.leave(st, gst)) return 1;
+    return rc_graph;
+}
+
+extern "C" int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
+                                       const long long* labels, const float* masks, int label_cols, const capb200_att2in2_grads* grads, float* logprobs,
+                                       float* loss, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_ATT2IN2, "capb200_att2in2_xe_step needs an Att2in2 engine");
+    CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
+    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1 && R >= 1, "seq_per_img must be in 1..16");
+    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
+    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
+    CAPB_REQUIRE(label_cols >= 2 && label_cols <= e->T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
+    CAPB_REQUIRE(opts->steps >= 1 && opts->steps <= label_cols - 1, "steps must be in 1..label_cols-1");
+    TrainArgs ta;
+    ta.xe = true;
+    ta.n = opts->seq_per_img; ta.T = opts->steps; ta.Tl = label_cols - 1; ta.p = opts->drop_prob; ta.upstream = opts->upstream; ta.seed = opts->seed;
+    ta.smoothing = opts->label_smoothing;
+    ta.labels = labels; ta.ld_labels = label_cols; ta.masks = masks; ta.ld_masks = label_cols; ta.logprobs = logprobs; ta.loss = loss;
+    ta.mask = opts->att_masks; ta.ss_prob = opts->ss_prob; ta.tokens_used = opts->tokens_used; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
+    CAPB_REQUIRE(ta.ss_prob >= 0.f && ta.ss_prob <= 1.f, "ss_prob must be in [0, 1]");
+    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->seq_per_img, "keep_rows must be in 0..rows");
+    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;
+    return att2in2_train_step(e, fc, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n) {
-    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 2, "UpDown has 2 gradient groups");
+    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 2, "UpDown and Att2in2 have 2 gradient groups");
     for (int i = 0; i < 2; ++i) e->grad_events[i] = (events != nullptr && i < n) ? static_cast<cudaEvent_t>(events[i]) : nullptr;
     return 0;
 }

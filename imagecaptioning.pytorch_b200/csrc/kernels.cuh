@@ -183,6 +183,10 @@ int xe_loss_backward_launch(const float* logp, long ld_row, const long long* lab
 int lstm_cell_backward_launch(int rows, int H, const float* gates, const float* c_prev, const float* c_new, const float* dh, const float* dh_extra,
                               long ld_extra, unsigned drop_site, unsigned drop_step, unsigned long long seed, float p, float* dc_carry, float* dgates,
                               cudaStream_t st);
+// Att2in2's maxout cell: dsums [rows, 5H] (i, f, o, a, b) from dh (+ dropout-masked dh_extra of site drop_site) and the carried dc
+int maxout_cell_backward_launch(int rows, int H, const float* sums, const float* c_prev, const float* c_new, const float* dh, const float* dh_extra,
+                                long ld_extra, unsigned drop_site, unsigned drop_step, unsigned long long seed, float p, float* dc_carry, float* dsums,
+                                cudaStream_t st);
 int attention_backward_launch(int n_images, int rpi, int R, int A, int H, const float* d_out, const float* alpha, const float* att_h, const float* p_att,
                               const float* att, const float* w, float* d_att_h, float* d_att, float* d_p_att, float* d_w, float* d_b, float* d_alpha_scratch,
                               cudaStream_t st);

@@ -5,6 +5,7 @@
 //   dropout sites            models/AttModel.py:74-88 (embed / fc_embed / att_embed Sequentials), :637 (core output)
 //   dlogits                  modules/losses.py:22-37 (RewardCriterion) composed with F.log_softmax (AttModel.py:172)
 //   lstm_cell_backward       nn.LSTMCell (AttModel.py:628,635)
+//   maxout_cell_backward     Att2in2Core's maxout cell (AttModel.py:773-787)
 //   attention_backward       models/AttModel.py:728-748
 // Dropout masks are never stored: keep(seed, site, step, element) is a pure function (Philox4x32-10), re-evaluated in the backward.
 #include "common.cuh"
@@ -206,6 +207,35 @@ __global__ void lstm_cell_backward_kernel(int rows, int H, const float* __restri
         dg[H + c] = dc * cp * fg * (1.f - fg);
         dg[2 * H + c] = dc * ig * (1.f - gg * gg);
         dg[3 * H + c] = dht * tc * og * (1.f - og);
+        dc_carry[i] = dc * fg;
+    }
+}
+
+// Maxout cell backward (Att2in2Core, AttModel.py:773-787; pre-activation sums saved): s [rows, 5H] = (i, f, o, a, b) with
+// c' = sigmoid(f) c + sigmoid(i) max(a, b), h' = sigmoid(o) tanh(c').  d max goes to the larger of a, b; a tie splits it half-and-half,
+// as torch.maximum's autograd does.  dh_extra / drop_* as in lstm_cell_backward.
+__global__ void maxout_cell_backward_kernel(int rows, int H, const float* __restrict__ sums, const float* __restrict__ c_prev, const float* __restrict__ c_new,
+                                            const float* __restrict__ dh, const float* __restrict__ dh_extra, long ld_extra, uint32_t drop_site,
+                                            uint32_t drop_step, unsigned long long seed, float p, float* __restrict__ dc_carry, float* __restrict__ dsums) {
+    const long total = (long)rows * H;
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(i / H), c = (int)(i % H);
+        const float* s = sums + (long)r * 5 * H;
+        const float ig = 1.f / (1.f + expf(-s[c])), fg = 1.f / (1.f + expf(-s[H + c])), og = 1.f / (1.f + expf(-s[2 * H + c]));
+        const float a = s[3 * H + c], b = s[4 * H + c];
+        const float gg = fmaxf(a, b);
+        const float cp = c_prev ? c_prev[i] : 0.f;
+        const float tc = tanhf(c_new[i]);
+        float dht = dh[i];
+        if (dh_extra != nullptr) dht += dh_extra[(long)r * ld_extra + c] * (drop_site ? drop_scale(seed, drop_site, drop_step, (uint32_t)i, p) : 1.f);
+        const float dc = dc_carry[i] + dht * og * (1.f - tc * tc);
+        const float dg = dc * ig;
+        float* ds = dsums + (long)r * 5 * H;
+        ds[c] = dc * gg * ig * (1.f - ig);
+        ds[H + c] = dc * cp * fg * (1.f - fg);
+        ds[2 * H + c] = dht * tc * og * (1.f - og);
+        ds[3 * H + c] = a > b ? dg : (a < b ? 0.f : 0.5f * dg);
+        ds[4 * H + c] = b > a ? dg : (b < a ? 0.f : 0.5f * dg);
         dc_carry[i] = dc * fg;
     }
 }
@@ -424,6 +454,13 @@ int lstm_cell_backward_launch(int rows, int H, const float* gates, const float* 
                               cudaStream_t st) {
     lstm_cell_backward_kernel<<<nblocks((long)rows * H), 256, 0, st>>>(rows, H, gates, c_prev, c_new, dh, dh_extra, ld_extra, drop_site, drop_step, seed, p,
                                                                         dc_carry, dgates);
+    LAUNCH_OK();
+}
+int maxout_cell_backward_launch(int rows, int H, const float* sums, const float* c_prev, const float* c_new, const float* dh, const float* dh_extra,
+                                long ld_extra, unsigned drop_site, unsigned drop_step, unsigned long long seed, float p, float* dc_carry, float* dsums,
+                                cudaStream_t st) {
+    maxout_cell_backward_kernel<<<nblocks((long)rows * H), 256, 0, st>>>(rows, H, sums, c_prev, c_new, dh, dh_extra, ld_extra, drop_site, drop_step, seed, p,
+                                                                          dc_carry, dsums);
     LAUNCH_OK();
 }
 int attention_backward_launch(int n_images, int rpi, int R, int A, int H, const float* d_out, const float* alpha, const float* att_h, const float* p_att,

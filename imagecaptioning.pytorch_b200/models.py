@@ -516,6 +516,9 @@ class B200UpDownModel(B200CaptionModel):
 
     family = _lib.FAMILY_UPDOWN
     family_name = 'updown'
+    # C entry points and gradient table of the fused training steps (include/capb200.h)
+    _scst_entry, _xe_entry = 'capb200_updown_scst_step', 'capb200_updown_xe_step'
+    _grads_struct, _grad_fields = _lib.UpdownGrads, _lib.GRAD_FIELDS
 
     def __init__(self, opt, numeric_mode=None):
         super().__init__(opt, numeric_mode)
@@ -548,10 +551,10 @@ class B200UpDownModel(B200CaptionModel):
         return [[(k, t[k]) for k in first], [(k, v) for k, v in t.items() if k not in first]]
 
     def _grad_table(self, lib, device):
-        """capb200_updown_grads pointing into the persistent flat buffer, the group events registered with the engine."""
+        """capb200_updown_grads (capb200_att2in2_grads) pointing into the persistent flat buffer, the group events registered with the engine."""
         fg = self._flat_grads(device)
-        g = _lib.UpdownGrads()
-        for name in _lib.GRAD_FIELDS:
+        g = self._grads_struct()
+        for name in self._grad_fields:
             setattr(g, name, fg.by_name[name].data_ptr())
         # the engine records the group events only for a listener (B200LossWrapper.enable_gradient_sync); without one the whole step may run as a CUDA graph
         table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
@@ -596,9 +599,9 @@ class B200UpDownModel(B200CaptionModel):
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None      # drop_worst: per-row losses (reduction 'none')
         so = _lib.ScstOpts(sample_n, float(temperature), seed, float(p), float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY,
                            _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss))
-        _lib.check(lib.capb200_updown_scst_step(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs),
-                                                _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq), _lib.ptr(greedy_seq), _lib.ptr(logprobs),
-                                                _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'updown_scst_step')
+        _lib.check(getattr(lib, self._scst_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs),
+                                                  _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq), _lib.ptr(greedy_seq), _lib.ptr(logprobs),
+                                                  _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), self._scst_entry[len('capb200_'):])
         res = {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
                'grads': {table_params[k]: grads[k] for k in table_params}, 'seed': seed, 'flat': fg, 'row_loss': row_loss}
         return res
@@ -636,10 +639,54 @@ class B200UpDownModel(B200CaptionModel):
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
         xo = _lib.XeOpts(N // B, steps, seed, float(p), float(label_smoothing), float(upstream), _lib.ptr(region_masks), float(self.ss_prob),
                          _lib.ptr(tokens_used), int(keep_rows), _lib.ptr(row_loss))
-        _lib.check(lib.capb200_updown_xe_step(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(xo), _lib.ptr(labels), _lib.ptr(masks), Lc,
-                                              ctypes.byref(g), _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), 'updown_xe_step')
+        _lib.check(getattr(lib, self._xe_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(xo), _lib.ptr(labels), _lib.ptr(masks), Lc,
+                                                ctypes.byref(g), _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), self._xe_entry[len('capb200_'):])
         return {'loss': loss[0], 'logprobs': logprobs, 'grads': {table_params[k]: grads[k] for k in table_params}, 'seed': seed, 'flat': fg,
                 'tokens_used': tokens_used, 'row_loss': row_loss}
+
+
+class _Att2in2CoreParams(nn.Module):
+    """Parameter container with the key names of Att2in2Core + Attention (AttModel.py:754-768,719-726)."""
+
+    def __init__(self, opt):
+        super().__init__()
+        self.a2c = nn.Linear(opt.rnn_size, 2 * opt.rnn_size)
+        self.i2h = nn.Linear(opt.input_encoding_size, 5 * opt.rnn_size)
+        self.h2h = nn.Linear(opt.rnn_size, 5 * opt.rnn_size)
+        self.attention = nn.Module()
+        self.attention.h2att = nn.Linear(opt.rnn_size, opt.att_hid_size)
+        self.attention.alpha_net = nn.Linear(opt.att_hid_size, 1)
+
+
+class B200Att2in2Model(B200UpDownModel):
+    """Drop-in for captioning.models.AttModel.Att2in2Model (AttModel.py:854-859): AttModel without fc_embed, one maxout-LSTM core that
+    attends with its previous hidden state.  Decoding, diverse beam search and the fused XE / SCST steps take UpDown's surface; the engine
+    runs the Att2in2 core (CAPB200_FAMILY_ATT2IN2)."""
+
+    family = _lib.FAMILY_ATT2IN2
+    family_name = 'att2in2'
+    _scst_entry, _xe_entry = 'capb200_att2in2_scst_step', 'capb200_att2in2_xe_step'
+    _grads_struct, _grad_fields = _lib.Att2in2Grads, _lib.ATT2IN2_GRAD_FIELDS
+
+    def __init__(self, opt, numeric_mode=None):
+        B200CaptionModel.__init__(self, opt, numeric_mode)
+        self.num_layers = 1
+        V1 = self.vocab_size + 1
+        self.embed = nn.Sequential(nn.Embedding(V1, self.input_encoding_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
+        self.att_embed = nn.Sequential(nn.Linear(self.att_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
+        self.logit = nn.Linear(self.rnn_size, V1)
+        self.ctx2att = nn.Linear(self.rnn_size, self.att_hid_size)
+        self.core = _Att2in2CoreParams(opt)
+
+    def _weight_table(self):
+        c = self.core
+        return {
+            'embed': self.embed[0].weight, 'att_embed_w': self.att_embed[0].weight, 'att_embed_b': self.att_embed[0].bias,
+            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
+            'h2att_w': c.attention.h2att.weight, 'h2att_b': c.attention.h2att.bias,
+            'alpha_w': c.attention.alpha_net.weight, 'alpha_b': c.attention.alpha_net.bias,
+            'i2h_w': c.i2h.weight, 'i2h_b': c.i2h.bias, 'h2h_w': c.h2h.weight, 'h2h_b': c.h2h.bias, 'a2c_w': c.a2c.weight, 'a2c_b': c.a2c.bias,
+        }
 
 
 class _MaxoutCoreParams(nn.Module):
@@ -1187,6 +1234,8 @@ def setup(opt, numeric_mode=None):
         return B200UpDownModel(opt, numeric_mode)
     if name == 'newfc':
         return B200NewFCModel(opt, numeric_mode)
+    if name == 'att2in2':
+        return B200Att2in2Model(opt, numeric_mode)
     if name == 'aoa':
         return B200AoAModel(opt, numeric_mode)
     if name == 'transformer':

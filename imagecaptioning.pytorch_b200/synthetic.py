@@ -104,6 +104,16 @@ def make_weights(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: 
         pe[:, 1::2] = torch.cos(position * div_term)
         W['model.tgt_embed.1.pe'] = pe.unsqueeze(0)
         xav('model.generator.proj', V1, D, logit_scale)
+    elif family == 'att2in2':
+        W['embed.0.weight'] = torch.randn(V1, E, generator=g)
+        lin('att_embed.0', H, F_att)
+        lin('logit', V1, H, logit_scale)
+        lin('ctx2att', A, H)
+        lin('core.a2c', 2 * H, H)
+        lin('core.i2h', 5 * H, E)
+        lin('core.h2h', 5 * H, H)
+        lin('core.attention.h2att', A, H)
+        lin('core.attention.alpha_net', 1, A)
     elif family == 'newfc':
         W['embed.weight'] = torch.randn(V1, E, generator=g)
         lin('fc_embed', E, F_fc)

@@ -34,6 +34,7 @@ extern "C" {
 
 #define CAPB200_FAMILY_UPDOWN 0 /* UpDownModel  captioning/models/AttModel.py:868 */
 #define CAPB200_FAMILY_NEWFC 1  /* NewFCModel   captioning/models/AttModel.py:904 */
+#define CAPB200_FAMILY_ATT2IN2 2 /* Att2in2Model captioning/models/AttModel.py:854 (no fc_embed; the core attends with the previous h) */
 
 typedef struct capb200_engine capb200_engine;
 typedef struct capb200_cider_table capb200_cider_table;
@@ -94,7 +95,9 @@ typedef struct {
     int numeric_mode;        /* CAPB200_MODE_* */
 } capb200_model_cfg;
 
-/* Borrowed fp32 device pointers in the reference's state_dict layouts (SURVEY.md section 8b key list). */
+/* Borrowed fp32 device pointers in the reference's state_dict layouts (SURVEY.md section 8b key list).
+ * Att2in2 uses embed, att_embed_*, ctx2att_*, logit_*, h2att_* / alpha_* (core.attention), i2h_* / h2h_* (core.i2h / core.h2h, [5H,E] [5H,H])
+ * and a2c_*; its fc_embed_* stay NULL (the model has no fc_embed, AttModel.py:858) and the core never reads the fc features. */
 typedef struct {
     const float* embed;                                                           /* [V+1,E]  embed.0.weight | embed.weight */
     const float *fc_embed_w, *fc_embed_b;                                         /* [H,F_fc] (newfc: [E,F_fc]) */
@@ -106,6 +109,7 @@ typedef struct {
     const float *h2att_w, *h2att_b;                                               /* [A,H] */
     const float *alpha_w, *alpha_b;                                               /* [1,A] [1] */
     const float *i2h_w, *i2h_b, *h2h_w, *h2h_b;                                   /* newfc _core: [5H,E] [5H] [5H,H] [5H] */
+    const float *a2c_w, *a2c_b;                                                   /* att2in2 core.a2c: [2H,H] [2H] */
 } capb200_weights;
 
 capb200_engine* capb200_engine_create(const capb200_model_cfg* cfg);
@@ -151,7 +155,7 @@ typedef struct {
     float diversity_lambda;   /* >= 0: a candidate word loses lambda for every beam of an earlier group holding it at the same position */
 } capb200_diverse_opts;
 
-/* Diverse beam search: AttModel._sample_beam + CaptionModel.beam_search with group_size > 1 (CaptionModel.py:35-209), UpDown only.
+/* Diverse beam search: AttModel._sample_beam + CaptionModel.beam_search with group_size > 1 (CaptionModel.py:35-209), UpDown and Att2in2.
  * Same output contract as capb200_decode_beam, except:
  *   done_*[B, beam]: for each group in order, its bdash best finished beams by score (the reference's group-concatenated done_beams);
  *   seq / seq_logprobs rows k < B: done_beams[k][0] (group 0's best); with sample_n == bdash the rows B .. B*sample_n-1 are pad / zero
@@ -371,6 +375,26 @@ int capb200_updown_xe_step(capb200_engine* e, const float* fc, const float* att,
                            const float* masks, int label_cols, const capb200_updown_grads* grads, float* logprobs, float* loss, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Training steps of the Att2in2 model (Att2in2Core, AttModel.py:770-790), same contracts as the UpDown steps above: an engine of
+ * CAPB200_FAMILY_ATT2IN2, the fc features are ignored (may be NULL), the options mean what they mean for UpDown (greedy or leave-one-out
+ * baseline, forced tokens, region masks, keep_rows / row_loss, scheduled sampling with tokens_used, label smoothing), dropout sites
+ * 1 att_embed, 2 word embedding, 3 core output (replayable through capb200_dropout_mask), the whole SCST step captured into one CUDA graph as
+ * capb200_updown_scst_step describes.  Gradient groups: see capb200_engine_set_grad_events.
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* Gradient buffers of the 17 Att2in2 parameters (same shapes as the capb200_weights fields, fp32, device); every one is OVERWRITTEN. */
+typedef struct {
+    float* embed;
+    float *att_embed_w, *att_embed_b, *ctx2att_w, *ctx2att_b, *logit_w, *logit_b;
+    float *h2att_w, *h2att_b, *alpha_w, *alpha_b;
+    float *i2h_w, *i2h_b, *h2h_w, *h2h_b, *a2c_w, *a2c_b;
+} capb200_att2in2_grads;
+int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                              const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L, const capb200_att2in2_grads* grads,
+                              long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, void* stream);
+int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const long long* labels,
+                            const float* masks, int label_cols, const capb200_att2in2_grads* grads, float* logprobs, float* loss, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * One self-critical training step of the AoANet model (BASELINE configs[3]): LossWrapper.forward with sc_flag (loss_wrapper.py:56-73)
  * over AoAModel (refiner + AoA decoder, AoAModel.py:56-226) in train mode, and its backward.  Dropout sites (replayable through
  * capb200_dropout_mask with the same seed): 1 att_embed [B*R,H]; 2 word embedding at `step` [N,E]; 3 core output at `step` [N,H];
@@ -440,14 +464,15 @@ int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int B, int R, c
  * same way).  A training step finishes its gradient buffers in a fixed order of groups; after the last write of group k it records
  * events[k] (cudaEvent_t, caller-owned) on the step's stream, so a communication stream can all-reduce group k while the rest of the
  * backward pass still runs.  n = 0 or events = NULL switches the recording off.  Groups:
- *   UpDown (capb200_engine_set_grad_events, n <= 2): 0 logit.{weight,bias}; 1 every other parameter.
+ *   UpDown and Att2in2 (capb200_engine_set_grad_events, n <= 2): 0 logit.{weight,bias}; 1 every other parameter.
  *   AoANet (capb200_aoa_set_grad_events, n <= 10):  0 logit; 1 decoder (att2ctx, attention q-projection and norm, att_lstm) + embed;
  *           2 ctx2att + refiner.norm; 3..8 refiner layers 5..0; 9 att_embed. */
 int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n);
 int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* events, int n);
 
 /* The dropout keep/scale mask (0 or 1/(1-p)) of one site and step, for tests that replay it in the oracle:
- * site 0 = fc_embed [B,H], 1 = att_embed [B*R,H], 2 = word embedding at `step` [N,E], 3 = core output at `step` [N,H]. */
+ * site 0 = fc_embed [B,H], 1 = att_embed [B*R,H], 2 = word embedding at `step` [N,E], 3 = core output at `step` [N,H].
+ * (Att2in2 has no site 0: it has no fc_embed.) */
 int capb200_dropout_mask(float* mask, long n, unsigned long long seed, int site, int step, float p, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
