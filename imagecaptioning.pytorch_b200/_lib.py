@@ -106,6 +106,13 @@ class Att2in2Grads(Structure):
     _fields_ = [(f, c_void_p) for f in ATT2IN2_GRAD_FIELDS]
 
 
+NEWFC_GRAD_FIELDS = ['embed', 'fc_embed_w', 'fc_embed_b', 'logit_w', 'logit_b', 'i2h_w', 'i2h_b', 'h2h_w', 'h2h_b']
+
+
+class NewfcGrads(Structure):
+    _fields_ = [(f, c_void_p) for f in NEWFC_GRAD_FIELDS]
+
+
 TFM_MAX_LAYERS = 8
 
 
@@ -217,6 +224,10 @@ SIGNATURES = {
                                           POINTER(Att2in2Grads), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'capb200_att2in2_xe_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), c_void_p, c_void_p, c_int, POINTER(Att2in2Grads),
                                         c_void_p, c_void_p, c_void_p]),
+    'capb200_newfc_scst_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), c_void_p, c_void_p, c_void_p, c_int,
+                                        POINTER(NewfcGrads), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_newfc_xe_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), c_void_p, c_void_p, c_int, POINTER(NewfcGrads),
+                                      c_void_p, c_void_p, c_void_p]),
     'capb200_dropout_mask': (c_int, [c_void_p, c_long, c_ulonglong, c_int, c_int, c_float, c_void_p]),
     'capb200_tfm_xe_step': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmXeOpts), c_void_p, c_void_p, c_int, POINTER(TfmWeights), c_void_p, c_void_p,
                                     c_void_p]),

@@ -1075,6 +1075,8 @@ struct Tape {
     int *s_tokens, *s_unfinished, *s_forced;   // sampling-loop state of the train step (its own copies: the greedy baseline runs concurrently)
     float* s_att_score;
     float *row_loss, *row_msum, *row_coef;     // drop_worst: per-row loss, mask count and gradient coefficient
+    float *im_sums, *im_h, *im_c, *im_ds, *im_dh, *im_dc;   // NewFC's image step on B rows: maxout sums, state and their gradients
+    int* img_row;                              // NewFC: image of each row (r / n)
 };
 
 void layout_tape(Tape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int A, int V1, int F_att, int F_fc) {
@@ -1559,6 +1561,183 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
     return rc;
 }
 
+// ---- NewFC (NewFCModel, AttModel.py:904-945; LSTMCore, FCModel.py:13-42) -------------------------------------------------------------
+// Att2in2's tape without the attention fields, plus the image step: fc_e [B,E] = fc_embed(fc), its maxout sums / state on B rows (image
+// features are never replicated per row) and their gradients.  h0 / c0 slot 0 holds the image step's state broadcast to each image's rows.
+void layout_tape_newfc(Tape& tp, Arena& a, int B, int N, int T, int E, int H, int V1) {
+    layout_tape_att2in2(tp, a, B, 0, N, T, E, H, 0, V1);
+    tp.fc_e = a.take<float>((long)B * E); tp.d_fc_e = a.take<float>((long)B * E);
+    tp.im_sums = a.take<float>((long)B * 5 * H); tp.im_ds = a.take<float>((long)B * 5 * H);
+    tp.im_h = a.take<float>((long)B * H); tp.im_c = a.take<float>((long)B * H);
+    tp.im_dh = a.take<float>((long)B * H); tp.im_dc = a.take<float>((long)B * H);
+    tp.img_row = a.take<int>(N);
+}
+
+// One NewFC training step.  The core starts from a zero state and first consumes fc_embed(fc) (the image step, AttModel.py:925-927: its
+// output is discarded, only (h, c) carries on), then <bos> at t = 0 and the words.  The embedding is a bare nn.Embedding and fc_embed a bare
+// nn.Linear (no ReLU, no dropout); the only dropout is site 3 on the core output.  Gradient paths of the image step: h2h(0) is h2h's bias, so
+// h2h.bias gets the image step's gradient and h2h.weight does not; i2h gets both the word steps' (input xt) and the image step's (input fc_e);
+// fc_embed is reached through the image step only.
+int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs& ta, const capb200_newfc_grads* grads, cudaStream_t st) {
+    const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, V1 = e->V1, H5 = 5 * H;
+    const int Ff = e->cfg.fc_feat_size;
+    const float p = ta.p;
+    const unsigned long long seed = ta.seed;
+    const capb200_weights& w = e->w;
+    float* const sample_logprobs = ta.logprobs;
+    const long ld_lp = (long)ta.Tl * V1;
+
+    Arena dry; Tape t0; layout_tape_newfc(t0, dry, B, N, T, E, H, V1);
+    if (grow_tape(e, dry.off + 256, st)) return 1;
+    Arena ar; ar.base = e->tape;
+    Tape tp; layout_tape_newfc(tp, ar, B, N, T, E, H, V1);
+    if (ensure_workspace(e, B, N, 1, 1, st)) return 1;      // R = 1: the region count the greedy baseline's decode call sizes its workspace for
+    bool greedy_on_side = false;
+    if (start_greedy_baseline(e, fc, nullptr, B, 0, ta, tp.glp, &greedy_on_side, st)) return 1;
+    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
+    tf32_context_new_step(e->tf32);
+    const long tf32_l0 = tf32_context_launches(e->tf32);
+    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};
+    sk.ctx = e->tf32;
+
+    // ---- image step on B rows: sums = fc_e i2h^T + (i2h_b + h2h_b), the maxout cell with c_prev = 0
+    nvtxRangePushA("capb200 newfc train step: forward on the tape");
+    const long NH = (long)N * H;
+    if (sk.lin(fc, Ff, w.fc_embed_w, Ff, w.fc_embed_b, tp.fc_e, E, B, E, Ff, 0)) return 1;
+    if (sk.lin(tp.fc_e, E, w.i2h_w, E, e->bsum_core, tp.im_sums, H5, B, H5, E, 0)) return 1;
+    if (maxout_pointwise_launch(B, H, tp.im_sums, H5, nullptr, nullptr, H, tp.im_c, H, ActView{tp.im_h, nullptr, nullptr, H}, st)) return 1;
+    iota_div_kernel<<<cdiv(N, 256), 256, 0, st>>>(tp.img_row, N, n);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    e->launches += 4;
+
+    // ---- T word steps with the tape
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
+    for (int t = 0; t < T; ++t) {
+        int* tok = tp.tok + (long)t * N;
+        if (ta.xe) {
+            if (t >= 1 && ta.ss_prob > 0.f) {      // scheduled sampling (AttModel.py:145-154)
+                if (ss_select_launch(N, V1, sample_logprobs + (long)(t - 1) * V1, ld_lp, ta.labels, ta.ld_labels, t, seed, ta.ss_prob, tok, st)) return 1;
+            } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
+            if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
+        }
+        else CAPB_CHECK_CUDA(cudaMemcpyAsync(tok, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        float* xt = tp.xt + (long)t * N * E;
+        float* sums = tp.g1 + (long)t * N * H5;
+        const float* hp = tp.h0 + (long)t * NH;
+        const float* cp = tp.c0 + (long)t * NH;
+        float *h = tp.h0 + (long)(t + 1) * NH, *c = tp.c0 + (long)(t + 1) * NH;
+        // xt = embed[tok]; at t = 0 the same launch broadcasts the image step's (h, c) into slot 0 of each image's rows (later steps copy no
+        // state: H = 0)
+        StateCopy s0, s1;
+        s0.src = tp.im_h; s0.ld_src = H; s0.dst = ActView{tp.h0, nullptr, nullptr, H};
+        s1.src = tp.im_c; s1.ld_src = H; s1.dst = ActView{tp.c0, nullptr, nullptr, H};
+        if (state_gather_embed_launch(N, tok, t == 0 ? tp.img_row : nullptr, w.embed, E, E, 0, ActView{xt, nullptr, nullptr, E}, t == 0 ? H : 0,
+                                      t == 0 ? 2 : 0, s0, s1, st)) return 1;
+        {   // sums = xt i2h^T + h_prev h2h^T + (i2h_b + h2h_b)
+            GemmProblem g; g.M = N; g.N = H5; g.nseg = 2;
+            g.seg[0].A = xt; g.seg[0].lda = E; g.seg[0].W = w.i2h_w; g.seg[0].ldw = E; g.seg[0].K = E;
+            g.seg[1].A = hp; g.seg[1].lda = H; g.seg[1].W = w.h2h_w; g.seg[1].ldw = H; g.seg[1].K = H;
+            g.epi.bias = e->bsum_core;
+            g.epi.C = sums; g.epi.ldc = H5;
+            if (sk.gates(g)) return 1;
+        }
+        if (maxout_pointwise_launch(N, H, sums, H5, nullptr, cp, H, c, H, ActView{h, nullptr, nullptr, H}, st)) return 1;
+        // core output = dropout(h) (FCModel.py:40), stored in (n, t) order for the batched logit backward
+        float* out = tp.out + (long)t * H;
+        if (dropout_copy_launch(h, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
+        float* logits = sample_logprobs + (long)t * V1;
+        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, logits, ld_lp, N, V1, H, 0)) return 1;
+        VocabStepArgs va;
+        va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
+        if (!ta.xe) {
+            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
+            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
+            va.seq_out = ta.sample_seq; va.ld_seq = T; va.t = t;
+            if (ta.forced != nullptr) {
+                if (load_token_column_launch(ta.forced, T, t, N, tp.s_forced, st)) return 1;
+                va.select = 3; va.forced = tp.s_forced;
+            }
+        }
+        if (vocab_step_launch(va, st)) return 1;
+        e->launches += 7;
+    }
+
+    // ---- loss, logit backward, back-propagation through time
+    nvtxRangePop();
+    CAPB_NVTX("capb200 newfc train step: loss, backward through time, weight gradients");
+    const long TN = (long)T * N;
+    const capb200_newfc_grads& G = *grads;
+    if (loss_and_logit_backward(e, ta, sk, tp, B, N, greedy_on_side, G.logit_w, G.logit_b, st)) return 1;
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(G.embed, 0, sizeof(float) * (size_t)V1 * E, st));
+    for (int t = T - 1; t >= 0; --t) {
+        const float* sums = tp.g1 + (long)t * N * H5;
+        float* ds = tp.DG1 + (long)t * N * H5;
+        // cell: dh = carried dh + dropout-masked dOUT[:, t]
+        if (maxout_cell_backward_launch(N, H, sums, tp.c0 + (long)t * NH, tp.c0 + (long)(t + 1) * NH, tp.dh0, tp.dOUT + (long)t * H, (long)T * H, 3,
+                                        (unsigned)t, seed, p, tp.dc0, ds, st)) return 1;
+        if (sk.dgrad(N, E, H5, ds, H5, w.i2h_w, E, tp.dxt, E, 0)) return 1;                     // d xt
+        if (sk.dgrad(N, H, H5, ds, H5, w.h2h_w, H, tp.dh0, H, 0)) return 1;                     // d h_prev (the carried dh is consumed)
+        if (embed_scatter_launch(N, E, tp.tok + (long)t * N, tp.dxt, E, G.embed, st)) return 1;
+        e->launches += 4;
+    }
+    // the image step: dh / dc carried out of step 0, summed over each image's rows, through the maxout cell (c_prev = 0) on B rows
+    int rc = 0;
+    rc |= per_image_sum_launch(1, N, n, H, tp.dh0, tp.im_dh, st);
+    rc |= per_image_sum_launch(1, N, n, H, tp.dc0, tp.im_dc, st);
+    rc |= maxout_cell_backward_launch(B, H, tp.im_sums, nullptr, tp.im_c, tp.im_dh, nullptr, 0, 0, 0, seed, p, tp.im_dc, tp.im_ds, st);
+    // weight gradients, batched over time (K = T*N; h0 slots 0..T-1 are the previous states h2h reads), plus the image step's terms (K = B)
+    rc |= sk.wgrad(H5, E, (int)TN, tp.DG1, H5, tp.xt, E, G.i2h_w, E, 0);
+    rc |= sk.wgrad(H5, E, B, tp.im_ds, H5, tp.fc_e, E, G.i2h_w, E, 1);
+    rc |= sk.wgrad(H5, H, (int)TN, tp.DG1, H5, tp.h0, H, G.h2h_w, H, 0);
+    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.i2h_b, 0, st);
+    rc |= colsum_launch(B, H5, tp.im_ds, H5, G.i2h_b, 1, st);
+    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.h2h_b, 0, st);
+    rc |= colsum_launch(B, H5, tp.im_ds, H5, G.h2h_b, 1, st);
+    // fc_embed, through the image step's input
+    rc |= sk.dgrad(B, E, H5, tp.im_ds, H5, w.i2h_w, E, tp.d_fc_e, E, 0);
+    rc |= sk.wgrad(E, Ff, B, tp.d_fc_e, E, fc, Ff, G.fc_embed_w, Ff, 0);
+    rc |= colsum_launch(B, E, tp.d_fc_e, E, G.fc_embed_b, 0, st);
+    e->launches += 13 + (tf32_context_launches(e->tf32) - tf32_l0);
+    if (!rc && record_group_event(e->grad_events[1], st)) return 1;
+    return rc;
+}
+
+// Argument checks and TrainArgs of the *_scst_step / *_xe_step entry points of UpDown, Att2in2 and NewFC (the options mean the same for all three).
+int scst_train_args(int B, const capb200_scst_opts* opts, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                    long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, int T, TrainArgs* ta) {
+    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
+    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
+    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
+    CAPB_REQUIRE(greedy_baseline || opts->sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
+    CAPB_REQUIRE(opts->sample_n >= 1 && opts->sample_n <= 16 && B >= 1, "sample_n must be in 1..16");
+    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
+    ta->n = opts->sample_n; ta->T = T; ta->Tl = T; ta->p = opts->drop_prob; ta->temperature = opts->temperature; ta->upstream = opts->upstream;
+    ta->seed = opts->seed; ta->greedy_baseline = greedy_baseline; ta->table = table; ta->refs = refs; ta->ref_offsets = ref_offsets; ta->L = L;
+    ta->sample_seq = sample_seq; ta->greedy_seq = greedy_seq; ta->reward = reward; ta->logprobs = sample_logprobs; ta->loss = loss;
+    ta->forced = opts->forced_tokens; ta->mask = opts->att_masks; ta->keep = opts->keep_rows; ta->row_loss = opts->row_loss;
+    CAPB_REQUIRE(ta->keep >= 0 && ta->keep <= B * opts->sample_n, "keep_rows must be in 0..rows");
+    return 0;
+}
+
+int xe_train_args(int B, const capb200_xe_opts* opts, const long long* labels, const float* masks, int label_cols, float* logprobs, float* loss, int T,
+                  TrainArgs* ta) {
+    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1, "seq_per_img must be in 1..16");
+    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
+    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
+    CAPB_REQUIRE(label_cols >= 2 && label_cols <= T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
+    CAPB_REQUIRE(opts->steps >= 1 && opts->steps <= label_cols - 1, "steps must be in 1..label_cols-1");
+    ta->xe = true;
+    ta->n = opts->seq_per_img; ta->T = opts->steps; ta->Tl = label_cols - 1; ta->p = opts->drop_prob; ta->upstream = opts->upstream; ta->seed = opts->seed;
+    ta->smoothing = opts->label_smoothing;
+    ta->labels = labels; ta->ld_labels = label_cols; ta->masks = masks; ta->ld_masks = label_cols; ta->logprobs = logprobs; ta->loss = loss;
+    ta->mask = opts->att_masks; ta->ss_prob = opts->ss_prob; ta->tokens_used = opts->tokens_used; ta->keep = opts->keep_rows; ta->row_loss = opts->row_loss;
+    CAPB_REQUIRE(ta->ss_prob >= 0.f && ta->ss_prob <= 1.f, "ss_prob must be in [0, 1]");
+    CAPB_REQUIRE(ta->keep >= 0 && ta->keep <= B * opts->seq_per_img, "keep_rows must be in 0..rows");
+    return 0;
+}
+
 }  // namespace
 
 extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
@@ -1568,18 +1747,9 @@ extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, cons
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_UPDOWN, "the SCST step is implemented for the UpDown family");
     CAPB_REQUIRE(opts && fc && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
-    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
-    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
-    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
-    CAPB_REQUIRE(greedy_baseline || opts->sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
-    CAPB_REQUIRE(opts->sample_n >= 1 && opts->sample_n <= 16 && B >= 1 && R >= 1, "sample_n must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
+    CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    ta.n = opts->sample_n; ta.T = e->T; ta.Tl = e->T; ta.p = opts->drop_prob; ta.temperature = opts->temperature; ta.upstream = opts->upstream;
-    ta.seed = opts->seed; ta.greedy_baseline = greedy_baseline; ta.table = table; ta.refs = refs; ta.ref_offsets = ref_offsets; ta.L = L;
-    ta.sample_seq = sample_seq; ta.greedy_seq = greedy_seq; ta.reward = reward; ta.logprobs = sample_logprobs; ta.loss = loss;
-    ta.forced = opts->forced_tokens; ta.mask = opts->att_masks; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->sample_n, "keep_rows must be in 0..rows");
+    if (scst_train_args(B, opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // the whole step as one CUDA graph (see capb200_aoa_scst_step and engine_common.cuh: StepGraph)
     if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
@@ -1615,18 +1785,9 @@ extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, con
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_ATT2IN2, "capb200_att2in2_scst_step needs an Att2in2 engine");
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
-    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
-    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
-    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
-    CAPB_REQUIRE(greedy_baseline || opts->sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
-    CAPB_REQUIRE(opts->sample_n >= 1 && opts->sample_n <= 16 && B >= 1 && R >= 1, "sample_n must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
+    CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    ta.n = opts->sample_n; ta.T = e->T; ta.Tl = e->T; ta.p = opts->drop_prob; ta.temperature = opts->temperature; ta.upstream = opts->upstream;
-    ta.seed = opts->seed; ta.greedy_baseline = greedy_baseline; ta.table = table; ta.refs = refs; ta.ref_offsets = ref_offsets; ta.L = L;
-    ta.sample_seq = sample_seq; ta.greedy_seq = greedy_seq; ta.reward = reward; ta.logprobs = sample_logprobs; ta.loss = loss;
-    ta.forced = opts->forced_tokens; ta.mask = opts->att_masks; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->sample_n, "keep_rows must be in 0..rows");
+    if (scst_train_args(B, opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // the whole step as one CUDA graph, as capb200_updown_scst_step (the fc features are not read: only att and the mask are staged)
     if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
@@ -1659,25 +1820,65 @@ extern "C" int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_ATT2IN2, "capb200_att2in2_xe_step needs an Att2in2 engine");
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
-    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1 && R >= 1, "seq_per_img must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
-    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
-    CAPB_REQUIRE(label_cols >= 2 && label_cols <= e->T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
-    CAPB_REQUIRE(opts->steps >= 1 && opts->steps <= label_cols - 1, "steps must be in 1..label_cols-1");
+    CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    ta.xe = true;
-    ta.n = opts->seq_per_img; ta.T = opts->steps; ta.Tl = label_cols - 1; ta.p = opts->drop_prob; ta.upstream = opts->upstream; ta.seed = opts->seed;
-    ta.smoothing = opts->label_smoothing;
-    ta.labels = labels; ta.ld_labels = label_cols; ta.masks = masks; ta.ld_masks = label_cols; ta.logprobs = logprobs; ta.loss = loss;
-    ta.mask = opts->att_masks; ta.ss_prob = opts->ss_prob; ta.tokens_used = opts->tokens_used; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.ss_prob >= 0.f && ta.ss_prob <= 1.f, "ss_prob must be in [0, 1]");
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->seq_per_img, "keep_rows must be in 0..rows");
+    if (xe_train_args(B, opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;
     return att2in2_train_step(e, fc, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
 }
 
+extern "C" int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
+                                       const capb200_scst_opts* opts, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                                       const capb200_newfc_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
+                                       float* reward, float* loss, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_NEWFC, "capb200_newfc_scst_step needs a NewFC engine");
+    CAPB_REQUIRE(opts && fc && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
+    CAPB_REQUIRE(R >= 0, "R must be >= 0");
+    CAPB_REQUIRE(opts->att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
+    TrainArgs ta;
+    if (scst_train_args(B, opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the whole step as one CUDA graph, as capb200_updown_scst_step (only the fc features are staged)
+    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
+        if (dropout_salt_set_all(0ull, st)) return 1;
+        return newfc_train_step(e, fc, B, ta, grads, st);
+    }
+    cudaStream_t gst = e->sg.enter(st);
+    const void* srcs[1] = {fc};
+    const size_t bytes[1] = {sizeof(float) * (size_t)B * e->cfg.fc_feat_size};
+    size_t off[1];
+    if (e->sg.stage_inputs(1, srcs, bytes, off, gst)) return 1;
+    const float* fc_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
+    unsigned long long key = 1469598103934665603ull;
+    capb200_scst_opts o2 = *opts; o2.seed = 0;
+    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
+    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
+    StepGraph::mix(key, ptrs, sizeof(ptrs));
+    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
+    const int dims[] = {B, L};
+    StepGraph::mix(key, dims, sizeof(dims));
+    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return newfc_train_step(e, fc_s, B, ta, grads, gst); });
+    if (e->sg.leave(st, gst)) return 1;
+    return rc_graph;
+}
+
+extern "C" int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
+                                     const capb200_xe_opts* opts, const long long* labels, const float* masks, int label_cols,
+                                     const capb200_newfc_grads* grads, float* logprobs, float* loss, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_NEWFC, "capb200_newfc_xe_step needs a NewFC engine");
+    CAPB_REQUIRE(opts && fc && labels && masks && grads && logprobs && loss, "null argument");
+    CAPB_REQUIRE(R >= 0, "R must be >= 0");
+    CAPB_REQUIRE(opts->att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
+    TrainArgs ta;
+    if (xe_train_args(B, opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
+    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;
+    return newfc_train_step(e, fc, B, ta, grads, static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n) {
-    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 2, "UpDown and Att2in2 have 2 gradient groups");
+    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 2, "UpDown, Att2in2 and NewFC have 2 gradient groups");
     for (int i = 0; i < 2; ++i) e->grad_events[i] = (events != nullptr && i < n) ? static_cast<cudaEvent_t>(events[i]) : nullptr;
     return 0;
 }
@@ -1688,19 +1889,9 @@ extern "C" int capb200_updown_xe_step(capb200_engine* e, const float* fc, const 
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_UPDOWN, "the XE step is implemented for the UpDown family");
     CAPB_REQUIRE(opts && fc && att && labels && masks && grads && logprobs && loss, "null argument");
-    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1 && R >= 1, "seq_per_img must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
-    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
-    CAPB_REQUIRE(label_cols >= 2 && label_cols <= e->T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
-    CAPB_REQUIRE(opts->steps >= 1 && opts->steps <= label_cols - 1, "steps must be in 1..label_cols-1");
+    CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    ta.xe = true;
-    ta.n = opts->seq_per_img; ta.T = opts->steps; ta.Tl = label_cols - 1; ta.p = opts->drop_prob; ta.upstream = opts->upstream; ta.seed = opts->seed;
-    ta.smoothing = opts->label_smoothing;
-    ta.labels = labels; ta.ld_labels = label_cols; ta.masks = masks; ta.ld_masks = label_cols; ta.logprobs = logprobs; ta.loss = loss;
-    ta.mask = opts->att_masks; ta.ss_prob = opts->ss_prob; ta.tokens_used = opts->tokens_used; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.ss_prob >= 0.f && ta.ss_prob <= 1.f, "ss_prob must be in [0, 1]");
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->seq_per_img, "keep_rows must be in 0..rows");
+    if (xe_train_args(B, opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;      // eager step: the seed arguments are the effective seeds
     return updown_train_step(e, fc, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
 }

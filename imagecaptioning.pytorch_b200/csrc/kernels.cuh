@@ -192,6 +192,7 @@ int attention_backward_launch(int n_images, int rpi, int R, int A, int H, const 
                               cudaStream_t st);
 int relu_dropout_backward_launch(long n, const float* x, const float* dy, float* dx, float scale, cudaStream_t st);
 int embed_backward_launch(int rows, int E, const int* tokens, const float* xt, const float* dxt, long ld_dxt, float scale, float* d_emb, cudaStream_t st);
+int embed_scatter_launch(int rows, int E, const int* tokens, const float* dxt, long ld_dxt, float* d_emb, cudaStream_t st);   // ungated (bare nn.Embedding)
 int per_image_sum_launch(int steps, int rows, int rpi, int cols, const float* x, float* out, cudaStream_t st);
 int add_strided_launch(float* a, const float* b, long ld_b, int rows, int cols, cudaStream_t st);
 

@@ -5,7 +5,7 @@
 //   dropout sites            models/AttModel.py:74-88 (embed / fc_embed / att_embed Sequentials), :637 (core output)
 //   dlogits                  modules/losses.py:22-37 (RewardCriterion) composed with F.log_softmax (AttModel.py:172)
 //   lstm_cell_backward       nn.LSTMCell (AttModel.py:628,635)
-//   maxout_cell_backward     Att2in2Core's maxout cell (AttModel.py:773-787)
+//   maxout_cell_backward     Att2in2Core's maxout cell (AttModel.py:773-787) and NewFC's LSTMCore (FCModel.py:25-42)
 //   attention_backward       models/AttModel.py:728-748
 // Dropout masks are never stored: keep(seed, site, step, element) is a pure function (Philox4x32-10), re-evaluated in the backward.
 #include "common.cuh"
@@ -366,6 +366,13 @@ __global__ void embed_backward_kernel(int rows, int E, const int* __restrict__ t
     }
 }
 
+// d_emb[tok[r], :] += d_xt[r, :]: backward of a bare nn.Embedding lookup (NewFC, AttModel.py:908), no ReLU gate and no dropout
+__global__ void embed_scatter_kernel(int rows, int E, const int* __restrict__ tokens, const float* __restrict__ dxt, long ld_dxt, float* __restrict__ d_emb) {
+    const int r = blockIdx.x;
+    float* d = d_emb + (long)tokens[r] * E;
+    for (int c = threadIdx.x; c < E; c += blockDim.x) atomicAdd(d + c, dxt[(long)r * ld_dxt + c]);
+}
+
 // out[img, c] (+)= sum over the image's rows and all steps of x[step][row, c]
 // grid (images, column slices of 256): one column per thread, the steps x rpi terms of a column four loads at a time
 // (the first version ran one CTA per image over all columns: 10 CTAs for the whole GPU, 196 us for [20 x 50 x 4096])
@@ -482,6 +489,10 @@ int relu_dropout_backward_launch(long n, const float* x, const float* dy, float*
 }
 int embed_backward_launch(int rows, int E, const int* tokens, const float* xt, const float* dxt, long ld_dxt, float scale, float* d_emb, cudaStream_t st) {
     embed_backward_kernel<<<rows, 128, 0, st>>>(rows, E, tokens, xt, dxt, ld_dxt, scale, d_emb);
+    LAUNCH_OK();
+}
+int embed_scatter_launch(int rows, int E, const int* tokens, const float* dxt, long ld_dxt, float* d_emb, cudaStream_t st) {
+    embed_scatter_kernel<<<rows, 128, 0, st>>>(rows, E, tokens, dxt, ld_dxt, d_emb);
     LAUNCH_OK();
 }
 int per_image_sum_launch(int steps, int rows, int rpi, int cols, const float* x, float* out, cudaStream_t st) {

@@ -7,7 +7,7 @@ sc_flag=True follows loss_wrapper.py:56-73 exactly: eval-mode greedy baseline, t
 self-critical reward and RewardCriterion -- every stage on the device through the C ABI.  sc_flag=False is the XE stage
 (loss_wrapper.py:54-55: teacher-forced forward + LanguageModelCriterion / LabelSmoothing) and struc_flag=True the structure-loss
 branch (loss_wrapper.py:25-53) with ``structure_loss_type='new_self_critical'`` (losses.py:168-187), the recipe of the reference's
-best models; both run as one fused device step incl. the backward pass (UpDown, AoANet, Transformer).
+best models; both run as one fused device step incl. the backward pass (UpDown, Att2in2, NewFC, AoANet, Transformer).
 """
 from __future__ import annotations
 
@@ -249,7 +249,7 @@ class B200LossWrapper(nn.Module):
         """loss_wrapper.py:54-55: crit(model(fc, att, labels[..., :-1], att_masks), labels[..., 1:], masks[..., 1:])."""
         if torch.is_grad_enabled() and self.model.training:
             if not hasattr(self.model, 'xe_step'):
-                raise NotImplementedError('the fused XE step covers the UpDown, Att2in2, AoANet and Transformer families')
+                raise NotImplementedError('the fused XE step covers the UpDown, Att2in2, NewFC, AoANet and Transformer families')
             rows = labels.shape[0] * (labels.shape[1] if labels.dim() == 3 else 1)
             keep = self._keep_rows(rows, drop_worst_flag)
             res = self.model.xe_step(fc_feats, att_feats, labels, masks, label_smoothing=getattr(self.opt, 'label_smoothing', 0), att_masks=att_masks,
@@ -313,7 +313,7 @@ class B200LossWrapper(nn.Module):
             # silently trains nothing) at backward()
             why = []
             if not hasattr(self.model, 'scst_step'):
-                why.append('model family %r has no fused SCST step (UpDown, Att2in2, AoANet and Transformer do)' % getattr(self.model, 'family_name', type(self.model).__name__))
+                why.append('model family %r has no fused SCST step (UpDown, Att2in2, NewFC, AoANet and Transformer do)' % getattr(self.model, 'family_name', type(self.model).__name__))
             if not plain_reward:
                 why.append('cider_reward_weight != 1 or bleu_reward_weight != 0')
             if opt.train_sample_method != 'sample' or opt.train_beam_size != 1:

@@ -499,51 +499,17 @@ class _LazyDoneBeams(list):
         return self._B
 
 
-class _UpDownCoreParams(nn.Module):
-    """Parameter container with the key names of UpDownCore + Attention (AttModel.py:615-622,719-726)."""
+class _FusedTrainSteps:
+    """The fused XE / SCST training steps of the families that share UpDown's option structs (include/capb200.h: capb200_scst_opts,
+    capb200_xe_opts): UpDown, Att2in2 and NewFC.  A class sets its C entry points (_scst_entry, _xe_entry) and gradient table
+    (_grads_struct, _grad_fields)."""
 
-    def __init__(self, opt):
-        super().__init__()
-        self.att_lstm = nn.LSTMCell(opt.input_encoding_size + opt.rnn_size * 2, opt.rnn_size)
-        self.lang_lstm = nn.LSTMCell(opt.rnn_size * 2, opt.rnn_size)
-        self.attention = nn.Module()
-        self.attention.h2att = nn.Linear(opt.rnn_size, opt.att_hid_size)
-        self.attention.alpha_net = nn.Linear(opt.att_hid_size, 1)
-
-
-class B200UpDownModel(B200CaptionModel):
-    """Drop-in for captioning.models.AttModel.UpDownModel (AttModel.py:868-872)."""
-
-    family = _lib.FAMILY_UPDOWN
-    family_name = 'updown'
-    # C entry points and gradient table of the fused training steps (include/capb200.h)
-    _scst_entry, _xe_entry = 'capb200_updown_scst_step', 'capb200_updown_xe_step'
-    _grads_struct, _grad_fields = _lib.UpdownGrads, _lib.GRAD_FIELDS
-
-    def __init__(self, opt, numeric_mode=None):
-        super().__init__(opt, numeric_mode)
-        self.num_layers = 2
-        V1 = self.vocab_size + 1
-        self.embed = nn.Sequential(nn.Embedding(V1, self.input_encoding_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
-        self.fc_embed = nn.Sequential(nn.Linear(self.fc_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
-        self.att_embed = nn.Sequential(nn.Linear(self.att_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
-        self.logit = nn.Linear(self.rnn_size, V1)
-        self.ctx2att = nn.Linear(self.rnn_size, self.att_hid_size)
-        self.core = _UpDownCoreParams(opt)
-
-    def _weight_table(self):
-        c = self.core
-        return {
-            'embed': self.embed[0].weight, 'fc_embed_w': self.fc_embed[0].weight, 'fc_embed_b': self.fc_embed[0].bias,
-            'att_embed_w': self.att_embed[0].weight, 'att_embed_b': self.att_embed[0].bias,
-            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
-            'att_lstm_w_ih': c.att_lstm.weight_ih, 'att_lstm_w_hh': c.att_lstm.weight_hh, 'att_lstm_b_ih': c.att_lstm.bias_ih,
-            'att_lstm_b_hh': c.att_lstm.bias_hh, 'lang_lstm_w_ih': c.lang_lstm.weight_ih, 'lang_lstm_w_hh': c.lang_lstm.weight_hh,
-            'lang_lstm_b_ih': c.lang_lstm.bias_ih, 'lang_lstm_b_hh': c.lang_lstm.bias_hh,
-            'h2att_w': c.attention.h2att.weight, 'h2att_b': c.attention.h2att.bias,
-            'alpha_w': c.attention.alpha_net.weight, 'alpha_b': c.attention.alpha_net.bias,
-        }
-
+    def _train_feats(self, fc_feats, att_feats, att_masks):
+        """(fc, att, region masks, B, R) as the training step reads them: clip_att cuts the region axis to the longest valid length
+        (AttModel.py:106-112)."""
+        fc = self._f32(fc_feats)
+        att, masks = self._clip(att_feats, att_masks)
+        return fc, att, masks, att.shape[0], att.shape[1]
 
     def _grad_groups(self):
         t = self._weight_table()
@@ -551,7 +517,8 @@ class B200UpDownModel(B200CaptionModel):
         return [[(k, t[k]) for k in first], [(k, v) for k, v in t.items() if k not in first]]
 
     def _grad_table(self, lib, device):
-        """capb200_updown_grads (capb200_att2in2_grads) pointing into the persistent flat buffer, the group events registered with the engine."""
+        """The family's gradient table (capb200_updown_grads, capb200_att2in2_grads, capb200_newfc_grads) pointing into the persistent flat
+        buffer, the group events registered with the engine."""
         fg = self._flat_grads(device)
         g = self._grads_struct()
         for name in self._grad_fields:
@@ -561,21 +528,19 @@ class B200UpDownModel(B200CaptionModel):
         _lib.check(lib.capb200_engine_set_grad_events(self._engine, table, n), 'set_grad_events')
         return fg, g
 
-    # ---- SCST training step (UpDown): greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----
+    # ---- SCST training step: greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----------------
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
                   forced_tokens=None, att_masks=None, keep_rows=0):
-        """Runs one self-critical step entirely on the device (capb200_updown_scst_step).  Returns a dict with 'loss' (0-dim),
-        'reward' [N, T], 'sample_seq', 'greedy_seq', 'sample_logprobs' and 'grads' {parameter: gradient tensor}.
+        """Runs one self-critical step entirely on the device (capb200_updown_scst_step and its Att2in2 / NewFC counterparts).  Returns a
+        dict with 'loss' (0-dim), 'reward' [N, T], 'sample_seq', 'greedy_seq', 'sample_logprobs' and 'grads' {parameter: gradient tensor}.
         ``baseline='greedy'`` is the self-critical step (loss_wrapper.py:56-73); ``'leave_one_out'`` the 'new_self_critical' structure
         loss (losses.py:168-187): no greedy decode, each sample is scored against the mean of the image's other samples, and the
         result carries 'scores' [B, n] (the raw CIDEr-D values the reference reports as out['reward'])."""
         from .rewards import pack_references
         lib = self._ensure_engine(fc_feats.device)
-        fc = self._f32(fc_feats)
-        att, masks = self._clip(att_feats, att_masks)          # clip_att: cut the region axis to the longest valid length (AttModel.py:106-112)
+        fc, att, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
         dev = fc.device
-        B, R = att.shape[0], att.shape[1]
         N, T, V1 = B * sample_n, self.seq_length, self.vocab_size + 1
         refs, offsets, L = pack_references(gts, dev)
         table_params = self._weight_table()
@@ -608,14 +573,12 @@ class B200UpDownModel(B200CaptionModel):
 
     @_on_device
     def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, att_masks=None, keep_rows=0):
-        """One cross-entropy step on the device (capb200_updown_xe_step): teacher-forced forward over ``labels[..., :-1]`` in train mode,
+        """One cross-entropy step on the device (capb200_updown_xe_step and its Att2in2 / NewFC counterparts): teacher-forced forward over ``labels[..., :-1]`` in train mode,
         LanguageModelCriterion / LabelSmoothing against ``labels[..., 1:]``, ``masks[..., 1:]`` (reduction 'mean'), BPTT.
         Returns {'loss', 'logprobs' [N, L-1, V+1], 'grads' {parameter: gradient}, 'seed'}."""
         lib = self._ensure_engine(fc_feats.device)
-        fc = self._f32(fc_feats)
-        att, region_masks = self._clip(att_feats, att_masks)
+        fc, att, region_masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
         dev = fc.device
-        B, R = att.shape[0], att.shape[1]
         if labels.dim() == 3:
             labels = labels.reshape(-1, labels.shape[2])
             masks = masks.reshape(-1, masks.shape[2])
@@ -643,6 +606,52 @@ class B200UpDownModel(B200CaptionModel):
                                                 ctypes.byref(g), _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), self._xe_entry[len('capb200_'):])
         return {'loss': loss[0], 'logprobs': logprobs, 'grads': {table_params[k]: grads[k] for k in table_params}, 'seed': seed, 'flat': fg,
                 'tokens_used': tokens_used, 'row_loss': row_loss}
+
+
+class _UpDownCoreParams(nn.Module):
+    """Parameter container with the key names of UpDownCore + Attention (AttModel.py:615-622,719-726)."""
+
+    def __init__(self, opt):
+        super().__init__()
+        self.att_lstm = nn.LSTMCell(opt.input_encoding_size + opt.rnn_size * 2, opt.rnn_size)
+        self.lang_lstm = nn.LSTMCell(opt.rnn_size * 2, opt.rnn_size)
+        self.attention = nn.Module()
+        self.attention.h2att = nn.Linear(opt.rnn_size, opt.att_hid_size)
+        self.attention.alpha_net = nn.Linear(opt.att_hid_size, 1)
+
+
+class B200UpDownModel(_FusedTrainSteps, B200CaptionModel):
+    """Drop-in for captioning.models.AttModel.UpDownModel (AttModel.py:868-872)."""
+
+    family = _lib.FAMILY_UPDOWN
+    family_name = 'updown'
+    # C entry points and gradient table of the fused training steps (include/capb200.h)
+    _scst_entry, _xe_entry = 'capb200_updown_scst_step', 'capb200_updown_xe_step'
+    _grads_struct, _grad_fields = _lib.UpdownGrads, _lib.GRAD_FIELDS
+
+    def __init__(self, opt, numeric_mode=None):
+        super().__init__(opt, numeric_mode)
+        self.num_layers = 2
+        V1 = self.vocab_size + 1
+        self.embed = nn.Sequential(nn.Embedding(V1, self.input_encoding_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
+        self.fc_embed = nn.Sequential(nn.Linear(self.fc_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
+        self.att_embed = nn.Sequential(nn.Linear(self.att_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
+        self.logit = nn.Linear(self.rnn_size, V1)
+        self.ctx2att = nn.Linear(self.rnn_size, self.att_hid_size)
+        self.core = _UpDownCoreParams(opt)
+
+    def _weight_table(self):
+        c = self.core
+        return {
+            'embed': self.embed[0].weight, 'fc_embed_w': self.fc_embed[0].weight, 'fc_embed_b': self.fc_embed[0].bias,
+            'att_embed_w': self.att_embed[0].weight, 'att_embed_b': self.att_embed[0].bias,
+            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
+            'att_lstm_w_ih': c.att_lstm.weight_ih, 'att_lstm_w_hh': c.att_lstm.weight_hh, 'att_lstm_b_ih': c.att_lstm.bias_ih,
+            'att_lstm_b_hh': c.att_lstm.bias_hh, 'lang_lstm_w_ih': c.lang_lstm.weight_ih, 'lang_lstm_w_hh': c.lang_lstm.weight_hh,
+            'lang_lstm_b_ih': c.lang_lstm.bias_ih, 'lang_lstm_b_hh': c.lang_lstm.bias_hh,
+            'h2att_w': c.attention.h2att.weight, 'h2att_b': c.attention.h2att.bias,
+            'alpha_w': c.attention.alpha_net.weight, 'alpha_b': c.attention.alpha_net.bias,
+        }
 
 
 class _Att2in2CoreParams(nn.Module):
@@ -698,11 +707,15 @@ class _MaxoutCoreParams(nn.Module):
         self.h2h = nn.Linear(opt.rnn_size, 5 * opt.rnn_size)
 
 
-class B200NewFCModel(B200CaptionModel):
-    """Drop-in for captioning.models.AttModel.NewFCModel (AttModel.py:904-945)."""
+class B200NewFCModel(_FusedTrainSteps, B200CaptionModel):
+    """Drop-in for captioning.models.AttModel.NewFCModel (AttModel.py:904-945).  The fused XE / SCST steps take UpDown's surface; the
+    model reads the fc features only, so ``att_feats`` of any shape (the loader's [B, 0, 0] included) and ``att_masks`` are ignored, as
+    in the reference (its _prepare_feature has no clip_att)."""
 
     family = _lib.FAMILY_NEWFC
     family_name = 'newfc'
+    _scst_entry, _xe_entry = 'capb200_newfc_scst_step', 'capb200_newfc_xe_step'
+    _grads_struct, _grad_fields = _lib.NewfcGrads, _lib.NEWFC_GRAD_FIELDS
     _no_diverse = ("the engine chooses NewFC's fresh-state pass (the image-embedding step, AttModel.py:925-936) per core call, not per row, "
                    "so its groups cannot start at different steps")
 
@@ -720,6 +733,10 @@ class B200NewFCModel(B200CaptionModel):
             'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
             'i2h_w': self._core.i2h.weight, 'i2h_b': self._core.i2h.bias, 'h2h_w': self._core.h2h.weight, 'h2h_b': self._core.h2h.bias,
         }
+
+    def _train_feats(self, fc_feats, att_feats, att_masks):
+        fc = self._f32(fc_feats)
+        return fc, None, None, fc.shape[0], 0
 
 
 def _mha_params(d_model):

@@ -82,4 +82,8 @@ class FusedAdam(torch.optim.Adam):
                                                      float(self.clip_value) if self.clip_value else 0.0, 1 if self.write_clamped_grad else 0,
                                                      _lib.current_stream()), 'adam_step')
                 self.launches += 1
+                # the kernel writes the parameters through raw pointers: bump their version counters as an in-place torch op would, so the
+                # engines see new weights and re-bind their derived copies (fp16 planes, bias sums) before the next call
+                for p in ps:
+                    torch.autograd.graph.increment_version(p)
         return loss

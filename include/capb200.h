@@ -340,8 +340,8 @@ typedef struct {
 /* fc[B,F_fc], att[B,R,F_att] (opts->att_masks for variable region counts); refs as in capb200_self_critical_reward.
  * Outputs: sample_seq[B*n,T] int64, greedy_seq[B,T] int64, sample_logprobs[B*n,T,V+1] (caller zero-fills), reward[B*n,T], loss[1].
  * Execution: the whole step (~900-4900 launches, none of them data dependent) is captured into ONE CUDA graph the second time a configuration
- * -- shapes, every pointer argument, every option except the seed -- is seen, and replayed afterwards (the *_scst_step entry points of all
- * three families; CAPB200_SCST_GRAPH=0 disables it).  For that the step runs on an engine-owned stream that first waits for `stream` and that
+ * -- shapes, every pointer argument, every option except the seed -- is seen, and replayed afterwards (the *_scst_step entry points of every
+ * family; CAPB200_SCST_GRAPH=0 disables it).  For that the step runs on an engine-owned stream that first waits for `stream` and that
  * `stream` is made to wait for before the call returns; the features (and the region mask) are copied into an engine-owned staging buffer, so
  * they may live anywhere, while refs / ref_offsets / the output and gradient buffers should keep their addresses from step to step (a changed
  * address is a new configuration: one eager step, one capture).  A replay draws new samples and masks from opts->seed exactly as the eager
@@ -393,6 +393,26 @@ int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, const float* a
                               long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, void* stream);
 int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const long long* labels,
                             const float* masks, int label_cols, const capb200_att2in2_grads* grads, float* logprobs, float* loss, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Training steps of the NewFC model (NewFCModel, AttModel.py:904-945, with FCModel.LSTMCore, FCModel.py:13-42), same contracts as the UpDown
+ * steps above: an engine of CAPB200_FAMILY_NEWFC; the options mean what they mean for UpDown (greedy or leave-one-out baseline, forced tokens,
+ * keep_rows / row_loss, scheduled sampling with tokens_used, label smoothing).  The model reads the fc features only: `att` is ignored (NULL
+ * with R = 0 is fine) and a non-NULL opts->att_masks is refused.  The core first consumes fc_embed(fc) from a zero state (once per image),
+ * then <bos> and the words; the only dropout is site 3, the core output (replayable through capb200_dropout_mask).  The SCST step is captured
+ * into one CUDA graph as capb200_updown_scst_step describes.  Gradient groups: see capb200_engine_set_grad_events.
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* Gradient buffers of the 9 NewFC parameters (same shapes as the capb200_weights fields, fp32, device); every one is OVERWRITTEN. */
+typedef struct {
+    float* embed;
+    float *fc_embed_w, *fc_embed_b, *logit_w, *logit_b;
+    float *i2h_w, *i2h_b, *h2h_w, *h2h_b;
+} capb200_newfc_grads;
+int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                            const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L, const capb200_newfc_grads* grads,
+                            long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, void* stream);
+int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const long long* labels,
+                          const float* masks, int label_cols, const capb200_newfc_grads* grads, float* logprobs, float* loss, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * One self-critical training step of the AoANet model (BASELINE configs[3]): LossWrapper.forward with sc_flag (loss_wrapper.py:56-73)
@@ -464,7 +484,7 @@ int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int B, int R, c
  * same way).  A training step finishes its gradient buffers in a fixed order of groups; after the last write of group k it records
  * events[k] (cudaEvent_t, caller-owned) on the step's stream, so a communication stream can all-reduce group k while the rest of the
  * backward pass still runs.  n = 0 or events = NULL switches the recording off.  Groups:
- *   UpDown and Att2in2 (capb200_engine_set_grad_events, n <= 2): 0 logit.{weight,bias}; 1 every other parameter.
+ *   UpDown, Att2in2 and NewFC (capb200_engine_set_grad_events, n <= 2): 0 logit.{weight,bias}; 1 every other parameter.
  *   AoANet (capb200_aoa_set_grad_events, n <= 10):  0 logit; 1 decoder (att2ctx, attention q-projection and norm, att_lstm) + embed;
  *           2 ctx2att + refiner.norm; 3..8 refiner layers 5..0; 9 att_embed. */
 int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n);
@@ -472,7 +492,7 @@ int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* events, int 
 
 /* The dropout keep/scale mask (0 or 1/(1-p)) of one site and step, for tests that replay it in the oracle:
  * site 0 = fc_embed [B,H], 1 = att_embed [B*R,H], 2 = word embedding at `step` [N,E], 3 = core output at `step` [N,H].
- * (Att2in2 has no site 0: it has no fc_embed.) */
+ * (Att2in2 has no site 0: it has no fc_embed.  NewFC has site 3 only: its embeddings are a bare nn.Embedding / nn.Linear.) */
 int capb200_dropout_mask(float* mask, long n, unsigned long long seed, int site, int step, float p, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
