@@ -14,6 +14,7 @@
 #include "common.cuh"
 #include "engine_common.cuh"
 #include "kernels.cuh"
+#include "train_common.cuh"
 
 using namespace capb200;
 
@@ -498,17 +499,13 @@ namespace {
 
 constexpr int NL = CAPB200_AOA_REFINER_LAYERS;
 
-struct ATape {
+struct ATape : StepTape {
     float *x[NL + 1], *ln[NL], *qkv[NL], *ratt[NL], *catd[NL], *t[NL], *g[NL];
     float *att_e, *mean, *kv;
     int* tok;
     float *xt, *x1c, *gates, *c, *h, *qln, *qp, *probs, *att, *t2, *out, *outd;
-    float *DL, *dOUTD, *D_T2, *D_QP, *DG, *dctx, *dh, *dc, *dX2, *d_qln, *d_hatt, *dxt, *d_x1c, *S, *d_mean, *d_kv, *d_att_e, *d_x, *d_g, *d_t,
-        *d_catd, *d_qkv, *d_ln, *dpre, *stats, *mask_sum, *skinny, *glp, *item_loss;
-    size_t skinny_floats;
-    double* scores;
-    int *s_tokens, *s_unfinished, *s_forced;   // sampling-loop state (own copies: the greedy baseline runs concurrently on the decode workspace)
-    float *row_loss, *row_msum, *row_coef;     // drop_worst
+    float *dOUTD, *D_T2, *D_QP, *DG, *dctx, *dh, *dc, *dX2, *d_qln, *d_hatt, *dxt, *d_x1c, *S, *d_mean, *d_kv, *d_att_e, *d_x, *d_g, *d_t,
+        *d_catd, *d_qkv, *d_ln, *dpre, *stats;
 };
 
 void layout_atape(ATape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int heads, int V1) {
@@ -523,7 +520,8 @@ void layout_atape(ATape& tp, Arena& a, int B, int R, int N, int T, int E, int H,
     tp.xt = a.take<float>(TN * E); tp.x1c = a.take<float>(TN * H); tp.gates = a.take<float>(TN * 4 * H); tp.c = a.take<float>(TN * H);
     tp.h = a.take<float>(TN * H); tp.qln = a.take<float>(TN * H); tp.qp = a.take<float>(TN * H); tp.probs = a.take<float>(TN * heads * R);
     tp.att = a.take<float>(TN * H); tp.t2 = a.take<float>(TN * 2 * H); tp.out = a.take<float>(TN * H); tp.outd = a.take<float>(TN * H);
-    tp.DL = a.take<float>(TN * V1); tp.dOUTD = a.take<float>(TN * H); tp.D_T2 = a.take<float>(TN * 2 * H); tp.D_QP = a.take<float>(TN * H);
+    tp.layout(a, B, N, TN, V1, (long)B * T * V1);
+    tp.dOUTD = a.take<float>(TN * H); tp.D_T2 = a.take<float>(TN * 2 * H); tp.D_QP = a.take<float>(TN * H);
     tp.DG = a.take<float>(TN * 4 * H);
     const long NH = (long)N * H;
     tp.dctx = a.take<float>(NH); tp.dh = a.take<float>(NH); tp.dc = a.take<float>(NH); tp.dX2 = a.take<float>(2 * NH);
@@ -531,51 +529,18 @@ void layout_atape(ATape& tp, Arena& a, int B, int R, int N, int T, int E, int H,
     tp.S = a.take<float>((long)B * 4 * H); tp.d_mean = a.take<float>((long)B * H); tp.d_kv = a.take<float>(BR * 2 * H); tp.d_att_e = a.take<float>(BR * H);
     tp.d_x = a.take<float>(BR * H); tp.d_g = a.take<float>(BR * H); tp.d_t = a.take<float>(BR * 2 * H); tp.d_catd = a.take<float>(BR * 2 * H);
     tp.d_qkv = a.take<float>(BR * 3 * H); tp.d_ln = a.take<float>(BR * H); tp.dpre = a.take<float>(BR * H);
-    tp.stats = a.take<float>(2 * (BR > N ? BR : N)); tp.mask_sum = a.take<float>(8);
-    tp.skinny_floats = (size_t)4 << 20;
-    tp.skinny = a.take<float>((long)tp.skinny_floats);
-    tp.glp = a.take<float>((long)B * T * V1);
-    tp.item_loss = a.take<float>(TN);
-    tp.scores = a.take<double>((long)N + B);
-    tp.s_tokens = a.take<int>(N); tp.s_unfinished = a.take<int>(N); tp.s_forced = a.take<int>(N);
-    tp.row_loss = a.take<float>(N); tp.row_msum = a.take<float>(N); tp.row_coef = a.take<float>(N);
+    tp.stats = a.take<float>(2 * (BR > N ? BR : N));
 }
 
-// dW[out, in] (+)= dY[rows, out]^T * X[rows, in]
-inline int wgrad_mode(int out_f, int in_f, int rows, const float* dY, long ld_dy, const float* X, long ld_x, float* G, long ld_g, int accumulate, int mode,
-                      cudaStream_t st) {
-    return gemm_wgrad_launch(out_f, in_f, rows, dY, ld_dy, X, ld_x, G, ld_g, accumulate, mode, st);
-}
-
-}  // namespace
-
-namespace {
-
-struct AoaTrainArgs {
-    bool xe = false;
-    int n = 1, T = 0, Tl = 0;              // rows per image, steps evaluated, log-prob columns
-    float p_lm = 0.f, p_at = 0.f, p_aoa = 0.f, p_sub = 0.f, temperature = 1.f, upstream = 1.f, smoothing = 0.f;
+// the shared arguments (p = drop_prob_lm) and AoANet's other dropout rates
+struct AoaTrainArgs : TrainArgs {
+    float p_at = 0.f, p_aoa = 0.f, p_sub = 0.f;
     int ctx_drop = 0;
-    unsigned long long seed = 0;
-    bool greedy_baseline = true;
-    const capb200_cider_table* table = nullptr;
-    const int* refs = nullptr; const int* ref_offsets = nullptr; int L = 0;
-    long long* sample_seq = nullptr; long long* greedy_seq = nullptr; float* reward = nullptr;
-    const long long* forced = nullptr;
-    const float* mask = nullptr;           // [B, R] region mask or null
-    float ss_prob = 0.f;
-    long long* tokens_used = nullptr;
-    int keep = 0;
-    float* row_loss = nullptr;
-    const long long* labels = nullptr; long ld_labels = 0; const float* masks = nullptr; long ld_masks = 0;
-    float* logprobs = nullptr; float* loss = nullptr;
 };
 
 int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const AoaTrainArgs& ta, const capb200_aoa_grads* grads, cudaStream_t st) {
-    void* stream = static_cast<void*>(st);
-    const bool greedy_baseline = !ta.xe && ta.greedy_baseline;
     const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, V1 = e->V1, F = e->F, heads = e->heads, dk = e->dk;
-    const float p_lm = ta.p_lm, p_at = ta.p_at, p_aoa = ta.p_aoa, p_sub = ta.p_sub;
+    const float p_lm = ta.p, p_at = ta.p_at, p_aoa = ta.p_aoa, p_sub = ta.p_sub;
     const float p_ctx = ta.ctx_drop ? p_lm : 0.f;
     const float keep_lm = 1.0f / (1.0f - p_lm);
     const unsigned long long seed = ta.seed;
@@ -583,106 +548,51 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
     const capb200_aoa_grads& G = *grads;
     const long BR = (long)B * R, NH = (long)N * H, TN = (long)T * N;
     const long ld_lp = (long)ta.Tl * V1;
-    float* const sample_logprobs = ta.logprobs;
-    long long* const sample_seq = ta.sample_seq;
-    long long* const greedy_seq = ta.greedy_seq;
-    float* const reward = ta.reward;
-    float* const loss = ta.loss;
 
-    {
-        Arena dry; ATape t0; layout_atape(t0, dry, B, R, N, T, E, H, heads, V1);
-        if (dry.off + 256 > e->tape_bytes) {
-            CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-            if (e->tape) CAPB_CHECK_CUDA(cudaFree(e->tape));
-            e->tape = nullptr;
-            CAPB_CHECK_CUDA(cudaMalloc(&e->tape, dry.off + 256));
-            e->tape_bytes = dry.off + 256;
-        }
-    }
-    Arena ar; ar.base = e->tape;
-    ATape tp; layout_atape(tp, ar, B, R, N, T, E, H, heads, V1);
-
-    // ---- (1) greedy baseline, eval mode: the regular decode path, on a side stream (joins before the reward): it and the train-mode
-    // sampling forward are independent chains of small latency-bound kernels
+    ATape tp;
+    if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](ATape& t, Arena& a) { layout_atape(t, a, B, R, N, T, E, H, heads, V1); })) return 1;
+    // ---- (1) greedy baseline, eval mode: the regular decode path, forked here, enqueued after the prologue
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;         // decode workspace sized before anything is in flight
-    bool greedy_on_side = false;
-    cudaStream_t gs_enqueue = st;
-    capb200_sample_opts so;
-    if (greedy_baseline) {
-        CAPB_NVTX("capb200 aoa scst: greedy baseline (eval mode, side stream)");
-        memset(&so, 0, sizeof(so)); so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.seed = 0; so.steps = T;
-        cudaStream_t gs = st;
-        static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
-        if (!serial) {
-            bool ok = true;
-            if (e->side == nullptr) ok = create_side_stream(&e->side) == cudaSuccess;
-            if (ok && e->ev_fork == nullptr) ok = cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess;
-            if (ok && e->ev_join == nullptr) ok = cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) == cudaSuccess;
-            if (ok) {
-                CAPB_CHECK_CUDA(cudaEventRecord(e->ev_fork, st));
-                CAPB_CHECK_CUDA(cudaStreamWaitEvent(e->side, e->ev_fork, 0));
-                gs = e->side;
-                greedy_on_side = true;
-            } else (void)cudaGetLastError();
-        }
-        gs_enqueue = gs;
-    }
-    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
-    tf32_context_new_step(e->tf32);
+    GreedyBaseline gb;
+    if (gb.fork(ta, &e->side, &e->ev_fork, &e->ev_join, st)) return 1;
+    const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
-    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};
-    sk.ctx = e->tf32;
-    auto act = [](float* p, long ld) { ActView v; v.f = p; v.hi = nullptr; v.lo = nullptr; v.ld = ld; return v; };
-    const int wmode = e->tc ? 1 : 0;
-    auto wgrad = [&](int out_f, int in_f, int rows, const float* dY, long ld_dy, const float* X, long ld_x, float* Gp, long ld_g, int accumulate, cudaStream_t) {
-        return sk.wgrad(out_f, in_f, rows, dY, ld_dy, X, ld_x, Gp, ld_g, accumulate);
-    };
-    (void)wmode;
 
     // ---- (2) train-mode prologue: att_embed (+dropout), six refiner layers, final norm, mean pooling, ctx2att
     nvtxRangePushA("capb200 aoa train step: forward on the tape");
     if (sk.lin(att, F, w.att_embed_w, F, w.att_embed_b, tp.x[0], H, (int)BR, H, F, 0)) return 1;
-    if (relu_copy_launch(tp.x[0], BR * H, act(tp.x[0], H), st)) return 1;
+    if (relu_copy_launch(tp.x[0], BR * H, f32_view(tp.x[0], H), st)) return 1;
     if (dropout_apply_launch(tp.x[0], (int)BR, H, H, seed, 1, 0, p_lm, st)) return 1;
     if (ta.mask != nullptr) {      // pack_wrapper(att_embed): padded regions embed to exactly zero (AoAModel.py:211, AttModel.py:44-49)
-        if (mask_rows_launch(act(tp.x[0], H), B, R, H, ta.mask, R, st)) return 1;
+        if (mask_rows_launch(f32_view(tp.x[0], H), B, R, H, ta.mask, R, st)) return 1;
         e->launches++;
     }
     for (int l = 0; l < NL; ++l) {
         const capb200_aoa_refiner_layer& Lw = w.refiner[l];
-        if (layer_norm_launch((int)BR, H, tp.x[l], H, Lw.ln_a, Lw.ln_b, 1e-6f, act(tp.ln[l], H), st)) return 1;
+        if (layer_norm_launch((int)BR, H, tp.x[l], H, Lw.ln_a, Lw.ln_b, 1e-6f, f32_view(tp.ln[l], H), st)) return 1;
         if (sk.lin(tp.ln[l], H, e->r_qkv_w[l], H, e->r_qkv_b[l], tp.qkv[l], 3 * H, (int)BR, 3 * H, H, 0)) return 1;
         if (enc_attn_train_launch(B, R, heads, dk, tp.qkv[l], tp.qkv[l] + H, tp.qkv[l] + 2 * H, 3 * H, seed, 10 + l, p_at, tp.ratt[l], H, st, ta.mask, R)) return 1;
         if (cat_dropout_launch((int)BR, H, H, tp.ratt[l], H, tp.ln[l], H, tp.catd[l], 2 * H, seed, 20 + l, 0, p_aoa, st)) return 1;
         if (sk.lin(tp.catd[l], 2 * H, Lw.aoa_w, 2 * H, Lw.aoa_b, tp.t[l], 2 * H, (int)BR, 2 * H, 2 * H, 0)) return 1;
-        if (glu_launch((int)BR, H, tp.t[l], 2 * H, nullptr, 0, act(tp.g[l], H), st)) return 1;
+        if (glu_launch((int)BR, H, tp.t[l], 2 * H, nullptr, 0, f32_view(tp.g[l], H), st)) return 1;
         if (add_dropout_launch((int)BR, H, tp.x[l], H, tp.g[l], H, tp.x[l + 1], H, seed, 30 + l, 0, p_sub, st)) return 1;
         e->launches += 9;
     }
-    if (layer_norm_launch((int)BR, H, tp.x[NL], H, w.refiner_norm_a, w.refiner_norm_b, 1e-6f, act(tp.att_e, H), st)) return 1;
-    if (masked_mean_launch(B, R, H, tp.att_e, H, ta.mask, R, act(tp.mean, H), st)) return 1;
+    if (layer_norm_launch((int)BR, H, tp.x[NL], H, w.refiner_norm_a, w.refiner_norm_b, 1e-6f, f32_view(tp.att_e, H), st)) return 1;
+    if (masked_mean_launch(B, R, H, tp.att_e, H, ta.mask, R, f32_view(tp.mean, H), st)) return 1;
     if (sk.lin(tp.att_e, H, w.ctx2att_w, H, w.ctx2att_b, tp.kv, 2 * H, (int)BR, 2 * H, H, 0)) return 1;
     e->launches += 8;
 
     // ---- the greedy baseline's ~220 launches are enqueued only now: the side stream forked at the top of the step (it does not wait for the
     // prologue), but the host needs ~0.7 ms to enqueue them, and the main stream should be busy with the prologue meanwhile, not idle
-    if (greedy_baseline) {
-        CAPB_CHECK_CUDA(cudaMemsetAsync(tp.glp, 0, sizeof(float) * (size_t)B * T * V1, gs_enqueue));
-        CAPB_CHECK_CUDA(cudaMemsetAsync(greedy_seq, 0, sizeof(long long) * (size_t)B * T, gs_enqueue));
-        if (capb200_aoa_decode_sample(e, att, ta.mask, B, R, &so, nullptr, 0, greedy_seq, tp.glp, nullptr, static_cast<void*>(gs_enqueue))) return 1;
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaEventRecord(e->ev_join, e->side));
-    
-    }
+    if (gb.enqueue(B, T, V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, long long* seq, float* lp, void* s) {
+            return capb200_aoa_decode_sample(e, att, ta.mask, B, R, so, nullptr, 0, seq, lp, nullptr, s);
+        })) return 1;
     // ---- (3) T sampling steps with the tape
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
     for (int t = 0; t < T; ++t) {
         int* tok = tp.tok + (long)t * N;
-        if (ta.xe) {
-            if (t >= 1 && ta.ss_prob > 0.f) {      // scheduled sampling (AttModel.py:145-154)
-                if (ss_select_launch(N, V1, sample_logprobs + (long)(t - 1) * V1, ld_lp, ta.labels, ta.ld_labels, t, seed, ta.ss_prob, tok, st)) return 1;
-            } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
-            if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
-        }
+        if (ta.xe && feed_tokens(ta, tp, N, V1, t, tok, st)) return 1;       // SCST: the fused input launch below reads the previous draw
         float* xt = tp.xt + (long)t * N * E;
         float* x1c = tp.x1c + (long)t * NH;
         float* gates = tp.gates + (long)t * N * 4 * H;
@@ -715,47 +625,15 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
         }
         float* outd = tp.outd + (long)t * H;                                   // [N][T][H]: batched logit backward
         if (glu_dropout_launch(N, H, t2, 2 * H, out_t, H, outd, (long)T * H, seed, t, p_lm, st)) return 1;
-        float* logits = sample_logprobs + (long)t * V1;
-        if (sk.lin(outd, (long)T * H, w.logit_w, H, w.logit_b, logits, ld_lp, N, V1, H, 0)) return 1;
-        VocabStepArgs va;
-        va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
-        if (!ta.xe) {
-            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
-            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
-            va.seq_out = sample_seq; va.ld_seq = T; va.t = t;
-            if (ta.forced != nullptr) {
-                if (load_token_column_launch(ta.forced, T, t, N, tp.s_forced, st)) return 1;
-                va.select = 3; va.forced = tp.s_forced;
-            }
-        }
-        if (vocab_step_launch(va, st)) return 1;
+        if (sk.lin(outd, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 15;
     }
 
-    // ---- (4) reward and loss
+    // ---- (4) reward and loss, (5) backward through the decoder, starting with the logit layer (group 0)
     nvtxRangePop();
     CAPB_NVTX("capb200 aoa train step: reward, loss, backward, weight gradients");
-    if (ta.xe) {
-        if (xe_loss_backward_launch(sample_logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
-                                    tp.mask_sum, tp.item_loss, tp.DL, loss, st, ta.keep, ta.row_loss ? ta.row_loss : tp.row_loss, tp.row_msum, tp.row_coef)) return 1;
-    } else {
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaStreamWaitEvent(st, e->ev_join, 0));      // join: the reward needs the baseline captions
-        if (cider_reward_launch(ta.table->t, sample_seq, N, greedy_baseline ? greedy_seq : nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores, reward, T, T,
-                                st)) return 1;
-        float* rl = ta.keep > 0 ? (ta.row_loss ? ta.row_loss : tp.row_loss) : nullptr;
-        if (reward_criterion_fwd_launch(sample_logprobs, ld_lp, V1, sample_seq, reward, N, T, loss, rl, tp.mask_sum, st)) return 1;
-        if (ta.keep > 0 && scst_drop_worst_launch(sample_seq, rl, N, T, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, loss, st)) return 1;
-        // ---- (5) backward through the decoder
-        if (scst_dlogits_launch(sample_logprobs, ld_lp, sample_seq, reward, tp.mask_sum, ta.upstream, N, T, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr)) return 1;
-    }
-    if (sk.dgrad((int)TN, H, V1, tp.DL, V1, w.logit_w, H, tp.dOUTD, H, 0)) return 1;
-    if (wgrad(V1, H, (int)TN, tp.DL, V1, tp.outd, H, G.logit_w, H, 0, st)) return 1;
-    if (colsum_launch((int)TN, V1, tp.DL, V1, G.logit_b, 0, st)) return 1;
-    auto group_done = [&](int k) -> int {
-        if (record_group_event(e->grad_events[k], st)) return 1;
-        return 0;
-    };
-    if (group_done(0)) return 1;                                        // logit
+    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.outd, tp.dOUTD, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dctx, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc, 0, sizeof(float) * NH, st));
@@ -790,14 +668,14 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
     // weight gradients batched over time (K = T*N rows)
     const int TN1 = (int)((long)(T - 1) * N);
     int rc = 0;
-    rc |= wgrad(2 * H, H, (int)TN, tp.D_T2, 2 * H, tp.att, H, G.att2ctx_w, 2 * H, 0, st);
-    rc |= wgrad(2 * H, H, (int)TN, tp.D_T2, 2 * H, tp.h, H, G.att2ctx_w + H, 2 * H, 0, st);
+    rc |= sk.wgrad(2 * H, H, (int)TN, tp.D_T2, 2 * H, tp.att, H, G.att2ctx_w, 2 * H, 0);
+    rc |= sk.wgrad(2 * H, H, (int)TN, tp.D_T2, 2 * H, tp.h, H, G.att2ctx_w + H, 2 * H, 0);
     rc |= colsum_launch((int)TN, 2 * H, tp.D_T2, 2 * H, G.att2ctx_b, 0, st);
-    rc |= wgrad(H, H, (int)TN, tp.D_QP, H, tp.qln, H, G.attn_q_w, H, 0, st);
+    rc |= sk.wgrad(H, H, (int)TN, tp.D_QP, H, tp.qln, H, G.attn_q_w, H, 0);
     rc |= colsum_launch((int)TN, H, tp.D_QP, H, G.attn_q_b, 0, st);
-    rc |= wgrad(4 * H, E, (int)TN, tp.DG, 4 * H, tp.xt, E, G.att_lstm_w_ih, E + H, 0, st);
-    rc |= wgrad(4 * H, H, (int)TN, tp.DG, 4 * H, tp.x1c, H, G.att_lstm_w_ih + E, E + H, 0, st);
-    if (TN1 > 0) rc |= wgrad(4 * H, H, TN1, tp.DG + (long)N * 4 * H, 4 * H, tp.h, H, G.att_lstm_w_hh, H, 0, st);
+    rc |= sk.wgrad(4 * H, E, (int)TN, tp.DG, 4 * H, tp.xt, E, G.att_lstm_w_ih, E + H, 0);
+    rc |= sk.wgrad(4 * H, H, (int)TN, tp.DG, 4 * H, tp.x1c, H, G.att_lstm_w_ih + E, E + H, 0);
+    if (TN1 > 0) rc |= sk.wgrad(4 * H, H, TN1, tp.DG + (long)N * 4 * H, 4 * H, tp.h, H, G.att_lstm_w_hh, H, 0);
     else CAPB_CHECK_CUDA(cudaMemsetAsync(G.att_lstm_w_hh, 0, sizeof(float) * 4 * H * H, st));
     rc |= colsum_launch((int)TN, 4 * H, tp.DG, 4 * H, G.att_lstm_b_ih, 0, st);
     rc |= colsum_launch((int)TN, 4 * H, tp.DG, 4 * H, G.att_lstm_b_hh, 0, st);
@@ -805,23 +683,23 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
     rc |= per_image_sum_launch(T, N, n, 4 * H, tp.DG, tp.S, st);
     rc |= sk.dgrad(B, H, 4 * H, tp.S, 4 * H, w.att_lstm_w_ih + E, E + H, tp.d_mean, H, 0);
     if (rc) return 1;
-    if (group_done(1)) return 1;                                        // decoder + embed
+    if (record_group_event(e->grad_events[1], st)) return 1;                                        // decoder + embed
 
     // ---- (6) backward through the prologue
     rc |= sk.dgrad((int)BR, H, 2 * H, tp.d_kv, 2 * H, w.ctx2att_w, H, tp.d_att_e, H, 0);
-    rc |= wgrad(2 * H, H, (int)BR, tp.d_kv, 2 * H, tp.att_e, H, G.ctx2att_w, H, 0, st);
+    rc |= sk.wgrad(2 * H, H, (int)BR, tp.d_kv, 2 * H, tp.att_e, H, G.ctx2att_w, H, 0);
     rc |= colsum_launch((int)BR, 2 * H, tp.d_kv, 2 * H, G.ctx2att_b, 0, st);
     rc |= mean_backward_launch(B, R, H, tp.d_mean, H, tp.d_att_e, H, st, ta.mask, R);
     rc |= ln_backward_launch((int)BR, H, tp.x[NL], H, w.refiner_norm_a, tp.d_att_e, H, 1e-6f, tp.d_x, H, 0, tp.stats, G.refiner_norm_a, G.refiner_norm_b, 0, st);
     if (rc) return 1;
-    if (group_done(2)) return 1;                                        // ctx2att + refiner.norm
+    if (record_group_event(e->grad_events[2], st)) return 1;                                        // ctx2att + refiner.norm
     for (int l = NL - 1; l >= 0; --l) {
         const capb200_aoa_refiner_layer& Lw = w.refiner[l];
         const capb200_aoa_refiner_layer_grads& Lg = G.refiner[l];
         // x[l+1] = x[l] + dropout(g): d_x carries to x[l] unchanged; d g = d_x * mask
         rc |= dropout_copy_launch(tp.d_x, H, tp.d_g, H, (int)BR, H, seed, 30 + l, 0, p_sub, st);
         rc |= glu_backward_launch((int)BR, H, tp.t[l], 2 * H, tp.d_g, H, tp.d_t, 2 * H, st);
-        rc |= wgrad(2 * H, 2 * H, (int)BR, tp.d_t, 2 * H, tp.catd[l], 2 * H, Lg.aoa_w, 2 * H, 0, st);
+        rc |= sk.wgrad(2 * H, 2 * H, (int)BR, tp.d_t, 2 * H, tp.catd[l], 2 * H, Lg.aoa_w, 2 * H, 0);
         rc |= colsum_launch((int)BR, 2 * H, tp.d_t, 2 * H, Lg.aoa_b, 0, st);
         rc |= sk.dgrad((int)BR, 2 * H, 2 * H, tp.d_t, 2 * H, Lw.aoa_w, 2 * H, tp.d_catd, 2 * H, 0);
         rc |= dropout_apply_launch(tp.d_catd, (int)BR, 2 * H, 2 * H, seed, 20 + l, 0, p_aoa, st);               // [d attended | d ln (query half)]
@@ -829,35 +707,20 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
         CAPB_CHECK_CUDA(cudaMemcpy2DAsync(tp.d_g, sizeof(float) * H, tp.d_catd, sizeof(float) * 2 * H, sizeof(float) * H, BR, cudaMemcpyDeviceToDevice, st));
         rc |= enc_attn_backward_launch(B, R, heads, dk, tp.qkv[l], tp.qkv[l] + H, tp.qkv[l] + 2 * H, 3 * H, seed, 10 + l, p_at, tp.d_g, H, tp.d_qkv, tp.d_qkv + H,
                                        tp.d_qkv + 2 * H, 3 * H, st, ta.mask, R);
-        // q | k | v gradients: one GEMM / one column reduction when the caller laid the three tensors out back to back (the Python
-        // mirror's flat gradient buffer does), else three
-        if (Lg.k_w == Lg.q_w + (long)H * H && Lg.v_w == Lg.k_w + (long)H * H) {
-            rc |= wgrad(3 * H, H, (int)BR, tp.d_qkv, 3 * H, tp.ln[l], H, Lg.q_w, H, 0, st);
-        } else {
-            rc |= wgrad(H, H, (int)BR, tp.d_qkv, 3 * H, tp.ln[l], H, Lg.q_w, H, 0, st);
-            rc |= wgrad(H, H, (int)BR, tp.d_qkv + H, 3 * H, tp.ln[l], H, Lg.k_w, H, 0, st);
-            rc |= wgrad(H, H, (int)BR, tp.d_qkv + 2 * H, 3 * H, tp.ln[l], H, Lg.v_w, H, 0, st);
-        }
-        if (Lg.k_b == Lg.q_b + H && Lg.v_b == Lg.k_b + H) {
-            rc |= colsum_launch((int)BR, 3 * H, tp.d_qkv, 3 * H, Lg.q_b, 0, st);
-        } else {
-            rc |= colsum_launch((int)BR, H, tp.d_qkv, 3 * H, Lg.q_b, 0, st);
-            rc |= colsum_launch((int)BR, H, tp.d_qkv + H, 3 * H, Lg.k_b, 0, st);
-            rc |= colsum_launch((int)BR, H, tp.d_qkv + 2 * H, 3 * H, Lg.v_b, 0, st);
-        }
+        rc |= qkv_grads(sk, (int)BR, H, tp.d_qkv, tp.ln[l], Lg, nullptr, st);     // (counted in the layer's launches)
         // d ln = query half of the AoA input + through the packed q|k|v projection
         CAPB_CHECK_CUDA(cudaMemcpy2DAsync(tp.d_ln, sizeof(float) * H, tp.d_catd + H, sizeof(float) * 2 * H, sizeof(float) * H, BR, cudaMemcpyDeviceToDevice, st));
         rc |= sk.dgrad((int)BR, H, 3 * H, tp.d_qkv, 3 * H, e->r_qkv_w[l], H, tp.d_ln, H, 1);
         rc |= ln_backward_launch((int)BR, H, tp.x[l], H, Lw.ln_a, tp.d_ln, H, 1e-6f, tp.d_x, H, 1, tp.stats, Lg.ln_a, Lg.ln_b, 0, st);
         if (rc) return 1;
-        if (group_done(3 + (NL - 1 - l))) return 1;                     // refiner layer l (layers finish 5 -> 0)
+        if (record_group_event(e->grad_events[3 + (NL - 1 - l)], st)) return 1;                     // refiner layer l (layers finish 5 -> 0)
         e->launches += 22;
     }
     rc |= relu_dropout_backward_launch(BR * H, tp.x[0], tp.d_x, tp.dpre, keep_lm, st);
-    rc |= wgrad(H, F, (int)BR, tp.dpre, H, att, F, G.att_embed_w, F, 0, st);
+    rc |= sk.wgrad(H, F, (int)BR, tp.dpre, H, att, F, G.att_embed_w, F, 0);
     rc |= colsum_launch((int)BR, H, tp.dpre, H, G.att_embed_b, 0, st);
     e->launches += tf32_context_launches(e->tf32) - tf32_l0;
-    if (!rc && group_done(9)) return 1;                                 // att_embed
+    if (!rc && record_group_event(e->grad_events[9], st)) return 1;                                 // att_embed
     return rc;
 }
 
@@ -868,50 +731,16 @@ extern "C" int capb200_aoa_scst_step(capb200_aoa_engine* e, const float* att, in
                                      long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, void* stream) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
-    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
-    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
-    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
-    const int n = opts->sample_n;
-    CAPB_REQUIRE(n >= 1 && n <= 16 && (greedy_baseline || n >= 2) && B >= 1 && R >= 1, "sample_n must be in 1..16 (>= 2 for the leave-one-out baseline)");
-    const float p_lm = opts->drop_prob_lm, p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
-    CAPB_REQUIRE(p_lm >= 0.f && p_lm < 1.f && p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
+    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss};
     AoaTrainArgs ta;
-    ta.n = n; ta.T = e->T; ta.Tl = e->T; ta.p_lm = p_lm; ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.temperature = opts->temperature;
-    ta.upstream = opts->upstream; ta.ctx_drop = opts->ctx_drop; ta.seed = opts->seed; ta.greedy_baseline = greedy_baseline; ta.table = table;
-    ta.refs = refs; ta.ref_offsets = ref_offsets; ta.L = L; ta.sample_seq = sample_seq; ta.greedy_seq = greedy_seq; ta.reward = reward;
-    ta.logprobs = sample_logprobs; ta.loss = loss; ta.forced = opts->forced_tokens; ta.mask = opts->att_masks; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * n, "keep_rows must be in 0..rows");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // ---- the step as ONE CUDA graph.  Its ~1100 kernels are 5-30 us each and every launch boundary costs ~2 us on the stream, the host
-    // needs ~3 ms to enqueue them, and nothing about the sequence depends on data: captured the second time a configuration is seen,
-    // replayed afterwards with a fresh seed (dropout.cuh: seed salt).  The features are copied to an engine-owned buffer first so that the
-    // graph reads a stable address.  The gradient-group events a data-parallel caller listens to (overlapped all-reduce) become external
-    // event-record nodes of the graph (record_group_event); the event handles are part of the key.  Not used when forced tokens are replayed.
-    static const bool graph_with_listener = !(getenv("CAPB200_SCST_GRAPH_SYNC") != nullptr && atoi(getenv("CAPB200_SCST_GRAPH_SYNC")) == 0);
-    bool listening = false;
-    for (int i = 0; i < 10; ++i) listening = listening || e->grad_events[i] != nullptr;
-    if (!StepGraph::enabled() || !e->tc || (listening && !graph_with_listener) || ta.forced != nullptr || e->sg.broken) {
-        if (dropout_salt_set_all(0ull, st)) return 1;
-        return aoa_train_step(e, att, B, R, ta, grads, st);
-    }
-    cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
-    const void* srcs[2] = {att, ta.mask};
-    const size_t bytes[2] = {sizeof(float) * (size_t)B * R * e->F, ta.mask ? sizeof(float) * (size_t)B * R : 0};
-    size_t off[2];
-    if (e->sg.stage_inputs(2, srcs, bytes, off, gst)) return 1;
-    const float* att_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
-    if (ta.mask) ta.mask = reinterpret_cast<const float*>(e->sg.stage + off[1]);
-    unsigned long long key = 1469598103934665603ull;
-    capb200_aoa_scst_opts o2 = *opts; o2.seed = 0; o2.att_masks = ta.mask;
-    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
-    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
-    StepGraph::mix(key, ptrs, sizeof(ptrs));
-    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
-    const int dims[] = {B, R, L};
-    StepGraph::mix(key, dims, sizeof(dims));
-    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return aoa_train_step(e, att_s, B, R, ta, grads, gst); });
-    if (e->sg.leave(st, gst)) return 1;
-    return rc_graph;
+    if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
+    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    return run_scst_step(e, opts, grads, ta, nullptr, 0, att, sizeof(float) * (size_t)B * R * e->F, B, R, static_cast<cudaStream_t>(stream),
+                         [&](const float*, const float* att_s, const AoaTrainArgs& t, cudaStream_t s) { return aoa_train_step(e, att_s, B, R, t, grads, s); });
 }
 
 extern "C" int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* events, int n) {
@@ -924,20 +753,14 @@ extern "C" int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int 
                                    const float* masks, int label_cols, const capb200_aoa_grads* grads, float* logprobs, float* loss, void* stream) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
-    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1 && R >= 1, "seq_per_img must be in 1..16");
-    const float p_lm = opts->drop_prob_lm, p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
-    CAPB_REQUIRE(p_lm >= 0.f && p_lm < 1.f && p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
-    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
-    CAPB_REQUIRE(label_cols >= 2 && label_cols <= e->T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
-    CAPB_REQUIRE(opts->steps >= 1 && opts->steps <= label_cols - 1, "steps must be in 1..label_cols-1");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
+    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_xe_opts shared = {opts->seq_per_img, opts->steps, opts->seed, opts->drop_prob_lm, opts->label_smoothing, opts->upstream,
+                                    opts->att_masks, opts->ss_prob, opts->tokens_used, opts->keep_rows, opts->row_loss};
     AoaTrainArgs ta;
-    ta.xe = true;
-    ta.n = opts->seq_per_img; ta.T = opts->steps; ta.Tl = label_cols - 1; ta.p_lm = p_lm; ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub;
-    ta.upstream = opts->upstream; ta.ctx_drop = opts->ctx_drop; ta.seed = opts->seed; ta.smoothing = opts->label_smoothing;
-    ta.labels = labels; ta.ld_labels = label_cols; ta.masks = masks; ta.ld_masks = label_cols; ta.logprobs = logprobs; ta.loss = loss;
-    ta.mask = opts->att_masks; ta.ss_prob = opts->ss_prob; ta.tokens_used = opts->tokens_used; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.ss_prob >= 0.f && ta.ss_prob <= 1.f, "ss_prob must be in [0, 1]");
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * opts->seq_per_img, "keep_rows must be in 0..rows");
-    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;      // eager step: the seed arguments are the effective seeds
-    return aoa_train_step(e, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
+    if (xe_train_args(B, shared, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
+    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_eager_step(st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
 }

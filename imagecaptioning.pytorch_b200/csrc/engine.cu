@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "kernels.cuh"
 #include "engine_common.cuh"
+#include "train_common.cuh"
 
 namespace capb200 {
 
@@ -532,16 +533,6 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
     g.epi.bias = w.logit_b;
     g.epi.C = logits; g.epi.ldc = ld_logits;
     return run_gemm(e, G_LOGIT, g, e->capRows, st);
-}
-
-bool ensure_side(capb200_engine* e) {
-    if (e->side != nullptr && e->ev_fork != nullptr && e->ev_join != nullptr && e->ev_gfork != nullptr && e->ev_gjoin != nullptr) return true;
-    if (e->side == nullptr && create_side_stream(&e->side) != cudaSuccess) { (void)cudaGetLastError(); e->side = nullptr; return false; }
-    if (e->ev_fork == nullptr && cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess) { (void)cudaGetLastError(); e->ev_fork = nullptr; return false; }
-    if (e->ev_join == nullptr && cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) != cudaSuccess) { (void)cudaGetLastError(); e->ev_join = nullptr; return false; }
-    if (e->ev_gfork == nullptr && cudaEventCreateWithFlags(&e->ev_gfork, cudaEventDisableTiming) != cudaSuccess) { (void)cudaGetLastError(); e->ev_gfork = nullptr; return false; }
-    if (e->ev_gjoin == nullptr && cudaEventCreateWithFlags(&e->ev_gjoin, cudaEventDisableTiming) != cudaSuccess) { (void)cudaGetLastError(); e->ev_gjoin = nullptr; return false; }
-    return true;
 }
 
 int check_ready(capb200_engine* e) {
@@ -1060,48 +1051,75 @@ int capb200_log_softmax_topk(float* logits, long ld, int rows, int V1, int twice
     return vocab_step_launch(va, static_cast<cudaStream_t>(stream));
 }
 
+}  // extern "C"
+
 // =====================================================================================================================
-// SCST training step (UpDown)
+// Training steps (UpDown, Att2in2, NewFC) on the scaffold of train_common.cuh
 // =====================================================================================================================
 namespace {
 
-struct Tape {
-    int* tok; float *xt, *g1, *h0, *c0, *atth, *alpha, *attres, *g2, *h1, *c1, *out;          // forward, [T][N][.] except out [N][T][H]
-    float *fc_e, *att_e, *p_att, *g_fc, *gl, *glp;                                              // prologue + greedy scratch
-    float *DL, *dOUT, *DG1, *DG2, *DATTH, *dh0, *dc0, *dh1, *dc1, *tmpH, *dX2, *dxt, *d_att_e, *d_p_att, *S, *d_fc_e, *dpre_att, *dpre_fc, *mask_sum, *dalpha, *skinny, *item_loss;
-    size_t skinny_floats;
-    double* scores;
-    long long* gseq_dummy;
-    int *s_tokens, *s_unfinished, *s_forced;   // sampling-loop state of the train step (its own copies: the greedy baseline runs concurrently)
+// UpDown's tape: the forward [T][N][.] except out [N][T][H], the prologue, and the gradients carried through time
+struct Tape : StepTape {
+    int* tok;
+    float *xt, *g1, *h0, *c0, *atth, *alpha, *attres, *g2, *h1, *c1, *out;
+    float *fc_e, *att_e, *p_att, *g_fc;
+    float *dOUT, *DG1, *DG2, *DATTH, *dh0, *dc0, *dh1, *dc1, *tmpH, *dX2, *dxt, *d_att_e, *d_p_att, *S, *d_fc_e, *dpre_att, *dpre_fc, *dalpha;
     float* s_att_score;
-    float *row_loss, *row_msum, *row_coef;     // drop_worst: per-row loss, mask count and gradient coefficient
-    float *im_sums, *im_h, *im_c, *im_ds, *im_dh, *im_dc;   // NewFC's image step on B rows: maxout sums, state and their gradients
-    int* img_row;                              // NewFC: image of each row (r / n)
 };
 
-void layout_tape(Tape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int A, int V1, int F_att, int F_fc) {
+void layout_tape(Tape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int A, int V1) {
     const long TN = (long)T * N, BR = (long)B * R;
+    tp.layout(a, B, N, TN, V1, (long)B * T * V1);
     tp.tok = a.take<int>(TN);
     tp.xt = a.take<float>(TN * E); tp.g1 = a.take<float>(TN * 4 * H); tp.h0 = a.take<float>(TN * H); tp.c0 = a.take<float>(TN * H);
     tp.atth = a.take<float>(TN * A); tp.alpha = a.take<float>(TN * R); tp.attres = a.take<float>(TN * H);
     tp.g2 = a.take<float>(TN * 4 * H); tp.h1 = a.take<float>(TN * H); tp.c1 = a.take<float>(TN * H); tp.out = a.take<float>(TN * H);
     tp.fc_e = a.take<float>((long)B * H); tp.att_e = a.take<float>(BR * H); tp.p_att = a.take<float>(BR * A); tp.g_fc = a.take<float>((long)B * 4 * H);
-    tp.gl = a.take<float>((long)N * H); tp.glp = a.take<float>((long)B * T * V1);
-    tp.DL = a.take<float>(TN * V1); tp.dOUT = a.take<float>(TN * H); tp.DG1 = a.take<float>(TN * 4 * H); tp.DG2 = a.take<float>(TN * 4 * H);
+    tp.dOUT = a.take<float>(TN * H); tp.DG1 = a.take<float>(TN * 4 * H); tp.DG2 = a.take<float>(TN * 4 * H);
     tp.DATTH = a.take<float>(TN * A);
     tp.dh0 = a.take<float>((long)N * H); tp.dc0 = a.take<float>((long)N * H); tp.dh1 = a.take<float>((long)N * H); tp.dc1 = a.take<float>((long)N * H);
     tp.tmpH = a.take<float>((long)N * H); tp.dX2 = a.take<float>((long)N * 2 * H); tp.dxt = a.take<float>((long)N * E);
     tp.d_att_e = a.take<float>(BR * H); tp.d_p_att = a.take<float>(BR * A); tp.S = a.take<float>((long)B * 4 * H); tp.d_fc_e = a.take<float>((long)B * H);
-    tp.dpre_att = a.take<float>(BR * H); tp.dpre_fc = a.take<float>((long)B * H); tp.mask_sum = a.take<float>(8);
-    tp.scores = a.take<double>((long)N + B);
+    tp.dpre_att = a.take<float>(BR * H); tp.dpre_fc = a.take<float>((long)B * H);
     tp.dalpha = a.take<float>((long)N * R);
-    tp.item_loss = a.take<float>(TN);
-    tp.skinny_floats = (size_t)4 << 20;                       // split-K partial sums (16 MB)
-    tp.skinny = a.take<float>((long)tp.skinny_floats);
-    tp.s_tokens = a.take<int>(N); tp.s_unfinished = a.take<int>(N); tp.s_forced = a.take<int>(N);
     tp.s_att_score = a.take<float>((long)N * R);
-    tp.row_loss = a.take<float>(N); tp.row_msum = a.take<float>(N); tp.row_coef = a.take<float>(N);
-    (void)F_att; (void)F_fc;
+}
+
+// The tape of the maxout-cell families (Att2in2, NewFC).  sums / DS hold the maxout sums (i, f, o, a, b) and their gradient [T][N][5H];
+// h / c hold T+1 slots (slot 0 = the initial state, slot t+1 = step t), so step t -- and the batched weight gradients of h2h and h2att --
+// read the previous state from slot t.
+struct MaxoutTape : StepTape {
+    int* tok;
+    float *xt, *sums, *h, *c, *out, *dOUT, *DS, *dh, *dc, *dxt;
+    // Att2in2's attention on the previous h
+    float *atth, *alpha, *attres, *att_e, *p_att, *DATTH, *d_attres, *d_att_e, *d_p_att, *dpre_att, *dalpha, *s_att_score;
+    // NewFC's image step on B rows: fc_e [B, E] = fc_embed(fc), its maxout sums and state and their gradients; img_row = the image of each row
+    float *fc_e, *d_fc_e, *im_sums, *im_ds, *im_h, *im_c, *im_dh, *im_dc;
+    int* img_row;
+};
+
+void layout_maxout_tape(MaxoutTape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int A, int V1) {
+    const long TN = (long)T * N, BR = (long)B * R, NH = (long)N * H;
+    tp = MaxoutTape{};
+    tp.layout(a, B, N, TN, V1, (long)B * T * V1);
+    tp.tok = a.take<int>(TN);
+    tp.xt = a.take<float>(TN * E); tp.sums = a.take<float>(TN * 5 * H); tp.h = a.take<float>(TN * H + NH); tp.c = a.take<float>(TN * H + NH);
+    tp.out = a.take<float>(TN * H); tp.dOUT = a.take<float>(TN * H); tp.DS = a.take<float>(TN * 5 * H);
+    tp.dh = a.take<float>(NH); tp.dc = a.take<float>(NH); tp.dxt = a.take<float>((long)N * E);
+    tp.atth = a.take<float>(TN * A); tp.alpha = a.take<float>(TN * R); tp.attres = a.take<float>(TN * H);
+    tp.att_e = a.take<float>(BR * H); tp.p_att = a.take<float>(BR * A); tp.DATTH = a.take<float>(TN * A); tp.d_attres = a.take<float>(NH);
+    tp.d_att_e = a.take<float>(BR * H); tp.d_p_att = a.take<float>(BR * A); tp.dpre_att = a.take<float>(BR * H);
+    tp.dalpha = a.take<float>((long)N * R); tp.s_att_score = a.take<float>((long)N * R);
+}
+
+// NewFC: the maxout tape without the attention, plus the image step
+void layout_newfc_tape(MaxoutTape& tp, Arena& a, int B, int N, int T, int E, int H, int V1) {
+    layout_maxout_tape(tp, a, B, 0, N, T, E, H, 0, V1);
+    tp.fc_e = a.take<float>((long)B * E); tp.d_fc_e = a.take<float>((long)B * E);
+    tp.im_sums = a.take<float>((long)B * 5 * H); tp.im_ds = a.take<float>((long)B * 5 * H);
+    tp.im_h = a.take<float>((long)B * H); tp.im_c = a.take<float>((long)B * H);
+    tp.im_dh = a.take<float>((long)B * H); tp.im_dc = a.take<float>((long)B * H);
+    tp.img_row = a.take<int>(N);
 }
 
 }  // namespace
@@ -1114,150 +1132,83 @@ extern "C" int capb200_dropout_mask(float* mask, long n, unsigned long long seed
 
 namespace {
 
-// One training step on the tape: SCST (sampled tokens, reward-weighted loss) or XE (teacher-forced tokens, cross-entropy).
-struct TrainArgs {
-    bool xe = false;
-    int n = 1;                 // rows per image: train_sample_n (SCST) or seq_per_img (XE)
-    int T = 0;                 // steps evaluated (and columns of the tape)
-    int Tl = 0;                // columns of the log-prob output [N, Tl, V1]
-    float p = 0.f, temperature = 1.f, upstream = 1.f, smoothing = 0.f;
-    unsigned long long seed = 0;
-    // SCST
-    bool greedy_baseline = true;
-    const capb200_cider_table* table = nullptr;
-    const int* refs = nullptr; const int* ref_offsets = nullptr; int L = 0;
-    long long* sample_seq = nullptr; long long* greedy_seq = nullptr; float* reward = nullptr;
-    const long long* forced = nullptr;      // replay these samples instead of drawing
-    const float* mask = nullptr;            // [B, R] region mask or null
-    float ss_prob = 0.f;                    // XE: scheduled sampling probability
-    long long* tokens_used = nullptr;       // XE: optional [N, Tl] record of the words fed
-    int keep = 0;                           // drop_worst: rows kept (0 = reduction 'mean')
-    float* row_loss = nullptr;              // drop_worst: optional per-row loss output
-    // XE
-    const long long* labels = nullptr; long ld_labels = 0; const float* masks = nullptr; long ld_masks = 0;
-    float* logprobs = nullptr; float* loss = nullptr;
-};
-
-// Grows the engine's training tape to `need` bytes (synchronises only when it has to reallocate).
-int grow_tape(capb200_engine* e, size_t need, cudaStream_t st) {
-    if (need <= e->tape_bytes) return 0;
-    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-    if (e->tape) CAPB_CHECK_CUDA(cudaFree(e->tape));
-    e->tape = nullptr;
-    CAPB_CHECK_CUDA(cudaMalloc(&e->tape, need));
-    e->tape_bytes = need;
-    return 0;
-}
-
-// (1) of an SCST step with the greedy baseline: the eval-mode greedy decode (no dropout) on the regular decode path.
-int start_greedy_baseline(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, float* glp, bool* on_side,
+// (1) of an SCST step with the greedy baseline: fork it and enqueue it right away on this engine's decode path (NewFC: att = null, R = 0).
+int start_greedy_baseline(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const StepTape& tp, GreedyBaseline& gb,
                           cudaStream_t st) {
-    *on_side = false;
-    if (ta.xe || !ta.greedy_baseline) return 0;
-    // The eval-mode greedy baseline (B rows, the regular decode path with its own workspace) and the train-mode sampling forward (B*n rows,
-    // on the tape) are independent chains of small, latency-bound kernels: the baseline runs on a side stream and joins before the reward.
-    CAPB_NVTX("capb200 scst: greedy baseline (eval mode, side stream)");
-    const int T = ta.T;
-    capb200_sample_opts so; memset(&so, 0, sizeof(so)); so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.seed = 0; so.steps = T;
-    cudaStream_t gs = st;
-    static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
-    if (!serial && ensure_side(e)) {
-        CAPB_CHECK_CUDA(cudaEventRecord(e->ev_gfork, st));
-        CAPB_CHECK_CUDA(cudaStreamWaitEvent(e->side, e->ev_gfork, 0));
-        gs = e->side;
-        *on_side = true;
+    if (gb.fork(ta, &e->side, &e->ev_gfork, &e->ev_gjoin, st)) return 1;
+    return gb.enqueue(B, ta.T, e->V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, long long* seq, float* lp, void* s) {
+        return capb200_decode_sample(e, fc, att, ta.mask, B, R, so, nullptr, 0, seq, lp, nullptr, s);
+    });
+}
+
+// The attention prologue UpDown and Att2in2 share, on the tape: att_embed (ReLU, dropout site 1, padded regions zeroed) and ctx2att.
+template <class Tp>
+int att_prologue_forward(capb200_engine* e, const Skinny& sk, Tp& tp, const float* att, int B, int R, const float* mask, unsigned long long seed, float p,
+                         cudaStream_t st) {
+    const int H = e->H, A = e->A, Fa = e->cfg.att_feat_size, BR = B * R;
+    const capb200_weights& w = e->w;
+    if (sk.lin(att, Fa, w.att_embed_w, Fa, w.att_embed_b, tp.att_e, H, BR, H, Fa, 0)) return 1;
+    if (relu_copy_launch(tp.att_e, (long)BR * H, f32_view(tp.att_e, H), st)) return 1;
+    if (dropout_apply_launch(tp.att_e, BR, H, H, seed, 1, 0, p, st)) return 1;
+    if (mask != nullptr) {      // pack_wrapper: the embedding of a padded region is exactly zero (AttModel.py:44-49); relu'(0) = 0 keeps its gradient zero
+        if (mask_rows_launch(f32_view(tp.att_e, H), B, R, H, mask, R, st)) return 1;
+        e->launches++;
     }
-    CAPB_CHECK_CUDA(cudaMemsetAsync(glp, 0, sizeof(float) * (size_t)B * T * e->V1, gs));
-    CAPB_CHECK_CUDA(cudaMemsetAsync(ta.greedy_seq, 0, sizeof(long long) * (size_t)B * T, gs));
-    if (capb200_decode_sample(e, fc, att, ta.mask, B, R, &so, nullptr, 0, ta.greedy_seq, glp, nullptr, static_cast<void*>(gs))) return 1;
-    if (*on_side) CAPB_CHECK_CUDA(cudaEventRecord(e->ev_gjoin, e->side));
+    if (sk.lin(tp.att_e, H, w.ctx2att_w, H, w.ctx2att_b, tp.p_att, A, BR, A, H, 0)) return 1;
+    e->launches += 4;
     return 0;
 }
 
-// (4) + (5) of a training step: reward and loss (SCST) or the XE criterion, d logits, then the logit layer's backward batched over all (n, t):
-// dOUT [N, T, H] and the logit gradients (group 0, whose event is recorded here).  tp.out holds the dropped-out core outputs [N, T, H].
-int loss_and_logit_backward(capb200_engine* e, const TrainArgs& ta, const Skinny& sk, const Tape& tp, int B, int N, bool greedy_on_side, float* g_logit_w,
-                            float* g_logit_b, cudaStream_t st) {
-    const int T = ta.T, H = e->H, V1 = e->V1;
-    const long TN = (long)T * N;
-    const long ld_lp = (long)ta.Tl * V1;
-    const capb200_weights& w = e->w;
-    if (ta.xe) {
-        if (xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
-                                    tp.mask_sum, tp.item_loss, tp.DL, ta.loss, st, ta.keep, ta.row_loss ? ta.row_loss : tp.row_loss, tp.row_msum, tp.row_coef)) return 1;
-    } else {
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaStreamWaitEvent(st, e->ev_gjoin, 0));     // join: the reward needs the baseline captions
-        if (cider_reward_launch(ta.table->t, ta.sample_seq, N, ta.greedy_baseline ? ta.greedy_seq : nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores,
-                                ta.reward, T, T, st)) return 1;
-        float* rl = ta.keep > 0 ? (ta.row_loss ? ta.row_loss : tp.row_loss) : nullptr;
-        if (reward_criterion_fwd_launch(ta.logprobs, ld_lp, V1, ta.sample_seq, ta.reward, N, T, ta.loss, rl, tp.mask_sum, st)) return 1;
-        if (ta.keep > 0 && scst_drop_worst_launch(ta.sample_seq, rl, N, T, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, ta.loss, st)) return 1;
-        // ---- (5) backward: logit layer, batched over all (n, t)
-        if (scst_dlogits_launch(ta.logprobs, ld_lp, ta.sample_seq, ta.reward, tp.mask_sum, ta.upstream, N, T, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr)) return 1;
-    }
-    e->launches += 3;
-    if (sk.dgrad((int)TN, H, V1, tp.DL, V1, w.logit_w, H, tp.dOUT, H, 0)) return 1;          // dOUT = DL * W
-    if (sk.wgrad(V1, H, (int)TN, tp.DL, V1, tp.out, H, g_logit_w, H, 0)) return 1;            // dW = DL^T * OUT
-    if (colsum_launch((int)TN, V1, tp.DL, V1, g_logit_b, 0, st)) return 1;
-    return record_group_event(e->grad_events[0], st);                                         // group 0 (logit) is final
+// Its backward: d att_e += d p_att * ctx2att, then the ctx2att and att_embed gradients (keep_scale = 1 / (1 - p)).
+template <class Tp, class Grads>
+int att_prologue_backward(capb200_engine* e, const Skinny& sk, const Tp& tp, const float* att, int B, int R, float keep_scale, const Grads& G, cudaStream_t st) {
+    const int H = e->H, A = e->A, Fa = e->cfg.att_feat_size, BR = B * R;
+    int rc = 0;
+    rc |= sk.dgrad(BR, H, A, tp.d_p_att, A, e->w.ctx2att_w, H, tp.d_att_e, H, 1);
+    rc |= sk.wgrad(A, H, BR, tp.d_p_att, A, tp.att_e, H, G.ctx2att_w, H, 0);
+    rc |= colsum_launch(BR, A, tp.d_p_att, A, G.ctx2att_b, 0, st);
+    rc |= relu_dropout_backward_launch((long)BR * H, tp.att_e, tp.d_att_e, tp.dpre_att, keep_scale, st);
+    rc |= sk.wgrad(H, Fa, BR, tp.dpre_att, H, att, Fa, G.att_embed_w, Fa, 0);
+    rc |= colsum_launch(BR, H, tp.dpre_att, H, G.att_embed_b, 0, st);
+    e->launches += 6;
+    return rc;
 }
 
 int updown_train_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const capb200_updown_grads* grads,
                       cudaStream_t st) {
-    void* stream = static_cast<void*>(st);
     const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, A = e->A, V1 = e->V1;
-    const int Fa = e->cfg.att_feat_size, Ff = e->cfg.fc_feat_size;
+    const int Ff = e->cfg.fc_feat_size;
     const float p = ta.p;
     const float keep_scale = 1.0f / (1.0f - p);
     const unsigned long long seed = ta.seed;
     const capb200_weights& w = e->w;
-    float* const sample_logprobs = ta.logprobs;
     const long ld_lp = (long)ta.Tl * V1;
-    long long* const sample_seq = ta.sample_seq;
 
     // ---- (1) greedy baseline, eval mode (no dropout): the regular decode path
-    Arena dry; Tape t0; layout_tape(t0, dry, B, R, N, T, E, H, A, V1, Fa, Ff);
-    if (grow_tape(e, dry.off + 256, st)) return 1;
-    Arena ar; ar.base = e->tape;
-    Tape tp; layout_tape(tp, ar, B, R, N, T, E, H, A, V1, Fa, Ff);
+    Tape tp;
+    if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](Tape& t, Arena& a) { layout_tape(t, a, B, R, N, T, E, H, A, V1); })) return 1;
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;        // decode workspace sized before anything is in flight
-    bool greedy_on_side = false;
-    if (start_greedy_baseline(e, fc, att, B, R, ta, tp.glp, &greedy_on_side, st)) return 1;
-    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
-    tf32_context_new_step(e->tf32);                                          // the weights may have changed since the last step
+    GreedyBaseline gb;
+    if (start_greedy_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
+    const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
-    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};              // wgmma 3xTF32 GEMMs unless the engine is in simt_fp32 mode
-    sk.ctx = e->tf32;
 
     // ---- (2) train-mode prologue: fc_embed / att_embed with dropout, ctx2att, per-image gate term
     nvtxRangePushA("capb200 train step: forward on the tape");
     const long BR = (long)B * R;
     if (sk.lin(fc, Ff, w.fc_embed_w, Ff, w.fc_embed_b, tp.fc_e, H, B, H, Ff, 0)) return 1;
-    if (relu_copy_launch(tp.fc_e, (long)B * H, ActView{tp.fc_e, nullptr, nullptr, H}, st)) return 1;
+    if (relu_copy_launch(tp.fc_e, (long)B * H, f32_view(tp.fc_e, H), st)) return 1;
     if (dropout_apply_launch(tp.fc_e, B, H, H, seed, 0, 0, p, st)) return 1;
-    if (sk.lin(att, Fa, w.att_embed_w, Fa, w.att_embed_b, tp.att_e, H, (int)BR, H, Fa, 0)) return 1;
-    if (relu_copy_launch(tp.att_e, BR * H, ActView{tp.att_e, nullptr, nullptr, H}, st)) return 1;
-    if (dropout_apply_launch(tp.att_e, (int)BR, H, H, seed, 1, 0, p, st)) return 1;
-    if (ta.mask != nullptr) {      // pack_wrapper: the embedding of a padded region is exactly zero (AttModel.py:44-49); relu'(0) = 0 keeps its gradient zero
-        if (mask_rows_launch(ActView{tp.att_e, nullptr, nullptr, H}, B, R, H, ta.mask, R, st)) return 1;
-        e->launches++;
-    }
-    if (sk.lin(tp.att_e, H, w.ctx2att_w, H, w.ctx2att_b, tp.p_att, A, (int)BR, A, H, 0)) return 1;
+    if (att_prologue_forward(e, sk, tp, att, B, R, ta.mask, seed, p, st)) return 1;
     if (sk.lin(tp.fc_e, H, w.att_lstm_w_ih + H, E + 2 * H, e->bsum_att, tp.g_fc, 4 * H, B, 4 * H, H, 0)) return 1;
-    e->launches += 8;
+    e->launches += 4;
 
     // ---- (3) T sampling steps with the tape
     const long NH = (long)N * H;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
     for (int t = 0; t < T; ++t) {
         int* tok = tp.tok + (long)t * N;
-        if (ta.xe) {
-            if (t >= 1 && ta.ss_prob > 0.f) {      // scheduled sampling: draw from the model's own previous prediction (AttModel.py:145-154)
-                if (ss_select_launch(N, V1, sample_logprobs + (long)(t - 1) * V1, ld_lp, ta.labels, ta.ld_labels, t, seed, ta.ss_prob, tok, st)) return 1;
-            } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
-            if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
-        }
-        else CAPB_CHECK_CUDA(cudaMemcpyAsync(tok, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        if (feed_tokens(ta, tp, N, V1, t, tok, st)) return 1;
         float* xt = tp.xt + (long)t * N * E;
         float* g1 = tp.g1 + (long)t * N * 4 * H;
         float* g2 = tp.g2 + (long)t * N * 4 * H;
@@ -1280,12 +1231,12 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
             g.epi.C = g1; g.epi.ldc = 4 * H;
             if (sk.gates(g)) return 1;
         }
-        if (lstm_pointwise_launch(N, H, g1, 4 * H, nullptr, c0p, H, c0, H, ActView{h0, nullptr, nullptr, H}, nullptr, 0, nullptr, st)) return 1;
+        if (lstm_pointwise_launch(N, H, g1, 4 * H, nullptr, c0p, H, c0, H, f32_view(h0, H), nullptr, 0, nullptr, st)) return 1;
         float* atth = tp.atth + (long)t * N * A;
         if (sk.lin(h0, H, w.h2att_w, H, w.h2att_b, atth, A, N, A, H, 0)) return 1;
         float* attres = tp.attres + (long)t * NH;
         if (additive_attention_launch(B, n, R, A, H, atth, A, tp.p_att, A, tp.att_e, H, ta.mask, R, w.alpha_w, w.alpha_b, tp.s_att_score,
-                                      ActView{attres, nullptr, nullptr, H}, st, tp.alpha + (long)t * N * R)) return 1;
+                                      f32_view(attres, H), st, tp.alpha + (long)t * N * R)) return 1;
         {
             GemmProblem g; g.M = N; g.N = 4 * H; g.nseg = 2;
             g.seg[0].A = attres; g.seg[0].lda = H; g.seg[0].W = w.lang_lstm_w_ih; g.seg[0].ldw = 2 * H; g.seg[0].K = H;
@@ -1295,33 +1246,21 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
             g.epi.C = g2; g.epi.ldc = 4 * H;
             if (sk.gates(g)) return 1;
         }
-        if (lstm_pointwise_launch(N, H, g2, 4 * H, nullptr, c1p, H, c1, H, ActView{h1, nullptr, nullptr, H}, nullptr, 0, nullptr, st)) return 1;
+        if (lstm_pointwise_launch(N, H, g2, 4 * H, nullptr, c1p, H, c1, H, f32_view(h1, H), nullptr, 0, nullptr, st)) return 1;
         // core output = dropout(h_lang), stored in (n, t) order for the batched logit backward
         float* out = tp.out + (long)t * H;
         if (dropout_copy_launch(h1, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
-        float* logits = sample_logprobs + (long)t * V1;
-        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, logits, ld_lp, N, V1, H, 0)) return 1;
-        VocabStepArgs va;
-        va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
-        if (!ta.xe) {
-            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
-            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
-            va.seq_out = sample_seq; va.ld_seq = T; va.t = t;
-            if (ta.forced != nullptr) {
-                if (load_token_column_launch(ta.forced, T, t, N, tp.s_forced, st)) return 1;
-                va.select = 3; va.forced = tp.s_forced;
-            }
-        }
-        if (vocab_step_launch(va, st)) return 1;
+        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 12;
     }
 
-    // ---- (4) reward and loss
+    // ---- (4) reward and loss, (5) the logit layer's backward
     nvtxRangePop();
     CAPB_NVTX("capb200 train step: reward, loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_updown_grads& G = *grads;
-    if (loss_and_logit_backward(e, ta, sk, tp, B, N, greedy_on_side, G.logit_w, G.logit_b, st)) return 1;
+    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh1, 0, sizeof(float) * NH, st));
@@ -1378,108 +1317,59 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     rc |= sk.wgrad(A, H, (int)TN, tp.DATTH, A, tp.h0, H, G.h2att_w, H, 0);
     rc |= colsum_launch((int)TN, A, tp.DATTH, A, G.h2att_b, 0, st);
     // prologue
-    rc |= sk.dgrad((int)BR, H, A, tp.d_p_att, A, w.ctx2att_w, H, tp.d_att_e, H, 1);
-    rc |= sk.wgrad(A, H, (int)BR, tp.d_p_att, A, tp.att_e, H, G.ctx2att_w, H, 0);
-    rc |= colsum_launch((int)BR, A, tp.d_p_att, A, G.ctx2att_b, 0, st);
-    rc |= relu_dropout_backward_launch(BR * H, tp.att_e, tp.d_att_e, tp.dpre_att, keep_scale, st);
-    rc |= sk.wgrad(H, Fa, (int)BR, tp.dpre_att, H, att, Fa, G.att_embed_w, Fa, 0);
-    rc |= colsum_launch((int)BR, H, tp.dpre_att, H, G.att_embed_b, 0, st);
+    rc |= att_prologue_backward(e, sk, tp, att, B, R, keep_scale, G, st);
     rc |= relu_dropout_backward_launch((long)B * H, tp.fc_e, tp.d_fc_e, tp.dpre_fc, keep_scale, st);
     rc |= sk.wgrad(H, Ff, B, tp.dpre_fc, H, fc, Ff, G.fc_embed_w, Ff, 0);
     rc |= colsum_launch(B, H, tp.dpre_fc, H, G.fc_embed_b, 0, st);
-    e->launches += 30 + (tf32_context_launches(e->tf32) - tf32_l0);     // + transposes of the wgmma path
+    e->launches += 27 + (tf32_context_launches(e->tf32) - tf32_l0);     // (incl. the loss's 3) + transposes of the wgmma path
     if (!rc && record_group_event(e->grad_events[1], st)) return 1;
     return rc;
 }
 
 // ---- Att2in2 (Att2in2Core, AttModel.py:770-790) ---------------------------------------------------------------------------------------
-// The Tape fields the Att2in2 step uses, sized for its core: g1 / DG1 hold the maxout sums (i, f, o, a, b) and their gradient [T][N][5H];
-// h0 / c0 hold T+1 slots (slot 0 = the zero initial state, slot t+1 = step t), so step t -- and the batched weight gradients of h2h and
-// h2att -- read the previous state from slot t.
-void layout_tape_att2in2(Tape& tp, Arena& a, int B, int R, int N, int T, int E, int H, int A, int V1) {
-    const long TN = (long)T * N, BR = (long)B * R, NH = (long)N * H;
-    tp = Tape{};
-    tp.tok = a.take<int>(TN);
-    tp.xt = a.take<float>(TN * E); tp.g1 = a.take<float>(TN * 5 * H); tp.h0 = a.take<float>(TN * H + NH); tp.c0 = a.take<float>(TN * H + NH);
-    tp.atth = a.take<float>(TN * A); tp.alpha = a.take<float>(TN * R); tp.attres = a.take<float>(TN * H); tp.out = a.take<float>(TN * H);
-    tp.att_e = a.take<float>(BR * H); tp.p_att = a.take<float>(BR * A); tp.glp = a.take<float>((long)B * T * V1);
-    tp.DL = a.take<float>(TN * V1); tp.dOUT = a.take<float>(TN * H); tp.DG1 = a.take<float>(TN * 5 * H); tp.DATTH = a.take<float>(TN * A);
-    tp.dh0 = a.take<float>(NH); tp.dc0 = a.take<float>(NH); tp.tmpH = a.take<float>(NH); tp.dxt = a.take<float>((long)N * E);
-    tp.d_att_e = a.take<float>(BR * H); tp.d_p_att = a.take<float>(BR * A); tp.dpre_att = a.take<float>(BR * H); tp.mask_sum = a.take<float>(8);
-    tp.scores = a.take<double>((long)N + B);
-    tp.dalpha = a.take<float>((long)N * R);
-    tp.item_loss = a.take<float>(TN);
-    tp.skinny_floats = (size_t)4 << 20;
-    tp.skinny = a.take<float>((long)tp.skinny_floats);
-    tp.s_tokens = a.take<int>(N); tp.s_unfinished = a.take<int>(N); tp.s_forced = a.take<int>(N);
-    tp.s_att_score = a.take<float>((long)N * R);
-    tp.row_loss = a.take<float>(N); tp.row_msum = a.take<float>(N); tp.row_coef = a.take<float>(N);
-}
-
 // One Att2in2 training step: the train-mode forward on the tape (dropout sites 1 att_embed, 2 word embedding, 3 core output, as UpDown),
 // the loss, and back-propagation through time.  fc is only handed to the greedy baseline's decode call, which ignores it.
 int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const capb200_att2in2_grads* grads,
                        cudaStream_t st) {
     const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, A = e->A, V1 = e->V1, H5 = 5 * H;
-    const int Fa = e->cfg.att_feat_size;
     const float p = ta.p;
     const float keep_scale = 1.0f / (1.0f - p);
     const unsigned long long seed = ta.seed;
     const capb200_weights& w = e->w;
-    float* const sample_logprobs = ta.logprobs;
     const long ld_lp = (long)ta.Tl * V1;
 
-    Arena dry; Tape t0; layout_tape_att2in2(t0, dry, B, R, N, T, E, H, A, V1);
-    if (grow_tape(e, dry.off + 256, st)) return 1;
-    Arena ar; ar.base = e->tape;
-    Tape tp; layout_tape_att2in2(tp, ar, B, R, N, T, E, H, A, V1);
+    MaxoutTape tp;
+    if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](MaxoutTape& t, Arena& a) { layout_maxout_tape(t, a, B, R, N, T, E, H, A, V1); })) return 1;
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;
-    bool greedy_on_side = false;
-    if (start_greedy_baseline(e, fc, att, B, R, ta, tp.glp, &greedy_on_side, st)) return 1;
-    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
-    tf32_context_new_step(e->tf32);
+    GreedyBaseline gb;
+    if (start_greedy_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
+    const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
-    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};
-    sk.ctx = e->tf32;
 
     // ---- train-mode prologue: att_embed (ReLU, dropout site 1, region mask), ctx2att
     nvtxRangePushA("capb200 att2in2 train step: forward on the tape");
     const long BR = (long)B * R, NH = (long)N * H;
-    if (sk.lin(att, Fa, w.att_embed_w, Fa, w.att_embed_b, tp.att_e, H, (int)BR, H, Fa, 0)) return 1;
-    if (relu_copy_launch(tp.att_e, BR * H, ActView{tp.att_e, nullptr, nullptr, H}, st)) return 1;
-    if (dropout_apply_launch(tp.att_e, (int)BR, H, H, seed, 1, 0, p, st)) return 1;
-    if (ta.mask != nullptr) {
-        if (mask_rows_launch(ActView{tp.att_e, nullptr, nullptr, H}, B, R, H, ta.mask, R, st)) return 1;
-        e->launches++;
-    }
-    if (sk.lin(tp.att_e, H, w.ctx2att_w, H, w.ctx2att_b, tp.p_att, A, (int)BR, A, H, 0)) return 1;
-    e->launches += 4;
+    if (att_prologue_forward(e, sk, tp, att, B, R, ta.mask, seed, p, st)) return 1;
 
     // ---- T steps with the tape
-    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.h0, 0, sizeof(float) * NH, st));     // slot 0: h = c = 0
-    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.c0, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.h, 0, sizeof(float) * NH, st));     // slot 0: h = c = 0
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.c, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
     for (int t = 0; t < T; ++t) {
         int* tok = tp.tok + (long)t * N;
-        if (ta.xe) {
-            if (t >= 1 && ta.ss_prob > 0.f) {      // scheduled sampling (AttModel.py:145-154)
-                if (ss_select_launch(N, V1, sample_logprobs + (long)(t - 1) * V1, ld_lp, ta.labels, ta.ld_labels, t, seed, ta.ss_prob, tok, st)) return 1;
-            } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
-            if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
-        }
-        else CAPB_CHECK_CUDA(cudaMemcpyAsync(tok, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        if (feed_tokens(ta, tp, N, V1, t, tok, st)) return 1;
         float* xt = tp.xt + (long)t * N * E;
-        float* sums = tp.g1 + (long)t * N * H5;
-        const float* hp = tp.h0 + (long)t * NH;
-        const float* cp = tp.c0 + (long)t * NH;
-        float *h = tp.h0 + (long)(t + 1) * NH, *c = tp.c0 + (long)(t + 1) * NH;
+        float* sums = tp.sums + (long)t * N * H5;
+        const float* hp = tp.h + (long)t * NH;
+        const float* cp = tp.c + (long)t * NH;
+        float *h = tp.h + (long)(t + 1) * NH, *c = tp.c + (long)(t + 1) * NH;
         if (embed_relu_dropout_launch(N, E, tok, w.embed, xt, seed, (unsigned)t, p, st)) return 1;
         // attention on the previous hidden state
         float* atth = tp.atth + (long)t * N * A;
         if (sk.lin(hp, H, w.h2att_w, H, w.h2att_b, atth, A, N, A, H, 0)) return 1;
         float* attres = tp.attres + (long)t * NH;
         if (additive_attention_launch(B, n, R, A, H, atth, A, tp.p_att, A, tp.att_e, H, ta.mask, R, w.alpha_w, w.alpha_b, tp.s_att_score,
-                                      ActView{attres, nullptr, nullptr, H}, st, tp.alpha + (long)t * N * R)) return 1;
+                                      f32_view(attres, H), st, tp.alpha + (long)t * N * R)) return 1;
         {   // sums = xt i2h^T + h_prev h2h^T + (i2h_b + h2h_b + [0 | a2c_b]), then sums[:, 3H:] += att_res a2c^T
             GemmProblem g; g.M = N; g.N = H5; g.nseg = 2;
             g.seg[0].A = xt; g.seg[0].lda = E; g.seg[0].W = w.i2h_w; g.seg[0].ldw = E; g.seg[0].K = E;
@@ -1489,24 +1379,12 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
             if (sk.gates(g)) return 1;
         }
         if (sk.lin(attres, H, w.a2c_w, H, nullptr, sums + 3 * H, H5, N, 2 * H, H, 1)) return 1;
-        if (maxout_pointwise_launch(N, H, sums, H5, nullptr, cp, H, c, H, ActView{h, nullptr, nullptr, H}, st)) return 1;
+        if (maxout_pointwise_launch(N, H, sums, H5, nullptr, cp, H, c, H, f32_view(h, H), st)) return 1;
         // core output = dropout(h), stored in (n, t) order for the batched logit backward
         float* out = tp.out + (long)t * H;
         if (dropout_copy_launch(h, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
-        float* logits = sample_logprobs + (long)t * V1;
-        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, logits, ld_lp, N, V1, H, 0)) return 1;
-        VocabStepArgs va;
-        va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
-        if (!ta.xe) {
-            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
-            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
-            va.seq_out = ta.sample_seq; va.ld_seq = T; va.t = t;
-            if (ta.forced != nullptr) {
-                if (load_token_column_launch(ta.forced, T, t, N, tp.s_forced, st)) return 1;
-                va.select = 3; va.forced = tp.s_forced;
-            }
-        }
-        if (vocab_step_launch(va, st)) return 1;
+        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 11;
     }
 
@@ -1515,97 +1393,75 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
     CAPB_NVTX("capb200 att2in2 train step: loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_att2in2_grads& G = *grads;
-    if (loss_and_logit_backward(e, ta, sk, tp, B, N, greedy_on_side, G.logit_w, G.logit_b, st)) return 1;
-    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
-    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
+    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.d_att_e, 0, sizeof(float) * BR * H, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.d_p_att, 0, sizeof(float) * BR * A, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(G.alpha_w, 0, sizeof(float) * A, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(G.alpha_b, 0, sizeof(float), st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(G.embed, 0, sizeof(float) * (size_t)V1 * E, st));
     for (int t = T - 1; t >= 0; --t) {
-        const float* sums = tp.g1 + (long)t * N * H5;
-        float* ds = tp.DG1 + (long)t * N * H5;
+        const float* sums = tp.sums + (long)t * N * H5;
+        float* ds = tp.DS + (long)t * N * H5;
         // cell: dh = carried dh + dropout-masked dOUT[:, t]
-        if (maxout_cell_backward_launch(N, H, sums, tp.c0 + (long)t * NH, tp.c0 + (long)(t + 1) * NH, tp.dh0, tp.dOUT + (long)t * H, (long)T * H, 3,
-                                        (unsigned)t, seed, p, tp.dc0, ds, st)) return 1;
+        if (maxout_cell_backward_launch(N, H, sums, tp.c + (long)t * NH, tp.c + (long)(t + 1) * NH, tp.dh, tp.dOUT + (long)t * H, (long)T * H, 3,
+                                        (unsigned)t, seed, p, tp.dc, ds, st)) return 1;
         if (sk.dgrad(N, E, H5, ds, H5, w.i2h_w, E, tp.dxt, E, 0)) return 1;                     // d xt
-        if (sk.dgrad(N, H, H5, ds, H5, w.h2h_w, H, tp.dh0, H, 0)) return 1;                     // d h_prev through h2h (the carried dh is consumed)
-        if (sk.dgrad(N, H, 2 * H, ds + 3 * H, H5, w.a2c_w, H, tp.tmpH, H, 0)) return 1;         // d att_res: a2c only feeds the candidate pair
+        if (sk.dgrad(N, H, H5, ds, H5, w.h2h_w, H, tp.dh, H, 0)) return 1;                      // d h_prev through h2h (the carried dh is consumed)
+        if (sk.dgrad(N, H, 2 * H, ds + 3 * H, H5, w.a2c_w, H, tp.d_attres, H, 0)) return 1;     // d att_res: a2c only feeds the candidate pair
         float* datth = tp.DATTH + (long)t * N * A;
-        if (attention_backward_launch(B, n, R, A, H, tp.tmpH, tp.alpha + (long)t * N * R, tp.atth + (long)t * N * A, tp.p_att, tp.att_e, w.alpha_w, datth,
+        if (attention_backward_launch(B, n, R, A, H, tp.d_attres, tp.alpha + (long)t * N * R, tp.atth + (long)t * N * A, tp.p_att, tp.att_e, w.alpha_w, datth,
                                       tp.d_att_e, tp.d_p_att, G.alpha_w, G.alpha_b, tp.dalpha, st)) return 1;
-        if (sk.dgrad(N, H, A, datth, A, w.h2att_w, H, tp.dh0, H, 1)) return 1;                  // + d h_prev through h2att
+        if (sk.dgrad(N, H, A, datth, A, w.h2att_w, H, tp.dh, H, 1)) return 1;                   // + d h_prev through h2att
         if (embed_backward_launch(N, E, tp.tok + (long)t * N, tp.xt + (long)t * N * E, tp.dxt, E, keep_scale, G.embed, st)) return 1;
         e->launches += 8;
     }
-    // weight gradients, batched over time (K = T*N); h0 slots 0..T-1 are the previous states h2h and h2att read
+    // weight gradients, batched over time (K = T*N); h slots 0..T-1 are the previous states h2h and h2att read
     int rc = 0;
-    rc |= sk.wgrad(H5, E, (int)TN, tp.DG1, H5, tp.xt, E, G.i2h_w, E, 0);
-    rc |= sk.wgrad(H5, H, (int)TN, tp.DG1, H5, tp.h0, H, G.h2h_w, H, 0);
-    rc |= sk.wgrad(2 * H, H, (int)TN, tp.DG1 + 3 * H, H5, tp.attres, H, G.a2c_w, H, 0);
-    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.i2h_b, 0, st);
-    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.h2h_b, 0, st);
-    rc |= colsum_launch((int)TN, 2 * H, tp.DG1 + 3 * H, H5, G.a2c_b, 0, st);
-    rc |= sk.wgrad(A, H, (int)TN, tp.DATTH, A, tp.h0, H, G.h2att_w, H, 0);
+    rc |= sk.wgrad(H5, E, (int)TN, tp.DS, H5, tp.xt, E, G.i2h_w, E, 0);
+    rc |= sk.wgrad(H5, H, (int)TN, tp.DS, H5, tp.h, H, G.h2h_w, H, 0);
+    rc |= sk.wgrad(2 * H, H, (int)TN, tp.DS + 3 * H, H5, tp.attres, H, G.a2c_w, H, 0);
+    rc |= colsum_launch((int)TN, H5, tp.DS, H5, G.i2h_b, 0, st);
+    rc |= colsum_launch((int)TN, H5, tp.DS, H5, G.h2h_b, 0, st);
+    rc |= colsum_launch((int)TN, 2 * H, tp.DS + 3 * H, H5, G.a2c_b, 0, st);
+    rc |= sk.wgrad(A, H, (int)TN, tp.DATTH, A, tp.h, H, G.h2att_w, H, 0);
     rc |= colsum_launch((int)TN, A, tp.DATTH, A, G.h2att_b, 0, st);
-    // prologue
-    rc |= sk.dgrad((int)BR, H, A, tp.d_p_att, A, w.ctx2att_w, H, tp.d_att_e, H, 1);
-    rc |= sk.wgrad(A, H, (int)BR, tp.d_p_att, A, tp.att_e, H, G.ctx2att_w, H, 0);
-    rc |= colsum_launch((int)BR, A, tp.d_p_att, A, G.ctx2att_b, 0, st);
-    rc |= relu_dropout_backward_launch(BR * H, tp.att_e, tp.d_att_e, tp.dpre_att, keep_scale, st);
-    rc |= sk.wgrad(H, Fa, (int)BR, tp.dpre_att, H, att, Fa, G.att_embed_w, Fa, 0);
-    rc |= colsum_launch((int)BR, H, tp.dpre_att, H, G.att_embed_b, 0, st);
-    e->launches += 14 + (tf32_context_launches(e->tf32) - tf32_l0);
+    rc |= att_prologue_backward(e, sk, tp, att, B, R, keep_scale, G, st);
+    e->launches += 11 + (tf32_context_launches(e->tf32) - tf32_l0);     // (incl. the loss's 3)
     if (!rc && record_group_event(e->grad_events[1], st)) return 1;
     return rc;
 }
 
 // ---- NewFC (NewFCModel, AttModel.py:904-945; LSTMCore, FCModel.py:13-42) -------------------------------------------------------------
-// Att2in2's tape without the attention fields, plus the image step: fc_e [B,E] = fc_embed(fc), its maxout sums / state on B rows (image
-// features are never replicated per row) and their gradients.  h0 / c0 slot 0 holds the image step's state broadcast to each image's rows.
-void layout_tape_newfc(Tape& tp, Arena& a, int B, int N, int T, int E, int H, int V1) {
-    layout_tape_att2in2(tp, a, B, 0, N, T, E, H, 0, V1);
-    tp.fc_e = a.take<float>((long)B * E); tp.d_fc_e = a.take<float>((long)B * E);
-    tp.im_sums = a.take<float>((long)B * 5 * H); tp.im_ds = a.take<float>((long)B * 5 * H);
-    tp.im_h = a.take<float>((long)B * H); tp.im_c = a.take<float>((long)B * H);
-    tp.im_dh = a.take<float>((long)B * H); tp.im_dc = a.take<float>((long)B * H);
-    tp.img_row = a.take<int>(N);
-}
-
 // One NewFC training step.  The core starts from a zero state and first consumes fc_embed(fc) (the image step, AttModel.py:925-927: its
 // output is discarded, only (h, c) carries on), then <bos> at t = 0 and the words.  The embedding is a bare nn.Embedding and fc_embed a bare
 // nn.Linear (no ReLU, no dropout); the only dropout is site 3 on the core output.  Gradient paths of the image step: h2h(0) is h2h's bias, so
 // h2h.bias gets the image step's gradient and h2h.weight does not; i2h gets both the word steps' (input xt) and the image step's (input fc_e);
-// fc_embed is reached through the image step only.
+// fc_embed is reached through the image step only.  The image features are never replicated per row: the image step runs on B rows and
+// h / c slot 0 holds its state broadcast to each image's rows.
 int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs& ta, const capb200_newfc_grads* grads, cudaStream_t st) {
     const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, V1 = e->V1, H5 = 5 * H;
     const int Ff = e->cfg.fc_feat_size;
     const float p = ta.p;
     const unsigned long long seed = ta.seed;
     const capb200_weights& w = e->w;
-    float* const sample_logprobs = ta.logprobs;
     const long ld_lp = (long)ta.Tl * V1;
 
-    Arena dry; Tape t0; layout_tape_newfc(t0, dry, B, N, T, E, H, V1);
-    if (grow_tape(e, dry.off + 256, st)) return 1;
-    Arena ar; ar.base = e->tape;
-    Tape tp; layout_tape_newfc(tp, ar, B, N, T, E, H, V1);
+    MaxoutTape tp;
+    if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](MaxoutTape& t, Arena& a) { layout_newfc_tape(t, a, B, N, T, E, H, V1); })) return 1;
     if (ensure_workspace(e, B, N, 1, 1, st)) return 1;      // R = 1: the region count the greedy baseline's decode call sizes its workspace for
-    bool greedy_on_side = false;
-    if (start_greedy_baseline(e, fc, nullptr, B, 0, ta, tp.glp, &greedy_on_side, st)) return 1;
-    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
-    tf32_context_new_step(e->tf32);
+    GreedyBaseline gb;
+    if (start_greedy_baseline(e, fc, nullptr, B, 0, ta, tp, gb, st)) return 1;
+    const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
-    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};
-    sk.ctx = e->tf32;
 
     // ---- image step on B rows: sums = fc_e i2h^T + (i2h_b + h2h_b), the maxout cell with c_prev = 0
     nvtxRangePushA("capb200 newfc train step: forward on the tape");
     const long NH = (long)N * H;
     if (sk.lin(fc, Ff, w.fc_embed_w, Ff, w.fc_embed_b, tp.fc_e, E, B, E, Ff, 0)) return 1;
     if (sk.lin(tp.fc_e, E, w.i2h_w, E, e->bsum_core, tp.im_sums, H5, B, H5, E, 0)) return 1;
-    if (maxout_pointwise_launch(B, H, tp.im_sums, H5, nullptr, nullptr, H, tp.im_c, H, ActView{tp.im_h, nullptr, nullptr, H}, st)) return 1;
+    if (maxout_pointwise_launch(B, H, tp.im_sums, H5, nullptr, nullptr, H, tp.im_c, H, f32_view(tp.im_h, H), st)) return 1;
     iota_div_kernel<<<cdiv(N, 256), 256, 0, st>>>(tp.img_row, N, n);
     CAPB_CHECK_CUDA(cudaGetLastError());
     e->launches += 4;
@@ -1614,24 +1470,18 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
     for (int t = 0; t < T; ++t) {
         int* tok = tp.tok + (long)t * N;
-        if (ta.xe) {
-            if (t >= 1 && ta.ss_prob > 0.f) {      // scheduled sampling (AttModel.py:145-154)
-                if (ss_select_launch(N, V1, sample_logprobs + (long)(t - 1) * V1, ld_lp, ta.labels, ta.ld_labels, t, seed, ta.ss_prob, tok, st)) return 1;
-            } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
-            if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
-        }
-        else CAPB_CHECK_CUDA(cudaMemcpyAsync(tok, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        if (feed_tokens(ta, tp, N, V1, t, tok, st)) return 1;
         float* xt = tp.xt + (long)t * N * E;
-        float* sums = tp.g1 + (long)t * N * H5;
-        const float* hp = tp.h0 + (long)t * NH;
-        const float* cp = tp.c0 + (long)t * NH;
-        float *h = tp.h0 + (long)(t + 1) * NH, *c = tp.c0 + (long)(t + 1) * NH;
+        float* sums = tp.sums + (long)t * N * H5;
+        const float* hp = tp.h + (long)t * NH;
+        const float* cp = tp.c + (long)t * NH;
+        float *h = tp.h + (long)(t + 1) * NH, *c = tp.c + (long)(t + 1) * NH;
         // xt = embed[tok]; at t = 0 the same launch broadcasts the image step's (h, c) into slot 0 of each image's rows (later steps copy no
         // state: H = 0)
         StateCopy s0, s1;
-        s0.src = tp.im_h; s0.ld_src = H; s0.dst = ActView{tp.h0, nullptr, nullptr, H};
-        s1.src = tp.im_c; s1.ld_src = H; s1.dst = ActView{tp.c0, nullptr, nullptr, H};
-        if (state_gather_embed_launch(N, tok, t == 0 ? tp.img_row : nullptr, w.embed, E, E, 0, ActView{xt, nullptr, nullptr, E}, t == 0 ? H : 0,
+        s0.src = tp.im_h; s0.ld_src = H; s0.dst = f32_view(tp.h, H);
+        s1.src = tp.im_c; s1.ld_src = H; s1.dst = f32_view(tp.c, H);
+        if (state_gather_embed_launch(N, tok, t == 0 ? tp.img_row : nullptr, w.embed, E, E, 0, f32_view(xt, E), t == 0 ? H : 0,
                                       t == 0 ? 2 : 0, s0, s1, st)) return 1;
         {   // sums = xt i2h^T + h_prev h2h^T + (i2h_b + h2h_b)
             GemmProblem g; g.M = N; g.N = H5; g.nseg = 2;
@@ -1641,24 +1491,12 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
             g.epi.C = sums; g.epi.ldc = H5;
             if (sk.gates(g)) return 1;
         }
-        if (maxout_pointwise_launch(N, H, sums, H5, nullptr, cp, H, c, H, ActView{h, nullptr, nullptr, H}, st)) return 1;
+        if (maxout_pointwise_launch(N, H, sums, H5, nullptr, cp, H, c, H, f32_view(h, H), st)) return 1;
         // core output = dropout(h) (FCModel.py:40), stored in (n, t) order for the batched logit backward
         float* out = tp.out + (long)t * H;
         if (dropout_copy_launch(h, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
-        float* logits = sample_logprobs + (long)t * V1;
-        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, logits, ld_lp, N, V1, H, 0)) return 1;
-        VocabStepArgs va;
-        va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
-        if (!ta.xe) {
-            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
-            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
-            va.seq_out = ta.sample_seq; va.ld_seq = T; va.t = t;
-            if (ta.forced != nullptr) {
-                if (load_token_column_launch(ta.forced, T, t, N, tp.s_forced, st)) return 1;
-                va.select = 3; va.forced = tp.s_forced;
-            }
-        }
-        if (vocab_step_launch(va, st)) return 1;
+        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 7;
     }
 
@@ -1667,79 +1505,46 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
     CAPB_NVTX("capb200 newfc train step: loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_newfc_grads& G = *grads;
-    if (loss_and_logit_backward(e, ta, sk, tp, B, N, greedy_on_side, G.logit_w, G.logit_b, st)) return 1;
-    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
-    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
+    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(G.embed, 0, sizeof(float) * (size_t)V1 * E, st));
     for (int t = T - 1; t >= 0; --t) {
-        const float* sums = tp.g1 + (long)t * N * H5;
-        float* ds = tp.DG1 + (long)t * N * H5;
+        const float* sums = tp.sums + (long)t * N * H5;
+        float* ds = tp.DS + (long)t * N * H5;
         // cell: dh = carried dh + dropout-masked dOUT[:, t]
-        if (maxout_cell_backward_launch(N, H, sums, tp.c0 + (long)t * NH, tp.c0 + (long)(t + 1) * NH, tp.dh0, tp.dOUT + (long)t * H, (long)T * H, 3,
-                                        (unsigned)t, seed, p, tp.dc0, ds, st)) return 1;
+        if (maxout_cell_backward_launch(N, H, sums, tp.c + (long)t * NH, tp.c + (long)(t + 1) * NH, tp.dh, tp.dOUT + (long)t * H, (long)T * H, 3,
+                                        (unsigned)t, seed, p, tp.dc, ds, st)) return 1;
         if (sk.dgrad(N, E, H5, ds, H5, w.i2h_w, E, tp.dxt, E, 0)) return 1;                     // d xt
-        if (sk.dgrad(N, H, H5, ds, H5, w.h2h_w, H, tp.dh0, H, 0)) return 1;                     // d h_prev (the carried dh is consumed)
+        if (sk.dgrad(N, H, H5, ds, H5, w.h2h_w, H, tp.dh, H, 0)) return 1;                      // d h_prev (the carried dh is consumed)
         if (embed_scatter_launch(N, E, tp.tok + (long)t * N, tp.dxt, E, G.embed, st)) return 1;
         e->launches += 4;
     }
     // the image step: dh / dc carried out of step 0, summed over each image's rows, through the maxout cell (c_prev = 0) on B rows
     int rc = 0;
-    rc |= per_image_sum_launch(1, N, n, H, tp.dh0, tp.im_dh, st);
-    rc |= per_image_sum_launch(1, N, n, H, tp.dc0, tp.im_dc, st);
+    rc |= per_image_sum_launch(1, N, n, H, tp.dh, tp.im_dh, st);
+    rc |= per_image_sum_launch(1, N, n, H, tp.dc, tp.im_dc, st);
     rc |= maxout_cell_backward_launch(B, H, tp.im_sums, nullptr, tp.im_c, tp.im_dh, nullptr, 0, 0, 0, seed, p, tp.im_dc, tp.im_ds, st);
-    // weight gradients, batched over time (K = T*N; h0 slots 0..T-1 are the previous states h2h reads), plus the image step's terms (K = B)
-    rc |= sk.wgrad(H5, E, (int)TN, tp.DG1, H5, tp.xt, E, G.i2h_w, E, 0);
+    // weight gradients, batched over time (K = T*N; h slots 0..T-1 are the previous states h2h reads), plus the image step's terms (K = B)
+    rc |= sk.wgrad(H5, E, (int)TN, tp.DS, H5, tp.xt, E, G.i2h_w, E, 0);
     rc |= sk.wgrad(H5, E, B, tp.im_ds, H5, tp.fc_e, E, G.i2h_w, E, 1);
-    rc |= sk.wgrad(H5, H, (int)TN, tp.DG1, H5, tp.h0, H, G.h2h_w, H, 0);
-    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.i2h_b, 0, st);
+    rc |= sk.wgrad(H5, H, (int)TN, tp.DS, H5, tp.h, H, G.h2h_w, H, 0);
+    rc |= colsum_launch((int)TN, H5, tp.DS, H5, G.i2h_b, 0, st);
     rc |= colsum_launch(B, H5, tp.im_ds, H5, G.i2h_b, 1, st);
-    rc |= colsum_launch((int)TN, H5, tp.DG1, H5, G.h2h_b, 0, st);
+    rc |= colsum_launch((int)TN, H5, tp.DS, H5, G.h2h_b, 0, st);
     rc |= colsum_launch(B, H5, tp.im_ds, H5, G.h2h_b, 1, st);
     // fc_embed, through the image step's input
     rc |= sk.dgrad(B, E, H5, tp.im_ds, H5, w.i2h_w, E, tp.d_fc_e, E, 0);
     rc |= sk.wgrad(E, Ff, B, tp.d_fc_e, E, fc, Ff, G.fc_embed_w, Ff, 0);
     rc |= colsum_launch(B, E, tp.d_fc_e, E, G.fc_embed_b, 0, st);
-    e->launches += 13 + (tf32_context_launches(e->tf32) - tf32_l0);
+    e->launches += 16 + (tf32_context_launches(e->tf32) - tf32_l0);     // (incl. the loss's 3)
     if (!rc && record_group_event(e->grad_events[1], st)) return 1;
     return rc;
 }
 
-// Argument checks and TrainArgs of the *_scst_step / *_xe_step entry points of UpDown, Att2in2 and NewFC (the options mean the same for all three).
-int scst_train_args(int B, const capb200_scst_opts* opts, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
-                    long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, int T, TrainArgs* ta) {
-    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
-    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
-    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
-    CAPB_REQUIRE(greedy_baseline || opts->sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
-    CAPB_REQUIRE(opts->sample_n >= 1 && opts->sample_n <= 16 && B >= 1, "sample_n must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
-    ta->n = opts->sample_n; ta->T = T; ta->Tl = T; ta->p = opts->drop_prob; ta->temperature = opts->temperature; ta->upstream = opts->upstream;
-    ta->seed = opts->seed; ta->greedy_baseline = greedy_baseline; ta->table = table; ta->refs = refs; ta->ref_offsets = ref_offsets; ta->L = L;
-    ta->sample_seq = sample_seq; ta->greedy_seq = greedy_seq; ta->reward = reward; ta->logprobs = sample_logprobs; ta->loss = loss;
-    ta->forced = opts->forced_tokens; ta->mask = opts->att_masks; ta->keep = opts->keep_rows; ta->row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta->keep >= 0 && ta->keep <= B * opts->sample_n, "keep_rows must be in 0..rows");
-    return 0;
-}
-
-int xe_train_args(int B, const capb200_xe_opts* opts, const long long* labels, const float* masks, int label_cols, float* logprobs, float* loss, int T,
-                  TrainArgs* ta) {
-    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1, "seq_per_img must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob >= 0.f && opts->drop_prob < 1.f, "drop_prob must be in [0, 1)");
-    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
-    CAPB_REQUIRE(label_cols >= 2 && label_cols <= T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
-    CAPB_REQUIRE(opts->steps >= 1 && opts->steps <= label_cols - 1, "steps must be in 1..label_cols-1");
-    ta->xe = true;
-    ta->n = opts->seq_per_img; ta->T = opts->steps; ta->Tl = label_cols - 1; ta->p = opts->drop_prob; ta->upstream = opts->upstream; ta->seed = opts->seed;
-    ta->smoothing = opts->label_smoothing;
-    ta->labels = labels; ta->ld_labels = label_cols; ta->masks = masks; ta->ld_masks = label_cols; ta->logprobs = logprobs; ta->loss = loss;
-    ta->mask = opts->att_masks; ta->ss_prob = opts->ss_prob; ta->tokens_used = opts->tokens_used; ta->keep = opts->keep_rows; ta->row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta->ss_prob >= 0.f && ta->ss_prob <= 1.f, "ss_prob must be in [0, 1]");
-    CAPB_REQUIRE(ta->keep >= 0 && ta->keep <= B * opts->seq_per_img, "keep_rows must be in 0..rows");
-    return 0;
-}
-
 }  // namespace
 
+// The UpDown, Att2in2 and NewFC entry points take the shared option structs (capb200_scst_opts / capb200_xe_opts) with the same meaning.
 extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
                                         const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
                                         const capb200_updown_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
@@ -1749,33 +1554,10 @@ extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, cons
     CAPB_REQUIRE(opts && fc && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    if (scst_train_args(B, opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the whole step as one CUDA graph (see capb200_aoa_scst_step and engine_common.cuh: StepGraph)
-    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
-        if (dropout_salt_set_all(0ull, st)) return 1;      // eager step: the seed arguments are the effective seeds
-        return updown_train_step(e, fc, att, B, R, ta, grads, st);
-    }
-    cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
-    const void* srcs[3] = {fc, att, ta.mask};
-    const size_t bytes[3] = {sizeof(float) * (size_t)B * e->cfg.fc_feat_size, sizeof(float) * (size_t)B * R * e->cfg.att_feat_size,
-                             ta.mask ? sizeof(float) * (size_t)B * R : 0};
-    size_t off[3];
-    if (e->sg.stage_inputs(3, srcs, bytes, off, gst)) return 1;
-    const float* fc_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
-    const float* att_s = reinterpret_cast<const float*>(e->sg.stage + off[1]);
-    if (ta.mask) ta.mask = reinterpret_cast<const float*>(e->sg.stage + off[2]);
-    unsigned long long key = 1469598103934665603ull;
-    capb200_scst_opts o2 = *opts; o2.seed = 0; o2.att_masks = ta.mask;
-    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
-    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
-    StepGraph::mix(key, ptrs, sizeof(ptrs));
-    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
-    const int dims[] = {B, R, L};
-    StepGraph::mix(key, dims, sizeof(dims));
-    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return updown_train_step(e, fc_s, att_s, B, R, ta, grads, gst); });
-    if (e->sg.leave(st, gst)) return 1;
-    return rc_graph;
+    if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
+    return run_scst_step(e, opts, grads, ta, fc, sizeof(float) * (size_t)B * e->cfg.fc_feat_size, att, sizeof(float) * (size_t)B * R * e->cfg.att_feat_size,
+                         B, R, static_cast<cudaStream_t>(stream),
+                         [&](const float* fc_s, const float* att_s, const TrainArgs& t, cudaStream_t s) { return updown_train_step(e, fc_s, att_s, B, R, t, grads, s); });
 }
 
 extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
@@ -1787,31 +1569,10 @@ extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, con
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    if (scst_train_args(B, opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the whole step as one CUDA graph, as capb200_updown_scst_step (the fc features are not read: only att and the mask are staged)
-    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
-        if (dropout_salt_set_all(0ull, st)) return 1;
-        return att2in2_train_step(e, fc, att, B, R, ta, grads, st);
-    }
-    cudaStream_t gst = e->sg.enter(st);
-    const void* srcs[2] = {att, ta.mask};
-    const size_t bytes[2] = {sizeof(float) * (size_t)B * R * e->cfg.att_feat_size, ta.mask ? sizeof(float) * (size_t)B * R : 0};
-    size_t off[2];
-    if (e->sg.stage_inputs(2, srcs, bytes, off, gst)) return 1;
-    const float* att_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
-    if (ta.mask) ta.mask = reinterpret_cast<const float*>(e->sg.stage + off[1]);
-    unsigned long long key = 1469598103934665603ull;
-    capb200_scst_opts o2 = *opts; o2.seed = 0; o2.att_masks = ta.mask;
-    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
-    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
-    StepGraph::mix(key, ptrs, sizeof(ptrs));
-    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
-    const int dims[] = {B, R, L};
-    StepGraph::mix(key, dims, sizeof(dims));
-    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return att2in2_train_step(e, nullptr, att_s, B, R, ta, grads, gst); });
-    if (e->sg.leave(st, gst)) return 1;
-    return rc_graph;
+    if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
+    // the fc features are not read (the greedy baseline's decode call ignores them): not staged
+    return run_scst_step(e, opts, grads, ta, fc, 0, att, sizeof(float) * (size_t)B * R * e->cfg.att_feat_size, B, R, static_cast<cudaStream_t>(stream),
+                         [&](const float* fc_s, const float* att_s, const TrainArgs& t, cudaStream_t s) { return att2in2_train_step(e, fc_s, att_s, B, R, t, grads, s); });
 }
 
 extern "C" int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
@@ -1822,9 +1583,9 @@ extern "C" int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    if (xe_train_args(B, opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
-    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;
-    return att2in2_train_step(e, fc, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
+    if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_eager_step(st, [&] { return att2in2_train_step(e, fc, att, B, R, ta, grads, st); });
 }
 
 extern "C" int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
@@ -1837,30 +1598,9 @@ extern "C" int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
     CAPB_REQUIRE(opts->att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
     TrainArgs ta;
-    if (scst_train_args(B, opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the whole step as one CUDA graph, as capb200_updown_scst_step (only the fc features are staged)
-    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
-        if (dropout_salt_set_all(0ull, st)) return 1;
-        return newfc_train_step(e, fc, B, ta, grads, st);
-    }
-    cudaStream_t gst = e->sg.enter(st);
-    const void* srcs[1] = {fc};
-    const size_t bytes[1] = {sizeof(float) * (size_t)B * e->cfg.fc_feat_size};
-    size_t off[1];
-    if (e->sg.stage_inputs(1, srcs, bytes, off, gst)) return 1;
-    const float* fc_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
-    unsigned long long key = 1469598103934665603ull;
-    capb200_scst_opts o2 = *opts; o2.seed = 0;
-    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
-    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
-    StepGraph::mix(key, ptrs, sizeof(ptrs));
-    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
-    const int dims[] = {B, L};
-    StepGraph::mix(key, dims, sizeof(dims));
-    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return newfc_train_step(e, fc_s, B, ta, grads, gst); });
-    if (e->sg.leave(st, gst)) return 1;
-    return rc_graph;
+    if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
+    return run_scst_step(e, opts, grads, ta, fc, sizeof(float) * (size_t)B * e->cfg.fc_feat_size, nullptr, 0, B, R, static_cast<cudaStream_t>(stream),
+                         [&](const float* fc_s, const float*, const TrainArgs& t, cudaStream_t s) { return newfc_train_step(e, fc_s, B, t, grads, s); });
 }
 
 extern "C" int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
@@ -1872,9 +1612,9 @@ extern "C" int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const f
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
     CAPB_REQUIRE(opts->att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
     TrainArgs ta;
-    if (xe_train_args(B, opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
-    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;
-    return newfc_train_step(e, fc, B, ta, grads, static_cast<cudaStream_t>(stream));
+    if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_eager_step(st, [&] { return newfc_train_step(e, fc, B, ta, grads, st); });
 }
 
 extern "C" int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n) {
@@ -1891,10 +1631,12 @@ extern "C" int capb200_updown_xe_step(capb200_engine* e, const float* fc, const 
     CAPB_REQUIRE(opts && fc && att && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     TrainArgs ta;
-    if (xe_train_args(B, opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
-    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;      // eager step: the seed arguments are the effective seeds
-    return updown_train_step(e, fc, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
+    if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_eager_step(st, [&] { return updown_train_step(e, fc, att, B, R, ta, grads, st); });
 }
+
+extern "C" {
 
 
 capb200_cider_table* capb200_cider_table_create(const int* keys, const double* df, long n, double ref_len, void* stream) {

@@ -484,7 +484,7 @@ int sample_decode_driver(DecodeBuffers& d, int V1, int T, int rows, int method, 
 // engines) every call runs on the wgmma tf32 3-pass kernel of gemm_tf32.cu; operands that are not K-major in HBM (W for the input
 // gradients, dY / X for the weight gradients) go through cached transposes.  Without a context (simt_fp32 engines), when an operand is not
 // TMA-compatible (rows not 16-byte aligned: tiny test shapes), or with CAPB200_SKINNY_LEGACY set, the split-K kernels of gemm_generic.cu run.
-// CUDA graph of a whole fused training step (see capb200_aoa_scst_step) + the engine-owned staging buffer that gives the graph stable input
+// CUDA graph of a whole fused training step (see run_scst_step in train_common.cuh) + the engine-owned staging buffer that gives the graph stable input
 // addresses.  CAPB200_SCST_GRAPH=0 keeps the steps eager.
 struct StepGraph {
     cudaGraphExec_t exec = nullptr;

@@ -11,6 +11,7 @@
 #include "../../include/capb200.h"
 #include "common.cuh"
 #include "engine_common.cuh"
+#include "train_common.cuh"
 #include "kernels.cuh"
 
 using namespace capb200;
@@ -72,7 +73,7 @@ int gemm(capb200_tfm_engine* e, int site, GemmProblem& g, int plan_rows, cudaStr
     return run_gemm_mode(e->mode, &e->plans[site], g, plan_rows, st);
 }
 
-// y = act(x * W^T + b) (+ residual); x given as an ActView, W as fp32 pointer + planes
+// y = f32_view(x * W^T + b) (+ residual); x given as an ActView, W as fp32 pointer + planes
 int linear(capb200_tfm_engine* e, int site, const ActView& x, int M, int K, const float* w, const Planes& wp, const float* b, int N, ActView out,
            bool relu, const float* residual, long ld_res, int plan_rows, cudaStream_t st) {
     GemmProblem g;
@@ -409,7 +410,7 @@ namespace {
 
 constexpr int TML = CAPB200_TFM_MAX_LAYERS;
 
-struct TTape {
+struct TTape : StepTape {
     // encoder, rows b * R + r
     float *X[TML + 1], *eln0[TML], *eqkv[TML], *eatt[TML], *xm[TML], *eln1[TML], *ehd[TML], *mem, *skv[TML];
     // decoder, rows t * N + n
@@ -418,16 +419,12 @@ struct TTape {
     int* tok;
     float* key_mask;
     // gradients / scratch
-    float *DL, *d_yln_nm, *dY, *d_tmp, *d_h, *d_ln, *d_att, *d_qs, *d_qkv, *d_skv[TML], *d_mem, *dX, *tmp, *stats, *mask_sum, *item_loss, *glp, *skinny;
-    size_t skinny_floats;
-    double* scores;
-    int *s_tokens, *s_unfinished, *s_forced;
-    float *row_loss, *row_msum, *row_coef;
+    float *d_yln_nm, *dY, *d_tmp, *d_h, *d_ln, *d_att, *d_qs, *d_qkv, *d_skv[TML], *d_mem, *dX, *tmp, *stats;
 };
 
-void layout_ttape(TTape& tp, Arena& a, int B, int R, int N, int L, int T, int D, int Dff, int heads, int V1, int NE, int ND, bool scst) {
-    const long BR = (long)B * R, LN = (long)L * N;
-    const long big = BR > LN ? BR : LN;
+void layout_ttape(TTape& tp, Arena& a, int B, int R, int N, int T, int D, int Dff, int heads, int V1, int NE, int ND, long glp_floats) {
+    const long BR = (long)B * R, TN = (long)T * N;
+    const long big = BR > TN ? BR : TN;
     for (int l = 0; l <= NE; ++l) tp.X[l] = a.take<float>(BR * D);
     for (int l = 0; l < NE; ++l) {
         tp.eln0[l] = a.take<float>(BR * D); tp.eqkv[l] = a.take<float>(BR * 3 * D); tp.eatt[l] = a.take<float>(BR * D); tp.xm[l] = a.take<float>(BR * D);
@@ -435,133 +432,81 @@ void layout_ttape(TTape& tp, Arena& a, int B, int R, int N, int L, int T, int D,
     }
     tp.mem = a.take<float>(BR * D);
     for (int l = 0; l < ND; ++l) { tp.skv[l] = a.take<float>(BR * 2 * D); tp.d_skv[l] = a.take<float>(BR * 2 * D); }
-    for (int l = 0; l <= ND; ++l) tp.Y[l] = a.take<float>(LN * D);
+    for (int l = 0; l <= ND; ++l) tp.Y[l] = a.take<float>(TN * D);
     for (int l = 0; l < ND; ++l) {
-        tp.dln0[l] = a.take<float>(LN * D); tp.dqkv[l] = a.take<float>(LN * 3 * D); tp.datt[l] = a.take<float>(LN * D); tp.ym1[l] = a.take<float>(LN * D);
-        tp.dln1[l] = a.take<float>(LN * D); tp.dqs[l] = a.take<float>(LN * D); tp.probs[l] = a.take<float>(LN * heads * R); tp.dcatt[l] = a.take<float>(LN * D);
-        tp.ym2[l] = a.take<float>(LN * D); tp.dln2[l] = a.take<float>(LN * D); tp.dhd[l] = a.take<float>(LN * Dff);
+        tp.dln0[l] = a.take<float>(TN * D); tp.dqkv[l] = a.take<float>(TN * 3 * D); tp.datt[l] = a.take<float>(TN * D); tp.ym1[l] = a.take<float>(TN * D);
+        tp.dln1[l] = a.take<float>(TN * D); tp.dqs[l] = a.take<float>(TN * D); tp.probs[l] = a.take<float>(TN * heads * R); tp.dcatt[l] = a.take<float>(TN * D);
+        tp.ym2[l] = a.take<float>(TN * D); tp.dln2[l] = a.take<float>(TN * D); tp.dhd[l] = a.take<float>(TN * Dff);
     }
-    tp.yln_tm = a.take<float>(LN * D); tp.yln_nm = a.take<float>(LN * D);
-    tp.tok = a.take<int>(LN);
-    tp.key_mask = a.take<float>(LN);
-    tp.DL = a.take<float>(LN * V1); tp.d_yln_nm = a.take<float>(LN * D); tp.dY = a.take<float>(LN * D);
+    tp.yln_tm = a.take<float>(TN * D); tp.yln_nm = a.take<float>(TN * D);
+    tp.tok = a.take<int>(TN);
+    tp.key_mask = a.take<float>(TN);
+    tp.layout(a, B, N, TN, V1, glp_floats);
+    tp.d_yln_nm = a.take<float>(TN * D); tp.dY = a.take<float>(TN * D);
     tp.d_tmp = a.take<float>(big * D); tp.d_h = a.take<float>(big * Dff); tp.d_ln = a.take<float>(big * D); tp.d_att = a.take<float>(big * D);
-    tp.d_qs = a.take<float>(LN * D); tp.d_qkv = a.take<float>(big * 3 * D); tp.d_mem = a.take<float>(BR * D); tp.dX = a.take<float>(BR * D);
+    tp.d_qs = a.take<float>(TN * D); tp.d_qkv = a.take<float>(big * 3 * D); tp.d_mem = a.take<float>(BR * D); tp.dX = a.take<float>(BR * D);
     tp.tmp = a.take<float>(big * D);
-    tp.stats = a.take<float>(2 * big); tp.mask_sum = a.take<float>(8); tp.item_loss = a.take<float>(LN);
-    tp.glp = a.take<float>(scst ? (long)B * T * V1 : 1);
-    tp.skinny_floats = (size_t)4 << 20;
-    tp.skinny = a.take<float>((long)tp.skinny_floats);
-    tp.scores = a.take<double>((long)N + B);
-    tp.s_tokens = a.take<int>(N); tp.s_unfinished = a.take<int>(N); tp.s_forced = a.take<int>(N);
-    tp.row_loss = a.take<float>(N); tp.row_msum = a.take<float>(N); tp.row_coef = a.take<float>(N);
+    tp.stats = a.take<float>(2 * big);
 }
 
-struct TfmTrainArgs {
-    bool xe = false;
-    int n = 1, L = 0;                      // rows per image; positions evaluated (XE: label_cols - 1, SCST: seq_length)
-    float p_lm = 0.f, p = 0.f, temperature = 1.f, upstream = 1.f, smoothing = 0.f;
-    unsigned long long seed = 0;
-    bool greedy_baseline = true;
-    const capb200_cider_table* table = nullptr;
-    const int* refs = nullptr; const int* ref_offsets = nullptr; int Lref = 0;
-    long long* sample_seq = nullptr; long long* greedy_seq = nullptr; float* reward = nullptr;
-    const long long* forced = nullptr;
-    const float* mask = nullptr;
-    int keep = 0;
-    float* row_loss = nullptr;
-    const long long* labels = nullptr; long ld_labels = 0; const float* masks = nullptr; long ld_masks = 0;
-    float* logprobs = nullptr; float* loss = nullptr;
+// the shared arguments (positions evaluated: XE label_cols - 1, SCST seq_length; p = the Transformer's `dropout`) and att_embed's rate
+struct TfmTrainArgs : TrainArgs {
+    float p_lm = 0.f;
 };
 
 int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const TfmTrainArgs& ta, const capb200_tfm_grads* grads, cudaStream_t st) {
-    const int n = ta.n, N = B * n, L = ta.L, D = e->D, Dff = e->Dff, V1 = e->V1, F = e->F, heads = e->H, dk = e->dk, NE = e->NE, ND = e->ND, T = e->T;
-    const int BR = B * R, LNr = L * N;
-    const int idxL = T + 2;                            // fixed pitch of the self-attention dropout index (positions never reach it)
+    const int n = ta.n, N = B * n, T = ta.T, D = e->D, Dff = e->Dff, V1 = e->V1, F = e->F, heads = e->H, dk = e->dk, NE = e->NE, ND = e->ND;
+    const int BR = B * R, TNr = T * N;
+    const int idxL = e->T + 2;                         // fixed pitch of the self-attention dropout index (positions never reach it)
     const float p = ta.p, p_lm = ta.p_lm;
     const unsigned long long seed = ta.seed;
     const capb200_tfm_weights& w = e->w;
     const capb200_tfm_grads& G = *grads;
     const float emb_scale = sqrtf((float)D);
-    CAPB_REQUIRE(L >= 1 && L <= T + 1 && L < 32, "positions out of range");
-    {
-        Arena dry; TTape t0; layout_ttape(t0, dry, B, R, N, L, T, D, Dff, heads, V1, NE, ND, !ta.xe);
-        if (dry.off + 256 > e->tape_bytes) {
-            CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-            if (e->tape) CAPB_CHECK_CUDA(cudaFree(e->tape));
-            e->tape = nullptr;
-            CAPB_CHECK_CUDA(cudaMalloc(&e->tape, dry.off + 256));
-            e->tape_bytes = dry.off + 256;
-        }
-    }
-    Arena ar; ar.base = e->tape;
-    TTape tp; layout_ttape(tp, ar, B, R, N, L, T, D, Dff, heads, V1, NE, ND, !ta.xe);
+    CAPB_REQUIRE(T >= 1 && T <= e->T + 1 && T < 32, "positions out of range");
+    TTape tp;
+    if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](TTape& tt, Arena& a) {
+            layout_ttape(tt, a, B, R, N, T, D, Dff, heads, V1, NE, ND, ta.xe ? 1 : (long)B * e->T * V1);
+        })) return 1;
 
-    // ---- greedy baseline (eval mode): the regular K/V-cached decode on a side stream, joined before the reward
-    const bool greedy_baseline = !ta.xe && ta.greedy_baseline;
-    bool greedy_on_side = false;
-    cudaStream_t gs_enqueue = st;
-    capb200_sample_opts so;
-    if (greedy_baseline) {
-        if (ensure_workspace(e, B, B, R, 1, st)) return 1;
-        memset(&so, 0, sizeof(so)); so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.steps = T;
-        cudaStream_t gs = st;
-        static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
-        if (!serial) {
-            bool ok = true;
-            if (e->side == nullptr) ok = create_side_stream(&e->side) == cudaSuccess;
-            if (ok && e->ev_fork == nullptr) ok = cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess;
-            if (ok && e->ev_join == nullptr) ok = cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) == cudaSuccess;
-            if (ok) {
-                CAPB_CHECK_CUDA(cudaEventRecord(e->ev_fork, st));
-                CAPB_CHECK_CUDA(cudaStreamWaitEvent(e->side, e->ev_fork, 0));
-                gs = e->side;
-                greedy_on_side = true;
-            } else (void)cudaGetLastError();
-        }
-        gs_enqueue = gs;
-    }
-    if (e->tc && e->tf32 == nullptr) e->tf32 = tf32_context_create();
-    tf32_context_new_step(e->tf32);
+    // ---- greedy baseline (eval mode): the regular K/V-cached decode, forked here, enqueued after the encoder
+    if (!ta.xe && ta.greedy_baseline && ensure_workspace(e, B, B, R, 1, st)) return 1;
+    GreedyBaseline gb;
+    if (gb.fork(ta, &e->side, &e->ev_fork, &e->ev_join, st)) return 1;
+    const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
-    Skinny sk{tp.skinny, tp.skinny_floats, e->tc ? 1 : 0, st};
-    sk.ctx = e->tf32;
-    auto act = [](float* ptr, long ld) { ActView v; v.f = ptr; v.hi = nullptr; v.lo = nullptr; v.ld = ld; return v; };
     long& nl = e->launches;
     int rc = 0;
 
     // ---- encoder forward on the tape (train mode)
     rc |= sk.lin(att, F, w.att_embed_w, F, w.att_embed_b, tp.X[0], D, BR, D, F, 0);
     rc |= relu_dropout_rows_launch(BR, BR, D, 0, tp.X[0], D, seed, 1, p_lm, st);
-    if (ta.mask != nullptr) { rc |= mask_rows_launch(act(tp.X[0], D), B, R, D, ta.mask, R, st); nl++; }
+    if (ta.mask != nullptr) { rc |= mask_rows_launch(f32_view(tp.X[0], D), B, R, D, ta.mask, R, st); nl++; }
     nl += 2;
     for (int l = 0; l < NE && !rc; ++l) {
         const capb200_tfm_enc_layer& Lw = w.enc[l];
-        rc |= layer_norm_launch(BR, D, tp.X[l], D, Lw.ln0_a, Lw.ln0_b, 1e-6f, act(tp.eln0[l], D), st);
+        rc |= layer_norm_launch(BR, D, tp.X[l], D, Lw.ln0_a, Lw.ln0_b, 1e-6f, f32_view(tp.eln0[l], D), st);
         rc |= sk.lin(tp.eln0[l], D, e->enc_qkv_w[l], D, e->enc_qkv_b[l], tp.eqkv[l], 3 * D, BR, 3 * D, D, 0);
         rc |= seq_attn_train_launch(B, R, 0, R, heads, dk, 0, R, R, 1, tp.eqkv[l], tp.eqkv[l] + D, tp.eqkv[l] + 2 * D, 3 * D, seed, 10 + l, p, tp.eatt[l], D, ta.mask, R, st);
         rc |= sk.lin(tp.eatt[l], D, Lw.self_attn.o_w, D, Lw.self_attn.o_b, tp.tmp, D, BR, D, D, 0);
         rc |= add_dropout_rows_launch(BR, BR, D, 0, tp.X[l], D, tp.tmp, D, tp.xm[l], D, seed, 20 + l, p, st);
-        rc |= layer_norm_launch(BR, D, tp.xm[l], D, Lw.ln1_a, Lw.ln1_b, 1e-6f, act(tp.eln1[l], D), st);
+        rc |= layer_norm_launch(BR, D, tp.xm[l], D, Lw.ln1_a, Lw.ln1_b, 1e-6f, f32_view(tp.eln1[l], D), st);
         rc |= sk.lin(tp.eln1[l], D, Lw.w1_w, D, Lw.w1_b, tp.ehd[l], Dff, BR, Dff, D, 0);
         rc |= relu_dropout_rows_launch(BR, BR, Dff, 0, tp.ehd[l], Dff, seed, 30 + l, p, st);
         rc |= sk.lin(tp.ehd[l], Dff, Lw.w2_w, Dff, Lw.w2_b, tp.tmp, D, BR, D, Dff, 0);
         rc |= add_dropout_rows_launch(BR, BR, D, 0, tp.xm[l], D, tp.tmp, D, tp.X[l + 1], D, seed, 40 + l, p, st);
         nl += 10;
     }
-    rc |= layer_norm_launch(BR, D, tp.X[NE], D, w.enc_norm_a, w.enc_norm_b, 1e-6f, act(tp.mem, D), st);
+    rc |= layer_norm_launch(BR, D, tp.X[NE], D, w.enc_norm_a, w.enc_norm_b, 1e-6f, f32_view(tp.mem, D), st);
     for (int l = 0; l < ND; ++l) rc |= sk.lin(tp.mem, D, e->dec_skv_w[l], D, e->dec_skv_b[l], tp.skv[l], 2 * D, BR, 2 * D, D, 0);
     nl += 1 + ND;
     if (rc) return 1;
 
     // ---- the greedy baseline's launches are enqueued only now: its stream forked at the top of the step, and while the host enqueues
     // them the main stream is busy with the encoder instead of idle
-    if (greedy_baseline) {
-        CAPB_CHECK_CUDA(cudaMemsetAsync(tp.glp, 0, sizeof(float) * (size_t)B * T * V1, gs_enqueue));
-        CAPB_CHECK_CUDA(cudaMemsetAsync(ta.greedy_seq, 0, sizeof(long long) * (size_t)B * T, gs_enqueue));
-        if (capb200_tfm_decode_sample(e, att, ta.mask, B, R, &so, nullptr, 0, ta.greedy_seq, tp.glp, nullptr, static_cast<void*>(gs_enqueue))) return 1;
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaEventRecord(e->ev_join, e->side));
-    }
+    if (gb.enqueue(B, e->T, V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, long long* seq, float* lp, void* s) {
+            return capb200_tfm_decode_sample(e, att, ta.mask, B, R, so, nullptr, 0, seq, lp, nullptr, s);
+        })) return 1;
 
     // ---- decoder forward over positions [t0, t1)
     const float* key_mask = ta.xe ? tp.key_mask : nullptr;
@@ -572,97 +517,61 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
         r |= embed_pe_dropout_launch(nr, N, D, tp.tok + r0, w.lut, w.pe, emb_scale, t0, seed, 2, p, tp.Y[0] + r0 * D, D, st);
         for (int l = 0; l < ND && !r; ++l) {
             const capb200_tfm_dec_layer& Lw = w.dec[l];
-            r |= layer_norm_launch(nr, D, tp.Y[l] + r0 * D, D, Lw.ln0_a, Lw.ln0_b, 1e-6f, act(tp.dln0[l] + r0 * D, D), st);
+            r |= layer_norm_launch(nr, D, tp.Y[l] + r0 * D, D, Lw.ln0_a, Lw.ln0_b, 1e-6f, f32_view(tp.dln0[l] + r0 * D, D), st);
             r |= sk.lin(tp.dln0[l] + r0 * D, D, e->dec_qkv_w[l], D, e->dec_qkv_b[l], tp.dqkv[l] + r0 * 3 * D, 3 * D, nr, 3 * D, D, 0);
             r |= seq_attn_train_launch(N, t1, t0, t1, heads, dk, 1, idxL, 1, N, tp.dqkv[l], tp.dqkv[l] + D, tp.dqkv[l] + 2 * D, 3 * D, seed, 50 + l, p, tp.datt[l], D,
-                                       key_mask, L, st);
+                                       key_mask, T, st);
             r |= sk.lin(tp.datt[l] + r0 * D, D, Lw.self_attn.o_w, D, Lw.self_attn.o_b, tp.tmp, D, nr, D, D, 0);
             r |= add_dropout_rows_launch(nr, N, D, t0, tp.Y[l] + r0 * D, D, tp.tmp, D, tp.ym1[l] + r0 * D, D, seed, 60 + l, p, st);
-            r |= layer_norm_launch(nr, D, tp.ym1[l] + r0 * D, D, Lw.ln1_a, Lw.ln1_b, 1e-6f, act(tp.dln1[l] + r0 * D, D), st);
+            r |= layer_norm_launch(nr, D, tp.ym1[l] + r0 * D, D, Lw.ln1_a, Lw.ln1_b, 1e-6f, f32_view(tp.dln1[l] + r0 * D, D), st);
             r |= sk.lin(tp.dln1[l] + r0 * D, D, Lw.src_attn.q_w, D, Lw.src_attn.q_b, tp.dqs[l] + r0 * D, D, nr, D, D, 0);
             r |= cross_attn_train_launch(nr, n, heads, dk, R, tp.dqs[l] + r0 * D, D, tp.skv[l], tp.skv[l] + D, 2 * D, seed, 70 + l, t0, p, tp.dcatt[l] + r0 * D, D,
                                          tp.probs[l] + r0 * heads * R, st, ta.mask, R, N);
             r |= sk.lin(tp.dcatt[l] + r0 * D, D, Lw.src_attn.o_w, D, Lw.src_attn.o_b, tp.tmp, D, nr, D, D, 0);
             r |= add_dropout_rows_launch(nr, N, D, t0, tp.ym1[l] + r0 * D, D, tp.tmp, D, tp.ym2[l] + r0 * D, D, seed, 80 + l, p, st);
-            r |= layer_norm_launch(nr, D, tp.ym2[l] + r0 * D, D, Lw.ln2_a, Lw.ln2_b, 1e-6f, act(tp.dln2[l] + r0 * D, D), st);
+            r |= layer_norm_launch(nr, D, tp.ym2[l] + r0 * D, D, Lw.ln2_a, Lw.ln2_b, 1e-6f, f32_view(tp.dln2[l] + r0 * D, D), st);
             r |= sk.lin(tp.dln2[l] + r0 * D, D, Lw.w1_w, D, Lw.w1_b, tp.dhd[l] + r0 * Dff, Dff, nr, Dff, D, 0);
             r |= relu_dropout_rows_launch(nr, N, Dff, t0, tp.dhd[l] + r0 * Dff, Dff, seed, 90 + l, p, st);
             r |= sk.lin(tp.dhd[l] + r0 * Dff, Dff, Lw.w2_w, Dff, Lw.w2_b, tp.tmp, D, nr, D, Dff, 0);
             r |= add_dropout_rows_launch(nr, N, D, t0, tp.ym2[l] + r0 * D, D, tp.tmp, D, tp.Y[l + 1] + r0 * D, D, seed, 100 + l, p, st);
             nl += 16;
         }
-        r |= layer_norm_launch(nr, D, tp.Y[ND] + r0 * D, D, w.dec_norm_a, w.dec_norm_b, 1e-6f, act(tp.yln_tm + r0 * D, D), st);
+        r |= layer_norm_launch(nr, D, tp.Y[ND] + r0 * D, D, w.dec_norm_a, w.dec_norm_b, 1e-6f, f32_view(tp.yln_tm + r0 * D, D), st);
         nl += 2;
         return r;
     };
 
-    const long ld_lp = (long)L * V1;                   // log-prob row pitch of one sequence: [N, L, V1]
+    const long ld_lp = (long)T * V1;                   // log-prob row pitch of one sequence: [N, T, V1]
     if (ta.xe) {
-        if (load_tokens_tm_launch(ta.labels, ta.ld_labels, N, L, tp.tok, tp.key_mask, L, st)) return 1;
-        if (dec_forward(0, L)) return 1;
-        rc |= permute_rows_launch(L, N, D, tp.yln_tm, D, tp.yln_nm, D, 1, st);
-        rc |= sk.lin(tp.yln_nm, D, w.gen_w, D, w.gen_b, ta.logprobs, V1, LNr, V1, D, 0);
-        VocabStepArgs va; va.rows = LNr; va.V1 = V1; va.logits = ta.logprobs; va.ld = V1;
+        if (load_tokens_tm_launch(ta.labels, ta.ld_labels, N, T, tp.tok, tp.key_mask, T, st)) return 1;
+        if (dec_forward(0, T)) return 1;
+        rc |= permute_rows_launch(T, N, D, tp.yln_tm, D, tp.yln_nm, D, 1, st);
+        rc |= sk.lin(tp.yln_nm, D, w.gen_w, D, w.gen_b, ta.logprobs, V1, TNr, V1, D, 0);
+        VocabStepArgs va; va.rows = TNr; va.V1 = V1; va.logits = ta.logprobs; va.ld = V1;
         rc |= vocab_step_launch(va, st);
         nl += 4;
         if (rc) return 1;
-        if (xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, L, L, V1, ta.smoothing, ta.upstream, tp.mask_sum,
-                                    tp.item_loss, tp.DL, ta.loss, st, ta.keep, ta.row_loss ? ta.row_loss : tp.row_loss, tp.row_msum, tp.row_coef)) return 1;
     } else {
         CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
-        for (int t = 0; t < L; ++t) {
-            CAPB_CHECK_CUDA(cudaMemcpyAsync(tp.tok + (long)t * N, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        for (int t = 0; t < T; ++t) {
+            if (feed_tokens(ta, tp, N, V1, t, tp.tok + (long)t * N, st)) return 1;
             if (dec_forward(t, t + 1)) return 1;
-            float* logits = ta.logprobs + (long)t * V1;
-            if (sk.lin(tp.yln_tm + (long)t * N * D, D, w.gen_w, D, w.gen_b, logits, ld_lp, N, V1, D, 0)) return 1;
-            VocabStepArgs va;
-            va.rows = N; va.V1 = V1; va.logits = logits; va.ld = ld_lp;
-            va.select = 2; va.temperature = ta.temperature; va.seed = seed; va.step = (unsigned long long)t;
-            va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
-            va.seq_out = ta.sample_seq; va.ld_seq = L; va.t = t;
-            if (ta.forced != nullptr) {
-                if (load_token_column_launch(ta.forced, L, t, N, tp.s_forced, st)) return 1;
-                va.select = 3; va.forced = tp.s_forced;
-            }
-            if (vocab_step_launch(va, st)) return 1;
+            if (sk.lin(tp.yln_tm + (long)t * N * D, D, w.gen_w, D, w.gen_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, D, 0)) return 1;
+            if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
             nl += 3;
         }
-        if (permute_rows_launch(L, N, D, tp.yln_tm, D, tp.yln_nm, D, 1, st)) return 1;
-        if (greedy_on_side) CAPB_CHECK_CUDA(cudaStreamWaitEvent(st, e->ev_join, 0));
-        if (cider_reward_launch(ta.table->t, ta.sample_seq, N, greedy_baseline ? ta.greedy_seq : nullptr, B, L, ta.refs, ta.ref_offsets, ta.Lref, tp.scores, ta.reward,
-                                L, L, st)) return 1;
-        float* rl = ta.keep > 0 ? (ta.row_loss ? ta.row_loss : tp.row_loss) : nullptr;
-        if (reward_criterion_fwd_launch(ta.logprobs, ld_lp, V1, ta.sample_seq, ta.reward, N, L, ta.loss, rl, tp.mask_sum, st)) return 1;
-        if (ta.keep > 0 && scst_drop_worst_launch(ta.sample_seq, rl, N, L, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, ta.loss, st)) return 1;
-        if (scst_dlogits_launch(ta.logprobs, ld_lp, ta.sample_seq, ta.reward, tp.mask_sum, ta.upstream, N, L, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr)) return 1;
+        if (permute_rows_launch(T, N, D, tp.yln_tm, D, tp.yln_nm, D, 1, st)) return 1;
         nl += 5;
     }
+    if (loss_backward(ta, tp, gb, B, N, V1, st)) return 1;
 
     // ---- backward: generator and the final LayerNorm
     auto colsum = [&](int rows, int cols, const float* x, long ld, float* out) { nl++; return colsum_launch(rows, cols, x, ld, out, 0, st); };
-    // q | k | v gradients of a self-attention block: one GEMM / one column reduction when the caller laid the three tensors out back to back
-    // (the Python mirror's flat gradient buffer does), else three
-    auto qkv_grads = [&](int rows, const float* x, const capb200_mha_grads& ag) -> int {
-        int r = 0;
-        if (ag.k_w == ag.q_w + (long)D * D && ag.v_w == ag.k_w + (long)D * D) r |= sk.wgrad(3 * D, D, rows, tp.d_qkv, 3 * D, x, D, ag.q_w, D, 0);
-        else {
-            r |= sk.wgrad(D, D, rows, tp.d_qkv, 3 * D, x, D, ag.q_w, D, 0);
-            r |= sk.wgrad(D, D, rows, tp.d_qkv + D, 3 * D, x, D, ag.k_w, D, 0);
-            r |= sk.wgrad(D, D, rows, tp.d_qkv + 2 * D, 3 * D, x, D, ag.v_w, D, 0);
-        }
-        if (ag.k_b == ag.q_b + D && ag.v_b == ag.k_b + D) r |= colsum(rows, 3 * D, tp.d_qkv, 3 * D, ag.q_b);
-        else {
-            r |= colsum(rows, D, tp.d_qkv, 3 * D, ag.q_b);
-            r |= colsum(rows, D, tp.d_qkv + D, 3 * D, ag.k_b);
-            r |= colsum(rows, D, tp.d_qkv + 2 * D, 3 * D, ag.v_b);
-        }
-        return r;
-    };
-    rc |= sk.dgrad(LNr, D, V1, tp.DL, V1, w.gen_w, D, tp.d_yln_nm, D, 0);
-    rc |= sk.wgrad(V1, D, LNr, tp.DL, V1, tp.yln_nm, D, G.gen_w, D, 0);
-    rc |= colsum(LNr, V1, tp.DL, V1, G.gen_b);
-    rc |= permute_rows_launch(L, N, D, tp.d_yln_nm, D, tp.d_tmp, D, 0, st);
-    rc |= ln_backward_launch(LNr, D, tp.Y[ND], D, w.dec_norm_a, tp.d_tmp, D, 1e-6f, tp.dY, D, 0, tp.stats, G.dec_norm_a, G.dec_norm_b, 0, st);
+    rc |= sk.dgrad(TNr, D, V1, tp.DL, V1, w.gen_w, D, tp.d_yln_nm, D, 0);
+    rc |= sk.wgrad(V1, D, TNr, tp.DL, V1, tp.yln_nm, D, G.gen_w, D, 0);
+    rc |= colsum(TNr, V1, tp.DL, V1, G.gen_b);
+    rc |= permute_rows_launch(T, N, D, tp.d_yln_nm, D, tp.d_tmp, D, 0, st);
+    rc |= ln_backward_launch(TNr, D, tp.Y[ND], D, w.dec_norm_a, tp.d_tmp, D, 1e-6f, tp.dY, D, 0, tp.stats, G.dec_norm_a, G.dec_norm_b, 0, st);
     nl += 3;
     for (int l = 0; l < ND; ++l) CAPB_CHECK_CUDA(cudaMemsetAsync(tp.d_skv[l], 0, sizeof(float) * (size_t)BR * 2 * D, st));
     if (rc) return 1;
@@ -670,41 +579,41 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
         const capb200_tfm_dec_layer& Lw = w.dec[l];
         const capb200_tfm_dec_layer_grads& Lg = G.dec[l];
         // feed-forward sublayer: Y[l+1] = ym2 + dropout(w2(dropout(relu(w1(ln2(ym2))))))
-        rc |= dropout_rows_copy_launch(LNr, N, D, 0, tp.dY, D, tp.d_tmp, D, seed, 100 + l, p, nullptr, 0, st);
-        rc |= sk.wgrad(D, Dff, LNr, tp.d_tmp, D, tp.dhd[l], Dff, Lg.w2_w, Dff, 0);
-        rc |= colsum(LNr, D, tp.d_tmp, D, Lg.w2_b);
-        rc |= sk.dgrad(LNr, Dff, D, tp.d_tmp, D, Lw.w2_w, Dff, tp.d_h, Dff, 0);
-        rc |= dropout_rows_copy_launch(LNr, N, Dff, 0, tp.d_h, Dff, tp.d_h, Dff, seed, 90 + l, p, tp.dhd[l], Dff, st);
-        rc |= sk.wgrad(Dff, D, LNr, tp.d_h, Dff, tp.dln2[l], D, Lg.w1_w, D, 0);
-        rc |= colsum(LNr, Dff, tp.d_h, Dff, Lg.w1_b);
-        rc |= sk.dgrad(LNr, D, Dff, tp.d_h, Dff, Lw.w1_w, D, tp.d_ln, D, 0);
-        rc |= ln_backward_launch(LNr, D, tp.ym2[l], D, Lw.ln2_a, tp.d_ln, D, 1e-6f, tp.dY, D, 1, tp.stats, Lg.ln2_a, Lg.ln2_b, 0, st);
+        rc |= dropout_rows_copy_launch(TNr, N, D, 0, tp.dY, D, tp.d_tmp, D, seed, 100 + l, p, nullptr, 0, st);
+        rc |= sk.wgrad(D, Dff, TNr, tp.d_tmp, D, tp.dhd[l], Dff, Lg.w2_w, Dff, 0);
+        rc |= colsum(TNr, D, tp.d_tmp, D, Lg.w2_b);
+        rc |= sk.dgrad(TNr, Dff, D, tp.d_tmp, D, Lw.w2_w, Dff, tp.d_h, Dff, 0);
+        rc |= dropout_rows_copy_launch(TNr, N, Dff, 0, tp.d_h, Dff, tp.d_h, Dff, seed, 90 + l, p, tp.dhd[l], Dff, st);
+        rc |= sk.wgrad(Dff, D, TNr, tp.d_h, Dff, tp.dln2[l], D, Lg.w1_w, D, 0);
+        rc |= colsum(TNr, Dff, tp.d_h, Dff, Lg.w1_b);
+        rc |= sk.dgrad(TNr, D, Dff, tp.d_h, Dff, Lw.w1_w, D, tp.d_ln, D, 0);
+        rc |= ln_backward_launch(TNr, D, tp.ym2[l], D, Lw.ln2_a, tp.d_ln, D, 1e-6f, tp.dY, D, 1, tp.stats, Lg.ln2_a, Lg.ln2_b, 0, st);
         // source attention sublayer: ym2 = ym1 + dropout(o(attention(q(ln1(ym1)), memory)))
-        rc |= dropout_rows_copy_launch(LNr, N, D, 0, tp.dY, D, tp.d_tmp, D, seed, 80 + l, p, nullptr, 0, st);
-        rc |= sk.wgrad(D, D, LNr, tp.d_tmp, D, tp.dcatt[l], D, Lg.src_attn.o_w, D, 0);
-        rc |= colsum(LNr, D, tp.d_tmp, D, Lg.src_attn.o_b);
-        rc |= sk.dgrad(LNr, D, D, tp.d_tmp, D, Lw.src_attn.o_w, D, tp.d_att, D, 0);
+        rc |= dropout_rows_copy_launch(TNr, N, D, 0, tp.dY, D, tp.d_tmp, D, seed, 80 + l, p, nullptr, 0, st);
+        rc |= sk.wgrad(D, D, TNr, tp.d_tmp, D, tp.dcatt[l], D, Lg.src_attn.o_w, D, 0);
+        rc |= colsum(TNr, D, tp.d_tmp, D, Lg.src_attn.o_b);
+        rc |= sk.dgrad(TNr, D, D, tp.d_tmp, D, Lw.src_attn.o_w, D, tp.d_att, D, 0);
         rc |= cross_attn_backward_launch(B, n, heads, dk, R, tp.dqs[l], D, tp.skv[l], tp.skv[l] + D, 2 * D, seed, 70 + l, 0, p, tp.probs[l], tp.d_att, D, tp.d_qs, D,
-                                         tp.d_skv[l], tp.d_skv[l] + D, 2 * D, st, L, N);
-        rc |= sk.wgrad(D, D, LNr, tp.d_qs, D, tp.dln1[l], D, Lg.src_attn.q_w, D, 0);
-        rc |= colsum(LNr, D, tp.d_qs, D, Lg.src_attn.q_b);
-        rc |= sk.dgrad(LNr, D, D, tp.d_qs, D, Lw.src_attn.q_w, D, tp.d_ln, D, 0);
-        rc |= ln_backward_launch(LNr, D, tp.ym1[l], D, Lw.ln1_a, tp.d_ln, D, 1e-6f, tp.dY, D, 1, tp.stats, Lg.ln1_a, Lg.ln1_b, 0, st);
+                                         tp.d_skv[l], tp.d_skv[l] + D, 2 * D, st, T, N);
+        rc |= sk.wgrad(D, D, TNr, tp.d_qs, D, tp.dln1[l], D, Lg.src_attn.q_w, D, 0);
+        rc |= colsum(TNr, D, tp.d_qs, D, Lg.src_attn.q_b);
+        rc |= sk.dgrad(TNr, D, D, tp.d_qs, D, Lw.src_attn.q_w, D, tp.d_ln, D, 0);
+        rc |= ln_backward_launch(TNr, D, tp.ym1[l], D, Lw.ln1_a, tp.d_ln, D, 1e-6f, tp.dY, D, 1, tp.stats, Lg.ln1_a, Lg.ln1_b, 0, st);
         // self-attention sublayer: ym1 = Y[l] + dropout(o(causal attention(q|k|v(ln0(Y[l])))))
-        rc |= dropout_rows_copy_launch(LNr, N, D, 0, tp.dY, D, tp.d_tmp, D, seed, 60 + l, p, nullptr, 0, st);
-        rc |= sk.wgrad(D, D, LNr, tp.d_tmp, D, tp.datt[l], D, Lg.self_attn.o_w, D, 0);
-        rc |= colsum(LNr, D, tp.d_tmp, D, Lg.self_attn.o_b);
-        rc |= sk.dgrad(LNr, D, D, tp.d_tmp, D, Lw.self_attn.o_w, D, tp.d_att, D, 0);
-        rc |= seq_attn_backward_launch(N, L, heads, dk, 1, idxL, 1, N, tp.dqkv[l], tp.dqkv[l] + D, tp.dqkv[l] + 2 * D, 3 * D, seed, 50 + l, p, tp.d_att, D, tp.d_qkv,
-                                       tp.d_qkv + D, tp.d_qkv + 2 * D, 3 * D, key_mask, L, st);
-        rc |= qkv_grads(LNr, tp.dln0[l], Lg.self_attn);
-        rc |= sk.dgrad(LNr, D, 3 * D, tp.d_qkv, 3 * D, e->dec_qkv_w[l], D, tp.d_ln, D, 0);
-        rc |= ln_backward_launch(LNr, D, tp.Y[l], D, Lw.ln0_a, tp.d_ln, D, 1e-6f, tp.dY, D, 1, tp.stats, Lg.ln0_a, Lg.ln0_b, 0, st);
+        rc |= dropout_rows_copy_launch(TNr, N, D, 0, tp.dY, D, tp.d_tmp, D, seed, 60 + l, p, nullptr, 0, st);
+        rc |= sk.wgrad(D, D, TNr, tp.d_tmp, D, tp.datt[l], D, Lg.self_attn.o_w, D, 0);
+        rc |= colsum(TNr, D, tp.d_tmp, D, Lg.self_attn.o_b);
+        rc |= sk.dgrad(TNr, D, D, tp.d_tmp, D, Lw.self_attn.o_w, D, tp.d_att, D, 0);
+        rc |= seq_attn_backward_launch(N, T, heads, dk, 1, idxL, 1, N, tp.dqkv[l], tp.dqkv[l] + D, tp.dqkv[l] + 2 * D, 3 * D, seed, 50 + l, p, tp.d_att, D, tp.d_qkv,
+                                       tp.d_qkv + D, tp.d_qkv + 2 * D, 3 * D, key_mask, T, st);
+        rc |= qkv_grads(sk, TNr, D, tp.d_qkv, tp.dln0[l], Lg.self_attn, &nl, st);
+        rc |= sk.dgrad(TNr, D, 3 * D, tp.d_qkv, 3 * D, e->dec_qkv_w[l], D, tp.d_ln, D, 0);
+        rc |= ln_backward_launch(TNr, D, tp.Y[l], D, Lw.ln0_a, tp.d_ln, D, 1e-6f, tp.dY, D, 1, tp.stats, Lg.ln0_a, Lg.ln0_b, 0, st);
         nl += 14;
     }
     if (rc) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(G.lut, 0, sizeof(float) * (size_t)V1 * D, st));
-    rc |= embed_pe_backward_launch(LNr, N, D, tp.tok, emb_scale, 0, seed, 2, p, tp.dY, D, G.lut, st);
+    rc |= embed_pe_backward_launch(TNr, N, D, tp.tok, emb_scale, 0, seed, 2, p, tp.dY, D, G.lut, st);
     // memory: K | V projections of every decoder layer
     for (int l = 0; l < ND; ++l) {
         const capb200_tfm_dec_layer_grads& Lg = G.dec[l];
@@ -741,7 +650,7 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
         rc |= sk.dgrad(BR, D, D, tp.d_tmp, D, Lw.self_attn.o_w, D, tp.d_att, D, 0);
         rc |= seq_attn_backward_launch(B, R, heads, dk, 0, R, R, 1, tp.eqkv[l], tp.eqkv[l] + D, tp.eqkv[l] + 2 * D, 3 * D, seed, 10 + l, p, tp.d_att, D, tp.d_qkv,
                                        tp.d_qkv + D, tp.d_qkv + 2 * D, 3 * D, ta.mask, R, st);
-        rc |= qkv_grads(BR, tp.eln0[l], Lg.self_attn);
+        rc |= qkv_grads(sk, BR, D, tp.d_qkv, tp.eln0[l], Lg.self_attn, &nl, st);
         rc |= sk.dgrad(BR, D, 3 * D, tp.d_qkv, 3 * D, e->enc_qkv_w[l], D, tp.d_ln, D, 0);
         rc |= ln_backward_launch(BR, D, tp.X[l], D, Lw.ln0_a, tp.d_ln, D, 1e-6f, tp.dX, D, 1, tp.stats, Lg.ln0_a, Lg.ln0_b, 0, st);
         nl += 8;
@@ -766,17 +675,16 @@ extern "C" int capb200_tfm_xe_step(capb200_tfm_engine* e, const float* att, int 
                                    const float* masks, int label_cols, const capb200_tfm_grads* grads, float* logprobs, float* loss, void* stream) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
-    CAPB_REQUIRE(opts->seq_per_img >= 1 && opts->seq_per_img <= 16 && B >= 1 && R >= 1, "seq_per_img must be in 1..16");
-    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f && opts->dropout >= 0.f && opts->dropout < 1.f, "dropout rates must be in [0, 1)");
-    CAPB_REQUIRE(opts->label_smoothing >= 0.f && opts->label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
-    CAPB_REQUIRE(label_cols >= 2 && label_cols <= e->T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
+    // every position is evaluated (one pass over label_cols - 1 positions), no scheduled sampling
+    const capb200_xe_opts shared = {opts->seq_per_img, label_cols - 1, opts->seed, opts->dropout, opts->label_smoothing, opts->upstream,
+                                    opts->att_masks, 0.f, nullptr, opts->keep_rows, opts->row_loss};
     TfmTrainArgs ta;
-    ta.xe = true; ta.n = opts->seq_per_img; ta.L = label_cols - 1; ta.p_lm = opts->drop_prob_lm; ta.p = opts->dropout; ta.upstream = opts->upstream;
-    ta.seed = opts->seed; ta.smoothing = opts->label_smoothing; ta.labels = labels; ta.ld_labels = label_cols; ta.masks = masks; ta.ld_masks = label_cols;
-    ta.logprobs = logprobs; ta.loss = loss; ta.mask = opts->att_masks; ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * ta.n, "keep_rows must be in 0..rows");
-    if (dropout_salt_set_all(0ull, static_cast<cudaStream_t>(stream))) return 1;      // eager step: the seed arguments are the effective seeds
-    return tfm_train_step(e, att, B, R, ta, grads, static_cast<cudaStream_t>(stream));
+    if (xe_train_args(B, shared, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
+    ta.p_lm = opts->drop_prob_lm;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_eager_step(st, [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
 }
 
 extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_scst_opts* opts, const capb200_cider_table* table,
@@ -784,41 +692,13 @@ extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, in
                                      float* sample_logprobs, float* reward, float* loss, void* stream) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
-    const bool greedy_baseline = opts->baseline == CAPB200_BASELINE_GREEDY;
-    CAPB_REQUIRE(greedy_baseline || opts->baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
-    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
-    const int n = opts->sample_n;
-    CAPB_REQUIRE(n >= 1 && n <= 16 && (greedy_baseline || n >= 2) && B >= 1 && R >= 1, "sample_n must be in 1..16 (>= 2 for the leave-one-out baseline)");
-    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f && opts->dropout >= 0.f && opts->dropout < 1.f, "dropout rates must be in [0, 1)");
-    CAPB_REQUIRE(opts->temperature > 0.f, "temperature must be positive");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss};
     TfmTrainArgs ta;
-    ta.n = n; ta.L = e->T; ta.p_lm = opts->drop_prob_lm; ta.p = opts->dropout; ta.temperature = opts->temperature; ta.upstream = opts->upstream; ta.seed = opts->seed;
-    ta.greedy_baseline = greedy_baseline; ta.table = table; ta.refs = refs; ta.ref_offsets = ref_offsets; ta.Lref = L; ta.sample_seq = sample_seq;
-    ta.greedy_seq = greedy_seq; ta.reward = reward; ta.logprobs = sample_logprobs; ta.loss = loss; ta.forced = opts->forced_tokens; ta.mask = opts->att_masks;
-    ta.keep = opts->keep_rows; ta.row_loss = opts->row_loss;
-    CAPB_REQUIRE(ta.keep >= 0 && ta.keep <= B * n, "keep_rows must be in 0..rows");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the whole step (~4900 launches at 6 + 6 layers) as one CUDA graph: see capb200_aoa_scst_step and engine_common.cuh (StepGraph)
-    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || e->sg.broken) {
-        if (dropout_salt_set_all(0ull, st)) return 1;      // eager step: the seed arguments are the effective seeds
-        return tfm_train_step(e, att, B, R, ta, grads, st);
-    }
-    cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
-    const void* srcs[2] = {att, ta.mask};
-    const size_t bytes[2] = {sizeof(float) * (size_t)B * R * e->F, ta.mask ? sizeof(float) * (size_t)B * R : 0};
-    size_t off[2];
-    if (e->sg.stage_inputs(2, srcs, bytes, off, gst)) return 1;
-    const float* att_s = reinterpret_cast<const float*>(e->sg.stage + off[0]);
-    if (ta.mask) ta.mask = reinterpret_cast<const float*>(e->sg.stage + off[1]);
-    unsigned long long key = 1469598103934665603ull;
-    capb200_tfm_scst_opts o2 = *opts; o2.seed = 0; o2.att_masks = ta.mask;
-    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
-    const void* ptrs[] = {table, refs, ref_offsets, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
-    StepGraph::mix(key, ptrs, sizeof(ptrs));
-    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
-    const int dims[] = {B, R, L};
-    StepGraph::mix(key, dims, sizeof(dims));
-    const int rc_graph = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return tfm_train_step(e, att_s, B, R, ta, grads, gst); });
-    if (e->sg.leave(st, gst)) return 1;
-    return rc_graph;
+    if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
+    ta.p_lm = opts->drop_prob_lm;
+    return run_scst_step(e, opts, grads, ta, nullptr, 0, att, sizeof(float) * (size_t)B * R * e->F, B, R, static_cast<cudaStream_t>(stream),
+                         [&](const float*, const float* att_s, const TfmTrainArgs& t, cudaStream_t s) { return tfm_train_step(e, att_s, B, R, t, grads, s); });
 }

@@ -1,0 +1,299 @@
+// The scaffold every fused training step shares (UpDown, Att2in2 and NewFC in engine.cu, AoANet in aoa_engine.cu, the Transformer in
+// tfm_engine.cu): the tape buffers of the loss and the sampler, tape growth, the greedy baseline on the side stream, the word feed and the
+// vocabulary step of the forward, the loss and its d logits, the option checks, and the eager-or-graph dispatch of the SCST step.  A family
+// keeps its prologue, its core step, the backward through time and the weight gradients.
+#pragma once
+#include "engine_common.cuh"
+
+namespace capb200 {
+
+// an fp32-only view (no fp16 planes) of a row-major activation
+inline ActView f32_view(float* f, long ld) { return ActView{f, nullptr, nullptr, ld}; }
+
+// One training step: SCST (sampled words, reward-weighted loss) or XE (teacher-forced words, cross-entropy).
+struct TrainArgs {
+    bool xe = false;
+    int n = 1;                 // rows per image: train_sample_n (SCST) or seq_per_img (XE)
+    int T = 0;                 // steps (positions) evaluated, and columns of the tape
+    int Tl = 0;                // columns of the log-prob output [N, Tl, V1]
+    float p = 0.f;             // the family's main dropout rate (drop_prob_lm; the Transformer's own `dropout`)
+    float temperature = 1.f, upstream = 1.f, smoothing = 0.f;
+    unsigned long long seed = 0;
+    // SCST
+    bool greedy_baseline = true;
+    const capb200_cider_table* table = nullptr;
+    const int* refs = nullptr; const int* ref_offsets = nullptr; int L = 0;     // CIDEr-D references; L = their length
+    long long* sample_seq = nullptr; long long* greedy_seq = nullptr; float* reward = nullptr;
+    const long long* forced = nullptr;      // replay these samples instead of drawing
+    const float* mask = nullptr;            // [B, R] region mask or null
+    float ss_prob = 0.f;                    // XE: scheduled sampling probability
+    long long* tokens_used = nullptr;       // XE: optional [N, Tl] record of the words fed
+    int keep = 0;                           // drop_worst: rows kept (0 = reduction 'mean')
+    float* row_loss = nullptr;              // drop_worst: optional per-row loss output
+    // XE
+    const long long* labels = nullptr; long ld_labels = 0; const float* masks = nullptr; long ld_masks = 0;
+    float* logprobs = nullptr; float* loss = nullptr;
+};
+
+// Checks the SCST options every family shares and fills `ta`.  A family hands its own options over as capb200_scst_opts (drop_prob = its
+// main dropout rate) and checks its other rates itself.
+inline int scst_train_args(int B, const capb200_scst_opts& o, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                           long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, int T, TrainArgs* ta) {
+    const bool greedy_baseline = o.baseline == CAPB200_BASELINE_GREEDY;
+    CAPB_REQUIRE(greedy_baseline || o.baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
+    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
+    CAPB_REQUIRE(greedy_baseline || o.sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
+    CAPB_REQUIRE(o.sample_n >= 1 && o.sample_n <= 16 && B >= 1, "sample_n must be in 1..16");
+    CAPB_REQUIRE(o.drop_prob >= 0.f && o.drop_prob < 1.f, "dropout rates must be in [0, 1)");
+    CAPB_REQUIRE(o.temperature > 0.f, "temperature must be positive");
+    CAPB_REQUIRE(o.keep_rows >= 0 && o.keep_rows <= B * o.sample_n, "keep_rows must be in 0..rows");
+    ta->n = o.sample_n; ta->T = T; ta->Tl = T; ta->p = o.drop_prob; ta->temperature = o.temperature; ta->upstream = o.upstream;
+    ta->seed = o.seed; ta->greedy_baseline = greedy_baseline; ta->table = table; ta->refs = refs; ta->ref_offsets = ref_offsets; ta->L = L;
+    ta->sample_seq = sample_seq; ta->greedy_seq = greedy_seq; ta->reward = reward; ta->logprobs = sample_logprobs; ta->loss = loss;
+    ta->forced = o.forced_tokens; ta->mask = o.att_masks; ta->keep = o.keep_rows; ta->row_loss = o.row_loss;
+    return 0;
+}
+
+// Checks the XE options every family shares and fills `ta`; a family hands its own options over as capb200_xe_opts, as above.  T is the
+// engine's seq_length.
+inline int xe_train_args(int B, const capb200_xe_opts& o, const long long* labels, const float* masks, int label_cols, float* logprobs, float* loss,
+                         int T, TrainArgs* ta) {
+    CAPB_REQUIRE(o.seq_per_img >= 1 && o.seq_per_img <= 16 && B >= 1, "seq_per_img must be in 1..16");
+    CAPB_REQUIRE(o.drop_prob >= 0.f && o.drop_prob < 1.f, "dropout rates must be in [0, 1)");
+    CAPB_REQUIRE(o.label_smoothing >= 0.f && o.label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
+    CAPB_REQUIRE(label_cols >= 2 && label_cols <= T + 2, "labels are [N, seq_length + 2] (BOS, words, EOS padding)");
+    CAPB_REQUIRE(o.steps >= 1 && o.steps <= label_cols - 1, "steps must be in 1..label_cols-1");
+    CAPB_REQUIRE(o.ss_prob >= 0.f && o.ss_prob <= 1.f, "ss_prob must be in [0, 1]");
+    CAPB_REQUIRE(o.keep_rows >= 0 && o.keep_rows <= B * o.seq_per_img, "keep_rows must be in 0..rows");
+    ta->xe = true;
+    ta->n = o.seq_per_img; ta->T = o.steps; ta->Tl = label_cols - 1; ta->p = o.drop_prob; ta->upstream = o.upstream; ta->seed = o.seed;
+    ta->smoothing = o.label_smoothing;
+    ta->labels = labels; ta->ld_labels = label_cols; ta->masks = masks; ta->ld_masks = label_cols; ta->logprobs = logprobs; ta->loss = loss;
+    ta->mask = o.att_masks; ta->ss_prob = o.ss_prob; ta->tokens_used = o.tokens_used; ta->keep = o.keep_rows; ta->row_loss = o.row_loss;
+    return 0;
+}
+
+// The buffers every training tape has: d loss / d logits, the criterion's scratch, the greedy baseline's log-probs, the split-K scratch of
+// the skinny GEMMs, and the sampling loop's own word state (the greedy baseline runs concurrently on the decode workspace).  Each family's
+// tape derives from it, so the helpers below take a StepTape&.
+struct StepTape {
+    float* DL;                                 // [N, T, V1]
+    float *mask_sum, *item_loss, *glp, *skinny;
+    size_t skinny_floats;
+    double* scores;
+    int *s_tokens, *s_unfinished, *s_forced;
+    float *row_loss, *row_msum, *row_coef;     // drop_worst: per-row loss, mask count and gradient coefficient
+
+    // TN = rows of the tape (positions x N); glp_floats = the greedy baseline's log-prob buffer
+    void layout(Arena& a, int B, int N, long TN, int V1, long glp_floats) {
+        DL = a.take<float>(TN * V1);
+        mask_sum = a.take<float>(8);
+        item_loss = a.take<float>(TN);
+        glp = a.take<float>(glp_floats);
+        skinny_floats = (size_t)4 << 20;       // split-K partial sums (16 MB)
+        skinny = a.take<float>((long)skinny_floats);
+        scores = a.take<double>((long)N + B);
+        s_tokens = a.take<int>(N); s_unfinished = a.take<int>(N); s_forced = a.take<int>(N);
+        row_loss = a.take<float>(N); row_msum = a.take<float>(N); row_coef = a.take<float>(N);
+    }
+};
+
+// Lays `tp` out on the engine's training tape (`layout(tp, arena)`), growing the tape first if the layout does not fit; growing synchronises.
+template <class Tape, class Layout>
+int carve_tape(char** tape, size_t* tape_bytes, Tape& tp, cudaStream_t st, Layout layout) {
+    Arena dry;
+    Tape sized;
+    layout(sized, dry);
+    if (grow_buffer(reinterpret_cast<void**>(tape), tape_bytes, dry.off + 256, st)) return 1;
+    Arena ar;
+    ar.base = *tape;
+    layout(tp, ar);
+    return 0;
+}
+
+// The skinny-GEMM runner of a training step on the tape's split-K scratch: wgmma 3xTF32 GEMMs through the engine's tf32 context unless
+// the engine is in simt_fp32 mode.  Each step starts a new context step: the weights may have changed since the last one.
+inline Skinny step_gemms(Tf32Context** ctx, bool tc, const StepTape& tp, cudaStream_t st) {
+    if (tc && *ctx == nullptr) *ctx = tf32_context_create();
+    tf32_context_new_step(*ctx);
+    Skinny sk{tp.skinny, tp.skinny_floats, tc ? 1 : 0, st};
+    sk.ctx = *ctx;
+    return sk;
+}
+
+// The eval-mode greedy baseline of an SCST step: the regular greedy decode on B rows, without dropout.  It and the train-mode sampling
+// forward are independent chains of small, latency-bound kernels, so the baseline runs on the engine's side stream -- forked from the step's
+// stream, joined before the reward -- unless CAPB200_SCST_SERIAL_GREEDY is set or the side stream cannot be created.  Three calls: fork at
+// the top of the step, enqueue where the family wants its launches issued, join (inside loss_backward).
+struct GreedyBaseline {
+    bool needed = false;
+    cudaStream_t st = nullptr;      // where its launches go
+    cudaEvent_t done = nullptr;     // recorded on the side stream after them; null when they run on the step's stream
+
+    int fork(const TrainArgs& ta, cudaStream_t* side, cudaEvent_t* ev_fork, cudaEvent_t* ev_join, cudaStream_t step_st) {
+        needed = !ta.xe && ta.greedy_baseline;
+        st = step_st;
+        done = nullptr;
+        static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
+        if (!needed || serial) return 0;
+        bool ok = *side != nullptr || create_side_stream(side) == cudaSuccess;
+        if (ok && *ev_fork == nullptr) ok = cudaEventCreateWithFlags(ev_fork, cudaEventDisableTiming) == cudaSuccess;
+        if (ok && *ev_join == nullptr) ok = cudaEventCreateWithFlags(ev_join, cudaEventDisableTiming) == cudaSuccess;
+        if (!ok) { (void)cudaGetLastError(); return 0; }
+        CAPB_CHECK_CUDA(cudaEventRecord(*ev_fork, step_st));
+        CAPB_CHECK_CUDA(cudaStreamWaitEvent(*side, *ev_fork, 0));
+        st = *side;
+        done = *ev_join;
+        return 0;
+    }
+    // decode(opts, greedy_seq, logprobs, stream) is the family's capb200_*decode_sample
+    template <class Decode>
+    int enqueue(int B, int T, int V1, long long* greedy_seq, float* glp, Decode decode) const {
+        if (!needed) return 0;
+        CAPB_NVTX("capb200 scst: greedy baseline (eval mode, side stream)");
+        capb200_sample_opts so;
+        memset(&so, 0, sizeof(so));
+        so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.seed = 0; so.steps = T;
+        CAPB_CHECK_CUDA(cudaMemsetAsync(glp, 0, sizeof(float) * (size_t)B * T * V1, st));
+        CAPB_CHECK_CUDA(cudaMemsetAsync(greedy_seq, 0, sizeof(long long) * (size_t)B * T, st));
+        if (decode(&so, greedy_seq, glp, static_cast<void*>(st))) return 1;
+        if (done != nullptr) CAPB_CHECK_CUDA(cudaEventRecord(done, st));
+        return 0;
+    }
+    int join(cudaStream_t step_st) const {
+        if (done != nullptr) CAPB_CHECK_CUDA(cudaStreamWaitEvent(step_st, done, 0));
+        return 0;
+    }
+};
+
+// The words fed at step t into `tok` (the tape's column t).  XE feeds the labels -- or, with scheduled sampling, draws from the model's
+// previous prediction (AttModel.py:145-154) -- and records them in ta.tokens_used if asked; SCST feeds the previous step's draw.
+inline int feed_tokens(const TrainArgs& ta, const StepTape& tp, int N, int V1, int t, int* tok, cudaStream_t st) {
+    if (!ta.xe) {
+        CAPB_CHECK_CUDA(cudaMemcpyAsync(tok, tp.s_tokens, sizeof(int) * N, cudaMemcpyDeviceToDevice, st));
+        return 0;
+    }
+    if (t >= 1 && ta.ss_prob > 0.f) {
+        if (ss_select_launch(N, V1, ta.logprobs + (long)(t - 1) * V1, (long)ta.Tl * V1, ta.labels, ta.ld_labels, t, ta.seed, ta.ss_prob, tok, st)) return 1;
+    } else if (load_token_column_launch(ta.labels, ta.ld_labels, t, N, tok, st)) return 1;
+    if (ta.tokens_used != nullptr && store_token_column_launch(tok, N, ta.tokens_used, ta.Tl, t, st)) return 1;
+    return 0;
+}
+
+// The vocabulary step at step t: log_softmax of the logits at ta.logprobs[:, t] in place; SCST also draws the next words (multinomial at
+// ta.temperature, or the replay of ta.forced) into tp.s_tokens and ta.sample_seq.
+inline int train_vocab_step(const TrainArgs& ta, const StepTape& tp, int N, int V1, int t, cudaStream_t st) {
+    VocabStepArgs va;
+    va.rows = N; va.V1 = V1; va.logits = ta.logprobs + (long)t * V1; va.ld = (long)ta.Tl * V1;
+    if (!ta.xe) {
+        va.select = 2; va.temperature = ta.temperature; va.seed = ta.seed; va.step = (unsigned long long)t;
+        va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
+        va.seq_out = ta.sample_seq; va.ld_seq = ta.T; va.t = t;
+        if (ta.forced != nullptr) {
+            if (load_token_column_launch(ta.forced, ta.T, t, N, tp.s_forced, st)) return 1;
+            va.select = 3; va.forced = tp.s_forced;
+        }
+    }
+    return vocab_step_launch(va, st);
+}
+
+// The loss and d loss / d logits into tp.DL: the XE criterion (LanguageModelCriterion / LabelSmoothing), or -- after joining the greedy
+// baseline -- the CIDEr-D reward, RewardCriterion, drop_worst and the d logits of the SCST loss.
+inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBaseline& gb, int B, int N, int V1, cudaStream_t st) {
+    const int T = ta.T;
+    const long ld_lp = (long)ta.Tl * V1;
+    float* row_loss = ta.row_loss ? ta.row_loss : tp.row_loss;
+    if (ta.xe)
+        return xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
+                                       tp.mask_sum, tp.item_loss, tp.DL, ta.loss, st, ta.keep, row_loss, tp.row_msum, tp.row_coef);
+    if (gb.join(st)) return 1;     // the reward needs the baseline captions
+    if (cider_reward_launch(ta.table->t, ta.sample_seq, N, ta.greedy_baseline ? ta.greedy_seq : nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores,
+                            ta.reward, T, T, st)) return 1;
+    float* rl = ta.keep > 0 ? row_loss : nullptr;
+    if (reward_criterion_fwd_launch(ta.logprobs, ld_lp, V1, ta.sample_seq, ta.reward, N, T, ta.loss, rl, tp.mask_sum, st)) return 1;
+    if (ta.keep > 0 && scst_drop_worst_launch(ta.sample_seq, rl, N, T, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, ta.loss, st)) return 1;
+    return scst_dlogits_launch(ta.logprobs, ld_lp, ta.sample_seq, ta.reward, tp.mask_sum, ta.upstream, N, T, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr);
+}
+
+// loss_backward, then the backward of a logit layer [V1, H] batched over all (n, t): dOUT [N, T, H] = DL W, and the logit gradients (group
+// 0, whose event `ev` is recorded here).  `out` holds the layer's inputs [N, T, H].
+inline int loss_and_logit_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBaseline& gb, const Skinny& sk, int B, int N, int V1, int H,
+                                   const float* logit_w, const float* out, float* dOUT, float* g_logit_w, float* g_logit_b, cudaEvent_t ev, cudaStream_t st) {
+    const int TN = ta.T * N;
+    if (loss_backward(ta, tp, gb, B, N, V1, st)) return 1;
+    if (sk.dgrad(TN, H, V1, tp.DL, V1, logit_w, H, dOUT, H, 0)) return 1;          // dOUT = DL * W
+    if (sk.wgrad(V1, H, TN, tp.DL, V1, out, H, g_logit_w, H, 0)) return 1;         // dW = DL^T * OUT
+    if (colsum_launch(TN, V1, tp.DL, V1, g_logit_b, 0, st)) return 1;
+    return record_group_event(ev, st);
+}
+
+// q | k | v weight and bias gradients of a self-attention block from d_qkv [rows, 3D] and its input x [rows, D]: one GEMM / one column
+// reduction when the caller laid the three tensors out back to back (the Python mirror's flat gradient buffer does), else three.  The column
+// reductions it launches are added to *colsums when that is given.
+template <class Grads>
+int qkv_grads(const Skinny& sk, int rows, int D, const float* d_qkv, const float* x, const Grads& g, long* colsums, cudaStream_t st) {
+    int rc = 0;
+    if (g.k_w == g.q_w + (long)D * D && g.v_w == g.k_w + (long)D * D) {
+        rc |= sk.wgrad(3 * D, D, rows, d_qkv, 3 * D, x, D, g.q_w, D, 0);
+    } else {
+        rc |= sk.wgrad(D, D, rows, d_qkv, 3 * D, x, D, g.q_w, D, 0);
+        rc |= sk.wgrad(D, D, rows, d_qkv + D, 3 * D, x, D, g.k_w, D, 0);
+        rc |= sk.wgrad(D, D, rows, d_qkv + 2 * D, 3 * D, x, D, g.v_w, D, 0);
+    }
+    const bool packed_b = g.k_b == g.q_b + D && g.v_b == g.k_b + D;
+    if (packed_b) {
+        rc |= colsum_launch(rows, 3 * D, d_qkv, 3 * D, g.q_b, 0, st);
+    } else {
+        rc |= colsum_launch(rows, D, d_qkv, 3 * D, g.q_b, 0, st);
+        rc |= colsum_launch(rows, D, d_qkv + D, 3 * D, g.k_b, 0, st);
+        rc |= colsum_launch(rows, D, d_qkv + 2 * D, 3 * D, g.v_b, 0, st);
+    }
+    if (colsums != nullptr) *colsums += packed_b ? 1 : 3;
+    return rc;
+}
+
+// An eager training step: the seed arguments are the effective seeds (a graph replay of an SCST step may have left a salt behind).
+template <class Step>
+int run_eager_step(cudaStream_t st, Step step) {
+    if (dropout_salt_set_all(0ull, st)) return 1;
+    return step();
+}
+
+// Runs one SCST step, `step(fc, att, ta, stream)`, as ONE CUDA graph.  Its ~900-4900 kernels are 5-30 us each, every launch boundary costs
+// ~2 us on the stream, the host needs milliseconds to enqueue them, and nothing about the sequence depends on data: the step is captured the
+// second time a configuration is seen and replayed afterwards with a fresh seed (dropout.cuh: seed salt).  The features fc / att and the
+// region mask ta.mask are copied into the engine-owned staging buffer first, so that the graph reads stable addresses (an input of zero
+// bytes is not staged and reaches the step as null); the key covers every option but the seed, the gradient and weight tables, every pointer
+// the step touches and the shapes.  The gradient-group events a data-parallel caller listens to become external event-record nodes of the
+// graph (record_group_event) and are part of the key; CAPB200_SCST_GRAPH_SYNC=0 keeps the step eager while any is set.  The step also stays
+// eager with CAPB200_SCST_GRAPH=0, in the simt_fp32 mode, when forced tokens are replayed, and once a capture has failed.
+template <class Engine, class Opts, class Grads, class Args, class Step>
+int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& ta, const float* fc, size_t fc_bytes, const float* att, size_t att_bytes,
+                  int B, int R, cudaStream_t st, Step step) {
+    static const bool graph_with_listener = !(getenv("CAPB200_SCST_GRAPH_SYNC") != nullptr && atoi(getenv("CAPB200_SCST_GRAPH_SYNC")) == 0);
+    bool listening = false;
+    for (cudaEvent_t ev : e->grad_events) listening = listening || ev != nullptr;
+    if (!StepGraph::enabled() || !e->tc || (listening && !graph_with_listener) || ta.forced != nullptr || e->sg.broken)
+        return run_eager_step(st, [&] { return step(fc, att, ta, st); });
+    cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
+    const void* srcs[3] = {fc, att, ta.mask};
+    const size_t bytes[3] = {fc_bytes, att_bytes, ta.mask ? sizeof(float) * (size_t)B * R : 0};
+    size_t off[3];
+    if (e->sg.stage_inputs(3, srcs, bytes, off, gst)) return 1;
+    auto staged = [&](int i) { return bytes[i] ? reinterpret_cast<const float*>(e->sg.stage + off[i]) : nullptr; };
+    Args ts = ta;
+    ts.mask = staged(2);
+    unsigned long long key = 1469598103934665603ull;
+    Opts o2 = *opts; o2.seed = 0; o2.att_masks = ts.mask;
+    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
+    const void* ptrs[] = {ta.table, ta.refs, ta.ref_offsets, ta.sample_seq, ta.greedy_seq, ta.logprobs, ta.reward, ta.loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
+    StepGraph::mix(key, ptrs, sizeof(ptrs));
+    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
+    const int dims[] = {B, R, ta.L};
+    StepGraph::mix(key, dims, sizeof(dims));
+    const int rc = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return step(staged(0), staged(1), ts, gst); });
+    if (e->sg.leave(st, gst)) return 1;
+    return rc;
+}
+
+}  // namespace capb200
