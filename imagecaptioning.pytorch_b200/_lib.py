@@ -64,9 +64,14 @@ class SampleOpts(Structure):
         super().__init__(sample_n, method, temperature, seed, steps, top, edits if edits is not None else DecodeEdits.none())
 
 
+class RewardWeights(Structure):
+    _fields_ = [('cider', c_double), ('bleu', c_double)]
+
+
 class ScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('drop_prob', c_float), ('upstream', c_float), ('baseline', c_int),
-                ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int), ('row_loss', c_void_p)]
+                ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int), ('row_loss', c_void_p),
+                ('reward_weights', POINTER(RewardWeights))]
 
 
 BASELINE_GREEDY, BASELINE_LEAVE_ONE_OUT = 0, 1
@@ -75,7 +80,8 @@ BASELINE_GREEDY, BASELINE_LEAVE_ONE_OUT = 0, 1
 class AoaScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('upstream', c_float), ('baseline', c_int),
                 ('drop_prob_lm', c_float), ('drop_attn', c_float), ('drop_aoa', c_float), ('drop_sublayer', c_float), ('ctx_drop', c_int),
-                ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int), ('row_loss', c_void_p)]
+                ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int), ('row_loss', c_void_p),
+                ('reward_weights', POINTER(RewardWeights))]
 
 
 class AoaXeOpts(Structure):
@@ -147,7 +153,7 @@ class TfmXeOpts(Structure):
 class TfmScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('upstream', c_float), ('baseline', c_int),
                 ('drop_prob_lm', c_float), ('dropout', c_float), ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int),
-                ('row_loss', c_void_p)]
+                ('row_loss', c_void_p), ('reward_weights', POINTER(RewardWeights))]
 
 
 AOA_REFINER_LAYERS = 6
@@ -241,6 +247,9 @@ SIGNATURES = {
     'capb200_cider_table_create': (c_void_p, [c_void_p, c_void_p, c_long, c_double, c_void_p]),
     'capb200_cider_table_destroy': (None, [c_void_p]),
     'capb200_cider_scores': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    'capb200_bleu4_scores': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    'capb200_weighted_reward': (c_int, [c_void_p, POINTER(RewardWeights), c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                        c_void_p, c_void_p, c_void_p]),
     'capb200_updown_xe_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                        c_void_p, c_void_p]),
     'capb200_self_critical_reward': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p,

@@ -735,7 +735,7 @@ extern "C" int capb200_aoa_scst_step(capb200_aoa_engine* e, const float* att, in
     const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
     CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
     const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss};
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->reward_weights};
     AoaTrainArgs ta;
     if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;

@@ -1666,6 +1666,21 @@ int capb200_cider_scores(const capb200_cider_table* t, const long long* sampled,
     return cider_reward_launch(t->t, sampled, S, nullptr, B, T, refs, ref_offsets, L, scores, reward, T, T, static_cast<cudaStream_t>(stream));
 }
 
+int capb200_bleu4_scores(const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs, const int* ref_offsets, int L,
+                         double* scores, void* stream) {
+    CAPB_REQUIRE(sampled && refs && ref_offsets && scores, "null argument");
+    return bleu_scores_launch(sampled, S, greedy, B, T, refs, ref_offsets, L, scores, static_cast<cudaStream_t>(stream));
+}
+
+int capb200_weighted_reward(const capb200_cider_table* t, const capb200_reward_weights* w, const long long* sampled, int S, const long long* greedy,
+                            int B, int T, const int* refs, const int* ref_offsets, int L, double* scores, double* bleu_scores, float* reward,
+                            void* stream) {
+    CAPB_REQUIRE(sampled && refs && ref_offsets && scores, "null argument");
+    const double wc = w ? w->cider : 1.0, wb = w ? w->bleu : 0.0;
+    return weighted_reward_launch(t ? t->t : nullptr, wc, wb, sampled, S, greedy, B, T, refs, ref_offsets, L, scores, bleu_scores, reward, T, T,
+                                  static_cast<cudaStream_t>(stream));
+}
+
 int capb200_reward_criterion_forward(const float* logprobs, const long long* seq, const float* reward, int N, int T, int V1, float* loss_mean,
                                      float* loss_rows, float* mask_sum, void* stream) {
     CAPB_REQUIRE(logprobs && seq && reward && N > 0 && T > 0, "bad argument");

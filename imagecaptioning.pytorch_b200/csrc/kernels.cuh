@@ -259,6 +259,15 @@ CiderTable* cider_table_create(const int* keys, const double* df, long n, double
 void cider_table_destroy(CiderTable* t);
 int cider_reward_launch(const CiderTable* t, const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs,
                         const int* ref_offsets, int L, double* scores, float* reward, long ld_reward, int reward_cols, cudaStream_t stream);
+// per-hypothesis BLEU-4 (float64), hypotheses and references laid out as for cider_reward_launch
+int bleu_scores_launch(const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs, const int* ref_offsets, int L,
+                       double* scores, cudaStream_t stream);
+// scores = w_cider * CIDEr-D + w_bleu * BLEU-4 (a term only when its weight is > 0; t may be null when w_cider <= 0, bleu [hyps] scratch may be null
+// when w_bleu <= 0), then the reward as cider_reward_launch writes it
+int weighted_reward_launch(const CiderTable* t, double w_cider, double w_bleu, const long long* sampled, int S, const long long* greedy, int B, int T,
+                           const int* refs, const int* ref_offsets, int L, double* scores, double* bleu, float* reward, long ld_reward, int reward_cols,
+                           cudaStream_t stream);
+int weighted_reward_launches(double w_cider, double w_bleu, bool with_reward);     // kernels weighted_reward_launch issues
 int reward_criterion_fwd_launch(const float* logprobs, long ld_row, long ld_t, const long long* seq, const float* reward, int N, int T,
                                 float* loss_mean, float* loss_rows, float* mask_sum, cudaStream_t stream);
 int reward_criterion_bwd_launch(const long long* seq, const float* reward, int N, int T, const float* mask_sum, float upstream,

@@ -10,6 +10,9 @@
 //   * per order n: sum over the hypothesis' distinct n-grams of min(w_h, w_r) * w_r, divided by |h||r| when both are
 //     non-zero, times exp(-(len_h - len_r)^2 / (2 * 6^2)) where len counts BIGRAMS (ciderD_scorer.py:177-178),
 //   * score = 10 * mean over references of the mean over n = 1..4.
+//
+// The BLEU-4 term of the reward (rewards.py:68-74, coco-caption/pycocoevalcap/bleu) and the weighted sum of the two terms are here too.
+#include <cmath>
 #include <vector>
 
 #include "common.cuh"
@@ -203,6 +206,105 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
     if (threadIdx.x == 0) scores[hyp] = (r1 > r0) ? total / (double)(r1 - r0) * 10.0 : 0.0;
 }
 
+// BLEU-4 of one hypothesis, the per-sentence bleu_list[3] of BleuScorer.compute_score(option='closest') (bleu_scorer.py:26-80,184-260):
+//   guess[k] = max(0, len_h - k);  correct[k] = sum over the hypothesis' distinct (k+1)-grams of min(count in h, max count in one reference)
+//   bleu = (prod_k (correct[k] + 1e-15) / (guess[k] + 1e-9)) ** (1/4), times exp(1 - 1/ratio) when ratio = (len_h + 1e-15) / (reflen + 1e-9) < 1,
+//   reflen = the reference length closest to len_h, the shorter one on a tie.  Lengths count words, the closing 0 included.
+// One CTA per hypothesis, laid out as cider_score_kernel; thread g owns the n-gram of order g / 64 + 1 starting at position g % 64.  The image's
+// references are staged in shared memory BLEU_REF_CHUNK at a time.  An image without references scores 0 (the Python layer refuses it).
+constexpr int BLEU_REF_CHUNK = 32;
+
+__global__ void __launch_bounds__(CIDER_N * CIDER_MAXL) bleu_score_kernel(const long long* __restrict__ sampled, int S, const long long* __restrict__ greedy,
+                                                                          int B, int T, const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L,
+                                                                          double* __restrict__ scores) {
+    __shared__ int h_tok[CIDER_MAXL];
+    __shared__ int r_tok[BLEU_REF_CHUNK][CIDER_MAXL];
+    __shared__ int r_len[BLEU_REF_CHUNK];
+    __shared__ int correct[CIDER_N];
+    __shared__ int h_len;
+    const int hyp = blockIdx.x;
+    const int n_per = (B > 0) ? S / B : 1;
+    const int img = hyp < S ? hyp / n_per : hyp - S;
+    const long long* src = hyp < S ? sampled + (long)hyp * T : greedy + (long)(hyp - S) * T;
+    if (threadIdx.x == 0) {
+        int len = 0;
+        for (int i = 0; i < T && i < CIDER_MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
+        h_len = len;
+    }
+    if (threadIdx.x < CIDER_N) correct[threadIdx.x] = 0;
+    __syncthreads();
+    const int hl = h_len;
+    const int n = threadIdx.x / CIDER_MAXL + 1, p = threadIdx.x % CIDER_MAXL;
+    // counted by its first occurrence only: tf = how often the n-gram occurs in the hypothesis
+    bool first = p + n <= hl;
+    int tf = 0;
+    for (int q = 0; first && q + n <= hl; ++q) {
+        if (same_gram(h_tok + p, h_tok + q, n)) {
+            if (q < p) first = false;
+            else ++tf;
+        }
+    }
+    int max_ref = 0;                                    // the n-gram's largest count in a single reference
+    int best_len = -1, best_diff = 0;                   // closest reference length (thread 0)
+    const int r0 = ref_offsets[img], r1 = ref_offsets[img + 1];
+    const int cols = L < CIDER_MAXL ? L : CIDER_MAXL;
+    for (int c0 = r0; c0 < r1; c0 += BLEU_REF_CHUNK) {
+        const int cnt = r1 - c0 < BLEU_REF_CHUNK ? r1 - c0 : BLEU_REF_CHUNK;
+        __syncthreads();                                // the previous chunk has been read
+        for (int i = threadIdx.x; i < cnt * CIDER_MAXL; i += blockDim.x) {
+            const int r = i / CIDER_MAXL, j = i % CIDER_MAXL;
+            r_tok[r][j] = j < cols ? refs[(long)(c0 + r) * L + j] : 0;
+        }
+        __syncthreads();
+        if (threadIdx.x < cnt) {
+            int len = 0;
+            for (int j = 0; j < cols; ++j) { ++len; if (r_tok[threadIdx.x][j] == 0) break; }
+            r_len[threadIdx.x] = len;
+        }
+        __syncthreads();
+        if (first) {
+            for (int r = 0; r < cnt; ++r) {
+                int c = 0;
+                for (int q = 0; q + n <= r_len[r]; ++q) c += same_gram(h_tok + p, r_tok[r] + q, n) ? 1 : 0;
+                max_ref = c > max_ref ? c : max_ref;
+            }
+        }
+        if (threadIdx.x == 0) {
+            for (int r = 0; r < cnt; ++r) {
+                const int d = abs(r_len[r] - hl);
+                if (best_len < 0 || d < best_diff || (d == best_diff && r_len[r] < best_len)) { best_len = r_len[r]; best_diff = d; }
+            }
+        }
+    }
+    if (first) atomicAdd(&correct[n - 1], tf < max_ref ? tf : max_ref);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        if (best_len >= 0) {
+            double prod = 1.0;
+            for (int k = 0; k < CIDER_N; ++k) {
+                const int guess = hl - k > 0 ? hl - k : 0;
+                prod *= ((double)correct[k] + 1e-15) / ((double)guess + 1e-9);
+            }
+            s = pow(prod, 0.25);
+            const double ratio = ((double)hl + 1e-15) / ((double)best_len + 1e-9);
+            if (ratio < 1.0) s *= exp(1.0 - 1.0 / ratio);
+        }
+        scores[hyp] = s;
+    }
+}
+
+// score = cider_weight * CIDEr-D + bleu_weight * BLEU-4 in place over `scores` (which holds CIDEr-D when its weight is > 0), in float64 as
+// rewards.py:74,112 computes it; a term whose weight is <= 0 was not computed and contributes weight * 0.  Rounded operations keep the
+// compiler from contracting the sum into an FMA that numpy does not perform.
+__global__ void reward_combine_kernel(double* __restrict__ scores, const double* __restrict__ bleu, int hyps, double wc, double wb) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= hyps) return;
+    const double c = __dmul_rn(wc, wc > 0.0 ? scores[i] : 0.0);
+    const double b = __dmul_rn(wb, wb > 0.0 ? bleu[i] : 0.0);
+    scores[i] = __dadd_rn(c, b);
+}
+
 __global__ void cider_reward_kernel(const double* __restrict__ scores, int S, int B, float* __restrict__ reward, long ld, int cols) {
     const int i = blockIdx.x;
     const int n_per = S / B;
@@ -263,28 +365,70 @@ __global__ void reward_criterion_bwd_kernel(const long long* __restrict__ seq, c
     grad[(long)n * ld_row + (long)t * ld_t + tok] = -reward[i] * m / (*mask_sum) * upstream;
 }
 
+// The reward from the hypothesis scores: the greedy difference (greedy != nullptr) or the leave-one-out baseline.
+int baseline_reward_launch(const double* scores, int S, const long long* greedy, int B, float* reward, long ld_reward, int reward_cols, cudaStream_t stream) {
+    if (reward == nullptr || S == 0) return 0;
+    if (greedy != nullptr) {
+        cider_reward_kernel<<<S, 32, 0, stream>>>(scores, S, B, reward, ld_reward, reward_cols);
+    } else {
+        CAPB_REQUIRE(S / B >= 2, "the leave-one-out baseline needs at least two samples per image");
+        cider_reward_loo_kernel<<<S, 32, 0, stream>>>(scores, S / B, reward, ld_reward, reward_cols);
+    }
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int check_reward_shapes(int S, int B, int T, int L) {
+    CAPB_REQUIRE(B > 0 && S % B == 0, "sample rows must be a multiple of the image count");
+    CAPB_REQUIRE(T <= CIDER_MAXL && L <= CIDER_MAXL, "caption length above 64 tokens");
+    return 0;
+}
+
 }  // namespace
 
 int cider_reward_launch(const CiderTable* t, const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs,
                         const int* ref_offsets, int L, double* scores, float* reward, long ld_reward, int reward_cols, cudaStream_t stream) {
     CAPB_REQUIRE(t != nullptr, "CIDEr-D table not initialised (init_scorer)");
-    CAPB_REQUIRE(B > 0 && S % B == 0, "sample rows must be a multiple of the image count");
-    CAPB_REQUIRE(T <= CIDER_MAXL && L <= CIDER_MAXL, "caption length above 64 tokens");
+    if (check_reward_shapes(S, B, T, L)) return 1;
     // greedy == nullptr: score the samples only; the reward baseline is then the mean of the image's other samples
     const int hyps = greedy != nullptr ? S + B : S;
     if (hyps == 0) return 0;
     cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, t->log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
     CAPB_CHECK_CUDA(cudaGetLastError());
-    if (reward != nullptr && S > 0) {
-        if (greedy != nullptr) {
-            cider_reward_kernel<<<S, 32, 0, stream>>>(scores, S, B, reward, ld_reward, reward_cols);
-        } else {
-            CAPB_REQUIRE(S / B >= 2, "the leave-one-out baseline needs at least two samples per image");
-            cider_reward_loo_kernel<<<S, 32, 0, stream>>>(scores, S / B, reward, ld_reward, reward_cols);
-        }
+    return baseline_reward_launch(scores, S, greedy, B, reward, ld_reward, reward_cols, stream);
+}
+
+int bleu_scores_launch(const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs, const int* ref_offsets, int L,
+                       double* scores, cudaStream_t stream) {
+    if (check_reward_shapes(S, B, T, L)) return 1;
+    const int hyps = greedy != nullptr ? S + B : S;
+    if (hyps == 0) return 0;
+    bleu_score_kernel<<<hyps, CIDER_N * CIDER_MAXL, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int weighted_reward_launches(double w_cider, double w_bleu, bool with_reward) {
+    return (w_cider > 0.0) + (w_bleu > 0.0) + 1 + (with_reward ? 1 : 0);
+}
+
+int weighted_reward_launch(const CiderTable* t, double w_cider, double w_bleu, const long long* sampled, int S, const long long* greedy, int B, int T,
+                           const int* refs, const int* ref_offsets, int L, double* scores, double* bleu, float* reward, long ld_reward, int reward_cols,
+                           cudaStream_t stream) {
+    CAPB_REQUIRE(std::isfinite(w_cider) && std::isfinite(w_bleu), "reward weights must be finite");
+    CAPB_REQUIRE(w_cider <= 0.0 || t != nullptr, "CIDEr-D table not initialised (init_scorer)");
+    CAPB_REQUIRE(w_bleu <= 0.0 || bleu != nullptr, "the BLEU-4 term needs its score buffer");
+    if (check_reward_shapes(S, B, T, L)) return 1;
+    const int hyps = greedy != nullptr ? S + B : S;
+    if (hyps == 0) return 0;
+    if (w_cider > 0.0) {
+        cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, t->log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
         CAPB_CHECK_CUDA(cudaGetLastError());
     }
-    return 0;
+    if (w_bleu > 0.0 && bleu_scores_launch(sampled, S, greedy, B, T, refs, ref_offsets, L, bleu, stream)) return 1;
+    reward_combine_kernel<<<cdiv(hyps, 256), 256, 0, stream>>>(scores, bleu, hyps, w_cider, w_bleu);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return baseline_reward_launch(scores, S, greedy, B, reward, ld_reward, reward_cols, stream);
 }
 
 int reward_criterion_fwd_launch(const float* logprobs, long ld_row, long ld_t, const long long* seq, const float* reward, int N, int T,

@@ -695,7 +695,7 @@ extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, in
     CAPB_REQUIRE(R >= 1, "attention features required");
     CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
     const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss};
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->reward_weights};
     TfmTrainArgs ta;
     if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     ta.p_lm = opts->drop_prob_lm;

@@ -3,6 +3,8 @@
 // vocabulary step of the forward, the loss and its d logits, the option checks, and the eager-or-graph dispatch of the SCST step.  A family
 // keeps its prologue, its core step, the backward through time and the weight gradients.
 #pragma once
+#include <cmath>
+
 #include "engine_common.cuh"
 
 namespace capb200 {
@@ -23,6 +25,7 @@ struct TrainArgs {
     bool greedy_baseline = true;
     const capb200_cider_table* table = nullptr;
     const int* refs = nullptr; const int* ref_offsets = nullptr; int L = 0;     // CIDEr-D references; L = their length
+    double w_cider = 1.0, w_bleu = 0.0;     // reward weights (capb200_reward_weights, by value)
     long long* sample_seq = nullptr; long long* greedy_seq = nullptr; float* reward = nullptr;
     const long long* forced = nullptr;      // replay these samples instead of drawing
     const float* mask = nullptr;            // [B, R] region mask or null
@@ -33,6 +36,11 @@ struct TrainArgs {
     // XE
     const long long* labels = nullptr; long ld_labels = 0; const float* masks = nullptr; long ld_masks = 0;
     float* logprobs = nullptr; float* loss = nullptr;
+
+    // The weighted reward runs only when it can differ from CIDEr-D alone: a BLEU weight <= 0 adds weight * 0.
+    bool weighted_reward() const { return !xe && (w_bleu > 0.0 || w_cider != 1.0); }
+    // kernels the weighted reward adds to the CIDEr-D reward's two (scores, reward)
+    int reward_extra_launches() const { return weighted_reward() ? weighted_reward_launches(w_cider, w_bleu, true) - 2 : 0; }
 };
 
 // Checks the SCST options every family shares and fills `ta`.  A family hands its own options over as capb200_scst_opts (drop_prob = its
@@ -47,6 +55,10 @@ inline int scst_train_args(int B, const capb200_scst_opts& o, const capb200_cide
     CAPB_REQUIRE(o.drop_prob >= 0.f && o.drop_prob < 1.f, "dropout rates must be in [0, 1)");
     CAPB_REQUIRE(o.temperature > 0.f, "temperature must be positive");
     CAPB_REQUIRE(o.keep_rows >= 0 && o.keep_rows <= B * o.sample_n, "keep_rows must be in 0..rows");
+    if (o.reward_weights != nullptr) {
+        CAPB_REQUIRE(std::isfinite(o.reward_weights->cider) && std::isfinite(o.reward_weights->bleu), "reward weights must be finite");
+        ta->w_cider = o.reward_weights->cider; ta->w_bleu = o.reward_weights->bleu;
+    }
     ta->n = o.sample_n; ta->T = T; ta->Tl = T; ta->p = o.drop_prob; ta->temperature = o.temperature; ta->upstream = o.upstream;
     ta->seed = o.seed; ta->greedy_baseline = greedy_baseline; ta->table = table; ta->refs = refs; ta->ref_offsets = ref_offsets; ta->L = L;
     ta->sample_seq = sample_seq; ta->greedy_seq = greedy_seq; ta->reward = reward; ta->logprobs = sample_logprobs; ta->loss = loss;
@@ -80,7 +92,7 @@ struct StepTape {
     float* DL;                                 // [N, T, V1]
     float *mask_sum, *item_loss, *glp, *skinny;
     size_t skinny_floats;
-    double* scores;
+    double* scores;                            // [N + B] hypothesis scores, then [N + B] BLEU-4 of the weighted reward
     int *s_tokens, *s_unfinished, *s_forced;
     float *row_loss, *row_msum, *row_coef;     // drop_worst: per-row loss, mask count and gradient coefficient
 
@@ -92,7 +104,7 @@ struct StepTape {
         glp = a.take<float>(glp_floats);
         skinny_floats = (size_t)4 << 20;       // split-K partial sums (16 MB)
         skinny = a.take<float>((long)skinny_floats);
-        scores = a.take<double>((long)N + B);
+        scores = a.take<double>(2 * ((long)N + B));
         s_tokens = a.take<int>(N); s_unfinished = a.take<int>(N); s_forced = a.take<int>(N);
         row_loss = a.take<float>(N); row_msum = a.take<float>(N); row_coef = a.take<float>(N);
     }
@@ -198,7 +210,7 @@ inline int train_vocab_step(const TrainArgs& ta, const StepTape& tp, int N, int 
 }
 
 // The loss and d loss / d logits into tp.DL: the XE criterion (LanguageModelCriterion / LabelSmoothing), or -- after joining the greedy
-// baseline -- the CIDEr-D reward, RewardCriterion, drop_worst and the d logits of the SCST loss.
+// baseline -- the reward (CIDEr-D, or the weighted CIDEr-D + BLEU-4), RewardCriterion, drop_worst and the d logits of the SCST loss.
 inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBaseline& gb, int B, int N, int V1, cudaStream_t st) {
     const int T = ta.T;
     const long ld_lp = (long)ta.Tl * V1;
@@ -207,8 +219,11 @@ inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBa
         return xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
                                        tp.mask_sum, tp.item_loss, tp.DL, ta.loss, st, ta.keep, row_loss, tp.row_msum, tp.row_coef);
     if (gb.join(st)) return 1;     // the reward needs the baseline captions
-    if (cider_reward_launch(ta.table->t, ta.sample_seq, N, ta.greedy_baseline ? ta.greedy_seq : nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores,
-                            ta.reward, T, T, st)) return 1;
+    const long long* greedy = ta.greedy_baseline ? ta.greedy_seq : nullptr;
+    if (!ta.weighted_reward()) {
+        if (cider_reward_launch(ta.table->t, ta.sample_seq, N, greedy, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores, ta.reward, T, T, st)) return 1;
+    } else if (weighted_reward_launch(ta.table ? ta.table->t : nullptr, ta.w_cider, ta.w_bleu, ta.sample_seq, N, greedy, B, T, ta.refs, ta.ref_offsets, ta.L,
+                                      tp.scores, tp.scores + N + B, ta.reward, T, T, st)) return 1;
     float* rl = ta.keep > 0 ? row_loss : nullptr;
     if (reward_criterion_fwd_launch(ta.logprobs, ld_lp, V1, ta.sample_seq, ta.reward, N, T, ta.loss, rl, tp.mask_sum, st)) return 1;
     if (ta.keep > 0 && scst_drop_worst_launch(ta.sample_seq, rl, N, T, ta.keep, ta.upstream, tp.row_msum, tp.row_coef, ta.loss, st)) return 1;
@@ -263,8 +278,8 @@ int run_eager_step(cudaStream_t st, Step step) {
 // ~2 us on the stream, the host needs milliseconds to enqueue them, and nothing about the sequence depends on data: the step is captured the
 // second time a configuration is seen and replayed afterwards with a fresh seed (dropout.cuh: seed salt).  The features fc / att and the
 // region mask ta.mask are copied into the engine-owned staging buffer first, so that the graph reads stable addresses (an input of zero
-// bytes is not staged and reaches the step as null); the key covers every option but the seed, the gradient and weight tables, every pointer
-// the step touches and the shapes.  The gradient-group events a data-parallel caller listens to become external event-record nodes of the
+// bytes is not staged and reaches the step as null); the key covers every option but the seed (the reward weights by value), the gradient and
+// weight tables, every pointer the step touches and the shapes.  The gradient-group events a data-parallel caller listens to become external event-record nodes of the
 // graph (record_group_event) and are part of the key; CAPB200_SCST_GRAPH_SYNC=0 keeps the step eager while any is set.  The step also stays
 // eager with CAPB200_SCST_GRAPH=0, in the simt_fp32 mode, when forced tokens are replayed, and once a capture has failed.
 template <class Engine, class Opts, class Grads, class Args, class Step>
@@ -273,8 +288,14 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
     static const bool graph_with_listener = !(getenv("CAPB200_SCST_GRAPH_SYNC") != nullptr && atoi(getenv("CAPB200_SCST_GRAPH_SYNC")) == 0);
     bool listening = false;
     for (cudaEvent_t ev : e->grad_events) listening = listening || ev != nullptr;
+    // the weighted reward's kernels are counted here, so that the families' hand-kept counts stay those of the CIDEr-D reward
+    auto counted = [&](const float* f, const float* a, const Args& t, cudaStream_t s) {
+        const int rc = step(f, a, t, s);
+        e->launches += t.reward_extra_launches();
+        return rc;
+    };
     if (!StepGraph::enabled() || !e->tc || (listening && !graph_with_listener) || ta.forced != nullptr || e->sg.broken)
-        return run_eager_step(st, [&] { return step(fc, att, ta, st); });
+        return run_eager_step(st, [&] { return counted(fc, att, ta, st); });
     cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
     const void* srcs[3] = {fc, att, ta.mask};
     const size_t bytes[3] = {fc_bytes, att_bytes, ta.mask ? sizeof(float) * (size_t)B * R : 0};
@@ -284,14 +305,16 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
     Args ts = ta;
     ts.mask = staged(2);
     unsigned long long key = 1469598103934665603ull;
-    Opts o2 = *opts; o2.seed = 0; o2.att_masks = ts.mask;
-    StepGraph::mix(key, &o2, sizeof(o2)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
+    Opts o2 = *opts; o2.seed = 0; o2.att_masks = ts.mask; o2.reward_weights = nullptr;
+    StepGraph::mix(key, &o2, sizeof(o2));
+    const double weights[2] = {ta.w_cider, ta.w_bleu};      // the values: the caller's struct may keep its address while they change
+    StepGraph::mix(key, weights, sizeof(weights)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
     const void* ptrs[] = {ta.table, ta.refs, ta.ref_offsets, ta.sample_seq, ta.greedy_seq, ta.logprobs, ta.reward, ta.loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
     StepGraph::mix(key, ptrs, sizeof(ptrs));
     StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
     const int dims[] = {B, R, ta.L};
     StepGraph::mix(key, dims, sizeof(dims));
-    const int rc = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return step(staged(0), staged(1), ts, gst); });
+    const int rc = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return counted(staged(0), staged(1), ts, gst); });
     if (e->sg.leave(st, gst)) return 1;
     return rc;
 }

@@ -3,8 +3,8 @@
     B200LossWrapper(model, opt).forward(fc_feats, att_feats, labels, masks, att_masks, gts, gt_indices,
                                         sc_flag, struc_flag, drop_worst_flag) -> {'loss', 'reward'}
 
-sc_flag=True follows loss_wrapper.py:56-73 exactly: eval-mode greedy baseline, train-mode multinomial samples, CIDEr-D
-self-critical reward and RewardCriterion -- every stage on the device through the C ABI.  sc_flag=False is the XE stage
+sc_flag=True follows loss_wrapper.py:56-73 exactly: eval-mode greedy baseline, train-mode multinomial samples, the self-critical
+reward (``cider_reward_weight * CIDEr-D + bleu_reward_weight * BLEU-4``) and RewardCriterion -- every stage on the device through the C ABI.  sc_flag=False is the XE stage
 (loss_wrapper.py:54-55: teacher-forced forward + LanguageModelCriterion / LabelSmoothing) and struc_flag=True the structure-loss
 branch (loss_wrapper.py:25-53) with ``structure_loss_type='new_self_critical'`` (losses.py:168-187), the recipe of the reference's
 best models; both run as one fused device step incl. the backward pass (UpDown, Att2in2, NewFC, AoANet, Transformer).
@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .rewards import cider_scores, get_self_critical_reward
+from .rewards import cider_scores, get_scores, get_self_critical_reward, reward_weights, weighted_scores
 
 
 class RewardCriterion(nn.Module):
@@ -86,8 +86,9 @@ class LabelSmoothing(nn.Module):
 
 
 class StructureLosses(nn.Module):
-    """losses.py:38-200 for ``structure_loss_type='new_self_critical'``: every sample is rewarded with its CIDEr-D minus the mean CIDEr-D
-    of the image's other samples.  Scores come from the device kernel (rewards.get_scores)."""
+    """losses.py:38-200 for ``structure_loss_type='new_self_critical'``: every sample is rewarded with its score (cider_reward_weight *
+    CIDEr-D + bleu_reward_weight * BLEU-4) minus the mean score of the image's other samples.  Scores come from the device kernels
+    (rewards.get_scores)."""
 
     def __init__(self, opt):
         super().__init__()
@@ -102,8 +103,7 @@ class StructureLosses(nn.Module):
         if getattr(self.opt, 'entropy_reward_weight', 0) > 0 or getattr(self.opt, 'self_cider_reward_weight', 0) > 0:
             raise NotImplementedError('entropy / self-CIDEr rewards are out of scope of the engine')
         mask = _shifted_mask(seq)
-        w = float(getattr(self.opt, 'cider_reward_weight', 1))
-        scores = (cider_scores(data_gts, seq) * w).to(input).view(-1, n)
+        scores = get_scores(data_gts, seq, self.opt).to(input).view(-1, n)
         out = {'reward': scores}
         adv = scores - (scores.sum(1, keepdim=True) - scores) / (n - 1)
         picked = torch.gather(input, 2, seq.unsqueeze(2)).squeeze(2)
@@ -263,13 +263,20 @@ class B200LossWrapper(nn.Module):
         reduction = 'none' if drop_worst_flag else 'mean'
         return self.crit(self.model(fc_feats, att_feats, labels[..., :-1], att_masks), labels[..., 1:], masks[..., 1:], reduction=reduction)
 
+    def _weights(self):
+        """(cider_reward_weight, bleu_reward_weight), or None for the CIDEr-D reward of the default weights (1, 0)."""
+        w = reward_weights(self.opt)
+        return None if w == (1.0, 0.0) else w
+
     def _sampled_step(self, fc_feats, att_feats, gts, baseline, att_masks=None, drop_worst_flag=False):
         opt = self.opt
         self.model.train()
         keep = self._keep_rows(len(gts) * opt.train_sample_n, drop_worst_flag)
         # the reference's training-time _sample call passes no temperature (loss_wrapper.py:63-67): 1.0, whatever opt.temperature says
+        w = self._weights()
+        extra = {} if w is None else {'reward_weights': w}          # the default weights call the step exactly as before
         res = self.model.scst_step(fc_feats, att_feats, gts, self._scorer(), opt.train_sample_n, temperature=1.0, baseline=baseline, att_masks=att_masks,
-                                   keep_rows=keep)
+                                   keep_rows=keep, **extra)
         res['keep_rows'] = keep
         self.last_step = res
         return res
@@ -278,8 +285,7 @@ class B200LossWrapper(nn.Module):
         opt = self.opt
         out = {}
         reduction = 'none' if drop_worst_flag else 'mean'
-        plain_reward = getattr(opt, 'bleu_reward_weight', 0) == 0 and getattr(opt, 'cider_reward_weight', 1) == 1
-        can_fuse = (hasattr(self.model, 'scst_step') and torch.is_grad_enabled() and plain_reward and
+        can_fuse = (hasattr(self.model, 'scst_step') and torch.is_grad_enabled() and
                     opt.train_sample_method == 'sample' and opt.train_beam_size == 1)
         if struc_flag:
             w = opt.structure_loss_weight
@@ -288,11 +294,16 @@ class B200LossWrapper(nn.Module):
             if w > 0:
                 if getattr(opt, 'use_ppo', 0) or opt.structure_loss_type != 'new_self_critical' or not can_fuse:
                     raise NotImplementedError("the structure-loss branch covers structure_loss_type='new_self_critical' on the fused SCST steps")
+                if getattr(opt, 'entropy_reward_weight', 0) > 0 or getattr(opt, 'self_cider_reward_weight', 0) > 0:
+                    raise NotImplementedError('entropy / self-CIDEr rewards are out of scope of the engine')
                 gts = [gts[_] for _ in gt_indices.tolist()]
                 if drop_worst_flag and 0 < w < 1:
                     raise NotImplementedError('drop_worst with a mixed XE / structure loss: the two fused steps would select rows independently')
                 res = self._sampled_step(fc_feats, att_feats, gts, 'leave_one_out', att_masks, drop_worst_flag)
-                struc = {'loss': self._bridge(res), 'reward': cider_scores(gts, res['sample_seq']).float().view(-1, opt.train_sample_n)}
+                rw = self._weights()
+                # out['reward'] is the score the step rewarded, in fp32 as losses.py:61-62 casts it
+                scores = cider_scores(gts, res['sample_seq']) if rw is None else weighted_scores(gts, res['sample_seq'], rw)
+                struc = {'loss': self._bridge(res), 'reward': scores.float().view(-1, opt.train_sample_n)}
             else:
                 struc = {'loss': torch.zeros((), device=fc_feats.device), 'reward': torch.zeros((), device=fc_feats.device)}
             out['lm_loss'], out['struc_loss'], out['reward'] = lm_loss, struc['loss'], struc['reward']
@@ -314,8 +325,6 @@ class B200LossWrapper(nn.Module):
             why = []
             if not hasattr(self.model, 'scst_step'):
                 why.append('model family %r has no fused SCST step (UpDown, Att2in2, NewFC, AoANet and Transformer do)' % getattr(self.model, 'family_name', type(self.model).__name__))
-            if not plain_reward:
-                why.append('cider_reward_weight != 1 or bleu_reward_weight != 0')
             if opt.train_sample_method != 'sample' or opt.train_beam_size != 1:
                 why.append('train_sample_method / train_beam_size other than multinomial sampling')
             if opt.sc_sample_method != 'greedy' or opt.sc_beam_size != 1:

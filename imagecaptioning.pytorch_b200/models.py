@@ -531,13 +531,15 @@ class _FusedTrainSteps:
     # ---- SCST training step: greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----------------
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
-                  forced_tokens=None, att_masks=None, keep_rows=0):
+                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None):
         """Runs one self-critical step entirely on the device (capb200_updown_scst_step and its Att2in2 / NewFC counterparts).  Returns a
         dict with 'loss' (0-dim), 'reward' [N, T], 'sample_seq', 'greedy_seq', 'sample_logprobs' and 'grads' {parameter: gradient tensor}.
         ``baseline='greedy'`` is the self-critical step (loss_wrapper.py:56-73); ``'leave_one_out'`` the 'new_self_critical' structure
         loss (losses.py:168-187): no greedy decode, each sample is scored against the mean of the image's other samples, and the
-        result carries 'scores' [B, n] (the raw CIDEr-D values the reference reports as out['reward'])."""
-        from .rewards import pack_references
+        result carries 'scores' [B, n] (the raw CIDEr-D values the reference reports as out['reward']).  ``reward_weights`` = (cider, bleu)
+        scores each caption with cider * CIDEr-D + bleu * BLEU-4 (opts.py:169-172); None is CIDEr-D alone."""
+        from .rewards import pack_references, weights_struct
+        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
         lib = self._ensure_engine(fc_feats.device)
         fc, att, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
         dev = fc.device
@@ -563,7 +565,7 @@ class _FusedTrainSteps:
             assert forced.shape == (N, T)
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None      # drop_worst: per-row losses (reduction 'none')
         so = _lib.ScstOpts(sample_n, float(temperature), seed, float(p), float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY,
-                           _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss))
+                           _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), None if rw is None else ctypes.pointer(rw))
         _lib.check(getattr(lib, self._scst_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs),
                                                   _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq), _lib.ptr(greedy_seq), _lib.ptr(logprobs),
                                                   _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), self._scst_entry[len('capb200_'):])
@@ -980,11 +982,12 @@ class B200TransformerModel(B200CaptionModel):
 
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy', dropout=None,
-                  forced_tokens=None, att_masks=None, keep_rows=0):
+                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None):
         """One self-critical step of the Transformer on the device (capb200_tfm_scst_step): eval-mode greedy baseline (or leave-one-out),
-        train-mode samples drawn position by position on the K/V tape, CIDEr-D reward, RewardCriterion, batched backward.  Result as
-        B200UpDownModel.scst_step."""
-        from .rewards import pack_references
+        train-mode samples drawn position by position on the K/V tape, CIDEr-D (or weighted, ``reward_weights``) reward, RewardCriterion,
+        batched backward.  Result as B200UpDownModel.scst_step."""
+        from .rewards import pack_references, weights_struct
+        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
         lib = self._ensure_engine(att_feats.device)
         att, masks = self._clip(att_feats, att_masks)
         dev = att.device
@@ -1009,7 +1012,7 @@ class B200TransformerModel(B200CaptionModel):
             assert forced.shape == (N, T)
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
         so = _lib.TfmScstOpts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, float(p_lm),
-                              float(p), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss))
+                              float(p), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), None if rw is None else ctypes.pointer(rw))
         _lib.check(lib.capb200_tfm_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs), _lib.ptr(offsets), L,
                                              ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq), _lib.ptr(logprobs),
                                              _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'tfm_scst_step')
@@ -1122,11 +1125,13 @@ class B200AoAModel(B200CaptionModel):
 
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
-                  drop_attn=0.1, drop_aoa=None, drop_sublayer=0.1, ctx_drop=None, forced_tokens=None, att_masks=None, keep_rows=0):
+                  drop_attn=0.1, drop_aoa=None, drop_sublayer=0.1, ctx_drop=None, forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None):
         """One self-critical step of AoANet on the device (capb200_aoa_scst_step): eval-mode greedy baseline (or the leave-one-out baseline of
         'new_self_critical'), train-mode samples with every dropout site of AoAModel.py active, CIDEr-D reward, RewardCriterion, BPTT through
-        the decoder and the six refiner layers.  ``fc_feats`` is unused (mean_feats=1).  Returns the dict of B200UpDownModel.scst_step."""
-        from .rewards import pack_references
+        the decoder and the six refiner layers.  ``fc_feats`` is unused (mean_feats=1).  ``reward_weights`` as in B200UpDownModel.scst_step.
+        Returns the dict of B200UpDownModel.scst_step."""
+        from .rewards import pack_references, weights_struct
+        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
         lib = self._ensure_engine(att_feats.device)
         att, masks = self._clip(att_feats, att_masks)
         dev = att.device
@@ -1152,7 +1157,8 @@ class B200AoAModel(B200CaptionModel):
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
         so = _lib.AoaScstOpts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, float(p),
                               float(drop_attn), float(self.dropout_aoa if drop_aoa is None else drop_aoa), float(drop_sublayer),
-                              int(self.ctx_drop if ctx_drop is None else ctx_drop), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss))
+                              int(self.ctx_drop if ctx_drop is None else ctx_drop), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss),
+                              None if rw is None else ctypes.pointer(rw))
         _lib.check(lib.capb200_aoa_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs), _lib.ptr(offsets), L,
                                              ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq), _lib.ptr(logprobs),
                                              _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'aoa_scst_step')

@@ -1,4 +1,4 @@
-"""Device-side mirror of captioning/utils/rewards.py for the SCST inner loop (CIDEr-D reward only).
+"""Device-side mirror of captioning/utils/rewards.py for the SCST inner loop.
 
     init_scorer(cached_tokens)                                   rewards.py:25-31
     get_self_critical_reward(greedy_res, data_gts, gen_result, opt)   rewards.py:41-81
@@ -7,10 +7,14 @@
 The reference moves both id tensors to the host, formats every id as a string and walks Python dicts; here the ids
 never leave the GPU: n-gram extraction, the document-frequency lookup (open-addressing hash table built once from the
 ``scripts/prepro_ngrams.py`` pickle), the clipped tf-idf cosine and the self-critical difference run in csrc/reward.cu.
-``bleu_reward_weight`` must be 0 (its default, opts.py:171).
+
+The reward is ``cider_reward_weight * CIDEr-D + bleu_reward_weight * BLEU-4`` (opts.py:169-172), a term computed only when its weight is
+> 0.  The BLEU-4 term is the per-sentence BLEU-4 of coco-caption's Bleu(4) scorer (closest reference length), also computed on the device.
+With ``bleu_reward_weight <= 0`` the functions below take the CIDEr-D-only path they always took.
 """
 from __future__ import annotations
 
+import ctypes
 import os
 import pickle
 import threading
@@ -180,12 +184,86 @@ def cider_scores_and_reward(greedy_res: torch.Tensor, data_gts: Sequence, gen_re
     return scores, reward
 
 
+def reward_weights(opt) -> Tuple[float, float]:
+    """(cider_reward_weight, bleu_reward_weight) of a training opt, with the reference's defaults (opts.py:169-172)."""
+    return float(getattr(opt, 'cider_reward_weight', 1)), float(getattr(opt, 'bleu_reward_weight', 0))
+
+
+def weights_struct(weights, data_gts: Sequence) -> Optional[_lib.RewardWeights]:
+    """capb200_reward_weights for (cider, bleu) weights, or None (the CIDEr-D reward) for None.  With the BLEU term on, every image needs
+    at least one reference (the reference asserts it, bleu.py): refused here, before any device work."""
+    if weights is None:
+        return None
+    wc, wb = (float(w) for w in weights)
+    if not (np.isfinite(wc) and np.isfinite(wb)):
+        raise ValueError('reward weights must be finite')
+    if wb > 0 and any(int(np.asarray(g).shape[0]) == 0 for g in data_gts):
+        raise ValueError('the BLEU-4 reward needs at least one reference per image')
+    return _lib.RewardWeights(wc, wb)
+
+
+def _check_scorer(table, weights):
+    table = table or CiderD_scorer
+    if table is None and float(weights[0]) > 0:
+        raise RuntimeError('init_scorer(cached_tokens) must be called before the SCST reward (tools/train.py:150-152)')
+    return table
+
+
+def weighted_scores(data_gts: Sequence, gen_result: torch.Tensor, weights, greedy_res: Optional[torch.Tensor] = None,
+                    table: Optional[CiderDTable] = None, with_reward: bool = False):
+    """``weights[0] * CIDEr-D + weights[1] * BLEU-4`` of every sampled caption -- and, with ``greedy_res``, of every greedy caption after
+    them -- as float64 [S (+B)] (capb200_weighted_reward).  with_reward: also the fp32 reward [S, T], the self-critical difference with
+    ``greedy_res``, else the leave-one-out reward of 'new_self_critical'."""
+    w = weights_struct(weights, data_gts)
+    table = _check_scorer(table, weights)
+    dev = gen_result.device
+    if dev.type != 'cuda':
+        raise RuntimeError('capb200: the reward kernel runs on CUDA tensors only')
+    B = len(data_gts)
+    S, T = gen_result.shape
+    assert S % B == 0 and (greedy_res is None or greedy_res.shape[0] == B)
+    sampled = gen_result.detach().to(torch.long).contiguous()
+    greedy = None if greedy_res is None else greedy_res.detach().to(torch.long).contiguous()
+    refs, offsets, L = pack_references(data_gts, dev)
+    hyps = S + (0 if greedy is None else B)
+    scores = torch.empty(hyps, dtype=torch.float64, device=dev)
+    bleu = torch.empty(hyps, dtype=torch.float64, device=dev)
+    reward = torch.empty(S, T, dtype=torch.float32, device=dev) if with_reward else None
+    lib = _lib.load()
+    _lib.check(lib.capb200_weighted_reward(table._h if table is not None else None, ctypes.byref(w), _lib.ptr(sampled), S, _lib.ptr(greedy), B, T,
+                                           _lib.ptr(refs), _lib.ptr(offsets), L, _lib.ptr(scores), _lib.ptr(bleu), _lib.ptr(reward),
+                                           _lib.current_stream()), 'weighted_reward')
+    return (scores, reward) if with_reward else scores
+
+
+def bleu_scores(data_gts: Sequence, gen_result: torch.Tensor, greedy_res: Optional[torch.Tensor] = None):
+    """Per-sentence BLEU-4 (Bleu(4).compute_score(...)[1][3], closest reference length) of every sampled caption against its image's
+    references -- and, with ``greedy_res``, of every greedy caption after them: float64 [S (+B)] on the device (capb200_bleu4_scores)."""
+    weights_struct((0.0, 1.0), data_gts)
+    dev = gen_result.device
+    if dev.type != 'cuda':
+        raise RuntimeError('capb200: the reward kernel runs on CUDA tensors only')
+    B = len(data_gts)
+    S, T = gen_result.shape
+    assert S % B == 0 and (greedy_res is None or greedy_res.shape[0] == B)
+    sampled = gen_result.detach().to(torch.long).contiguous()
+    greedy = None if greedy_res is None else greedy_res.detach().to(torch.long).contiguous()
+    refs, offsets, L = pack_references(data_gts, dev)
+    scores = torch.empty(S + (0 if greedy is None else B), dtype=torch.float64, device=dev)
+    _lib.check(_lib.load().capb200_bleu4_scores(_lib.ptr(sampled), S, _lib.ptr(greedy), B, T, _lib.ptr(refs), _lib.ptr(offsets), L, _lib.ptr(scores),
+                                                _lib.current_stream()), 'bleu4_scores')
+    return scores
+
+
 def get_self_critical_reward(greedy_res, data_gts, gen_result, opt):
-    """reward[i*n+j, :] = CIDEr-D(sample j of image i) - CIDEr-D(greedy of image i), as a device fp32 tensor [S, T]
-    (the reference returns the same values as a host float64 array that LossWrapper immediately moves back to the GPU)."""
-    if getattr(opt, 'bleu_reward_weight', 0) > 0:
-        raise NotImplementedError('BLEU reward is out of scope of the engine (bleu_reward_weight defaults to 0)')
-    w = float(getattr(opt, 'cider_reward_weight', 1))
+    """reward[i*n+j, :] = score(sample j of image i) - score(greedy of image i), score = cider_reward_weight * CIDEr-D + bleu_reward_weight
+    * BLEU-4, as a device fp32 tensor [S, T] (the reference returns the same values as a host float64 array that LossWrapper immediately
+    moves back to the GPU)."""
+    wc, wb = reward_weights(opt)
+    if wb > 0:
+        _, reward = weighted_scores(data_gts, gen_result, (wc, wb), greedy_res=greedy_res, with_reward=True)
+        return reward
+    w = wc
     _, reward = cider_scores_and_reward(greedy_res, data_gts, gen_result)
     return reward if w == 1.0 else reward * w
 
@@ -212,10 +290,11 @@ def cider_scores(data_gts: Sequence, gen_result: torch.Tensor, table: Optional[C
 
 
 def get_scores(data_gts, gen_result, opt):
-    """rewards.py:83-114 with the CIDEr-D term only: ``cider_reward_weight * CIDEr-D`` per sampled caption, float64 [S] on the device
+    """rewards.py:83-114: ``cider_reward_weight * CIDEr-D + bleu_reward_weight * BLEU-4`` per sampled caption, float64 [S] on the device
     (the reference returns the same values as a host numpy array)."""
-    if getattr(opt, 'bleu_reward_weight', 0) > 0:
-        raise NotImplementedError('BLEU reward is out of scope of the engine (bleu_reward_weight defaults to 0)')
-    w = float(getattr(opt, 'cider_reward_weight', 1))
+    wc, wb = reward_weights(opt)
+    if wb > 0:
+        return weighted_scores(data_gts, gen_result, (wc, wb))
+    w = wc
     scores = cider_scores(data_gts, gen_result)
     return scores if w == 1.0 else scores * w

@@ -299,6 +299,29 @@ int capb200_self_critical_reward(const capb200_cider_table* t, const long long* 
 int capb200_cider_scores(const capb200_cider_table* t, const long long* sampled, int S, int B, int T, const int* refs, const int* ref_offsets,
                          int L, double* scores, float* reward, void* stream);
 
+/* Weights of the two reward terms (opts.py:169-172): score = cider * CIDEr-D + bleu * BLEU-4 (rewards.py:63-74, :100-112).  A term is
+ * computed only when its weight is > 0; otherwise it contributes weight * 0.  A NULL pointer to this struct means {1, 0}, the CIDEr-D reward. */
+typedef struct {
+    double cider;
+    double bleu;
+} capb200_reward_weights;
+
+/* BLEU-4 of every hypothesis against its image's references: the per-sentence bleu_list[3] of Bleu(4).compute_score (closest reference
+ * length, coco-caption/pycocoevalcap/bleu/bleu_scorer.py), float64.  Hypotheses sampled[S,T] (image i / (S/B)) and, if greedy[B,T] is not
+ * NULL, greedy rows S..S+B-1; refs / ref_offsets / L as in capb200_self_critical_reward.  scores[S (+B)].  An image without references
+ * scores 0 (the reference asserts that every image has one). */
+int capb200_bleu4_scores(const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs, const int* ref_offsets, int L,
+                         double* scores, void* stream);
+
+/* get_self_critical_reward (greedy != NULL) and get_scores (greedy == NULL) with both reward terms.  scores[S (+B)] float64: the weighted
+ * score of every hypothesis.  bleu_scores[S (+B)] float64: BLEU-4 of every hypothesis (required when w->bleu > 0, else ignored).  t may be
+ * NULL when w->cider <= 0.  reward (optional, [S,T] fp32): score(sample) - score(greedy of its image) in float64 then cast, or -- without
+ * greedy -- the leave-one-out reward of capb200_cider_scores over the fp32-cast scores.  With w = NULL or {1, 0} the result equals
+ * capb200_self_critical_reward / capb200_cider_scores. */
+int capb200_weighted_reward(const capb200_cider_table* t, const capb200_reward_weights* w, const long long* sampled, int S, const long long* greedy,
+                            int B, int T, const int* refs, const int* ref_offsets, int L, double* scores, double* bleu_scores, float* reward,
+                            void* stream);
+
 /* RewardCriterion.forward (captioning/modules/losses.py:22-37). logprobs[N,T,V1]; seq[N,T] int64; reward[N,T].
  * loss_mean[1], loss_rows[N] (reduction 'none'), mask_sum[1]; any output may be NULL. */
 int capb200_reward_criterion_forward(const float* logprobs, const long long* seq, const float* reward, int N, int T, int V1, float* loss_mean,
@@ -310,7 +333,8 @@ int capb200_reward_criterion_backward(const long long* seq, const float* reward,
 /* ------------------------------------------------------------------------------------------------------------------
  * One self-critical training step of the UpDown model (LossWrapper.forward with sc_flag, loss_wrapper.py:56-73, plus the
  * loss.backward() of tools/train.py:189): eval-mode greedy baseline, train-mode multinomial samples (dropout on, AttModel.py:74-88,
- * :637), CIDEr-D self-critical reward, RewardCriterion, then back-propagation through time into every parameter gradient.
+ * :637), self-critical reward (CIDEr-D, or weighted CIDEr-D + BLEU-4 with opts->reward_weights), RewardCriterion, then back-propagation
+ * through time into every parameter gradient.
  * ---------------------------------------------------------------------------------------------------------------- */
 typedef struct {
     int sample_n;              /* opt.train_sample_n */
@@ -327,6 +351,8 @@ typedef struct {
     int keep_rows;             /* drop_worst (tools/train.py:187-191): 0 = reduction 'mean'; k > 0 = the criterion runs with reduction 'none' (one loss per
                                   caption row) and the k rows with the smallest loss are averaged: loss[0] = that mean, gradients accordingly */
     float* row_loss;           /* optional [rows] output of the per-row losses (what LossWrapper returns as out['loss'] under drop_worst_flag) */
+    const capb200_reward_weights* reward_weights; /* optional, read during the call: the reward is cider * CIDEr-D + bleu * BLEU-4 as
+                                  capb200_weighted_reward computes it; NULL = CIDEr-D only (weight 1) */
 } capb200_scst_opts;
 #define CAPB200_BASELINE_GREEDY 0
 #define CAPB200_BASELINE_LEAVE_ONE_OUT 1
@@ -438,6 +464,7 @@ typedef struct {
     int keep_rows;             /* drop_worst (tools/train.py:187-191): 0 = reduction 'mean'; k > 0 = the criterion runs with reduction 'none' (one loss per
                                   caption row) and the k rows with the smallest loss are averaged: loss[0] = that mean, gradients accordingly */
     float* row_loss;           /* optional [rows] output of the per-row losses (what LossWrapper returns as out['loss'] under drop_worst_flag) */
+    const capb200_reward_weights* reward_weights; /* optional reward weights, see capb200_scst_opts; NULL = CIDEr-D only */
 } capb200_aoa_scst_opts;
 /* Gradient buffers, laid out field by field like the weights struct above: parameter shapes, fp32, device; every one is OVERWRITTEN. */
 typedef struct {
@@ -550,6 +577,7 @@ typedef struct {
     const float* att_masks;
     int keep_rows;
     float* row_loss;
+    const capb200_reward_weights* reward_weights;   /* optional reward weights, see capb200_scst_opts; NULL = CIDEr-D only */
 } capb200_tfm_scst_opts;
 int capb200_tfm_xe_step(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_xe_opts* opts, const long long* labels, const float* masks,
                         int label_cols, const capb200_tfm_grads* grads, float* logprobs, float* loss, void* stream);
