@@ -1007,6 +1007,8 @@ int capb200_gemm_trace(const float* x, const float* w, float* y, int M, int N, i
     return rc;
 }
 
+int capb200_gemm_tile_n(int M, int N) { return gemm_tc_tile_n(M, N); }
+
 int capb200_lstm_cell(const float* x, int Kx, const float* h, const float* c, const float* w_ih, const float* w_hh, const float* b_ih,
                       const float* b_hh, float* h_out, float* c_out, int M, int H, int mode, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);

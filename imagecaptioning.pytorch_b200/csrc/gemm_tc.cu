@@ -9,7 +9,7 @@
 // one fp32 register accumulator:  hi*lo + lo*hi + hi*hi  (the lo*lo term, <= 2^-22 relative, is dropped).
 // PASSES == 1 is the throughput mode (hi plane only) and is never used for parity claims.
 //
-// Structure (persistent: one 128 x BN output tile at a time per CTA, 384 threads = three warpgroups):
+// Structure (persistent: one 128 x BN output tile at a time per CTA, BN = 64, 128 or 160 chosen by the plan, 384 threads = three warpgroups):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2-D boxes [64 k x rows] (128B swizzle) for A_hi, A_lo, W_hi,
 //                   W_lo of the current K-block into a STAGES-deep shared-memory ring, mbarrier complete_tx signalling.  It runs ahead
 //                   into the next tile while the consumers are in their epilogue.
@@ -83,9 +83,10 @@ struct TcCfg {
     static constexpr uint32_t kABytes = BM * BK * 2;
     static constexpr uint32_t kWBytes = BN * BK * 2;
     static constexpr uint32_t kStageBytes = kPlanes * (kABytes + kWBytes);
-    static constexpr int kStages = (200 * 1024) / kStageBytes >= 8 ? 8 : (200 * 1024) / kStageBytes;
+    static constexpr uint32_t kRingBudget = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/;   // per-block shared-memory limit
+    static constexpr int kStages = kRingBudget / kStageBytes >= 8 ? 8 : kRingBudget / kStageBytes;
     static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-    static_assert(BN == 64 || BN == 128, "wgmma wrappers exist for N = 64 and 128");
+    static_assert(BN == 64 || BN == 128 || BN == 160, "wgmma wrappers exist for N = 64, 128 and 160");
     static_assert(kWBytes % 1024 == 0, "operand tiles must keep the 1024-byte swizzle-atom alignment");
     static_assert(kStages >= 2, "need at least a double buffer");
     static_assert(kSmemBytes <= 227 * 1024, "shared memory of one H100 block");
@@ -93,7 +94,8 @@ struct TcCfg {
 
 template <int BN>
 __device__ __forceinline__ void wgmma_f16(float* acc, uint64_t da, uint64_t db, int scale_d) {
-    if (BN == 128) ptx::wgmma_f16_n128(acc, da, db, scale_d);
+    if (BN == 160) ptx::wgmma_f16_n160(acc, da, db, scale_d);
+    else if (BN == 128) ptx::wgmma_f16_n128(acc, da, db, scale_d);
     else ptx::wgmma_f16_n64(acc, da, db, scale_d);
 }
 
@@ -381,6 +383,18 @@ bool gemm_tc_supported(const GemmProblem& p, std::string* why) {
     return true;
 }
 
+// Tile width.  Problems with fewer 128-wide tiles than half the SMs are latency-bound: 64-wide tiles double the CTAs.  Otherwise the
+// width of 128 or 160 with the fewest waves x BN, ties to 128 (at equal column-waves the 160-wide tile only adds epilogue work; measured
+// on an H100 80GB HBM3 with tools/decode_gemm_rate.py, 160 pays for the 1280 x 4000 LSTM gates: 2 waves instead of 3 on 132 SMs).
+int gemm_tc_tile_n(int M, int N) {
+    const int sms = sm_count();
+    const int tiles_m = cdiv(M, BM);
+    if (tiles_m * cdiv(N, 128) < sms / 2 && N > 64) return 64;
+    const long cost128 = (long)cdiv(tiles_m * cdiv(N, 128), sms) * 128;
+    const long cost160 = (long)cdiv(tiles_m * cdiv(N, 160), sms) * 160;
+    return cost160 < cost128 ? 160 : 128;
+}
+
 GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes) {
     std::string why;
     if (!gemm_tc_supported(p, &why)) { set_error("gemm_tc: unsupported problem: " + why); return nullptr; }
@@ -388,8 +402,7 @@ GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes) {
     GemmTcPlan* plan = new GemmTcPlan();
     memset(&plan->prm, 0, sizeof(TcParams));
     plan->passes = passes;
-    // problems with fewer 128-wide tiles than half the SMs are latency-bound: halve the tile width to double the CTAs
-    plan->bn = (cdiv(p.M, BM) * cdiv(p.N, 128) < sm_count() / 2 && p.N > 64) ? 64 : 128;
+    plan->bn = gemm_tc_tile_n(p.M, p.N);
     TcParams& t = plan->prm;
     t.nseg = p.nseg;
     t.M = p.M;
@@ -427,8 +440,10 @@ int gemm_tc_plan_launch(GemmTcPlan* plan, const GemmEpilogue* epi_override, int 
     if (prm.M <= 0 || prm.N <= 0) return 0;
     if (prm.trace != nullptr) {                                  // capb200_gemm_trace only
         if (plan->passes != 3) { set_error("gemm_tc: the traced kernel is the 3-pass one"); return 1; }
+        if (plan->bn == 160) return launch_cfg<160, 3, true>(prm, stream);
         return plan->bn == 128 ? launch_cfg<128, 3, true>(prm, stream) : launch_cfg<64, 3, true>(prm, stream);
     }
+    if (plan->bn == 160) return plan->passes == 3 ? launch_cfg<160, 3>(prm, stream) : launch_cfg<160, 1>(prm, stream);
     if (plan->bn == 128) return plan->passes == 3 ? launch_cfg<128, 3>(prm, stream) : launch_cfg<128, 1>(prm, stream);
     return plan->passes == 3 ? launch_cfg<64, 3>(prm, stream) : launch_cfg<64, 1>(prm, stream);
 }

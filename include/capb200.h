@@ -61,10 +61,13 @@ int capb200_linear(const float* x, long ldx, const float* w, long ldw, const flo
 int capb200_bench_linear(const float* x, const float* w, const float* b, float* y, int M, int N, int K, int mode, int iters, float* ms_per_launch,
                          void* stream);
 
-/* Diagnostics: one traced launch of the decode GEMM y[M,N] = x[M,K] w[N,K]^T (tc_f16x3, CTA-pair kernel).  trace_host receives 296 x 16
- * %globaltimer stamps (ns), one row per CTA: 0 set-up done, 1 first operands landed, 2/3 all MMAs of the CTA pair's first / second tile
- * issued, 4/5 accumulator of tile 0 / 1 complete (epilogue starts), 6/7 epilogue of tile 0 / 1 done, 8 kernel end (tools/gemm_trace.py). */
+/* Diagnostics: one traced launch of the decode GEMM y[M,N] = x[M,K] w[N,K]^T (tc_f16x3, persistent kernel, one CTA per SM at most).
+ * trace_host receives 296 x 16 %globaltimer stamps (ns), one row per CTA: 0 set-up done, 1 first operands landed, 2/3 main loop of the
+ * CTA's first / second tile done (accumulator complete), 6/7 epilogue of tile 0 / 1 done, 8 kernel end; 4/5 are unused (tools/gemm_trace.py). */
 int capb200_gemm_trace(const float* x, const float* w, float* y, int M, int N, int K, unsigned long long* trace_host, int n_slots, void* stream);
+
+/* Diagnostics: the output-tile width (64, 128 or 160 columns) the tc_f16x3 / tc_f16x1 GEMM picks for an M x N problem on the current device. */
+int capb200_gemm_tile_n(int M, int N);
 
 /* nn.LSTMCell: gates = x*w_ih^T + b_ih + h*w_hh^T + b_hh; (i,f,g,o)           AttModel.py:628,635
  * x[M,Kx], h/c[M,H] -> h_out/c_out[M,H] */
