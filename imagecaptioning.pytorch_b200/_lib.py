@@ -174,6 +174,14 @@ class AoaWeights(Structure):
                                         'logit_b')]
 
 
+class GemmEpilogue(Structure):
+    _fields_ = [('bias', c_void_p), ('row_bias', c_void_p), ('ld_row_bias', c_long), ('rows_per_group', c_int), ('residual', c_void_p),
+                ('ld_res', c_long), ('relu', c_int), ('C', c_void_p), ('ldc', c_long), ('C_hi', c_void_p), ('C_lo', c_void_p), ('ldcs', c_long),
+                ('lstm', c_int), ('H', c_int), ('c_prev', c_void_p), ('ld_cprev', c_long), ('src_row', c_void_p), ('c_out', c_void_p),
+                ('ld_cout', c_long), ('gather_bias', c_void_p), ('ld_gb', c_long), ('gather_idx', c_void_p), ('h_f', c_void_p), ('h_hi', c_void_p),
+                ('h_lo', c_void_p), ('ld_h', c_long)]
+
+
 # every exported symbol of include/capb200.h: (restype, argtypes)
 SIGNATURES = {
     'capb200_last_error': (c_char_p, []),
@@ -181,7 +189,6 @@ SIGNATURES = {
     'capb200_range_status': (c_int, [c_int]),
     'capb200_linear': (c_int, [c_void_p, c_long, c_void_p, c_long, c_void_p, c_void_p, c_long, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'capb200_bench_linear': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    'capb200_gemm_trace': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     'capb200_gemm_tile_n': (c_int, [c_int, c_int]),
     'capb200_lstm_cell': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                   c_int, c_void_p]),
@@ -257,6 +264,7 @@ SIGNATURES = {
                                              c_void_p]),
     'capb200_reward_criterion_forward': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'capb200_reward_criterion_backward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_void_p]),
+    'capb200_decode_gemm': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(GemmEpilogue), c_void_p, c_int, c_void_p]),
 }
 
 _lib = None

@@ -972,38 +972,56 @@ int capb200_bench_linear(const float* x, const float* w, const float* b, float* 
     return rc;
 }
 
-int capb200_gemm_trace(const float* x, const float* w, float* y, int M, int N, int K, unsigned long long* trace_host, int n_slots, void* stream) {
-    // one traced launch of the decode GEMM (3-pass wgmma) after three warm launches: trace_host[296][16] %globaltimer stamps
+int capb200_decode_gemm(const float* x, const float* w, int M, int N, int K, int mode, const capb200_gemm_epilogue* epi, unsigned long long* trace_host,
+                        int n_slots, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(x && w && y && trace_host && n_slots >= 296 * 16, "bad argument");
+    CAPB_REQUIRE(x && w && epi && M > 0 && N > 0 && K > 0, "bad argument");
+    CAPB_REQUIRE(mode == CAPB200_MODE_TC_F16X3 || mode == CAPB200_MODE_TC_F16X1, "the decode GEMM runs in the tc_f16x3 / tc_f16x1 modes");
+    CAPB_REQUIRE(trace_host == nullptr || (n_slots >= 296 * 16 && mode == CAPB200_MODE_TC_F16X3), "the trace needs 296 x 16 slots and tc_f16x3");
     GemmProblem g;
     g.M = M; g.N = N; g.nseg = 1;
-    g.seg[0].A = x; g.seg[0].lda = K; g.seg[0].W = w; g.seg[0].ldw = K; g.seg[0].K = K;
-    g.epi.C = y; g.epi.ldc = N;
+    g.seg[0].K = K;
+    GemmEpilogue& e = g.epi;
+    e.bias = epi->bias; e.row_bias = epi->row_bias; e.ld_row_bias = epi->ld_row_bias; e.rows_per_group = epi->rows_per_group;
+    e.residual = epi->residual; e.ld_res = epi->ld_res; e.relu = epi->relu;
+    e.C = epi->C; e.ldc = epi->ldc;
+    e.C_hi = reinterpret_cast<__half*>(epi->C_hi); e.C_lo = reinterpret_cast<__half*>(epi->C_lo); e.ldcs = epi->ldcs;
+    e.lstm = epi->lstm; e.H = epi->H;
+    e.c_prev = epi->c_prev; e.ld_cprev = epi->ld_cprev; e.src_row = epi->src_row;
+    e.c_out = epi->c_out; e.ld_cout = epi->ld_cout;
+    e.gather_bias = epi->gather_bias; e.ld_gb = epi->ld_gb; e.gather_idx = epi->gather_idx;
+    e.h_f = epi->h_f; e.h_hi = reinterpret_cast<__half*>(epi->h_hi); e.h_lo = reinterpret_cast<__half*>(epi->h_lo); e.ld_h = epi->ld_h;
+    CAPB_REQUIRE(e.C_hi == nullptr || e.C_lo != nullptr, "C_hi needs C_lo");
+    CAPB_REQUIRE(e.h_hi == nullptr || e.h_lo != nullptr, "h_hi needs h_lo");
+    CAPB_REQUIRE(e.row_bias == nullptr || e.rows_per_group >= 1, "rows_per_group must be >= 1");
+    CAPB_REQUIRE(e.gather_bias == nullptr || e.gather_idx != nullptr, "gather_bias needs gather_idx");
     const long ldh = round_up(K, 64);
     __half* scratch = nullptr;
     unsigned long long* trace = nullptr;
     CAPB_CHECK_CUDA(cudaMalloc(&scratch, (size_t)(M + N) * ldh * 2 * sizeof(__half)));
-    CAPB_CHECK_CUDA(cudaMalloc(&trace, sizeof(unsigned long long) * 296 * 16));
-    CAPB_CHECK_CUDA(cudaMemsetAsync(trace, 0, sizeof(unsigned long long) * 296 * 16, st));
+    if (trace_host != nullptr) {
+        CAPB_CHECK_CUDA(cudaMalloc(&trace, sizeof(unsigned long long) * 296 * 16));
+        CAPB_CHECK_CUDA(cudaMemsetAsync(trace, 0, sizeof(unsigned long long) * 296 * 16, st));
+    }
     __half* xh = scratch; __half* xl = xh + (size_t)M * ldh;
     __half* wh = xl + (size_t)M * ldh; __half* wl = wh + (size_t)N * ldh;
     int rc = split_planes_launch(x, K, M, K, xh, xl, ldh, st) | split_planes_launch(w, K, N, K, wh, wl, ldh, st);
     g.seg[0].A_hi = xh; g.seg[0].A_lo = xl; g.seg[0].lda_h = ldh;
     g.seg[0].W_hi = wh; g.seg[0].W_lo = wl; g.seg[0].ldw_h = ldh;
-    GemmTcPlan* plan = rc ? nullptr : gemm_tc_plan_create(g, 3);
+    GemmTcPlan* plan = rc ? nullptr : gemm_tc_plan_create(g, mode == CAPB200_MODE_TC_F16X3 ? 3 : 1);
     if (plan == nullptr) rc = 1;
-    for (int i = 0; i < 3 && !rc; ++i) rc = gemm_tc_plan_launch(plan, nullptr, 0, st);
-    if (!rc) {
+    // traced: three warm launches first, so the stamps show the steady state (outputs must not overlap inputs)
+    for (int i = 0; i < (trace ? 3 : 1) && !rc; ++i) rc = gemm_tc_plan_launch(plan, nullptr, 0, st);
+    if (!rc && trace) {
         GemmEpilogue ep = g.epi;
         ep.trace = trace;
         rc = gemm_tc_plan_launch(plan, &ep, 0, st);
     }
-    if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { set_error("gemm_trace: kernel failed"); rc = 1; }
-    if (!rc) CAPB_CHECK_CUDA(cudaMemcpy(trace_host, trace, sizeof(unsigned long long) * 296 * 16, cudaMemcpyDeviceToHost));
+    if (cudaStreamSynchronize(st) != cudaSuccess) { set_error(std::string("decode_gemm: ") + cudaGetErrorString(cudaGetLastError())); rc = 1; }
+    if (!rc && trace) CAPB_CHECK_CUDA(cudaMemcpy(trace_host, trace, sizeof(unsigned long long) * 296 * 16, cudaMemcpyDeviceToHost));
     if (plan) gemm_tc_plan_destroy(plan);
     cudaFree(scratch);
-    cudaFree(trace);
+    if (trace) cudaFree(trace);
     return rc;
 }
 

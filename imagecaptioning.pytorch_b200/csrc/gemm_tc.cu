@@ -15,7 +15,8 @@
 //                   into the next tile while the consumers are in their epilogue.
 //   warpgroups 1,2  consumers: each owns 64 rows of the tile, issues wgmma.m64nBNk16 straight from shared-memory descriptors, releases
 //                   the ring slot once its wgmmas retired, and runs the fused epilogue (bias / row-bias / ReLU, fp32 store, optional
-//                   split-fp16 copy for the next GEMM, or the fused LSTM cell) from the register accumulator.
+//                   split-fp16 copy for the next GEMM, or the fused LSTM cell) from the register accumulator.  The epilogue kind is a
+//                   template parameter (EpiKind), so each kernel carries the code of one kind only.
 // K-segments (up to 3 activation/weight pairs) are walked back to back so concatenated LSTM inputs are never built.
 #include <cstdlib>
 
@@ -99,98 +100,174 @@ __device__ __forceinline__ void wgmma_f16(float* acc, uint64_t da, uint64_t db, 
     else ptx::wgmma_f16_n64(acc, da, db, scale_d);
 }
 
-// Bias / row bias / gathered bias / residual / ReLU of one accumulator element (row < M, col < N checked by the caller).
-__device__ __forceinline__ float epi_add(const TcParams& p, const float* rb, const float* gb, int row, int col, float x) {
-    if (p.bias != nullptr) x += __ldg(p.bias + col);
-    if (rb != nullptr) x += __ldg(rb + col);
-    if (gb != nullptr) x += __ldg(gb + col);
-    if (p.residual != nullptr) x += p.residual[(long)row * p.ld_res + col];
-    if (p.relu) x = fmaxf(x, 0.0f);
-    return x;
-}
+// Epilogue kinds.  Each is its own kernel instantiation: one epilogue that inlined every variant unrolled to 70-170 KB of machine
+// code per kernel, more than an SM's instruction cache holds, and every CTA fetched it from L2 at the same moment (DESIGN §6.1).
+enum EpiKind : int {
+    kEpiStore = 0,    // fp32 C
+    kEpiPlanes = 1,   // optional fp32 C + split fp16 planes C_hi / C_lo
+    kEpiLstm = 2,     // fused nn.LSTMCell: c_out, h_f, optional h_hi / h_lo
+};
 
-// Drains this warpgroup's 64 x BN accumulator.  Thread (w, lane) owns rows r0 = 16w + lane/4 and r0 + 8, columns 8j + 2*(lane%4) (+1).
+// Accumulator element acc[4j + e] of thread (w, lane) is row r0 + 8 * (e / 2), column c0 + 8j + e % 2, with r0 = m0 + 16w + lane/4 and
+// c0 = n0 + 2 * (lane % 4).  Every column pair starts at an even column.
+//
+// Bias, row bias, gathered bias, residual, then ReLU, each applied to the whole tile in turn: every element gets the same adds in the
+// same order as one element at a time would give it, each option is tested once per tile, and all of the tile's loads come before its
+// first store.  Elements outside [M, N) are left alone; no kind stores them.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const TcParams& p, float* acc, int m0, int n0, int tid) {
-    const int warp = tid >> 5, lane = tid & 31;
-    int rows[2];
-    rows[0] = m0 + warp * 16 + (lane >> 2);
-    rows[1] = rows[0] + 8;
-    const float* rb[2];
-    const float* gb[2];
+__device__ __forceinline__ void epi_adds(const TcParams& p, float* acc, int r0, int c0) {
+    const int ncol = p.N - c0;                                  // column c0 + k is in range iff k < ncol
+    const int lim[2] = {r0 < p.M ? ncol : 0, r0 + 8 < p.M ? ncol : 0};     // ... and on a row in range
+    if (p.bias != nullptr) {
+        const float* b = p.bias + c0;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (8 * j + e < ncol) {
+                    const float x = __ldg(b + 8 * j + e);
+                    acc[4 * j + e] += x;
+                    acc[4 * j + 2 + e] += x;
+                }
+            }
+        }
+    }
+    // row bias, gathered bias, residual: one row pointer per accumulator row, indexed by column like the bias.  One loop body serves
+    // all three (not unrolled: the code is fetched once per tile whichever options are on).
+    const float* tab[3][2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const bool ok = rows[h] < p.M;
-        rb[h] = (p.row_bias != nullptr && ok) ? p.row_bias + (long)(rows[h] / p.rows_per_group) * p.ld_row_bias : nullptr;
-        gb[h] = (p.gather_bias != nullptr && ok) ? p.gather_bias + (long)p.gather_idx[rows[h]] * p.ld_gb : nullptr;
+        const int row = lim[h] > 0 ? r0 + 8 * h : 0;
+        tab[0][h] = p.row_bias != nullptr ? p.row_bias + (long)(row / p.rows_per_group) * p.ld_row_bias + c0 : nullptr;
+        tab[1][h] = p.gather_bias != nullptr ? p.gather_bias + (long)(lim[h] > 0 ? p.gather_idx[row] : 0) * p.ld_gb + c0 : nullptr;
+        tab[2][h] = p.residual != nullptr ? p.residual + (long)row * p.ld_res + c0 : nullptr;
     }
+#pragma unroll 1
+    for (int t = 0; t < 3; ++t) {
+        const float* const t0 = t == 0 ? tab[0][0] : t == 1 ? tab[1][0] : tab[2][0];
+        const float* const t1 = t == 0 ? tab[0][1] : t == 1 ? tab[1][1] : tab[2][1];
+        if (t0 == nullptr) continue;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int k = 8 * j + (e & 1);
+                if (k < lim[e >> 1]) acc[4 * j + e] += (e >> 1 ? t1 : t0)[k];
+            }
+        }
+    }
+    if (p.relu) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = fmaxf(acc[i], 0.0f);
+    }
+}
+
+// Fused LSTM cell.  Gates (i,f,g,o) of hidden unit c/4 sit in lanes 2k (i,f) and 2k+1 (g,o): the even lane finishes the unit for row r0,
+// the odd lane for row r0 + 8, each taking the two gates it lacks from its neighbour.  src_row and the c_prev values of the thread's
+// BN/8 units are loaded before the first store.
+template <int BN>
+__device__ __forceinline__ void epi_lstm(const TcParams& p, const float* acc, int r0, int c0, int lane) {
+    const bool odd = lane & 1;
+    const int row = r0 + (odd ? 8 : 0);
+    const int u0 = c0 >> 2;                                     // unit of column pair j is u0 + 2j
+    const bool row_ok = row < p.M;
+    int src = row;
+    if (p.src_row != nullptr && row_ok) src = p.src_row[row];
+    const float* cprev = (src >= 0 && p.c_prev != nullptr) ? p.c_prev + (long)src * p.ld_cprev : nullptr;
+    float cp[BN / 8];
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) cp[j] = (row_ok && cprev != nullptr && u0 + 2 * j < p.H) ? cprev[u0 + 2 * j] : 0.0f;
+    float* const c_out = p.c_out + (long)row * p.ld_cout;
+    float* const h_f = p.h_f + (long)row * p.ld_h;
+    __half* const h_hi = p.h_hi + (long)row * p.ld_h;
+    __half* const h_lo = p.h_lo + (long)row * p.ld_h;
+    const bool planes = p.h_hi != nullptr;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
-        const int col = n0 + 8 * j + 2 * (lane & 3);
-        float v[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int row = rows[e >> 1], c = col + (e & 1);
-            v[e] = (row < p.M && c < p.N) ? epi_add(p, rb[e >> 1], gb[e >> 1], row, c, acc[4 * j + e]) : 0.0f;
+        const float* v = acc + 4 * j;
+        const float s0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 1);
+        const float s1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 1);
+        const float gi = odd ? s0 : v[0], gf = odd ? s1 : v[1], gg = odd ? v[2] : s0, go = odd ? v[3] : s1;
+        const int unit = u0 + 2 * j;
+        if (row_ok && unit < p.H) {
+            const float cn = fast_sigmoid(gf) * cp[j] + fast_sigmoid(gi) * fast_tanh(gg);
+            const float hn = fast_sigmoid(go) * fast_tanh(cn);
+            c_out[unit] = cn;
+            h_f[unit] = hn;
+            if (planes) {
+                __half hh, hl;
+                split_f32(hn, hh, hl);
+                h_hi[unit] = hh;
+                h_lo[unit] = hl;
+            }
         }
-        if (p.lstm) {
-            // gates (i,f,g,o) of hidden unit col/4 sit in lanes 2k (i,f) and 2k+1 (g,o): the even lane finishes the unit for row r0,
-            // the odd lane for row r0 + 8, each taking the two gates it lacks from its neighbour
-            const bool odd = lane & 1;
-            const float s0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 1);
-            const float s1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 1);
-            const float gi = odd ? s0 : v[0], gf = odd ? s1 : v[1], gg = odd ? v[2] : s0, go = odd ? v[3] : s1;
-            const int row = rows[odd ? 1 : 0];
-            const int unit = (col & ~3) >> 2;
-            if (row < p.M && unit < p.H) {
-                int src = row;
-                if (p.src_row != nullptr) src = p.src_row[row];
-                const float cp = (src >= 0 && p.c_prev != nullptr) ? p.c_prev[(long)src * p.ld_cprev + unit] : 0.0f;
-                const float cn = fast_sigmoid(gf) * cp + fast_sigmoid(gi) * fast_tanh(gg);
-                const float hn = fast_sigmoid(go) * fast_tanh(cn);
-                p.c_out[(long)row * p.ld_cout + unit] = cn;
-                p.h_f[(long)row * p.ld_h + unit] = hn;
-                if (p.h_hi != nullptr) {
-                    __half hh, hl;
-                    split_f32(hn, hh, hl);
-                    p.h_hi[(long)row * p.ld_h + unit] = hh;
-                    p.h_lo[(long)row * p.ld_h + unit] = hl;
+    }
+}
+
+// fp32 C and / or the split planes of rows r0, r0 + 8.  Columns come in pairs starting at an even column, so whether the pairs of a row
+// can be stored as vectors depends on the row alone: a row whose pointers are aligned and whose columns are all in range takes the
+// vector loop, any other the element loop.
+template <int BN, bool PLANES>
+__device__ __forceinline__ void epi_store(const TcParams& p, const float* acc, int r0, int c0) {
+    const int ncol = p.N - c0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (row >= p.M) continue;
+        if (p.C != nullptr) {
+            float* const dst = p.C + (long)row * p.ldc + c0;
+            if (ncol >= BN && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            } else {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    if (8 * j < ncol) dst[8 * j] = acc[4 * j + 2 * h];
+                    if (8 * j + 1 < ncol) dst[8 * j + 1] = acc[4 * j + 2 * h + 1];
                 }
             }
-            continue;
         }
+        if (PLANES) {
+            __half* const dh = p.C_hi + (long)row * p.ldcs + c0;
+            __half* const dl = p.C_lo + (long)row * p.ldcs + c0;
+            if (ncol >= BN && ((reinterpret_cast<uintptr_t>(dh) | reinterpret_cast<uintptr_t>(dl)) & 3) == 0) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int row = rows[h];
-            if (row >= p.M || col >= p.N) continue;
-            const float x0 = v[2 * h], x1 = v[2 * h + 1];
-            const bool pair = col + 1 < p.N;
-            if (p.C != nullptr) {
-                float* dst = p.C + (long)row * p.ldc + col;
-                if (pair && ((reinterpret_cast<uintptr_t>(dst) & 7) == 0)) *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
-                else { dst[0] = x0; if (pair) dst[1] = x1; }
-            }
-            if (p.C_hi != nullptr) {
-                __half h0, l0, h1, l1;
-                split_f32(x0, h0, l0);
-                split_f32(x1, h1, l1);
-                __half* dh = p.C_hi + (long)row * p.ldcs + col;
-                __half* dl = p.C_lo + (long)row * p.ldcs + col;
-                if (pair && ((reinterpret_cast<uintptr_t>(dh) & 3) == 0) && ((reinterpret_cast<uintptr_t>(dl) & 3) == 0)) {
-                    *reinterpret_cast<__half2*>(dh) = __halves2half2(h0, h1);
-                    *reinterpret_cast<__half2*>(dl) = __halves2half2(l0, l1);
-                } else {
-                    dh[0] = h0; dl[0] = l0;
-                    if (pair) { dh[1] = h1; dl[1] = l1; }
+                for (int j = 0; j < BN / 8; ++j) {
+                    __half h0, l0, h1, l1;
+                    split_f32(acc[4 * j + 2 * h], h0, l0);
+                    split_f32(acc[4 * j + 2 * h + 1], h1, l1);
+                    *reinterpret_cast<__half2*>(dh + 8 * j) = __halves2half2(h0, h1);
+                    *reinterpret_cast<__half2*>(dl + 8 * j) = __halves2half2(l0, l1);
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        __half hi, lo;
+                        split_f32(acc[4 * j + 2 * h + e], hi, lo);
+                        if (8 * j + e < ncol) { dh[8 * j + e] = hi; dl[8 * j + e] = lo; }
+                    }
                 }
             }
         }
     }
+}
+
+// Drains this warpgroup's 64 x BN accumulator (layout above).
+template <int BN, int EPI>
+__device__ __forceinline__ void epilogue_tile(const TcParams& p, float* acc, int m0, int n0, int tid) {
+    const int warp = tid >> 5, lane = tid & 31;
+    const int r0 = m0 + warp * 16 + (lane >> 2);
+    const int c0 = n0 + 2 * (lane & 3);
+    epi_adds<BN>(p, acc, r0, c0);
+    if (EPI == kEpiLstm) epi_lstm<BN>(p, acc, r0, c0, lane);
+    else epi_store<BN, EPI == kEpiPlanes>(p, acc, r0, c0);
 }
 
 // Persistent schedule: gridDim.x = min(tiles, SMs); CTA b walks tiles b, b + gridDim.x, ... in m-fastest order so that concurrently
 // running CTAs share the same weight columns (the W tile comes from HBM once, then from L2).
-template <int BN, int PASSES, bool TRACE = false>
+template <int BN, int PASSES, int EPI, bool TRACE = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
     using Cfg = TcCfg<BN, PASSES>;
     extern __shared__ uint8_t smem_raw[];
@@ -289,7 +366,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 }
             }
             if (TRACE && it < 2 && tid == 0 && cw == 0) CAPB_TRACE(2 + it);          // main loop of tile `it` done
-            epilogue_tile<BN>(p, acc, m0 + cw * 64, n0, tid);
+            epilogue_tile<BN, EPI>(p, acc, m0 + cw * 64, n0, tid);
             if (TRACE && it < 2 && tid == 0 && cw == 0) CAPB_TRACE(6 + it);          // epilogue of tile `it` done
         }
     }
@@ -330,21 +407,33 @@ bool encode_plane(CUtensorMap* map, const __half* base, long rows, long K, long 
     return true;
 }
 
-template <int BN, int PASSES, bool TRACE = false>
+template <int BN, int PASSES, int EPI, bool TRACE = false>
 int launch_cfg(const TcParams& prm, cudaStream_t stream) {
     using Cfg = TcCfg<BN, PASSES>;
     static std::atomic<unsigned long long> attr_set{0};
     if (first_use_on_device(attr_set)) {
-        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, EPI, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     }
     TcParams prm2 = prm;
     prm2.tiles_n = cdiv(prm.N, BN);
     prm2.tiles_m = cdiv(prm.M, BM);
     const int n_tiles = prm2.tiles_n * prm2.tiles_m;
     const int sms = sm_count();
-    gemm_tc_kernel<BN, PASSES, TRACE><<<n_tiles < sms ? n_tiles : sms, kThreads, Cfg::kSmemBytes, stream>>>(prm2);
+    gemm_tc_kernel<BN, PASSES, EPI, TRACE><<<n_tiles < sms ? n_tiles : sms, kThreads, Cfg::kSmemBytes, stream>>>(prm2);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+// kind x BN x passes, plus the traced 3-pass kernels (capb200_decode_gemm with a trace buffer)
+template <int EPI>
+int launch_kind(int bn, int passes, const TcParams& prm, cudaStream_t stream) {
+    if (prm.trace != nullptr) {
+        if (bn == 160) return launch_cfg<160, 3, EPI, true>(prm, stream);
+        return bn == 128 ? launch_cfg<128, 3, EPI, true>(prm, stream) : launch_cfg<64, 3, EPI, true>(prm, stream);
+    }
+    if (bn == 160) return passes == 3 ? launch_cfg<160, 3, EPI>(prm, stream) : launch_cfg<160, 1, EPI>(prm, stream);
+    if (bn == 128) return passes == 3 ? launch_cfg<128, 3, EPI>(prm, stream) : launch_cfg<128, 1, EPI>(prm, stream);
+    return passes == 3 ? launch_cfg<64, 3, EPI>(prm, stream) : launch_cfg<64, 1, EPI>(prm, stream);
 }
 
 }  // namespace
@@ -384,8 +473,9 @@ bool gemm_tc_supported(const GemmProblem& p, std::string* why) {
 }
 
 // Tile width.  Problems with fewer 128-wide tiles than half the SMs are latency-bound: 64-wide tiles double the CTAs.  Otherwise the
-// width of 128 or 160 with the fewest waves x BN, ties to 128 (at equal column-waves the 160-wide tile only adds epilogue work; measured
-// on an H100 80GB HBM3 with tools/decode_gemm_rate.py, 160 pays for the 1280 x 4000 LSTM gates: 2 waves instead of 3 on 132 SMs).
+// width of 128 or 160 with the fewest waves x BN; 160 pays for the 1280 x 4000 LSTM gates (2 waves instead of 3 on 132 SMs, measured on
+// an H100 80GB HBM3 with tools/decode_gemm_rate.py).  Ties go to 128, the narrower tile that wastes fewer columns on a ragged last n-tile;
+// no measurement has yet compared the two widths at a tie.
 int gemm_tc_tile_n(int M, int N) {
     const int sms = sm_count();
     const int tiles_m = cdiv(M, BM);
@@ -438,14 +528,12 @@ int gemm_tc_plan_launch(GemmTcPlan* plan, const GemmEpilogue* epi_override, int 
         return 1;
     }
     if (prm.M <= 0 || prm.N <= 0) return 0;
-    if (prm.trace != nullptr) {                                  // capb200_gemm_trace only
-        if (plan->passes != 3) { set_error("gemm_tc: the traced kernel is the 3-pass one"); return 1; }
-        if (plan->bn == 160) return launch_cfg<160, 3, true>(prm, stream);
-        return plan->bn == 128 ? launch_cfg<128, 3, true>(prm, stream) : launch_cfg<64, 3, true>(prm, stream);
-    }
-    if (plan->bn == 160) return plan->passes == 3 ? launch_cfg<160, 3>(prm, stream) : launch_cfg<160, 1>(prm, stream);
-    if (plan->bn == 128) return plan->passes == 3 ? launch_cfg<128, 3>(prm, stream) : launch_cfg<128, 1>(prm, stream);
-    return plan->passes == 3 ? launch_cfg<64, 3>(prm, stream) : launch_cfg<64, 1>(prm, stream);
+    // the kind follows the epilogue this launch asks for: launches override the planned one whole
+    const int kind = prm.lstm ? kEpiLstm : prm.C_hi != nullptr ? kEpiPlanes : kEpiStore;
+    if (prm.trace != nullptr && plan->passes != 3) { set_error("gemm_tc: the traced kernel is the 3-pass one"); return 1; }
+    if (kind == kEpiLstm) return launch_kind<kEpiLstm>(plan->bn, plan->passes, prm, stream);
+    if (kind == kEpiPlanes) return launch_kind<kEpiPlanes>(plan->bn, plan->passes, prm, stream);
+    return launch_kind<kEpiStore>(plan->bn, plan->passes, prm, stream);
 }
 
 }  // namespace capb200

@@ -61,11 +61,6 @@ int capb200_linear(const float* x, long ldx, const float* w, long ldw, const flo
 int capb200_bench_linear(const float* x, const float* w, const float* b, float* y, int M, int N, int K, int mode, int iters, float* ms_per_launch,
                          void* stream);
 
-/* Diagnostics: one traced launch of the decode GEMM y[M,N] = x[M,K] w[N,K]^T (tc_f16x3, persistent kernel, one CTA per SM at most).
- * trace_host receives 296 x 16 %globaltimer stamps (ns), one row per CTA: 0 set-up done, 1 first operands landed, 2/3 main loop of the
- * CTA's first / second tile done (accumulator complete), 6/7 epilogue of tile 0 / 1 done, 8 kernel end; 4/5 are unused (tools/gemm_trace.py). */
-int capb200_gemm_trace(const float* x, const float* w, float* y, int M, int N, int K, unsigned long long* trace_host, int n_slots, void* stream);
-
 /* Diagnostics: the output-tile width (64, 128 or 160 columns) the tc_f16x3 / tc_f16x1 GEMM picks for an M x N problem on the current device. */
 int capb200_gemm_tile_n(int M, int N);
 
@@ -602,6 +597,49 @@ int capb200_tfm_set_grad_events(capb200_tfm_engine* e, void* const* events, int 
 int capb200_adam_chunk_elems(void);
 int capb200_adam_step(const unsigned long long* table, const long long* numel, const int* chunks, int n_chunks, double lr, double beta1, double beta2,
                       double eps, double weight_decay, long step, double clip_value, int write_clamped, void* stream);
+
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Decode GEMM with any fused epilogue (tests and tools/gemm_trace.py): y = x[M,K] w[N,K]^T on fp32 device inputs, split into fp16 planes
+ * in scratch memory, in mode CAPB200_MODE_TC_F16X3 or _TC_F16X1.  Every pointer in the epilogue is a device pointer; NULL turns an option
+ * off.  Per element: + bias[col] + row_bias[row / rows_per_group, col] + gather_bias[gather_idx[row], col] + residual[row, col], then ReLU.
+ * The kind follows from the fields: lstm != 0 is the fused nn.LSTMCell (N == 4H, gate-interleaved columns 4u+g, g in (i,f,g,o);
+ * c_prev is read at row src_row[row], identity when src_row is NULL, zero state when src_row[row] < 0; writes c_out, h_f and, when h_hi
+ * is set, the split planes h_hi / h_lo); otherwise C_hi != NULL stores the split planes C_hi / C_lo (fp16, as unsigned short) and C when
+ * set; otherwise fp32 C.  Outputs must not overlap inputs.  Synchronous.
+ * trace_host (or NULL): 296 x 16 %globaltimer stamps (ns) of one launch after three warm ones (tc_f16x3 only), one row per CTA: 0 set-up
+ * done, 1 first operands landed, 2/3 main loop of the CTA's first / second tile done, 6/7 epilogue of tile 0 / 1 done, 8 kernel end.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct {
+    const float* bias;
+    const float* row_bias;
+    long ld_row_bias;
+    int rows_per_group;
+    const float* residual;
+    long ld_res;
+    int relu;
+    float* C;
+    long ldc;
+    unsigned short* C_hi;
+    unsigned short* C_lo;
+    long ldcs;
+    int lstm;
+    int H;
+    const float* c_prev;
+    long ld_cprev;
+    const int* src_row;
+    float* c_out;
+    long ld_cout;
+    const float* gather_bias;
+    long ld_gb;
+    const int* gather_idx;
+    float* h_f;
+    unsigned short* h_hi;
+    unsigned short* h_lo;
+    long ld_h;
+} capb200_gemm_epilogue;
+int capb200_decode_gemm(const float* x, const float* w, int M, int N, int K, int mode, const capb200_gemm_epilogue* epi, unsigned long long* trace_host,
+                        int n_slots, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,9 +1,15 @@
 """GPU: where the time of one decode GEMM launch goes.  Runs the 3-pass wgmma kernel on a decode-step shape with the phase stamps on
-(capb200_gemm_trace) and prints, relative to the earliest set-up stamp, when each phase happened (median / max over the CTAs).
+(capb200_decode_gemm with a trace buffer) and prints, relative to the earliest set-up stamp, when each phase happened (median / max over
+the CTAs), and the epilogue time per tile.
 
-    python tools/gemm_trace.py [M N K]        default: the language-LSTM gates of the headline shape, 1280 x 4000 x 3000
+    python tools/gemm_trace.py [--epilogue store|planes|lstm] [M N K]
+
+default shape: the language-LSTM gates of the headline shape, 1280 x 4000 x 3000.  Epilogues as the decode step runs them:
+    store    fp32 C + bias (logit, h2att, ctx2att)
+    planes   fp32 C + split fp16 planes + bias + ReLU (fc_embed, att_embed)
+    lstm     fused LSTM cell: bias, c_prev read through a permuted src_row, c_out, h and its split planes (language LSTM, N = 4H)
 """
-import os, sys
+import argparse, os, sys
 import numpy as np
 import torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -11,16 +17,44 @@ sys.path.insert(0, REPO)
 import imagecaptioning.pytorch_b200 as b200
 L = b200._lib
 lib = L.load()
-M, N, K = (int(v) for v in sys.argv[1:4]) if len(sys.argv) >= 4 else (1280, 4000, 3000)
-x = torch.randn(M, K, device='cuda'); w = torch.randn(N, K, device='cuda') / K ** 0.5; y = torch.empty(M, N, device='cuda')
+ap = argparse.ArgumentParser()
+ap.add_argument('--epilogue', choices=['store', 'planes', 'lstm'], default='store')
+ap.add_argument('shape', nargs='*', type=int, default=[1280, 4000, 3000])
+args = ap.parse_args()
+M, N, K = args.shape
+x = torch.randn(M, K, device='cuda'); w = torch.randn(N, K, device='cuda') / K ** 0.5
+epi = L.GemmEpilogue()
+bias = torch.randn(N, device='cuda')
+epi.bias = L.ptr(bias)
+keep = [bias]
+if args.epilogue == 'lstm':
+    H = N // 4
+    c_prev = torch.randn(M, H, device='cuda'); c_out = torch.empty(M, H, device='cuda'); h = torch.empty(M, H, device='cuda')
+    hp = torch.empty(2, M, H, dtype=torch.float16, device='cuda')
+    src = torch.randperm(M, device='cuda').int()
+    keep += [c_prev, c_out, h, hp, src]
+    epi.lstm, epi.H = 1, H
+    epi.c_prev, epi.ld_cprev, epi.src_row = L.ptr(c_prev), H, L.ptr(src)
+    epi.c_out, epi.ld_cout = L.ptr(c_out), H
+    epi.h_f, epi.h_hi, epi.h_lo, epi.ld_h = L.ptr(h), L.ptr(hp[0]), L.ptr(hp[1]), H
+else:
+    y = torch.empty(M, N, device='cuda')
+    keep.append(y)
+    epi.C, epi.ldc = L.ptr(y), N
+    if args.epilogue == 'planes':
+        yp = torch.empty(2, M, N, dtype=torch.float16, device='cuda')
+        keep.append(yp)
+        epi.C_hi, epi.C_lo, epi.ldcs, epi.relu = L.ptr(yp[0]), L.ptr(yp[1]), N, 1
 tr = np.zeros((296, 16), dtype=np.uint64)
-L.check(lib.capb200_gemm_trace(L.ptr(x), L.ptr(w), L.ptr(y), M, N, K, tr.ctypes.data, tr.size, L.current_stream()), 'gemm_trace')
+L.check(lib.capb200_decode_gemm(L.ptr(x), L.ptr(w), M, N, K, L.OP_MODES['tc_f16x3'], epi, tr.ctypes.data, tr.size, L.current_stream()),
+        'decode_gemm')
 used = tr[:, 0] > 0
 t = tr[used].astype(np.float64)
 t0 = t[:, 0].min()
 names = ['set-up done', 'first operands landed', 'tile 0: main loop done', 'tile 1: main loop done', '(unused)', '(unused)',
          'tile 0: epilogue done', 'tile 1: epilogue done', 'kernel end']
-print('decode GEMM %d x %d x %d, %d CTAs traced; times in us after the first CTA finished its set-up' % (M, N, K, int(used.sum())))
+print('decode GEMM %d x %d x %d, %s epilogue, BN %d, %d CTAs traced; times in us after the first CTA finished its set-up'
+      % (M, N, K, args.epilogue, lib.capb200_gemm_tile_n(M, N), int(used.sum())))
 for i, n in enumerate(names):
     col = t[:, i]
     col = col[col > 0]
@@ -31,7 +65,11 @@ lead = t[(t[:, 2] > 0)]
 if lead.size:
     d01 = (lead[:, 2] - lead[:, 1]) / 1e3
     print('first operands -> tile 0 main loop done: median %.2f us (%d K-blocks => %.3f us per K-block)' % (np.median(d01), -(-K // 64), np.median(d01) / (-(-K // 64))))
+    epi0 = (lead[:, 6] - lead[:, 2]) / 1e3
+    print('epilogue of tile 0: median %.2f us, max %.2f us' % (np.median(epi0), epi0.max()))
     two = lead[lead[:, 3] > 0]
     if two.size:
         d12 = (two[:, 3] - two[:, 2]) / 1e3
-        print('CTAs with two tiles: tile 0 main loop -> tile 1 main loop: median %.2f us' % np.median(d12))
+        epi1 = (two[:, 7] - two[:, 3]) / 1e3
+        print('CTAs with two tiles: tile 0 main loop -> tile 1 main loop: median %.2f us; epilogue of tile 1: median %.2f us, max %.2f us'
+              % (np.median(d12), np.median(epi1), epi1.max()))
