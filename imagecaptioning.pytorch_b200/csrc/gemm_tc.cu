@@ -12,11 +12,16 @@
 // Structure (persistent: one 128 x BN output tile at a time per CTA, BN = 64, 128 or 160 chosen by the plan, 384 threads = three warpgroups):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2-D boxes [64 k x rows] (128B swizzle) for A_hi, A_lo, W_hi,
 //                   W_lo of the current K-block into a STAGES-deep shared-memory ring, mbarrier complete_tx signalling.  It runs ahead
-//                   into the next tile while the consumers are in their epilogue.
-//   warpgroups 1,2  consumers: each owns 64 rows of the tile, issues wgmma.m64nBNk16 straight from shared-memory descriptors, releases
-//                   the ring slot once its wgmmas retired, and runs the fused epilogue (bias / row-bias / ReLU, fp32 store, optional
-//                   split-fp16 copy for the next GEMM, or the fused LSTM cell) from the register accumulator.  The epilogue kind is a
-//                   template parameter (EpiKind), so each kernel carries the code of one kind only.
+//                   into the next tile.  40 registers (setmaxnreg), the consumers 232.
+//   warpgroups 1,2  ping-pong consumers: warpgroup 1 runs the CTA's even tiles, warpgroup 2 its odd ones, each holding the whole
+//                   128 x BN accumulator as two m64 halves.  They take turns at the main loop (wgmma.m64nBNk16 straight from
+//                   shared-memory descriptors, the ring slot released once the wgmmas retired), so one tile's fused epilogue (bias /
+//                   row-bias / ReLU, fp32 store, optional split-fp16 copy for the next GEMM, or the fused LSTM cell) runs from registers
+//                   under the next tile's main loop; only a CTA's last epilogue is exposed.  The epilogue kind is a template parameter
+//                   (EpiKind), so each kernel carries the code of one kind only.
+// On an H100 80GB HBM3 at a 400 W power limit, the ping-pong schedule and the vectorised LSTM stores take the UpDown decode step's LSTM
+// gate GEMMs from 3.34 to 3.02-3.06 ms (att_lstm) and 4.10-4.14 to 3.74-3.81 ms (lang_lstm) per batch; logit and h2att are unchanged
+// (DESIGN §5.1).
 // K-segments (up to 3 activation/weight pairs) are walked back to back so concatenated LSTM inputs are never built.
 #include <cstdlib>
 
@@ -29,7 +34,7 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;   // fp16 elements: one 128-byte swizzle row
-constexpr int kConsumers = 2;                  // consumer warpgroups, 64 accumulator rows each
+constexpr int kConsumers = 2;                  // consumer warpgroups, one whole tile each, taking turns
 constexpr int kThreads = 128 * (1 + kConsumers);
 
 struct TcParams {
@@ -162,46 +167,129 @@ __device__ __forceinline__ void epi_adds(const TcParams& p, float* acc, int r0, 
     }
 }
 
-// Fused LSTM cell.  Gates (i,f,g,o) of hidden unit c/4 sit in lanes 2k (i,f) and 2k+1 (g,o): the even lane finishes the unit for row r0,
-// the odd lane for row r0 + 8, each taking the two gates it lacks from its neighbour.  src_row and the c_prev values of the thread's
-// BN/8 units are loaded before the first store.
-template <int BN>
-__device__ __forceinline__ void epi_lstm(const TcParams& p, const float* acc, int r0, int c0, int lane) {
+// Fused LSTM cell.  Gates (i,f,g,o) of hidden unit c/4 sit in lanes 2k (i,f) and 2k+1 (g,o) of a quad: the even lane takes the unit for
+// row r0, the odd lane for row r0 + 8, each taking the two gates it lacks from its neighbour (shfl.xor 1).  Quad lanes q and q ^ 2 then
+// hold the even and the odd units of the same row; they trade (shfl.xor 2) so that each lane holds runs of 4 consecutive units of its
+// row, one run per 16 gate columns, and c_prev, c_out and h_f move as 16-byte vectors, h_hi and h_lo as 8-byte ones.  A row whose
+// pointers are not aligned for that, or whose units run past H, takes the element path.  Units of run k of lane q: u0 + 8k + 4 * (q >> 1)
+// + o, o = 0..3; unit o of run k comes from column pair j = 4k + (o >> 1) + 2 * (o & 1).  Every load comes before the first store.
+// TRACE: thread `slot >= 0` stamps slots slot, slot + 1, slot + 2 when its c_prev values have landed, the cell math is done and its
+// last store is issued.
+template <int BN, bool TRACE>
+__device__ __forceinline__ void epi_lstm(const TcParams& p, float* acc, int r0, int c0, int lane, int slot) {
+    constexpr int kRuns = BN / 32;
     const bool odd = lane & 1;
+    const bool upper = lane & 2;
     const int row = r0 + (odd ? 8 : 0);
-    const int u0 = c0 >> 2;                                     // unit of column pair j is u0 + 2j
+    const int u0 = ((c0 - 2 * (lane & 3)) >> 2) + (upper ? 4 : 0);   // first unit of run 0
     const bool row_ok = row < p.M;
+    const bool full = u0 + 8 * (kRuns - 1) + 4 <= p.H;                  // every unit of the lane in range
     int src = row;
     if (p.src_row != nullptr && row_ok) src = p.src_row[row];
-    const float* cprev = (src >= 0 && p.c_prev != nullptr) ? p.c_prev + (long)src * p.ld_cprev : nullptr;
+    const float* cprev = (row_ok && src >= 0 && p.c_prev != nullptr) ? p.c_prev + (long)src * p.ld_cprev + u0 : nullptr;
     float cp[BN / 8];
+    if (cprev != nullptr && full && (reinterpret_cast<uintptr_t>(cprev) & 15) == 0) {
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) cp[j] = (row_ok && cprev != nullptr && u0 + 2 * j < p.H) ? cprev[u0 + 2 * j] : 0.0f;
-    float* const c_out = p.c_out + (long)row * p.ld_cout;
-    float* const h_f = p.h_f + (long)row * p.ld_h;
-    __half* const h_hi = p.h_hi + (long)row * p.ld_h;
-    __half* const h_lo = p.h_lo + (long)row * p.ld_h;
-    const bool planes = p.h_hi != nullptr;
+        for (int k = 0; k < kRuns; ++k) {
+            const float4 v = *reinterpret_cast<const float4*>(cprev + 8 * k);
+            cp[4 * k] = v.x; cp[4 * k + 1] = v.y; cp[4 * k + 2] = v.z; cp[4 * k + 3] = v.w;
+        }
+    } else {
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-        const float* v = acc + 4 * j;
+        for (int i = 0; i < BN / 8; ++i) {
+            const int du = 8 * (i / 4) + i % 4;
+            cp[i] = (cprev != nullptr && u0 + du < p.H) ? cprev[du] : 0.0f;
+        }
+    }
+    if (TRACE && slot >= 0) {
+        float s = 0.0f;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) s += cp[i];
+        asm volatile("" ::"f"(s));
+        CAPB_TRACE(slot);
+    }
+    __syncwarp();                                               // the load paths above diverge; the shuffles below need no fallback
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {                          // gates of unit (u0 - 4 * upper) + 2j + (upper): acc[4j .. 4j + 3] = i, f, g, o
+        float* v = acc + 4 * j;
         const float s0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 1);
         const float s1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 1);
         const float gi = odd ? s0 : v[0], gf = odd ? s1 : v[1], gg = odd ? v[2] : s0, go = odd ? v[3] : s1;
-        const int unit = u0 + 2 * j;
-        if (row_ok && unit < p.H) {
-            const float cn = fast_sigmoid(gf) * cp[j] + fast_sigmoid(gi) * fast_tanh(gg);
-            const float hn = fast_sigmoid(go) * fast_tanh(cn);
-            c_out[unit] = cn;
-            h_f[unit] = hn;
-            if (planes) {
-                __half hh, hl;
-                split_f32(hn, hh, hl);
-                h_hi[unit] = hh;
-                h_lo[unit] = hl;
+        v[0] = gi; v[1] = gf; v[2] = gg; v[3] = go;
+    }
+#pragma unroll
+    for (int k = 0; k < kRuns; ++k) {                           // lower lane keeps pairs 4k, 4k + 1, upper lane pairs 4k + 2, 4k + 3
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+            float* x = acc + 4 * (4 * k + t);                   // becomes unit o = 2t of run k
+            float* y = acc + 4 * (4 * k + 2 + t);               // becomes unit o = 2t + 1
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+                const float keep = upper ? y[g] : x[g];
+                const float recv = __shfl_xor_sync(0xffffffffu, upper ? x[g] : y[g], 2);
+                x[g] = upper ? recv : keep;
+                y[g] = upper ? keep : recv;
             }
         }
     }
+    float cn[BN / 8], hn[BN / 8];
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+        const int k = i / 4, o = i % 4;
+        const float* g = acc + 4 * (4 * k + (o >> 1) + 2 * (o & 1));
+        cn[i] = fast_sigmoid(g[1]) * cp[i] + fast_sigmoid(g[0]) * fast_tanh(g[2]);
+        hn[i] = fast_sigmoid(g[3]) * fast_tanh(cn[i]);
+    }
+    if (TRACE && slot >= 0) {
+        float s = 0.0f;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) s += hn[i];
+        asm volatile("" ::"f"(s));
+        CAPB_TRACE(slot + 1);
+    }
+    if (row_ok) {
+        float* const c_out = p.c_out + (long)row * p.ld_cout + u0;
+        float* const h_f = p.h_f + (long)row * p.ld_h + u0;
+        __half* const h_hi = p.h_hi + (long)row * p.ld_h + u0;
+        __half* const h_lo = p.h_lo + (long)row * p.ld_h + u0;
+        const bool planes = p.h_hi != nullptr;
+        const uintptr_t a16 = reinterpret_cast<uintptr_t>(c_out) | reinterpret_cast<uintptr_t>(h_f);
+        const uintptr_t a8 = planes ? reinterpret_cast<uintptr_t>(h_hi) | reinterpret_cast<uintptr_t>(h_lo) : 0;
+        if (full && (a16 & 15) == 0 && (a8 & 7) == 0) {
+#pragma unroll
+            for (int k = 0; k < kRuns; ++k) {
+                const float* c = cn + 4 * k;
+                const float* h = hn + 4 * k;
+                *reinterpret_cast<float4*>(c_out + 8 * k) = make_float4(c[0], c[1], c[2], c[3]);
+                *reinterpret_cast<float4*>(h_f + 8 * k) = make_float4(h[0], h[1], h[2], h[3]);
+                if (planes) {
+                    __half hh[4], hl[4];
+#pragma unroll
+                    for (int o = 0; o < 4; ++o) split_f32(h[o], hh[o], hl[o]);
+                    const __half2 hi01 = __halves2half2(hh[0], hh[1]), hi23 = __halves2half2(hh[2], hh[3]);
+                    const __half2 lo01 = __halves2half2(hl[0], hl[1]), lo23 = __halves2half2(hl[2], hl[3]);
+                    *reinterpret_cast<uint2*>(h_hi + 8 * k) = make_uint2(*reinterpret_cast<const uint32_t*>(&hi01), *reinterpret_cast<const uint32_t*>(&hi23));
+                    *reinterpret_cast<uint2*>(h_lo + 8 * k) = make_uint2(*reinterpret_cast<const uint32_t*>(&lo01), *reinterpret_cast<const uint32_t*>(&lo23));
+                }
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < BN / 8; ++i) {
+                const int du = 8 * (i / 4) + i % 4;
+                if (u0 + du < p.H) {
+                    c_out[du] = cn[i];
+                    h_f[du] = hn[i];
+                    if (planes) {
+                        __half hh, hl;
+                        split_f32(hn[i], hh, hl);
+                        h_hi[du] = hh;
+                        h_lo[du] = hl;
+                    }
+                }
+            }
+        }
+    }
+    if (TRACE && slot >= 0) CAPB_TRACE(slot + 2);
 }
 
 // fp32 C and / or the split planes of rows r0, r0 + 8.  Columns come in pairs starting at an even column, so whether the pairs of a row
@@ -254,19 +342,24 @@ __device__ __forceinline__ void epi_store(const TcParams& p, const float* acc, i
     }
 }
 
-// Drains this warpgroup's 64 x BN accumulator (layout above).
-template <int BN, int EPI>
-__device__ __forceinline__ void epilogue_tile(const TcParams& p, float* acc, int m0, int n0, int tid) {
+// Drains 64 rows x BN of a warpgroup's accumulator (layout above).  TRACE: `slot` as for epi_lstm.
+template <int BN, int EPI, bool TRACE>
+__device__ __forceinline__ void epilogue_tile(const TcParams& p, float* acc, int m0, int n0, int tid, int slot) {
     const int warp = tid >> 5, lane = tid & 31;
     const int r0 = m0 + warp * 16 + (lane >> 2);
     const int c0 = n0 + 2 * (lane & 3);
     epi_adds<BN>(p, acc, r0, c0);
-    if (EPI == kEpiLstm) epi_lstm<BN>(p, acc, r0, c0, lane);
+    if (EPI == kEpiLstm) epi_lstm<BN, TRACE>(p, acc, r0, c0, lane, slot);
     else epi_store<BN, EPI == kEpiPlanes>(p, acc, r0, c0);
 }
 
 // Persistent schedule: gridDim.x = min(tiles, SMs); CTA b walks tiles b, b + gridDim.x, ... in m-fastest order so that concurrently
 // running CTAs share the same weight columns (the W tile comes from HBM once, then from L2).
+//
+// Ping-pong consumers: warpgroup 1 takes the CTA's even tile ordinals, warpgroup 2 the odd ones, each with the whole 128 x BN
+// accumulator.  Their main loops take turns (turn_bar), so the epilogue of tile k runs under the main loop of tile k + 1.  The ring is
+// consumed in the producer's order: tile ordinal `it` starts at K-block it * kb_tile of the ring's sequence, and a warpgroup only waits
+// on the ring after the other one has waited on every earlier K-block, so a parity wait never matches a phase two uses behind.
 template <int BN, int PASSES, int EPI, bool TRACE = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
     using Cfg = TcCfg<BN, PASSES>;
@@ -274,6 +367,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + Cfg::kStages;
+    uint64_t* turn_bar = empty_bar + Cfg::kStages;              // [cw]: consumer warpgroup cw may start its next main loop
 
     const int wg = threadIdx.x >> 7;
     const int n_tiles = p.tiles_m * p.tiles_n;
@@ -289,14 +383,16 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
         for (int i = 0; i < Cfg::kStages; ++i) {
             ptx::mbar_init(&full_bar[i], 1);
-            ptx::mbar_init(&empty_bar[i], kConsumers);        // one release per consumer warpgroup
+            ptx::mbar_init(&empty_bar[i], 1);                  // released by the one warpgroup that read the slot
         }
+        for (int c = 0; c < kConsumers; ++c) ptx::mbar_init(&turn_bar[c], 1);
         ptx::fence_mbar_init();
     }
     __syncthreads();
     if (threadIdx.x == 0) CAPB_TRACE(0);                       // set-up done
 
     if (wg == 0) {
+        ptx::setmaxnreg_dec<40>();
         if (threadIdx.x == 0) {
             int stage = 0;
             uint32_t phase = 0;
@@ -324,50 +420,76 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
         }
     } else {
-        const int cw = wg - 1;                                  // rows [64 cw, 64 cw + 64) of every tile
+        ptx::setmaxnreg_inc<232>();
+        const int cw = wg - 1;                                  // tile ordinals cw, cw + 2, ... of this CTA
         const int tid = threadIdx.x & 127;
-        const uint32_t a_off = cw * 64 * 128;                   // 64 rows of 128 bytes: a whole number of swizzle atoms
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        for (int t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
+        constexpr uint32_t kHalf = 64 * 128;                    // rows 64..127 of an A box: a whole number of swizzle atoms
+        int kb_tile = 0;
+        for (int s = 0; s < p.nseg; ++s) kb_tile += p.kblocks[s];
+        int mine = 0;                                           // tiles this warpgroup has run
+        for (int it = cw, t = blockIdx.x + cw * gridDim.x; t < n_tiles; it += 2, t += 2 * gridDim.x, ++mine) {
             const int m0 = (t % p.tiles_m) * BM;
             const int n0 = (t / p.tiles_m) * BN;
-            float acc[BN / 2];
+            // Turn: arrivals on turn_bar[cw] come from the other warpgroup at the end of ordinals cw - 1, cw + 1, ...
+            if (it > 0) ptx::mbar_wait(&turn_bar[cw], (cw == 1 ? mine : mine - 1) & 1);
+            if (TRACE && it == 1 && tid == 0) CAPB_TRACE(4);                           // main loop of tile 1 starts
+            const long g0 = (long)it * kb_tile;
+            int stage = (int)(g0 % Cfg::kStages);
+            uint32_t phase = (uint32_t)(g0 / Cfg::kStages) & 1;
+            float acc0[BN / 2], acc1[BN / 2];                   // rows 0..63 and 64..127 of the tile
 #pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+            for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
             for (int s = 0; s < p.nseg; ++s) {
                 for (int kb = 0; kb < p.kblocks[s]; ++kb) {
                     ptx::mbar_wait(&full_bar[stage], phase);
-                    if (TRACE && it == 0 && s == 0 && kb == 0 && tid == 0 && cw == 0) CAPB_TRACE(1);    // first operands landed
+                    if (TRACE && it == 0 && s == 0 && kb == 0 && tid == 0) CAPB_TRACE(1);    // first operands landed
                     const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-                    const uint32_t a_hi = st + a_off;
-                    const uint32_t a_lo = st + Cfg::kABytes + a_off;                  // only valid when PASSES == 3
+                    const uint32_t a_hi = st;
+                    const uint32_t a_lo = st + Cfg::kABytes;                          // only valid when PASSES == 3
                     const uint32_t w_hi = st + Cfg::kABytes * Cfg::kPlanes;
                     const uint32_t w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;       // only valid when PASSES == 3
 #pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) ptx::reg_fence(acc[i]);
+                    for (int i = 0; i < BN / 2; ++i) { ptx::reg_fence(acc0[i]); ptx::reg_fence(acc1[i]); }
                     ptx::wgmma_fence();
 #pragma unroll
                     for (int k = 0; k < BK / 16; ++k) {
                         const uint32_t koff = k * 32;   // 16 fp16 = 32 bytes inside the 128-byte swizzle row
+                        const uint64_t dwh = ptx::make_smem_desc_sw128(w_hi + koff);
+                        // the same hi*lo, lo*hi, hi*hi order into each half (per element the sums of a 64-row warpgroup), the halves
+                        // alternating so that no wgmma waits on the accumulator of the one just before it
                         if (PASSES == 3) {
-                            wgmma_f16<BN>(acc, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_lo + koff), 1);
-                            wgmma_f16<BN>(acc, ptx::make_smem_desc_sw128(a_lo + koff), ptx::make_smem_desc_sw128(w_hi + koff), 1);
+                            const uint64_t dwl = ptx::make_smem_desc_sw128(w_lo + koff);
+                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwl, 1);
+                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwl, 1);
+                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_lo + koff), dwh, 1);
+                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_lo + kHalf + koff), dwh, 1);
+                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwh, 1);
+                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwh, 1);
+                        } else {
+                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwh, 1);
+                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwh, 1);
                         }
-                        wgmma_f16<BN>(acc, ptx::make_smem_desc_sw128(a_hi + koff), ptx::make_smem_desc_sw128(w_hi + koff), 1);
                     }
                     ptx::wgmma_commit();
                     ptx::wgmma_wait<0>();
 #pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) ptx::reg_fence(acc[i]);
-                    if (tid == 0) ptx::mbar_arrive(&empty_bar[stage]);                // this warpgroup no longer reads the slot
+                    for (int i = 0; i < BN / 2; ++i) { ptx::reg_fence(acc0[i]); ptx::reg_fence(acc1[i]); }
+                    if (tid == 0) ptx::mbar_arrive(&empty_bar[stage]);                // the slot is free again
                     if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
                 }
             }
-            if (TRACE && it < 2 && tid == 0 && cw == 0) CAPB_TRACE(2 + it);          // main loop of tile `it` done
-            epilogue_tile<BN, EPI>(p, acc, m0 + cw * 64, n0, tid);
-            if (TRACE && it < 2 && tid == 0 && cw == 0) CAPB_TRACE(6 + it);          // epilogue of tile `it` done
+            // Every thread of the warpgroup has waited on all of this tile's K-blocks (its wgmmas, issued by all 128, retired).
+            if (tid == 0) ptx::mbar_arrive(&turn_bar[cw ^ 1]);
+            if (TRACE && it < 2 && tid == 0) CAPB_TRACE(2 + it);                       // main loop of tile `it` done
+            // rows 0..63, then rows 64..127 moved into acc0: one copy of the epilogue's code, indexed statically
+#pragma unroll 1
+            for (int h = 0; h < 2; ++h) {
+                const int slot = (TRACE && it < 2 && h == 0 && tid == 0) ? 9 + 3 * it : -1;
+                epilogue_tile<BN, EPI, TRACE>(p, acc0, m0 + 64 * h, n0, tid, slot);
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
+            }
+            if (TRACE && it < 2 && tid == 0) CAPB_TRACE(6 + it);                       // epilogue of tile `it` done
         }
     }
     __syncthreads();

@@ -61,6 +61,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// ---- per-warpgroup register budget ----------------------------------------------------------------
+// Executed by all threads of a warpgroup: hands registers back to the pool (dec) or takes them from it (inc).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- TMA ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");

@@ -1,6 +1,8 @@
 """GPU: where the time of one decode GEMM launch goes.  Runs the 3-pass wgmma kernel on a decode-step shape with the phase stamps on
 (capb200_decode_gemm with a trace buffer) and prints, relative to the earliest set-up stamp, when each phase happened (median / max over
-the CTAs), and the epilogue time per tile.
+the CTAs), the epilogue time per tile and whether tile 0's epilogue (consumer warpgroup 1) ended before tile 1's main loop (warpgroup 2)
+did.  With --epilogue lstm it also splits the first 64 rows of each tile's LSTM epilogue into bias adds and c_prev loads, cell math, and
+stores.
 
     python tools/gemm_trace.py [--epilogue store|planes|lstm] [M N K]
 
@@ -51,8 +53,10 @@ L.check(lib.capb200_decode_gemm(L.ptr(x), L.ptr(w), M, N, K, L.OP_MODES['tc_f16x
 used = tr[:, 0] > 0
 t = tr[used].astype(np.float64)
 t0 = t[:, 0].min()
-names = ['set-up done', 'first operands landed', 'tile 0: main loop done', 'tile 1: main loop done', '(unused)', '(unused)',
-         'tile 0: epilogue done', 'tile 1: epilogue done', 'kernel end']
+names = ['set-up done', 'first operands landed', 'tile 0: main loop done', 'tile 1: main loop done', 'tile 1: main loop starts', '(unused)',
+         'tile 0: epilogue done', 'tile 1: epilogue done', 'kernel end',
+         'tile 0 lstm: c_prev landed', 'tile 0 lstm: cell math done', 'tile 0 lstm: stores issued',
+         'tile 1 lstm: c_prev landed', 'tile 1 lstm: cell math done', 'tile 1 lstm: stores issued']
 print('decode GEMM %d x %d x %d, %s epilogue, BN %d, %d CTAs traced; times in us after the first CTA finished its set-up'
       % (M, N, K, args.epilogue, lib.capb200_gemm_tile_n(M, N), int(used.sum())))
 for i, n in enumerate(names):
@@ -73,3 +77,13 @@ if lead.size:
         epi1 = (two[:, 7] - two[:, 3]) / 1e3
         print('CTAs with two tiles: tile 0 main loop -> tile 1 main loop: median %.2f us; epilogue of tile 1: median %.2f us, max %.2f us'
               % (np.median(d12), np.median(epi1), epi1.max()))
+        hidden = two[:, 6] <= two[:, 3]
+        print('tile 0 epilogue ended before tile 1 main loop did: %d of %d CTAs' % (int(hidden.sum()), len(two)))
+    if args.epilogue == 'lstm':
+        for tile, (done, first) in enumerate([(2, 9), (3, 12)]):
+            r = lead[(lead[:, done] > 0) & (lead[:, first + 2] > 0)]
+            if r.size == 0:
+                continue
+            parts = [(r[:, first] - r[:, done]) / 1e3, (r[:, first + 1] - r[:, first]) / 1e3, (r[:, first + 2] - r[:, first + 1]) / 1e3]
+            print('tile %d lstm epilogue, rows 0..63, median (max) us: adds + c_prev loads %.2f (%.2f), cell math %.2f (%.2f), stores %.2f (%.2f)'
+                  % ((tile,) + tuple(v for q in parts for v in (np.median(q), q.max()))))
