@@ -5,7 +5,7 @@ host-side mirrors of the reference interfaces (``models``, ``loss_wrapper``, ``r
 (``parallel``, ``grad_sync``).  See DESIGN.md.
 """
 from . import _lib                                    # noqa: F401
-from .models import B200UpDownModel, B200NewFCModel, B200Att2in2Model, B200TransformerModel, B200AoAModel, B200CaptionModel, setup      # noqa: F401
+from .models import B200UpDownModel, B200NewFCModel, B200Att2in2Model, B200TransformerModel, B200AoAModel, B200AttEnsemble, B200CaptionModel, setup      # noqa: F401
 from .loss_wrapper import B200LossWrapper, RewardCriterion                        # noqa: F401
 from . import rewards                                 # noqa: F401
 from . import parallel                                # noqa: F401
@@ -15,5 +15,5 @@ from . import grad_sync                               # noqa: F401
 from . import optim                                   # noqa: F401
 from .utils import decode_sequence                    # noqa: F401
 
-__all__ = ['setup', 'B200UpDownModel', 'B200NewFCModel', 'B200Att2in2Model', 'B200TransformerModel', 'B200AoAModel', 'B200CaptionModel', 'B200LossWrapper', 'RewardCriterion',
+__all__ = ['setup', 'B200UpDownModel', 'B200NewFCModel', 'B200Att2in2Model', 'B200TransformerModel', 'B200AoAModel', 'B200AttEnsemble', 'B200CaptionModel', 'B200LossWrapper', 'RewardCriterion',
            'rewards', 'parallel', 'utils', 'eval_utils', 'grad_sync', 'decode_sequence']

@@ -15,6 +15,8 @@ MODES = {'simt_fp32': MODE_SIMT_FP32, 'tc_f16x3': MODE_TC_F16X3, 'tc_f16x1': MOD
 # capb200_linear additionally exposes the training step's split-K GEMM variants
 OP_MODES = dict(MODES, skinny_tf32x3=3, skinny_fp32=4, tf32x3_tc=5, tf32x3_tc_dgrad=6, tf32x3_tc_wgrad=7)
 FAMILY_UPDOWN, FAMILY_NEWFC, FAMILY_ATT2IN2 = 0, 1, 2
+FAMILY_AOA = 3                    # ensemble members only (capb200_ensemble_member)
+ENSEMBLE_MAX_MEMBERS = 8
 SAMPLE_GREEDY, SAMPLE_MULTINOMIAL, SAMPLE_FORCED, SAMPLE_TEACHER, SAMPLE_TOPK, SAMPLE_TOPP = 0, 1, 2, 3, 4, 5
 
 
@@ -62,6 +64,10 @@ class SampleOpts(Structure):
 
     def __init__(self, sample_n, method, temperature=1.0, seed=0, steps=0, top=0.0, edits=None):
         super().__init__(sample_n, method, temperature, seed, steps, top, edits if edits is not None else DecodeEdits.none())
+
+
+class EnsembleMember(Structure):
+    _fields_ = [('family', c_int), ('engine', c_void_p), ('weight', c_float)]
 
 
 class RewardWeights(Structure):
@@ -232,6 +238,14 @@ SIGNATURES = {
     'capb200_aoa_xe_step': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(AoaXeOpts), c_void_p, c_void_p, c_int, POINTER(AoaWeights), c_void_p,
                                     c_void_p, c_void_p]),
     'capb200_aoa_launch_count': (c_long, [c_void_p]),
+    'capb200_ensemble_create': (c_void_p, []),
+    'capb200_ensemble_destroy': (None, [c_void_p]),
+    'capb200_ensemble_decode_beam': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_ensemble_beam_record_logprobs': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    'capb200_ensemble_decode_sample': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(SampleOpts), c_void_p, c_long,
+                                               c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_ensemble_launch_count': (c_long, [c_void_p]),
     'capb200_updown_scst_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), c_void_p, c_void_p, c_void_p, c_int,
                                          POINTER(UpdownGrads), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'capb200_att2in2_scst_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), c_void_p, c_void_p, c_void_p, c_int,

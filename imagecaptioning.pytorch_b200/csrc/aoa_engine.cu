@@ -305,6 +305,38 @@ int check_ready(capb200_aoa_engine* e) {
 
 }  // namespace
 
+// ---- the decode pieces (engine_common.cuh) ----------------------------------------------------------------------------
+namespace capb200 {
+
+int aoa_member_info(capb200_aoa_engine* e, MemberInfo* m) {
+    if (check_ready(e)) return 1;
+    m->family = CAPB200_FAMILY_AOA;
+    m->V1 = e->V1; m->T = e->T;
+    m->attends = true;
+    m->graph_ok = true;
+    m->ws = e->ws; m->wblock = e->wblock;
+    m->fresh = e->d.neg1;
+    m->launches = &e->launches;
+    return 0;
+}
+
+int aoa_decode_workspace(capb200_aoa_engine* e, int B, int rows, int R, int beam, cudaStream_t st) {
+    return ensure_workspace(e, B, rows, R, beam, st);
+}
+
+int aoa_decode_prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, cudaStream_t st) {
+    if (prepare(e, att, mask, B, R, st)) return 1;
+    e->core_cur = 0;
+    return 0;
+}
+
+int aoa_decode_core(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int R,
+                    const float* mask, cudaStream_t st) {
+    return core_step(e, rows, rpi, tokens, src_row, logits, ld, 0, R, mask, st);
+}
+
+}  // namespace capb200
+
 extern "C" {
 
 capb200_aoa_engine* capb200_aoa_create(const capb200_aoa_cfg* c) {
@@ -432,11 +464,10 @@ int capb200_aoa_decode_beam(capb200_aoa_engine* e, const float* att, const float
     const int beam = opts->beam_size, keep = opts->sample_n;
     CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= e->V1, "beam_size must be in 1..16 and <= V+1");
     CAPB_REQUIRE(keep == 1 || keep == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
-    if (ensure_workspace(e, B, B * beam, R, beam, st)) return 1;
-    if (prepare(e, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
+    if (aoa_decode_workspace(e, B, B * beam, R, beam, st)) return 1;
+    if (aoa_decode_prepare(e, att, mask, B, R, st)) return 1;
     auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return core_step(e, nrows, live, tokens, src_row, logits, ld, B, R, mask, st);
+        return aoa_decode_core(e, nrows, live, tokens, src_row, logits, ld, R, mask, st);
     };
     return beam_decode_driver(e->d, e->V1, e->T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
                               done_raw, core, &e->launches, st, loop_graph_key(e->ws, e->wblock, mask, R, 9), to_edits(opts->edits), opts->temperature);
@@ -450,11 +481,10 @@ int capb200_aoa_decode_beam_diverse(capb200_aoa_engine* e, const float* att, con
     if (opts->group_size == 1) return capb200_aoa_decode_beam(e, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream);
     const int beam = opts->base.beam_size;
     CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= e->V1, "beam_size must be in 2..16 and <= V+1");
-    if (ensure_workspace(e, B, B * beam, R, beam, st)) return 1;
-    if (prepare(e, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
+    if (aoa_decode_workspace(e, B, B * beam, R, beam, st)) return 1;
+    if (aoa_decode_prepare(e, att, mask, B, R, st)) return 1;
     auto core = [&](int nrows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return core_step(e, nrows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
+        return aoa_decode_core(e, nrows, rpi, tokens, src_row, logits, ld, R, mask, st);
     };
     return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
                                       opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
@@ -480,11 +510,10 @@ int capb200_aoa_decode_sample(capb200_aoa_engine* e, const float* att, const flo
     const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : e->T;
     const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : e->T;
     CAPB_REQUIRE(steps >= 0 && steps <= t_out, "steps out of range");
-    if (ensure_workspace(e, B, rows, R, 1, st)) return 1;
-    if (prepare(e, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
+    if (aoa_decode_workspace(e, B, rows, R, 1, st)) return 1;
+    if (aoa_decode_prepare(e, att, mask, B, R, st)) return 1;
     auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return core_step(e, nrows, n, tokens, src_row, logits, ld, B, R, mask, st);
+        return aoa_decode_core(e, nrows, n, tokens, src_row, logits, ld, R, mask, st);
     };
     return sample_decode_driver(e->d, e->V1, e->T, rows, method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked,
                                 core, &e->launches, st, to_edits(opts->edits), opts->top);

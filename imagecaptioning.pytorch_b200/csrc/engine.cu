@@ -544,6 +544,41 @@ int check_ready(capb200_engine* e) {
 
 }  // namespace
 
+// ---- the decode pieces (engine_common.cuh) ----------------------------------------------------------------------------
+namespace capb200 {
+
+int lstm_member_info(capb200_engine* e, MemberInfo* m) {
+    if (check_ready(e)) return 1;
+    m->family = e->cfg.family;
+    m->V1 = e->V1; m->T = e->T;
+    m->attends = attends(e);
+    m->graph_ok = !e->profiling;
+    m->ws = e->ws; m->wblock = e->wblock;
+    m->fresh = e->d.neg1;
+    m->launches = &e->launches;
+    return 0;
+}
+
+// rows_per_image: the rows of one image in the first core call (NewFC feeds each row its image's embedding there)
+int lstm_decode_workspace(capb200_engine* e, int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) {
+    if (ensure_workspace(e, B, rows, R, beam, st)) return 1;
+    if (!attends(e)) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, rows_per_image); e->launches++; }
+    return 0;
+}
+
+int lstm_decode_prepare(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, cudaStream_t st) {
+    if (prepare(e, fc, att, mask, B, R, st)) return 1;
+    e->core_cur = 0;
+    return 0;
+}
+
+int lstm_decode_core(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int B, int R,
+                     const float* mask, cudaStream_t st) {
+    return core_step(e, rows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
+}
+
+}  // namespace capb200
+
 // =====================================================================================================================
 // C ABI
 // =====================================================================================================================
@@ -774,12 +809,10 @@ int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, co
     if (!attn) R = 1;
     const int T = e->T, V1 = e->V1;
     const int rows = B * beam;
-    if (ensure_workspace(e, B, rows, R, beam, st)) return 1;
-    if (!attn) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, 1); e->launches++; }
-    if (prepare(e, fc, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
+    if (lstm_decode_workspace(e, B, rows, R, beam, 1, st)) return 1;
+    if (lstm_decode_prepare(e, fc, att, mask, B, R, st)) return 1;
     auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return core_step(e, nrows, live, tokens, src_row, logits, ld, B, R, mask, st);
+        return lstm_decode_core(e, nrows, live, tokens, src_row, logits, ld, B, R, mask, st);
     };
     return beam_decode_driver(e->d, V1, T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
                               done_raw, core, &e->launches, st, e->profiling ? 0ull : loop_graph_key(e->ws, e->wblock, mask, R, (int)e->cfg.family),
@@ -799,11 +832,10 @@ int capb200_decode_beam_diverse(capb200_engine* e, const float* fc, const float*
     CAPB_REQUIRE(B >= 1, "empty batch");
     CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
     const int rows = B * beam;
-    if (ensure_workspace(e, B, rows, R, beam, st)) return 1;
-    if (prepare(e, fc, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
+    if (lstm_decode_workspace(e, B, rows, R, beam, 1, st)) return 1;      // attending families only: no NewFC row table
+    if (lstm_decode_prepare(e, fc, att, mask, B, R, st)) return 1;
     auto core = [&](int nrows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return core_step(e, nrows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
+        return lstm_decode_core(e, nrows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
     };
     return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
                                       opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
@@ -836,12 +868,10 @@ int capb200_decode_sample(capb200_engine* e, const float* fc, const float* att, 
     const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : T;
     const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : T;
     CAPB_REQUIRE(steps >= 0 && steps <= t_out, "steps out of range");
-    if (ensure_workspace(e, B, rows, R, 1, st)) return 1;
-    if (!attn) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, n); e->launches++; }
-    if (prepare(e, fc, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
+    if (lstm_decode_workspace(e, B, rows, R, 1, n, st)) return 1;
+    if (lstm_decode_prepare(e, fc, att, mask, B, R, st)) return 1;
     auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return core_step(e, nrows, n, tokens, src_row, logits, ld, B, R, mask, st);
+        return lstm_decode_core(e, nrows, n, tokens, src_row, logits, ld, B, R, mask, st);
     };
     return sample_decode_driver(e->d, V1, T, rows, method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked, core,
                                 &e->launches, st, to_edits(opts->edits), opts->top);

@@ -480,6 +480,33 @@ int sample_decode_driver(DecodeBuffers& d, int V1, int T, int rows, int method, 
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The three pieces every eval-mode decode of the LSTM engine (engine.cu) and the AoA engine (aoa_engine.cu) is built from: workspace sizing
+// for `rows` rows, the prologue (_prepare_feature) for B images, and one application of the recurrent core.  The single-model entry points
+// and the test-time ensemble (ensemble.cu) run the same three.
+// ---------------------------------------------------------------------------------------------------------------------
+struct MemberInfo {
+    int family = 0;                  // CAPB200_FAMILY_*
+    int V1 = 0, T = 0;
+    bool attends = true;             // reads the region features (NewFC reads the fc features only)
+    bool graph_ok = true;            // false while the engine times its GEMMs (per-launch events are not captured)
+    const void* ws = nullptr;        // workspace and weight block: what captured launches of the core read
+    const void* wblock = nullptr;
+    const int* fresh = nullptr;      // the engine's all -1 parent-row table: src_row of a fresh zero state
+    long* launches = nullptr;        // the engine's launch counter
+};
+
+int lstm_member_info(capb200_engine* e, MemberInfo* m);
+int lstm_decode_workspace(capb200_engine* e, int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st);
+int lstm_decode_prepare(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, cudaStream_t st);
+int lstm_decode_core(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int B, int R,
+                     const float* mask, cudaStream_t st);
+int aoa_member_info(capb200_aoa_engine* e, MemberInfo* m);
+int aoa_decode_workspace(capb200_aoa_engine* e, int B, int rows, int R, int beam, cudaStream_t st);
+int aoa_decode_prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, cudaStream_t st);
+int aoa_decode_core(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int R,
+                    const float* mask, cudaStream_t st);
+
 // Training-step GEMMs on the raw fp32 PyTorch weights (always current, no repack after optimizer steps).  With a Tf32Context (tensor-core
 // engines) every call runs on the wgmma tf32 3-pass kernel of gemm_tf32.cu; operands that are not K-major in HBM (W for the input
 // gradients, dY / X for the weight gradients) go through cached transposes.  Without a context (simt_fp32 engines), when an operand is not

@@ -1249,6 +1249,94 @@ class B200AoAModel(B200CaptionModel):
         return lib.capb200_aoa_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
 
 
+class B200AttEnsemble(B200CaptionModel):
+    """Drop-in for captioning.models.AttEnsemble.AttEnsemble (test-time ensemble, tools/eval_ensemble.py): ``models`` are engine models of
+    the UpDown, Att2in2, NewFC and AoANet families (any mix), ``weights`` a buffer that defaults to ``[1.0] * K``; vocab_size, seq_length and
+    bad_endings_ix come from ``models[0]``.  Every step mixes the members' word distributions into log(sum_k softmax(z_k) w_k / sum_k w_k)
+    (AttEnsemble.get_logprobs_state) on the device and decodes from that row: greedy and sampling ``forward(fc, att, masks, opt,
+    mode='sample')``, beam search (with ``done_beams``) and teacher forcing ``forward(fc, att, seq, masks)``, with the reference's shapes.
+
+    AttEnsemble skips AttModel.__init__, so the reference class lacks bos_idx / eos_idx / pad_idx / unk_idx / vocab, which its decode loops
+    and eval_split read; this mirror takes them from ``models[0]`` as well.  Eval only: diverse beam search, output_logsoftmax=0,
+    Transformer members and training raise NotImplementedError."""
+
+    family_name = 'AttEnsemble'
+    _no_diverse = 'an ensemble runs group_size 1 only'
+
+    def __init__(self, models, weights=None):
+        nn.Module.__init__(self)
+        models = list(models)
+        if not 1 <= len(models) <= _lib.ENSEMBLE_MAX_MEMBERS:
+            raise ValueError('an ensemble has 1..%d members (got %d)' % (_lib.ENSEMBLE_MAX_MEMBERS, len(models)))
+        for m in models:
+            if not isinstance(m, (B200UpDownModel, B200NewFCModel, B200AoAModel)):       # B200Att2in2Model is a B200UpDownModel
+                raise NotImplementedError('ensemble members are UpDown, Att2in2, NewFC or AoANet engine models (got %s)' % type(m).__name__)
+        m0 = models[0]
+        for m in models[1:]:
+            if m.vocab_size != m0.vocab_size or m.seq_length != m0.seq_length:
+                raise ValueError('every member needs the first member\'s vocab_size and seq_length (%d, %d); got (%d, %d)'
+                                 % (m0.vocab_size, m0.seq_length, m.vocab_size, m.seq_length))
+        weights = weights or [1.0] * len(models)
+        if len(weights) != len(models):
+            raise ValueError('one weight per member (%d members, %d weights)' % (len(models), len(weights)))
+        if any(not float(w) >= 0.0 or float(w) == float('inf') for w in weights) or not sum(float(w) for w in weights) > 0.0:
+            raise ValueError('ensemble weights must be finite, >= 0 and not all zero (got %r)' % (list(weights),))
+        self.models = nn.ModuleList(models)
+        self.vocab_size, self.seq_length, self.bad_endings_ix = m0.vocab_size, m0.seq_length, m0.bad_endings_ix
+        self.vocab, self.bos_idx, self.eos_idx, self.pad_idx, self.unk_idx = m0.vocab, m0.bos_idx, m0.eos_idx, m0.pad_idx, m0.unk_idx
+        self.numeric_mode = m0.numeric_mode
+        self.ss_prob = 0
+        self.register_buffer('weights', torch.tensor(weights))
+        self.done_beams = []
+        self._store = _EngineStore(self)
+
+    def _ensure_engine(self, device):
+        devices = {p.device for m in self.models for p in m.parameters()}
+        if devices != {device}:
+            raise ValueError('every ensemble member must live on the device of the inputs (%s); members are on %s' % (device, sorted(map(str, devices))))
+        if any(m.seq_length != self.seq_length or m.vocab_size != self.vocab_size for m in self.models):
+            raise ValueError('the ensemble decodes with its members\' vocab_size and seq_length: set max_length on every member, not on the ensemble')
+        weights = [float(w) for w in self.weights.tolist()]
+        if any(not w >= 0.0 or w == float('inf') for w in weights) or not sum(weights) > 0.0:
+            raise ValueError('ensemble weights must be finite, >= 0 and not all zero (got %r)' % weights)
+        for m in self.models:
+            m._ensure_engine(device)
+        members = (_lib.EnsembleMember * len(self.models))()
+        for k, (m, w) in enumerate(zip(self.models, weights)):
+            members[k].family = _lib.FAMILY_AOA if isinstance(m, B200AoAModel) else m.family
+            members[k].engine, members[k].weight = m._engine, w
+        lib = self._enter_device(device)
+        if self._engine is None:
+            self._engine = lib.capb200_ensemble_create()
+        self._members = members
+        return lib
+
+    def _free_engine(self, handle):
+        _lib.load().capb200_ensemble_destroy(handle)
+
+    @property
+    def launch_count(self) -> int:
+        return 0 if self._engine is None else int(_lib.load().capb200_ensemble_launch_count(self._engine))
+
+    def _call_sample(self, lib, fc, att, masks, B, R, so, tok, ld_tok, seq, logprobs):
+        return lib.capb200_ensemble_decode_sample(self._engine, self._members, len(self._members), _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R,
+                                                  ctypes.byref(so), _lib.ptr(tok), ld_tok, _lib.ptr(seq), _lib.ptr(logprobs), None, _lib.current_stream())
+
+    def _call_beam(self, lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw):
+        return lib.capb200_ensemble_decode_beam(self._engine, self._members, len(self._members), _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R,
+                                                ctypes.byref(bo), _lib.ptr(seq), _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p),
+                                                _lib.ptr(d_raw), _lib.current_stream())
+
+    def _call_record(self, lib, image, rank, dst):
+        return lib.capb200_ensemble_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
+
+    def scst_step(self, *args, **kwargs):
+        raise NotImplementedError('an ensemble is a test-time model: train its members')
+
+    def xe_step(self, *args, **kwargs):
+        raise NotImplementedError('an ensemble is a test-time model: train its members')
+
+
 def setup(opt, numeric_mode=None):
     """Factory with the contract of captioning.models.setup (captioning/models/__init__.py:20-73) for the families on the
     engine hot path."""

@@ -278,6 +278,37 @@ int capb200_aoa_decode_sample(capb200_aoa_engine* e, const float* att, const flo
 long capb200_aoa_launch_count(const capb200_aoa_engine* e);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Test-time ensemble (AttEnsemble, captioning/models/AttEnsemble.py): K members decode the same rows; every step mixes their word
+ * distributions into log( sum_k softmax(z_k) * w_k / sum_k w_k ) (get_logprobs_state :50-58) and searches / samples on that row exactly as
+ * a single model does on its log-probs.  Eval mode only; group_size 1.
+ * ---------------------------------------------------------------------------------------------------------------- */
+#define CAPB200_FAMILY_AOA 3              /* ensemble members only: `engine` is a capb200_aoa_engine */
+#define CAPB200_ENSEMBLE_MAX_MEMBERS 8
+typedef struct {
+    int family;       /* CAPB200_FAMILY_UPDOWN / NEWFC / ATT2IN2 (engine: capb200_engine*) or CAPB200_FAMILY_AOA (engine: capb200_aoa_engine*) */
+    void* engine;     /* bound; every member on the current device, with the first member's vocab_size and seq_length */
+    float weight;     /* >= 0, not all zero */
+} capb200_ensemble_member;
+/* Owns the ensemble's decode state: the [K, rows, V+1] member logits, beam records and the CUDA graph of the beam loop.  Member engines
+ * stay owned by the caller and may also decode on their own between ensemble calls. */
+typedef struct capb200_ensemble capb200_ensemble;
+capb200_ensemble* capb200_ensemble_create(void);
+void capb200_ensemble_destroy(capb200_ensemble* s);
+/* Same contract as capb200_decode_beam, over K = 1..CAPB200_ENSEMBLE_MAX_MEMBERS members.  fc may be NULL when no member reads it (AoA,
+ * Att2in2), att when none attends (NewFC only).  Members, K and weights are checked before any device work. */
+int capb200_ensemble_decode_beam(capb200_ensemble* s, const capb200_ensemble_member* members, int K, const float* fc, const float* att,
+                                 const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq, float* seq_logprobs,
+                                 long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream);
+/* done_beams[image][rank]['logps'] of the last capb200_ensemble_decode_beam call (contract of capb200_beam_record_logprobs) */
+int capb200_ensemble_beam_record_logprobs(capb200_ensemble* s, int image, int rank, float* dst, void* stream);
+/* Same contract as capb200_decode_sample: greedy, multinomial / top-k / nucleus sampling, forced replay and teacher forcing. */
+int capb200_ensemble_decode_sample(capb200_ensemble* s, const capb200_ensemble_member* members, int K, const float* fc, const float* att,
+                                   const float* mask, int B, int R, const capb200_sample_opts* opts, const long long* tokens_in, long ld_tok,
+                                   long long* seq, float* seq_logprobs, float* picked, void* stream);
+/* Kernel launches of the ensemble's decodes (its own and its members' on its behalf, replayed graph launches included). */
+long capb200_ensemble_launch_count(const capb200_ensemble* s);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * SCST reward and criterion
  * ---------------------------------------------------------------------------------------------------------------- */
 /* Document-frequency table in the scripts/prepro_ngrams.py format, flattened: keys[n,4] int32 token ids padded with -1,
