@@ -196,6 +196,7 @@ SIGNATURES = {
     'capb200_linear': (c_int, [c_void_p, c_long, c_void_p, c_long, c_void_p, c_void_p, c_long, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'capb200_bench_linear': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'capb200_gemm_tile_n': (c_int, [c_int, c_int]),
+    'capb200_gemm_tile_m': (c_int, [c_int, c_int]),
     'capb200_lstm_cell': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                   c_int, c_void_p]),
     'capb200_additive_attention': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

@@ -151,6 +151,7 @@ int gemm_simt_launch(const GemmProblem& p, cudaStream_t stream);
 struct GemmTcPlan;
 GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes);   // nullptr on failure (see last_error)
 int gemm_tc_tile_n(int M, int N);                                     // output-tile width the plan picks for an M x N problem
+int gemm_tc_tile_m(int M, int N, int bn);                             // output-tile height of an M-row launch of a plan of width bn
 void gemm_tc_plan_destroy(GemmTcPlan* plan);
 // Launch-time overrides: the whole epilogue (output pointers, biases, fused-LSTM state pointers change per decode step) and
 // M (rows actually valid, <= planned rows; 0 keeps).  The tensor maps keep the planned extents; rows beyond M are computed

@@ -1057,6 +1057,8 @@ int capb200_decode_gemm(const float* x, const float* w, int M, int N, int K, int
 
 int capb200_gemm_tile_n(int M, int N) { return gemm_tc_tile_n(M, N); }
 
+int capb200_gemm_tile_m(int M, int N) { return gemm_tc_tile_m(M, N, gemm_tc_tile_n(M, N)); }
+
 int capb200_lstm_cell(const float* x, int Kx, const float* h, const float* c, const float* w_ih, const float* w_hh, const float* b_ih,
                       const float* b_hh, float* h_out, float* c_out, int M, int H, int mode, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);

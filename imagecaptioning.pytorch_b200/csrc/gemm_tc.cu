@@ -19,11 +19,15 @@
 //                   row-bias / ReLU, fp32 store, optional split-fp16 copy for the next GEMM, or the fused LSTM cell) runs from registers
 //                   under the next tile's main loop; only a CTA's last epilogue is exposed.  The epilogue kind is a template parameter
 //                   (EpiKind), so each kernel carries the code of one kind only.
+// gemm_tc256_kernel is the cooperative schedule of the same roles over 256 x BN tiles (BN 128 or 160): both consumer warpgroups read
+// every stage, each its own 128 rows of A against the one W tile, so a K-block feeds twice the outputs for 1.4-1.5x the bytes.  At
+// three passes two stages fit.  gemm_tc_tile_m picks the schedule per launch.
 // On an H100 80GB HBM3 at a 400 W power limit, the ping-pong schedule and the vectorised LSTM stores take the UpDown decode step's LSTM
 // gate GEMMs from 3.34 to 3.02-3.06 ms (att_lstm) and 4.10-4.14 to 3.74-3.81 ms (lang_lstm) per batch; logit and h2att are unchanged
 // (DESIGN §5.1).
 // K-segments (up to 3 activation/weight pairs) are walked back to back so concatenated LSTM inputs are never built.
 #include <cstdlib>
+#include <cstring>
 
 #include "common.cuh"
 #include "ptx.cuh"
@@ -83,16 +87,20 @@ __device__ __forceinline__ unsigned long long gtimer() {
 // compiled in only for the TRACE = true instantiation (tools/gemm_trace.py): the production kernels carry no trace branches
 #define CAPB_TRACE(slot) do { if (TRACE && p.trace != nullptr) p.trace[(long)blockIdx.x * 16 + (slot)] = gtimer(); } while (0)
 
-template <int BN, int PASSES>
+// TM: rows of A per stage, BM for the ping-pong kernel and 2 * BM for the cooperative one (gemm_tc256_kernel)
+template <int BN, int PASSES, int TM = BM>
 struct TcCfg {
+    static constexpr int kTileM = TM;
+    static constexpr int kPasses = PASSES;
     static constexpr int kPlanes = (PASSES == 3) ? 2 : 1;
-    static constexpr uint32_t kABytes = BM * BK * 2;
+    static constexpr uint32_t kABytes = TM * BK * 2;
     static constexpr uint32_t kWBytes = BN * BK * 2;
     static constexpr uint32_t kStageBytes = kPlanes * (kABytes + kWBytes);
     static constexpr uint32_t kRingBudget = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/;   // per-block shared-memory limit
     static constexpr int kStages = kRingBudget / kStageBytes >= 8 ? 8 : kRingBudget / kStageBytes;
     static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
     static_assert(BN == 64 || BN == 128 || BN == 160, "wgmma wrappers exist for N = 64, 128 and 160");
+    static_assert(TM == BM || TM == 2 * BM, "one or two 128-row A boxes per plane");
     static_assert(kWBytes % 1024 == 0, "operand tiles must keep the 1024-byte swizzle-atom alignment");
     static_assert(kStages >= 2, "need at least a double buffer");
     static_assert(kSmemBytes <= 227 * 1024, "shared memory of one H100 block");
@@ -353,6 +361,88 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, float* acc, int
     else epi_store<BN, EPI == kEpiPlanes>(p, acc, r0, c0);
 }
 
+// Drains a warpgroup's 128 rows: rows 0..63 from acc0, then rows 64..127 moved into acc0, so the epilogue's code exists once, indexed
+// statically.  `slot` stamps the first 64 rows only.
+template <int BN, int EPI, bool TRACE>
+__device__ __forceinline__ void epilogue_rows128(const TcParams& p, float* acc0, const float* acc1, int m0, int n0, int tid, int slot) {
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+        epilogue_tile<BN, EPI, TRACE>(p, acc0, m0 + 64 * h, n0, tid, h == 0 ? slot : -1);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
+    }
+}
+
+// Set-up shared by both schedules (thread 0): the tensor maps prefetched, the ring's barriers initialised.  A stage's empty barrier
+// takes one arrival per warpgroup that reads the stage.
+template <int PASSES>
+__device__ __forceinline__ void init_ring(const TcParams& p, uint64_t* full_bar, uint64_t* empty_bar, int stages, int readers) {
+    for (int s = 0; s < p.nseg; ++s) {
+        ptx::prefetch_tmap(&p.a_hi[s]);
+        ptx::prefetch_tmap(&p.w_hi[s]);
+        if (PASSES == 3) {
+            ptx::prefetch_tmap(&p.a_lo[s]);
+            ptx::prefetch_tmap(&p.w_lo[s]);
+        }
+    }
+    for (int i = 0; i < stages; ++i) {
+        ptx::mbar_init(&full_bar[i], 1);
+        ptx::mbar_init(&empty_bar[i], readers);
+    }
+}
+
+// Producer: K-block kb of segment s into one stage, laid out [A_hi | A_lo | W_hi | W_lo] (the lo planes only for three passes).  A's
+// kTileM rows from m0 come as 128-row boxes (the plan's A maps serve both schedules), W's BN rows from n0 as one box.
+template <typename Cfg>
+__device__ __forceinline__ void fill_stage(const TcParams& p, uint8_t* st, uint64_t* bar, int s, int kb, int m0, int n0) {
+    uint8_t* a_hi = st;
+    uint8_t* a_lo = st + Cfg::kABytes;
+    uint8_t* w_hi = st + Cfg::kABytes * Cfg::kPlanes;
+    uint8_t* w_lo = w_hi + Cfg::kWBytes;
+    ptx::mbar_arrive_expect_tx(bar, Cfg::kStageBytes);
+#pragma unroll
+    for (int r = 0; r < Cfg::kTileM; r += BM) ptx::tma_load_2d(a_hi + r * BK * 2, &p.a_hi[s], bar, kb * BK, m0 + r);
+    ptx::tma_load_2d(w_hi, &p.w_hi[s], bar, kb * BK, n0);
+    if (Cfg::kPasses == 3) {
+#pragma unroll
+        for (int r = 0; r < Cfg::kTileM; r += BM) ptx::tma_load_2d(a_lo + r * BK * 2, &p.a_lo[s], bar, kb * BK, m0 + r);
+        ptx::tma_load_2d(w_lo, &p.w_lo[s], bar, kb * BK, n0);
+    }
+}
+
+// Consumer: one K-block of a warpgroup's 128 rows (two m64 halves of A at a_hi / a_lo, 128-byte swizzled rows) against the stage's W,
+// issued and retired.  Per k16 slice the same hi*lo, lo*hi, hi*hi order into each half (per element the sums of a 64-row warpgroup),
+// the halves alternating so that no wgmma waits on the accumulator of the one just before it.  Both schedules run exactly this, so
+// they give every output bit for bit the same value.  a_lo and w_lo are only read when PASSES == 3.
+template <int BN, int PASSES>
+__device__ __forceinline__ void mma_kblock(float* acc0, float* acc1, uint32_t a_hi, uint32_t a_lo, uint32_t w_hi, uint32_t w_lo) {
+    constexpr uint32_t kHalf = 64 * 128;                        // rows 64..127 of an A box: a whole number of swizzle atoms
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { ptx::reg_fence(acc0[i]); ptx::reg_fence(acc1[i]); }
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+        const uint32_t koff = k * 32;   // 16 fp16 = 32 bytes inside the 128-byte swizzle row
+        const uint64_t dwh = ptx::make_smem_desc_sw128(w_hi + koff);
+        if (PASSES == 3) {
+            const uint64_t dwl = ptx::make_smem_desc_sw128(w_lo + koff);
+            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwl, 1);
+            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwl, 1);
+            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_lo + koff), dwh, 1);
+            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_lo + kHalf + koff), dwh, 1);
+            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwh, 1);
+            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwh, 1);
+        } else {
+            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwh, 1);
+            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwh, 1);
+        }
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { ptx::reg_fence(acc0[i]); ptx::reg_fence(acc1[i]); }
+}
+
 // Persistent schedule: gridDim.x = min(tiles, SMs); CTA b walks tiles b, b + gridDim.x, ... in m-fastest order so that concurrently
 // running CTAs share the same weight columns (the W tile comes from HBM once, then from L2).
 //
@@ -373,18 +463,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int n_tiles = p.tiles_m * p.tiles_n;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.nseg; ++s) {
-            ptx::prefetch_tmap(&p.a_hi[s]);
-            ptx::prefetch_tmap(&p.w_hi[s]);
-            if (PASSES == 3) {
-                ptx::prefetch_tmap(&p.a_lo[s]);
-                ptx::prefetch_tmap(&p.w_lo[s]);
-            }
-        }
-        for (int i = 0; i < Cfg::kStages; ++i) {
-            ptx::mbar_init(&full_bar[i], 1);
-            ptx::mbar_init(&empty_bar[i], 1);                  // released by the one warpgroup that read the slot
-        }
+        init_ring<PASSES>(p, full_bar, empty_bar, Cfg::kStages, 1);   // a slot is read by one warpgroup
         for (int c = 0; c < kConsumers; ++c) ptx::mbar_init(&turn_bar[c], 1);
         ptx::fence_mbar_init();
     }
@@ -402,18 +481,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 for (int s = 0; s < p.nseg; ++s) {
                     for (int kb = 0; kb < p.kblocks[s]; ++kb) {
                         ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-                        uint8_t* st = smem + stage * Cfg::kStageBytes;
-                        uint8_t* a_hi = st;
-                        uint8_t* a_lo = st + Cfg::kABytes;
-                        uint8_t* w_hi = st + Cfg::kABytes * Cfg::kPlanes;
-                        uint8_t* w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;
-                        ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-                        ptx::tma_load_2d(a_hi, &p.a_hi[s], &full_bar[stage], kb * BK, m0);
-                        ptx::tma_load_2d(w_hi, &p.w_hi[s], &full_bar[stage], kb * BK, n0);
-                        if (PASSES == 3) {
-                            ptx::tma_load_2d(a_lo, &p.a_lo[s], &full_bar[stage], kb * BK, m0);
-                            ptx::tma_load_2d(w_lo, &p.w_lo[s], &full_bar[stage], kb * BK, n0);
-                        }
+                        fill_stage<Cfg>(p, smem + stage * Cfg::kStageBytes, &full_bar[stage], s, kb, m0, n0);
                         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
                     }
                 }
@@ -423,7 +491,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         ptx::setmaxnreg_inc<232>();
         const int cw = wg - 1;                                  // tile ordinals cw, cw + 2, ... of this CTA
         const int tid = threadIdx.x & 127;
-        constexpr uint32_t kHalf = 64 * 128;                    // rows 64..127 of an A box: a whole number of swizzle atoms
         int kb_tile = 0;
         for (int s = 0; s < p.nseg; ++s) kb_tile += p.kblocks[s];
         int mine = 0;                                           // tiles this warpgroup has run
@@ -444,36 +511,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     ptx::mbar_wait(&full_bar[stage], phase);
                     if (TRACE && it == 0 && s == 0 && kb == 0 && tid == 0) CAPB_TRACE(1);    // first operands landed
                     const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-                    const uint32_t a_hi = st;
-                    const uint32_t a_lo = st + Cfg::kABytes;                          // only valid when PASSES == 3
                     const uint32_t w_hi = st + Cfg::kABytes * Cfg::kPlanes;
-                    const uint32_t w_lo = st + Cfg::kABytes * 2 + Cfg::kWBytes;       // only valid when PASSES == 3
-#pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) { ptx::reg_fence(acc0[i]); ptx::reg_fence(acc1[i]); }
-                    ptx::wgmma_fence();
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint32_t koff = k * 32;   // 16 fp16 = 32 bytes inside the 128-byte swizzle row
-                        const uint64_t dwh = ptx::make_smem_desc_sw128(w_hi + koff);
-                        // the same hi*lo, lo*hi, hi*hi order into each half (per element the sums of a 64-row warpgroup), the halves
-                        // alternating so that no wgmma waits on the accumulator of the one just before it
-                        if (PASSES == 3) {
-                            const uint64_t dwl = ptx::make_smem_desc_sw128(w_lo + koff);
-                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwl, 1);
-                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwl, 1);
-                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_lo + koff), dwh, 1);
-                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_lo + kHalf + koff), dwh, 1);
-                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwh, 1);
-                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwh, 1);
-                        } else {
-                            wgmma_f16<BN>(acc0, ptx::make_smem_desc_sw128(a_hi + koff), dwh, 1);
-                            wgmma_f16<BN>(acc1, ptx::make_smem_desc_sw128(a_hi + kHalf + koff), dwh, 1);
-                        }
-                    }
-                    ptx::wgmma_commit();
-                    ptx::wgmma_wait<0>();
-#pragma unroll
-                    for (int i = 0; i < BN / 2; ++i) { ptx::reg_fence(acc0[i]); ptx::reg_fence(acc1[i]); }
+                    mma_kblock<BN, PASSES>(acc0, acc1, st, st + Cfg::kABytes, w_hi, w_hi + Cfg::kWBytes);
                     if (tid == 0) ptx::mbar_arrive(&empty_bar[stage]);                // the slot is free again
                     if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
                 }
@@ -481,15 +520,83 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             // Every thread of the warpgroup has waited on all of this tile's K-blocks (its wgmmas, issued by all 128, retired).
             if (tid == 0) ptx::mbar_arrive(&turn_bar[cw ^ 1]);
             if (TRACE && it < 2 && tid == 0) CAPB_TRACE(2 + it);                       // main loop of tile `it` done
-            // rows 0..63, then rows 64..127 moved into acc0: one copy of the epilogue's code, indexed statically
-#pragma unroll 1
-            for (int h = 0; h < 2; ++h) {
-                const int slot = (TRACE && it < 2 && h == 0 && tid == 0) ? 9 + 3 * it : -1;
-                epilogue_tile<BN, EPI, TRACE>(p, acc0, m0 + 64 * h, n0, tid, slot);
-#pragma unroll
-                for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i];
-            }
+            epilogue_rows128<BN, EPI, TRACE>(p, acc0, acc1, m0, n0, tid, (TRACE && it < 2 && tid == 0) ? 9 + 3 * it : -1);
             if (TRACE && it < 2 && tid == 0) CAPB_TRACE(6 + it);                       // epilogue of tile `it` done
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) CAPB_TRACE(8);                       // every role is done
+}
+
+// Cooperative schedule over 256 x BN output tiles (same persistent tile walk): both consumer warpgroups read every stage, warpgroup c
+// rows 128c .. 128c + 127 of the tile against the one W tile, so a K-block moves (256 + BN) rows of operands for 256 x BN outputs where
+// two 128-row tiles move 2 x (128 + BN).  The main loop is bound by that feed from L2, not by the tensor cores (DESIGN §6.1).  The two
+// warpgroups run their epilogues side by side, under only the producer's run-ahead into the next tile.
+// TRACE slots: 1 first operands landed, 5 the producer has issued tile 0's last K-block, 2 + c / 6 + c warpgroup c's main loop /
+// epilogue of tile 0 done, 9 + 3c .. 11 + 3c its LSTM stamps of rows 0..63.
+template <int BN, int PASSES, int EPI, bool TRACE = false>
+__global__ void __launch_bounds__(kThreads, 1) gemm_tc256_kernel(const __grid_constant__ TcParams p) {
+    using Cfg = TcCfg<BN, PASSES, 2 * BM>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+    uint64_t* empty_bar = full_bar + Cfg::kStages;
+
+    const int wg = threadIdx.x >> 7;
+    const int n_tiles = p.tiles_m * p.tiles_n;
+
+    if (threadIdx.x == 0) {
+        init_ring<PASSES>(p, full_bar, empty_bar, Cfg::kStages, kConsumers);   // a slot is read by both warpgroups
+        ptx::fence_mbar_init();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) CAPB_TRACE(0);                       // set-up done
+
+    if (wg == 0) {
+        ptx::setmaxnreg_dec<40>();
+        if (threadIdx.x == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+                const int m0 = (t % p.tiles_m) * Cfg::kTileM;
+                const int n0 = (t / p.tiles_m) * BN;
+                for (int s = 0; s < p.nseg; ++s) {
+                    for (int kb = 0; kb < p.kblocks[s]; ++kb) {
+                        ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+                        fill_stage<Cfg>(p, smem + stage * Cfg::kStageBytes, &full_bar[stage], s, kb, m0, n0);
+                        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+                    }
+                }
+                if (TRACE && t == (int)blockIdx.x) CAPB_TRACE(5);
+            }
+        }
+    } else {
+        ptx::setmaxnreg_inc<232>();
+        const int cw = wg - 1;                                  // rows 128 cw .. 128 cw + 127 of every tile
+        const int tid = threadIdx.x & 127;
+        const uint32_t a_rows = cw * BM * BK * 2;               // those rows inside each A plane of a stage
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int it = 0, t = blockIdx.x; t < n_tiles; ++it, t += gridDim.x) {
+            const int m0 = (t % p.tiles_m) * Cfg::kTileM + BM * cw;
+            const int n0 = (t / p.tiles_m) * BN;
+            float acc0[BN / 2], acc1[BN / 2];                   // rows 0..63 and 64..127 of the warpgroup's half
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+            for (int s = 0; s < p.nseg; ++s) {
+                for (int kb = 0; kb < p.kblocks[s]; ++kb) {
+                    ptx::mbar_wait(&full_bar[stage], phase);
+                    if (TRACE && it == 0 && s == 0 && kb == 0 && cw == 0 && tid == 0) CAPB_TRACE(1);    // first operands landed
+                    const uint32_t st = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
+                    const uint32_t w_hi = st + Cfg::kABytes * Cfg::kPlanes;
+                    mma_kblock<BN, PASSES>(acc0, acc1, st + a_rows, st + Cfg::kABytes + a_rows, w_hi, w_hi + Cfg::kWBytes);
+                    if (tid == 0) ptx::mbar_arrive(&empty_bar[stage]);                // this warpgroup is done with the slot
+                    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+                }
+            }
+            if (TRACE && it == 0 && tid == 0) CAPB_TRACE(2 + cw);                     // main loop of tile 0 done
+            epilogue_rows128<BN, EPI, TRACE>(p, acc0, acc1, m0, n0, tid, (TRACE && it == 0 && tid == 0) ? 9 + 3 * cw : -1);
+            if (TRACE && it == 0 && tid == 0) CAPB_TRACE(6 + cw);                     // epilogue of tile 0 done
         }
     }
     __syncthreads();
@@ -529,33 +636,45 @@ bool encode_plane(CUtensorMap* map, const __half* base, long rows, long K, long 
     return true;
 }
 
-template <int BN, int PASSES, int EPI, bool TRACE = false>
+// TM = BM: the ping-pong gemm_tc_kernel; TM = 2 * BM: the cooperative gemm_tc256_kernel (BN 128 and 160 only)
+template <int BN, int PASSES, int EPI, bool TRACE, int TM>
 int launch_cfg(const TcParams& prm, cudaStream_t stream) {
-    using Cfg = TcCfg<BN, PASSES>;
+    using Cfg = TcCfg<BN, PASSES, TM>;
+    void (*kernel)(TcParams);
+    if constexpr (TM == BM) kernel = gemm_tc_kernel<BN, PASSES, EPI, TRACE>;
+    else kernel = gemm_tc256_kernel<BN, PASSES, EPI, TRACE>;
     static std::atomic<unsigned long long> attr_set{0};
     if (first_use_on_device(attr_set)) {
-        CAPB_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, PASSES, EPI, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        CAPB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     }
     TcParams prm2 = prm;
     prm2.tiles_n = cdiv(prm.N, BN);
-    prm2.tiles_m = cdiv(prm.M, BM);
+    prm2.tiles_m = cdiv(prm.M, TM);
     const int n_tiles = prm2.tiles_n * prm2.tiles_m;
     const int sms = sm_count();
-    gemm_tc_kernel<BN, PASSES, EPI, TRACE><<<n_tiles < sms ? n_tiles : sms, kThreads, Cfg::kSmemBytes, stream>>>(prm2);
+    kernel<<<n_tiles < sms ? n_tiles : sms, kThreads, Cfg::kSmemBytes, stream>>>(prm2);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-// kind x BN x passes, plus the traced 3-pass kernels (capb200_decode_gemm with a trace buffer)
-template <int EPI>
-int launch_kind(int bn, int passes, const TcParams& prm, cudaStream_t stream) {
+// BN x passes of one schedule, plus the traced 3-pass kernels (capb200_decode_gemm with a trace buffer)
+template <int EPI, int TM>
+int launch_width(int bn, int passes, const TcParams& prm, cudaStream_t stream) {
     if (prm.trace != nullptr) {
-        if (bn == 160) return launch_cfg<160, 3, EPI, true>(prm, stream);
-        return bn == 128 ? launch_cfg<128, 3, EPI, true>(prm, stream) : launch_cfg<64, 3, EPI, true>(prm, stream);
+        if (bn == 160) return launch_cfg<160, 3, EPI, true, TM>(prm, stream);
+        if constexpr (TM == BM) if (bn == 64) return launch_cfg<64, 3, EPI, true, TM>(prm, stream);
+        return launch_cfg<128, 3, EPI, true, TM>(prm, stream);
     }
-    if (bn == 160) return passes == 3 ? launch_cfg<160, 3, EPI>(prm, stream) : launch_cfg<160, 1, EPI>(prm, stream);
-    if (bn == 128) return passes == 3 ? launch_cfg<128, 3, EPI>(prm, stream) : launch_cfg<128, 1, EPI>(prm, stream);
-    return passes == 3 ? launch_cfg<64, 3, EPI>(prm, stream) : launch_cfg<64, 1, EPI>(prm, stream);
+    if (bn == 160) return passes == 3 ? launch_cfg<160, 3, EPI, false, TM>(prm, stream) : launch_cfg<160, 1, EPI, false, TM>(prm, stream);
+    if constexpr (TM == BM) {
+        if (bn == 64) return passes == 3 ? launch_cfg<64, 3, EPI, false, TM>(prm, stream) : launch_cfg<64, 1, EPI, false, TM>(prm, stream);
+    }
+    return passes == 3 ? launch_cfg<128, 3, EPI, false, TM>(prm, stream) : launch_cfg<128, 1, EPI, false, TM>(prm, stream);
+}
+
+template <int EPI>
+int launch_kind(int bm, int bn, int passes, const TcParams& prm, cudaStream_t stream) {
+    return bm == 2 * BM ? launch_width<EPI, 2 * BM>(bn, passes, prm, stream) : launch_width<EPI, BM>(bn, passes, prm, stream);
 }
 
 }  // namespace
@@ -607,6 +726,24 @@ int gemm_tc_tile_n(int M, int N) {
     return cost160 < cost128 ? 160 : 128;
 }
 
+// Tile height of one launch: M rows (the launch's own, which may be fewer than the plan's) on a plan of width bn.  The main loop is fed,
+// not computed (DESIGN §6.1): a K-block moves (BM + BN) rows of operands into a CTA, so 256-row tiles move 28 % (BN 160) or 25 %
+// (BN 128) fewer bytes per output than 128-row ones.  But the cooperative schedule exposes the epilogue of every tile a CTA runs, where
+// the ping-pong one exposes only the last.  So 256 rows are taken where they fit the launch in one wave and 128 rows would need more:
+// there both expose one epilogue per CTA (the 1280 x 4000 LSTM gates of the decode step).  Where 256-row tiles take several waves (logit,
+// att_embed) or 128-row ones already take one (the t = 0 gate launches of 256 rows, the few-row baseline launches), the ping-pong
+// schedule measured faster (tools/decode_gemm_rate.py, DESIGN §6.1).  BN 64 has no 256-row kernel.  CAPB200_GEMM_BM=128 or 256 forces
+// a height for A/B timing and tests; it is read at every call, so a process can switch it between launches.
+int gemm_tc_tile_m(int M, int N, int bn) {
+    if (bn == 64) return BM;
+    const char* force = getenv("CAPB200_GEMM_BM");
+    if (force != nullptr && strcmp(force, "128") == 0) return BM;
+    if (force != nullptr && strcmp(force, "256") == 0) return 2 * BM;
+    const int sms = sm_count();
+    const int tiles_n = cdiv(N, bn);
+    return cdiv(M, 2 * BM) * tiles_n <= sms && cdiv(M, BM) * tiles_n > sms ? 2 * BM : BM;
+}
+
 GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes) {
     std::string why;
     if (!gemm_tc_supported(p, &why)) { set_error("gemm_tc: unsupported problem: " + why); return nullptr; }
@@ -639,12 +776,11 @@ GemmTcPlan* gemm_tc_plan_create(const GemmProblem& p, int passes) {
 void gemm_tc_plan_destroy(GemmTcPlan* plan) { delete plan; }
 
 int gemm_tc_plan_launch(GemmTcPlan* plan, const GemmEpilogue* epi_override, int M_override, cudaStream_t stream) {
+    if (M_override > plan->prm.M) { set_error("gemm_tc: M override exceeds the planned row count"); return 1; }
+    const int M = M_override > 0 ? M_override : plan->prm.M;
     TcParams prm = plan->prm;
     if (epi_override != nullptr) fill_epilogue(prm, *epi_override);
-    if (M_override > 0) {
-        if (M_override > prm.M) { set_error("gemm_tc: M override exceeds the planned row count"); return 1; }
-        prm.M = M_override;
-    }
+    prm.M = M;
     if (prm.lstm && (prm.N != 4 * prm.H || prm.c_out == nullptr || prm.h_f == nullptr)) {
         set_error("gemm_tc: fused LSTM epilogue needs N == 4H, c_out and h_f");
         return 1;
@@ -653,9 +789,10 @@ int gemm_tc_plan_launch(GemmTcPlan* plan, const GemmEpilogue* epi_override, int 
     // the kind follows the epilogue this launch asks for: launches override the planned one whole
     const int kind = prm.lstm ? kEpiLstm : prm.C_hi != nullptr ? kEpiPlanes : kEpiStore;
     if (prm.trace != nullptr && plan->passes != 3) { set_error("gemm_tc: the traced kernel is the 3-pass one"); return 1; }
-    if (kind == kEpiLstm) return launch_kind<kEpiLstm>(plan->bn, plan->passes, prm, stream);
-    if (kind == kEpiPlanes) return launch_kind<kEpiPlanes>(plan->bn, plan->passes, prm, stream);
-    return launch_kind<kEpiStore>(plan->bn, plan->passes, prm, stream);
+    const int bm = gemm_tc_tile_m(prm.M, prm.N, plan->bn);            // per launch: M may be fewer rows than planned
+    if (kind == kEpiLstm) return launch_kind<kEpiLstm>(bm, plan->bn, plan->passes, prm, stream);
+    if (kind == kEpiPlanes) return launch_kind<kEpiPlanes>(bm, plan->bn, plan->passes, prm, stream);
+    return launch_kind<kEpiStore>(bm, plan->bn, plan->passes, prm, stream);
 }
 
 }  // namespace capb200

@@ -63,6 +63,9 @@ int capb200_bench_linear(const float* x, const float* w, const float* b, float* 
 
 /* Diagnostics: the output-tile width (64, 128 or 160 columns) the tc_f16x3 / tc_f16x1 GEMM picks for an M x N problem on the current device. */
 int capb200_gemm_tile_n(int M, int N);
+/* The output-tile height (128 or 256 rows) the same GEMM picks for an M x N problem; CAPB200_GEMM_BM=128 or 256 in the environment forces
+ * it where the tile width has a kernel of that height. */
+int capb200_gemm_tile_m(int M, int N);
 
 /* nn.LSTMCell: gates = x*w_ih^T + b_ih + h*w_hh^T + b_hh; (i,f,g,o)           AttModel.py:628,635
  * x[M,Kx], h/c[M,H] -> h_out/c_out[M,H] */

@@ -53,12 +53,18 @@ L.check(lib.capb200_decode_gemm(L.ptr(x), L.ptr(w), M, N, K, L.OP_MODES['tc_f16x
 used = tr[:, 0] > 0
 t = tr[used].astype(np.float64)
 t0 = t[:, 0].min()
-names = ['set-up done', 'first operands landed', 'tile 0: main loop done', 'tile 1: main loop done', 'tile 1: main loop starts', '(unused)',
-         'tile 0: epilogue done', 'tile 1: epilogue done', 'kernel end',
-         'tile 0 lstm: c_prev landed', 'tile 0 lstm: cell math done', 'tile 0 lstm: stores issued',
-         'tile 1 lstm: c_prev landed', 'tile 1 lstm: cell math done', 'tile 1 lstm: stores issued']
-print('decode GEMM %d x %d x %d, %s epilogue, BN %d, %d CTAs traced; times in us after the first CTA finished its set-up'
-      % (M, N, K, args.epilogue, lib.capb200_gemm_tile_n(M, N), int(used.sum())))
+BM = lib.capb200_gemm_tile_m(M, N)    # CAPB200_GEMM_BM=128 / 256 picks the schedule to trace
+if BM == 128:   # ping-pong: warpgroup 1 runs tile 0, warpgroup 2 tile 1
+    part = ['tile 0', 'tile 1']
+    names = ['set-up done', 'first operands landed', 'tile 0: main loop done', 'tile 1: main loop done', 'tile 1: main loop starts', '(unused)',
+             'tile 0: epilogue done', 'tile 1: epilogue done', 'kernel end']
+else:           # cooperative: both warpgroups run rows 0..127 / 128..255 of tile 0
+    part = ['warpgroup 1', 'warpgroup 2']
+    names = ['set-up done', 'first operands landed', 'warpgroup 1: tile 0 main loop done', 'warpgroup 2: tile 0 main loop done', '(unused)',
+             'producer: tile 0 last K-block issued', 'warpgroup 1: tile 0 epilogue done', 'warpgroup 2: tile 0 epilogue done', 'kernel end']
+names += ['%s lstm: %s' % (w, s) for w in part for s in ('c_prev landed', 'cell math done', 'stores issued')]
+print('decode GEMM %d x %d x %d, %s epilogue, BM %d, BN %d, %d CTAs traced; times in us after the first CTA finished its set-up'
+      % (M, N, K, args.epilogue, BM, lib.capb200_gemm_tile_n(M, N), int(used.sum())))
 for i, n in enumerate(names):
     col = t[:, i]
     col = col[col > 0]
@@ -72,7 +78,7 @@ if lead.size:
     epi0 = (lead[:, 6] - lead[:, 2]) / 1e3
     print('epilogue of tile 0: median %.2f us, max %.2f us' % (np.median(epi0), epi0.max()))
     two = lead[lead[:, 3] > 0]
-    if two.size:
+    if two.size and BM == 128:
         d12 = (two[:, 3] - two[:, 2]) / 1e3
         epi1 = (two[:, 7] - two[:, 3]) / 1e3
         print('CTAs with two tiles: tile 0 main loop -> tile 1 main loop: median %.2f us; epilogue of tile 1: median %.2f us, max %.2f us'
@@ -80,10 +86,10 @@ if lead.size:
         hidden = two[:, 6] <= two[:, 3]
         print('tile 0 epilogue ended before tile 1 main loop did: %d of %d CTAs' % (int(hidden.sum()), len(two)))
     if args.epilogue == 'lstm':
-        for tile, (done, first) in enumerate([(2, 9), (3, 12)]):
+        for who, (done, first) in zip(part, [(2, 9), (3, 12)]):
             r = lead[(lead[:, done] > 0) & (lead[:, first + 2] > 0)]
             if r.size == 0:
                 continue
             parts = [(r[:, first] - r[:, done]) / 1e3, (r[:, first + 1] - r[:, first]) / 1e3, (r[:, first + 2] - r[:, first + 1]) / 1e3]
-            print('tile %d lstm epilogue, rows 0..63, median (max) us: adds + c_prev loads %.2f (%.2f), cell math %.2f (%.2f), stores %.2f (%.2f)'
-                  % ((tile,) + tuple(v for q in parts for v in (np.median(q), q.max()))))
+            print('%s lstm epilogue, its first 64 rows, median (max) us: adds + c_prev loads %.2f (%.2f), cell math %.2f (%.2f), stores %.2f (%.2f)'
+                  % ((who,) + tuple(v for q in parts for v in (np.median(q), q.max()))))
