@@ -202,6 +202,9 @@ SIGNATURES = {
     'capb200_additive_attention': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                            c_void_p]),
     'capb200_log_softmax_topk': (c_int, [c_void_p, c_long, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    'capb200_vocab_stats_topk': (c_int, [c_void_p, c_long, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_vocab_select': (c_int, [c_void_p, c_long, c_int, c_int, c_int, c_float, c_float, c_ulonglong, c_ulonglong, c_void_p, c_int, c_void_p,
+                                     c_void_p, c_void_p]),
     'capb200_engine_create': (c_void_p, [POINTER(ModelCfg)]),
     'capb200_engine_destroy': (None, [c_void_p]),
     'capb200_engine_bind_weights': (c_int, [c_void_p, POINTER(Weights), c_void_p]),

@@ -1103,6 +1103,32 @@ int capb200_log_softmax_topk(float* logits, long ld, int rows, int V1, int twice
     return vocab_step_launch(va, static_cast<cudaStream_t>(stream));
 }
 
+int capb200_vocab_stats_topk(const float* logits, long ld, int rows, int V1, int twice, int k, float* stats, float* top_val, int* top_idx, void* stream) {
+    CAPB_REQUIRE(logits != nullptr && stats != nullptr && top_val != nullptr && top_idx != nullptr, "null argument");
+    CAPB_REQUIRE(rows > 0 && V1 > 0 && ld >= V1 && k > 0, "bad argument");
+    CAPB_REQUIRE((reinterpret_cast<uintptr_t>(stats) & 7) == 0, "stats must be 8-byte aligned");
+    VocabStepArgs va;
+    va.rows = rows; va.V1 = V1; va.logits = const_cast<float*>(logits); va.ld = ld; va.twice = twice;      // stats mode only reads the rows
+    va.topk = k; va.top_val = top_val; va.top_idx = top_idx;
+    va.stats = reinterpret_cast<float2*>(stats);
+    return vocab_step_launch(va, static_cast<cudaStream_t>(stream));
+}
+
+int capb200_vocab_select(float* logits, long ld, int rows, int V1, int select, float top, float temperature, unsigned long long seed,
+                         unsigned long long step, int* unfinished, int first_step, int* tokens_out, float* picked_lp, void* stream) {
+    CAPB_REQUIRE(logits != nullptr && tokens_out != nullptr && picked_lp != nullptr, "null argument");
+    CAPB_REQUIRE(rows > 0 && V1 > 0 && ld >= V1, "bad argument");
+    CAPB_REQUIRE(select == 1 || select == 2 || select == 4 || select == 5, "select must be 1 (greedy), 2 (multinomial), 4 (top-k) or 5 (nucleus)");
+    CAPB_REQUIRE(temperature > 0.f, "temperature must be positive");
+    CAPB_REQUIRE(select != 4 || top >= 1.f, "top-k sampling needs k >= 1");
+    CAPB_REQUIRE(select != 5 || (top > 0.f && top <= 1.f), "nucleus sampling needs 0 < p <= 1");
+    VocabStepArgs va;
+    va.rows = rows; va.V1 = V1; va.logits = logits; va.ld = ld;
+    va.select = select; va.top = top; va.temperature = temperature; va.seed = seed; va.step = step;
+    va.unfinished = unfinished; va.first_step = first_step; va.tokens_out = tokens_out; va.picked_lp = picked_lp;
+    return vocab_step_launch(va, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 
 // =====================================================================================================================

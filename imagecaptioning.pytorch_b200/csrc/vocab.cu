@@ -345,6 +345,25 @@ __global__ void __launch_bounds__(VT) vocab_stats_kernel(const VocabStepArgs a) 
     }
 }
 
+// Per-thread online softmax in base 2 (the single-pass kernels below).  A thread's partial sum holds sum 2^(x*log2e - mL), where
+// mL = fl(m*log2e) belongs to its running maximum m.  mL carries the rounding of that product -- up to half an ulp of |m|*log2e, 1e-4 at
+// |m| = 1000 -- so the rescale to a new maximum and the final rescale to the row maximum are both taken against mL itself, not against m:
+// the rounding then cancels and the log-sum-exp does not degrade with the magnitude of the logits (log_softmax is shift-invariant).
+__device__ __forceinline__ void online_raise(float& part, float& m, float& mL, float m4) {
+    const float nL = m4 * 1.4426950408889634f;
+    float sc;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"(mL - nL));
+    part = (m == -INFINITY) ? 0.f : part * sc;      // a thread that has only seen -inf holds NaN (-inf - -inf), not a sum
+    m = m4;
+    mL = nL;
+}
+// the thread's share of sum exp(x - mx), mx = the row maximum
+__device__ __forceinline__ float online_finish(float part, float m, float mL, float mx) {
+    float sc;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"(fmaf(-mx, 1.4426950408889634f, mL)));
+    return (m == -INFINITY) ? 0.f : part * sc;
+}
+
 // Single-pass variant of vocab_stats_kernel (one CTA per row, loads straight from global memory, 8 CTAs per SM): per-thread online
 // softmax (running max, partial sum rescaled when the max grows) and one max-of-four test in front of the top-2 bookkeeping, so the
 // row is read once and the common path is ~5 instructions per element.
@@ -362,11 +381,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_online_kernel(const VocabStepA
         const float4 x = g4[v];
         const float m4 = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
         if (m4 > m) {
-            float sc;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"((m - m4) * kL2E));
-            part = (m == -INFINITY) ? 0.f : part * sc;
-            m = m4;
-            mL = m4 * kL2E;
+            online_raise(part, m, mL, m4);
         }
         float e0, e1, e2, e3;
         asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(x.x, kL2E, -mL)));
@@ -386,7 +401,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_online_kernel(const VocabStepA
         }
     }
     const float mx = block_max(m, s_red);
-    float sum = (m == -INFINITY) ? 0.f : part * __expf(m - mx);
+    float sum = online_finish(part, m, mL, mx);
     sum = block_sum(sum, s_red);
     const float lsum = logf(sum);
     const float m2 = (mx - mx) - lsum, l2 = lsum;
@@ -472,11 +487,7 @@ __global__ void __launch_bounds__(VT2) vocab_stats_online128_kernel(const VocabS
     auto consume = [&](const float4 x, int v) {
         const float m4 = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
         if (m4 > m) {
-            float sc;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"((m - m4) * kL2E));
-            part = (m == -INFINITY) ? 0.f : part * sc;
-            m = m4;
-            mL = m4 * kL2E;
+            online_raise(part, m, mL, m4);
         }
         float e0, e1, e2, e3;
         asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(x.x, kL2E, -mL)));
@@ -502,7 +513,7 @@ __global__ void __launch_bounds__(VT2) vocab_stats_online128_kernel(const VocabS
     }
     for (; v < n4; v += VT2) consume(g4[v], v);
     const float mx = block_max4(m, s_red);
-    float sum = (m == -INFINITY) ? 0.f : part * __expf(m - mx);
+    float sum = online_finish(part, m, mL, mx);
     sum = block_sum4(sum, s_red);
     const float lsum = logf(sum);
     const float m2 = (mx - mx) - lsum, l2 = lsum;
@@ -649,11 +660,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_stream_kernel(const VocabStepA
             const float4 x = g4[v];
             const float m4 = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
             if (m4 > m) {
-                float sc;
-                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"((m - m4) * kL2E));
-                part = (m == -INFINITY) ? 0.f : part * sc;
-                m = m4;
-                mL = m4 * kL2E;
+                online_raise(part, m, mL, m4);
             }
             float e0, e1, e2, e3;
             asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(x.x, kL2E, -mL)));
@@ -673,7 +680,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_stream_kernel(const VocabStepA
             }
         }
         const float mx = block_max(m, s_red);
-        float sum = (m == -INFINITY) ? 0.f : part * __expf(m - mx);
+        float sum = online_finish(part, m, mL, mx);
         sum = block_sum(sum, s_red);
         const float lsum = logf(sum);
         const float m2 = (mx - mx) - lsum, l2 = lsum;

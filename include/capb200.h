@@ -81,6 +81,21 @@ int capb200_additive_attention(const float* att_h, const float* p_att, const flo
  * the per-row top-k (values and indices, descending, lowest index first on ties). top_val/top_idx may be NULL if k == 0. */
 int capb200_log_softmax_topk(float* logits, long ld, int rows, int V1, int twice, int k, float* top_val, int* top_idx, void* stream);
 
+/* Beam search's form of the same step: logits[rows,V1] (pitch ld) are only read; stats[rows,2] receives each row's maximum and
+ * log(sum(exp(x - max))), top_val/top_idx[rows,k] the k best log-probs (normalised a second time if twice != 0) and their columns,
+ * ranked on the raw logits (descending, lowest index first on ties), 1 <= k <= 16.  A row with fewer than k entries above -inf
+ * fills the rest with value -inf and index 0x7fffffff or a column that holds -inf. */
+int capb200_vocab_stats_topk(const float* logits, long ld, int rows, int V1, int twice, int k, float* stats, float* top_val, int* top_idx,
+                             void* stream);
+
+/* The word choice of _sample (CaptionModel.py:366-406) on one step's logits[rows,V1] (pitch ld), which are overwritten with their
+ * log_softmax.  select: 1 greedy, 2 multinomial, 4 top-k (top = k), 5 nucleus (top = p); the sampled kinds draw from
+ * softmax(log-probs / temperature) over the kept words with one Philox block per (word, row, step, seed).  tokens_out[rows] gets the
+ * word, picked_lp[rows] its log-prob.  unfinished[rows] (or NULL): unless first_step != 0, a row whose flag is 0 emits word 0, log-prob 0
+ * and an all-zero row; the flag is rewritten to word != 0. */
+int capb200_vocab_select(float* logits, long ld, int rows, int V1, int select, float top, float temperature, unsigned long long seed,
+                         unsigned long long step, int* unfinished, int first_step, int* tokens_out, float* picked_lp, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Engine level
  * ---------------------------------------------------------------------------------------------------------------- */

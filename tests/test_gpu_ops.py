@@ -174,21 +174,33 @@ def test_additive_attention(L, rpi, masked, B, A, H):
     assert float((out.cpu() - ref).abs().max()) < (5e-6 if A <= 64 else 3e-5)
 
 
-@pytest.mark.parametrize('V1,twice,k', [(61, 0, 3), (9488, 1, 5), (9488, 0, 10), (1000, 1, 1)])
-def test_log_softmax_topk(L, V1, twice, k):
+@pytest.mark.parametrize('V1,twice,k,case', [(61, 0, 3, 'dense'), (9488, 1, 5, 'dense'), (9488, 0, 10, 'dense'), (1000, 1, 1, 'dense'),
+                                            (9488, 1, 16, 'dense'), (9488, 1, 5, 'pitched'), (9488, 1, 16, 'owned')],
+                         ids=['61-0-3', '9488-1-5', '9488-0-10', '1000-1-1', '9488-1-16', '9488-1-5-pitched', '9488-1-16-owned'])
+def test_log_softmax_topk(L, V1, twice, k, case):
+    """'pitched': the rows sit in a slab of pitch V1 + 4 whose other columns hold 1e30 and must be neither read nor written.
+    'owned': in every row the k best all belong to one thread of the 256-thread kernel (columns congruent modulo 256)."""
     g = torch.Generator().manual_seed(V1 + k)
     rows = 17
     x = torch.randn(rows, V1, generator=g) * 4
+    if case == 'owned':
+        for r in range(rows):
+            cols = torch.arange(r * 13 % 256, V1, 256)[torch.randperm(V1 // 256, generator=g)[:k]]
+            x[r, cols] = 20.0 + 0.5 * torch.randperm(k, generator=g).float()
     ref = torch.log_softmax(x, 1)
     if twice:
         ref = torch.log_softmax(ref, 1)
     tv, ti = ref.topk(k, dim=1)
-    xd = x.cuda()
+    ld = V1 + 4 if case == 'pitched' else V1
+    slab = torch.full((rows, ld), 1e30, device='cuda')
+    slab[:, :V1] = x.cuda()
+    xd = slab[:, :V1]
     top_val = torch.empty(rows, k, device='cuda')
     top_idx = torch.empty(rows, k, dtype=torch.int32, device='cuda')
-    L.check(L.load().capb200_log_softmax_topk(L.ptr(xd), V1, rows, V1, twice, k, L.ptr(top_val), L.ptr(top_idx), L.current_stream()), 'log_softmax_topk')
+    L.check(L.load().capb200_log_softmax_topk(L.ptr(xd), ld, rows, V1, twice, k, L.ptr(top_val), L.ptr(top_idx), L.current_stream()), 'log_softmax_topk')
     torch.cuda.synchronize()
     assert float((xd.cpu() - ref).abs().max()) < 1e-5
+    assert bool((slab[:, V1:] == 1e30).all())
     assert np.array_equal(top_idx.cpu().numpy(), ti.numpy().astype(np.int32))
     assert float((top_val.cpu() - tv).abs().max()) < 1e-5
 
