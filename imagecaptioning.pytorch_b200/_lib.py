@@ -162,6 +162,10 @@ class TfmScstOpts(Structure):
                 ('row_loss', c_void_p), ('reward_weights', POINTER(RewardWeights))]
 
 
+class VjpOpts(Structure):
+    _fields_ = [('forward_only', c_int), ('dlogprobs', c_void_p), ('greedy', c_int)]
+
+
 AOA_REFINER_LAYERS = 6
 
 
@@ -283,6 +287,28 @@ SIGNATURES = {
     'capb200_reward_criterion_forward': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'capb200_reward_criterion_backward': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_void_p]),
     'capb200_decode_gemm': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(GemmEpilogue), c_void_p, c_int, c_void_p]),
+    # autograd entry points: (engine, [fc,] att, B, R, opts, vjp, labels, label_cols, grads, logprobs, stream) /
+    #                        (engine, [fc,] att, B, R, opts, vjp, grads, sample_seq, sample_logprobs, stream)
+    'capb200_updown_xe_vjp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), POINTER(VjpOpts), c_void_p, c_int,
+                                      POINTER(UpdownGrads), c_void_p, c_void_p]),
+    'capb200_updown_scst_vjp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), POINTER(VjpOpts), POINTER(UpdownGrads),
+                                        c_void_p, c_void_p, c_void_p]),
+    'capb200_att2in2_xe_vjp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), POINTER(VjpOpts), c_void_p, c_int,
+                                       POINTER(Att2in2Grads), c_void_p, c_void_p]),
+    'capb200_att2in2_scst_vjp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), POINTER(VjpOpts), POINTER(Att2in2Grads),
+                                         c_void_p, c_void_p, c_void_p]),
+    'capb200_newfc_xe_vjp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(XeOpts), POINTER(VjpOpts), c_void_p, c_int,
+                                     POINTER(NewfcGrads), c_void_p, c_void_p]),
+    'capb200_newfc_scst_vjp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), POINTER(VjpOpts), POINTER(NewfcGrads),
+                                       c_void_p, c_void_p, c_void_p]),
+    'capb200_aoa_xe_vjp': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(AoaXeOpts), POINTER(VjpOpts), c_void_p, c_int, POINTER(AoaWeights),
+                                   c_void_p, c_void_p]),
+    'capb200_aoa_scst_vjp': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(AoaScstOpts), POINTER(VjpOpts), POINTER(AoaWeights), c_void_p,
+                                     c_void_p, c_void_p]),
+    'capb200_tfm_xe_vjp': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmXeOpts), POINTER(VjpOpts), c_void_p, c_int, POINTER(TfmWeights),
+                                   c_void_p, c_void_p]),
+    'capb200_tfm_scst_vjp': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmScstOpts), POINTER(VjpOpts), POINTER(TfmWeights), c_void_p,
+                                     c_void_p, c_void_p]),
 }
 
 _lib = None

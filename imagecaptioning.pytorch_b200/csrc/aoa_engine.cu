@@ -574,7 +574,6 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
     const float keep_lm = 1.0f / (1.0f - p_lm);
     const unsigned long long seed = ta.seed;
     const capb200_aoa_weights& w = e->w;
-    const capb200_aoa_grads& G = *grads;
     const long BR = (long)B * R, NH = (long)N * H, TN = (long)T * N;
     const long ld_lp = (long)ta.Tl * V1;
 
@@ -661,7 +660,9 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
 
     // ---- (4) reward and loss, (5) backward through the decoder, starting with the logit layer (group 0)
     nvtxRangePop();
+    if (ta.forward_only) return 0;
     CAPB_NVTX("capb200 aoa train step: reward, loss, backward, weight gradients");
+    const capb200_aoa_grads& G = *grads;
     if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.outd, tp.dOUTD, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dctx, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
@@ -792,4 +793,37 @@ extern "C" int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int 
     ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_eager_step(st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
+}
+
+// The autograd entry points (include/capb200.h: capb200_vjp_opts) on AoANet's option structs.
+extern "C" int capb200_aoa_xe_vjp(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_xe_opts* opts, const capb200_vjp_opts* vjp,
+                                  const long long* labels, int label_cols, const capb200_aoa_grads* grads, float* logprobs, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && vjp && att && labels && logprobs && (grads || vjp->forward_only), "null argument");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
+    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_xe_opts shared = {opts->seq_per_img, opts->steps, opts->seed, opts->drop_prob_lm, opts->label_smoothing, opts->upstream,
+                                    opts->att_masks, opts->ss_prob, opts->tokens_used, opts->keep_rows, opts->row_loss};
+    AoaTrainArgs ta;
+    if (xe_train_args(B, shared, labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
+    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_vjp_step(e, st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_aoa_scst_vjp(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_scst_opts* opts, const capb200_vjp_opts* vjp,
+                                    const capb200_aoa_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && vjp && att && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
+    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, nullptr};
+    AoaTrainArgs ta;
+    if (scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
+    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_vjp_step(e, st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
 }

@@ -1335,6 +1335,7 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
 
     // ---- (4) reward and loss, (5) the logit layer's backward
     nvtxRangePop();
+    if (ta.forward_only) return 0;
     CAPB_NVTX("capb200 train step: reward, loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_updown_grads& G = *grads;
@@ -1468,6 +1469,7 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
 
     // ---- loss, logit backward, back-propagation through time
     nvtxRangePop();
+    if (ta.forward_only) return 0;
     CAPB_NVTX("capb200 att2in2 train step: loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_att2in2_grads& G = *grads;
@@ -1580,6 +1582,7 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
 
     // ---- loss, logit backward, back-propagation through time
     nvtxRangePop();
+    if (ta.forward_only) return 0;
     CAPB_NVTX("capb200 newfc train step: loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_newfc_grads& G = *grads;
@@ -1712,6 +1715,86 @@ extern "C" int capb200_updown_xe_step(capb200_engine* e, const float* fc, const 
     if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_eager_step(st, [&] { return updown_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+// ---- autograd entry points of UpDown, Att2in2 and NewFC (include/capb200.h: capb200_vjp_opts) ----------------------------------------------
+namespace {
+
+// the feature checks of a family: UpDown reads fc and att, Att2in2 att, NewFC fc (and has no regions)
+int check_vjp_feats(const capb200_engine* e, int family, const float* fc, const float* att, int R, const float* att_masks) {
+    CAPB_REQUIRE(e->cfg.family == family, "the entry point does not match the engine's family");
+    if (family != CAPB200_FAMILY_ATT2IN2) CAPB_REQUIRE(fc != nullptr, "null argument");
+    if (family == CAPB200_FAMILY_NEWFC) CAPB_REQUIRE(att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
+    else CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
+    return 0;
+}
+
+template <class Grads, class Step>
+int xe_vjp(capb200_engine* e, int family, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const capb200_vjp_opts* vjp,
+           const long long* labels, int label_cols, const Grads* grads, float* logprobs, void* stream, Step step) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && vjp && labels && logprobs && (grads || vjp->forward_only), "null argument");
+    if (check_vjp_feats(e, family, fc, att, R, opts->att_masks)) return 1;
+    TrainArgs ta;
+    if (xe_train_args(B, *opts, labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_vjp_step(e, st, [&] { return step(ta, st); });
+}
+
+template <class Grads, class Step>
+int scst_vjp(capb200_engine* e, int family, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts, const capb200_vjp_opts* vjp,
+             const Grads* grads, long long* sample_seq, float* sample_logprobs, void* stream, Step step) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && vjp && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
+    if (check_vjp_feats(e, family, fc, att, R, opts->att_masks)) return 1;
+    TrainArgs ta;
+    if (scst_train_args(B, *opts, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_vjp_step(e, st, [&] { return step(ta, st); });
+}
+
+}  // namespace
+
+extern "C" int capb200_updown_xe_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
+                                     const capb200_vjp_opts* vjp, const long long* labels, int label_cols, const capb200_updown_grads* grads,
+                                     float* logprobs, void* stream) {
+    return xe_vjp(e, CAPB200_FAMILY_UPDOWN, fc, att, B, R, opts, vjp, labels, label_cols, grads, logprobs, stream,
+                  [&](const TrainArgs& ta, cudaStream_t st) { return updown_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_updown_scst_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                                       const capb200_vjp_opts* vjp, const capb200_updown_grads* grads, long long* sample_seq, float* sample_logprobs,
+                                       void* stream) {
+    return scst_vjp(e, CAPB200_FAMILY_UPDOWN, fc, att, B, R, opts, vjp, grads, sample_seq, sample_logprobs, stream,
+                    [&](const TrainArgs& ta, cudaStream_t st) { return updown_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_att2in2_xe_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
+                                      const capb200_vjp_opts* vjp, const long long* labels, int label_cols, const capb200_att2in2_grads* grads,
+                                      float* logprobs, void* stream) {
+    return xe_vjp(e, CAPB200_FAMILY_ATT2IN2, fc, att, B, R, opts, vjp, labels, label_cols, grads, logprobs, stream,
+                  [&](const TrainArgs& ta, cudaStream_t st) { return att2in2_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_att2in2_scst_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                                        const capb200_vjp_opts* vjp, const capb200_att2in2_grads* grads, long long* sample_seq, float* sample_logprobs,
+                                        void* stream) {
+    return scst_vjp(e, CAPB200_FAMILY_ATT2IN2, fc, att, B, R, opts, vjp, grads, sample_seq, sample_logprobs, stream,
+                    [&](const TrainArgs& ta, cudaStream_t st) { return att2in2_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_newfc_xe_vjp(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
+                                    const capb200_xe_opts* opts, const capb200_vjp_opts* vjp, const long long* labels, int label_cols,
+                                    const capb200_newfc_grads* grads, float* logprobs, void* stream) {
+    return xe_vjp(e, CAPB200_FAMILY_NEWFC, fc, nullptr, B, R, opts, vjp, labels, label_cols, grads, logprobs, stream,
+                  [&](const TrainArgs& ta, cudaStream_t st) { return newfc_train_step(e, fc, B, ta, grads, st); });
+}
+
+extern "C" int capb200_newfc_scst_vjp(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
+                                      const capb200_scst_opts* opts, const capb200_vjp_opts* vjp, const capb200_newfc_grads* grads, long long* sample_seq,
+                                      float* sample_logprobs, void* stream) {
+    return scst_vjp(e, CAPB200_FAMILY_NEWFC, fc, nullptr, B, R, opts, vjp, grads, sample_seq, sample_logprobs, stream,
+                    [&](const TrainArgs& ta, cudaStream_t st) { return newfc_train_step(e, fc, B, ta, grads, st); });
 }
 
 extern "C" {

@@ -180,6 +180,9 @@ int scst_drop_worst_launch(const long long* seq, const float* row_loss, int N, i
 int xe_loss_backward_launch(const float* logp, long ld_row, const long long* labels, long ld_l, const float* masks, long ld_m, int N, int steps, int Ls, int V1,
                             float smoothing, float upstream, float* mask_sum, float* item_loss, float* dl, float* loss, cudaStream_t st, int keep = 0,
                             float* row_loss = nullptr, float* row_msum = nullptr, float* row_coef = nullptr);
+// Backward of log_softmax for an outside gradient g = dL/dlogp over [N, T, V1] rows (pitch ld_row between sequences): dl [N, T, V1] =
+// g - exp(logp) * rowsum(g); with seq [N, T] (sampling form) the rows of sequences finished before step t get zero.
+int logsoftmax_vjp_launch(const float* logp, const float* g, long ld_row, const long long* seq, int N, int T, int V1, float* dl, cudaStream_t st);
 int lstm_cell_backward_launch(int rows, int H, const float* gates, const float* c_prev, const float* c_new, const float* dh, const float* dh_extra,
                               long ld_extra, unsigned drop_site, unsigned drop_step, unsigned long long seed, float p, float* dc_carry, float* dgates,
                               cudaStream_t st);

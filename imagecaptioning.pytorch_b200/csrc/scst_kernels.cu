@@ -8,6 +8,8 @@
 //   maxout_cell_backward     Att2in2Core's maxout cell (AttModel.py:773-787) and NewFC's LSTMCore (FCModel.py:25-42)
 //   attention_backward       models/AttModel.py:728-748
 // Dropout masks are never stored: keep(seed, site, step, element) is a pure function (Philox4x32-10), re-evaluated in the backward.
+#include <type_traits>
+
 #include "common.cuh"
 #include "dropout.cuh"
 #include "kernels.cuh"
@@ -66,6 +68,51 @@ __global__ void scst_dlogits_kernel(const float* __restrict__ logp, long ld_row,
         return;
     }
     for (int v = threadIdx.x; v < V1; v += blockDim.x) d[v] = coef * ((v == tok ? 1.f : 0.f) - expf(lp[v]));
+}
+
+// Backward of log_softmax for an outside gradient G = dL/dlogp: dl[n,t,v] = G[n,t,v] - exp(logp[n,t,v]) * sum_v' G[n,t,v'].  One CTA per
+// (n, t), VEC floats per load.  With `seq` (sampling form) a row that had finished before step t was written as zeros by the forward
+// (AttModel.py:341: logprobs * unfinished), so its d logits are zero.
+template <int VEC>
+__global__ void __launch_bounds__(256) logsoftmax_vjp_kernel(const float* __restrict__ logp, const float* __restrict__ g, long ld_row,
+                                                             const long long* __restrict__ seq, int T, int V1, float* __restrict__ dl) {
+    using V = typename std::conditional<VEC == 4, float4, float>::type;
+    __shared__ float red[32];
+    const long item = blockIdx.x;                 // n * T + t
+    const int t = (int)(item % T);
+    const long n = item / T;
+    const int nv = V1 / VEC;
+    V* d = reinterpret_cast<V*>(dl + item * V1);
+    if (seq != nullptr && t > 0 && seq[n * T + t - 1] == 0) {
+        const V z = {};
+        for (int i = threadIdx.x; i < nv; i += blockDim.x) d[i] = z;
+        return;
+    }
+    const V* gr = reinterpret_cast<const V*>(g + n * ld_row + (long)t * V1);
+    const V* lr = reinterpret_cast<const V*>(logp + n * ld_row + (long)t * V1);
+    auto hsum = [](const V& x) {
+        if constexpr (VEC == 4) return (x.x + x.y) + (x.z + x.w);
+        else return x;
+    };
+    float s = 0.f;
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) s += hsum(gr[i]);
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        s = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (threadIdx.x == 0) red[0] = s;
+    }
+    __syncthreads();
+    s = red[0];
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+        const V gv = gr[i], lv = lr[i];
+        V o;
+        if constexpr (VEC == 4) o = make_float4(gv.x - expf(lv.x) * s, gv.y - expf(lv.y) * s, gv.z - expf(lv.z) * s, gv.w - expf(lv.w) * s);
+        else o = gv - expf(lv) * s;
+        d[i] = o;
+    }
 }
 
 // ---- cross-entropy stage (LanguageModelCriterion / LabelSmoothing, losses.py:204-265) on teacher-forced log-probs [N, Ls, V1]:
@@ -454,6 +501,12 @@ int xe_loss_backward_launch(const float* logp, long ld_row, const long long* lab
         LAUNCH_OK();
     }
     xe_loss_kernel<<<1, 256, 0, st>>>(item_loss, N, steps, Ls, masks, ld_m, smoothing, V1, mask_sum, loss);
+    LAUNCH_OK();
+}
+int logsoftmax_vjp_launch(const float* logp, const float* g, long ld_row, const long long* seq, int N, int T, int V1, float* dl, cudaStream_t st) {
+    const bool vec = V1 % 4 == 0 && ld_row % 4 == 0 && (reinterpret_cast<uintptr_t>(logp) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dl)) % 16 == 0;
+    if (vec) logsoftmax_vjp_kernel<4><<<N * T, 256, 0, st>>>(logp, g, ld_row, seq, T, V1, dl);
+    else logsoftmax_vjp_kernel<1><<<N * T, 256, 0, st>>>(logp, g, ld_row, seq, T, V1, dl);
     LAUNCH_OK();
 }
 int lstm_cell_backward_launch(int rows, int H, const float* gates, const float* c_prev, const float* c_new, const float* dh, const float* dh_extra,

@@ -461,7 +461,6 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
     const float p = ta.p, p_lm = ta.p_lm;
     const unsigned long long seed = ta.seed;
     const capb200_tfm_weights& w = e->w;
-    const capb200_tfm_grads& G = *grads;
     const float emb_scale = sqrtf((float)D);
     CAPB_REQUIRE(T >= 1 && T <= e->T + 1 && T < 32, "positions out of range");
     TTape tp;
@@ -563,7 +562,9 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
         if (permute_rows_launch(T, N, D, tp.yln_tm, D, tp.yln_nm, D, 1, st)) return 1;
         nl += 5;
     }
+    if (ta.forward_only) return 0;
     if (loss_backward(ta, tp, gb, B, N, V1, st)) return 1;
+    const capb200_tfm_grads& G = *grads;
 
     // ---- backward: generator and the final LayerNorm
     auto colsum = [&](int rows, int cols, const float* x, long ld, float* out) { nl++; return colsum_launch(rows, cols, x, ld, out, 0, st); };
@@ -701,4 +702,35 @@ extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, in
     ta.p_lm = opts->drop_prob_lm;
     return run_scst_step(e, opts, grads, ta, nullptr, 0, att, sizeof(float) * (size_t)B * R * e->F, B, R, static_cast<cudaStream_t>(stream),
                          [&](const float*, const float* att_s, const TfmTrainArgs& t, cudaStream_t s) { return tfm_train_step(e, att_s, B, R, t, grads, s); });
+}
+
+// The autograd entry points (include/capb200.h: capb200_vjp_opts) on the Transformer's option structs.
+extern "C" int capb200_tfm_xe_vjp(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_xe_opts* opts, const capb200_vjp_opts* vjp,
+                                  const long long* labels, int label_cols, const capb200_tfm_grads* grads, float* logprobs, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && vjp && att && labels && logprobs && (grads || vjp->forward_only), "null argument");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_xe_opts shared = {opts->seq_per_img, label_cols - 1, opts->seed, opts->dropout, opts->label_smoothing, opts->upstream,
+                                    opts->att_masks, 0.f, nullptr, opts->keep_rows, opts->row_loss};
+    TfmTrainArgs ta;
+    if (xe_train_args(B, shared, labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
+    ta.p_lm = opts->drop_prob_lm;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_vjp_step(e, st, [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_tfm_scst_vjp(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_scst_opts* opts, const capb200_vjp_opts* vjp,
+                                    const capb200_tfm_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && vjp && att && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
+    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, nullptr};
+    TfmTrainArgs ta;
+    if (scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
+    ta.p_lm = opts->drop_prob_lm;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_vjp_step(e, st, [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
 }

@@ -36,6 +36,10 @@ struct TrainArgs {
     // XE
     const long long* labels = nullptr; long ld_labels = 0; const float* masks = nullptr; long ld_masks = 0;
     float* logprobs = nullptr; float* loss = nullptr;
+    // the autograd entry points (capb200_*_vjp): stop after the forward, or replace the criterion by an outside dL/dlogprobs [N, Tl, V1]
+    bool forward_only = false;
+    const float* dlogprobs = nullptr;
+    bool greedy = false;                    // SCST form: draw the argmax instead of a multinomial sample
 
     // The weighted reward runs only when it can differ from CIDEr-D alone: a BLEU weight <= 0 adds weight * 0.
     bool weighted_reward() const { return !xe && (w_bleu > 0.0 || w_cider != 1.0); }
@@ -43,14 +47,19 @@ struct TrainArgs {
     int reward_extra_launches() const { return weighted_reward() ? weighted_reward_launches(w_cider, w_bleu, true) - 2 : 0; }
 };
 
+inline int vjp_train_args(const capb200_vjp_opts* v, TrainArgs* ta);
+
 // Checks the SCST options every family shares and fills `ta`.  A family hands its own options over as capb200_scst_opts (drop_prob = its
-// main dropout rate) and checks its other rates itself.
+// main dropout rate) and checks its other rates itself.  With `vjp` (an autograd entry point) no reward runs: the baseline is not read.
 inline int scst_train_args(int B, const capb200_scst_opts& o, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
-                           long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, int T, TrainArgs* ta) {
-    const bool greedy_baseline = o.baseline == CAPB200_BASELINE_GREEDY;
-    CAPB_REQUIRE(greedy_baseline || o.baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
-    CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
-    CAPB_REQUIRE(greedy_baseline || o.sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
+                           long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, int T, TrainArgs* ta,
+                           const capb200_vjp_opts* vjp = nullptr) {
+    const bool greedy_baseline = vjp == nullptr && o.baseline == CAPB200_BASELINE_GREEDY;
+    if (vjp == nullptr) {
+        CAPB_REQUIRE(greedy_baseline || o.baseline == CAPB200_BASELINE_LEAVE_ONE_OUT, "unknown baseline");
+        CAPB_REQUIRE(!greedy_baseline || greedy_seq != nullptr, "the greedy baseline needs greedy_seq");
+        CAPB_REQUIRE(greedy_baseline || o.sample_n >= 2, "the leave-one-out baseline needs sample_n >= 2");
+    }
     CAPB_REQUIRE(o.sample_n >= 1 && o.sample_n <= 16 && B >= 1, "sample_n must be in 1..16");
     CAPB_REQUIRE(o.drop_prob >= 0.f && o.drop_prob < 1.f, "dropout rates must be in [0, 1)");
     CAPB_REQUIRE(o.temperature > 0.f, "temperature must be positive");
@@ -63,13 +72,13 @@ inline int scst_train_args(int B, const capb200_scst_opts& o, const capb200_cide
     ta->seed = o.seed; ta->greedy_baseline = greedy_baseline; ta->table = table; ta->refs = refs; ta->ref_offsets = ref_offsets; ta->L = L;
     ta->sample_seq = sample_seq; ta->greedy_seq = greedy_seq; ta->reward = reward; ta->logprobs = sample_logprobs; ta->loss = loss;
     ta->forced = o.forced_tokens; ta->mask = o.att_masks; ta->keep = o.keep_rows; ta->row_loss = o.row_loss;
-    return 0;
+    return vjp != nullptr ? vjp_train_args(vjp, ta) : 0;
 }
 
 // Checks the XE options every family shares and fills `ta`; a family hands its own options over as capb200_xe_opts, as above.  T is the
 // engine's seq_length.
 inline int xe_train_args(int B, const capb200_xe_opts& o, const long long* labels, const float* masks, int label_cols, float* logprobs, float* loss,
-                         int T, TrainArgs* ta) {
+                         int T, TrainArgs* ta, const capb200_vjp_opts* vjp = nullptr) {
     CAPB_REQUIRE(o.seq_per_img >= 1 && o.seq_per_img <= 16 && B >= 1, "seq_per_img must be in 1..16");
     CAPB_REQUIRE(o.drop_prob >= 0.f && o.drop_prob < 1.f, "dropout rates must be in [0, 1)");
     CAPB_REQUIRE(o.label_smoothing >= 0.f && o.label_smoothing < 1.f, "label_smoothing must be in [0, 1)");
@@ -82,6 +91,19 @@ inline int xe_train_args(int B, const capb200_xe_opts& o, const long long* label
     ta->smoothing = o.label_smoothing;
     ta->labels = labels; ta->ld_labels = label_cols; ta->masks = masks; ta->ld_masks = label_cols; ta->logprobs = logprobs; ta->loss = loss;
     ta->mask = o.att_masks; ta->ss_prob = o.ss_prob; ta->tokens_used = o.tokens_used; ta->keep = o.keep_rows; ta->row_loss = o.row_loss;
+    return vjp != nullptr ? vjp_train_args(vjp, ta) : 0;
+}
+
+// The options of an autograd entry point: the forward alone (no criterion, no reward, no gradients), or the backward of an outside
+// dL/dlogprobs.  Neither has a loss: drop_worst has no meaning there.
+inline int vjp_train_args(const capb200_vjp_opts* v, TrainArgs* ta) {
+    CAPB_REQUIRE(v->forward_only || v->dlogprobs != nullptr, "the backward needs dlogprobs");
+    CAPB_REQUIRE(ta->keep == 0, "keep_rows belongs to the fused steps' criterion");
+    CAPB_REQUIRE(ta->xe || !v->greedy || ta->forced == nullptr, "greedy draws and forced tokens exclude each other");
+    ta->forward_only = v->forward_only != 0;
+    ta->dlogprobs = ta->forward_only ? nullptr : v->dlogprobs;
+    ta->greedy = v->greedy != 0;
+    ta->greedy_baseline = false;
     return 0;
 }
 
@@ -198,7 +220,7 @@ inline int train_vocab_step(const TrainArgs& ta, const StepTape& tp, int N, int 
     VocabStepArgs va;
     va.rows = N; va.V1 = V1; va.logits = ta.logprobs + (long)t * V1; va.ld = (long)ta.Tl * V1;
     if (!ta.xe) {
-        va.select = 2; va.temperature = ta.temperature; va.seed = ta.seed; va.step = (unsigned long long)t;
+        va.select = ta.greedy ? 1 : 2; va.temperature = ta.temperature; va.seed = ta.seed; va.step = (unsigned long long)t;
         va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
         va.seq_out = ta.sample_seq; va.ld_seq = ta.T; va.t = t;
         if (ta.forced != nullptr) {
@@ -215,6 +237,8 @@ inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBa
     const int T = ta.T;
     const long ld_lp = (long)ta.Tl * V1;
     float* row_loss = ta.row_loss ? ta.row_loss : tp.row_loss;
+    if (ta.dlogprobs != nullptr)
+        return logsoftmax_vjp_launch(ta.logprobs, ta.dlogprobs, ld_lp, ta.xe ? nullptr : ta.sample_seq, N, T, V1, tp.DL, st);
     if (ta.xe)
         return xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
                                        tp.mask_sum, tp.item_loss, tp.DL, ta.loss, st, ta.keep, row_loss, tp.row_msum, tp.row_coef);
@@ -272,6 +296,18 @@ template <class Step>
 int run_eager_step(cudaStream_t st, Step step) {
     if (dropout_salt_set_all(0ull, st)) return 1;
     return step();
+}
+
+// A step of an autograd entry point (capb200_*_vjp): eager, and with the engine's gradient-group events unset -- its gradients go to the
+// caller's own table, which no data-parallel listener waits on.
+template <class Engine, class Step>
+int run_vjp_step(Engine* e, cudaStream_t st, Step step) {
+    constexpr int n = sizeof(e->grad_events) / sizeof(e->grad_events[0]);
+    cudaEvent_t saved[n];
+    for (int i = 0; i < n; ++i) { saved[i] = e->grad_events[i]; e->grad_events[i] = nullptr; }
+    const int rc = run_eager_step(st, step);
+    for (int i = 0; i < n; ++i) e->grad_events[i] = saved[i];
+    return rc;
 }
 
 // Runs one SCST step, `step(fc, att, ta, stream)`, as ONE CUDA graph.  Its ~900-4900 kernels are 5-30 us each, every launch boundary costs

@@ -154,6 +154,8 @@ class B200CaptionModel(nn.Module):
             raise ValueError('numeric_mode must be one of %s' % sorted(_lib.MODES))
         self.done_beams = []
         self._store = _EngineStore(self)
+        # differentiable _forward / _sample (the autograd entry points, include/capb200.h: capb200_vjp_opts); off = the calls as before
+        self.autograd = bool(getattr(opt, 'b200_autograd', 0))
 
     # ---- engine plumbing --------------------------------------------------------------------------------------------
     _engine = _slot_property('engine')
@@ -338,6 +340,8 @@ class B200CaptionModel(nn.Module):
         beam_size = opt.get('beam_size', 1)
         temperature = float(opt.get('temperature', 1.0))
         sample_n = int(opt.get('sample_n', 1))
+        if self._autograd_active():
+            return self._sample_autograd(fc_feats, att_feats, att_masks, opt, forced_tokens)
         if beam_size > 1 and sample_method in ('greedy', 'beam_search'):
             return self._sample_beam(fc_feats, att_feats, att_masks, opt)
         self._check_opts(opt)
@@ -446,8 +450,11 @@ class B200CaptionModel(nn.Module):
 
     @_on_device
     def _forward(self, fc_feats, att_feats, seq, att_masks=None):
-        """Teacher forcing (AttModel.py:126-164).  Scheduled sampling (training with ss_prob > 0) lives in the fused XE step (xe_step /
-        B200LossWrapper), which is what trains; this inference-style call is plain teacher forcing."""
+        """Teacher forcing (AttModel.py:126-164).  With model.autograd off this is an inference-style call (plain teacher forcing, no
+        grad_fn): training runs in the fused XE step (xe_step / B200LossWrapper), scheduled sampling included.  With it on, under grad, the
+        log-probs are differentiable (_forward_autograd)."""
+        if self._autograd_active():
+            return self._forward_autograd(fc_feats, att_feats, seq, att_masks)
         if self.training and self.ss_prob > 0.0 and torch.is_grad_enabled():
             raise NotImplementedError('scheduled sampling runs inside the fused XE step (B200LossWrapper / model.xe_step), not in a bare _forward call')
         lib = self._ensure_engine(fc_feats.device)
@@ -467,6 +474,136 @@ class B200CaptionModel(nn.Module):
         so = _lib.SampleOpts(spi, _lib.SAMPLE_TEACHER, 1.0, 0, steps)
         _lib.check(self._call_sample(lib, fc, att, masks, B, R, so, seq, L, None, out), 'forward_teacher')
         return out
+
+    # ---- autograd path (model.autograd): the forward of the fused training steps, and the backward of an outside dL/dlogprobs -----------
+    # A family provides _vjp_prefix (capb200_<prefix>_xe_vjp / _scst_vjp), _grads_struct, _fill_table, _vjp_params, _vjp_feats,
+    # _vjp_feat_args, _vjp_xe_opts and _vjp_scst_opts.
+    _vjp_prefix = None
+
+    def _autograd_active(self):
+        """model.autograd, grad mode on, and some parameter that wants a gradient."""
+        return (getattr(self, 'autograd', False) and self._vjp_prefix is not None and torch.is_grad_enabled()
+                and any(p.requires_grad for p in self._vjp_params()))
+
+    @staticmethod
+    def _refuse_feature_grads(*feats):
+        if any(f is not None and f.requires_grad for f in feats):
+            raise NotImplementedError('capb200 autograd: gradients with respect to the features are out of scope (detach them)')
+
+    def _vjp_run(self, form, feats, B, R, make_opts, words, logprobs_shape, dev, greedy=False, out_seq=None):
+        """The closure _EngineVjp calls: run(None) is the forward (log-probs), run(G) the backward of G = dL/dlogprobs (one fresh gradient
+        tensor per parameter).  make_opts(replay) builds the option struct: replay=False for the forward, True for the backward, which
+        feeds the same words (words()) with the same seed."""
+        params = self._vjp_params()
+        entry = 'capb200_%s_%s_vjp' % (self._vjp_prefix, form)
+
+        def run(G):
+            lib = self._ensure_engine(dev)
+            lp = torch.zeros(logprobs_shape, dtype=torch.float32, device=dev)
+            if G is None:
+                opts, vo, g, grads = make_opts(False), _lib.VjpOpts(1, None, int(greedy)), None, None
+            else:
+                G = G.detach().to(torch.float32).contiguous()
+                grads = [torch.empty_like(p) for p in params]
+                g = self._grads_struct()
+                self._fill_table(g, {id(p): t for p, t in zip(params, grads)})
+                opts, vo = make_opts(True), _lib.VjpOpts(0, G.data_ptr(), 0)
+            tail = (words(G is not None), logprobs_shape[1] + 1) if form == 'xe' else ()
+            seq = out_seq if G is None or out_seq is None else torch.empty_like(out_seq)
+            outs = (_lib.ptr(lp),) if form == 'xe' else (_lib.ptr(seq), _lib.ptr(lp))
+            args = self._vjp_feat_args(*feats) + (B, R, ctypes.byref(opts), ctypes.byref(vo))
+            if form == 'xe':
+                args += (_lib.ptr(tail[0]), tail[1])
+            _lib.check(getattr(lib, entry)(self._engine, *args, None if g is None else ctypes.byref(g), *outs, _lib.current_stream()),
+                       entry[len('capb200_'):])
+            return lp if G is None else grads
+        return run, params
+
+    def _forward_autograd(self, fc_feats, att_feats, seq, att_masks):
+        """Differentiable teacher forcing: train mode runs the fused XE step's forward (its dropout masks and, with ss_prob > 0, its
+        scheduled sampling), eval mode the same forward without dropout."""
+        self._refuse_feature_grads(fc_feats, att_feats)
+        if seq.dim() == 3:
+            seq = seq.reshape(-1, seq.shape[2])
+        seq = seq.detach().to(torch.long).contiguous()
+        N, L = seq.shape
+        if L > self.seq_length + 1:
+            raise ValueError('label width %d exceeds what the engine trains (seq_length + 1 = %d)' % (L, self.seq_length + 1))
+        train = self.training
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if train else 0      # where xe_step draws it: torch.manual_seed reproduces both
+        fc, att, masks, B, R = self._vjp_feats(fc_feats, att_feats, att_masks)
+        dev = (fc if fc is not None else att).device
+        seq = seq.to(dev)
+        steps = self._teacher_steps(seq)
+        ss = float(self.ss_prob) if train and self._vjp_ss else 0.0
+        tokens_used = torch.zeros(N, L, dtype=torch.long, device=dev) if ss > 0 else None
+        pad = seq.new_zeros(N, 1)
+        labels = torch.cat([seq, pad], 1)       # [N, L + 1]: the entry points take labels with the target column; it is never read
+
+        def words(replay):
+            return torch.cat([tokens_used, pad], 1) if replay and tokens_used is not None else labels
+
+        def make_opts(replay):
+            return self._vjp_xe_opts(N // B, steps, seed, train, masks, 0.0 if replay else ss, None if replay else tokens_used)
+        run, params = self._vjp_run('xe', (fc, att), B, R, make_opts, words, (N, L, self.vocab_size + 1), dev)
+        return _EngineVjp.apply(run, *params)
+
+    def _sample_autograd(self, fc_feats, att_feats, att_masks, opt, forced_tokens):
+        """Differentiable sampling: greedy or multinomial draws of the fused SCST step's sampler (train mode: with its dropout, the same
+        draws as scst_step for the same seed), seq [B*n, T] and log-probs [B*n, T, V+1] with the reference's finished-row zeros."""
+        method = opt.get('sample_method', 'greedy')
+        if opt.get('beam_size', 1) > 1 and method in ('greedy', 'beam_search'):
+            raise NotImplementedError('capb200 autograd: beam search under grad (train_beam_size > 1) is out of scope')
+        self._check_opts(opt)
+        edits = [k for k in ('decoding_constraint', 'remove_bad_endings', 'suppress_UNK', 'block_trigrams') if opt.get(k, 0)]
+        if edits:
+            raise NotImplementedError('capb200 autograd: decode edits (%s) are not differentiated' % ', '.join(edits))
+        if forced_tokens is None and method not in ('greedy', 'sample'):
+            if method != 'gumbel' and not method.startswith('top'):
+                raise NotImplementedError('sample_method %r is out of scope of the engine' % method)
+            if self.training:
+                raise NotImplementedError('capb200 autograd: sample_method %r in train mode is out of scope (greedy and sample are covered)' % method)
+        self._refuse_feature_grads(fc_feats, att_feats)
+        sample_n, temperature, train = int(opt.get('sample_n', 1)), float(opt.get('temperature', 1.0)), self.training
+        forced = None
+        if forced_tokens is None and method not in ('greedy', 'sample'):
+            with torch.no_grad():                # eval mode: the decode path draws, the autograd forward replays the draw
+                forced, _ = self._sample(fc_feats, att_feats, att_masks, opt)
+        elif forced_tokens is not None:
+            forced = forced_tokens
+        draws = forced is None and method == 'sample'
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if train or draws else 0     # where scst_step / _sample draw it
+        fc, att, masks, B, R = self._vjp_feats(fc_feats, att_feats, att_masks)
+        dev = (fc if fc is not None else att).device
+        N, T = B * sample_n, self.seq_length
+        if forced is not None:
+            forced = forced.detach().to(device=dev, dtype=torch.long).contiguous()
+            assert forced.shape == (N, T)
+        seq = torch.zeros(N, T, dtype=torch.long, device=dev)
+
+        def make_opts(replay):
+            return self._vjp_scst_opts(sample_n, temperature, seed, train, masks, seq if replay else forced)
+        run, params = self._vjp_run('scst', (fc, att), B, R, make_opts, None, (N, T, self.vocab_size + 1), dev,
+                                    greedy=forced is None and method == 'greedy', out_seq=seq)
+        logprobs = _EngineVjp.apply(run, *params)
+        return seq, logprobs
+
+
+class _EngineVjp(torch.autograd.Function):
+    """One node per autograd call of an engine model, with the parameters as inputs.  The backward recomputes the forward instead of
+    keeping its tape: the engine's training tape is shared by every training call, and whatever runs between the forward and the backward
+    (another forward, a fused step, PPO's old-policy pass) may overwrite it."""
+
+    @staticmethod
+    def forward(ctx, run, *params):
+        ctx.run = run
+        ctx.save_for_backward(*params)          # an in-place update of a weight before the backward raises torch's version error
+        return run(None)
+
+    @staticmethod
+    def backward(ctx, grad):
+        _ = ctx.saved_tensors
+        return (None,) + tuple(ctx.run(grad))
 
 
 class _LazyDoneBeams(list):
@@ -510,6 +647,31 @@ class _FusedTrainSteps:
         fc = self._f32(fc_feats)
         att, masks = self._clip(att_feats, att_masks)
         return fc, att, masks, att.shape[0], att.shape[1]
+
+    # ---- autograd path hooks (B200CaptionModel._vjp_run)
+    _vjp_ss = True             # AttModel._forward's scheduled sampling
+
+    def _vjp_params(self):
+        return list(self._weight_table().values())
+
+    def _fill_table(self, table, tensor_of):
+        for name, prm in self._weight_table().items():
+            setattr(table, name, tensor_of[id(prm)].data_ptr())
+
+    def _vjp_feats(self, fc_feats, att_feats, att_masks):
+        return self._train_feats(fc_feats, att_feats, att_masks)
+
+    @staticmethod
+    def _vjp_feat_args(fc, att):
+        return (_lib.ptr(fc), _lib.ptr(att))
+
+    def _vjp_xe_opts(self, spi, steps, seed, train, masks, ss_prob, tokens_used):
+        return _lib.XeOpts(spi, steps, seed, float(self.drop_prob_lm) if train else 0.0, 0.0, 1.0, _lib.ptr(masks), float(ss_prob),
+                           _lib.ptr(tokens_used), 0, None)
+
+    def _vjp_scst_opts(self, sample_n, temperature, seed, train, masks, forced):
+        return _lib.ScstOpts(sample_n, float(temperature), seed, float(self.drop_prob_lm) if train else 0.0, 1.0, _lib.BASELINE_GREEDY, _lib.ptr(forced),
+                             _lib.ptr(masks), 0, None, None)
 
     def _grad_groups(self):
         t = self._weight_table()
@@ -629,6 +791,7 @@ class B200UpDownModel(_FusedTrainSteps, B200CaptionModel):
     family_name = 'updown'
     # C entry points and gradient table of the fused training steps (include/capb200.h)
     _scst_entry, _xe_entry = 'capb200_updown_scst_step', 'capb200_updown_xe_step'
+    _vjp_prefix = 'updown'
     _grads_struct, _grad_fields = _lib.UpdownGrads, _lib.GRAD_FIELDS
 
     def __init__(self, opt, numeric_mode=None):
@@ -677,6 +840,7 @@ class B200Att2in2Model(B200UpDownModel):
     family = _lib.FAMILY_ATT2IN2
     family_name = 'att2in2'
     _scst_entry, _xe_entry = 'capb200_att2in2_scst_step', 'capb200_att2in2_xe_step'
+    _vjp_prefix = 'att2in2'
     _grads_struct, _grad_fields = _lib.Att2in2Grads, _lib.ATT2IN2_GRAD_FIELDS
 
     def __init__(self, opt, numeric_mode=None):
@@ -717,6 +881,7 @@ class B200NewFCModel(_FusedTrainSteps, B200CaptionModel):
     family = _lib.FAMILY_NEWFC
     family_name = 'newfc'
     _scst_entry, _xe_entry = 'capb200_newfc_scst_step', 'capb200_newfc_xe_step'
+    _vjp_prefix = 'newfc'
     _grads_struct, _grad_fields = _lib.NewfcGrads, _lib.NEWFC_GRAD_FIELDS
     _no_diverse = ("the engine chooses NewFC's fresh-state pass (the image-embedding step, AttModel.py:925-936) per core call, not per row, "
                    "so its groups cannot start at different steps")
@@ -947,6 +1112,37 @@ class B200TransformerModel(B200CaptionModel):
     def _result_grads(self, fg):
         return {prm: fg.by_name[self._slot_name(path)] for path, prm in self._slots()}
 
+    # ---- autograd path hooks (B200CaptionModel._vjp_run); no scheduled sampling, as in TransformerModel._forward
+    _vjp_prefix, _grads_struct, _vjp_ss = 'tfm', _lib.TfmWeights, False
+
+    def _vjp_params(self):
+        return [prm for _, prm in self._slots()]
+
+    def _fill_table(self, table, tensor_of):
+        for path, prm in self._slots():
+            dst = table
+            for key in path[:-1]:
+                dst = getattr(dst, key) if isinstance(key, str) else dst[key]
+            setattr(dst, path[-1], tensor_of[id(prm)].data_ptr())
+
+    def _vjp_feats(self, fc_feats, att_feats, att_masks):
+        att, masks = self._clip(att_feats, att_masks)
+        return None, att, masks, att.shape[0], att.shape[1]
+
+    @staticmethod
+    def _vjp_feat_args(fc, att):
+        return (_lib.ptr(att),)
+
+    def _vjp_rates(self, train):
+        return (float(self.drop_prob_lm), float(self.dropout)) if train else (0.0, 0.0)
+
+    def _vjp_xe_opts(self, spi, steps, seed, train, masks, ss_prob, tokens_used):
+        return _lib.TfmXeOpts(spi, seed, 0.0, 1.0, *self._vjp_rates(train), _lib.ptr(masks), 0, None)
+
+    def _vjp_scst_opts(self, sample_n, temperature, seed, train, masks, forced):
+        return _lib.TfmScstOpts(sample_n, float(temperature), seed, 1.0, _lib.BASELINE_GREEDY, *self._vjp_rates(train), _lib.ptr(forced), _lib.ptr(masks),
+                                0, None, None)
+
     @_on_device
     def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, dropout=None, att_masks=None,
                 keep_rows=0):
@@ -1113,6 +1309,31 @@ class B200AoAModel(B200CaptionModel):
         table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
         _lib.check(lib.capb200_aoa_set_grad_events(self._engine, table, n), 'aoa_set_grad_events')
         return fg, g
+
+    # ---- autograd path hooks (B200CaptionModel._vjp_run); the rates xe_step / scst_step default to
+    _vjp_prefix, _grads_struct, _vjp_ss = 'aoa', _lib.AoaWeights, True
+
+    def _vjp_params(self):
+        return self._tensors()
+
+    def _vjp_feats(self, fc_feats, att_feats, att_masks):
+        att, masks = self._clip(att_feats, att_masks)
+        return None, att, masks, att.shape[0], att.shape[1]
+
+    @staticmethod
+    def _vjp_feat_args(fc, att):
+        return (_lib.ptr(att),)
+
+    def _vjp_rates(self, train):
+        """drop_prob_lm, drop_attn, drop_aoa, drop_sublayer, ctx_drop"""
+        return (float(self.drop_prob_lm), 0.1, float(self.dropout_aoa), 0.1, int(self.ctx_drop)) if train else (0.0, 0.0, 0.0, 0.0, 0)
+
+    def _vjp_xe_opts(self, spi, steps, seed, train, masks, ss_prob, tokens_used):
+        return _lib.AoaXeOpts(spi, steps, seed, 0.0, 1.0, *self._vjp_rates(train), _lib.ptr(masks), float(ss_prob), _lib.ptr(tokens_used), 0, None)
+
+    def _vjp_scst_opts(self, sample_n, temperature, seed, train, masks, forced):
+        return _lib.AoaScstOpts(sample_n, float(temperature), seed, 1.0, _lib.BASELINE_GREEDY, *self._vjp_rates(train), _lib.ptr(forced), _lib.ptr(masks),
+                                0, None, None)
 
     def _fill_table(self, table, tensor_of):
         """Writes data pointers into an AoaWeights-layout ctypes struct; ``tensor_of`` maps id(parameter) -> tensor to point at."""

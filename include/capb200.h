@@ -635,6 +635,47 @@ int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, int B, int R,
 int capb200_tfm_set_grad_events(capb200_tfm_engine* e, void* const* events, int n);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Autograd entry points of every family: the forward of the fused training steps without their criterion, and the backward of a
+ * caller-given dL/dlogprobs, so that any loss written in PyTorch trains an engine model (models.py: model.autograd).
+ *   *_xe_vjp    teacher form: the forward of the family's xe_step over labels[..., :label_cols-1] (scheduled sampling included; the
+ *               words fed land in opts->tokens_used), logprobs [N, label_cols-1, V+1] (caller zero-fills; columns >= steps stay zero).
+ *   *_scst_vjp  sampling form: the sampler of the family's scst_step (multinomial at opts->temperature, the argmax with vjp->greedy, or
+ *               the replay of opts->forced_tokens), sample_seq [N, T] and sample_logprobs [N, T, V+1]; rows already finished are zero.
+ * The option structs are the fused steps' own: seed, dropout rates (0 = eval mode), att_masks, seq_per_img / sample_n, steps, ss_prob,
+ * tokens_used and forced_tokens mean what they mean there; baseline, upstream, label_smoothing and reward_weights are not read, keep_rows
+ * must be 0.  With vjp->forward_only nothing else runs and grads may be NULL.  Otherwise the same forward (same seed, same words: pass
+ * the recorded tokens_used as labels with ss_prob = 0, or the drawn seq as forced_tokens) is followed by the backward of
+ * dlogprobs [N, Tl, V+1] (Tl = label_cols-1 or T) through log_softmax and the model: d logits = G - exp(logprobs) * sum_v G per row, zero
+ * for rows the forward did not produce.  Every grads buffer is OVERWRITTEN.  The calls run eagerly (no CUDA graph), record no
+ * gradient-group events, and reuse the engine's training tape: one call at a time per engine.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct {
+    int forward_only;          /* 1: the forward alone */
+    const float* dlogprobs;    /* [N, Tl, V+1] fp32 device, the upstream gradient of the backward (forward_only = 0) */
+    int greedy;                /* sampling form: draw the argmax (sample_method 'greedy') instead of a multinomial sample */
+} capb200_vjp_opts;
+int capb200_updown_xe_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const capb200_vjp_opts* vjp,
+                          const long long* labels, int label_cols, const capb200_updown_grads* grads, float* logprobs, void* stream);
+int capb200_updown_scst_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts, const capb200_vjp_opts* vjp,
+                            const capb200_updown_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream);
+int capb200_att2in2_xe_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const capb200_vjp_opts* vjp,
+                           const long long* labels, int label_cols, const capb200_att2in2_grads* grads, float* logprobs, void* stream);
+int capb200_att2in2_scst_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts, const capb200_vjp_opts* vjp,
+                             const capb200_att2in2_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream);
+int capb200_newfc_xe_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const capb200_vjp_opts* vjp,
+                         const long long* labels, int label_cols, const capb200_newfc_grads* grads, float* logprobs, void* stream);
+int capb200_newfc_scst_vjp(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts, const capb200_vjp_opts* vjp,
+                           const capb200_newfc_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream);
+int capb200_aoa_xe_vjp(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_xe_opts* opts, const capb200_vjp_opts* vjp,
+                       const long long* labels, int label_cols, const capb200_aoa_grads* grads, float* logprobs, void* stream);
+int capb200_aoa_scst_vjp(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_scst_opts* opts, const capb200_vjp_opts* vjp,
+                         const capb200_aoa_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream);
+int capb200_tfm_xe_vjp(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_xe_opts* opts, const capb200_vjp_opts* vjp,
+                       const long long* labels, int label_cols, const capb200_tfm_grads* grads, float* logprobs, void* stream);
+int capb200_tfm_scst_vjp(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_scst_opts* opts, const capb200_vjp_opts* vjp,
+                         const capb200_tfm_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Optimizer step of the training loop: utils.clip_gradient(optimizer, grad_clip_value) (captioning/utils/misc.py:156-160, called at
  * tools/train.py:193) + torch.optim.Adam.step() (built by build_optimizer, misc.py:186-205; tools/train.py:196) in ONE launch.
  *   table  [n_tensors][4] device pointers {param, grad, exp_avg, exp_avg_sq} (fp32, contiguous), itself in device memory
