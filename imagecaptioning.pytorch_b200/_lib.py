@@ -74,10 +74,14 @@ class RewardWeights(Structure):
     _fields_ = [('cider', c_double), ('bleu', c_double)]
 
 
+class SamplerOpts(Structure):
+    _fields_ = [('train_method', c_int), ('train_top', c_float), ('baseline_method', c_int), ('baseline_top', c_float), ('forced_baseline', c_void_p)]
+
+
 class ScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('drop_prob', c_float), ('upstream', c_float), ('baseline', c_int),
                 ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int), ('row_loss', c_void_p),
-                ('reward_weights', POINTER(RewardWeights))]
+                ('sampler', POINTER(SamplerOpts)), ('reward_weights', POINTER(RewardWeights))]
 
 
 BASELINE_GREEDY, BASELINE_LEAVE_ONE_OUT = 0, 1
@@ -87,7 +91,7 @@ class AoaScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('upstream', c_float), ('baseline', c_int),
                 ('drop_prob_lm', c_float), ('drop_attn', c_float), ('drop_aoa', c_float), ('drop_sublayer', c_float), ('ctx_drop', c_int),
                 ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int), ('row_loss', c_void_p),
-                ('reward_weights', POINTER(RewardWeights))]
+                ('sampler', POINTER(SamplerOpts)), ('reward_weights', POINTER(RewardWeights))]
 
 
 class AoaXeOpts(Structure):
@@ -159,7 +163,7 @@ class TfmXeOpts(Structure):
 class TfmScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('upstream', c_float), ('baseline', c_int),
                 ('drop_prob_lm', c_float), ('dropout', c_float), ('forced_tokens', c_void_p), ('att_masks', c_void_p), ('keep_rows', c_int),
-                ('row_loss', c_void_p), ('reward_weights', POINTER(RewardWeights))]
+                ('row_loss', c_void_p), ('sampler', POINTER(SamplerOpts)), ('reward_weights', POINTER(RewardWeights))]
 
 
 class VjpOpts(Structure):
@@ -276,6 +280,9 @@ SIGNATURES = {
     'capb200_aoa_set_grad_events': (c_int, [c_void_p, c_void_p, c_int]),
     'capb200_cider_table_create': (c_void_p, [c_void_p, c_void_p, c_long, c_double, c_void_p]),
     'capb200_cider_table_destroy': (None, [c_void_p]),
+    'capb200_cider_corpus_table_create': (c_void_p, []),
+    'capb200_cider_table_reserve': (c_int, [c_void_p, c_long, c_int]),
+    'capb200_cider_table_is_corpus': (c_int, [c_void_p]),
     'capb200_cider_scores': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'capb200_bleu4_scores': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     'capb200_weighted_reward': (c_int, [c_void_p, POINTER(RewardWeights), c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,

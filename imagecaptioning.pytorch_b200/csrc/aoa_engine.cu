@@ -581,7 +581,7 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](ATape& t, Arena& a) { layout_atape(t, a, B, R, N, T, E, H, heads, V1); })) return 1;
     // ---- (1) greedy baseline, eval mode: the regular decode path, forked here, enqueued after the prologue
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;         // decode workspace sized before anything is in flight
-    GreedyBaseline gb;
+    StepBaseline gb;
     if (gb.fork(ta, &e->side, &e->ev_fork, &e->ev_join, st)) return 1;
     const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
@@ -613,8 +613,8 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
 
     // ---- the greedy baseline's ~220 launches are enqueued only now: the side stream forked at the top of the step (it does not wait for the
     // prologue), but the host needs ~0.7 ms to enqueue them, and the main stream should be busy with the prologue meanwhile, not idle
-    if (gb.enqueue(B, T, V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, long long* seq, float* lp, void* s) {
-            return capb200_aoa_decode_sample(e, att, ta.mask, B, R, so, nullptr, 0, seq, lp, nullptr, s);
+    if (gb.enqueue(B, T, V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, const long long* tok, long long* seq, float* lp, void* s) {
+            return capb200_aoa_decode_sample(e, att, ta.mask, B, R, so, tok, tok ? T : 0, seq, lp, nullptr, s);
         })) return 1;
     // ---- (3) T sampling steps with the tape
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.s_tokens, 0, sizeof(int) * N, st));
@@ -765,7 +765,7 @@ extern "C" int capb200_aoa_scst_step(capb200_aoa_engine* e, const float* att, in
     const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
     CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
     const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->reward_weights};
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, opts->reward_weights};
     AoaTrainArgs ta;
     if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
@@ -820,7 +820,7 @@ extern "C" int capb200_aoa_scst_vjp(capb200_aoa_engine* e, const float* att, int
     const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
     CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
     const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, nullptr};
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, nullptr};
     AoaTrainArgs ta;
     if (scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
     ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;

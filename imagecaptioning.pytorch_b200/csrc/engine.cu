@@ -1210,12 +1210,12 @@ extern "C" int capb200_dropout_mask(float* mask, long n, unsigned long long seed
 
 namespace {
 
-// (1) of an SCST step with the greedy baseline: fork it and enqueue it right away on this engine's decode path (NewFC: att = null, R = 0).
-int start_greedy_baseline(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const StepTape& tp, GreedyBaseline& gb,
+// (1) of an SCST step with the eval-mode baseline: fork it and enqueue it right away on this engine's decode path (NewFC: att = null, R = 0).
+int start_baseline(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const StepTape& tp, StepBaseline& gb,
                           cudaStream_t st) {
     if (gb.fork(ta, &e->side, &e->ev_gfork, &e->ev_gjoin, st)) return 1;
-    return gb.enqueue(B, ta.T, e->V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, long long* seq, float* lp, void* s) {
-        return capb200_decode_sample(e, fc, att, ta.mask, B, R, so, nullptr, 0, seq, lp, nullptr, s);
+    return gb.enqueue(B, ta.T, e->V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, const long long* tok, long long* seq, float* lp, void* s) {
+        return capb200_decode_sample(e, fc, att, ta.mask, B, R, so, tok, tok ? ta.T : 0, seq, lp, nullptr, s);
     });
 }
 
@@ -1266,8 +1266,8 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     Tape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](Tape& t, Arena& a) { layout_tape(t, a, B, R, N, T, E, H, A, V1); })) return 1;
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;        // decode workspace sized before anything is in flight
-    GreedyBaseline gb;
-    if (start_greedy_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
+    StepBaseline gb;
+    if (start_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
     const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
 
@@ -1420,8 +1420,8 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
     MaxoutTape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](MaxoutTape& t, Arena& a) { layout_maxout_tape(t, a, B, R, N, T, E, H, A, V1); })) return 1;
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;
-    GreedyBaseline gb;
-    if (start_greedy_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
+    StepBaseline gb;
+    if (start_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
     const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
 
@@ -1531,8 +1531,8 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
     MaxoutTape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](MaxoutTape& t, Arena& a) { layout_newfc_tape(t, a, B, N, T, E, H, V1); })) return 1;
     if (ensure_workspace(e, B, N, 1, 1, st)) return 1;      // R = 1: the region count the greedy baseline's decode call sizes its workspace for
-    GreedyBaseline gb;
-    if (start_greedy_baseline(e, fc, nullptr, B, 0, ta, tp, gb, st)) return 1;
+    StepBaseline gb;
+    if (start_baseline(e, fc, nullptr, B, 0, ta, tp, gb, st)) return 1;
     const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
 
@@ -1808,6 +1808,21 @@ capb200_cider_table* capb200_cider_table_create(const int* keys, const double* d
     h->t = t;
     return h;
 }
+
+capb200_cider_table* capb200_cider_corpus_table_create(void) {
+    CiderTable* t = cider_corpus_table_create();
+    if (t == nullptr) return nullptr;
+    capb200_cider_table* h = new capb200_cider_table();
+    h->t = t;
+    return h;
+}
+
+int capb200_cider_table_reserve(capb200_cider_table* t, long n_refs, int L) {
+    CAPB_REQUIRE(t != nullptr, "null argument");
+    return cider_corpus_table_reserve(t->t, n_refs, L);
+}
+
+int capb200_cider_table_is_corpus(const capb200_cider_table* t) { return t != nullptr && cider_table_is_corpus(t->t) ? 1 : 0; }
 
 void capb200_cider_table_destroy(capb200_cider_table* t) {
     if (t == nullptr) return;

@@ -260,6 +260,12 @@ int cat_dropout_launch(int rows, int c1, int c2, const float* a, long ld_a, cons
 struct CiderTable;   // device hash table of n-gram -> idf
 CiderTable* cider_table_create(const int* keys, const double* df, long n, double ref_len, cudaStream_t stream);
 void cider_table_destroy(CiderTable* t);
+// corpus document frequencies (CiderD(df='corpus')): rebuilt on the device by every reward launch below from its own references
+CiderTable* cider_corpus_table_create();
+int cider_corpus_table_reserve(CiderTable* t, long n_refs, int L);
+bool cider_table_is_corpus(const CiderTable* t);
+int corpus_build_launches(const CiderTable* t);       // kernels a reward launch adds to build the table (3 for a corpus table, else 0)
+void cider_table_key(const CiderTable* t, unsigned long long key[3]);   // what a captured reward reads: slots, capacity - 1, table kind
 int cider_reward_launch(const CiderTable* t, const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs,
                         const int* ref_offsets, int L, double* scores, float* reward, long ld_reward, int reward_cols, cudaStream_t stream);
 // per-hypothesis BLEU-4 (float64), hypotheses and references laid out as for cider_reward_launch

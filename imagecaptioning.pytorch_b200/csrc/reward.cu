@@ -33,6 +33,10 @@ struct CiderTable {
     unsigned long long mask = 0;  // capacity - 1
     double log_ref_len = 0.0;
     long entries = 0;
+    // corpus mode (CiderD(df='corpus'), ciderD_scorer.py:143-147,182-186,210-216): the slots are rebuilt on the device from the references of
+    // every reward call; `used` [1] counts the occupied slots of the build under way
+    bool corpus = false;
+    unsigned int* used = nullptr;
 };
 
 __host__ __device__ inline unsigned long long cider_hash(int a, int b, int c, int d) {
@@ -84,10 +88,54 @@ CiderTable* cider_table_create(const int* keys, const double* df, long n, double
 void cider_table_destroy(CiderTable* t) {
     if (t == nullptr) return;
     cudaFree(t->slots);
+    if (t->used) cudaFree(t->used);
     delete t;
 }
 
+CiderTable* cider_corpus_table_create() {
+    CiderTable* t = new CiderTable();
+    t->corpus = true;
+    if (cudaMalloc(&t->used, sizeof(unsigned int)) != cudaSuccess) {
+        (void)cudaGetLastError();
+        set_error("cider_corpus_table_create: cudaMalloc failed");
+        delete t;
+        return nullptr;
+    }
+    return t;
+}
+
+// A corpus table holds at most every n-gram of `n_refs` reference rows of `L` tokens (4 orders x min(L, 64) positions each), at a load of at most
+// one half.  Growing frees the old slots after a device synchronisation; the slots' address is part of a step graph's key.
+int cider_corpus_table_reserve(CiderTable* t, long n_refs, int L) {
+    CAPB_REQUIRE(t != nullptr && t->corpus, "not a corpus CIDEr-D table");
+    CAPB_REQUIRE(n_refs >= 0 && L >= 0, "bad reference shape");
+    const long grams = (long)CIDER_N * n_refs * (L < CIDER_MAXL ? L : CIDER_MAXL);
+    unsigned long long cap = 64;
+    while (cap < (unsigned long long)(2 * grams + 2)) cap <<= 1;
+    if (t->slots != nullptr && cap <= t->mask + 1) return 0;
+    CAPB_CHECK_CUDA(cudaDeviceSynchronize());
+    if (t->slots) CAPB_CHECK_CUDA(cudaFree(t->slots));
+    t->slots = nullptr;
+    t->mask = 0;
+    CAPB_CHECK_CUDA(cudaMalloc(&t->slots, cap * sizeof(CiderSlot)));
+    t->mask = cap - 1;
+    return 0;
+}
+
+bool cider_table_is_corpus(const CiderTable* t) { return t != nullptr && t->corpus; }
+
+void cider_table_key(const CiderTable* t, unsigned long long key[3]) {
+    key[0] = t ? reinterpret_cast<unsigned long long>(t->slots) : 0ull;
+    key[1] = t ? t->mask : 0ull;
+    key[2] = t && t->corpus ? 1ull : 0ull;
+}
+
 namespace {
+
+__device__ __forceinline__ bool same_gram(const int* a, const int* b, int n) {
+    for (int i = 0; i < n; ++i) if (a[i] != b[i]) return false;
+    return true;
+}
 
 __device__ __forceinline__ double cider_idf(const CiderSlot* __restrict__ slots, unsigned long long mask, double log_ref_len, const int* tok, int n) {
     const int k0 = tok[0], k1 = n > 1 ? tok[1] : -1, k2 = n > 2 ? tok[2] : -1, k3 = n > 3 ? tok[3] : -1;
@@ -100,9 +148,93 @@ __device__ __forceinline__ double cider_idf(const CiderSlot* __restrict__ slots,
     }
 }
 
-__device__ __forceinline__ bool same_gram(const int* a, const int* b, int n) {
-    for (int i = 0; i < n; ++i) if (a[i] != b[i]) return false;
-    return true;
+
+// ---- corpus document frequencies, built on the device in three launches: clear, insert, finalise
+
+__global__ void corpus_clear_kernel(CiderSlot* __restrict__ slots, unsigned long long cap, unsigned int* used) {
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) *used = 0u;
+    if (i >= cap) return;
+    slots[i].key[0] = -2; slots[i].key[1] = -2; slots[i].key[2] = -2; slots[i].key[3] = -2;
+    slots[i].idf = 0.0;
+}
+
+// the tokens of reference row r up to and including its first 0, at most min(L, 64)
+__device__ __forceinline__ int ref_len(const int* __restrict__ refs, long r, int L) {
+    const int cols = L < CIDER_MAXL ? L : CIDER_MAXL;
+    int len = 0;
+    for (int j = 0; j < cols; ++j) { ++len; if (refs[r * L + j] == 0) break; }
+    return len;
+}
+
+// One CTA per image: every distinct n-gram of the image's references (set() over all of them, ciderD_scorer.py:143-147) adds `mult` -- the
+// number of scored hypotheses (crefs entries) of the image -- to its document frequency.  Thread items are (reference, order, position); an
+// item inserts when no earlier item of the image holds the same n-gram.  A slot is claimed by swapping its key[0] from -2 (empty) to -3
+// (being written); readers that meet -3 wait for the writer to publish key[0].  The occupied slots stay at most half the capacity (`used`),
+// so every probe sequence, here and in the scoring kernels' lookups, reaches an empty slot.
+__global__ void __launch_bounds__(256) corpus_insert_kernel(CiderSlot* __restrict__ slots, unsigned long long mask, unsigned int* used,
+                                                            const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L, double mult) {
+    const int img = blockIdx.x;
+    const int r0 = ref_offsets[img], r1 = ref_offsets[img + 1];
+    const int cols = L < CIDER_MAXL ? L : CIDER_MAXL;
+    const long items = (long)(r1 - r0) * CIDER_N * cols;
+    for (long it = threadIdx.x; it < items; it += blockDim.x) {
+        const long r = r0 + it / (CIDER_N * cols);
+        const int n = (int)((it / cols) % CIDER_N) + 1, p = (int)(it % cols);
+        const int len = ref_len(refs, r, L);
+        if (p + n > len) continue;
+        const int* g = refs + r * L + p;
+        bool first = true;
+        for (long q = r0; q <= r && first; ++q) {
+            const int lq = q == r ? p + n - 1 : ref_len(refs, q, L);          // earlier positions of this row, every position of earlier rows
+            for (int j = 0; j + n <= lq && first; ++j) first = !same_gram(g, refs + q * L + j, n);
+        }
+        if (!first) continue;
+        const int k0 = g[0], k1 = n > 1 ? g[1] : -1, k2 = n > 2 ? g[2] : -1, k3 = n > 3 ? g[3] : -1;
+        unsigned long long h = cider_hash(k0, k1, k2, k3) & mask;
+        for (unsigned long long probe = 0; probe <= mask; ++probe, h = (h + 1) & mask) {
+            CiderSlot* s = slots + h;
+            int cur = atomicCAS(&s->key[0], -2, -3);
+            if (cur == -2) {
+                if (atomicAdd(used, 1u) >= (unsigned int)((mask + 1) / 2)) { atomicExch(&s->key[0], -2); break; }    // over the reservation
+                s->key[1] = k1; s->key[2] = k2; s->key[3] = k3;
+                __threadfence();
+                atomicExch(&s->key[0], k0);
+                atomicAdd(&s->idf, mult);
+                break;
+            }
+            while (cur == -3) cur = *(volatile int*)&s->key[0];
+            __threadfence();
+            const volatile int* vk = s->key;
+            if (cur == k0 && vk[1] == k1 && vk[2] == k2 && vk[3] == k3) { atomicAdd(&s->idf, mult); break; }
+        }
+    }
+}
+
+// df -> log(ref_len) - log(max(1, df)), the weight the pickle table stores (cider_table_create)
+__global__ void corpus_finalise_kernel(CiderSlot* __restrict__ slots, unsigned long long cap, double log_ref_len) {
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= cap || slots[i].key[0] == -2) return;
+    const double df = slots[i].idf;
+    slots[i].idf = log_ref_len - log(df > 1.0 ? df : 1.0);
+}
+
+// Builds the corpus table for one reward call over `hyps` scored hypotheses, `per_image` of them per image, and returns its log(ref_len) =
+// log(hyps) (ciderD_scorer.py:182-186); a pickle table is left alone and returns its own.
+int corpus_build_launch(const CiderTable* t, int B, int hyps, int per_image, const int* refs, const int* ref_offsets, int L, double* log_ref_len,
+                        cudaStream_t stream) {
+    if (!t->corpus) { *log_ref_len = t->log_ref_len; return 0; }
+    CAPB_REQUIRE(t->slots != nullptr, "corpus CIDEr-D table without reserved slots (capb200_cider_table_reserve)");
+    *log_ref_len = log((double)hyps);
+    const unsigned long long cap = t->mask + 1;
+    const unsigned int grid = (unsigned int)((cap + 255) / 256);
+    corpus_clear_kernel<<<grid, 256, 0, stream>>>(t->slots, cap, t->used);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    corpus_insert_kernel<<<B, 256, 0, stream>>>(t->slots, t->mask, t->used, refs, ref_offsets, L, (double)per_image);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    corpus_finalise_kernel<<<grid, 256, 0, stream>>>(t->slots, cap, *log_ref_len);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 // Builds the tf-idf description of one caption held in shared memory.
@@ -393,7 +525,9 @@ int cider_reward_launch(const CiderTable* t, const long long* sampled, int S, co
     // greedy == nullptr: score the samples only; the reward baseline is then the mean of the image's other samples
     const int hyps = greedy != nullptr ? S + B : S;
     if (hyps == 0) return 0;
-    cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, t->log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    double log_ref_len = 0.0;
+    if (corpus_build_launch(t, B, hyps, hyps / B, refs, ref_offsets, L, &log_ref_len, stream)) return 1;
+    cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return baseline_reward_launch(scores, S, greedy, B, reward, ld_reward, reward_cols, stream);
 }
@@ -412,6 +546,8 @@ int weighted_reward_launches(double w_cider, double w_bleu, bool with_reward) {
     return (w_cider > 0.0) + (w_bleu > 0.0) + 1 + (with_reward ? 1 : 0);
 }
 
+int corpus_build_launches(const CiderTable* t) { return t != nullptr && t->corpus ? 3 : 0; }
+
 int weighted_reward_launch(const CiderTable* t, double w_cider, double w_bleu, const long long* sampled, int S, const long long* greedy, int B, int T,
                            const int* refs, const int* ref_offsets, int L, double* scores, double* bleu, float* reward, long ld_reward, int reward_cols,
                            cudaStream_t stream) {
@@ -422,7 +558,9 @@ int weighted_reward_launch(const CiderTable* t, double w_cider, double w_bleu, c
     const int hyps = greedy != nullptr ? S + B : S;
     if (hyps == 0) return 0;
     if (w_cider > 0.0) {
-        cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, t->log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+        double log_ref_len = 0.0;
+        if (corpus_build_launch(t, B, hyps, hyps / B, refs, ref_offsets, L, &log_ref_len, stream)) return 1;
+        cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
         CAPB_CHECK_CUDA(cudaGetLastError());
     }
     if (w_bleu > 0.0 && bleu_scores_launch(sampled, S, greedy, B, T, refs, ref_offsets, L, bleu, stream)) return 1;

@@ -470,7 +470,7 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
 
     // ---- greedy baseline (eval mode): the regular K/V-cached decode, forked here, enqueued after the encoder
     if (!ta.xe && ta.greedy_baseline && ensure_workspace(e, B, B, R, 1, st)) return 1;
-    GreedyBaseline gb;
+    StepBaseline gb;
     if (gb.fork(ta, &e->side, &e->ev_fork, &e->ev_join, st)) return 1;
     const Skinny sk = step_gemms(&e->tf32, e->tc, tp, st);
     const long tf32_l0 = tf32_context_launches(e->tf32);
@@ -503,8 +503,8 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
 
     // ---- the greedy baseline's launches are enqueued only now: its stream forked at the top of the step, and while the host enqueues
     // them the main stream is busy with the encoder instead of idle
-    if (gb.enqueue(B, e->T, V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, long long* seq, float* lp, void* s) {
-            return capb200_tfm_decode_sample(e, att, ta.mask, B, R, so, nullptr, 0, seq, lp, nullptr, s);
+    if (gb.enqueue(B, e->T, V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, const long long* tok, long long* seq, float* lp, void* s) {
+            return capb200_tfm_decode_sample(e, att, ta.mask, B, R, so, tok, tok ? e->T : 0, seq, lp, nullptr, s);
         })) return 1;
 
     // ---- decoder forward over positions [t0, t1)
@@ -696,7 +696,7 @@ extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, in
     CAPB_REQUIRE(R >= 1, "attention features required");
     CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
     const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->reward_weights};
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, opts->reward_weights};
     TfmTrainArgs ta;
     if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     ta.p_lm = opts->drop_prob_lm;
@@ -727,7 +727,7 @@ extern "C" int capb200_tfm_scst_vjp(capb200_tfm_engine* e, const float* att, int
     CAPB_REQUIRE(R >= 1, "attention features required");
     CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
     const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, nullptr};
+                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, nullptr};
     TfmTrainArgs ta;
     if (scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
     ta.p_lm = opts->drop_prob_lm;

@@ -39,15 +39,34 @@ struct TrainArgs {
     // the autograd entry points (capb200_*_vjp): stop after the forward, or replace the criterion by an outside dL/dlogprobs [N, Tl, V1]
     bool forward_only = false;
     const float* dlogprobs = nullptr;
-    bool greedy = false;                    // SCST form: draw the argmax instead of a multinomial sample
+    // SCST: how the samples are drawn -- the vocabulary step's select code (1 argmax, 2 multinomial, 4 top-k, 5 nucleus) and its k or p --
+    // and how the eval-mode baseline is drawn (CAPB200_SAMPLE_*; forced_baseline [B, T] replays given captions instead)
+    int select = 2;
+    float top = 0.f;
+    int baseline_method = CAPB200_SAMPLE_GREEDY;
+    float baseline_top = 0.f;
+    const long long* forced_baseline = nullptr;
 
     // The weighted reward runs only when it can differ from CIDEr-D alone: a BLEU weight <= 0 adds weight * 0.
     bool weighted_reward() const { return !xe && (w_bleu > 0.0 || w_cider != 1.0); }
-    // kernels the weighted reward adds to the CIDEr-D reward's two (scores, reward)
-    int reward_extra_launches() const { return weighted_reward() ? weighted_reward_launches(w_cider, w_bleu, true) - 2 : 0; }
+    // kernels the weighted reward and a corpus table's build add to the CIDEr-D reward's two (scores, reward)
+    int reward_extra_launches() const {
+        const int build = table != nullptr && (!weighted_reward() || w_cider > 0.0) ? corpus_build_launches(table->t) : 0;
+        return (weighted_reward() ? weighted_reward_launches(w_cider, w_bleu, true) - 2 : 0) + build;
+    }
 };
 
 inline int vjp_train_args(const capb200_vjp_opts* v, TrainArgs* ta);
+
+// A sampling method of capb200_sampler_opts -> the vocabulary step's select code, after checking its k or p.
+inline int sampler_select(int method, float top, int* select) {
+    CAPB_REQUIRE(method == CAPB200_SAMPLE_GREEDY || method == CAPB200_SAMPLE_MULTINOMIAL || method == CAPB200_SAMPLE_TOPK || method == CAPB200_SAMPLE_TOPP,
+                 "unknown sampling method (greedy, multinomial, top-k or nucleus)");
+    if (method == CAPB200_SAMPLE_TOPK) CAPB_REQUIRE(top >= 1.f && top <= 1e9f, "top-k sampling needs k >= 1");
+    if (method == CAPB200_SAMPLE_TOPP) CAPB_REQUIRE(top > 0.f && top < 1.f, "nucleus sampling needs 0 < p < 1");
+    *select = method == CAPB200_SAMPLE_GREEDY ? 1 : (method == CAPB200_SAMPLE_MULTINOMIAL ? 2 : method);
+    return 0;
+}
 
 // Checks the SCST options every family shares and fills `ta`.  A family hands its own options over as capb200_scst_opts (drop_prob = its
 // main dropout rate) and checks its other rates itself.  With `vjp` (an autograd entry point) no reward runs: the baseline is not read.
@@ -64,6 +83,18 @@ inline int scst_train_args(int B, const capb200_scst_opts& o, const capb200_cide
     CAPB_REQUIRE(o.drop_prob >= 0.f && o.drop_prob < 1.f, "dropout rates must be in [0, 1)");
     CAPB_REQUIRE(o.temperature > 0.f, "temperature must be positive");
     CAPB_REQUIRE(o.keep_rows >= 0 && o.keep_rows <= B * o.sample_n, "keep_rows must be in 0..rows");
+    if (o.sampler != nullptr) {
+        const capb200_sampler_opts& s = *o.sampler;
+        CAPB_REQUIRE(vjp == nullptr, "the autograd entry points draw through vjp->greedy or forced tokens, not a sampler struct");
+        int baseline_select = 0;
+        if (sampler_select(s.train_method, s.train_top, &ta->select) || sampler_select(s.baseline_method, s.baseline_top, &baseline_select)) return 1;
+        CAPB_REQUIRE(greedy_baseline || (s.baseline_method == CAPB200_SAMPLE_GREEDY && s.forced_baseline == nullptr),
+                     "a sampled or forced baseline needs CAPB200_BASELINE_GREEDY");
+        ta->top = s.train_method == CAPB200_SAMPLE_TOPK || s.train_method == CAPB200_SAMPLE_TOPP ? s.train_top : 0.f;
+        ta->baseline_method = s.baseline_method;
+        ta->baseline_top = s.baseline_method == CAPB200_SAMPLE_TOPK || s.baseline_method == CAPB200_SAMPLE_TOPP ? s.baseline_top : 0.f;
+        ta->forced_baseline = s.forced_baseline;
+    }
     if (o.reward_weights != nullptr) {
         CAPB_REQUIRE(std::isfinite(o.reward_weights->cider) && std::isfinite(o.reward_weights->bleu), "reward weights must be finite");
         ta->w_cider = o.reward_weights->cider; ta->w_bleu = o.reward_weights->bleu;
@@ -102,7 +133,7 @@ inline int vjp_train_args(const capb200_vjp_opts* v, TrainArgs* ta) {
     CAPB_REQUIRE(ta->xe || !v->greedy || ta->forced == nullptr, "greedy draws and forced tokens exclude each other");
     ta->forward_only = v->forward_only != 0;
     ta->dlogprobs = ta->forward_only ? nullptr : v->dlogprobs;
-    ta->greedy = v->greedy != 0;
+    if (v->greedy) ta->select = 1;
     ta->greedy_baseline = false;
     return 0;
 }
@@ -155,17 +186,27 @@ inline Skinny step_gemms(Tf32Context** ctx, bool tc, const StepTape& tp, cudaStr
     return sk;
 }
 
-// The eval-mode greedy baseline of an SCST step: the regular greedy decode on B rows, without dropout.  It and the train-mode sampling
+// The eval-mode baseline of an SCST step: the regular decode on B rows, without dropout -- greedy, or drawn as sc_sample_method says from the
+// step's seed XOR kBaselineSalt (an XOR, so that the salt of a graph replay carries over: dropout.cuh), or the replay of given captions.  It and the train-mode sampling
 // forward are independent chains of small, latency-bound kernels, so the baseline runs on the engine's side stream -- forked from the step's
 // stream, joined before the reward -- unless CAPB200_SCST_SERIAL_GREEDY is set or the side stream cannot be created.  Three calls: fork at
 // the top of the step, enqueue where the family wants its launches issued, join (inside loss_backward).
-struct GreedyBaseline {
+struct StepBaseline {
+    static constexpr unsigned long long kBaselineSalt = 0x5bd1e9955bd1e995ull;
     bool needed = false;
     cudaStream_t st = nullptr;      // where its launches go
     cudaEvent_t done = nullptr;     // recorded on the side stream after them; null when they run on the step's stream
+    int method = CAPB200_SAMPLE_GREEDY;
+    float top = 0.f;
+    unsigned long long seed = 0;
+    const long long* forced = nullptr;
 
     int fork(const TrainArgs& ta, cudaStream_t* side, cudaEvent_t* ev_fork, cudaEvent_t* ev_join, cudaStream_t step_st) {
         needed = !ta.xe && ta.greedy_baseline;
+        forced = ta.forced_baseline;
+        method = forced != nullptr ? CAPB200_SAMPLE_FORCED : ta.baseline_method;
+        top = ta.baseline_top;
+        seed = method == CAPB200_SAMPLE_GREEDY || method == CAPB200_SAMPLE_FORCED ? 0ull : ta.seed ^ kBaselineSalt;
         st = step_st;
         done = nullptr;
         static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
@@ -180,17 +221,17 @@ struct GreedyBaseline {
         done = *ev_join;
         return 0;
     }
-    // decode(opts, greedy_seq, logprobs, stream) is the family's capb200_*decode_sample
+    // decode(opts, tokens_in, greedy_seq, logprobs, stream) is the family's capb200_*decode_sample (tokens_in [B, T]: the forced captions or null)
     template <class Decode>
     int enqueue(int B, int T, int V1, long long* greedy_seq, float* glp, Decode decode) const {
         if (!needed) return 0;
-        CAPB_NVTX("capb200 scst: greedy baseline (eval mode, side stream)");
+        CAPB_NVTX("capb200 scst: baseline (eval mode, side stream)");
         capb200_sample_opts so;
         memset(&so, 0, sizeof(so));
-        so.edits.unk_col = -1; so.sample_n = 1; so.method = CAPB200_SAMPLE_GREEDY; so.temperature = 1.f; so.seed = 0; so.steps = T;
+        so.edits.unk_col = -1; so.sample_n = 1; so.method = method; so.temperature = 1.f; so.seed = seed; so.steps = T; so.top = top;
         CAPB_CHECK_CUDA(cudaMemsetAsync(glp, 0, sizeof(float) * (size_t)B * T * V1, st));
         CAPB_CHECK_CUDA(cudaMemsetAsync(greedy_seq, 0, sizeof(long long) * (size_t)B * T, st));
-        if (decode(&so, greedy_seq, glp, static_cast<void*>(st))) return 1;
+        if (decode(&so, forced, greedy_seq, glp, static_cast<void*>(st))) return 1;
         if (done != nullptr) CAPB_CHECK_CUDA(cudaEventRecord(done, st));
         return 0;
     }
@@ -214,13 +255,14 @@ inline int feed_tokens(const TrainArgs& ta, const StepTape& tp, int N, int V1, i
     return 0;
 }
 
-// The vocabulary step at step t: log_softmax of the logits at ta.logprobs[:, t] in place; SCST also draws the next words (multinomial at
-// ta.temperature, or the replay of ta.forced) into tp.s_tokens and ta.sample_seq.
+// The vocabulary step at step t: log_softmax of the logits at ta.logprobs[:, t] in place; SCST also draws the next words (ta.select at
+// ta.temperature, or the replay of ta.forced) into tp.s_tokens and ta.sample_seq.  The full log-softmax row stays in ta.logprobs whatever
+// the sampler keeps: it is what the criterion and the gradient read (AttModel.py:337,347).
 inline int train_vocab_step(const TrainArgs& ta, const StepTape& tp, int N, int V1, int t, cudaStream_t st) {
     VocabStepArgs va;
     va.rows = N; va.V1 = V1; va.logits = ta.logprobs + (long)t * V1; va.ld = (long)ta.Tl * V1;
     if (!ta.xe) {
-        va.select = ta.greedy ? 1 : 2; va.temperature = ta.temperature; va.seed = ta.seed; va.step = (unsigned long long)t;
+        va.select = ta.select; va.top = ta.top; va.temperature = ta.temperature; va.seed = ta.seed; va.step = (unsigned long long)t;
         va.unfinished = tp.s_unfinished; va.first_step = (t == 0); va.tokens_out = tp.s_tokens;
         va.seq_out = ta.sample_seq; va.ld_seq = ta.T; va.t = t;
         if (ta.forced != nullptr) {
@@ -233,7 +275,7 @@ inline int train_vocab_step(const TrainArgs& ta, const StepTape& tp, int N, int 
 
 // The loss and d loss / d logits into tp.DL: the XE criterion (LanguageModelCriterion / LabelSmoothing), or -- after joining the greedy
 // baseline -- the reward (CIDEr-D, or the weighted CIDEr-D + BLEU-4), RewardCriterion, drop_worst and the d logits of the SCST loss.
-inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBaseline& gb, int B, int N, int V1, cudaStream_t st) {
+inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const StepBaseline& gb, int B, int N, int V1, cudaStream_t st) {
     const int T = ta.T;
     const long ld_lp = (long)ta.Tl * V1;
     float* row_loss = ta.row_loss ? ta.row_loss : tp.row_loss;
@@ -256,7 +298,7 @@ inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBa
 
 // loss_backward, then the backward of a logit layer [V1, H] batched over all (n, t): dOUT [N, T, H] = DL W, and the logit gradients (group
 // 0, whose event `ev` is recorded here).  `out` holds the layer's inputs [N, T, H].
-inline int loss_and_logit_backward(const TrainArgs& ta, const StepTape& tp, const GreedyBaseline& gb, const Skinny& sk, int B, int N, int V1, int H,
+inline int loss_and_logit_backward(const TrainArgs& ta, const StepTape& tp, const StepBaseline& gb, const Skinny& sk, int B, int N, int V1, int H,
                                    const float* logit_w, const float* out, float* dOUT, float* g_logit_w, float* g_logit_b, cudaEvent_t ev, cudaStream_t st) {
     const int TN = ta.T * N;
     if (loss_backward(ta, tp, gb, B, N, V1, st)) return 1;
@@ -314,10 +356,10 @@ int run_vjp_step(Engine* e, cudaStream_t st, Step step) {
 // ~2 us on the stream, the host needs milliseconds to enqueue them, and nothing about the sequence depends on data: the step is captured the
 // second time a configuration is seen and replayed afterwards with a fresh seed (dropout.cuh: seed salt).  The features fc / att and the
 // region mask ta.mask are copied into the engine-owned staging buffer first, so that the graph reads stable addresses (an input of zero
-// bytes is not staged and reaches the step as null); the key covers every option but the seed (the reward weights by value), the gradient and
+// bytes is not staged and reaches the step as null); the key covers every option but the seed (the samplers and the reward weights by value), the gradient and
 // weight tables, every pointer the step touches and the shapes.  The gradient-group events a data-parallel caller listens to become external event-record nodes of the
 // graph (record_group_event) and are part of the key; CAPB200_SCST_GRAPH_SYNC=0 keeps the step eager while any is set.  The step also stays
-// eager with CAPB200_SCST_GRAPH=0, in the simt_fp32 mode, when forced tokens are replayed, and once a capture has failed.
+// eager with CAPB200_SCST_GRAPH=0, in the simt_fp32 mode, when forced samples or baseline captions are replayed, and once a capture has failed.
 template <class Engine, class Opts, class Grads, class Args, class Step>
 int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& ta, const float* fc, size_t fc_bytes, const float* att, size_t att_bytes,
                   int B, int R, cudaStream_t st, Step step) {
@@ -330,7 +372,7 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
         e->launches += t.reward_extra_launches();
         return rc;
     };
-    if (!StepGraph::enabled() || !e->tc || (listening && !graph_with_listener) || ta.forced != nullptr || e->sg.broken)
+    if (!StepGraph::enabled() || !e->tc || (listening && !graph_with_listener) || ta.forced != nullptr || ta.forced_baseline != nullptr || e->sg.broken)
         return run_eager_step(st, [&] { return counted(fc, att, ta, st); });
     cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
     const void* srcs[3] = {fc, att, ta.mask};
@@ -341,10 +383,15 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
     Args ts = ta;
     ts.mask = staged(2);
     unsigned long long key = 1469598103934665603ull;
-    Opts o2 = *opts; o2.seed = 0; o2.att_masks = ts.mask; o2.reward_weights = nullptr;
+    Opts o2 = *opts; o2.seed = 0; o2.att_masks = ts.mask; o2.sampler = nullptr; o2.reward_weights = nullptr;
     StepGraph::mix(key, &o2, sizeof(o2));
-    const double weights[2] = {ta.w_cider, ta.w_bleu};      // the values: the caller's struct may keep its address while they change
-    StepGraph::mix(key, weights, sizeof(weights)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
+    const double weights[2] = {ta.w_cider, ta.w_bleu};      // the values: the caller's structs may keep their addresses while they change
+    StepGraph::mix(key, weights, sizeof(weights));
+    const int methods[2] = {ta.select, ta.baseline_method};
+    const float tops[2] = {ta.top, ta.baseline_top};
+    unsigned long long table_key[3];                          // a corpus table's slots move when it grows; the kind decides the build
+    cider_table_key(ta.table ? ta.table->t : nullptr, table_key);
+    StepGraph::mix(key, methods, sizeof(methods)); StepGraph::mix(key, tops, sizeof(tops)); StepGraph::mix(key, table_key, sizeof(table_key)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
     const void* ptrs[] = {ta.table, ta.refs, ta.ref_offsets, ta.sample_seq, ta.greedy_seq, ta.logprobs, ta.reward, ta.loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
     StepGraph::mix(key, ptrs, sizeof(ptrs));
     StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));

@@ -3,7 +3,8 @@
     B200LossWrapper(model, opt).forward(fc_feats, att_feats, labels, masks, att_masks, gts, gt_indices,
                                         sc_flag, struc_flag, drop_worst_flag) -> {'loss', 'reward'}
 
-sc_flag=True follows loss_wrapper.py:56-73 exactly: eval-mode greedy baseline, train-mode multinomial samples, the self-critical
+sc_flag=True follows loss_wrapper.py:56-73 exactly: the eval-mode baseline (opt.sc_sample_method), the train-mode samples
+(opt.train_sample_method: 'sample', 'greedy', 'gumbel', 'top<k>' or 'top<p>'), the self-critical
 reward (``cider_reward_weight * CIDEr-D + bleu_reward_weight * BLEU-4``) and RewardCriterion -- every stage on the device through the C ABI.  sc_flag=False is the XE stage
 (loss_wrapper.py:54-55: teacher-forced forward + LanguageModelCriterion / LabelSmoothing) and struc_flag=True the structure-loss
 branch (loss_wrapper.py:25-53) with ``structure_loss_type='new_self_critical'`` (losses.py:168-187), the recipe of the reference's
@@ -45,6 +46,21 @@ class RewardCriterion(nn.Module):
         _lib.check(_lib.load().capb200_reward_criterion_backward(_lib.ptr(sq), _lib.ptr(rw), N, L, V1, _lib.ptr(self.mask_sum), float(upstream),
                                                                  _lib.ptr(grad), _lib.current_stream()), 'reward_criterion_backward')
         return grad
+
+
+_FUSED_SAMPLERS = "'sample', 'greedy', 'gumbel', 'top<k>' or 'top<p>' with beam size 1"
+
+
+def _fused_sampler(method):
+    """Whether the fused steps draw with ``method`` (CaptionModel.sample_next_word's methods; beam search and the others are not)."""
+    if method in ('sample', 'greedy', 'gumbel'):
+        return True
+    if not (isinstance(method, str) and method.startswith('top')):
+        return False
+    try:
+        return float(method[3:]) > 0
+    except ValueError:
+        return False
 
 
 def _shifted_mask(seq):
@@ -274,7 +290,11 @@ class B200LossWrapper(nn.Module):
         keep = self._keep_rows(len(gts) * opt.train_sample_n, drop_worst_flag)
         # the reference's training-time _sample call passes no temperature (loss_wrapper.py:63-67): 1.0, whatever opt.temperature says
         w = self._weights()
-        extra = {} if w is None else {'reward_weights': w}          # the default weights call the step exactly as before
+        extra = {} if w is None else {'reward_weights': w}          # the default weights and samplers call the step exactly as before
+        if opt.train_sample_method != 'sample':
+            extra['sample_method'] = opt.train_sample_method
+        if baseline == 'greedy' and opt.sc_sample_method != 'greedy':
+            extra['baseline_method'] = opt.sc_sample_method
         res = self.model.scst_step(fc_feats, att_feats, gts, self._scorer(), opt.train_sample_n, temperature=1.0, baseline=baseline, att_masks=att_masks,
                                    keep_rows=keep, **extra)
         res['keep_rows'] = keep
@@ -286,7 +306,7 @@ class B200LossWrapper(nn.Module):
         out = {}
         reduction = 'none' if drop_worst_flag else 'mean'
         can_fuse = (hasattr(self.model, 'scst_step') and torch.is_grad_enabled() and
-                    opt.train_sample_method == 'sample' and opt.train_beam_size == 1)
+                    _fused_sampler(opt.train_sample_method) and opt.train_beam_size == 1)
         if struc_flag:
             w = opt.structure_loss_weight
             lm_loss = self._xe_loss(fc_feats, att_feats, labels, masks, att_masks, drop_worst_flag, snapshot=w > 0) if w < 1 else \
@@ -312,7 +332,7 @@ class B200LossWrapper(nn.Module):
         if not sc_flag:
             out['loss'] = self._xe_loss(fc_feats, att_feats, labels, masks, att_masks, drop_worst_flag)
             return out
-        if can_fuse and opt.sc_sample_method == 'greedy' and opt.sc_beam_size == 1:
+        if can_fuse and _fused_sampler(opt.sc_sample_method) and opt.sc_beam_size == 1:
             # whole step on the device incl. the backward pass; dropout as in model.train()
             gts = [gts[_] for _ in gt_indices.tolist()]
             res = self._sampled_step(fc_feats, att_feats, gts, 'greedy', att_masks, drop_worst_flag)
@@ -325,10 +345,10 @@ class B200LossWrapper(nn.Module):
             why = []
             if not hasattr(self.model, 'scst_step'):
                 why.append('model family %r has no fused SCST step (UpDown, Att2in2, NewFC, AoANet and Transformer do)' % getattr(self.model, 'family_name', type(self.model).__name__))
-            if opt.train_sample_method != 'sample' or opt.train_beam_size != 1:
-                why.append('train_sample_method / train_beam_size other than multinomial sampling')
-            if opt.sc_sample_method != 'greedy' or opt.sc_beam_size != 1:
-                why.append('sc_sample_method / sc_beam_size other than a greedy baseline')
+            if not _fused_sampler(opt.train_sample_method) or opt.train_beam_size != 1:
+                why.append('train_sample_method / train_beam_size other than ' + _FUSED_SAMPLERS)
+            if not _fused_sampler(opt.sc_sample_method) or opt.sc_beam_size != 1:
+                why.append('sc_sample_method / sc_beam_size other than a baseline drawn by ' + _FUSED_SAMPLERS)
             raise NotImplementedError('self-critical training step outside the fused engine path: ' + '; '.join(why or ['unsupported configuration']))
         # no-grad evaluation of the sc branch (reward monitoring): host-level composition of the engine calls, dropout off
         self.model.eval()

@@ -110,6 +110,44 @@ def _on_device(fn):
     return wrapped
 
 
+def sampling_method(sample_method):
+    """The engine's form of a reference ``sample_method`` (CaptionModel.sample_next_word, CaptionModel.py:370-407): (CAPB200_SAMPLE_* code,
+    top, gumbel).  'gumbel' is the argmax of logprobs + Gumbel noise, a multinomial draw at temperature 1 (the caller pins the temperature);
+    'top<x>' is nucleus sampling for 0 < x < 1 and top-k sampling with k = int(x) otherwise."""
+    if sample_method == 'greedy':
+        return _lib.SAMPLE_GREEDY, 0.0, False
+    if sample_method == 'sample':
+        return _lib.SAMPLE_MULTINOMIAL, 0.0, False
+    if sample_method == 'gumbel':
+        return _lib.SAMPLE_MULTINOMIAL, 0.0, True
+    if isinstance(sample_method, str) and sample_method.startswith('top'):
+        top = float(sample_method[3:])
+        if not top > 0:
+            raise ValueError('sample_method %r: top-k needs k >= 1, nucleus sampling 0 < p < 1' % sample_method)
+        return (_lib.SAMPLE_TOPP if top < 1 else _lib.SAMPLE_TOPK), top, False
+    raise NotImplementedError("sample_method %r is out of scope of the engine" % sample_method)
+
+
+def _scst_sampler(sample_method, baseline_method, forced_baseline, loo, B, T, V1, temperature, dev):
+    """(capb200_sampler_opts pointer or None, what must outlive the call, the samples' temperature) of a fused SCST step.  The default
+    multinomial samples with the greedy baseline pass no struct, so the step runs exactly as it did before samplers were selectable."""
+    if sample_method == 'sample' and baseline_method == 'greedy' and forced_baseline is None:
+        return None, None, temperature
+    train, train_top, gumbel = sampling_method(sample_method)
+    base, base_top, _ = sampling_method(baseline_method)
+    for top in (train_top, base_top):
+        if top >= 1 and int(top) > V1:
+            raise ValueError('top-k sampling needs k <= vocab_size + 1 (%d), got %d' % (V1, int(top)))
+    if loo and (base != _lib.SAMPLE_GREEDY or forced_baseline is not None):
+        raise ValueError("the leave-one-out baseline draws no baseline captions: baseline_method belongs to baseline='greedy'")
+    fb = None
+    if forced_baseline is not None:       # replay given baseline captions (parity tests against the reference's own draw)
+        fb = forced_baseline.detach().to(device=dev, dtype=torch.long).contiguous()
+        assert fb.shape == (B, T)
+    so = _lib.SamplerOpts(train, train_top, base, base_top, _lib.ptr(fb))
+    return ctypes.pointer(so), (so, fb), 1.0 if gumbel else temperature
+
+
 def _slot_property(field):
     def get(self):
         return self._store.slot(getattr(_tls, 'dev', None))[field]
@@ -348,20 +386,10 @@ class B200CaptionModel(nn.Module):
         top = 0.0
         if forced_tokens is not None:
             method = _lib.SAMPLE_FORCED
-        elif sample_method == 'greedy':
-            method = _lib.SAMPLE_GREEDY
-        elif sample_method == 'sample':
-            method = _lib.SAMPLE_MULTINOMIAL
-        elif sample_method == 'gumbel':
-            # argmax(logprobs + Gumbel noise) / temperature-free: a multinomial draw at temperature 1 (CaptionModel.py:375-385)
-            method, temperature = _lib.SAMPLE_MULTINOMIAL, 1.0
-        elif sample_method.startswith('top'):
-            top = float(sample_method[3:])           # CaptionModel.py:387-402: 0 < x < 1 nucleus, else top-k
-            if top <= 0:
-                raise ValueError('sample_method %r: top-k needs k >= 1, nucleus sampling 0 < p < 1' % sample_method)
-            method = _lib.SAMPLE_TOPP if top < 1 else _lib.SAMPLE_TOPK
         else:
-            raise NotImplementedError("sample_method %r is out of scope of the engine" % sample_method)
+            method, top, gumbel = sampling_method(sample_method)
+            if gumbel:
+                temperature = 1.0
         lib = self._ensure_engine(fc_feats.device)
         fc = self._f32(fc_feats)
         att, masks = self._clip(att_feats, att_masks)
@@ -693,15 +721,21 @@ class _FusedTrainSteps:
     # ---- SCST training step: greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----------------
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
-                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None):
+                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None, sample_method='sample', baseline_method='greedy',
+                  forced_baseline=None):
         """Runs one self-critical step entirely on the device (capb200_updown_scst_step and its Att2in2 / NewFC counterparts).  Returns a
         dict with 'loss' (0-dim), 'reward' [N, T], 'sample_seq', 'greedy_seq', 'sample_logprobs' and 'grads' {parameter: gradient tensor}.
         ``baseline='greedy'`` is the self-critical step (loss_wrapper.py:56-73); ``'leave_one_out'`` the 'new_self_critical' structure
         loss (losses.py:168-187): no greedy decode, each sample is scored against the mean of the image's other samples, and the
         result carries 'scores' [B, n] (the raw CIDEr-D values the reference reports as out['reward']).  ``reward_weights`` = (cider, bleu)
-        scores each caption with cider * CIDEr-D + bleu * BLEU-4 (opts.py:169-172); None is CIDEr-D alone."""
+        scores each caption with cider * CIDEr-D + bleu * BLEU-4 (opts.py:169-172); None is CIDEr-D alone.  ``sample_method`` draws the
+        train-mode samples and ``baseline_method`` the eval-mode baseline (LossWrapper's train_sample_method / sc_sample_method: 'sample',
+        'greedy', 'gumbel', 'top<k>', 'top<p>'); the loss and the gradients read the full log-softmax rows whatever the sampler keeps.
+        ``forced_baseline`` [B, T] replays given baseline captions, as ``forced_tokens`` [N, T] replays samples."""
         from .rewards import pack_references, weights_struct
         rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
+        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', fc_feats.shape[0],
+                                                    self.seq_length, self.vocab_size + 1, temperature, fc_feats.device)
         lib = self._ensure_engine(fc_feats.device)
         fc, att, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
         dev = fc.device
@@ -727,8 +761,8 @@ class _FusedTrainSteps:
             assert forced.shape == (N, T)
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None      # drop_worst: per-row losses (reduction 'none')
         so = _lib.ScstOpts(sample_n, float(temperature), seed, float(p), float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY,
-                           _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), None if rw is None else ctypes.pointer(rw))
-        _lib.check(getattr(lib, self._scst_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs),
+                           _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), sampler, None if rw is None else ctypes.pointer(rw))
+        _lib.check(getattr(lib, self._scst_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs),
                                                   _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq), _lib.ptr(greedy_seq), _lib.ptr(logprobs),
                                                   _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), self._scst_entry[len('capb200_'):])
         res = {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
@@ -1178,12 +1212,15 @@ class B200TransformerModel(B200CaptionModel):
 
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy', dropout=None,
-                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None):
+                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None, sample_method='sample', baseline_method='greedy',
+                  forced_baseline=None):
         """One self-critical step of the Transformer on the device (capb200_tfm_scst_step): eval-mode greedy baseline (or leave-one-out),
         train-mode samples drawn position by position on the K/V tape, CIDEr-D (or weighted, ``reward_weights``) reward, RewardCriterion,
-        batched backward.  Result as B200UpDownModel.scst_step."""
+        batched backward.  ``sample_method`` / ``baseline_method`` / ``forced_baseline`` and the result as B200UpDownModel.scst_step."""
         from .rewards import pack_references, weights_struct
         rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
+        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', att_feats.shape[0],
+                                                    self.seq_length, self.vocab_size + 1, temperature, att_feats.device)
         lib = self._ensure_engine(att_feats.device)
         att, masks = self._clip(att_feats, att_masks)
         dev = att.device
@@ -1208,8 +1245,9 @@ class B200TransformerModel(B200CaptionModel):
             assert forced.shape == (N, T)
         row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
         so = _lib.TfmScstOpts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, float(p_lm),
-                              float(p), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), None if rw is None else ctypes.pointer(rw))
-        _lib.check(lib.capb200_tfm_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs), _lib.ptr(offsets), L,
+                              float(p), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), sampler,
+                              None if rw is None else ctypes.pointer(rw))
+        _lib.check(lib.capb200_tfm_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs), _lib.ptr(offsets), L,
                                              ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq), _lib.ptr(logprobs),
                                              _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'tfm_scst_step')
         return {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
@@ -1346,13 +1384,17 @@ class B200AoAModel(B200CaptionModel):
 
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
-                  drop_attn=0.1, drop_aoa=None, drop_sublayer=0.1, ctx_drop=None, forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None):
+                  drop_attn=0.1, drop_aoa=None, drop_sublayer=0.1, ctx_drop=None, forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None,
+                  sample_method='sample', baseline_method='greedy', forced_baseline=None):
         """One self-critical step of AoANet on the device (capb200_aoa_scst_step): eval-mode greedy baseline (or the leave-one-out baseline of
         'new_self_critical'), train-mode samples with every dropout site of AoAModel.py active, CIDEr-D reward, RewardCriterion, BPTT through
-        the decoder and the six refiner layers.  ``fc_feats`` is unused (mean_feats=1).  ``reward_weights`` as in B200UpDownModel.scst_step.
+        the decoder and the six refiner layers.  ``fc_feats`` is unused (mean_feats=1).  ``reward_weights``, ``sample_method``,
+        ``baseline_method`` and ``forced_baseline`` as in B200UpDownModel.scst_step.
         Returns the dict of B200UpDownModel.scst_step."""
         from .rewards import pack_references, weights_struct
         rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
+        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', att_feats.shape[0],
+                                                    self.seq_length, self.vocab_size + 1, temperature, att_feats.device)
         lib = self._ensure_engine(att_feats.device)
         att, masks = self._clip(att_feats, att_masks)
         dev = att.device
@@ -1379,8 +1421,8 @@ class B200AoAModel(B200CaptionModel):
         so = _lib.AoaScstOpts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, float(p),
                               float(drop_attn), float(self.dropout_aoa if drop_aoa is None else drop_aoa), float(drop_sublayer),
                               int(self.ctx_drop if ctx_drop is None else ctx_drop), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss),
-                              None if rw is None else ctypes.pointer(rw))
-        _lib.check(lib.capb200_aoa_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table._h, _lib.ptr(refs), _lib.ptr(offsets), L,
+                              sampler, None if rw is None else ctypes.pointer(rw))
+        _lib.check(lib.capb200_aoa_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs), _lib.ptr(offsets), L,
                                              ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq), _lib.ptr(logprobs),
                                              _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'aoa_scst_step')
         return {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,

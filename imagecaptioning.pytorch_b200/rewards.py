@@ -62,6 +62,10 @@ class CiderDTable:
         """Handle of the table on the calling thread's current CUDA device."""
         return self._handle(torch.cuda.current_device())
 
+    def handle_for(self, refs: torch.Tensor):
+        """The handle a reward call over the packed reference rows `refs` [n_refs, L] passes to the C ABI."""
+        return self._h
+
     @classmethod
     def from_pickle(cls, path: str, device=None):
         with open(path, 'rb') as f:
@@ -77,17 +81,51 @@ class CiderDTable:
             pass
 
 
+class CorpusCiderDTable(CiderDTable):
+    """CiderD(df='corpus') (ciderD_scorer.py:143-147, 182-186, 210-216): no pickle; every reward call rebuilds the document frequencies on
+    the device from its own references (capb200_cider_corpus_table_create).  df counts the scored hypotheses whose image has the n-gram
+    among its references, ref_len = log(number of hypotheses): an SCST call counts each image n + 1 times, get_scores n times."""
+
+    def __init__(self, device=None):
+        self.ref_len = None
+        self.entries = 0
+        self._handles = {}
+        self._lock = threading.Lock()
+        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        self._handle(self.device.index if self.device.index is not None else torch.cuda.current_device())
+
+    def _handle(self, index: int):
+        with self._lock:
+            h = self._handles.get(index)
+            if h is None:
+                lib = _lib.load()
+                with torch.cuda.device(index):
+                    h = lib.capb200_cider_corpus_table_create()
+                if not h:
+                    raise RuntimeError('capb200 cider_corpus_table_create failed: %s' % lib.capb200_last_error().decode())
+                self._handles[index] = h
+            return h
+
+    def handle_for(self, refs: torch.Tensor):
+        h = self._h
+        _lib.check(_lib.load().capb200_cider_table_reserve(h, int(refs.shape[0]), int(refs.shape[1])), 'cider_table_reserve')
+        return h
+
+
 CiderD_scorer: Optional[CiderDTable] = None
 
 
 def init_scorer(cached_tokens, device=None):
     """Same contract as the reference: ``cached_tokens`` names ``data/<cached_tokens>.p`` relative to the cwd
-    (ciderD_scorer.py:109); an existing path or an already built CiderDTable is accepted too.  Idempotent."""
+    (ciderD_scorer.py:109), and ``'corpus'`` takes the document frequencies from the references of each call (no file); an existing path
+    or an already built CiderDTable is accepted too.  Idempotent."""
     global CiderD_scorer
     if CiderD_scorer is not None:
         return CiderD_scorer
     if isinstance(cached_tokens, CiderDTable):
         CiderD_scorer = cached_tokens
+    elif cached_tokens == 'corpus':
+        CiderD_scorer = CorpusCiderDTable(device)
     else:
         path = cached_tokens if os.path.exists(str(cached_tokens)) else os.path.join('data', str(cached_tokens) + '.p')
         CiderD_scorer = CiderDTable.from_pickle(path, device)
@@ -179,7 +217,7 @@ def cider_scores_and_reward(greedy_res: torch.Tensor, data_gts: Sequence, gen_re
     scores = torch.empty(S + B, dtype=torch.float64, device=dev)
     reward = torch.empty(S, T, dtype=torch.float32, device=dev)
     lib = _lib.load()
-    _lib.check(lib.capb200_self_critical_reward(table._h, _lib.ptr(sampled), S, _lib.ptr(greedy), B, T, _lib.ptr(refs), _lib.ptr(offsets), L,
+    _lib.check(lib.capb200_self_critical_reward(table.handle_for(refs), _lib.ptr(sampled), S, _lib.ptr(greedy), B, T, _lib.ptr(refs), _lib.ptr(offsets), L,
                                                 _lib.ptr(scores), _lib.ptr(reward), _lib.current_stream()), 'self_critical_reward')
     return scores, reward
 
@@ -230,7 +268,7 @@ def weighted_scores(data_gts: Sequence, gen_result: torch.Tensor, weights, greed
     bleu = torch.empty(hyps, dtype=torch.float64, device=dev)
     reward = torch.empty(S, T, dtype=torch.float32, device=dev) if with_reward else None
     lib = _lib.load()
-    _lib.check(lib.capb200_weighted_reward(table._h if table is not None else None, ctypes.byref(w), _lib.ptr(sampled), S, _lib.ptr(greedy), B, T,
+    _lib.check(lib.capb200_weighted_reward(table.handle_for(refs) if table is not None else None, ctypes.byref(w), _lib.ptr(sampled), S, _lib.ptr(greedy), B, T,
                                            _lib.ptr(refs), _lib.ptr(offsets), L, _lib.ptr(scores), _lib.ptr(bleu), _lib.ptr(reward),
                                            _lib.current_stream()), 'weighted_reward')
     return (scores, reward) if with_reward else scores
@@ -284,7 +322,7 @@ def cider_scores(data_gts: Sequence, gen_result: torch.Tensor, table: Optional[C
     scores = torch.empty(S, dtype=torch.float64, device=dev)
     reward = torch.empty(S, T, dtype=torch.float32, device=dev) if with_reward else None
     lib = _lib.load()
-    _lib.check(lib.capb200_cider_scores(table._h, _lib.ptr(sampled), S, B, T, _lib.ptr(refs), _lib.ptr(offsets), L, _lib.ptr(scores),
+    _lib.check(lib.capb200_cider_scores(table.handle_for(refs), _lib.ptr(sampled), S, B, T, _lib.ptr(refs), _lib.ptr(offsets), L, _lib.ptr(scores),
                                         _lib.ptr(reward) if with_reward else None, _lib.current_stream()), 'cider_scores')
     return (scores, reward) if with_reward else scores
 

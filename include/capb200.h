@@ -333,6 +333,16 @@ long capb200_ensemble_launch_count(const capb200_ensemble* s);
  * df[n] float64, ref_len = number of reference images (ciderD_scorer.py:108-111).  Host pointers; synchronous. */
 capb200_cider_table* capb200_cider_table_create(const int* keys, const double* df, long n, double ref_len, void* stream);
 void capb200_cider_table_destroy(capb200_cider_table* t);
+/* Corpus document frequencies (init_scorer('corpus') -> CiderD(df='corpus'), ciderD_scorer.py:143-147,182-186,210-216): no pickle; every
+ * reward call that reads the table (the entry points below and every family's SCST / new_self_critical step) first rebuilds it on the device
+ * from its own references, in three kernels inside the same stream (and step graph).  df[ngram] counts the scored hypotheses (crefs entries)
+ * whose reference set holds the n-gram -- each image's distinct n-grams count once per hypothesis of the image: n + 1 with greedy captions,
+ * n without -- and ref_len = log(number of hypotheses).  Before a call, reserve room for its references: n_refs rows of L tokens (growing
+ * synchronises the device and moves the slots, which a captured step graph notices).  A call with more reference rows than reserved
+ * undercounts instead of overflowing the table. */
+capb200_cider_table* capb200_cider_corpus_table_create(void);
+int capb200_cider_table_reserve(capb200_cider_table* t, long n_refs, int L);
+int capb200_cider_table_is_corpus(const capb200_cider_table* t);
 
 /* get_self_critical_reward (captioning/utils/rewards.py:41-81) with CIDEr-D only:
  * sampled[S,T], greedy[B,T] int64 device; refs[n_refs_total,L] int32 device (0 padded), ref_offsets[B+1] int32 device;
@@ -383,6 +393,19 @@ int capb200_reward_criterion_backward(const long long* seq, const float* reward,
  * :637), self-critical reward (CIDEr-D, or weighted CIDEr-D + BLEU-4 with opts->reward_weights), RewardCriterion, then back-propagation
  * through time into every parameter gradient.
  * ---------------------------------------------------------------------------------------------------------------- */
+/* How a fused self-critical step draws its words: LossWrapper's train_sample_method (the train-mode samples, loss_wrapper.py:63-67) and
+ * sc_sample_method (the eval-mode baseline, :57-62), both at temperature 1 for the baseline and opts->temperature for the samples.  Methods
+ * are CAPB200_SAMPLE_GREEDY, _MULTINOMIAL, _TOPK (top = k >= 1) and _TOPP (0 < top < 1), drawn as capb200_decode_sample draws them; 'gumbel'
+ * is a multinomial draw at temperature 1.  The criterion and the gradient always use the full log-softmax row (AttModel.py:337,347).  The
+ * baseline draws from its own Philox key, derived from opts->seed, so a replayed step graph draws fresh baseline captions too.  A NULL
+ * pointer to this struct means {MULTINOMIAL, 0, GREEDY, 0, NULL}.  A sampled baseline needs CAPB200_BASELINE_GREEDY. */
+typedef struct {
+    int train_method;
+    float train_top;
+    int baseline_method;
+    float baseline_top;
+    const long long* forced_baseline;   /* optional [B, T] int64 device: replay these baseline captions instead of drawing them (parity checks) */
+} capb200_sampler_opts;
 typedef struct {
     int sample_n;              /* opt.train_sample_n */
     float temperature;
@@ -398,6 +421,8 @@ typedef struct {
     int keep_rows;             /* drop_worst (tools/train.py:187-191): 0 = reduction 'mean'; k > 0 = the criterion runs with reduction 'none' (one loss per
                                   caption row) and the k rows with the smallest loss are averaged: loss[0] = that mean, gradients accordingly */
     float* row_loss;           /* optional [rows] output of the per-row losses (what LossWrapper returns as out['loss'] under drop_worst_flag) */
+    const capb200_sampler_opts* sampler; /* optional, read during the call: the train and baseline samplers; NULL = multinomial samples and the
+                                  greedy baseline.  The autograd entry points (*_scst_vjp) refuse it */
     const capb200_reward_weights* reward_weights; /* optional, read during the call: the reward is cider * CIDEr-D + bleu * BLEU-4 as
                                   capb200_weighted_reward computes it; NULL = CIDEr-D only (weight 1) */
 } capb200_scst_opts;
@@ -511,6 +536,7 @@ typedef struct {
     int keep_rows;             /* drop_worst (tools/train.py:187-191): 0 = reduction 'mean'; k > 0 = the criterion runs with reduction 'none' (one loss per
                                   caption row) and the k rows with the smallest loss are averaged: loss[0] = that mean, gradients accordingly */
     float* row_loss;           /* optional [rows] output of the per-row losses (what LossWrapper returns as out['loss'] under drop_worst_flag) */
+    const capb200_sampler_opts* sampler;          /* optional samplers, see capb200_scst_opts; NULL = multinomial + greedy baseline */
     const capb200_reward_weights* reward_weights; /* optional reward weights, see capb200_scst_opts; NULL = CIDEr-D only */
 } capb200_aoa_scst_opts;
 /* Gradient buffers, laid out field by field like the weights struct above: parameter shapes, fp32, device; every one is OVERWRITTEN. */
@@ -624,6 +650,7 @@ typedef struct {
     const float* att_masks;
     int keep_rows;
     float* row_loss;
+    const capb200_sampler_opts* sampler;            /* optional samplers, see capb200_scst_opts; NULL = multinomial + greedy baseline */
     const capb200_reward_weights* reward_weights;   /* optional reward weights, see capb200_scst_opts; NULL = CIDEr-D only */
 } capb200_tfm_scst_opts;
 int capb200_tfm_xe_step(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_xe_opts* opts, const long long* labels, const float* masks,
