@@ -75,9 +75,8 @@ __global__ void iota_div_kernel(int* p, int n, int div) {
 }
 
 
-enum GemmId { G_FC = 0, G_ATT, G_CTX, G_GFC, G_LSTM1, G_H2ATT, G_LSTM2, G_LOGIT, G_CORE, G_LSTM2A, G_LSTM2B, G_A2C, G_COUNT };
-constexpr int G_REPORTED = 9;      // ids exposed through capb200_engine_read_profile (the split language-LSTM launches are folded into G_LSTM2,
-                                   // Att2in2's a2c launch into G_CORE)
+enum GemmId { G_FC = 0, G_ATT, G_CTX, G_GFC, G_LSTM1, G_H2ATT, G_LSTM2, G_LOGIT, G_CORE, G_A2C, G_COUNT };
+constexpr int G_REPORTED = 9;      // ids exposed through capb200_engine_read_profile (Att2in2's a2c launch is folded into G_CORE)
 
 }  // namespace
 }  // namespace capb200
@@ -125,11 +124,7 @@ struct capb200_engine {
     Tf32Context* tf32 = nullptr;       // tensor maps + transposed operands of the training GEMMs (tensor-core modes)
     StepGraph sg;                                      // CUDA graph of the whole SCST step
     cudaEvent_t grad_events[2] = {nullptr, nullptr};   // caller-owned: recorded when a gradient group is complete (capb200_engine_set_grad_events)
-    // Optional overlap of the additive attention (SFU / FMA pipes) with the tensor-core work of the language LSTM that does not depend on it:
-    // gates = W_h h_att + W_hh h_lang_prev (side stream, while the attention runs) and then + W_a att_res with the fused cell (main stream).
-    bool split_lang = false;
     cudaStream_t side = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     cudaEvent_t ev_gfork = nullptr, ev_gjoin = nullptr;     // fork / join of the SCST step's concurrent greedy baseline
 
     // optional per-GEMM device timing (cudaEvent pairs on the launching stream), off by default
@@ -396,34 +391,10 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
             g.epi.C = e->att_h.v.f; g.epi.ldc = e->att_h.v.ld;
             if (run_gemm(e, G_H2ATT, g, e->capRows, st)) return 1;
         }
-        const bool split = e->split_lang && e->tc && e->side != nullptr;
-        if (split) {   // fork: the part of the language-LSTM gates that does not need the attention result, on the side stream
-            CAPB_CHECK_CUDA(cudaEventRecord(e->ev_fork, st));
-            CAPB_CHECK_CUDA(cudaStreamWaitEvent(e->side, e->ev_fork, 0));
-            GemmProblem g;
-            g.M = rows; g.N = 4 * H; g.nseg = 2;
-            g.seg[0] = seg_of(e->h0_out.v, w.lang_lstm_w_ih + H, 2 * H, e->p_l_ih_h, H);
-            g.seg[1] = seg_of(e->h1_in.v, w.lang_lstm_w_hh, H, e->p_l_hh, H);
-            g.epi.bias = e->bsum_lang_il;
-            g.epi.C = e->gates.v.f; g.epi.ldc = e->gates.v.ld;          // gate-interleaved partial sums [rows, 4H]
-            if (run_gemm(e, G_LSTM2A, g, e->capRows, e->side)) return 1;
-            CAPB_CHECK_CUDA(cudaEventRecord(e->ev_join, e->side));
-        }
         e->launches += 2;
         if (additive_attention_launch(n_images, rpi, R, A, H, e->att_h.v.f, e->att_h.v.ld, e->p_att.v.f, e->p_att.v.ld, e->att_e.v.f, e->att_e.v.ld,
                                       mask, R, w.alpha_w, w.alpha_b, e->att_score, e->att_res.v, st)) return 1;
-        if (split) {   // join: add the attention term and apply the cell
-            CAPB_CHECK_CUDA(cudaStreamWaitEvent(st, e->ev_join, 0));
-            GemmProblem g;
-            g.M = rows; g.N = 4 * H; g.nseg = 1;
-            g.seg[0] = seg_of(e->att_res.v, w.lang_lstm_w_ih, 2 * H, e->p_l_ih_a, H);
-            g.epi.residual = e->gates.v.f; g.epi.ld_res = e->gates.v.ld;
-            g.epi.lstm = 1; g.epi.H = H;
-            g.epi.c_prev = e->c1[cur]; g.epi.ld_cprev = e->ld_c; g.epi.src_row = src_row;
-            g.epi.c_out = e->c1[nxt]; g.epi.ld_cout = e->ld_c;
-            g.epi.h_f = e->h1_out.v.f; g.epi.h_hi = e->h1_out.v.hi; g.epi.h_lo = e->h1_out.v.lo; g.epi.ld_h = e->h1_out.v.ld;
-            if (run_gemm(e, G_LSTM2B, g, e->capRows, st)) return 1;
-        } else {   // language LSTM gates: [att_res | h_att | h_lang_prev]
+        {   // language LSTM gates: [att_res | h_att | h_lang_prev]
             GemmProblem g;
             g.M = rows; g.N = 4 * H; g.nseg = 3;
             g.seg[0] = seg_of(e->att_res.v, w.lang_lstm_w_ih, 2 * H, e->p_l_ih_a, H);
@@ -610,12 +581,6 @@ capb200_engine* capb200_engine_create(const capb200_model_cfg* cfg) {
     e->T = cfg->seq_length;
     e->mode = cfg->numeric_mode;
     e->tc = cfg->numeric_mode != CAPB200_MODE_SIMT_FP32;
-    if (e->tc && getenv("CAPB200_SPLIT_LANG") != nullptr && atoi(getenv("CAPB200_SPLIT_LANG")) != 0) {
-        if (create_side_stream(&e->side) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) == cudaSuccess &&
-            cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) == cudaSuccess) e->split_lang = true;
-        else (void)cudaGetLastError();
-    }
     return e;
 }
 
@@ -629,8 +594,6 @@ void capb200_engine_destroy(capb200_engine* e) {
     cudaFree(e->tape);
     e->sg.destroy();
     tf32_context_destroy(e->tf32);
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
     if (e->ev_gfork) cudaEventDestroy(e->ev_gfork);
     if (e->ev_gjoin) cudaEventDestroy(e->ev_gjoin);
     if (e->side) cudaStreamDestroy(e->side);
@@ -658,11 +621,9 @@ int capb200_engine_read_profile(capb200_engine* e, int reset, double* ms, double
     e->ev_ids.clear();
     e->ev_flops.clear();
     e->ev_used = 0;
-    for (int i = G_LSTM2A; i <= G_A2C; ++i) {       // the split language-LSTM launches report under the language-LSTM id, a2c under the core id
-        const int to = i == G_A2C ? G_CORE : G_LSTM2;
-        e->prof_ms[to] += e->prof_ms[i]; e->prof_flops[to] += e->prof_flops[i]; e->prof_calls[to] += e->prof_calls[i];
-        e->prof_ms[i] = 0; e->prof_flops[i] = 0; e->prof_calls[i] = 0;
-    }
+    // Att2in2's a2c launch reports under the core id
+    e->prof_ms[G_CORE] += e->prof_ms[G_A2C]; e->prof_flops[G_CORE] += e->prof_flops[G_A2C]; e->prof_calls[G_CORE] += e->prof_calls[G_A2C];
+    e->prof_ms[G_A2C] = 0; e->prof_flops[G_A2C] = 0; e->prof_calls[G_A2C] = 0;
     for (int i = 0; i < G_REPORTED; ++i) {
         if (ms) ms[i] = e->prof_ms[i];
         if (flops) flops[i] = e->prof_flops[i];

@@ -507,10 +507,6 @@ int aoa_decode_prepare(capb200_aoa_engine* e, const float* att, const float* mas
 int aoa_decode_core(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int R,
                     const float* mask, cudaStream_t st);
 
-// Training-step GEMMs on the raw fp32 PyTorch weights (always current, no repack after optimizer steps).  With a Tf32Context (tensor-core
-// engines) every call runs on the wgmma tf32 3-pass kernel of gemm_tf32.cu; operands that are not K-major in HBM (W for the input
-// gradients, dY / X for the weight gradients) go through cached transposes.  Without a context (simt_fp32 engines), when an operand is not
-// TMA-compatible (rows not 16-byte aligned: tiny test shapes), or with CAPB200_SKINNY_LEGACY set, the split-K kernels of gemm_generic.cu run.
 // CUDA graph of a whole fused training step (see run_scst_step in train_common.cuh) + the engine-owned staging buffer that gives the graph stable input
 // addresses.  CAPB200_SCST_GRAPH=0 keeps the steps eager.
 struct StepGraph {
@@ -620,20 +616,22 @@ inline int record_group_event(cudaEvent_t ev, cudaStream_t st) {
 }
 
 // Side stream of the SCST steps (the eval-mode greedy baseline runs on it while the train-mode sampling pass runs on the caller's stream).
-// Lowest priority by default: both chains are latency-bound and compete for SMs (a persistent GEMM CTA owns its SM's shared memory), and
-// the sampling pass is the critical path -- its pending CTAs should be placed first.  CAPB200_SIDE_PRIORITY=0 gives both equal priority.
+// Lowest priority: both chains are latency-bound and compete for SMs (a persistent GEMM CTA owns its SM's shared memory), and the
+// sampling pass is the critical path -- its pending CTAs should be placed first.
 inline cudaError_t create_side_stream(cudaStream_t* s) {
-    static const bool equal = getenv("CAPB200_SIDE_PRIORITY") != nullptr && atoi(getenv("CAPB200_SIDE_PRIORITY")) == 0;
     int least = 0, greatest = 0;
-    if (!equal && cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess) return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, least);
+    if (cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess) return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, least);
     return cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
 }
 
+// Training-step GEMMs on the raw fp32 PyTorch weights (always current, no repack after optimizer steps).  With a Tf32Context (tensor-core
+// engines) every call runs on the wgmma tf32 3-pass kernel of gemm_tf32.cu; operands that are not K-major in HBM (W for the input
+// gradients, dY / X for the weight gradients) go through cached transposes.  Without a context (simt_fp32 engines), or when an operand is
+// not TMA-compatible (rows not 16-byte aligned: tiny test shapes), the split-K kernels of gemm_generic.cu run.
 struct Skinny {
     float* scratch; size_t cap; int mode; cudaStream_t st;
     Tf32Context* ctx = nullptr;
-    static bool legacy() { static const bool v = getenv("CAPB200_SKINNY_LEGACY") != nullptr; return v; }
-    bool tc() const { return ctx != nullptr && mode != 0 && !legacy(); }
+    bool tc() const { return ctx != nullptr && mode != 0; }
     // y = x * W^T (+ b)          (nn.Linear forward; W stored [N, K])
     int lin(const float* x, long ldx, const float* w, long ldw, const float* b, float* y, long ldy, int M, int N, int K, int accumulate) const {
         if (tc() && gemm_tf32_supported(1, &x, &ldx, &w, &ldw, &K))

@@ -4,7 +4,6 @@
 //   TB = 0: B stored [K, N] (pitch ldb)      TB = 1: B stored [N, K]   (nn.Linear forward: x * W^T)
 // The training shapes are skinny (M = B * sample_n = 50..60 rows, or K = T * rows ~ 1000 for the weight gradients), i.e. weight-
 // streaming bound; 64x64x16 tiles with 4x4 register blocks keep enough CTAs in flight for those shapes.
-#include <cstdlib>
 #include <cstring>
 
 #include "common.cuh"
@@ -218,7 +217,7 @@ __global__ void __launch_bounds__(256) gemm_skinny_kernel(const SkinnyParams p) 
 
 // Same problem on the tensor cores: 3xTF32 (hi*lo + lo*hi + hi*hi, fp32 accumulate) through mma.sync.m16n8k8, reading the fp32 weights
 // as they are (no repack after optimizer steps; TF32 keeps the fp32 exponent, so small gradients do not underflow the way fp16 planes
-// would).  The shapes are weight-streaming bound, so the legacy mma path is enough; tile 64 x 64 x 16, 8 warps as 2 (M) x 4 (N).
+// would).  The shapes are weight-streaming bound, so the legacy mma path is enough; tile 64 x 64 x 32, 8 warps as 2 (M) x 4 (N).
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
     const float r = x - __uint_as_float(hi);
@@ -230,116 +229,9 @@ __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], 
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-constexpr int SA_LD = GK + 4;      // A / B^T tiles [64][16] padded: fragment loads hit 32 distinct banks
-constexpr int SB_LD = GT + 8;      // B tile [16][64] padded (TB = 0)
-
-template <int TB>
-__global__ void __launch_bounds__(256) gemm_skinny_tf32_kernel(const SkinnyParams p) {
-    __shared__ uint32_t As[2][GT * SA_LD];                              // [hi/lo][m][k]
-    __shared__ uint32_t Bs[2][TB ? GT * SA_LD : GK * SB_LD];            // TB: [n][k]   else [k][n]
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, tig = lane & 3;
-    const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
-    const int n0 = blockIdx.x * GT, m0 = blockIdx.z * GT;
-    const int per = (p.ksteps_total + p.ksplit - 1) / p.ksplit;
-    const int ks0 = blockIdx.y * per, ks1 = min(p.ksteps_total, ks0 + per);
-    float acc[2][2][4];
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.f;
-    // global -> register staging: one float4 of A and one of B per thread
-    const int a_row = tid >> 2, a_k = (tid & 3) * 4;
-    const int b_r = TB ? (tid >> 2) : (tid >> 4), b_c = TB ? (tid & 3) * 4 : (tid & 15) * 4;          // TB: (n, k)   else (k, n)
-    float4 ra, rb;
-    int seg = 0, seg_first = 0;
-    auto fetch = [&](int ks) {
-        while (seg < p.nseg - 1 && ks >= seg_first + (p.K[seg] + GK - 1) / GK) { seg_first += (p.K[seg] + GK - 1) / GK; ++seg; }
-        const int k0 = (ks - seg_first) * GK, K = p.K[seg];
-        ra = make_float4(0.f, 0.f, 0.f, 0.f);
-        rb = ra;
-        if (m0 + a_row < p.M && k0 + a_k < K) ra = *reinterpret_cast<const float4*>(p.A[seg] + (long)(m0 + a_row) * p.lda[seg] + k0 + a_k);
-        if (TB) {
-            if (n0 + b_r < p.N && k0 + b_c < K) rb = *reinterpret_cast<const float4*>(p.B[seg] + (long)(n0 + b_r) * p.ldb[seg] + k0 + b_c);
-        } else {
-            if (k0 + b_r < K && n0 + b_c < p.N) rb = *reinterpret_cast<const float4*>(p.B[seg] + (long)(k0 + b_r) * p.ldb[seg] + n0 + b_c);
-        }
-    };
-    if (ks0 < ks1) fetch(ks0);
-    for (int ks = ks0; ks < ks1; ++ks) {
-        {
-            const float av[4] = {ra.x, ra.y, ra.z, ra.w}, bv[4] = {rb.x, rb.y, rb.z, rb.w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                uint32_t hi, lo;
-                split_tf32(av[q], hi, lo);
-                As[0][a_row * SA_LD + a_k + q] = hi; As[1][a_row * SA_LD + a_k + q] = lo;
-                split_tf32(bv[q], hi, lo);
-                const int o = TB ? b_r * SA_LD + b_c + q : b_r * SB_LD + b_c + q;
-                Bs[0][o] = hi; Bs[1][o] = lo;
-            }
-        }
-        __syncthreads();
-        if (ks + 1 < ks1) fetch(ks + 1);
-#pragma unroll
-        for (int kk = 0; kk < GK; kk += 8) {
-            uint32_t ah[2][4], al[2][4], bh[2][2], bl[2][2];
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int r = wm + i * 16 + g;
-                ah[i][0] = As[0][r * SA_LD + kk + tig];       ah[i][1] = As[0][(r + 8) * SA_LD + kk + tig];
-                ah[i][2] = As[0][r * SA_LD + kk + tig + 4];   ah[i][3] = As[0][(r + 8) * SA_LD + kk + tig + 4];
-                al[i][0] = As[1][r * SA_LD + kk + tig];       al[i][1] = As[1][(r + 8) * SA_LD + kk + tig];
-                al[i][2] = As[1][r * SA_LD + kk + tig + 4];   al[i][3] = As[1][(r + 8) * SA_LD + kk + tig + 4];
-            }
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                const int c = wn + j * 8 + g;
-                if (TB) {
-                    bh[j][0] = Bs[0][c * SA_LD + kk + tig]; bh[j][1] = Bs[0][c * SA_LD + kk + tig + 4];
-                    bl[j][0] = Bs[1][c * SA_LD + kk + tig]; bl[j][1] = Bs[1][c * SA_LD + kk + tig + 4];
-                } else {
-                    bh[j][0] = Bs[0][(kk + tig) * SB_LD + c]; bh[j][1] = Bs[0][(kk + tig + 4) * SB_LD + c];
-                    bl[j][0] = Bs[1][(kk + tig) * SB_LD + c]; bl[j][1] = Bs[1][(kk + tig + 4) * SB_LD + c];
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    mma_tf32(acc[i][j], ah[i], bl[j]);
-                    mma_tf32(acc[i][j], al[i], bh[j]);
-                    mma_tf32(acc[i][j], ah[i], bh[j]);
-                }
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const int row = m0 + wm + i * 16 + g + (q >> 1) * 8;
-                const int col = n0 + wn + j * 8 + 2 * tig + (q & 1);
-                if (row >= p.M || col >= p.N) continue;
-                float v = acc[i][j][q];
-                if (p.ksplit == 1) {
-                    if (p.bias) v += p.bias[col];
-                    if (p.row_bias) v += p.row_bias[(long)(row / p.rpg) * p.ld_rb + col];
-                    float* c = p.out + (long)row * p.ldo + col;
-                    *c = p.accumulate ? (*c + v) : v;
-                } else {
-                    p.out[((long)blockIdx.y * p.M + row) * p.N + col] = v;
-                }
-            }
-}
-
-// Second generation of the 3xTF32 skinny kernel: the first one kept only one 16-deep K-slice per thread in flight (two float4 loads),
-// which caps a weight-streaming GEMM at ~1 TB/s.  Here raw fp32 tiles are staged with cp.async through a 4-stage ring of 32-deep
-// K-slices (18 KB per stage, 3 CTAs per SM => ~160 KB of loads in flight per SM); the TF32 hi/lo split happens on the fragments.
+// One 16-deep K-slice per thread in flight (two float4 loads) would cap a weight-streaming GEMM at ~1 TB/s, so raw fp32 tiles are
+// staged with cp.async through a 4-stage ring of 32-deep K-slices (18 KB per stage, 3 CTAs per SM => ~160 KB of loads in flight per SM);
+// the TF32 hi/lo split happens on the fragments.
 constexpr int S2_BK = 32, S2_STAGES = 4;
 constexpr int S2_ALD = S2_BK + 4;        // A / B^T rows: 36 floats (16-byte multiples, conflict-free fragment loads)
 constexpr int S2_BLD = GT + 8;           // B rows [k][n]: 72 floats
@@ -499,15 +391,13 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
     SkinnyParams p;
     memset(&p, 0, sizeof(p));
     p.nseg = nseg; p.M = M; p.N = N;
-    // tensor-core variants need 16-byte aligned float4 rows and one storage order for all segments
+    // the tensor-core kernel needs 16-byte aligned float4 rows and one storage order for all segments
     bool tc = (mode != 0);
     for (int s = 0; s < nseg; ++s) {
         tc = tc && tb[s] == tb[0] && K[s] % 4 == 0 && lda[s] % 4 == 0 && ldb[s] % 4 == 0 && (reinterpret_cast<uintptr_t>(A[s]) & 15) == 0 &&
              (reinterpret_cast<uintptr_t>(B[s]) & 15) == 0 && (tb[s] || N % 4 == 0);
     }
-    static const bool v1_only = getenv("CAPB200_SKINNY_V1") != nullptr;
-    const bool v2 = tc && !v1_only;
-    const int bk = v2 ? S2_BK : GK;
+    const int bk = tc ? S2_BK : GK;
     int ksteps = 0;
     for (int s = 0; s < nseg; ++s) {
         p.A[s] = A[s]; p.B[s] = B[s]; p.lda[s] = lda[s]; p.ldb[s] = ldb[s]; p.K[s] = K[s]; p.tb[s] = tb[s];
@@ -515,7 +405,7 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
     }
     p.ksteps_total = ksteps;
     const int tiles = cdiv(N, GT) * cdiv(M, GT);
-    int ksplit = ((v2 ? 3 : 2) * sm_count() + tiles - 1) / tiles;          // CTAs resident per SM: 3 (v2, 74 KB of shared memory each) or 2
+    int ksplit = ((tc ? 3 : 2) * sm_count() + tiles - 1) / tiles;          // CTAs resident per SM: 3 (tensor cores, 74 KB of shared memory each) or 2
     if (ksplit > ksteps / 4) ksplit = ksteps / 4;                  // at least 4 K-steps per CTA
     if (ksplit < 1) ksplit = 1;
     while (ksplit > 1 && (size_t)ksplit * M * N > scratch_floats) --ksplit;
@@ -523,7 +413,7 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
     p.bias = bias; p.row_bias = row_bias; p.ld_rb = ld_rb; p.rpg = rpg < 1 ? 1 : rpg; p.accumulate = accumulate;
     if (ksplit == 1) { p.out = C; p.ldo = ldc; } else { p.out = scratch; p.ldo = N; }
     dim3 grid(cdiv(N, GT), ksplit, cdiv(M, GT));
-    if (v2) {
+    if (tc) {
         constexpr int smem = S2_STAGES * S2_STAGE_FLOATS * (int)sizeof(float);
         static std::atomic<unsigned long long> configured{0};
         if (first_use_on_device(configured)) {
@@ -532,9 +422,9 @@ int gemm_skinny_launch(int M, int N, int nseg, const float* const* A, const long
         }
         if (tb[0]) gemm_skinny_tf32_v2_kernel<1, 0><<<grid, 256, smem, st>>>(p);
         else gemm_skinny_tf32_v2_kernel<0, 0><<<grid, 256, smem, st>>>(p);
-    } else if (tc && tb[0]) gemm_skinny_tf32_kernel<1><<<grid, 256, 0, st>>>(p);
-    else if (tc) gemm_skinny_tf32_kernel<0><<<grid, 256, 0, st>>>(p);
-    else gemm_skinny_kernel<<<grid, 256, 0, st>>>(p);
+    } else {
+        gemm_skinny_kernel<<<grid, 256, 0, st>>>(p);
+    }
     CAPB_CHECK_CUDA(cudaGetLastError());
     if (ksplit > 1) {
         long blocks = ((long)M * N + 255) / 256;
@@ -552,8 +442,7 @@ int gemm_wgrad_launch(int M, int N, int K, const float* dY, long ld_dy, const fl
     if (M <= 0 || N <= 0) return 0;
     const bool ok = mode != 0 && K > 0 && M % 4 == 0 && N % 4 == 0 && ld_dy % 4 == 0 && ld_x % 4 == 0 && (reinterpret_cast<uintptr_t>(dY) & 15) == 0 &&
                     (reinterpret_cast<uintptr_t>(X) & 15) == 0;
-    static const bool v1_only = getenv("CAPB200_SKINNY_V1") != nullptr;
-    if (!ok || v1_only) return gemm_generic_launch(1, 0, M, N, K, dY, ld_dy, X, ld_x, G, ld_g, accumulate, nullptr, st);
+    if (!ok) return gemm_generic_launch(1, 0, M, N, K, dY, ld_dy, X, ld_x, G, ld_g, accumulate, nullptr, st);
     SkinnyParams p;
     memset(&p, 0, sizeof(p));
     p.nseg = 1; p.M = M; p.N = N;

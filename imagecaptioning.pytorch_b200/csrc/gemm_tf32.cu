@@ -23,7 +23,6 @@
 // Operand roles: the A side always supplies 128 accumulator rows, the B side BN columns.  Skinny problems (M <= 256 activation rows:
 // the 50-row sampling steps) run SWAPPED -- weights on the A side, activations on the B side -- so no tensor-core row is padding and
 // the weights are streamed exactly once; problems with many rows (refiner: B*R rows; batched-over-time gradients: T*N rows) run normally.
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <unordered_map>
@@ -477,18 +476,16 @@ int gemm_tf32_launch(Tf32Context* ctx, int M, int N, int nseg, const float* cons
     p.ksteps_total = ksteps;
     const int tiles_a = (int)cdiv((int)a_rows, TM), tiles_b = (int)cdiv((int)b_rows, bn);
     // split-K so that ~all SMs stream disjoint K-slices.
-    //  * default: across a thread-block cluster with the DSMEM reduction (largest power of two <= 8 with tiles * ksplit <= SMs), except
-    //    for the shape class named below.
-    //  * CAPB200_TF32_SCRATCH=1 (0 = never): finer splits (up to 24 K-ranks, >= 2 K-blocks each) with the partial tiles in a global scratch buffer and a
-    //    last-arriver reduction in rank order.  It helps where the cluster form tops out on a large K and few tiles, and loses where the last
-    //    CTA re-reads many partial tiles, so the cluster form stays the default.
-    static const int scratch_mode = getenv("CAPB200_TF32_SCRATCH") != nullptr ? atoi(getenv("CAPB200_TF32_SCRATCH")) : -1;     // 1 always, 0 never, unset: hybrid
+    //  * across a thread-block cluster with the DSMEM reduction (largest power of two <= 8 with tiles * ksplit <= SMs), except for the
+    //    shape class named below.
+    //  * 16 or more clusters of 8 (att2ctx and its input gradient, 2048 x 2048): finer splits (up to 24 K-ranks, >= 2 K-blocks each) with
+    //    the partial tiles in a global scratch buffer and a last-arriver reduction in rank order.  The scratch form wins where the cluster
+    //    form tops out on a large K, and loses elsewhere, where the last CTA re-reads many partial tiles.
     const long tiles = (long)tiles_a * tiles_b;
     const int sms = sm_count();
     int ksplit = 1;
     while (ksplit < 8 && tiles * (ksplit * 2) <= sms && ksteps / (ksplit * 2) >= 2) ksplit *= 2;
-    // hybrid default: the shape class where the cluster form loses is 16 or more clusters of 8 (att2ctx and its input gradient, 2048 x 2048)
-    bool use_scratch = scratch_mode == 1 || (scratch_mode != 0 && ksplit == 8 && tiles >= 16);
+    const bool use_scratch = ksplit == 8 && tiles >= 16;
     if (use_scratch) {
         ksplit = (int)(sms / tiles);
         if (ksplit > ksteps / 2) ksplit = ksteps / 2;

@@ -189,7 +189,7 @@ inline Skinny step_gemms(Tf32Context** ctx, bool tc, const StepTape& tp, cudaStr
 // The eval-mode baseline of an SCST step: the regular decode on B rows, without dropout -- greedy, or drawn as sc_sample_method says from the
 // step's seed XOR kBaselineSalt (an XOR, so that the salt of a graph replay carries over: dropout.cuh), or the replay of given captions.  It and the train-mode sampling
 // forward are independent chains of small, latency-bound kernels, so the baseline runs on the engine's side stream -- forked from the step's
-// stream, joined before the reward -- unless CAPB200_SCST_SERIAL_GREEDY is set or the side stream cannot be created.  Three calls: fork at
+// stream, joined before the reward -- unless the side stream or its events cannot be created.  Three calls: fork at
 // the top of the step, enqueue where the family wants its launches issued, join (inside loss_backward).
 struct StepBaseline {
     static constexpr unsigned long long kBaselineSalt = 0x5bd1e9955bd1e995ull;
@@ -209,8 +209,7 @@ struct StepBaseline {
         seed = method == CAPB200_SAMPLE_GREEDY || method == CAPB200_SAMPLE_FORCED ? 0ull : ta.seed ^ kBaselineSalt;
         st = step_st;
         done = nullptr;
-        static const bool serial = getenv("CAPB200_SCST_SERIAL_GREEDY") != nullptr;
-        if (!needed || serial) return 0;
+        if (!needed) return 0;
         bool ok = *side != nullptr || create_side_stream(side) == cudaSuccess;
         if (ok && *ev_fork == nullptr) ok = cudaEventCreateWithFlags(ev_fork, cudaEventDisableTiming) == cudaSuccess;
         if (ok && *ev_join == nullptr) ok = cudaEventCreateWithFlags(ev_join, cudaEventDisableTiming) == cudaSuccess;
@@ -358,21 +357,18 @@ int run_vjp_step(Engine* e, cudaStream_t st, Step step) {
 // region mask ta.mask are copied into the engine-owned staging buffer first, so that the graph reads stable addresses (an input of zero
 // bytes is not staged and reaches the step as null); the key covers every option but the seed (the samplers and the reward weights by value), the gradient and
 // weight tables, every pointer the step touches and the shapes.  The gradient-group events a data-parallel caller listens to become external event-record nodes of the
-// graph (record_group_event) and are part of the key; CAPB200_SCST_GRAPH_SYNC=0 keeps the step eager while any is set.  The step also stays
-// eager with CAPB200_SCST_GRAPH=0, in the simt_fp32 mode, when forced samples or baseline captions are replayed, and once a capture has failed.
+// graph (record_group_event) and are part of the key.  The step stays eager with CAPB200_SCST_GRAPH=0, in the simt_fp32 mode, when forced
+// samples or baseline captions are replayed, and once a capture has failed.
 template <class Engine, class Opts, class Grads, class Args, class Step>
 int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& ta, const float* fc, size_t fc_bytes, const float* att, size_t att_bytes,
                   int B, int R, cudaStream_t st, Step step) {
-    static const bool graph_with_listener = !(getenv("CAPB200_SCST_GRAPH_SYNC") != nullptr && atoi(getenv("CAPB200_SCST_GRAPH_SYNC")) == 0);
-    bool listening = false;
-    for (cudaEvent_t ev : e->grad_events) listening = listening || ev != nullptr;
     // the weighted reward's kernels are counted here, so that the families' hand-kept counts stay those of the CIDEr-D reward
     auto counted = [&](const float* f, const float* a, const Args& t, cudaStream_t s) {
         const int rc = step(f, a, t, s);
         e->launches += t.reward_extra_launches();
         return rc;
     };
-    if (!StepGraph::enabled() || !e->tc || (listening && !graph_with_listener) || ta.forced != nullptr || ta.forced_baseline != nullptr || e->sg.broken)
+    if (!StepGraph::enabled() || !e->tc || ta.forced != nullptr || ta.forced_baseline != nullptr || e->sg.broken)
         return run_eager_step(st, [&] { return counted(fc, att, ta, st); });
     cudaStream_t gst = e->sg.enter(st);             // a capturable engine-owned stream, ordered after the caller's stream
     const void* srcs[3] = {fc, att, ta.mask};

@@ -6,11 +6,8 @@
 //                             torch.max / Categorical(logits).sample()     CaptionModel.py:372,405
 //                             finished-row masking                         AttModel.py:340-347
 // One CTA per row; the row lives in shared memory between the passes so HBM sees one read and one write.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.cuh"
-#include "ptx.cuh"
 
 namespace capb200 {
 
@@ -345,7 +342,7 @@ __global__ void __launch_bounds__(VT) vocab_stats_kernel(const VocabStepArgs a) 
     }
 }
 
-// Per-thread online softmax in base 2 (the single-pass kernels below).  A thread's partial sum holds sum 2^(x*log2e - mL), where
+// Per-thread online softmax in base 2 (the single-pass kernel below).  A thread's partial sum holds sum 2^(x*log2e - mL), where
 // mL = fl(m*log2e) belongs to its running maximum m.  mL carries the rounding of that product -- up to half an ulp of |m|*log2e, 1e-4 at
 // |m| = 1000 -- so the rescale to a new maximum and the final rescale to the row maximum are both taken against mL itself, not against m:
 // the rounding then cancels and the log-sum-exp does not degrade with the magnitude of the logits (log_softmax is shift-invariant).
@@ -364,78 +361,9 @@ __device__ __forceinline__ float online_finish(float part, float m, float mL, fl
     return (m == -INFINITY) ? 0.f : part * sc;
 }
 
-// Single-pass variant of vocab_stats_kernel (one CTA per row, loads straight from global memory, 8 CTAs per SM): per-thread online
-// softmax (running max, partial sum rescaled when the max grows) and one max-of-four test in front of the top-2 bookkeeping, so the
-// row is read once and the common path is ~5 instructions per element.
-__global__ void __launch_bounds__(VT) vocab_stats_online_kernel(const VocabStepArgs a) {
-    __shared__ float s_red[VT / 32];
-    __shared__ int s_idx[VT / 32];
-    const int r = blockIdx.x;
-    const int n4 = a.V1 >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(a.logits + (long)r * a.ld);
-    constexpr float kL2E = 1.4426950408889634f;
-    float t0v = -INFINITY, t1v = -INFINITY;
-    int t0i = 0x7fffffff, t1i = 0x7fffffff;
-    float m = -INFINITY, mL = -INFINITY, part = 0.f;
-    for (int v = threadIdx.x; v < n4; v += VT) {
-        const float4 x = g4[v];
-        const float m4 = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
-        if (m4 > m) {
-            online_raise(part, m, mL, m4);
-        }
-        float e0, e1, e2, e3;
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(x.x, kL2E, -mL)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(x.y, kL2E, -mL)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(fmaf(x.z, kL2E, -mL)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e3) : "f"(fmaf(x.w, kL2E, -mL)));
-        part += (e0 + e1) + (e2 + e3);
-        if (m4 > t1v) {                             // strict: earlier (lower) indices win ties
-            const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                if (xs[u] > t1v) {
-                    if (xs[u] > t0v) { t1v = t0v; t1i = t0i; t0v = xs[u]; t0i = 4 * v + u; }
-                    else { t1v = xs[u]; t1i = 4 * v + u; }
-                }
-            }
-        }
-    }
-    const float mx = block_max(m, s_red);
-    float sum = online_finish(part, m, mL, mx);
-    sum = block_sum(sum, s_red);
-    const float lsum = logf(sum);
-    const float m2 = (mx - mx) - lsum, l2 = lsum;
-    if (threadIdx.x == 0) a.stats[r] = make_float2(mx, lsum);
-    int popped = 0;
-    for (int k = 0; k < a.topk; ++k) {
-        float ov;
-        int oi;
-        block_argmax(t0v, t0i, s_red, s_idx, ov, oi);
-        if (t0i == oi && oi != 0x7fffffff) {
-            const float lastv = t0v;
-            const int lasti = t0i;
-            t0v = t1v; t0i = t1i;
-            t1v = -INFINITY; t1i = 0x7fffffff;
-            if (++popped >= 2 && t0i == 0x7fffffff) {
-                auto consider = [&](float x, int v) {
-                    const bool after = (x < lastv) || (x == lastv && v > lasti);
-                    if (after && (x > t0v || (x == t0v && v < t0i))) { t0v = x; t0i = v; }
-                };
-                for (int v = threadIdx.x; v < n4; v += VT) {
-                    const float4 x = g4[v];
-                    consider(x.x, 4 * v); consider(x.y, 4 * v + 1); consider(x.z, 4 * v + 2); consider(x.w, 4 * v + 3);
-                }
-            }
-        }
-        if (threadIdx.x == 0) {
-            const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
-            a.top_idx[(long)r * a.topk + k] = oi;
-        }
-    }
-}
-
-// 128-thread form of the single-pass kernel: 16 CTAs per SM (all 1280 rows of the headline shape resident at once, no tail wave) and
+// Single-pass variant of vocab_stats_kernel for 16-byte aligned rows: per-thread online softmax (running max, partial sum rescaled when
+// the max grows) and one max-of-four test in front of the top-2 bookkeeping, so the row is read once and the common path is ~5
+// instructions per element.  128 threads: 16 CTAs per SM (all 1280 rows of the headline shape resident at once, no tail wave) and
 // four independent 128-bit loads in flight per thread.
 constexpr int VT2 = 128;
 __device__ __forceinline__ float block_max4(float v, float* scratch) {
@@ -547,175 +475,6 @@ __global__ void __launch_bounds__(VT2) vocab_stats_online128_kernel(const VocabS
     }
 }
 
-// Register-resident variant for rows of up to VT * 4 * NV elements (16-byte aligned): the row is read from L2/HBM exactly once, with
-// all of a thread's loads in flight together; max, sum-exp, per-thread top-2 and the rare rescan then work on registers.  Same
-// arithmetic (and the same tie order) as vocab_stats_kernel.
-template <int NV>
-__global__ void __launch_bounds__(VT) vocab_stats_reg_kernel(const VocabStepArgs a) {
-    __shared__ float s_red[VT / 32];
-    __shared__ int s_idx[VT / 32];
-    const int r = blockIdx.x;
-    const int n4 = a.V1 >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(a.logits + (long)r * a.ld);
-    float4 xs[NV];
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const int v = threadIdx.x + i * VT;
-        xs[i] = v < n4 ? g4[v] : make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-    }
-    float mx = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) mx = fmaxf(mx, fmaxf(fmaxf(xs[i].x, xs[i].y), fmaxf(xs[i].z, xs[i].w)));
-    mx = block_max(mx, s_red);
-    float t0v = -INFINITY, t1v = -INFINITY;
-    int t0i = 0x7fffffff, t1i = 0x7fffffff;
-    float sum = 0.f;
-    auto visit = [&](float x, int v) {
-        sum += __expf(x - mx);                      // padding lanes hold -inf: exp -> 0, never a candidate
-        if (x > t1v) {                              // strict: earlier (lower) indices win ties
-            if (x > t0v) { t1v = t0v; t1i = t0i; t0v = x; t0i = v; }
-            else { t1v = x; t1i = v; }
-        }
-    };
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const int v = 4 * (threadIdx.x + i * VT);
-        visit(xs[i].x, v); visit(xs[i].y, v + 1); visit(xs[i].z, v + 2); visit(xs[i].w, v + 3);
-    }
-    sum = block_sum(sum, s_red);
-    const float lsum = logf(sum);
-    const float m2 = (mx - mx) - lsum, l2 = lsum;
-    if (threadIdx.x == 0) a.stats[r] = make_float2(mx, lsum);
-    int popped = 0;
-    for (int k = 0; k < a.topk; ++k) {
-        float ov;
-        int oi;
-        block_argmax(t0v, t0i, s_red, s_idx, ov, oi);
-        if (t0i == oi && oi != 0x7fffffff) {
-            const float lastv = t0v;
-            const int lasti = t0i;
-            t0v = t1v; t0i = t1i;
-            t1v = -INFINITY; t1i = 0x7fffffff;
-            if (++popped >= 2 && t0i == 0x7fffffff) {
-                auto consider = [&](float x, int v) {
-                    const bool after = (x < lastv) || (x == lastv && v > lasti);
-                    if (after && (x > t0v || (x == t0v && v < t0i))) { t0v = x; t0i = v; }
-                };
-#pragma unroll
-                for (int i = 0; i < NV; ++i) {
-                    const int v = 4 * (threadIdx.x + i * VT);
-                    if (v < a.V1) { consider(xs[i].x, v); consider(xs[i].y, v + 1); consider(xs[i].z, v + 2); consider(xs[i].w, v + 3); }
-                }
-            }
-        }
-        if (threadIdx.x == 0) {
-            const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
-            a.top_idx[(long)r * a.topk + k] = oi;
-        }
-    }
-}
-
-// Streaming variant: persistent CTAs walk the rows; each row (V1 * 4 bytes, 16-byte aligned) arrives in shared memory through one
-// cp.async.bulk while the previous row is being reduced (double buffer), so the L2/HBM read of row i+1 overlaps the arithmetic of
-// row i and no thread ever waits on its own global loads.  Same arithmetic and tie order as vocab_stats_kernel.
-__global__ void __launch_bounds__(VT) vocab_stats_stream_kernel(const VocabStepArgs a) {
-    extern __shared__ __align__(16) unsigned char vs_smem[];
-    __shared__ float s_red[VT / 32];
-    __shared__ int s_idx[VT / 32];
-    __shared__ __align__(8) uint64_t bar[2];
-    const int V1 = a.V1, n4 = V1 >> 2;
-    const uint32_t row_bytes = (uint32_t)V1 * 4u;
-    float* buf0 = reinterpret_cast<float*>(vs_smem);
-    float* buf1 = buf0 + V1;
-    if (threadIdx.x == 0) {
-        ptx::mbar_init(&bar[0], 1);
-        ptx::mbar_init(&bar[1], 1);
-        ptx::fence_mbar_init();
-    }
-    __syncthreads();
-    int r = blockIdx.x;
-    if (threadIdx.x == 0 && r < a.rows) {
-        ptx::mbar_arrive_expect_tx(&bar[0], row_bytes);
-        ptx::bulk_load_1d(buf0, a.logits + (long)r * a.ld, row_bytes, &bar[0]);
-    }
-    for (int it = 0; r < a.rows; r += gridDim.x, ++it) {
-        const int cur = it & 1;
-        const float* g = cur ? buf1 : buf0;
-        const int rn = r + gridDim.x;
-        if (threadIdx.x == 0 && rn < a.rows) {          // the other buffer was released by the __syncthreads that ended iteration it-1
-            ptx::mbar_arrive_expect_tx(&bar[cur ^ 1], row_bytes);
-            ptx::bulk_load_1d(cur ? buf0 : buf1, a.logits + (long)rn * a.ld, row_bytes, &bar[cur ^ 1]);
-        }
-        ptx::mbar_wait(&bar[cur], (it >> 1) & 1);
-        const float4* g4 = reinterpret_cast<const float4*>(g);
-        // One pass, online softmax per thread: running max m with the partial sum rescaled when it grows (rare after the first few
-        // elements), one max-of-four test guards the top-2 bookkeeping.  The r01f capture showed the two-pass form issue-bound at
-        // ~40 thread-instructions per element; this form needs about half.
-        constexpr float kL2E = 1.4426950408889634f;
-        float t0v = -INFINITY, t1v = -INFINITY;
-        int t0i = 0x7fffffff, t1i = 0x7fffffff;
-        float m = -INFINITY, mL = -INFINITY, part = 0.f;
-        for (int v = threadIdx.x; v < n4; v += VT) {
-            const float4 x = g4[v];
-            const float m4 = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
-            if (m4 > m) {
-                online_raise(part, m, mL, m4);
-            }
-            float e0, e1, e2, e3;
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(x.x, kL2E, -mL)));
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(x.y, kL2E, -mL)));
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(fmaf(x.z, kL2E, -mL)));
-            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e3) : "f"(fmaf(x.w, kL2E, -mL)));
-            part += (e0 + e1) + (e2 + e3);
-            if (m4 > t1v) {                             // strict: earlier (lower) indices win ties
-                const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    if (xs[u] > t1v) {
-                        if (xs[u] > t0v) { t1v = t0v; t1i = t0i; t0v = xs[u]; t0i = 4 * v + u; }
-                        else { t1v = xs[u]; t1i = 4 * v + u; }
-                    }
-                }
-            }
-        }
-        const float mx = block_max(m, s_red);
-        float sum = online_finish(part, m, mL, mx);
-        sum = block_sum(sum, s_red);
-        const float lsum = logf(sum);
-        const float m2 = (mx - mx) - lsum, l2 = lsum;
-        if (threadIdx.x == 0) a.stats[r] = make_float2(mx, lsum);
-        int popped = 0;
-        for (int k = 0; k < a.topk; ++k) {
-            float ov;
-            int oi;
-            block_argmax(t0v, t0i, s_red, s_idx, ov, oi);
-            if (t0i == oi && oi != 0x7fffffff) {
-                const float lastv = t0v;
-                const int lasti = t0i;
-                t0v = t1v; t0i = t1i;
-                t1v = -INFINITY; t1i = 0x7fffffff;
-                if (++popped >= 2 && t0i == 0x7fffffff) {
-                    auto consider = [&](float x, int v) {
-                        const bool after = (x < lastv) || (x == lastv && v > lasti);
-                        if (after && (x > t0v || (x == t0v && v < t0i))) { t0v = x; t0i = v; }
-                    };
-                    for (int v = threadIdx.x; v < n4; v += VT) {
-                        const float4 x = g4[v];
-                        consider(x.x, 4 * v); consider(x.y, 4 * v + 1); consider(x.z, 4 * v + 2); consider(x.w, 4 * v + 3);
-                    }
-                }
-            }
-            if (threadIdx.x == 0) {
-                const float lp = (ov - mx) - lsum;
-                a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
-                a.top_idx[(long)r * a.topk + k] = oi;
-            }
-        }
-        __syncthreads();                                // everyone is done with buffer `cur` before it is refilled
-    }
-}
-
 // Scheduled sampling (AttModel.py:145-154): with probability `prob` the word fed into step `col` is drawn from the model's own previous
 // prediction exp(logprobs[:, col-1]) instead of the label.  One CTA per row; per-row uniform and the Gumbel-max draw come from the Philox
 // stream (seed, site 6, step col).  Non-differentiable by construction (the reference samples from a detached tensor).
@@ -765,26 +524,8 @@ int vocab_step_launch(const VocabStepArgs& a, cudaStream_t stream) {
     if (a.stats != nullptr) {
         CAPB_REQUIRE(a.select == 0 && a.topk > 0, "stats mode is the beam-search epilogue");
         const bool vec = ((a.V1 & 3) == 0) && ((a.ld & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.logits) & 15) == 0);
-        const size_t stream_smem = sizeof(float) * 2 * (size_t)a.V1;
-        // default: single-pass online kernel; "stream" / "reg" / "plain" select the other variants for A/B timing
-        static const char* variant = getenv("CAPB200_VOCAB_STATS");
-        const char vsel = variant ? variant[0] : 'o';
-        if (vec && vsel == 'o' && !(variant && variant[1] == '2')) {
-            vocab_stats_online128_kernel<<<a.rows, VT2, 0, stream>>>(a);
-        } else if (vec && vsel == 'o') {                                  // "o2": the 256-thread form
-            vocab_stats_online_kernel<<<a.rows, VT, 0, stream>>>(a);
-        } else if (vec && vsel == 's' && stream_smem <= 100 * 1024) {
-            static std::atomic<unsigned long long> configured{0};
-            if (first_use_on_device(configured)) {
-                CAPB_CHECK_CUDA(cudaFuncSetAttribute(vocab_stats_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(100 * 1024)));
-            }
-            const int grid = a.rows < 2 * sm_count() ? a.rows : 2 * sm_count();       // two resident CTAs per SM, each double-buffering one row
-            vocab_stats_stream_kernel<<<grid, VT, stream_smem, stream>>>(a);
-        } else if (vec && vsel == 'r' && a.V1 <= VT * 4 * 10) {
-            vocab_stats_reg_kernel<10><<<a.rows, VT, 0, stream>>>(a);
-        } else {
-            vocab_stats_kernel<<<a.rows, VT, 0, stream>>>(a);
-        }
+        if (vec) vocab_stats_online128_kernel<<<a.rows, VT2, 0, stream>>>(a);
+        else vocab_stats_kernel<<<a.rows, VT, 0, stream>>>(a);        // scalar loads: misaligned rows or V1 not a multiple of 4
         CAPB_CHECK_CUDA(cudaGetLastError());
         return 0;
     }

@@ -6,8 +6,8 @@ References are a few lines of torch float64 below: the row maximum and log(sum(e
 inputs (value descending, index ascending), and the kept sets of sample_next_word (CaptionModel.py:375-406).  One CPU test checks
 those helpers against brute-force loops, so a wrong reference cannot hide a wrong kernel.
 
-The statistics kernel has timing variants behind CAPB200_VOCAB_STATS (read once per process): the tests whose name contains `stats`
-must pass under each value, one pytest process per value.
+The statistics kernel has two forms: the 128-thread single-pass kernel for 16-byte aligned rows and the two-pass scalar kernel for the
+rest (a width or pitch that is not a multiple of four, a misaligned base); the `stats` tests reach both.
 
 Largest errors against float64 observed on one H100 (80 GB HBM3, 700 W): log-sum-exp 4.8e-7 with the default single-pass kernel and
 6.0e-7 with the two-pass forms, candidate log-probs 1.4e-6, the sampling kernel's stored row 1.2e-6, its picked log-prob 1.2e-6; the

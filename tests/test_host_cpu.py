@@ -153,23 +153,32 @@ def test_decode_option_guards():
         unk_model(fc, att, None, opt={'beam_size': 15, 'sample_n': 1, 'suppress_UNK': 1, 'decoding_constraint': 1}, mode='sample')
 
 
-def test_documented_switches_exist_in_the_sources():
-    """Every CAPB200_* environment variable INTEGRATION.md documents is read somewhere in the package or bench.py (no stale documentation)."""
+def test_switch_table_matches_the_sources():
+    """Every CAPB200_* environment variable INTEGRATION.md documents is read somewhere in the package or bench.py (no stale documentation),
+    and every one the package reads is in INTEGRATION.md's switch table (no hidden switches)."""
     import re
     root = os.path.dirname(os.path.dirname(__file__))
     doc = open(os.path.join(root, 'INTEGRATION.md')).read()
     documented = set(re.findall(r'`(CAPB200_[A-Z0-9_]+)', doc))
-    assert len(documented) >= 8
+    table = doc.split('### Switches', 1)[1].split('\n#', 1)[0]
+    in_table = set(re.findall(r'^\| `(CAPB200_[A-Z0-9_]+)', table, re.M))
     blob = open(os.path.join(root, 'bench.py')).read()
+    read = set()
     pkg = os.path.join(root, 'imagecaptioning.pytorch_b200')
     for d, _, files in os.walk(pkg):
         if os.path.basename(d) == 'build':
             continue
         for f in files:
             if f.endswith(('.py', '.cu', '.cuh')):
-                blob += open(os.path.join(d, f)).read()
+                src = open(os.path.join(d, f)).read()
+                blob += src
+                read |= set(re.findall(r'getenv\(\s*"(CAPB200_[A-Z0-9_]+)"', src))
+                read |= set(re.findall(r'''os\.(?:environ(?:\.get|\.setdefault|\.pop)?|getenv)\s*[\[(]\s*['"](CAPB200_[A-Z0-9_]+)''', src))
+    assert 'CAPB200_SCST_GRAPH' in read, sorted(read)        # the patterns still find the reads
     missing = sorted(v for v in documented if v not in blob)
     assert missing == [], missing
+    undocumented = sorted(read - in_table)
+    assert undocumented == [], undocumented
 
 
 def test_fused_adam_is_a_torch_adam():
