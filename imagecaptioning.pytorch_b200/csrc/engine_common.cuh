@@ -199,7 +199,15 @@ inline int grow_buffer(void** p, size_t* bytes, size_t need, cudaStream_t st) {
     if (*p) CAPB_CHECK_CUDA(cudaFree(*p));
     *p = nullptr;
     *bytes = 0;
-    CAPB_CHECK_CUDA(cudaMalloc(p, need));
+    const cudaError_t e = cudaMalloc(p, need);
+    if (e != cudaSuccess) {
+        // not sticky: clear it, or the next launch check of this thread would report it again
+        (void)cudaGetLastError();
+        *p = nullptr;
+        set_error("cannot allocate " + std::to_string(need >> 20) + " MB of device workspace (" + cudaGetErrorString(e) +
+                  "); its size grows with batch, length and V + 1: DESIGN.md, 'Vocabularies above 51 199 words'");
+        return 1;
+    }
     *bytes = need;
     return 0;
 }

@@ -92,7 +92,11 @@ int capb200_vocab_stats_topk(const float* logits, long ld, int rows, int V1, int
  * log_softmax.  select: 1 greedy, 2 multinomial, 4 top-k (top = k), 5 nucleus (top = p); the sampled kinds draw from
  * softmax(log-probs / temperature) over the kept words with one Philox block per (word, row, step, seed).  tokens_out[rows] gets the
  * word, picked_lp[rows] its log-prob.  unfinished[rows] (or NULL): unless first_step != 0, a row whose flag is 0 emits word 0, log-prob 0
- * and an all-zero row; the flag is rewritten to word != 0. */
+ * and an all-zero row; the flag is rewritten to word != 0.
+ * Supported row lengths: 1 <= V1 <= 409600.  Up to 51200 one CTA holds a row; longer rows are spread over a thread-block cluster of
+ * ceil(V1 / 51200) CTAs with the same results (same tie order, same draw for the same seed and step).  V1 > 409600 returns nonzero with
+ * the limit in capb200_last_error() before anything is launched (capb200_log_softmax_topk and every sampling / training entry point
+ * likewise; capb200_vocab_stats_topk and beam search have no length limit). */
 int capb200_vocab_select(float* logits, long ld, int rows, int V1, int select, float top, float temperature, unsigned long long seed,
                          unsigned long long step, int* unfinished, int first_step, int* tokens_out, float* picked_lp, void* stream);
 
