@@ -11,9 +11,10 @@ from . import rewards                                 # noqa: F401
 from . import parallel                                # noqa: F401
 from . import utils                                   # noqa: F401
 from . import eval_utils                              # noqa: F401
+from . import eval_multi                              # noqa: F401
 from . import grad_sync                               # noqa: F401
 from . import optim                                   # noqa: F401
 from .utils import decode_sequence                    # noqa: F401
 
 __all__ = ['setup', 'B200UpDownModel', 'B200NewFCModel', 'B200Att2in2Model', 'B200TransformerModel', 'B200AoAModel', 'B200AttEnsemble', 'B200CaptionModel', 'B200LossWrapper', 'RewardCriterion',
-           'rewards', 'parallel', 'utils', 'eval_utils', 'grad_sync', 'decode_sequence']
+           'rewards', 'parallel', 'utils', 'eval_utils', 'eval_multi', 'grad_sync', 'decode_sequence']

@@ -88,7 +88,10 @@ def eval_split_n(model, n_predictions, input_data, eval_kwargs: Dict[str, Any] =
     ``sample_n_method`` 'bs' (the sample_n best beams), 'sample' / 'gumbel' / 'top<k>' / 'top<p>' (sample_n draws, with their perplexity:
     read back with ONE transfer for the batch instead of one .item() per caption).  'dbs' is diverse beam search: sample_n groups of
     beam_size beams, one caption per group (each group's best), on the engine for UpDown and AoANet.  The remaining branch is diverse
-    sampling (group_size > 1 with beam_size 1), which the engine refuses; the model's own NotImplementedError surfaces."""
+    sampling (group_size > 1 with beam_size 1), which the engine refuses; the model's own NotImplementedError surfaces.
+
+    Returns the captions' ids, int64 [n_images * sample_n, T] on the model's device, in the order they were appended to ``n_predictions``
+    (sample_n consecutive rows per image): ``eval_multi.div_stats`` / ``eval_multi.self_cider`` score them without re-tokenising."""
     verbose = eval_kwargs.get('verbose', True)
     beam_size = eval_kwargs.get('beam_size', 1)
     sample_n = eval_kwargs.get('sample_n', 1)
@@ -100,8 +103,10 @@ def eval_split_n(model, n_predictions, input_data, eval_kwargs: Dict[str, Any] =
         kw.update({'sample_n': 1, 'beam_size': sample_n, 'group_size': 1})
         with torch.no_grad():
             model(fc_feats, att_feats, att_masks, opt=kw, mode='sample')
+        rows = []
         for k in range(n_images):
-            sents = decode_sequence(model.vocab, torch.stack([model.done_beams[k][_]['seq'] for _ in range(sample_n)]))
+            rows.append(torch.stack([model.done_beams[k][_]['seq'] for _ in range(sample_n)]))
+            sents = decode_sequence(model.vocab, rows[-1])
             for sent in sents:
                 n_predictions.append({'image_id': data['infos'][k]['id'], 'caption': sent})
     elif sample_n_method in ('sample', 'gumbel') or sample_n_method.startswith('top'):
@@ -115,8 +120,10 @@ def eval_split_n(model, n_predictions, input_data, eval_kwargs: Dict[str, Any] =
         kw.update({'beam_size': sample_n * beam_size, 'group_size': sample_n})
         with torch.no_grad():
             model(fc_feats, att_feats, att_masks, opt=kw, mode='sample')
+        rows = []
         for k in range(n_images):
-            sents = decode_sequence(model.vocab, torch.stack([model.done_beams[k][_]['seq'] for _ in range(0, sample_n * beam_size, beam_size)]))
+            rows.append(torch.stack([model.done_beams[k][_]['seq'] for _ in range(0, sample_n * beam_size, beam_size)]))
+            sents = decode_sequence(model.vocab, rows[-1])
             for sent in sents:
                 n_predictions.append({'image_id': data['infos'][k]['id'], 'caption': sent})
     else:
@@ -128,6 +135,10 @@ def eval_split_n(model, n_predictions, input_data, eval_kwargs: Dict[str, Any] =
     if verbose:
         for entry in sorted(n_predictions[-n_images * sample_n:], key=lambda x: x['image_id']):
             print('image %s: %s' % (entry['image_id'], entry['caption']))
+    if sample_n_method in ('bs', 'dbs'):
+        T = max(r.shape[1] for r in rows)
+        seq = torch.cat([torch.nn.functional.pad(r, (0, T - r.shape[1])) for r in rows])
+    return seq
 
 
 def eval_split(model, crit, loader, eval_kwargs: Dict[str, Any] = {}):

@@ -3,6 +3,7 @@
     init_scorer(cached_tokens)                                   rewards.py:25-31
     get_self_critical_reward(greedy_res, data_gts, gen_result, opt)   rewards.py:41-81
     get_scores(data_gts, gen_result, opt)                             rewards.py:83-114
+    get_self_cider_scores(data_gts, gen_result, opt)                  rewards.py:116-138
 
 The reference moves both id tensors to the host, formats every id as a string and walks Python dicts; here the ids
 never leave the GPU: n-gram extraction, the document-frequency lookup (open-addressing hash table built once from the
@@ -336,3 +337,54 @@ def get_scores(data_gts, gen_result, opt):
     w = wc
     scores = cider_scores(data_gts, gen_result)
     return scores if w == 1.0 else scores * w
+
+
+def _self_cider_table(table: Optional[CiderDTable]) -> CiderDTable:
+    table = table or CiderD_scorer
+    if table is None:
+        raise RuntimeError('init_scorer(cached_tokens) must be called before the self-CIDEr scores (tools/train.py:150-152)')
+    if isinstance(table, CorpusCiderDTable):
+        raise NotImplementedError("self-CIDEr needs document frequencies with a reference length; a corpus table (init_scorer('corpus')) has "
+                                  "none until a CIDEr-D score has been computed, and the reference fails its assert there too")
+    return table
+
+
+def check_caption_sets(rows: int, n: int, T: int) -> int:
+    """Number of images of ``rows`` captions in sets of ``n``; raises ValueError for the shapes the diversity kernels refuse."""
+    if n < 2:
+        raise ValueError('diversity needs at least 2 captions per image (log(n) = 0 below that), got %d' % n)
+    if n > 32:
+        raise ValueError('at most 32 captions per image, got %d' % n)
+    if rows % n:
+        raise ValueError('%d captions do not split into sets of %d' % (rows, n))
+    if T < 1 or T > 64:
+        raise ValueError('caption length between 1 and 64 tokens, got %d' % T)
+    return rows // n
+
+
+def self_cider(seqs: torch.Tensor, n: int, table: Optional[CiderDTable] = None, with_eos: bool = True):
+    """(matrices float64 [B, n, n], scores float64 [B]) on the device (capb200_self_cider): each image's n x n self-CIDEr matrix
+    (CiderScorer.my_get_self_cider) and its eigenvalue diversity.  with_eos keeps each caption through its first 0, as array_to_str does;
+    without it the caption stops before the 0, as the decoded words do."""
+    rows, T = seqs.shape
+    B = check_caption_sets(int(rows), int(n), int(T))
+    table = _self_cider_table(table)
+    dev = seqs.device
+    if dev.type != 'cuda':
+        raise RuntimeError('capb200: the diversity kernels run on CUDA tensors only')
+    ids = seqs.detach().to(torch.long).contiguous()
+    out = torch.empty(B * n * n + B, dtype=torch.float64, device=dev)
+    _lib.check(_lib.load().capb200_self_cider(table._h, _lib.ptr(ids), B, n, T, 1 if with_eos else 0, _lib.ptr(out), _lib.ptr(out[B * n * n:]),
+                                              _lib.current_stream()), 'self_cider')
+    return out[:B * n * n].view(B, n, n), out[B * n * n:]
+
+
+def get_self_cider_scores(data_gts, gen_result, opt):
+    """rewards.py:116-138: the eigenvalue diversity of each image's self-CIDEr matrix, float64 [len(data_gts)] on the device (the
+    reference returns the same values as a host numpy array, as get_scores does).  Captions are cut through their first 0, as array_to_str
+    writes them; the document frequencies and ref_len are those init_scorer loaded (the reference's Cider(df=cached_tokens) reads the
+    same pickle).  An n-gram missing from the table counts as df 0 where the reference's plain dict raises KeyError."""
+    rows = int(gen_result.shape[0])
+    n = rows // max(len(data_gts), 1)
+    check_caption_sets(rows, n, int(gen_result.shape[1]))
+    return self_cider(gen_result, n, with_eos=True)[1]

@@ -392,6 +392,29 @@ int capb200_reward_criterion_backward(const long long* seq, const float* reward,
                                       float* grad, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Diversity of caption sets (captioning/utils/rewards.py:116-138 get_self_cider_scores, captioning/utils/eval_multi.py:121-217)
+ * seqs[n_images * n, T] int64 device: n consecutive captions per image, 2 <= n <= 32, T <= 64.  Nothing is allocated; every output is
+ * float64 device memory unless stated.
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* Self-CIDEr: out_mat[n_images, n, n] = CiderScorer.my_get_self_cider (plain CIDEr: tf-idf cosine per order, mean over orders 1..4, x 10)
+ * with the document frequencies and ref_len of `t`; an n-gram the table does not hold has df 0.  with_eos = 1 keeps each caption through
+ * its first 0 (array_to_str, the reward form), 0 stops before it (the decoded words of eval_self_cider).  out_score[n_images] = the
+ * eigenvalue diversity of out_mat, as capb200_self_cider_div computes it.  A corpus table is refused. */
+int capb200_self_cider(const capb200_cider_table* t, const long long* seqs, int n_images, int n, int T, int with_eos, double* out_mat,
+                       double* out_score, void* stream);
+/* out_score[i] = -log(sqrt(l_max) / sum_k sqrt(l_k)) / log(n) over the eigenvalues l of mat[i] / 10 clipped at 0 (rewards.py:130-133);
+ * like numpy's eigvalsh, only the lower triangle of mat[n_images, n, n] is read.  All-zero eigenvalues give nan, as in the reference. */
+int capb200_self_cider_div(const double* mat, int n_images, int n, double* out_score, void* stream);
+/* Div-n and mutual BLEU over the words of each caption (the ids before its first 0), ids in [1, V1):
+ *   out_div1[n_images], out_div2[n_images]   distinct uni- / bigrams of the image's captions / (1e-6 + words) (div_utils.compute_div_n)
+ *   out_gdiv1[1]                             distinct words over every caption (compute_global_div_n), -1 if an id is outside [1, V1)
+ *   out_mbleu[n, 4]                          corpus BLEU-1..4 of leave-one-out round j: caption j of every image against its other n - 1
+ *   out_bleu2[n_images, n]                   per-sentence BLEU-2 of caption j against the image's other captions (Bleu(4) scores[1])
+ *   out_bleu_stats[n_images, n, 6] int32     correct 1..4-grams, length and closest reference length of each caption in its round */
+int capb200_div_stats(const long long* seqs, int n_images, int n, int T, int V1, double* out_div1, double* out_div2, double* out_gdiv1,
+                      double* out_mbleu, double* out_bleu2, int* out_bleu_stats, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * One self-critical training step of the UpDown model (LossWrapper.forward with sc_flag, loss_wrapper.py:56-73, plus the
  * loss.backward() of tools/train.py:189): eval-mode greedy baseline, train-mode multinomial samples (dropout on, AttModel.py:74-88,
  * :637), self-critical reward (CIDEr-D, or weighted CIDEr-D + BLEU-4 with opts->reward_weights), RewardCriterion, then back-propagation
