@@ -514,10 +514,16 @@ inline int attn_chunks(int seqs, int heads, int units) {      // query chunks so
 }
 int seq_attn_train_launch(int seqs, int n_keys, int q_lo, int q_hi, int heads, int dk, int causal, int idx_L, long b_stride, long p_stride, const float* q,
                           const float* k, const float* v, long ld, unsigned long long seed, int site, float p, float* out, long ld_out, const float* key_mask,
-                          long ld_mask, cudaStream_t st) {
+                          long ld_mask, cudaStream_t st, int form) {
     if (seqs <= 0 || q_hi <= q_lo) return 0;
     CAPB_REQUIRE((dk & 3) == 0, "self-attention (train): the head width must be a multiple of 4");
     const size_t smem = sizeof(float) * ((size_t)2 * n_keys * (dk + 4) + 8 * n_keys + 8 * dk);
+    if (form == 2 || (form == 0 && smem > 200 * 1024)) {
+        CAPB_REQUIRE(!causal && q_lo == 0 && q_hi == n_keys, "self-attention (train): the key-tiled form runs every query against every key");
+        ActView o;
+        o.f = out; o.ld = ld_out;
+        return attn_tiled_forward_launch(seqs, n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, key_mask, ld_mask, seed, site, p, o, st);
+    }
     CAPB_REQUIRE(smem <= 200 * 1024, "self-attention (train): keys * head width too large for the shared-memory staging");
     static std::atomic<unsigned long long> configured{0};
     if (first_use_on_device(configured)) {
@@ -531,10 +537,15 @@ int seq_attn_train_launch(int seqs, int n_keys, int q_lo, int q_hi, int heads, i
 }
 int seq_attn_backward_launch(int seqs, int n_keys, int heads, int dk, int causal, int idx_L, long b_stride, long p_stride, const float* q, const float* k,
                              const float* v, long ld, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dk_,
-                             float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st) {
+                             float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st, int form) {
     if (seqs <= 0) return 0;
     CAPB_REQUIRE((dk & 3) == 0, "self-attention backward: the head width must be a multiple of 4");
     const size_t smem = sizeof(float) * ((size_t)4 * n_keys * (dk + 4) + 2 * n_keys * n_keys);
+    if (form == 2 || (form == 0 && smem > 200 * 1024)) {
+        CAPB_REQUIRE(!causal, "self-attention backward: the key-tiled form has no causal mask");
+        return attn_tiled_self_backward_launch(seqs, n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, seed, site, p, d_out, ld_do, dq, dk_, dv, ld_d,
+                                               key_mask, ld_mask, st);
+    }
     CAPB_REQUIRE(smem <= 200 * 1024, "self-attention backward: shared-memory footprint too large");
     static std::atomic<unsigned long long> configured{0};
     if (first_use_on_device(configured)) {
@@ -571,10 +582,13 @@ int cross_attn_train_launch(int rows, int rpi, int heads, int dk, int R, const f
 }
 int cross_attn_backward_launch(int B, int rpi, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv, long ld_kv,
                                unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out, long ld_do, float* dq, long ld_dq,
-                               float* dkk, float* dvv, long ld_dkv, cudaStream_t st, int n_steps, int row_mod) {
+                               float* dkk, float* dvv, long ld_dkv, cudaStream_t st, int n_steps, int row_mod, int form) {
     const int rpi1 = rpi;
     rpi = rpi1 * (n_steps > 0 ? n_steps : 1);          // all of the image's rows in this launch
-    const size_t smem = sizeof(float) * ((size_t)2 * R * (dk + 1) + 2 * rpi * (dk + 1) + 2 * rpi * R);
+    const size_t smem = sizeof(float) * ((size_t)2 * R * (dk + 1) + 2 * rpi * (dk + 1) + 2 * (size_t)rpi * R);
+    if (form == 2 || (form == 0 && smem > 200 * 1024))
+        return attn_tiled_cross_backward_launch(B, rpi1, rpi / rpi1, row_mod > 0 ? row_mod : B * rpi1, heads, dk, R, q, ld_q, kk, vv, ld_kv, seed, site, step, p,
+                                                probs, d_out, ld_do, dq, ld_dq, dkk, dvv, ld_dkv, st);
     CAPB_REQUIRE(smem <= 200 * 1024, "decoder attention backward: shared-memory footprint too large");
     static std::atomic<unsigned long long> configured{0};
     if (first_use_on_device(configured)) {

@@ -137,8 +137,10 @@ int gather_logprob_rows_launch(const float* slab, long step_stride, long ld_slab
 // ---- transformer.cu
 int layer_norm_launch(int rows, int D, const float* x, long ld_x, const float* a, const float* b, float eps, ActView out, cudaStream_t st);
 int embed_pe_launch(int rows, int D, const int* tokens, const float* lut, const float* pe_row, float scale, ActView out, cudaStream_t st);
+// form (here and in the self / cross attention train launchers below): 0 = the staged kernel when its shared-memory footprint fits in 200 KB,
+// else the key-tiled one (attn_tiled.cu); 1 = staged only; 2 = key-tiled only (capb200_mha_* op tests)
 int enc_self_attention_launch(int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* mask,
-                              long ld_mask, ActView out, cudaStream_t st);
+                              long ld_mask, ActView out, cudaStream_t st, int form = 0);
 int dec_self_attention_launch(int rows, int heads, int dk, int t, const float* qkv, long ld_qkv, float* kcache, float* vcache, long step_stride,
                               long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, ActView out, cudaStream_t st);
 int cross_attention_launch(int rows, int rpi, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv, long ld_kv,
@@ -216,8 +218,10 @@ int dropout_salt_set_scst(unsigned long long salt, cudaStream_t st);
 int dropout_salt_set_aoa(unsigned long long salt, cudaStream_t st);
 int dropout_salt_set_tfm(unsigned long long salt, cudaStream_t st);
 int dropout_salt_set_vocab(unsigned long long salt, cudaStream_t st);
+int dropout_salt_set_attn(unsigned long long salt, cudaStream_t st);
 inline int dropout_salt_set_all(unsigned long long salt, cudaStream_t st) {
-    return dropout_salt_set_scst(salt, st) | dropout_salt_set_aoa(salt, st) | dropout_salt_set_tfm(salt, st) | dropout_salt_set_vocab(salt, st);
+    return dropout_salt_set_scst(salt, st) | dropout_salt_set_aoa(salt, st) | dropout_salt_set_tfm(salt, st) | dropout_salt_set_vocab(salt, st) |
+           dropout_salt_set_attn(salt, st);
 }
 // ---- tfm_train_kernels.cu: element-wise pieces of the Transformer training steps on TIME-major rows (row = t * rps + n; dropout keyed by (t, n))
 int embed_pe_dropout_launch(int rows, int rps, int D, const int* tok, const float* lut, const float* pe, float scale, int t0, unsigned long long seed, int site,
@@ -234,10 +238,10 @@ int load_tokens_tm_launch(const long long* labels, long ld, int N, int L, int* t
 // sequence self-attention with replayable dropout (aoa_train_kernels.cu): row(b, pos) = b * b_stride + pos * p_stride
 int seq_attn_train_launch(int seqs, int n_keys, int q_lo, int q_hi, int heads, int dk, int causal, int idx_L, long b_stride, long p_stride, const float* q,
                           const float* k, const float* v, long ld, unsigned long long seed, int site, float p, float* out, long ld_out, const float* key_mask,
-                          long ld_mask, cudaStream_t st);
+                          long ld_mask, cudaStream_t st, int form = 0);
 int seq_attn_backward_launch(int seqs, int n_keys, int heads, int dk, int causal, int idx_L, long b_stride, long p_stride, const float* q, const float* k,
                              const float* v, long ld, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dk_,
-                             float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st);
+                             float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st, int form = 0);
 int enc_attn_train_launch(int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, unsigned long long seed, int site, float p,
                           float* out, long ld_out, cudaStream_t st, const float* mask = nullptr, long ld_mask = 0);
 int enc_attn_backward_launch(int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, unsigned long long seed, int site, float p,
@@ -248,7 +252,16 @@ int cross_attn_train_launch(int rows, int rpi, int heads, int dk, int R, const f
                             const float* mask = nullptr, long ld_mask = 0, int row_mod = 0);
 int cross_attn_backward_launch(int B, int rpi, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv, long ld_kv,
                                unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out, long ld_do, float* dq, long ld_dq,
-                               float* dkk, float* dvv, long ld_dkv, cudaStream_t st, int n_steps = 1, int row_mod = 0);
+                               float* dkk, float* dvv, long ld_dkv, cudaStream_t st, int n_steps = 1, int row_mod = 0, int form = 0);
+// ---- attn_tiled.cu: key-tiled forms of the above (non-causal self-attention; cross-attention backward), no footprint grows with the keys
+int attn_tiled_forward_launch(int seqs, int n_keys, int heads, int dk, int idx_L, long b_stride, long p_stride, const float* q, const float* k, const float* v,
+                              long ld, const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, ActView out, cudaStream_t st);
+int attn_tiled_self_backward_launch(int seqs, int n_keys, int heads, int dk, int idx_L, long b_stride, long p_stride, const float* q, const float* k,
+                                    const float* v, long ld, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dk_,
+                                    float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st);
+int attn_tiled_cross_backward_launch(int B, int rpi1, int n_steps, int row_mod, int heads, int dk, int R, const float* q, long ld_q, const float* kk,
+                                     const float* vv, long ld_kv, unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out,
+                                     long ld_do, float* dq, long ld_dq, float* dkk, float* dvv, long ld_dkv, cudaStream_t st);
 int mean_backward_launch(int B, int R, int H, const float* d_mean, long ld_dm, float* dx, long ld_dx, cudaStream_t st, const float* mask = nullptr,
                          long ld_mask = 0);
 int add_dropout_launch(int rows, int cols, const float* a, long ld_a, const float* b, long ld_b, float* out, long ld_o, unsigned long long seed, int site, int step,

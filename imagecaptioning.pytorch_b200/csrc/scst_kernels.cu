@@ -531,7 +531,14 @@ int attention_backward_launch(int n_images, int rpi, int R, int A, int H, const 
     const int items = n_images * rpi * R;
     attention_dalpha_kernel<<<cdiv(items, 8), 256, 0, st>>>(items, rpi, R, H, d_out, att, d_alpha_scratch);
     CAPB_CHECK_CUDA(cudaGetLastError());
-    const size_t smem = sizeof(float) * (2 * rpi * R + 256 * (rpi + 1));
+    const size_t smem = sizeof(float) * (2 * (size_t)rpi * R + 256 * (rpi + 1));
+    // d alpha and alpha of the image's rows are staged whole: past the default 48 KB above about 248 regions at 16 rows per image
+    // (148 KB at 1024 regions)
+    CAPB_REQUIRE(smem <= 200 * 1024, "attention backward: rows per image x regions too large for the shared-memory staging");
+    static std::atomic<unsigned long long> configured{0};
+    if (first_use_on_device(configured)) {
+        CAPB_CHECK_CUDA(cudaFuncSetAttribute(attention_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    }
     attention_backward_kernel<<<dim3(n_images, cdiv(A, 32)), 256, smem, st>>>(rpi, R, A, H, d_out, alpha, d_alpha_scratch, att_h, p_att, w, d_att_h, d_att, d_p_att,
                                                                              d_w, d_b);
     LAUNCH_OK();

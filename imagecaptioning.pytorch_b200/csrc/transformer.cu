@@ -250,9 +250,11 @@ int embed_pe_launch(int rows, int D, const int* tokens, const float* lut, const 
 }
 
 int enc_self_attention_launch(int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* mask,
-                              long ld_mask, ActView out, cudaStream_t st) {
+                              long ld_mask, ActView out, cudaStream_t st, int form) {
     if (B <= 0) return 0;
     const size_t smem = sizeof(float) * ((size_t)2 * R * (dk + 1) + 8 * R + 8 * dk);
+    if (form == 2 || (form == 0 && smem > 200 * 1024))
+        return attn_tiled_forward_launch(B, R, heads, dk, R, R, 1, q, k, v, ld, mask, ld_mask, 0ull, 0, 0.f, out, st);
     CAPB_REQUIRE(smem <= 200 * 1024, "self-attention: region count x head width too large for the shared-memory staging");
     int chunks = (296 + B * heads - 1) / (B * heads);           // query chunks: about two CTAs per SM even for a 10-image batch
     chunks = chunks > 4 ? 4 : (chunks < 1 ? 1 : chunks);

@@ -622,6 +622,27 @@ int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* events, int 
  * (Att2in2 has no site 0: it has no fc_embed.  NewFC has site 3 only: its embeddings are a bare nn.Embedding / nn.Linear.) */
 int capb200_dropout_mask(float* mask, long n, unsigned long long seed, int site, int step, float p, void* stream);
 
+/* Multi-head attention operations of the AoANet refiner / Transformer encoder and of the decoders' attention over the regions, for tests.
+ * `form`: 0 picks the kernel as the training steps and the decoder do (the staged kernel when its shared-memory footprint fits in 200 KB,
+ * else the key-tiled one), 1 forces the staged kernel (an error where it does not fit), 2 forces the key-tiled kernel (head width a multiple
+ * of 4, at most 256).  Head h of a row is columns [h*dk, (h+1)*dk); scale 1/sqrt(dk); mask [B, ld_mask] (0 = masked key) or NULL.
+ * Dropout on the probabilities uses element ((b*heads + h)*R + i)*R + r at step 0 of `site` (self-attention) and item*R + r with
+ * item = (row within its time block)*heads + h at step `step` + time block (cross-attention): capb200_dropout_mask replays both.
+ *   capb200_mha_forward        out = softmax(q k^T / sqrt(dk)) v over the R regions of each of B images, rows image-major [B*R, ld];
+ *                              train = 0: the decode form (no dropout; seed, site and p unused), 1: the training form with dropout p
+ *   capb200_mha_self_backward  dq, dkey, dval (written, pitch ld_d; dq must not alias an input) of capb200_mha_forward(train = 1)
+ *   capb200_mha_cross_backward rows TIME-major: row = t*(B*rpi) + b*rpi + j for t < n_steps; keys / values [B*R, ld_kv]; probs [rows*heads, R]
+ *                              the saved probabilities before dropout; dq written, dk / dv ADDED into [B*R, ld_dkv]
+ * Return 0 or 1 (capb200_last_error). */
+int capb200_mha_forward(int form, int train, int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* mask,
+                        long ld_mask, unsigned long long seed, int site, float p, float* out, long ld_out, void* stream);
+int capb200_mha_self_backward(int form, int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* mask,
+                              long ld_mask, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dkey, float* dval,
+                              long ld_d, void* stream);
+int capb200_mha_cross_backward(int form, int B, int rpi, int n_steps, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv,
+                               long ld_kv, unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out, long ld_do, float* dq,
+                               long ld_dq, float* dkk, float* dvv, long ld_dkv, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Training steps of the Transformer captioner (TransformerModel.py:262-363 under LossWrapper, loss_wrapper.py:25-73, + loss.backward()).
  *   capb200_tfm_xe_step    the teacher-forced TransformerModel._forward (:340-348: one pass over all label_cols - 1 positions; keys that
