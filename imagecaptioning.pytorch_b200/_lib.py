@@ -275,6 +275,12 @@ SIGNATURES = {
                                           c_float, c_void_p, c_long, c_void_p, c_void_p, c_void_p, c_long, c_void_p]),
     'capb200_mha_cross_backward': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_long, c_void_p, c_void_p, c_long, c_ulonglong,
                                            c_int, c_int, c_float, c_void_p, c_void_p, c_long, c_void_p, c_long, c_void_p, c_void_p, c_long, c_void_p]),
+    'capb200_mha_causal_forward': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_long, c_void_p, c_long,
+                                           c_ulonglong, c_int, c_float, c_void_p, c_long, c_void_p]),
+    'capb200_mha_causal_backward': (c_int, [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_long, c_void_p, c_long, c_ulonglong,
+                                            c_int, c_float, c_void_p, c_long, c_void_p, c_void_p, c_void_p, c_long, c_void_p]),
+    'capb200_tfm_dec_self_attention': (c_int, [c_int, c_int, c_int, c_int, c_int, c_void_p, c_long, c_void_p, c_void_p, c_long, c_long, c_void_p,
+                                               c_long, c_void_p, c_long, c_void_p, c_long, c_void_p]),
     'capb200_tfm_xe_step': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmXeOpts), c_void_p, c_void_p, c_int, POINTER(TfmWeights), c_void_p, c_void_p,
                                     c_void_p]),
     'capb200_tfm_scst_step': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmScstOpts), c_void_p, c_void_p, c_void_p, c_int, POINTER(TfmWeights),

@@ -343,7 +343,7 @@ capb200_aoa_engine* capb200_aoa_create(const capb200_aoa_cfg* c) {
     if (c == nullptr) { set_error("null cfg"); return nullptr; }
     if (c->heads < 1 || c->rnn_size % c->heads != 0) { set_error("rnn_size must be divisible by the head count"); return nullptr; }
     if (c->numeric_mode < 0 || c->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
-    if (c->seq_length < 1 || c->seq_length > 64) { set_error("seq_length must be in 1..64"); return nullptr; }
+    if (c->seq_length < 1 || c->seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device: the capb200 engine has no CPU fallback"); return nullptr; }
     capb200_aoa_engine* e = new capb200_aoa_engine();

@@ -519,10 +519,10 @@ int seq_attn_train_launch(int seqs, int n_keys, int q_lo, int q_hi, int heads, i
     CAPB_REQUIRE((dk & 3) == 0, "self-attention (train): the head width must be a multiple of 4");
     const size_t smem = sizeof(float) * ((size_t)2 * n_keys * (dk + 4) + 8 * n_keys + 8 * dk);
     if (form == 2 || (form == 0 && smem > 200 * 1024)) {
-        CAPB_REQUIRE(!causal && q_lo == 0 && q_hi == n_keys, "self-attention (train): the key-tiled form runs every query against every key");
         ActView o;
         o.f = out; o.ld = ld_out;
-        return attn_tiled_forward_launch(seqs, n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, key_mask, ld_mask, seed, site, p, o, st);
+        return attn_tiled_forward_launch(seqs, n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, key_mask, ld_mask, seed, site, p, o, st, causal,
+                                         q_lo, q_hi);
     }
     CAPB_REQUIRE(smem <= 200 * 1024, "self-attention (train): keys * head width too large for the shared-memory staging");
     static std::atomic<unsigned long long> configured{0};
@@ -542,9 +542,8 @@ int seq_attn_backward_launch(int seqs, int n_keys, int heads, int dk, int causal
     CAPB_REQUIRE((dk & 3) == 0, "self-attention backward: the head width must be a multiple of 4");
     const size_t smem = sizeof(float) * ((size_t)4 * n_keys * (dk + 4) + 2 * n_keys * n_keys);
     if (form == 2 || (form == 0 && smem > 200 * 1024)) {
-        CAPB_REQUIRE(!causal, "self-attention backward: the key-tiled form has no causal mask");
         return attn_tiled_self_backward_launch(seqs, n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, seed, site, p, d_out, ld_do, dq, dk_, dv, ld_d,
-                                               key_mask, ld_mask, st);
+                                               key_mask, ld_mask, st, causal);
     }
     CAPB_REQUIRE(smem <= 200 * 1024, "self-attention backward: shared-memory footprint too large");
     static std::atomic<unsigned long long> configured{0};

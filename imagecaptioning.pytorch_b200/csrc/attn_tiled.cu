@@ -1,6 +1,8 @@
-// Key-tiled multi-head attention: the forms of the refiner / encoder self-attention and of the decoder's cross-attention backward that
-// the staged kernels (transformer.cu, aoa_train_kernels.cu) cannot hold in 200 KB of shared memory.  K, V and the scores stream through
-// shared memory one tile of 32 keys at a time, so no shared-memory footprint grows with the region count.
+// Key-tiled multi-head attention: the forms of the refiner / encoder self-attention, of the Transformer decoder's causal self-attention and of
+// the decoder's cross-attention backward that the staged kernels (transformer.cu, aoa_train_kernels.cu) cannot hold in 200 KB of shared
+// memory.  K, V and the scores stream through shared memory one tile of 32 keys at a time, so no shared-memory footprint grows with the
+// region count or the caption length.  Causal (key r visible to query i iff r <= i): the key tiles past a query tile's last query are
+// skipped, and the tile that straddles the diagonal masks the keys past each query.
 //
 //   forward        one CTA per (sequence, head, tile of 32 queries); online softmax over the key tiles, key mask (-inf) and the
 //                  replayable probability dropout (p = 0: the decode form)
@@ -61,6 +63,7 @@ struct TiledAttn {
     unsigned long long seed;
     uint32_t site, step;
     int cross, idx_L;
+    int causal, q_lo;               // causal self-attention; forward: the queries are [q_lo, nq)
     const float* key_mask;          // self-attention: [seqs, ld_mask], 0 = masked key
     long ld_mask;
     const float* probs;             // cross-attention: saved probabilities [(row * heads + head) * nk + r]
@@ -76,6 +79,12 @@ struct TiledAttn {
         return drop_scale(seed, site, 0u, (uint32_t)((((long)s * heads + head) * idx_L + i) * idx_L + r), p_drop);
     }
     __device__ bool key_on(int s, int r) const { return key_mask == nullptr || key_mask[(long)s * ld_mask + r] != 0.f; }
+    // keys [0, key_end) can be visible to the queries [q0, q0 + 32) of a tile
+    __device__ int key_end(int q0) const {
+        if (!causal) return nk;
+        const int e = q0 + kTile < nq ? q0 + kTile : nq;
+        return e < nk ? e : nk;
+    }
 };
 
 // rows [row0, row0 + 32) of a head slice into shared memory [32][W]; rows past n are zero
@@ -97,7 +106,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_forward_kernel(TiledAt
     float* sK = sm;
     float* sV = sK + kTile * W;
     float* sQ = sV + kTile * W;
-    const int s = blockIdx.x, head = blockIdx.y, q0 = blockIdx.z * kTile;
+    const int s = blockIdx.x, head = blockIdx.y, q0 = a.q_lo + blockIdx.z * kTile;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     stage_rows(sQ, W, dk, a.nq, a.q, a.ld_q, head, a, s, q0, false);
     float m[kPerWarp], l[kPerWarp], acc[kPerWarp][NC];
@@ -107,17 +116,19 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_forward_kernel(TiledAt
 #pragma unroll
         for (int i = 0; i < NC; ++i) acc[u][i] = 0.f;
     }
-    for (int k0 = 0; k0 < a.nk; k0 += kTile) {
+    const int k_end = a.key_end(q0);
+    for (int k0 = 0; k0 < k_end; k0 += kTile) {
         __syncthreads();
         stage_rows(sK, W, dk, a.nk, a.k, a.ld_kv, head, a, s, k0, true);
         stage_rows(sV, W, dk, a.nk, a.v, a.ld_kv, head, a, s, k0, true);
         __syncthreads();
         const int r = k0 + lane;
-        const bool on = r < a.nk && a.key_on(s, r);
+        const bool key = r < a.nk && a.key_on(s, r);
 #pragma unroll
         for (int u = 0; u < kPerWarp; ++u) {
             const int ql = warp * kPerWarp + u, qi = q0 + ql;
             if (qi >= a.nq) break;
+            const bool on = key && (!a.causal || r <= qi);
             const float sc = on ? __fmul_rn(t_dot(sQ + ql * W, sK + lane * W, dk4), a.scale) : -INFINITY;
             const float m_new = fmaxf(m[u], t_wmax(sc));
             if (m_new == -INFINITY) continue;                   // every key so far masked: nothing to add
@@ -171,7 +182,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_rows_kernel(TiledAttn 
     float m[kPerWarp], l[kPerWarp], d[kPerWarp];
 #pragma unroll
     for (int u = 0; u < kPerWarp; ++u) { m[u] = -INFINITY; l[u] = 0.f; d[u] = 0.f; }
-    for (int k0 = 0; k0 < a.nk; k0 += kTile) {
+    const int k_end = a.key_end(q0);
+    for (int k0 = 0; k0 < k_end; k0 += kTile) {
         __syncthreads();
         if (!a.cross) stage_rows(sK, W, dk, a.nk, a.k, a.ld_kv, head, a, s, k0, true);
         stage_rows(sV, W, dk, a.nk, a.v, a.ld_kv, head, a, s, k0, true);
@@ -187,7 +199,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_rows_kernel(TiledAttn 
                 d[u] += t_wsum(p * dov);
                 continue;
             }
-            const bool on = r < a.nk && a.key_on(s, r);
+            const bool on = r < a.nk && a.key_on(s, r) && (!a.causal || r <= qi);
             const float sc = on ? __fmul_rn(t_dot(sQ + ql * W, sK + lane * W, dk4), a.scale) : -INFINITY;
             const float m_new = fmaxf(m[u], t_wmax(sc));
             if (m_new == -INFINITY) continue;
@@ -217,7 +229,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_rows_kernel(TiledAttn 
 __device__ __forceinline__ void tiled_p_ds(const TiledAttn& a, int s, int head, int i, int r, const float* qv, const float* dov_row, const float* kv,
                                            const float* vv, const float* st, float& pz, float& ds) {
     pz = 0.f; ds = 0.f;
-    if (i >= a.nq || r >= a.nk) return;
+    if (i >= a.nq || r >= a.nk || (a.causal && r > i)) return;
     const int dk4 = a.dk >> 2;
     float p, delta;
     if (a.cross) {
@@ -252,7 +264,7 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_dkv_kernel(TiledAttn a
     for (int u = 0; u < kPerWarp; ++u)
 #pragma unroll
         for (int i = 0; i < NC; ++i) { gk[u][i] = 0.f; gv[u][i] = 0.f; }
-    for (int q0 = 0; q0 < a.nq; q0 += kTile) {
+    for (int q0 = a.causal ? k0 : 0; q0 < a.nq; q0 += kTile) {          // causal: the query tiles before this key tile see none of its keys
         __syncthreads();
         stage_rows(sQ, W, dk, a.nq, a.q, a.ld_q, head, a, s, q0, false);
         stage_rows(sD, W, dk, a.nq, a.d_out, a.ld_do, head, a, s, q0, false);
@@ -319,7 +331,8 @@ __global__ void __launch_bounds__(kThreads, 1) attn_tiled_dq_kernel(TiledAttn a)
     for (int u = 0; u < kPerWarp; ++u)
 #pragma unroll
         for (int i = 0; i < NC; ++i) g[u][i] = 0.f;
-    for (int k0 = 0; k0 < a.nk; k0 += kTile) {
+    const int k_end = a.key_end(q0);
+    for (int k0 = 0; k0 < k_end; k0 += kTile) {
         __syncthreads();
         stage_rows(sK, W, dk, a.nk, a.k, a.ld_kv, head, a, s, k0, true);
         stage_rows(sV, W, dk, a.nk, a.v, a.ld_kv, head, a, s, k0, true);
@@ -370,7 +383,7 @@ int forward_nc(const TiledAttn& a, int seqs, ActView out, cudaStream_t st) {
     static std::atomic<unsigned long long> configured{0};
     const size_t smem = tiled_smem(a.dk, 3);
     if (set_smem(attn_tiled_forward_kernel<NC>, configured)) return 1;
-    attn_tiled_forward_kernel<NC><<<dim3(seqs, a.heads, cdiv(a.nq, kTile)), kThreads, smem, st>>>(a, out);
+    attn_tiled_forward_kernel<NC><<<dim3(seqs, a.heads, cdiv(a.nq - a.q_lo, kTile)), kThreads, smem, st>>>(a, out);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -422,10 +435,15 @@ TiledAttn self_args(int n_keys, int heads, int dk, int idx_L, long b_stride, lon
 }  // namespace
 
 int attn_tiled_forward_launch(int seqs, int n_keys, int heads, int dk, int idx_L, long b_stride, long p_stride, const float* q, const float* k, const float* v,
-                              long ld, const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, ActView out, cudaStream_t st) {
-    if (seqs <= 0 || n_keys <= 0) return 0;
+                              long ld, const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, ActView out, cudaStream_t st, int causal,
+                              int q_lo, int q_hi) {
+    if (q_hi < 0) q_hi = n_keys;
+    if (seqs <= 0 || n_keys <= 0 || q_hi <= q_lo) return 0;
     if (check_shape(dk, "self-attention") || check_index((long)seqs * heads * idx_L * idx_L, p, "self-attention")) return 1;
-    const TiledAttn a = self_args(n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, key_mask, ld_mask, seed, site, p);
+    CAPB_REQUIRE(q_lo >= 0 && (causal ? q_hi <= n_keys : (q_lo == 0 && q_hi == n_keys)),
+                 "self-attention (key-tiled form): a query range needs the causal form, and stays within the keys");
+    TiledAttn a = self_args(n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, key_mask, ld_mask, seed, site, p);
+    a.nq = q_hi; a.q_lo = q_lo; a.causal = causal;
     switch (tiled_nc(dk)) {
         case 1: return forward_nc<1>(a, seqs, out, st);
         case 2: return forward_nc<2>(a, seqs, out, st);
@@ -445,11 +463,12 @@ int attn_tiled_backward(const TiledAttn& a, int seqs, int accumulate, cudaStream
 
 int attn_tiled_self_backward_launch(int seqs, int n_keys, int heads, int dk, int idx_L, long b_stride, long p_stride, const float* q, const float* k,
                                     const float* v, long ld, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dk_,
-                                    float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st) {
+                                    float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st, int causal) {
     if (seqs <= 0 || n_keys <= 0) return 0;
     if (check_shape(dk, "self-attention backward") || check_index((long)seqs * heads * idx_L * idx_L, p, "self-attention backward")) return 1;
     CAPB_REQUIRE(dq != q && dq != k && dq != v && dq != d_out, "self-attention backward (key-tiled form): dq holds the row statistics, it must not alias an input");
     TiledAttn a = self_args(n_keys, heads, dk, idx_L, b_stride, p_stride, q, k, v, ld, key_mask, ld_mask, seed, site, p);
+    a.causal = causal;
     a.d_out = d_out; a.ld_do = ld_do; a.dq = dq; a.dk_ = dk_; a.dv = dv; a.ld_dq = ld_d; a.ld_dkv = ld_d;
     return attn_tiled_backward(a, seqs, 0, st);
 }
@@ -500,6 +519,25 @@ int capb200_mha_self_backward(int form, int B, int R, int heads, int dk, const f
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (dropout_salt_set_all(0ull, st)) return 1;
     return seq_attn_backward_launch(B, R, heads, dk, 0, R, R, 1, q, k, v, ld, seed, site, p, d_out, ld_do, dq, dk_, dv, ld_d, mask, ld_mask, st, form);
+}
+
+int capb200_mha_causal_forward(int form, int B, int T, int q_lo, int q_hi, int heads, int dk, const float* q, const float* k, const float* v, long ld,
+                               const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, float* out, long ld_out, void* stream) {
+    CAPB_REQUIRE(form >= 0 && form <= 2, "form is 0 (automatic), 1 (staged) or 2 (key-tiled)");
+    CAPB_REQUIRE(B > 0 && T > 0 && heads > 0 && dk > 0 && 0 <= q_lo && q_lo < q_hi && q_hi <= T && q && k && v && out, "bad argument");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (dropout_salt_set_all(0ull, st)) return 1;
+    return seq_attn_train_launch(B, q_hi, q_lo, q_hi, heads, dk, 1, T, T, 1, q, k, v, ld, seed, site, p, out, ld_out, key_mask, ld_mask, st, form);
+}
+
+int capb200_mha_causal_backward(int form, int B, int T, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* key_mask,
+                                long ld_mask, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dk_, float* dv,
+                                long ld_d, void* stream) {
+    CAPB_REQUIRE(form >= 0 && form <= 2, "form is 0 (automatic), 1 (staged) or 2 (key-tiled)");
+    CAPB_REQUIRE(B > 0 && T > 0 && heads > 0 && dk > 0 && q && k && v && d_out && dq && dk_ && dv, "bad argument");
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (dropout_salt_set_all(0ull, st)) return 1;
+    return seq_attn_backward_launch(B, T, heads, dk, 1, T, T, 1, q, k, v, ld, seed, site, p, d_out, ld_do, dq, dk_, dv, ld_d, key_mask, ld_mask, st, form);
 }
 
 int capb200_mha_cross_backward(int form, int B, int rpi, int n_steps, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv,

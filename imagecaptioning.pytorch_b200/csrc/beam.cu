@@ -10,6 +10,7 @@
 //     is lowered by 1000 but it stays in the beam and keeps being expanded (CaptionModel.py:183-198),
 //   * the full log-prob rows are never copied while searching: each step's [rows, V+1] slab stays where the vocab kernel
 //     wrote it and the winner's rows are gathered once at the end (AttModel.py:245-254 semantics).
+#include "../../include/capb200.h"
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -164,7 +165,8 @@ __global__ void __launch_bounds__(32) diverse_beam_step_kernel(BeamState s, int 
     }
 }
 
-// one warp per image: stable selection of the `keep` best records by penalised score (CaptionModel.py:207)
+// one warp per image: stable selection of the `keep` best records by penalised score (CaptionModel.py:207); dynamic shared memory holds one
+// `taken` flag per record (beam * T bytes)
 __global__ void __launch_bounds__(32) beam_finalize_kernel(BeamState s, int keep, const double* __restrict__ done_p, long long* __restrict__ out_seq,
                                                            int* __restrict__ out_len, float* __restrict__ out_p, float* __restrict__ out_raw,
                                                            int* __restrict__ out_hist) {
@@ -172,7 +174,7 @@ __global__ void __launch_bounds__(32) beam_finalize_kernel(BeamState s, int keep
     const int b = s.beam, T = s.T;
     const int cnt = s.done_cnt[img];
     const long base = (long)img * b * T;
-    __shared__ unsigned char taken[MAXB * 64];
+    extern __shared__ unsigned char taken[];
     for (int i = lane; i < cnt; i += 32) taken[i] = 0;
     __syncwarp();
     for (int k = 0; k < keep; ++k) {
@@ -345,7 +347,7 @@ int scale_rows_launch(float* x, long ld, int rows, int cols, float factor, cudaS
 int beam_step_launch(const BeamState& s, int t, int live, const float* top_val, const int* top_idx, int penalty_kind, float penalty_alpha,
                      cudaStream_t stream) {
     CAPB_REQUIRE(s.beam >= 1 && s.beam <= MAXB, "beam size 1..16");
-    CAPB_REQUIRE(s.beam * s.T <= MAXB * 64, "beam*T record capacity");
+    CAPB_REQUIRE(s.beam * s.T <= MAXB * CAPB200_MAX_SEQ_LENGTH, "beam*T record capacity (16 x CAPB200_MAX_SEQ_LENGTH)");
     beam_step_kernel<<<s.B, 32, 0, stream>>>(s, t, live, top_val, top_idx, penalty_kind, penalty_alpha, s.done_p);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -355,7 +357,7 @@ int diverse_beam_step_launch(const BeamState& s, int G, int t, int k, const floa
                              int penalty_kind, float penalty_alpha, cudaStream_t stream) {
     CAPB_REQUIRE(G >= 2 && s.beam >= 1 && G * s.beam <= MAXB, "group_size * beams per group must be in 2..16");
     CAPB_REQUIRE(k >= s.beam && k <= MAXB && s.beam * k <= 256, "candidate list width");
-    CAPB_REQUIRE(s.beam * s.T <= MAXB * 64, "beam*T record capacity");
+    CAPB_REQUIRE(s.beam * s.T <= MAXB * CAPB200_MAX_SEQ_LENGTH, "beam*T record capacity (16 x CAPB200_MAX_SEQ_LENGTH)");
     CAPB_REQUIRE(lambda >= 0.f, "diversity_lambda must be >= 0 (the candidate lists rely on the penalty only lowering values)");
     diverse_beam_step_kernel<<<s.B / G, 32, 0, stream>>>(s, G, t, k, top_val, top_idx, lambda, rows_total, penalty_kind, penalty_alpha, s.done_p);
     CAPB_CHECK_CUDA(cudaGetLastError());
@@ -365,7 +367,7 @@ int diverse_beam_step_launch(const BeamState& s, int G, int t, int k, const floa
 int beam_finalize_launch(const BeamState& s, int keep, long long* out_seq, int* out_len, float* out_p, float* out_raw, int* out_hist,
                          cudaStream_t stream) {
     CAPB_REQUIRE(keep >= 1 && keep <= s.beam, "keep must be in 1..beam");
-    beam_finalize_kernel<<<s.B, 32, 0, stream>>>(s, keep, s.done_p, out_seq, out_len, out_p, out_raw, out_hist);
+    beam_finalize_kernel<<<s.B, 32, (size_t)s.beam * s.T, stream>>>(s, keep, s.done_p, out_seq, out_len, out_p, out_raw, out_hist);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -4,7 +4,8 @@
 
 namespace capb200 {
 
-constexpr int CIDER_MAXL = 64;     // max tokens in a caption incl. the closing 0
+constexpr int CIDER_MAXL = 64;        // max tokens in a caption incl. the closing 0 (diversity kernels; the rewards' short form)
+constexpr int CIDER_MAXL_LONG = 256;  // the rewards' long form, for hypotheses or references past 64 tokens (= CAPB200_MAX_SEQ_LENGTH)
 constexpr int CIDER_N = 4;
 
 struct CiderSlot {

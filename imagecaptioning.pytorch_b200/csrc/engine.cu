@@ -566,7 +566,7 @@ capb200_engine* capb200_engine_create(const capb200_model_cfg* cfg) {
         return nullptr;
     }
     if (cfg->numeric_mode < 0 || cfg->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
-    if (cfg->seq_length < 1 || cfg->seq_length > 64) { set_error("seq_length must be in 1..64"); return nullptr; }
+    if (cfg->seq_length < 1 || cfg->seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         set_error("no CUDA device: the capb200 engine has no CPU fallback");

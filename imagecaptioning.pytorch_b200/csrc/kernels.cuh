@@ -141,8 +141,9 @@ int embed_pe_launch(int rows, int D, const int* tokens, const float* lut, const 
 // else the key-tiled one (attn_tiled.cu); 1 = staged only; 2 = key-tiled only (capb200_mha_* op tests)
 int enc_self_attention_launch(int B, int R, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* mask,
                               long ld_mask, ActView out, cudaStream_t st, int form = 0);
+// form 0: one lane per position for t < 32 (dec_self_attention_kernel), the chunked online-softmax kernel past it; 1 / 2 force one of the two
 int dec_self_attention_launch(int rows, int heads, int dk, int t, const float* qkv, long ld_qkv, float* kcache, float* vcache, long step_stride,
-                              long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, ActView out, cudaStream_t st);
+                              long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, ActView out, cudaStream_t st, int form = 0);
 int cross_attention_launch(int rows, int rpi, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv, long ld_kv,
                            const float* mask, long ld_mask, ActView out, cudaStream_t st);
 
@@ -253,12 +254,14 @@ int cross_attn_train_launch(int rows, int rpi, int heads, int dk, int R, const f
 int cross_attn_backward_launch(int B, int rpi, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv, long ld_kv,
                                unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out, long ld_do, float* dq, long ld_dq,
                                float* dkk, float* dvv, long ld_dkv, cudaStream_t st, int n_steps = 1, int row_mod = 0, int form = 0);
-// ---- attn_tiled.cu: key-tiled forms of the above (non-causal self-attention; cross-attention backward), no footprint grows with the keys
+// ---- attn_tiled.cu: key-tiled forms of the above (self-attention, causal or not; cross-attention backward), no footprint grows with the keys.
+// causal forward: queries [q_lo, q_hi) (q_hi < 0: n_keys); without causal every query runs against every key
 int attn_tiled_forward_launch(int seqs, int n_keys, int heads, int dk, int idx_L, long b_stride, long p_stride, const float* q, const float* k, const float* v,
-                              long ld, const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, ActView out, cudaStream_t st);
+                              long ld, const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, ActView out, cudaStream_t st,
+                              int causal = 0, int q_lo = 0, int q_hi = -1);
 int attn_tiled_self_backward_launch(int seqs, int n_keys, int heads, int dk, int idx_L, long b_stride, long p_stride, const float* q, const float* k,
                                     const float* v, long ld, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dk_,
-                                    float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st);
+                                    float* dv, long ld_d, const float* key_mask, long ld_mask, cudaStream_t st, int causal = 0);
 int attn_tiled_cross_backward_launch(int B, int rpi1, int n_steps, int row_mod, int heads, int dk, int R, const float* q, long ld_q, const float* kk,
                                      const float* vv, long ld_kv, unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out,
                                      long ld_do, float* dq, long ld_dq, float* dkk, float* dvv, long ld_dkv, cudaStream_t st);

@@ -15,11 +15,14 @@
 #include <cmath>
 #include <vector>
 
+#include "../../include/capb200.h"
 #include "common.cuh"
 #include "cider_table.cuh"
 #include "kernels.cuh"
 
 namespace capb200 {
+
+static_assert(CIDER_MAXL_LONG == CAPB200_MAX_SEQ_LENGTH, "the rewards' long form holds the longest caption the engines produce");
 
 CiderTable* cider_table_create(const int* keys, const double* df, long n, double ref_len, cudaStream_t stream) {
     unsigned long long cap = 64;
@@ -75,12 +78,12 @@ CiderTable* cider_corpus_table_create() {
     return t;
 }
 
-// A corpus table holds at most every n-gram of `n_refs` reference rows of `L` tokens (4 orders x min(L, 64) positions each), at a load of at most
+// A corpus table holds at most every n-gram of `n_refs` reference rows of `L` tokens (4 orders x min(L, 256) positions each), at a load of at most
 // one half.  Growing frees the old slots after a device synchronisation; the slots' address is part of a step graph's key.
 int cider_corpus_table_reserve(CiderTable* t, long n_refs, int L) {
     CAPB_REQUIRE(t != nullptr && t->corpus, "not a corpus CIDEr-D table");
     CAPB_REQUIRE(n_refs >= 0 && L >= 0, "bad reference shape");
-    const long grams = (long)CIDER_N * n_refs * (L < CIDER_MAXL ? L : CIDER_MAXL);
+    const long grams = (long)CIDER_N * n_refs * (L < CIDER_MAXL_LONG ? L : CIDER_MAXL_LONG);
     unsigned long long cap = 64;
     while (cap < (unsigned long long)(2 * grams + 2)) cap <<= 1;
     if (t->slots != nullptr && cap <= t->mask + 1) return 0;
@@ -113,9 +116,9 @@ __global__ void corpus_clear_kernel(CiderSlot* __restrict__ slots, unsigned long
     slots[i].idf = 0.0;
 }
 
-// the tokens of reference row r up to and including its first 0, at most min(L, 64)
+// the tokens of reference row r up to and including its first 0, at most min(L, 256)
 __device__ __forceinline__ int ref_len(const int* __restrict__ refs, long r, int L) {
-    const int cols = L < CIDER_MAXL ? L : CIDER_MAXL;
+    const int cols = L < CIDER_MAXL_LONG ? L : CIDER_MAXL_LONG;
     int len = 0;
     for (int j = 0; j < cols; ++j) { ++len; if (refs[r * L + j] == 0) break; }
     return len;
@@ -130,7 +133,7 @@ __global__ void __launch_bounds__(256) corpus_insert_kernel(CiderSlot* __restric
                                                             const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L, double mult) {
     const int img = blockIdx.x;
     const int r0 = ref_offsets[img], r1 = ref_offsets[img + 1];
-    const int cols = L < CIDER_MAXL ? L : CIDER_MAXL;
+    const int cols = L < CIDER_MAXL_LONG ? L : CIDER_MAXL_LONG;
     const long items = (long)(r1 - r0) * CIDER_N * cols;
     for (long it = threadIdx.x; it < items; it += blockDim.x) {
         const long r = r0 + it / (CIDER_N * cols);
@@ -194,10 +197,12 @@ int corpus_build_launch(const CiderTable* t, int B, int hyps, int per_image, con
 // Builds the tf-idf description of one caption held in shared memory.
 //   gram index g = n * MAXL + p (order n+1 starting at position p);  w[g] = tf * idf for the first occurrence, else 0
 //   nrm[n] = sqrt(sum w^2);  returns through `w`, `valid` (1 = distinct n-gram present)
+// MAXL: CIDER_MAXL (captions and references of at most 64 tokens) or CIDER_MAXL_LONG (the long form, dispatched only past 64)
+template <int MAXL>
 __device__ void cider_vectorise(const CiderSlot* slots, unsigned long long mask, double log_ref_len, const int* tok, int len, double* w,
                                 unsigned char* valid, double* nrm) {
-    for (int g = threadIdx.x; g < CIDER_N * CIDER_MAXL; g += blockDim.x) {
-        const int n = g / CIDER_MAXL + 1, p = g % CIDER_MAXL;
+    for (int g = threadIdx.x; g < CIDER_N * MAXL; g += blockDim.x) {
+        const int n = g / MAXL + 1, p = g % MAXL;
         double wv = 0.0;
         unsigned char ok = 0;
         if (p + n <= len) {
@@ -220,8 +225,8 @@ __device__ void cider_vectorise(const CiderSlot* slots, unsigned long long mask,
     __syncthreads();
     if (threadIdx.x < CIDER_N) {
         double s = 0.0;
-        for (int p = 0; p < CIDER_MAXL; ++p) {
-            const int g = threadIdx.x * CIDER_MAXL + p;
+        for (int p = 0; p < MAXL; ++p) {
+            const int g = threadIdx.x * MAXL + p;
             if (valid[g]) s += w[g] * w[g];
         }
         nrm[threadIdx.x] = sqrt(s);
@@ -230,13 +235,14 @@ __device__ void cider_vectorise(const CiderSlot* slots, unsigned long long mask,
 }
 
 // one CTA per hypothesis: hyps 0..S-1 are the samples (image i / n), S..S+B-1 the greedy captions (image i - S)
+template <int MAXL>
 __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __restrict__ slots, unsigned long long mask, double log_ref_len,
                                                           const long long* __restrict__ sampled, int S, const long long* __restrict__ greedy, int B,
                                                           int T, const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L,
                                                           double* __restrict__ scores) {
-    __shared__ int h_tok[CIDER_MAXL], r_tok[CIDER_MAXL];
-    __shared__ double h_w[CIDER_N * CIDER_MAXL], r_w[CIDER_N * CIDER_MAXL], contrib[CIDER_N * CIDER_MAXL];
-    __shared__ unsigned char h_valid[CIDER_N * CIDER_MAXL], r_valid[CIDER_N * CIDER_MAXL];
+    __shared__ int h_tok[MAXL], r_tok[MAXL];
+    __shared__ double h_w[CIDER_N * MAXL], r_w[CIDER_N * MAXL], contrib[CIDER_N * MAXL];
+    __shared__ unsigned char h_valid[CIDER_N * MAXL], r_valid[CIDER_N * MAXL];
     __shared__ double h_nrm[CIDER_N], r_nrm[CIDER_N], acc[CIDER_N];
     __shared__ int h_len, r_len;
     const int hyp = blockIdx.x;
@@ -245,29 +251,29 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
     const long long* src = hyp < S ? sampled + (long)hyp * T : greedy + (long)(hyp - S) * T;
     if (threadIdx.x == 0) {
         int len = 0;
-        for (int i = 0; i < T && i < CIDER_MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
+        for (int i = 0; i < T && i < MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
         h_len = len;
     }
     __syncthreads();
-    cider_vectorise(slots, mask, log_ref_len, h_tok, h_len, h_w, h_valid, h_nrm);
+    cider_vectorise<MAXL>(slots, mask, log_ref_len, h_tok, h_len, h_w, h_valid, h_nrm);
     const int hl = h_len > 1 ? h_len - 1 : 0;               // "length" = number of bigrams
     const int r0 = ref_offsets[img], r1 = ref_offsets[img + 1];
     double total = 0.0;                                       // only thread 0 uses it
     for (int r = r0; r < r1; ++r) {
         if (threadIdx.x == 0) {
             int len = 0;
-            for (int i = 0; i < L && i < CIDER_MAXL; ++i) { const int v = refs[(long)r * L + i]; r_tok[len++] = v; if (v == 0) break; }
+            for (int i = 0; i < L && i < MAXL; ++i) { const int v = refs[(long)r * L + i]; r_tok[len++] = v; if (v == 0) break; }
             r_len = len;
         }
         __syncthreads();
-        cider_vectorise(slots, mask, log_ref_len, r_tok, r_len, r_w, r_valid, r_nrm);
-        for (int g = threadIdx.x; g < CIDER_N * CIDER_MAXL; g += blockDim.x) {
+        cider_vectorise<MAXL>(slots, mask, log_ref_len, r_tok, r_len, r_w, r_valid, r_nrm);
+        for (int g = threadIdx.x; g < CIDER_N * MAXL; g += blockDim.x) {
             double c = 0.0;
             if (h_valid[g]) {
-                const int n = g / CIDER_MAXL + 1, p = g % CIDER_MAXL;
+                const int n = g / MAXL + 1, p = g % MAXL;
                 double wr = 0.0;
                 for (int q = 0; q + n <= r_len; ++q) {
-                    const int gr = (n - 1) * CIDER_MAXL + q;
+                    const int gr = (n - 1) * MAXL + q;
                     if (r_valid[gr] && same_gram(h_tok + p, r_tok + q, n)) { wr = r_w[gr]; break; }
                 }
                 c = fmin(h_w[g], wr) * wr;
@@ -278,7 +284,7 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
         if (threadIdx.x < CIDER_N) {
             const int n = threadIdx.x;
             double v = 0.0;
-            for (int p = 0; p < CIDER_MAXL; ++p) v += contrib[n * CIDER_MAXL + p];
+            for (int p = 0; p < MAXL; ++p) v += contrib[n * MAXL + p];
             if (h_nrm[n] != 0.0 && r_nrm[n] != 0.0) v /= (h_nrm[n] * r_nrm[n]);
             const int rl = r_len > 1 ? r_len - 1 : 0;
             const double delta = (double)(hl - rl);
@@ -296,15 +302,17 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
 //   guess[k] = max(0, len_h - k);  correct[k] = sum over the hypothesis' distinct (k+1)-grams of min(count in h, max count in one reference)
 //   bleu = (prod_k (correct[k] + 1e-15) / (guess[k] + 1e-9)) ** (1/4), times exp(1 - 1/ratio) when ratio = (len_h + 1e-15) / (reflen + 1e-9) < 1,
 //   reflen = the reference length closest to len_h, the shorter one on a tie.  Lengths count words, the closing 0 included.
-// One CTA per hypothesis, laid out as cider_score_kernel; thread g owns the n-gram of order g / 64 + 1 starting at position g % 64.  The image's
+// One CTA per hypothesis, laid out as cider_score_kernel; thread g owns the n-gram of order g / MAXL + 1 starting at position g % MAXL (4 x 256 =
+// 1024 threads in the long form: the CTA limit sets CAPB200_MAX_SEQ_LENGTH).  The image's
 // references are staged in shared memory BLEU_REF_CHUNK at a time.  An image without references scores 0 (the Python layer refuses it).
 constexpr int BLEU_REF_CHUNK = 32;
 
-__global__ void __launch_bounds__(CIDER_N * CIDER_MAXL) bleu_score_kernel(const long long* __restrict__ sampled, int S, const long long* __restrict__ greedy,
+template <int MAXL>
+__global__ void __launch_bounds__(CIDER_N * MAXL) bleu_score_kernel(const long long* __restrict__ sampled, int S, const long long* __restrict__ greedy,
                                                                           int B, int T, const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L,
                                                                           double* __restrict__ scores) {
-    __shared__ int h_tok[CIDER_MAXL];
-    __shared__ int r_tok[BLEU_REF_CHUNK][CIDER_MAXL];
+    __shared__ int h_tok[MAXL];
+    __shared__ int r_tok[BLEU_REF_CHUNK][MAXL];
     __shared__ int r_len[BLEU_REF_CHUNK];
     __shared__ int correct[CIDER_N];
     __shared__ int h_len;
@@ -314,13 +322,13 @@ __global__ void __launch_bounds__(CIDER_N * CIDER_MAXL) bleu_score_kernel(const 
     const long long* src = hyp < S ? sampled + (long)hyp * T : greedy + (long)(hyp - S) * T;
     if (threadIdx.x == 0) {
         int len = 0;
-        for (int i = 0; i < T && i < CIDER_MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
+        for (int i = 0; i < T && i < MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
         h_len = len;
     }
     if (threadIdx.x < CIDER_N) correct[threadIdx.x] = 0;
     __syncthreads();
     const int hl = h_len;
-    const int n = threadIdx.x / CIDER_MAXL + 1, p = threadIdx.x % CIDER_MAXL;
+    const int n = threadIdx.x / MAXL + 1, p = threadIdx.x % MAXL;
     // counted by its first occurrence only: tf = how often the n-gram occurs in the hypothesis
     bool first = p + n <= hl;
     int tf = 0;
@@ -333,12 +341,12 @@ __global__ void __launch_bounds__(CIDER_N * CIDER_MAXL) bleu_score_kernel(const 
     int max_ref = 0;                                    // the n-gram's largest count in a single reference
     int best_len = -1, best_diff = 0;                   // closest reference length (thread 0)
     const int r0 = ref_offsets[img], r1 = ref_offsets[img + 1];
-    const int cols = L < CIDER_MAXL ? L : CIDER_MAXL;
+    const int cols = L < MAXL ? L : MAXL;
     for (int c0 = r0; c0 < r1; c0 += BLEU_REF_CHUNK) {
         const int cnt = r1 - c0 < BLEU_REF_CHUNK ? r1 - c0 : BLEU_REF_CHUNK;
         __syncthreads();                                // the previous chunk has been read
-        for (int i = threadIdx.x; i < cnt * CIDER_MAXL; i += blockDim.x) {
-            const int r = i / CIDER_MAXL, j = i % CIDER_MAXL;
+        for (int i = threadIdx.x; i < cnt * MAXL; i += blockDim.x) {
+            const int r = i / MAXL, j = i % MAXL;
             r_tok[r][j] = j < cols ? refs[(long)(c0 + r) * L + j] : 0;
         }
         __syncthreads();
@@ -466,8 +474,19 @@ int baseline_reward_launch(const double* scores, int S, const long long* greedy,
 
 int check_reward_shapes(int S, int B, int T, int L) {
     CAPB_REQUIRE(B > 0 && S % B == 0, "sample rows must be a multiple of the image count");
-    CAPB_REQUIRE(T <= CIDER_MAXL && L <= CIDER_MAXL, "caption length above 64 tokens");
+    CAPB_REQUIRE(T <= CIDER_MAXL_LONG && L <= CIDER_MAXL_LONG, "caption or reference length above 256 tokens (CAPB200_MAX_SEQ_LENGTH)");
     return 0;
+}
+
+// the short kernels up to 64 tokens (hypotheses and references), the long ones past it
+bool long_form(int T, int L) { return T > CIDER_MAXL || L > CIDER_MAXL; }
+
+void cider_score_launch(const CiderTable* t, double log_ref_len, const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs,
+                        const int* ref_offsets, int L, double* scores, int hyps, cudaStream_t stream) {
+    if (long_form(T, L))
+        cider_score_kernel<CIDER_MAXL_LONG><<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    else
+        cider_score_kernel<CIDER_MAXL><<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
 }
 
 }  // namespace
@@ -481,7 +500,7 @@ int cider_reward_launch(const CiderTable* t, const long long* sampled, int S, co
     if (hyps == 0) return 0;
     double log_ref_len = 0.0;
     if (corpus_build_launch(t, B, hyps, hyps / B, refs, ref_offsets, L, &log_ref_len, stream)) return 1;
-    cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    cider_score_launch(t, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores, hyps, stream);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return baseline_reward_launch(scores, S, greedy, B, reward, ld_reward, reward_cols, stream);
 }
@@ -491,7 +510,10 @@ int bleu_scores_launch(const long long* sampled, int S, const long long* greedy,
     if (check_reward_shapes(S, B, T, L)) return 1;
     const int hyps = greedy != nullptr ? S + B : S;
     if (hyps == 0) return 0;
-    bleu_score_kernel<<<hyps, CIDER_N * CIDER_MAXL, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    if (long_form(T, L))
+        bleu_score_kernel<CIDER_MAXL_LONG><<<hyps, CIDER_N * CIDER_MAXL_LONG, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    else
+        bleu_score_kernel<CIDER_MAXL><<<hyps, CIDER_N * CIDER_MAXL, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -514,7 +536,7 @@ int weighted_reward_launch(const CiderTable* t, double w_cider, double w_bleu, c
     if (w_cider > 0.0) {
         double log_ref_len = 0.0;
         if (corpus_build_launch(t, B, hyps, hyps / B, refs, ref_offsets, L, &log_ref_len, stream)) return 1;
-        cider_score_kernel<<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+        cider_score_launch(t, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores, hyps, stream);
         CAPB_CHECK_CUDA(cudaGetLastError());
     }
     if (w_bleu > 0.0 && bleu_scores_launch(sampled, S, greedy, B, T, refs, ref_offsets, L, bleu, stream)) return 1;

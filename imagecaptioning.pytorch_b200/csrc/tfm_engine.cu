@@ -259,7 +259,7 @@ capb200_tfm_engine* capb200_tfm_create(const capb200_tfm_cfg* c) {
     if (c->n_enc < 0 || c->n_enc > CAPB200_TFM_MAX_LAYERS || c->n_dec < 1 || c->n_dec > CAPB200_TFM_MAX_LAYERS) { set_error("layer count must be within 1..8"); return nullptr; }
     if (c->heads < 1 || c->d_model % c->heads != 0) { set_error("d_model must be divisible by the head count"); return nullptr; }
     if (c->numeric_mode < 0 || c->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
-    if (c->seq_length < 1 || c->seq_length > 31) { set_error("seq_length must be in 1..31 on the transformer path"); return nullptr; }
+    if (c->seq_length < 1 || c->seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device: the capb200 engine has no CPU fallback"); return nullptr; }
     capb200_tfm_engine* e = new capb200_tfm_engine();
@@ -371,7 +371,7 @@ int capb200_tfm_decode_sample(capb200_tfm_engine* e, const float* att, const flo
     const int rows = B * n;
     const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : e->T;
     const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : e->T;
-    CAPB_REQUIRE(steps >= 0 && steps <= t_out && steps <= e->T + 1 && steps <= 31, "steps out of range");
+    CAPB_REQUIRE(steps >= 0 && steps <= t_out && steps <= e->T + 1, "steps out of range");
     if (ensure_workspace(e, B, rows, R, 1, st)) return 1;
     if (prepare(e, att, mask, B, R, st)) return 1;
     const long long* labels = (method == CAPB200_SAMPLE_TEACHER) ? tokens_in : nullptr;
@@ -462,7 +462,7 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
     const unsigned long long seed = ta.seed;
     const capb200_tfm_weights& w = e->w;
     const float emb_scale = sqrtf((float)D);
-    CAPB_REQUIRE(T >= 1 && T <= e->T + 1 && T < 32, "positions out of range");
+    CAPB_REQUIRE(T >= 1 && T <= e->T + 1, "positions out of range");
     TTape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](TTape& tt, Arena& a) {
             layout_ttape(tt, a, B, R, N, T, D, Dff, heads, V1, NE, ND, ta.xe ? 1 : (long)B * e->T * V1);

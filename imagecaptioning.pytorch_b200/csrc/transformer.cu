@@ -8,6 +8,7 @@
 //                       K/V of earlier positions never change, so they are cached per (layer, step, row) and a row reads its
 //                       ancestors' entries through the beam history (no cache reordering by parent beam)
 //   cross_attention     src_attn over the image's encoder memory; K/V are per IMAGE, rows index them by row / rows_per_image
+#include "../../include/capb200.h"
 #include "common.cuh"
 #include "kernels.cuh"
 #include "attn.cuh"
@@ -138,7 +139,7 @@ __global__ void __launch_bounds__(128) dec_self_attention_kernel(int rows, int h
         kcache[(long)t * step_stride + (long)row * ld_c + head * dk + c] = kr[c];
         vcache[(long)t * step_stride + (long)row * ld_c + head * dk + c] = vr[c];
     }
-    // scores over positions 0..t (lane s handles position s; t < 32 is guaranteed by seq_length <= 31 on this path)
+    // scores over positions 0..t (lane s handles position s; dec_self_attention_launch runs this kernel only for t < 32)
     float sc = -INFINITY;
     if (lane <= t) {
         const float* ks;
@@ -156,10 +157,14 @@ __global__ void __launch_bounds__(128) dec_self_attention_kernel(int rows, int h
     const float mx = warp_max(sc);
     const float e = (lane <= t && sc > -INFINITY) ? expf(sc - mx) : 0.f;
     const float inv = 1.0f / warp_sum(e);
-    for (int c = lane; c < dk; c += 32) {
+    // every lane runs every round, so the shuffles always see the whole warp: with a head narrower than 32 columns the lanes without a
+    // column used to leave the loop, and the weights of positions >= the head width were read from exited lanes (undefined values)
+    for (int c0 = 0; c0 < dk; c0 += 32) {
+        const int c = c0 + lane;
         float acc = 0.f;
         for (int s = 0; s <= t; ++s) {
             const float w = __shfl_sync(0xffffffffu, e, s);
+            if (c >= dk) continue;
             const float* vs;
             if (s == t) vs = vr;
             else {
@@ -168,7 +173,68 @@ __global__ void __launch_bounds__(128) dec_self_attention_kernel(int rows, int h
             }
             acc = fmaf(w, vs[c], acc);
         }
-        store_act2(out, row, head * dk + c, acc * inv);
+        if (c < dk) store_act2(out, row, head * dk + c, acc * inv);
+    }
+}
+
+// The same attention at any step t (the positions past 31 that one lane per key cannot hold): one warp per (row, head) walks the positions
+// 0..t in chunks of 32, one key per lane, with a running max and sum (online softmax).  Lane i owns output columns i, i + 32, ... (NC of them).
+template <int NC>
+__global__ void __launch_bounds__(128) dec_self_attention_long_kernel(int rows, int heads, int dk, int t, const float* __restrict__ qkv, long ld_qkv,
+                                                                      float* __restrict__ kcache, float* __restrict__ vcache, long step_stride, long ld_c,
+                                                                      const int* __restrict__ anc, long ld_anc, const long long* __restrict__ labels,
+                                                                      long ld_lab, float scale, ActView out) {
+    const int item = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (item >= rows * heads) return;
+    const int lane = threadIdx.x & 31;
+    const int row = item / heads, head = item % heads;
+    const int D = heads * dk;
+    const float* qr = qkv + (long)row * ld_qkv + head * dk;
+    const float* kr = qr + D;
+    const float* vr = qr + 2 * D;
+    for (int c = lane; c < dk; c += 32) {
+        kcache[(long)t * step_stride + (long)row * ld_c + head * dk + c] = kr[c];
+        vcache[(long)t * step_stride + (long)row * ld_c + head * dk + c] = vr[c];
+    }
+    float m = -INFINITY, l = 0.f, acc[NC];
+#pragma unroll
+    for (int i = 0; i < NC; ++i) acc[i] = 0.f;
+    for (int s0 = 0; s0 <= t; s0 += 32) {
+        const int s = s0 + lane;
+        const int ar = (s < t && anc != nullptr) ? anc[(long)row * ld_anc + s] : row;      // ancestor row holding position s
+        float sc = -INFINITY;
+        if (s <= t) {
+            const float* ks = (s == t) ? kr : kcache + (long)s * step_stride + (long)ar * ld_c + head * dk;
+            float d = 0.f;
+            for (int c = 0; c < dk; ++c) d = fmaf(qr[c], ks[c], d);
+            sc = d * scale;
+            if (labels != nullptr && s > 0 && labels[(long)row * ld_lab + s] == 0) sc = -INFINITY;   // TransformerModel.py:324-328
+        }
+        const float m_new = fmaxf(m, warp_max(sc));
+        if (m_new == -INFINITY) continue;                       // every position so far masked
+        const float corr = expf(m - m_new);
+        const float e = (sc > -INFINITY) ? expf(sc - m_new) : 0.f;
+        l = l * corr + warp_sum(e);
+        m = m_new;
+#pragma unroll
+        for (int i = 0; i < NC; ++i) acc[i] *= corr;
+        const int n = (t + 1 - s0) < 32 ? (t + 1 - s0) : 32;
+        for (int j = 0; j < n; ++j) {
+            const float w = __shfl_sync(0xffffffffu, e, j);
+            const int aj = __shfl_sync(0xffffffffu, ar, j);
+            const float* vs = (s0 + j == t) ? vr : vcache + (long)(s0 + j) * step_stride + (long)aj * ld_c + head * dk;
+#pragma unroll
+            for (int i = 0; i < NC; ++i) {
+                const int c = lane + 32 * i;
+                if (c < dk) acc[i] = fmaf(w, vs[c], acc[i]);
+            }
+        }
+    }
+    const float inv = 1.0f / l;
+#pragma unroll
+    for (int i = 0; i < NC; ++i) {
+        const int c = lane + 32 * i;
+        if (c < dk) store_act2(out, row, head * dk + c, acc[i] * inv);
     }
 }
 
@@ -269,11 +335,27 @@ int enc_self_attention_launch(int B, int R, int heads, int dk, const float* q, c
 }
 
 int dec_self_attention_launch(int rows, int heads, int dk, int t, const float* qkv, long ld_qkv, float* kcache, float* vcache, long step_stride,
-                              long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, ActView out, cudaStream_t st) {
+                              long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, ActView out, cudaStream_t st, int form) {
     if (rows <= 0) return 0;
-    CAPB_REQUIRE(t < 32, "decoder self-attention handles up to 32 positions");
-    dec_self_attention_kernel<<<cdiv(rows * heads, 4), 128, 0, st>>>(rows, heads, dk, t, qkv, ld_qkv, kcache, vcache, step_stride, ld_c, anc, ld_anc,
-                                                                      labels, ld_lab, 1.0f / sqrtf((float)dk), out);
+    CAPB_REQUIRE(t >= 0 && t <= CAPB200_MAX_SEQ_LENGTH, "decoder self-attention: position out of range (teacher forcing reaches seq_length)");
+    const float scale = 1.0f / sqrtf((float)dk);
+    if (form == 1 || (form == 0 && t < 32)) {
+        CAPB_REQUIRE(t < 32, "decoder self-attention (one lane per position): handles up to 32 positions");
+        dec_self_attention_kernel<<<cdiv(rows * heads, 4), 128, 0, st>>>(rows, heads, dk, t, qkv, ld_qkv, kcache, vcache, step_stride, ld_c, anc, ld_anc,
+                                                                          labels, ld_lab, scale, out);
+        CAPB_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
+    CAPB_REQUIRE(dk >= 1 && dk <= 256, "decoder self-attention: head width above 256");
+    const int nc = dk <= 32 ? 1 : dk <= 64 ? 2 : dk <= 128 ? 4 : 8;
+    const dim3 grid(cdiv(rows * heads, 4));
+#define CAPB_DEC_LONG(N) dec_self_attention_long_kernel<N><<<grid, 128, 0, st>>>(rows, heads, dk, t, qkv, ld_qkv, kcache, vcache, step_stride, ld_c, anc, \
+                                                                                 ld_anc, labels, ld_lab, scale, out)
+    if (nc == 1) CAPB_DEC_LONG(1);
+    else if (nc == 2) CAPB_DEC_LONG(2);
+    else if (nc == 4) CAPB_DEC_LONG(4);
+    else CAPB_DEC_LONG(8);
+#undef CAPB_DEC_LONG
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -290,3 +372,14 @@ int cross_attention_launch(int rows, int rpi, int heads, int dk, int R, const fl
 }
 
 }  // namespace capb200
+
+extern "C" int capb200_tfm_dec_self_attention(int form, int rows, int heads, int dk, int t, const float* qkv, long ld_qkv, float* kcache, float* vcache,
+                                              long step_stride, long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, float* out,
+                                              long ld_out, void* stream) {
+    CAPB_REQUIRE(form >= 0 && form <= 2, "form is 0 (automatic), 1 (one lane per position) or 2 (chunked)");
+    CAPB_REQUIRE(rows > 0 && heads > 0 && dk > 0 && qkv && kcache && vcache && out, "bad argument");
+    capb200::ActView o;
+    o.f = out; o.ld = ld_out;
+    return capb200::dec_self_attention_launch(rows, heads, dk, t, qkv, ld_qkv, kcache, vcache, step_stride, ld_c, anc, ld_anc, labels, ld_lab, o,
+                                              static_cast<cudaStream_t>(stream), form);
+}

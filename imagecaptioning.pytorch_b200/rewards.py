@@ -350,7 +350,8 @@ def _self_cider_table(table: Optional[CiderDTable]) -> CiderDTable:
 
 
 def check_caption_sets(rows: int, n: int, T: int) -> int:
-    """Number of images of ``rows`` captions in sets of ``n``; raises ValueError for the shapes the diversity kernels refuse."""
+    """Number of images of ``rows`` captions in sets of ``n``; raises ValueError for the shapes the diversity kernels refuse.  Those keep
+    captions of at most 64 tokens, while the CIDEr-D / BLEU-4 rewards take up to 256 (CAPB200_MAX_SEQ_LENGTH)."""
     if n < 2:
         raise ValueError('diversity needs at least 2 captions per image (log(n) = 0 below that), got %d' % n)
     if n > 32:

@@ -32,6 +32,13 @@ extern "C" {
 #define CAPB200_MODE_TF32X3_TC_DGRAD 6 /* same kernel, input-gradient form: y[M,N] = x[M,K] * w[K,N]  (w row-major [K,N], transposed internally) */
 #define CAPB200_MODE_TF32X3_TC_WGRAD 7 /* same kernel, weight-gradient form: y[M,N] = x[K,M]^T * w[K,N] (both row-major, transposed internally) */
 
+/* Longest caption every family decodes and trains (seq_length), and the widest hypothesis / reference row the CIDEr-D and BLEU-4
+ * rewards score (T and L of the reward entry points, including the closing 0).  256 is what the long BLEU-4 kernel holds: one thread per
+ * n-gram (4 orders x 256 positions = 1024 threads, the CTA limit).  Up to 64 tokens the rewards run their original kernels, and up to 31
+ * positions the Transformer runs its original decoder self-attention; longer shapes dispatch to the long forms (DESIGN.md, "Caption
+ * length").  The diversity entry points (capb200_self_cider, capb200_div_stats) stay at 64 tokens. */
+#define CAPB200_MAX_SEQ_LENGTH 256
+
 #define CAPB200_FAMILY_UPDOWN 0 /* UpDownModel  captioning/models/AttModel.py:868 */
 #define CAPB200_FAMILY_NEWFC 1  /* NewFCModel   captioning/models/AttModel.py:904 */
 #define CAPB200_FAMILY_ATT2IN2 2 /* Att2in2Model captioning/models/AttModel.py:854 (no fc_embed; the core attends with the previous h) */
@@ -111,7 +118,7 @@ typedef struct {
     int att_hid_size;        /* A */
     int fc_feat_size;        /* F_fc */
     int att_feat_size;       /* F_att */
-    int seq_length;          /* T = max_length (AttModel.py:60) */
+    int seq_length;          /* T = max_length (AttModel.py:60), 1..CAPB200_MAX_SEQ_LENGTH */
     int numeric_mode;        /* CAPB200_MODE_* */
 } capb200_model_cfg;
 
@@ -225,7 +232,7 @@ int capb200_engine_read_profile(capb200_engine* e, int reset, double* ms, double
 #define CAPB200_TFM_MAX_LAYERS 8
 typedef struct capb200_tfm_engine capb200_tfm_engine;
 typedef struct {
-    int vocab_size, d_model, d_ff, heads, n_enc, n_dec, att_feat_size, seq_length, numeric_mode;
+    int vocab_size, d_model, d_ff, heads, n_enc, n_dec, att_feat_size, seq_length, numeric_mode;   /* seq_length 1..CAPB200_MAX_SEQ_LENGTH */
 } capb200_tfm_cfg;
 typedef struct { const float *q_w, *q_b, *k_w, *k_b, *v_w, *v_b, *o_w, *o_b; } capb200_mha_weights;          /* linears.0..3 */
 typedef struct {
@@ -266,7 +273,7 @@ long capb200_tfm_launch_count(const capb200_tfm_engine* e);
 #define CAPB200_AOA_REFINER_LAYERS 6
 typedef struct capb200_aoa_engine capb200_aoa_engine;
 typedef struct {
-    int vocab_size, input_encoding_size, rnn_size, heads, att_feat_size, seq_length, numeric_mode;
+    int vocab_size, input_encoding_size, rnn_size, heads, att_feat_size, seq_length, numeric_mode;   /* seq_length 1..CAPB200_MAX_SEQ_LENGTH */
 } capb200_aoa_cfg;
 typedef struct {
     const float *q_w, *q_b, *k_w, *k_b, *v_w, *v_b;   /* refiner.layers.i.self_attn.linears.{0,1,2} [H,H] */
@@ -350,6 +357,7 @@ int capb200_cider_table_is_corpus(const capb200_cider_table* t);
 
 /* get_self_critical_reward (captioning/utils/rewards.py:41-81) with CIDEr-D only:
  * sampled[S,T], greedy[B,T] int64 device; refs[n_refs_total,L] int32 device (0 padded), ref_offsets[B+1] int32 device;
+ * T and L up to CAPB200_MAX_SEQ_LENGTH (every reward entry point below takes the same bound; a caption ends at its first 0);
  * scores[S+B] float64 device (CIDEr-D of every hypothesis); reward[S,T] fp32 = score(sample) - score(greedy of its image). */
 int capb200_self_critical_reward(const capb200_cider_table* t, const long long* sampled, int S, const long long* greedy, int B, int T,
                                  const int* refs, const int* ref_offsets, int L, double* scores, float* reward, void* stream);
@@ -642,6 +650,26 @@ int capb200_mha_self_backward(int form, int B, int R, int heads, int dk, const f
 int capb200_mha_cross_backward(int form, int B, int rpi, int n_steps, int heads, int dk, int R, const float* q, long ld_q, const float* kk, const float* vv,
                                long ld_kv, unsigned long long seed, int site, int step, float p, const float* probs, const float* d_out, long ld_do, float* dq,
                                long ld_dq, float* dkk, float* dvv, long ld_dkv, void* stream);
+
+/* The Transformer decoder's causal self-attention in training, for tests: B sequences of T positions, rows image-major [B*T, ld]; key r is
+ * visible to query i iff r <= i and key_mask[b, r] != 0 (key_mask [B, ld_mask] or NULL).  Dropout element ((b*heads + h)*T + i)*T + r at
+ * step 0 of `site`.  `form` as for capb200_mha_forward; the key-tiled form skips the key tiles past each query tile.
+ *   capb200_mha_causal_forward   out rows of the queries [q_lo, q_hi) (every key up to the query is read)
+ *   capb200_mha_causal_backward  dq, dkey, dval of capb200_mha_causal_forward over all T queries (dq must not alias an input) */
+int capb200_mha_causal_forward(int form, int B, int T, int q_lo, int q_hi, int heads, int dk, const float* q, const float* k, const float* v, long ld,
+                               const float* key_mask, long ld_mask, unsigned long long seed, int site, float p, float* out, long ld_out, void* stream);
+int capb200_mha_causal_backward(int form, int B, int T, int heads, int dk, const float* q, const float* k, const float* v, long ld, const float* key_mask,
+                                long ld_mask, unsigned long long seed, int site, float p, const float* d_out, long ld_do, float* dq, float* dkey, float* dval,
+                                long ld_d, void* stream);
+
+/* The Transformer's decoder self-attention at step t, for tests.  qkv [rows, ld_qkv] holds this step's q | k | v (D = heads*dk columns
+ * each); kcache / vcache [t+1][step_stride] hold the keys / values of positions < t at row * ld_c (+ head*dk) and receive this step's k, v;
+ * anc [rows, ld_anc] the row whose cache entry position s < t reads (beam search), or NULL for the row itself; labels [rows, ld_lab] int64
+ * or NULL: teacher forcing masks positions s > 0 whose label is 0.  out [rows, ld_out].  form 0 picks the kernel as the decoder does (one
+ * lane per position for t < 32, the chunked online softmax beyond), 1 forces the first (t < 32 only), 2 the second (head width <= 256). */
+int capb200_tfm_dec_self_attention(int form, int rows, int heads, int dk, int t, const float* qkv, long ld_qkv, float* kcache, float* vcache,
+                                   long step_stride, long ld_c, const int* anc, long ld_anc, const long long* labels, long ld_lab, float* out, long ld_out,
+                                   void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Training steps of the Transformer captioner (TransformerModel.py:262-363 under LossWrapper, loss_wrapper.py:25-73, + loss.backward()).
