@@ -218,6 +218,8 @@ SIGNATURES = {
     'capb200_engine_bind_weights': (c_int, [c_void_p, POINTER(Weights), c_void_p]),
     'capb200_decode_beam': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
+    'capb200_decode_beam_form': (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_void_p, c_void_p, c_void_p]),
     'capb200_beam_record_logprobs': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     'capb200_decode_beam_diverse': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(DiverseOpts), c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p, c_void_p]),

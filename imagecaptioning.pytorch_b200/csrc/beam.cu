@@ -13,6 +13,7 @@
 #include "../../include/capb200.h"
 #include "common.cuh"
 #include "kernels.cuh"
+#include "vocab_row.cuh"
 
 namespace capb200 {
 
@@ -27,29 +28,31 @@ __device__ __forceinline__ double apply_penalty(int kind, float alpha, int lengt
 }
 
 // One step of the search for one image (or one group of an image in diverse beam search), run by one warp.  `img` indexes the sums /
-// sequence tables / records (s.beam beams each); the `live` parent rows of this step are top-list rows row0 .. row0 + live - 1 with `kl`
-// candidates each.  The n_pen words at `pen` (shared memory) lower a candidate by lambda per occurrence (add_diversity,
+// sequence tables / records (s.beam beams each); the `live` parent rows of this step are rows row0 .. row0 + live - 1, whose `kl`
+// candidates each are top_val / top_idx[(row - row0) * kl + k] (global memory, or shared memory in beam_search_step_kernel).  The n_pen
+// words at `pen` (shared memory) lower a candidate by lambda per occurrence (add_diversity,
 // CaptionModel.py:38-55).  Chosen words go to s.tokens / s.src_row[img * beam + j] with parent row row0 + parent; the log-prob slab row
-// of a record is hist0 + parent.
-__device__ __forceinline__ void select_step(const BeamState& s, int img, int t, int live, int kl, int row0, int hist0, const float* __restrict__ top_val,
-                                            const int* __restrict__ top_idx, const int* pen, int n_pen, float lambda, int penalty_kind,
+// of a record is hist0 + parent.  Each lane holds U candidates (lane, lane + 32, ...): live * kl <= 32 * U.  Slots past the candidates
+// never win, so U does not change the result.
+template <int U = 8>
+__device__ __forceinline__ void select_step(const BeamState& s, int img, int t, int live, int kl, int row0, int hist0, const float* top_val,
+                                            const int* top_idx, const int* pen, int n_pen, float lambda, int penalty_kind,
                                             float penalty_alpha, double* __restrict__ done_p) {
     const int lane = threadIdx.x;
     const int b = s.beam, T = s.T;
     const int ncand = live * kl;
-    // each lane owns candidates lane, lane+32, ... (ncand <= 256)
-    float cv[8];
-    int cf[8];
+    // each lane owns candidates lane, lane+32, ... (ncand <= 32 * U)
+    float cv[U];
+    int cf[U];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) {
+    for (int u = 0; u < U; ++u) {
         const int c = lane + 32 * u;
         cv[u] = -INFINITY;
         cf[u] = 0x7fffffff;
         if (c < ncand) {
             const int pb = c / kl, k = c % kl;
-            const long row = (long)row0 + pb;
-            const int w = top_idx[row * kl + k];
-            float v = top_val[row * kl + k];
+            const int w = top_idx[pb * kl + k];
+            float v = top_val[pb * kl + k];
             int cnt = 0;
             for (int q = 0; q < n_pen; ++q) cnt += (pen[q] == w);
             if (cnt) v = __fsub_rn(v, __fmul_rn((float)cnt, lambda));     // logprobs - change * diversity_lambda
@@ -57,6 +60,7 @@ __device__ __forceinline__ void select_step(const BeamState& s, int img, int t, 
             cf[u] = pb * s.V1 + w;                                           // flat index into the [live*(V+1)] candidate list
         }
     }
+
     const int* seq_old = (t & 1) ? s.seq_b : s.seq_a;
     int* seq_new = (t & 1) ? s.seq_a : s.seq_b;
     const int* hist_old = (t & 1) ? s.hist_b : s.hist_a;
@@ -70,7 +74,7 @@ __device__ __forceinline__ void select_step(const BeamState& s, int img, int t, 
         float bv = -INFINITY;
         int bf = 0x7fffffff, bu = -1;
 #pragma unroll
-        for (int u = 0; u < 8; ++u)
+        for (int u = 0; u < U; ++u)
             if (cv[u] > bv || (cv[u] == bv && cf[u] < bf)) { bv = cv[u]; bf = cf[u]; bu = u; }
         float wv = bv;
         int wf = bf;
@@ -82,7 +86,7 @@ __device__ __forceinline__ void select_step(const BeamState& s, int img, int t, 
         }
         if (bu >= 0 && bf == wf && bv == wv) {       // the owning lane retires the winner
 #pragma unroll
-            for (int u = 0; u < 8; ++u) if (u == bu) { cv[u] = -INFINITY; cf[u] = 0x7fffffff; }
+            for (int u = 0; u < U; ++u) if (u == bu) { cv[u] = -INFINITY; cf[u] = 0x7fffffff; }
         }
         if (lane == j) { my_v = wv; my_f = wf; }
     }
@@ -97,6 +101,7 @@ __device__ __forceinline__ void select_step(const BeamState& s, int img, int t, 
     const int slot = cnt0 + __popc(em & ((1u << lane) - 1u));          // records are appended in winner order
     if (has) { sh_parent[lane] = parent; sh_word[lane] = word; sh_slot[lane] = ended ? slot : -1; }
     __syncwarp();
+#pragma unroll 1      // not unrolled: the 48-register beam_search_step_kernel holds this loop without spills
     for (int idx = lane; idx < b * t; idx += 32) {
         const int j = idx / t, q = idx - j * t;
         const long dst = ((long)img * b + j) * T, src = ((long)img * b + sh_parent[j]) * T;
@@ -104,6 +109,7 @@ __device__ __forceinline__ void select_step(const BeamState& s, int img, int t, 
         hist_new[dst + q] = hist_old[src + q];
     }
     if (em != 0u) {
+#pragma unroll 1
         for (int idx = lane; idx < b * (t + 1); idx += 32) {
             const int j = idx / (t + 1), q = idx - j * (t + 1);
             if (sh_slot[j] < 0) continue;
@@ -136,7 +142,40 @@ __global__ void __launch_bounds__(32) beam_step_kernel(BeamState s, int t, int l
                                                        const int* __restrict__ top_idx, int penalty_kind, float penalty_alpha,
                                                        double* __restrict__ done_p) {
     const int img = blockIdx.x;
-    select_step(s, img, t, live, s.beam, img * live, img * live, top_val, top_idx, nullptr, 0, 0.f, penalty_kind, penalty_alpha, done_p);
+    const long row0 = (long)img * live;
+    select_step(s, img, t, live, s.beam, (int)row0, (int)row0, top_val + row0 * s.beam, top_idx + row0 * s.beam, nullptr, 0, 0.f, penalty_kind,
+                penalty_alpha, done_p);
+}
+
+// One CTA per image: vocab_stats_online128_kernel over the image's `live` rows, beam_step_kernel, and (t < T - 1) the parent-state gather
+// of state_gather_embed_kernel for the next step, in one launch.  Rows are image-major and a row's parent is a row of the same image, so
+// nothing crosses CTAs.  min(live, 8) groups of 128 threads; group g takes rows g, g + 8, ... and runs exactly the per-row work of
+// vocab_stats_online128_kernel (same partition and reduction order, named barrier 1 + g for its reductions), so the row statistics and
+// the top lists are bitwise those of the separate kernels; the top lists stay in shared memory.  U = 2 (beam <= 8, at most 64 candidates)
+// fits 48 registers: two CTAs of 640 threads (beam 5) per SM, so the 256 images of the headline shape are resident in one wave on 132 SMs.
+// U = 8 (beam 9..16) runs 1024 threads, one CTA per SM, and gets 64.
+constexpr int kStepGroups = 8;
+template <int U>
+__global__ void __maxnreg__(U <= 2 ? 48 : 64) beam_search_step_kernel(BeamState s, const VocabStepArgs a, int t, int live, int penalty_kind, float penalty_alpha,
+                                                        double* __restrict__ done_p, NextStateGather next) {
+    __shared__ float s_red[kStepGroups][VT2 / 32];
+    __shared__ int s_ridx[kStepGroups][VT2 / 32];
+    __shared__ float s_val[MAXB * MAXB];
+    __shared__ int s_idx[MAXB * MAXB];
+    const int img = blockIdx.x, g = threadIdx.x / VT2, ng = blockDim.x / VT2;
+    const int b = s.beam, row0 = img * live;
+    for (int j = g; j < live; j += ng)
+        stats_online128_row(a, row0 + j, threadIdx.x % VT2, GroupBarrier{1 + g}, s_red[g], s_ridx[g], s_val + j * b, s_idx + j * b);
+    __syncthreads();
+    if (threadIdx.x < 32) select_step<U>(s, img, t, live, b, row0, row0, s_val, s_idx, nullptr, 0, 0.f, penalty_kind, penalty_alpha, done_p);
+    if (t == s.T - 1) return;
+    __syncthreads();                 // s.src_row of this image is written
+    const int n4 = next.H >> 2;
+    for (int i = threadIdx.x; i < b * n4; i += blockDim.x) {
+        const int j = i / n4, c4 = i - j * n4;
+        const long r = (long)img * b + j;
+        copy_states4(r, s.src_row[r], c4, 2, next.s0, next.s1);
+    }
 }
 
 // one warp per real image; its groups step in order, each seeing the words the earlier groups chose at this global step
@@ -160,8 +199,8 @@ __global__ void __launch_bounds__(32) diverse_beam_step_kernel(BeamState s, int 
         __syncwarp();
         const int vimg = i * G + g;
         // the group's first step reads the one bos row of the group (its row j = 0), like the B-row first step of beam_step
-        select_step(s, vimg, lt, lt == 0 ? 1 : b, k, vimg * b, g * rows_total + vimg * b, top_val, top_idx, sh_pen, n_pen, lambda, penalty_kind,
-                    penalty_alpha, done_p);
+        select_step(s, vimg, lt, lt == 0 ? 1 : b, k, vimg * b, g * rows_total + vimg * b, top_val + (long)vimg * b * k, top_idx + (long)vimg * b * k,
+                    sh_pen, n_pen, lambda, penalty_kind, penalty_alpha, done_p);
     }
 }
 
@@ -349,6 +388,29 @@ int beam_step_launch(const BeamState& s, int t, int live, const float* top_val, 
     CAPB_REQUIRE(s.beam >= 1 && s.beam <= MAXB, "beam size 1..16");
     CAPB_REQUIRE(s.beam * s.T <= MAXB * CAPB200_MAX_SEQ_LENGTH, "beam*T record capacity (16 x CAPB200_MAX_SEQ_LENGTH)");
     beam_step_kernel<<<s.B, 32, 0, stream>>>(s, t, live, top_val, top_idx, penalty_kind, penalty_alpha, s.done_p);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+bool beam_search_step_applies(const VocabStepArgs& a, const NextStateGather& next) {
+    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    auto al8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };
+    auto state_ok = [&](const StateCopy& c) {
+        return c.src != nullptr && c.dst.f != nullptr && (c.ld_src & 3) == 0 && (c.dst.ld & 3) == 0 && al16(c.src) && al16(c.dst.f) &&
+               ((c.dst.hi == nullptr) == (c.dst.lo == nullptr)) && (c.dst.hi == nullptr || (al8(c.dst.hi) && al8(c.dst.lo)));
+    };
+    return (a.V1 & 3) == 0 && (a.ld & 3) == 0 && al16(a.logits) && next.H > 0 && (next.H & 3) == 0 && state_ok(next.s0) && state_ok(next.s1);
+}
+
+int beam_search_step_launch(const BeamState& s, const VocabStepArgs& a, int t, int live, int penalty_kind, float penalty_alpha,
+                            const NextStateGather& next, cudaStream_t stream) {
+    CAPB_REQUIRE(s.beam >= 1 && s.beam <= MAXB, "beam size 1..16");
+    CAPB_REQUIRE(s.beam * s.T <= MAXB * CAPB200_MAX_SEQ_LENGTH, "beam*T record capacity (16 x CAPB200_MAX_SEQ_LENGTH)");
+    CAPB_REQUIRE(a.topk == s.beam && a.stats != nullptr && a.rows == s.B * live && live >= 1 && live <= s.beam, "fused beam step arguments");
+    CAPB_REQUIRE(beam_search_step_applies(a, next), "the fused beam step needs 16-byte aligned logit and state rows (V + 1 and H multiples of 4)");
+    const int threads = min(live, kStepGroups) * VT2;
+    if (s.beam <= 8) beam_search_step_kernel<2><<<s.B, threads, 0, stream>>>(s, a, t, live, penalty_kind, penalty_alpha, s.done_p, next);
+    else beam_search_step_kernel<8><<<s.B, threads, 0, stream>>>(s, a, t, live, penalty_kind, penalty_alpha, s.done_p, next);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

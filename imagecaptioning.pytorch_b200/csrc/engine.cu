@@ -347,8 +347,9 @@ int prepare(capb200_engine* e, const float* fc, const float* att, const float* m
 
 // ---- one application of the recurrent core on `rows` rows (rpi rows per image) -----------------------------------------
 // tokens: input word per row; src_row: parent row per row (nullptr = identity, e->neg1 = fresh zero state)
+// states_gathered (UpDown): h0_in / h1_in already hold the parents' states (the previous step's beam_search_step_kernel wrote them)
 int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld_logits, int n_images, int R,
-              const float* mask, cudaStream_t st) {
+              const float* mask, cudaStream_t st, bool states_gathered = false) {
     const int H = e->H, E = e->E, A = e->A, V1 = e->V1;
     const capb200_weights& w = e->w;
     if (e->cfg.family == CAPB200_FAMILY_UPDOWN) {
@@ -356,8 +357,11 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
         s0.src = e->h0_out.v.f; s0.ld_src = e->h0_out.v.ld; s0.dst = e->h0_in.v;
         s1.src = e->h1_out.v.f; s1.ld_src = e->h1_out.v.ld; s1.dst = e->h1_in.v;
         const bool xg = e->use_xgate;     // word contribution comes from the per-token table instead of a K-segment
-        e->launches++;
-        if (state_gather_embed_launch(rows, tokens, src_row, w.embed, E, xg ? 0 : E, 1, e->xt.v, H, 2, s0, s1, st)) return 1;
+        CAPB_REQUIRE(!states_gathered || xg, "the fused beam step gathers the states only; the word embedding needs the separate gather");
+        if (!states_gathered) {
+            e->launches++;
+            if (state_gather_embed_launch(rows, tokens, src_row, w.embed, E, xg ? 0 : E, 1, e->xt.v, H, 2, s0, s1, st)) return 1;
+        }
         const int cur = e->core_cur, nxt = cur ^ 1;
         {   // attention LSTM gates: [h_lang_prev | (xt) | h_att_prev] segments + per-image fc' term
             GemmProblem g;
@@ -545,7 +549,7 @@ int lstm_decode_prepare(capb200_engine* e, const float* fc, const float* att, co
 
 int lstm_decode_core(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int B, int R,
                      const float* mask, cudaStream_t st) {
-    return core_step(e, rows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
+    return core_step(e, rows, rpi, tokens, src_row, logits, ld, B, R, mask, st, e->d.states_gathered);
 }
 
 }  // namespace capb200
@@ -756,8 +760,8 @@ int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, voi
     return 0;
 }
 
-int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
-                        long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
+static int decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
+                       long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream, int form) {
     if (check_ready(e)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq != nullptr, "null argument");
@@ -775,9 +779,28 @@ int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, co
     auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
         return lstm_decode_core(e, nrows, live, tokens, src_row, logits, ld, B, R, mask, st);
     };
+    // UpDown's two states can be gathered by the fused beam step (the word enters through the per-token gate table, not an embedding copy)
+    NextStateGather next;
+    const bool gather = e->cfg.family == CAPB200_FAMILY_UPDOWN && e->use_xgate;
+    if (gather) {
+        next.s0.src = e->h0_out.v.f; next.s0.ld_src = e->h0_out.v.ld; next.s0.dst = e->h0_in.v;
+        next.s1.src = e->h1_out.v.f; next.s1.ld_src = e->h1_out.v.ld; next.s1.dst = e->h1_in.v;
+        next.H = e->H;
+    }
     return beam_decode_driver(e->d, V1, T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
                               done_raw, core, &e->launches, st, e->profiling ? 0ull : loop_graph_key(e->ws, e->wblock, mask, R, (int)e->cfg.family),
-                              to_edits(opts->edits), opts->temperature);
+                              to_edits(opts->edits), opts->temperature, gather ? &next : nullptr, form);
+}
+
+int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
+                        long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
+    return decode_beam(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream, 0);
+}
+
+int capb200_decode_beam_form(int form, capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R,
+                             const capb200_beam_opts* opts, long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p,
+                             float* done_raw, void* stream) {
+    return decode_beam(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream, form);
 }
 
 int capb200_decode_beam_diverse(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,

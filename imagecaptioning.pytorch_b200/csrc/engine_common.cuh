@@ -126,6 +126,8 @@ struct DecodeBuffers {
     unsigned long long loop_key[8] = {0, 0, 0, 0, 0, 0, 0, 0}, seen_key[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     long loop_launches = 0;
     bool graph_broken = false;
+    // set by beam_decode_driver around a core call whose parent-state gather the previous step's beam_search_step_kernel already did
+    bool states_gathered = false;
 
     void release() {
         if (loop_exec) cudaGraphExecDestroy(loop_exec);
@@ -252,15 +254,22 @@ int run_beam_loop(DecodeBuffers& d, const unsigned long long (&key)[8], bool use
     return 0;
 }
 
+// `next` (optional): the engine's recurrent states, which the core gathers by parent row at the start of every step.  Where it applies
+// (no decode edits, temperature 1, 16-byte aligned logit and state rows), each step's vocabulary statistics / top-k, beam step and the
+// next step's state gather run as one beam_search_step_kernel per image, and from t = 1 on the core is called with d.states_gathered
+// set and skips its own gather: 2T - 1 fewer launches per decode.  `form`: 0 picks that automatically, 1 always runs the separate
+// kernels, 2 requires the fused kernel (an error where it does not apply); 1 and 2 are for tests.
 template <class CoreFn>
 int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int keep, int penalty_kind, float penalty_alpha, long long* seq,
                        float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, CoreFn core, long* launches,
-                       cudaStream_t st, unsigned long long graph_key = 0, const DecodeEdits& ed = DecodeEdits(), float temperature = 1.0f) {
+                       cudaStream_t st, unsigned long long graph_key = 0, const DecodeEdits& ed = DecodeEdits(), float temperature = 1.0f,
+                       const NextStateGather* next = nullptr, int form = 0) {
     const int rows = B * beam;
     const bool edits = ed.any();
     const int k_in = beam + ed.kinds();
     CAPB_REQUIRE(!ed.trigrams, "block_trigrams applies to _sample only (AttModel.py:306)");
     CAPB_REQUIRE(k_in <= 16, "beam_size + number of active decode edits (decoding_constraint, remove_bad_endings, UNK suppression) must be <= 16");
+    CAPB_REQUIRE(form >= 0 && form <= 2, "beam step form must be 0 (automatic), 1 (separate kernels) or 2 (fused)");
     if (temperature == 0.f) temperature = 1.0f;
     CAPB_REQUIRE(temperature > 0.f, "temperature must be positive");
     if (grow_buffer(reinterpret_cast<void**>(&d.slab), &d.slab_bytes, (size_t)T * rows * V1 * sizeof(float), st)) return 1;
@@ -269,6 +278,14 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
     d.last_beam = beam;
     BeamState s = d.bs;
     s.B = B; s.beam = beam; s.T = T; s.V1 = V1;
+    bool fused = false;
+    if (form != 1 && next != nullptr && !edits && temperature == 1.0f) {
+        VocabStepArgs probe;            // every step's slab has the alignment of step 0 (V1 % 4 == 0 makes the step stride 16-byte aligned)
+        probe.V1 = V1; probe.ld = V1; probe.logits = d.slab;
+        fused = beam_search_step_applies(probe, *next);
+    }
+    CAPB_REQUIRE(form != 2 || fused, "the fused beam step needs the engine's state descriptor, no decode edits, temperature 1 and 16-byte aligned "
+                                     "logit and state rows (V + 1 and H multiples of 4)");
     auto run_loop = [&]() -> int {
         CAPB_NVTX("capb200 beam loop (T steps: core, vocab stats, beam step)");
         CAPB_CHECK_CUDA(cudaMemsetAsync(s.sums, 0, sizeof(float) * B * beam, st));
@@ -278,7 +295,10 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
             const int live = (t == 0) ? 1 : beam;
             const int nrows = B * live;
             float* logits = d.slab + (long)t * d.slab_step_stride;
-            if (core(nrows, live, d.tokens, t == 0 ? d.neg1 : d.src_row, t, logits, (long)V1)) return 1;
+            d.states_gathered = fused && t > 0;
+            const int rc = core(nrows, live, d.tokens, t == 0 ? d.neg1 : d.src_row, t, logits, (long)V1);
+            d.states_gathered = false;
+            if (rc) return 1;
             if (t > 0 && temperature != 1.0f) {      // log_softmax(logprobs / temperature) = log_softmax(logits / temperature)  (CaptionModel.py:204)
                 if (scale_rows_launch(logits, V1, nrows, V1, 1.0f / temperature, st)) return 1;
                 *launches += 1;
@@ -288,6 +308,11 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
             va.twice = (t > 0) ? 1 : 0;      // init_logprobs went through one log_softmax only (AttModel.py:239, CaptionModel.py:204)
             va.topk = edits ? k_in : beam; va.top_val = d.top_val; va.top_idx = d.top_idx;
             va.stats = d.slab_stats + (long)t * rows;
+            if (fused) {
+                if (beam_search_step_launch(s, va, t, live, penalty_kind, penalty_alpha, *next, st)) return 1;
+                *launches += 1;
+                continue;
+            }
             if (vocab_step_launch(va, st)) return 1;
             const float* tv = d.top_val;
             const int* ti = d.top_idx;
@@ -308,6 +333,7 @@ int beam_decode_driver(DecodeBuffers& d, int V1, int T, int B, int beam, int kee
     memcpy(reinterpret_cast<char*>(&key[6]) + 4, &temperature, sizeof(float));
     // decode edits are baked into the captured launches too
     key[5] ^= ((unsigned long long)(ed.constraint & 1) << 8) ^ ((unsigned long long)(unsigned)(ed.unk_col + 1) << 16) ^ ((unsigned long long)ed.n_bad << 48);
+    key[5] ^= (unsigned long long)fused << 9;       // and the form of the step
     key[0] ^= (unsigned long long)reinterpret_cast<uintptr_t>(ed.bad) * 0x9E3779B97F4A7C15ull;
     d.last_edits = ed;
     d.last_stats = d.slab_stats;

@@ -19,6 +19,28 @@ struct StateCopy {
     ActView dst;
 };
 
+// Columns 4*c4 .. 4*c4+3 of row r of one or two states: dst[r] = src[src_row] (zeros for src_row < 0), as fp32 and the split-fp16 planes
+// when dst has them.  16-byte aligned rows (H, ld_src and dst.ld multiples of 4).  The loads of both states are issued before any store.
+__device__ __forceinline__ void copy_states4(long r, int src, int c4, int nstate, const StateCopy& sc0, const StateCopy& sc1) {
+    float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+    if (src >= 0) {
+        v0 = *reinterpret_cast<const float4*>(sc0.src + (long)src * sc0.ld_src + 4 * c4);
+        if (nstate > 1) v1 = *reinterpret_cast<const float4*>(sc1.src + (long)src * sc1.ld_src + 4 * c4);
+    }
+    for (int s = 0; s < nstate; ++s) {
+        const ActView& o = (s == 0) ? sc0.dst : sc1.dst;
+        const float4 v = (s == 0) ? v0 : v1;
+        *reinterpret_cast<float4*>(o.f + r * o.ld + 4 * c4) = v;
+        if (o.hi != nullptr) {
+            __align__(8) __half h[4];
+            __align__(8) __half l[4];
+            split_f32(v.x, h[0], l[0]); split_f32(v.y, h[1], l[1]); split_f32(v.z, h[2], l[2]); split_f32(v.w, h[3], l[3]);
+            *reinterpret_cast<uint2*>(o.hi + r * o.ld + 4 * c4) = *reinterpret_cast<const uint2*>(h);
+            *reinterpret_cast<uint2*>(o.lo + r * o.ld + 4 * c4) = *reinterpret_cast<const uint2*>(l);
+        }
+    }
+}
+
 // ---- pointwise.cu
 int state_gather_embed_launch(int rows, const int* tokens, const int* src_row, const float* emb, long ld_emb, int E, int relu,
                               ActView xt, int H, int nstate, StateCopy sc0, StateCopy sc1, cudaStream_t stream);
@@ -115,6 +137,16 @@ struct BeamState {
 };
 int beam_step_launch(const BeamState& s, int t, int live, const float* top_val, const int* top_idx, int penalty_kind, float penalty_alpha,
                      cudaStream_t stream);
+// The two recurrent states (H columns each) a fused beam step gathers by the chosen parents for the next step: dst[r] = src[s.src_row[r]]
+struct NextStateGather {
+    StateCopy s0, s1;
+    int H = 0;
+};
+// Step t of the search in one launch per image: the vocabulary statistics / top-k of `a` (stats form, a.topk = s.beam, a.rows = B * live),
+// beam_step, and for t < T - 1 the gather of `next`.  beam_search_step_applies: 16-byte aligned logit and state rows.
+bool beam_search_step_applies(const VocabStepArgs& a, const NextStateGather& next);
+int beam_search_step_launch(const BeamState& s, const VocabStepArgs& a, int t, int live, int penalty_kind, float penalty_alpha,
+                            const NextStateGather& next, cudaStream_t stream);
 // Diverse beam search, global step t (CaptionModel.py:35-209 with G = group_size groups of bdash = s.beam beams, staggered by one step per group).
 // `s` describes B*G virtual images of bdash beams (virtual image i*G + g = group g of image i, rows i*G*bdash + g*bdash + j); every group
 // active at t (0 <= t - g < T) takes one step in group order: its candidates [rows, k] (k = G*bdash per row) are lowered by lambda times the

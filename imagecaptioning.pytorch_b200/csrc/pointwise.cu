@@ -48,25 +48,7 @@ __global__ void state_gather_embed_kernel(int rows, const int* __restrict__ toke
     const bool vec = (H & 3) == 0 && (sc0.ld_src & 3) == 0 && (sc0.dst.ld & 3) == 0 && (nstate < 2 || ((sc1.ld_src & 3) == 0 && (sc1.dst.ld & 3) == 0));
     if (vec) {
         // 128-bit copies with the loads of both states issued before any store (the scalar loop was latency-bound: r01f capture)
-        for (int c4 = threadIdx.x; c4 < (H >> 2); c4 += blockDim.x) {
-            float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-            if (src >= 0) {
-                v0 = *reinterpret_cast<const float4*>(sc0.src + (long)src * sc0.ld_src + 4 * c4);
-                if (nstate > 1) v1 = *reinterpret_cast<const float4*>(sc1.src + (long)src * sc1.ld_src + 4 * c4);
-            }
-            for (int s = 0; s < nstate; ++s) {
-                const ActView& o = (s == 0) ? sc0.dst : sc1.dst;
-                const float4 v = (s == 0) ? v0 : v1;
-                *reinterpret_cast<float4*>(o.f + (long)r * o.ld + 4 * c4) = v;
-                if (o.hi != nullptr) {
-                    __align__(8) __half h[4];
-                    __align__(8) __half l[4];
-                    split_f32(v.x, h[0], l[0]); split_f32(v.y, h[1], l[1]); split_f32(v.z, h[2], l[2]); split_f32(v.w, h[3], l[3]);
-                    *reinterpret_cast<uint2*>(o.hi + (long)r * o.ld + 4 * c4) = *reinterpret_cast<const uint2*>(h);
-                    *reinterpret_cast<uint2*>(o.lo + (long)r * o.ld + 4 * c4) = *reinterpret_cast<const uint2*>(l);
-                }
-            }
-        }
+        for (int c4 = threadIdx.x; c4 < (H >> 2); c4 += blockDim.x) copy_states4(r, src, c4, nstate, sc0, sc1);
         return;
     }
     for (int s = 0; s < nstate; ++s) {

@@ -10,6 +10,7 @@
 #include <cooperative_groups.h>
 #include "common.cuh"
 #include "kernels.cuh"
+#include "vocab_row.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -467,137 +468,13 @@ __global__ void __launch_bounds__(VT) vocab_stats_kernel(const VocabStepArgs a) 
     }
 }
 
-// Per-thread online softmax in base 2 (the single-pass kernel below).  A thread's partial sum holds sum 2^(x*log2e - mL), where
-// mL = fl(m*log2e) belongs to its running maximum m.  mL carries the rounding of that product -- up to half an ulp of |m|*log2e, 1e-4 at
-// |m| = 1000 -- so the rescale to a new maximum and the final rescale to the row maximum are both taken against mL itself, not against m:
-// the rounding then cancels and the log-sum-exp does not degrade with the magnitude of the logits (log_softmax is shift-invariant).
-__device__ __forceinline__ void online_raise(float& part, float& m, float& mL, float m4) {
-    const float nL = m4 * 1.4426950408889634f;
-    float sc;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"(mL - nL));
-    part = (m == -INFINITY) ? 0.f : part * sc;      // a thread that has only seen -inf holds NaN (-inf - -inf), not a sum
-    m = m4;
-    mL = nL;
-}
-// the thread's share of sum exp(x - mx), mx = the row maximum
-__device__ __forceinline__ float online_finish(float part, float m, float mL, float mx) {
-    float sc;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(sc) : "f"(fmaf(-mx, 1.4426950408889634f, mL)));
-    return (m == -INFINITY) ? 0.f : part * sc;
-}
-
-// Single-pass variant of vocab_stats_kernel for 16-byte aligned rows: per-thread online softmax (running max, partial sum rescaled when
-// the max grows) and one max-of-four test in front of the top-2 bookkeeping, so the row is read once and the common path is ~5
-// instructions per element.  128 threads: 16 CTAs per SM (all 1280 rows of the headline shape resident at once, no tail wave) and
-// four independent 128-bit loads in flight per thread.
-constexpr int VT2 = 128;
-__device__ __forceinline__ float block_max4(float v, float* scratch) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = v;
-    __syncthreads();
-    return fmaxf(fmaxf(scratch[0], scratch[1]), fmaxf(scratch[2], scratch[3]));
-}
-__device__ __forceinline__ float block_sum4(float v, float* scratch) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = v;
-    __syncthreads();
-    return (scratch[0] + scratch[1]) + (scratch[2] + scratch[3]);
-}
-__device__ __forceinline__ void block_argmax4(float v, int i, float* sval, int* sidx, float& out_v, int& out_i) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, i, o);
-        if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
-    }
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) { sval[threadIdx.x >> 5] = v; sidx[threadIdx.x >> 5] = i; }
-    __syncthreads();
-    out_v = sval[0];
-    out_i = sidx[0];
-#pragma unroll
-    for (int w = 1; w < VT2 / 32; ++w) {
-        const float ov = sval[w];
-        const int oi = sidx[w];
-        if (ov > out_v || (ov == out_v && oi < out_i)) { out_v = ov; out_i = oi; }
-    }
-}
-
+// Single-pass variant of vocab_stats_kernel for 16-byte aligned rows (stats_online128_row, vocab_row.cuh).  128 threads: 16 CTAs per SM
+// (all 1280 rows of the headline shape resident at once, no tail wave) and four independent 128-bit loads in flight per thread.
 __global__ void __launch_bounds__(VT2) vocab_stats_online128_kernel(const VocabStepArgs a) {
     __shared__ float s_red[VT2 / 32];
     __shared__ int s_idx[VT2 / 32];
     const int r = blockIdx.x;
-    const int n4 = a.V1 >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(a.logits + (long)r * a.ld);
-    constexpr float kL2E = 1.4426950408889634f;
-    float t0v = -INFINITY, t1v = -INFINITY;
-    int t0i = 0x7fffffff, t1i = 0x7fffffff;
-    float m = -INFINITY, mL = -INFINITY, part = 0.f;
-    auto consume = [&](const float4 x, int v) {
-        const float m4 = fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w));
-        if (m4 > m) {
-            online_raise(part, m, mL, m4);
-        }
-        float e0, e1, e2, e3;
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(x.x, kL2E, -mL)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(x.y, kL2E, -mL)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e2) : "f"(fmaf(x.z, kL2E, -mL)));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e3) : "f"(fmaf(x.w, kL2E, -mL)));
-        part += (e0 + e1) + (e2 + e3);
-        if (m4 > t1v) {                             // strict: earlier (lower) indices win ties
-            const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                if (xs[u] > t1v) {
-                    if (xs[u] > t0v) { t1v = t0v; t1i = t0i; t0v = xs[u]; t0i = 4 * v + u; }
-                    else { t1v = xs[u]; t1i = 4 * v + u; }
-                }
-            }
-        }
-    };
-    int v = threadIdx.x;
-    for (; v + 3 * VT2 < n4; v += 4 * VT2) {        // four loads in flight, consumed in index order (tie order is preserved)
-        const float4 x0 = g4[v], x1 = g4[v + VT2], x2 = g4[v + 2 * VT2], x3 = g4[v + 3 * VT2];
-        consume(x0, v); consume(x1, v + VT2); consume(x2, v + 2 * VT2); consume(x3, v + 3 * VT2);
-    }
-    for (; v < n4; v += VT2) consume(g4[v], v);
-    const float mx = block_max4(m, s_red);
-    float sum = online_finish(part, m, mL, mx);
-    sum = block_sum4(sum, s_red);
-    const float lsum = logf(sum);
-    const float m2 = (mx - mx) - lsum, l2 = lsum;
-    if (threadIdx.x == 0) a.stats[r] = make_float2(mx, lsum);
-    int popped = 0;
-    for (int k = 0; k < a.topk; ++k) {
-        float ov;
-        int oi;
-        block_argmax4(t0v, t0i, s_red, s_idx, ov, oi);
-        if (t0i == oi && oi != 0x7fffffff) {
-            const float lastv = t0v;
-            const int lasti = t0i;
-            t0v = t1v; t0i = t1i;
-            t1v = -INFINITY; t1i = 0x7fffffff;
-            if (++popped >= 2 && t0i == 0x7fffffff) {
-                auto consider = [&](float x, int w) {
-                    const bool after = (x < lastv) || (x == lastv && w > lasti);
-                    if (after && (x > t0v || (x == t0v && w < t0i))) { t0v = x; t0i = w; }
-                };
-                for (int w = threadIdx.x; w < n4; w += VT2) {
-                    const float4 x = g4[w];
-                    consider(x.x, 4 * w); consider(x.y, 4 * w + 1); consider(x.z, 4 * w + 2); consider(x.w, 4 * w + 3);
-                }
-            }
-        }
-        if (threadIdx.x == 0) {
-            const float lp = (ov - mx) - lsum;
-            a.top_val[(long)r * a.topk + k] = a.row_twice(r) ? (lp - m2) - l2 : lp;
-            a.top_idx[(long)r * a.topk + k] = oi;
-        }
-    }
+    stats_online128_row(a, r, threadIdx.x, CtaBarrier{}, s_red, s_idx, a.top_val + (long)r * a.topk, a.top_idx + (long)r * a.topk);
 }
 
 // Scheduled sampling (AttModel.py:145-154): with probability `prob` the word fed into step `col` is drawn from the model's own previous

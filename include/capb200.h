@@ -172,6 +172,13 @@ typedef struct {
  * done_seq[B,b,T] int64, done_len[B,b], done_p[B,b], done_raw[B,b]: each image's finished beams sorted by score (may be NULL). */
 int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
                         long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream);
+/* capb200_decode_beam with the form of the search step chosen, for tests.  form 0 picks as capb200_decode_beam does: UpDown decodes
+ * without edits, at temperature 1 and with 16-byte aligned rows run each step's vocabulary statistics / top-k, beam step and the next
+ * step's state gather as one kernel per image.  1 always runs the separate kernels; 2 requires the fused kernel and fails where it does
+ * not apply.  Both forms give the same bits. */
+int capb200_decode_beam_form(int form, capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R,
+                             const capb200_beam_opts* opts, long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p,
+                             float* done_raw, void* stream);
 /* Full log-prob rows [len, V+1] of finished beam `rank` of image `image` from the most recent capb200_decode_beam call
  * (done_beams[image][rank]['logps'], CaptionModel.py:192); dst must hold T*(V+1) floats, rows beyond the length are zeroed. */
 int capb200_beam_record_logprobs(capb200_engine* e, int image, int rank, float* dst, void* stream);
