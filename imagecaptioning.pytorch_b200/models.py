@@ -157,11 +157,22 @@ def _slot_property(field):
     return property(get, put)
 
 
+def _slot_name(path):
+    return '/'.join(str(x) for x in path)
+
+
 class B200CaptionModel(nn.Module):
-    """Common machinery: engine life-cycle, weight binding and the three call surfaces."""
+    """Common machinery: engine life-cycle, weight binding, the call surfaces and the fused training steps.  The per-family data below
+    defaults to the UpDown engine's (UpDown, Att2in2, NewFC); AoANet and the Transformer have engines of their own."""
 
     family = None           # _lib.FAMILY_*
     family_name = ''
+    _abi = 'engine'         # capb200_<abi>_create / _destroy / _bind_weights / _launch_count / _set_grad_events
+    _takes_fc = True        # the engine's entry points take the fc features ahead of the region features
+    _entry = None           # capb200_<entry>_{xe,scst}_{step,vjp}: the training entry points (None: the model does not train)
+    _weights_struct, _grads_struct = _lib.Weights, None
+    _bind_only = frozenset()                # slot paths that are bound as weights but have no gradient
+    _parallel_pass = False  # the teacher-forced pass computes every position in one pass: no scheduled sampling, no early stop
 
     def __init__(self, opt, numeric_mode: Optional[str] = None):
         super().__init__()
@@ -203,15 +214,18 @@ class B200CaptionModel(nn.Module):
     _flat = _slot_property('flat')            # grad_sync.FlatGrads of this device (persistent flat gradient buffer of the fused training steps)
     _bufs = _slot_property('bufs')            # persistent per-shape output buffers of the fused training steps
 
-    def _grad_groups(self):
-        """[(name, parameter)] lists in the order the engine completes the gradients (include/capb200.h: *_set_grad_events)."""
-        raise NotImplementedError
+    def _grad_groups(self, named):
+        """The [(slot name, parameter)] of _grad_slots split into lists in the order the engine completes the gradients (include/capb200.h:
+        *_set_grad_events): the logit layer first."""
+        slots = dict(named)
+        first = ('logit_w', 'logit_b')
+        return [[(k, slots[k]) for k in first], [(k, v) for k, v in named if k not in first]]
 
-    def _flat_grads(self, device):
+    def _flat_grads(self, device, slots):
         """The persistent flat gradient buffer of this device, its {name: view} table and the engine-recorded group events.  Keyed by name:
         nn.DataParallel replicas carry different Parameter objects every forward but the same names and shapes."""
         from .grad_sync import FlatGrads
-        groups = self._grad_groups()
+        groups = self._grad_groups([(_slot_name(path), p) for path, p in slots])
         sig = tuple((n, tuple(p.shape)) for g in groups for n, p in g)
         fg = self._flat
         if fg is None or fg.sig != sig:
@@ -237,8 +251,33 @@ class B200CaptionModel(nn.Module):
             self._store.owner = id(self)
         return _lib.load()
 
-    def _weight_table(self):
-        raise NotImplementedError
+    def _slots(self):
+        """[(path of the field in the family's weights / gradient struct, parameter)]; UpDown's engine takes flat structs named by
+        _weight_table."""
+        return [((name,), t) for name, t in self._weight_table().items()]
+
+    def _grad_slots(self):
+        return [(path, p) for path, p in self._slots() if path not in self._bind_only]
+
+    @staticmethod
+    def _fill_struct(struct, pairs):
+        """Points the fields of a weights / gradient struct at tensors: pairs of (slot path, tensor)."""
+        for path, t in pairs:
+            dst = struct
+            for key in path[:-1]:
+                dst = getattr(dst, key) if isinstance(key, str) else dst[key]
+            setattr(dst, path[-1], t.data_ptr())
+
+    def _grad_table(self, lib, device, slots=None):
+        """The family's gradient struct pointing into the persistent flat buffer, the group events registered with the engine."""
+        slots = self._grad_slots() if slots is None else slots
+        fg = self._flat_grads(device, slots)
+        g = self._grads_struct()
+        self._fill_struct(g, [(path, fg.by_name[_slot_name(path)]) for path, _ in slots])
+        # the engine records the group events only for a listener (B200LossWrapper.enable_gradient_sync); without one the whole step may run as a CUDA graph
+        table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
+        _lib.check(getattr(lib, 'capb200_%s_set_grad_events' % self._abi)(self._engine, table, n), '%s_set_grad_events' % self._abi)
+        return fg, g
 
     def _bind_key(self, tensors):
         """What the engine's derived weight copies (fp16 planes, fused QKV blocks, gate tables) were built from.  (data_ptr, _version)
@@ -254,31 +293,34 @@ class B200CaptionModel(nn.Module):
         key = (_tls.dev, self.numeric_mode)
         if self._engine is None or self._engine_key != key:
             self._destroy_engine()
-            cfg = _lib.ModelCfg(self.family, self.vocab_size, self.input_encoding_size, self.rnn_size, self.att_hid_size, self.fc_feat_size,
-                                self.att_feat_size, self.seq_length, _lib.MODES[self.numeric_mode])
+            cfg = self._cfg()
             with torch.cuda.device(device):
-                eng = lib.capb200_engine_create(ctypes.byref(cfg))
+                eng = getattr(lib, 'capb200_%s_create' % self._abi)(ctypes.byref(cfg))
             if not eng:
-                raise RuntimeError('capb200 engine_create failed: %s' % lib.capb200_last_error().decode())
+                raise RuntimeError('capb200 %s_create failed: %s' % (self._abi, lib.capb200_last_error().decode()))
             self._engine, self._engine_key, self._bound_versions = eng, key, None
-        table = self._weight_table()
-        versions = self._bind_key(list(table.values()))
+        slots = self._slots()
+        versions = self._bind_key([t for _, t in slots])
         if versions is None or versions != self._bound_versions:
-            w = _lib.Weights()
             keep = []
-            for name, t in table.items():
+            for path, t in slots:
                 if t.device != device or t.dtype != torch.float32:
-                    raise RuntimeError('capb200: parameter %s must be a float32 tensor on %s' % (name, device))
-                tc = t.detach().contiguous()
-                keep.append(tc)
-                setattr(w, name, tc.data_ptr())
-            _lib.check(lib.capb200_engine_bind_weights(self._engine, ctypes.byref(w), _lib.current_stream()), 'bind_weights')
+                    raise RuntimeError('capb200: parameter %s must be a float32 tensor on %s' % (_slot_name(path), device))
+                keep.append(t.detach().contiguous())
+            w = self._weights_struct()
+            self._fill_struct(w, [(path, t) for (path, _), t in zip(slots, keep)])
+            _lib.check(getattr(lib, 'capb200_%s_bind_weights' % self._abi)(self._engine, ctypes.byref(w), _lib.current_stream()),
+                       '%s_bind_weights' % self._abi)
             self._keepalive = keep
             self._bound_versions = versions
         return lib
 
+    def _cfg(self):
+        return _lib.ModelCfg(self.family, self.vocab_size, self.input_encoding_size, self.rnn_size, self.att_hid_size, self.fc_feat_size,
+                             self.att_feat_size, self.seq_length, _lib.MODES[self.numeric_mode])
+
     def _free_engine(self, handle):
-        _lib.load().capb200_engine_destroy(handle)
+        getattr(_lib.load(), 'capb200_%s_destroy' % self._abi)(handle)
 
     def _destroy_engine(self):
         if self._engine is not None:
@@ -299,7 +341,7 @@ class B200CaptionModel(nn.Module):
 
     @property
     def launch_count(self) -> int:
-        return 0 if self._engine is None else int(_lib.load().capb200_engine_launch_count(self._engine))
+        return 0 if self._engine is None else int(getattr(_lib.load(), 'capb200_%s_launch_count' % self._abi)(self._engine))
 
     GEMM_IDS = ('fc_embed', 'att_embed', 'ctx2att', 'fc_gate_bias', 'att_lstm', 'h2att', 'lang_lstm', 'logit', 'newfc_core')
 
@@ -410,23 +452,32 @@ class B200CaptionModel(nn.Module):
         _lib.check(self._call_sample(lib, fc, att, masks, B, R, so, tok, T, seq, logprobs), 'decode_sample')
         return seq, logprobs
 
-    # family-specific C-ABI entry points (overridden by the Transformer / AoA mirrors)
+    # the decode entry points: capb200_decode_* / capb200_beam_record_logprobs of the UpDown engine, capb200_<abi>_* of the others
+    def _decode_fn(self, lib, name):
+        return getattr(lib, 'capb200_%s%s' % ('' if self._abi == 'engine' else self._abi + '_', name))
+
+    def _feat_ptrs(self, fc, att):
+        return (_lib.ptr(fc), _lib.ptr(att)) if self._takes_fc else (_lib.ptr(att),)
+
     def _call_sample(self, lib, fc, att, masks, B, R, so, tok, ld_tok, seq, logprobs):
-        return lib.capb200_decode_sample(self._engine, _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(so), _lib.ptr(tok), ld_tok,
-                                         _lib.ptr(seq), _lib.ptr(logprobs), None, _lib.current_stream())
+        return self._decode_fn(lib, 'decode_sample')(self._engine, *self._feat_ptrs(fc, att), _lib.ptr(masks), B, R, ctypes.byref(so), _lib.ptr(tok),
+                                                     ld_tok, _lib.ptr(seq), _lib.ptr(logprobs), None, _lib.current_stream())
 
     def _call_beam(self, lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw):
-        return lib.capb200_decode_beam(self._engine, _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(bo), _lib.ptr(seq),
-                                       _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
+        return self._decode_fn(lib, 'decode_beam')(self._engine, *self._feat_ptrs(fc, att), _lib.ptr(masks), B, R, ctypes.byref(bo), _lib.ptr(seq),
+                                                   _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
 
     def _call_beam_diverse(self, lib, fc, att, masks, B, R, do, seq, logprobs, d_seq, d_len, d_p, d_raw):
-        return lib.capb200_decode_beam_diverse(self._engine, _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(do), _lib.ptr(seq),
-                                               _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
+        return self._decode_fn(lib, 'decode_beam_diverse')(self._engine, *self._feat_ptrs(fc, att), _lib.ptr(masks), B, R, ctypes.byref(do), _lib.ptr(seq),
+                                                           _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw),
+                                                           _lib.current_stream())
 
     def _call_record(self, lib, image, rank, dst):
-        return lib.capb200_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
+        return self._decode_fn(lib, 'beam_record_logprobs')(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
 
     def _teacher_steps(self, seq):
+        if self._parallel_pass:
+            return seq.shape[1]         # one parallel pass in the reference: every position is computed (TransformerModel.py:340-348)
         # the reference stops at the first column i >= 1 whose labels are all pad (AttModel.py:158-159)
         col_empty = (seq[:, 1:].sum(0) == 0).nonzero()
         return int(col_empty[0].item()) + 1 if col_empty.numel() > 0 else seq.shape[1]
@@ -503,15 +554,133 @@ class B200CaptionModel(nn.Module):
         _lib.check(self._call_sample(lib, fc, att, masks, B, R, so, seq, L, None, out), 'forward_teacher')
         return out
 
+    # ---- fused training steps (capb200_<entry>_xe_step / capb200_<entry>_scst_step) ---------------------------------------------------------
+    # A family supplies _train_feats, _entry, _rates (its dropout rates, in the order of its option structs), _xe_opts and _scst_opts; the
+    # public xe_step / scst_step gather the rates and call the shared bodies.  The defaults are UpDown's, also taken by Att2in2 and NewFC.
+
+    def _train_feats(self, fc_feats, att_feats, att_masks):
+        """(what the C entry points take ahead of B, R: (fc, att) or (att,), region masks, B, R): clip_att cuts the region axis to the longest
+        valid length (AttModel.py:106-112)."""
+        fc = self._f32(fc_feats) if self._takes_fc else None
+        att, masks = self._clip(att_feats, att_masks)
+        return ((fc, att) if self._takes_fc else (att,)), masks, att.shape[0], att.shape[1]
+
+    def _rates(self, train, drop_prob=None):
+        """drop_prob_lm"""
+        return (float(self.drop_prob_lm if drop_prob is None else drop_prob),) if train else (0.0,)
+
+    def _xe_opts(self, spi, steps, seed, label_smoothing, upstream, rates, masks, ss_prob, tokens_used, keep_rows, row_loss):
+        return _lib.XeOpts(spi, steps, seed, *rates, label_smoothing, upstream, _lib.ptr(masks), ss_prob, _lib.ptr(tokens_used), keep_rows, _lib.ptr(row_loss))
+
+    def _scst_opts(self, sample_n, temperature, seed, upstream, baseline, rates, forced, masks, keep_rows, row_loss, sampler, rw):
+        return _lib.ScstOpts(sample_n, temperature, seed, *rates, upstream, baseline, _lib.ptr(forced), _lib.ptr(masks), keep_rows, _lib.ptr(row_loss), sampler, rw)
+
+    @staticmethod
+    def _grads_of(fg, slots):
+        return {prm: fg.by_name[_slot_name(path)] for path, prm in slots}
+
+    # ---- SCST training step: greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----------------
+    @_on_device
+    def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
+                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None, sample_method='sample', baseline_method='greedy',
+                  forced_baseline=None):
+        """Runs one self-critical step entirely on the device (capb200_updown_scst_step and its Att2in2 / NewFC counterparts).  Returns a
+        dict with 'loss' (0-dim), 'reward' [N, T], 'sample_seq', 'greedy_seq', 'sample_logprobs' and 'grads' {parameter: gradient tensor}.
+        ``baseline='greedy'`` is the self-critical step (loss_wrapper.py:56-73); ``'leave_one_out'`` the 'new_self_critical' structure
+        loss (losses.py:168-187): no greedy decode, each sample is scored against the mean of the image's other samples, and the
+        result carries 'scores' [B, n] (the raw CIDEr-D values the reference reports as out['reward']).  ``reward_weights`` = (cider, bleu)
+        scores each caption with cider * CIDEr-D + bleu * BLEU-4 (opts.py:169-172); None is CIDEr-D alone.  ``sample_method`` draws the
+        train-mode samples and ``baseline_method`` the eval-mode baseline (LossWrapper's train_sample_method / sc_sample_method: 'sample',
+        'greedy', 'gumbel', 'top<k>', 'top<p>'); the loss and the gradients read the full log-softmax rows whatever the sampler keeps.
+        ``forced_baseline`` [B, T] replays given baseline captions, as ``forced_tokens`` [N, T] replays samples."""
+        return self._scst_step(fc_feats, att_feats, gts, table, sample_n, self._rates(True, drop_prob), temperature, seed, upstream, baseline,
+                               forced_tokens, att_masks, keep_rows, reward_weights, sample_method, baseline_method, forced_baseline)
+
+    def _scst_step(self, fc_feats, att_feats, gts, table, sample_n, rates, temperature, seed, upstream, baseline, forced_tokens, att_masks, keep_rows,
+                   reward_weights, sample_method, baseline_method, forced_baseline):
+        from .rewards import pack_references, weights_struct
+        lead = fc_feats if self._takes_fc else att_feats
+        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
+        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', lead.shape[0],
+                                                    self.seq_length, self.vocab_size + 1, temperature, lead.device)
+        lib = self._ensure_engine(lead.device)
+        feats, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
+        dev = feats[0].device
+        N, T, V1 = B * sample_n, self.seq_length, self.vocab_size + 1
+        refs, offsets, L = pack_references(gts, dev)
+        slots = self._grad_slots()
+        fg, g = self._grad_table(lib, dev, slots)
+        if baseline not in ('greedy', 'leave_one_out'):
+            raise ValueError("baseline must be 'greedy' or 'leave_one_out'")
+        loo = baseline == 'leave_one_out'
+        # outputs live in persistent buffers (overwritten by the next step of the same shape): the step writes every row of every one
+        sample_seq, greedy_seq, logprobs, reward, loss = self._step_buffers(('scst', B, sample_n), lambda: (
+            torch.zeros(N, T, dtype=torch.long, device=dev), torch.zeros(B, T, dtype=torch.long, device=dev),
+            torch.zeros(N, T, V1, dtype=torch.float32, device=dev), torch.empty(N, T, dtype=torch.float32, device=dev),
+            torch.empty(1, dtype=torch.float32, device=dev)))
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        forced = None
+        if forced_tokens is not None:       # replay a given draw (parity tests against the reference's own samples)
+            forced = forced_tokens.detach().to(device=dev, dtype=torch.long).contiguous()
+            assert forced.shape == (N, T)
+        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None      # drop_worst: per-row losses (reduction 'none')
+        so = self._scst_opts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, rates,
+                             forced, masks, int(keep_rows), row_loss, sampler, None if rw is None else ctypes.pointer(rw))
+        entry = 'capb200_%s_scst_step' % self._entry
+        _lib.check(getattr(lib, entry)(self._engine, *map(_lib.ptr, feats), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs),
+                                       _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq),
+                                       _lib.ptr(logprobs), _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), entry[len('capb200_'):])
+        return {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
+                'grads': self._grads_of(fg, slots), 'seed': seed, 'flat': fg, 'row_loss': row_loss}
+
+    @_on_device
+    def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, att_masks=None, keep_rows=0):
+        """One cross-entropy step on the device (capb200_updown_xe_step and its Att2in2 / NewFC counterparts): teacher-forced forward over ``labels[..., :-1]`` in train mode,
+        LanguageModelCriterion / LabelSmoothing against ``labels[..., 1:]``, ``masks[..., 1:]`` (reduction 'mean'), BPTT.
+        Returns {'loss', 'logprobs' [N, L-1, V+1], 'grads' {parameter: gradient}, 'seed'}."""
+        return self._xe_step(fc_feats, att_feats, labels, masks, self._rates(True, drop_prob), label_smoothing, seed, upstream, att_masks, keep_rows)
+
+    def _xe_step(self, fc_feats, att_feats, labels, masks, rates, label_smoothing, seed, upstream, att_masks, keep_rows):
+        lib = self._ensure_engine((fc_feats if self._takes_fc else att_feats).device)
+        feats, region_masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
+        dev = feats[0].device
+        if labels.dim() == 3:
+            labels = labels.reshape(-1, labels.shape[2])
+            masks = masks.reshape(-1, masks.shape[2])
+        labels = labels.detach().to(torch.long).contiguous()
+        masks = masks.detach().to(torch.float32).contiguous()
+        N, Lc = labels.shape
+        if N % B != 0 or Lc > self.seq_length + 2 or masks.shape != labels.shape:
+            raise ValueError('labels/masks must be [B * seq_per_img, <= seq_length + 2]')
+        steps = self._teacher_steps(labels[:, :-1])
+        V1 = self.vocab_size + 1
+        slots = self._grad_slots()
+        fg, g = self._grad_table(lib, dev, slots)
+        # a pass that stops at the first all-pad column leaves the rows after it as they are: zero them (a parallel pass writes every position)
+        logprobs = (torch.empty if self._parallel_pass else torch.zeros)(N, Lc - 1, V1, dtype=torch.float32, device=dev)
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        # scheduled sampling (self.ss_prob, set by the trainer: tools/train.py:147-148): the words actually fed are returned as 'tokens_used'
+        ss = 0.0 if self._parallel_pass else float(self.ss_prob)
+        tokens_used = torch.zeros(N, Lc - 1, dtype=torch.long, device=dev) if ss > 0.0 else None
+        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
+        xo = self._xe_opts(N // B, steps, seed, float(label_smoothing), float(upstream), rates, region_masks, ss, tokens_used, int(keep_rows), row_loss)
+        entry = 'capb200_%s_xe_step' % self._entry
+        _lib.check(getattr(lib, entry)(self._engine, *map(_lib.ptr, feats), B, R, ctypes.byref(xo), _lib.ptr(labels), _lib.ptr(masks), Lc,
+                                       ctypes.byref(g), _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), entry[len('capb200_'):])
+        return {'loss': loss[0], 'logprobs': logprobs, 'grads': self._grads_of(fg, slots), 'seed': seed, 'flat': fg, 'tokens_used': tokens_used,
+                'row_loss': row_loss}
+
+
     # ---- autograd path (model.autograd): the forward of the fused training steps, and the backward of an outside dL/dlogprobs -----------
-    # A family provides _vjp_prefix (capb200_<prefix>_xe_vjp / _scst_vjp), _grads_struct, _fill_table, _vjp_params, _vjp_feats,
-    # _vjp_feat_args, _vjp_xe_opts and _vjp_scst_opts.
-    _vjp_prefix = None
+    # capb200_<entry>_xe_vjp / _scst_vjp take the fused steps' features, option structs (_xe_opts, _scst_opts) and gradient struct.
 
     def _autograd_active(self):
         """model.autograd, grad mode on, and some parameter that wants a gradient."""
-        return (getattr(self, 'autograd', False) and self._vjp_prefix is not None and torch.is_grad_enabled()
-                and any(p.requires_grad for p in self._vjp_params()))
+        return (getattr(self, 'autograd', False) and self._entry is not None and torch.is_grad_enabled()
+                and any(p.requires_grad for _, p in self._grad_slots()))
 
     @staticmethod
     def _refuse_feature_grads(*feats):
@@ -522,8 +691,9 @@ class B200CaptionModel(nn.Module):
         """The closure _EngineVjp calls: run(None) is the forward (log-probs), run(G) the backward of G = dL/dlogprobs (one fresh gradient
         tensor per parameter).  make_opts(replay) builds the option struct: replay=False for the forward, True for the backward, which
         feeds the same words (words()) with the same seed."""
-        params = self._vjp_params()
-        entry = 'capb200_%s_%s_vjp' % (self._vjp_prefix, form)
+        slots = self._grad_slots()
+        params = [p for _, p in slots]
+        entry = 'capb200_%s_%s_vjp' % (self._entry, form)
 
         def run(G):
             lib = self._ensure_engine(dev)
@@ -534,12 +704,12 @@ class B200CaptionModel(nn.Module):
                 G = G.detach().to(torch.float32).contiguous()
                 grads = [torch.empty_like(p) for p in params]
                 g = self._grads_struct()
-                self._fill_table(g, {id(p): t for p, t in zip(params, grads)})
+                self._fill_struct(g, [(path, t) for (path, _), t in zip(slots, grads)])
                 opts, vo = make_opts(True), _lib.VjpOpts(0, G.data_ptr(), 0)
             tail = (words(G is not None), logprobs_shape[1] + 1) if form == 'xe' else ()
             seq = out_seq if G is None or out_seq is None else torch.empty_like(out_seq)
             outs = (_lib.ptr(lp),) if form == 'xe' else (_lib.ptr(seq), _lib.ptr(lp))
-            args = self._vjp_feat_args(*feats) + (B, R, ctypes.byref(opts), ctypes.byref(vo))
+            args = tuple(map(_lib.ptr, feats)) + (B, R, ctypes.byref(opts), ctypes.byref(vo))
             if form == 'xe':
                 args += (_lib.ptr(tail[0]), tail[1])
             _lib.check(getattr(lib, entry)(self._engine, *args, None if g is None else ctypes.byref(g), *outs, _lib.current_stream()),
@@ -559,11 +729,11 @@ class B200CaptionModel(nn.Module):
             raise ValueError('label width %d exceeds what the engine trains (seq_length + 1 = %d)' % (L, self.seq_length + 1))
         train = self.training
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if train else 0      # where xe_step draws it: torch.manual_seed reproduces both
-        fc, att, masks, B, R = self._vjp_feats(fc_feats, att_feats, att_masks)
-        dev = (fc if fc is not None else att).device
+        feats, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
+        dev = feats[0].device
         seq = seq.to(dev)
         steps = self._teacher_steps(seq)
-        ss = float(self.ss_prob) if train and self._vjp_ss else 0.0
+        ss = float(self.ss_prob) if train and not self._parallel_pass else 0.0
         tokens_used = torch.zeros(N, L, dtype=torch.long, device=dev) if ss > 0 else None
         pad = seq.new_zeros(N, 1)
         labels = torch.cat([seq, pad], 1)       # [N, L + 1]: the entry points take labels with the target column; it is never read
@@ -572,8 +742,9 @@ class B200CaptionModel(nn.Module):
             return torch.cat([tokens_used, pad], 1) if replay and tokens_used is not None else labels
 
         def make_opts(replay):
-            return self._vjp_xe_opts(N // B, steps, seed, train, masks, 0.0 if replay else ss, None if replay else tokens_used)
-        run, params = self._vjp_run('xe', (fc, att), B, R, make_opts, words, (N, L, self.vocab_size + 1), dev)
+            return self._xe_opts(N // B, steps, seed, 0.0, 1.0, self._rates(train), masks, 0.0 if replay else ss, None if replay else tokens_used, 0,
+                                 None)
+        run, params = self._vjp_run('xe', feats, B, R, make_opts, words, (N, L, self.vocab_size + 1), dev)
         return _EngineVjp.apply(run, *params)
 
     def _sample_autograd(self, fc_feats, att_feats, att_masks, opt, forced_tokens):
@@ -601,8 +772,8 @@ class B200CaptionModel(nn.Module):
             forced = forced_tokens
         draws = forced is None and method == 'sample'
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if train or draws else 0     # where scst_step / _sample draw it
-        fc, att, masks, B, R = self._vjp_feats(fc_feats, att_feats, att_masks)
-        dev = (fc if fc is not None else att).device
+        feats, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
+        dev = feats[0].device
         N, T = B * sample_n, self.seq_length
         if forced is not None:
             forced = forced.detach().to(device=dev, dtype=torch.long).contiguous()
@@ -610,8 +781,9 @@ class B200CaptionModel(nn.Module):
         seq = torch.zeros(N, T, dtype=torch.long, device=dev)
 
         def make_opts(replay):
-            return self._vjp_scst_opts(sample_n, temperature, seed, train, masks, seq if replay else forced)
-        run, params = self._vjp_run('scst', (fc, att), B, R, make_opts, None, (N, T, self.vocab_size + 1), dev,
+            return self._scst_opts(sample_n, temperature, seed, 1.0, _lib.BASELINE_GREEDY, self._rates(train), seq if replay else forced, masks, 0, None,
+                                   None, None)
+        run, params = self._vjp_run('scst', feats, B, R, make_opts, None, (N, T, self.vocab_size + 1), dev,
                                     greedy=forced is None and method == 'greedy', out_seq=seq)
         logprobs = _EngineVjp.apply(run, *params)
         return seq, logprobs
@@ -664,148 +836,6 @@ class _LazyDoneBeams(list):
         return self._B
 
 
-class _FusedTrainSteps:
-    """The fused XE / SCST training steps of the families that share UpDown's option structs (include/capb200.h: capb200_scst_opts,
-    capb200_xe_opts): UpDown, Att2in2 and NewFC.  A class sets its C entry points (_scst_entry, _xe_entry) and gradient table
-    (_grads_struct, _grad_fields)."""
-
-    def _train_feats(self, fc_feats, att_feats, att_masks):
-        """(fc, att, region masks, B, R) as the training step reads them: clip_att cuts the region axis to the longest valid length
-        (AttModel.py:106-112)."""
-        fc = self._f32(fc_feats)
-        att, masks = self._clip(att_feats, att_masks)
-        return fc, att, masks, att.shape[0], att.shape[1]
-
-    # ---- autograd path hooks (B200CaptionModel._vjp_run)
-    _vjp_ss = True             # AttModel._forward's scheduled sampling
-
-    def _vjp_params(self):
-        return list(self._weight_table().values())
-
-    def _fill_table(self, table, tensor_of):
-        for name, prm in self._weight_table().items():
-            setattr(table, name, tensor_of[id(prm)].data_ptr())
-
-    def _vjp_feats(self, fc_feats, att_feats, att_masks):
-        return self._train_feats(fc_feats, att_feats, att_masks)
-
-    @staticmethod
-    def _vjp_feat_args(fc, att):
-        return (_lib.ptr(fc), _lib.ptr(att))
-
-    def _vjp_xe_opts(self, spi, steps, seed, train, masks, ss_prob, tokens_used):
-        return _lib.XeOpts(spi, steps, seed, float(self.drop_prob_lm) if train else 0.0, 0.0, 1.0, _lib.ptr(masks), float(ss_prob),
-                           _lib.ptr(tokens_used), 0, None)
-
-    def _vjp_scst_opts(self, sample_n, temperature, seed, train, masks, forced):
-        return _lib.ScstOpts(sample_n, float(temperature), seed, float(self.drop_prob_lm) if train else 0.0, 1.0, _lib.BASELINE_GREEDY, _lib.ptr(forced),
-                             _lib.ptr(masks), 0, None, None)
-
-    def _grad_groups(self):
-        t = self._weight_table()
-        first = ('logit_w', 'logit_b')
-        return [[(k, t[k]) for k in first], [(k, v) for k, v in t.items() if k not in first]]
-
-    def _grad_table(self, lib, device):
-        """The family's gradient table (capb200_updown_grads, capb200_att2in2_grads, capb200_newfc_grads) pointing into the persistent flat
-        buffer, the group events registered with the engine."""
-        fg = self._flat_grads(device)
-        g = self._grads_struct()
-        for name in self._grad_fields:
-            setattr(g, name, fg.by_name[name].data_ptr())
-        # the engine records the group events only for a listener (B200LossWrapper.enable_gradient_sync); without one the whole step may run as a CUDA graph
-        table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
-        _lib.check(lib.capb200_engine_set_grad_events(self._engine, table, n), 'set_grad_events')
-        return fg, g
-
-    # ---- SCST training step: greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----------------
-    @_on_device
-    def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
-                  forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None, sample_method='sample', baseline_method='greedy',
-                  forced_baseline=None):
-        """Runs one self-critical step entirely on the device (capb200_updown_scst_step and its Att2in2 / NewFC counterparts).  Returns a
-        dict with 'loss' (0-dim), 'reward' [N, T], 'sample_seq', 'greedy_seq', 'sample_logprobs' and 'grads' {parameter: gradient tensor}.
-        ``baseline='greedy'`` is the self-critical step (loss_wrapper.py:56-73); ``'leave_one_out'`` the 'new_self_critical' structure
-        loss (losses.py:168-187): no greedy decode, each sample is scored against the mean of the image's other samples, and the
-        result carries 'scores' [B, n] (the raw CIDEr-D values the reference reports as out['reward']).  ``reward_weights`` = (cider, bleu)
-        scores each caption with cider * CIDEr-D + bleu * BLEU-4 (opts.py:169-172); None is CIDEr-D alone.  ``sample_method`` draws the
-        train-mode samples and ``baseline_method`` the eval-mode baseline (LossWrapper's train_sample_method / sc_sample_method: 'sample',
-        'greedy', 'gumbel', 'top<k>', 'top<p>'); the loss and the gradients read the full log-softmax rows whatever the sampler keeps.
-        ``forced_baseline`` [B, T] replays given baseline captions, as ``forced_tokens`` [N, T] replays samples."""
-        from .rewards import pack_references, weights_struct
-        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
-        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', fc_feats.shape[0],
-                                                    self.seq_length, self.vocab_size + 1, temperature, fc_feats.device)
-        lib = self._ensure_engine(fc_feats.device)
-        fc, att, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
-        dev = fc.device
-        N, T, V1 = B * sample_n, self.seq_length, self.vocab_size + 1
-        refs, offsets, L = pack_references(gts, dev)
-        table_params = self._weight_table()
-        fg, g = self._grad_table(lib, dev)
-        grads = fg.by_name
-        # outputs live in persistent buffers (overwritten by the next step of the same shape): the step writes every row of every one
-        sample_seq, greedy_seq, logprobs, reward, loss = self._step_buffers(('scst', B, sample_n), lambda: (
-            torch.zeros(N, T, dtype=torch.long, device=dev), torch.zeros(B, T, dtype=torch.long, device=dev),
-            torch.zeros(N, T, V1, dtype=torch.float32, device=dev), torch.empty(N, T, dtype=torch.float32, device=dev),
-            torch.empty(1, dtype=torch.float32, device=dev)))
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        p = self.drop_prob_lm if drop_prob is None else drop_prob
-        if baseline not in ('greedy', 'leave_one_out'):
-            raise ValueError("baseline must be 'greedy' or 'leave_one_out'")
-        loo = baseline == 'leave_one_out'
-        forced = None
-        if forced_tokens is not None:       # replay a given draw (parity tests against the reference's own samples)
-            forced = forced_tokens.detach().to(device=dev, dtype=torch.long).contiguous()
-            assert forced.shape == (N, T)
-        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None      # drop_worst: per-row losses (reduction 'none')
-        so = _lib.ScstOpts(sample_n, float(temperature), seed, float(p), float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY,
-                           _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), sampler, None if rw is None else ctypes.pointer(rw))
-        _lib.check(getattr(lib, self._scst_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs),
-                                                  _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq), _lib.ptr(greedy_seq), _lib.ptr(logprobs),
-                                                  _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), self._scst_entry[len('capb200_'):])
-        res = {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
-               'grads': {table_params[k]: grads[k] for k in table_params}, 'seed': seed, 'flat': fg, 'row_loss': row_loss}
-        return res
-
-    @_on_device
-    def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, att_masks=None, keep_rows=0):
-        """One cross-entropy step on the device (capb200_updown_xe_step and its Att2in2 / NewFC counterparts): teacher-forced forward over ``labels[..., :-1]`` in train mode,
-        LanguageModelCriterion / LabelSmoothing against ``labels[..., 1:]``, ``masks[..., 1:]`` (reduction 'mean'), BPTT.
-        Returns {'loss', 'logprobs' [N, L-1, V+1], 'grads' {parameter: gradient}, 'seed'}."""
-        lib = self._ensure_engine(fc_feats.device)
-        fc, att, region_masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
-        dev = fc.device
-        if labels.dim() == 3:
-            labels = labels.reshape(-1, labels.shape[2])
-            masks = masks.reshape(-1, masks.shape[2])
-        labels = labels.detach().to(torch.long).contiguous()
-        masks = masks.detach().to(torch.float32).contiguous()
-        N, Lc = labels.shape
-        if N % B != 0 or Lc > self.seq_length + 2 or masks.shape != labels.shape:
-            raise ValueError('labels/masks must be [B * seq_per_img, <= seq_length + 2]')
-        steps = self._teacher_steps(labels[:, :-1])
-        V1 = self.vocab_size + 1
-        table_params = self._weight_table()
-        fg, g = self._grad_table(lib, dev)
-        grads = fg.by_name
-        logprobs = torch.zeros(N, Lc - 1, V1, dtype=torch.float32, device=dev)
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        p = self.drop_prob_lm if drop_prob is None else drop_prob
-        # scheduled sampling (self.ss_prob, set by the trainer: tools/train.py:147-148): the words actually fed are returned as 'tokens_used'
-        tokens_used = torch.zeros(N, Lc - 1, dtype=torch.long, device=dev) if self.ss_prob > 0.0 else None
-        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
-        xo = _lib.XeOpts(N // B, steps, seed, float(p), float(label_smoothing), float(upstream), _lib.ptr(region_masks), float(self.ss_prob),
-                         _lib.ptr(tokens_used), int(keep_rows), _lib.ptr(row_loss))
-        _lib.check(getattr(lib, self._xe_entry)(self._engine, _lib.ptr(fc), _lib.ptr(att), B, R, ctypes.byref(xo), _lib.ptr(labels), _lib.ptr(masks), Lc,
-                                                ctypes.byref(g), _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), self._xe_entry[len('capb200_'):])
-        return {'loss': loss[0], 'logprobs': logprobs, 'grads': {table_params[k]: grads[k] for k in table_params}, 'seed': seed, 'flat': fg,
-                'tokens_used': tokens_used, 'row_loss': row_loss}
-
-
 class _UpDownCoreParams(nn.Module):
     """Parameter container with the key names of UpDownCore + Attention (AttModel.py:615-622,719-726)."""
 
@@ -818,15 +848,12 @@ class _UpDownCoreParams(nn.Module):
         self.attention.alpha_net = nn.Linear(opt.att_hid_size, 1)
 
 
-class B200UpDownModel(_FusedTrainSteps, B200CaptionModel):
+class B200UpDownModel(B200CaptionModel):
     """Drop-in for captioning.models.AttModel.UpDownModel (AttModel.py:868-872)."""
 
     family = _lib.FAMILY_UPDOWN
     family_name = 'updown'
-    # C entry points and gradient table of the fused training steps (include/capb200.h)
-    _scst_entry, _xe_entry = 'capb200_updown_scst_step', 'capb200_updown_xe_step'
-    _vjp_prefix = 'updown'
-    _grads_struct, _grad_fields = _lib.UpdownGrads, _lib.GRAD_FIELDS
+    _entry, _grads_struct = 'updown', _lib.UpdownGrads
 
     def __init__(self, opt, numeric_mode=None):
         super().__init__(opt, numeric_mode)
@@ -873,9 +900,7 @@ class B200Att2in2Model(B200UpDownModel):
 
     family = _lib.FAMILY_ATT2IN2
     family_name = 'att2in2'
-    _scst_entry, _xe_entry = 'capb200_att2in2_scst_step', 'capb200_att2in2_xe_step'
-    _vjp_prefix = 'att2in2'
-    _grads_struct, _grad_fields = _lib.Att2in2Grads, _lib.ATT2IN2_GRAD_FIELDS
+    _entry, _grads_struct = 'att2in2', _lib.Att2in2Grads
 
     def __init__(self, opt, numeric_mode=None):
         B200CaptionModel.__init__(self, opt, numeric_mode)
@@ -907,16 +932,14 @@ class _MaxoutCoreParams(nn.Module):
         self.h2h = nn.Linear(opt.rnn_size, 5 * opt.rnn_size)
 
 
-class B200NewFCModel(_FusedTrainSteps, B200CaptionModel):
+class B200NewFCModel(B200CaptionModel):
     """Drop-in for captioning.models.AttModel.NewFCModel (AttModel.py:904-945).  The fused XE / SCST steps take UpDown's surface; the
     model reads the fc features only, so ``att_feats`` of any shape (the loader's [B, 0, 0] included) and ``att_masks`` are ignored, as
     in the reference (its _prepare_feature has no clip_att)."""
 
     family = _lib.FAMILY_NEWFC
     family_name = 'newfc'
-    _scst_entry, _xe_entry = 'capb200_newfc_scst_step', 'capb200_newfc_xe_step'
-    _vjp_prefix = 'newfc'
-    _grads_struct, _grad_fields = _lib.NewfcGrads, _lib.NEWFC_GRAD_FIELDS
+    _entry, _grads_struct = 'newfc', _lib.NewfcGrads
     _no_diverse = ("the engine chooses NewFC's fresh-state pass (the image-embedding step, AttModel.py:925-936) per core call, not per row, "
                    "so its groups cannot start at different steps")
 
@@ -937,7 +960,7 @@ class B200NewFCModel(_FusedTrainSteps, B200CaptionModel):
 
     def _train_feats(self, fc_feats, att_feats, att_masks):
         fc = self._f32(fc_feats)
-        return fc, None, None, fc.shape[0], 0
+        return (fc, None), None, fc.shape[0], 0
 
 
 def _mha_params(d_model):
@@ -976,6 +999,11 @@ class B200TransformerModel(B200CaptionModel):
 
     family_name = 'transformer'
     _no_diverse = 'the decoder K/V cache and positional encoding take one position per launch, so its groups cannot be at different positions'
+    # the transformer ignores fc_feats (TransformerModel.py:305-310); its positional-encoding buffer is bound but never trained
+    _abi, _takes_fc, _entry = 'tfm', False, 'tfm'
+    _weights_struct = _grads_struct = _lib.TfmWeights
+    _bind_only = frozenset({('pe',)})
+    _parallel_pass = True
 
     def __init__(self, opt, numeric_mode=None):
         super().__init__(opt, numeric_mode)
@@ -1013,86 +1041,10 @@ class B200TransformerModel(B200CaptionModel):
             if p_.dim() > 1:
                 nn.init.xavier_uniform_(p_)
 
-    # ---- engine plumbing (own C-ABI entry points: capb200_tfm_*) ------------------------------------------------------
-    def _tensors(self):
-        out = [self.att_embed[0].weight, self.att_embed[0].bias, self.model.tgt_embed[0].lut.weight, self.model.tgt_embed[1].pe,
-               self.model.generator.proj.weight, self.model.generator.proj.bias]
-        out += list(self.model.encoder.parameters()) + list(self.model.decoder.parameters())
-        return out
+    def _cfg(self):
+        return _lib.TfmCfg(self.vocab_size, self.d_model, self.d_ff, self.h, self.N_enc, self.N_dec, self.att_feat_size, self.seq_length,
+                           _lib.MODES[self.numeric_mode])
 
-    def _ensure_engine(self, device):
-        lib = self._enter_device(device)
-        key = (_tls.dev, self.numeric_mode)
-        if self._engine is None or self._engine_key != key:
-            self._destroy_engine()
-            cfg = _lib.TfmCfg(self.vocab_size, self.d_model, self.d_ff, self.h, self.N_enc, self.N_dec, self.att_feat_size, self.seq_length,
-                              _lib.MODES[self.numeric_mode])
-            with torch.cuda.device(device):
-                eng = lib.capb200_tfm_create(ctypes.byref(cfg))
-            if not eng:
-                raise RuntimeError('capb200 tfm_create failed: %s' % lib.capb200_last_error().decode())
-            self._engine, self._engine_key, self._bound_versions = eng, key, None
-        tensors = self._tensors()
-        versions = self._bind_key(tensors)
-        if versions is None or versions != self._bound_versions:
-            for t in tensors:
-                if t.device != device or t.dtype != torch.float32 or not t.is_contiguous():
-                    raise RuntimeError('capb200: parameters must be contiguous float32 tensors on %s' % device)
-            w = _lib.TfmWeights()
-            P = lambda t: t.data_ptr()
-
-            def mha(dst, src):
-                for name, lin in zip(('q', 'k', 'v', 'o'), src.linears):
-                    setattr(dst, name + '_w', P(lin.weight))
-                    setattr(dst, name + '_b', P(lin.bias))
-
-            def common(dst, layer, n_sub):
-                dst.w1_w, dst.w1_b = P(layer.feed_forward.w_1.weight), P(layer.feed_forward.w_1.bias)
-                dst.w2_w, dst.w2_b = P(layer.feed_forward.w_2.weight), P(layer.feed_forward.w_2.bias)
-                for j in range(n_sub):
-                    setattr(dst, 'ln%d_a' % j, P(layer.sublayer[j].norm.a_2))
-                    setattr(dst, 'ln%d_b' % j, P(layer.sublayer[j].norm.b_2))
-
-            w.att_embed_w, w.att_embed_b = P(self.att_embed[0].weight), P(self.att_embed[0].bias)
-            for i, layer in enumerate(self.model.encoder.layers):
-                mha(w.enc[i].self_attn, layer.self_attn)
-                common(w.enc[i], layer, 2)
-            for i, layer in enumerate(self.model.decoder.layers):
-                mha(w.dec[i].self_attn, layer.self_attn)
-                mha(w.dec[i].src_attn, layer.src_attn)
-                common(w.dec[i], layer, 3)
-            w.enc_norm_a, w.enc_norm_b = P(self.model.encoder.norm.a_2), P(self.model.encoder.norm.b_2)
-            w.dec_norm_a, w.dec_norm_b = P(self.model.decoder.norm.a_2), P(self.model.decoder.norm.b_2)
-            w.lut, w.pe = P(self.model.tgt_embed[0].lut.weight), P(self.model.tgt_embed[1].pe)
-            w.gen_w, w.gen_b = P(self.model.generator.proj.weight), P(self.model.generator.proj.bias)
-            _lib.check(lib.capb200_tfm_bind_weights(self._engine, ctypes.byref(w), _lib.current_stream()), 'tfm_bind_weights')
-            self._keepalive = tensors
-            self._bound_versions = versions
-        return lib
-
-    def _free_engine(self, handle):
-        _lib.load().capb200_tfm_destroy(handle)
-
-    @property
-    def launch_count(self) -> int:
-        return 0 if self._engine is None else int(_lib.load().capb200_tfm_launch_count(self._engine))
-
-    # ---- calls: the transformer ignores fc_feats (TransformerModel.py:305-310) ---------------------------------------
-    def _call_sample(self, lib, fc, att, masks, B, R, so, tok, ld_tok, seq, logprobs):
-        return lib.capb200_tfm_decode_sample(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(so), _lib.ptr(tok), ld_tok,
-                                             _lib.ptr(seq), _lib.ptr(logprobs), None, _lib.current_stream())
-
-    def _call_beam(self, lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw):
-        return lib.capb200_tfm_decode_beam(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(bo), _lib.ptr(seq), _lib.ptr(logprobs),
-                                           _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
-
-    def _call_record(self, lib, image, rank, dst):
-        return lib.capb200_tfm_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
-
-    def _teacher_steps(self, seq):
-        return seq.shape[1]            # one parallel pass in the reference: every position is computed (TransformerModel.py:340-348)
-
-    # ---- training steps (capb200_tfm_xe_step / capb200_tfm_scst_step) ---------------------------------------------------------------
     def _slots(self):
         """[(path into capb200_tfm_weights / capb200_tfm_grads, parameter)]: path = (field,) | ('enc'|'dec', layer, field) | ('enc'|'dec', layer, attn, field)."""
         out = [(('att_embed_w',), self.att_embed[0].weight), (('att_embed_b',), self.att_embed[0].bias)]
@@ -1116,99 +1068,37 @@ class B200TransformerModel(B200CaptionModel):
         for i, layer in enumerate(self.model.decoder.layers):
             layer_slots('dec', i, layer, ('self_attn', 'src_attn'), 3)
         out += [(('dec_norm_a',), self.model.decoder.norm.a_2), (('dec_norm_b',), self.model.decoder.norm.b_2),
-                (('lut',), self.model.tgt_embed[0].lut.weight), (('gen_w',), self.model.generator.proj.weight), (('gen_b',), self.model.generator.proj.bias)]
+                (('lut',), self.model.tgt_embed[0].lut.weight), (('pe',), self.model.tgt_embed[1].pe),
+                (('gen_w',), self.model.generator.proj.weight), (('gen_b',), self.model.generator.proj.bias)]
         return out
 
-    @staticmethod
-    def _slot_name(path):
-        return '/'.join(str(x) for x in path)
-
-    def _grad_groups(self):
-        slots = [(self._slot_name(path), prm) for path, prm in self._slots()]
-        late = [s for s in slots if s[0].startswith(('enc', 'att_embed'))]              # encoder + att_embed finish last
-        early = [s for s in slots if not s[0].startswith(('enc', 'att_embed'))]
+    def _grad_groups(self, named):
+        late = [s for s in named if s[0].startswith(('enc', 'att_embed'))]              # encoder + att_embed finish last
+        early = [s for s in named if not s[0].startswith(('enc', 'att_embed'))]
         return [early, late]
 
-    def _grad_table(self, lib, device):
-        fg = self._flat_grads(device)
-        g = _lib.TfmWeights()
-        for path, _ in self._slots():
-            ptr = fg.by_name[self._slot_name(path)].data_ptr()
-            dst = g
-            for key in path[:-1]:
-                dst = getattr(dst, key) if isinstance(key, str) else dst[key]
-            setattr(dst, path[-1], ptr)
-        # the engine records the group events only for a listener (B200LossWrapper.enable_gradient_sync); without one the whole step may run as a CUDA graph
-        table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
-        _lib.check(lib.capb200_tfm_set_grad_events(self._engine, table, n), 'tfm_set_grad_events')
-        return fg, g
+    def _rates(self, train, drop_prob=None, dropout=None):
+        """drop_prob_lm (att_embed's dropout), dropout (the Transformer's own rate)"""
+        if not train:
+            return 0.0, 0.0
+        return float(self.drop_prob_lm if drop_prob is None else drop_prob), float(self.dropout if dropout is None else dropout)
 
-    def _result_grads(self, fg):
-        return {prm: fg.by_name[self._slot_name(path)] for path, prm in self._slots()}
+    def _xe_opts(self, spi, steps, seed, label_smoothing, upstream, rates, masks, ss_prob, tokens_used, keep_rows, row_loss):
+        return _lib.TfmXeOpts(spi, seed, label_smoothing, upstream, *rates, _lib.ptr(masks), keep_rows, _lib.ptr(row_loss))
 
-    # ---- autograd path hooks (B200CaptionModel._vjp_run); no scheduled sampling, as in TransformerModel._forward
-    _vjp_prefix, _grads_struct, _vjp_ss = 'tfm', _lib.TfmWeights, False
-
-    def _vjp_params(self):
-        return [prm for _, prm in self._slots()]
-
-    def _fill_table(self, table, tensor_of):
-        for path, prm in self._slots():
-            dst = table
-            for key in path[:-1]:
-                dst = getattr(dst, key) if isinstance(key, str) else dst[key]
-            setattr(dst, path[-1], tensor_of[id(prm)].data_ptr())
-
-    def _vjp_feats(self, fc_feats, att_feats, att_masks):
-        att, masks = self._clip(att_feats, att_masks)
-        return None, att, masks, att.shape[0], att.shape[1]
-
-    @staticmethod
-    def _vjp_feat_args(fc, att):
-        return (_lib.ptr(att),)
-
-    def _vjp_rates(self, train):
-        return (float(self.drop_prob_lm), float(self.dropout)) if train else (0.0, 0.0)
-
-    def _vjp_xe_opts(self, spi, steps, seed, train, masks, ss_prob, tokens_used):
-        return _lib.TfmXeOpts(spi, seed, 0.0, 1.0, *self._vjp_rates(train), _lib.ptr(masks), 0, None)
-
-    def _vjp_scst_opts(self, sample_n, temperature, seed, train, masks, forced):
-        return _lib.TfmScstOpts(sample_n, float(temperature), seed, 1.0, _lib.BASELINE_GREEDY, *self._vjp_rates(train), _lib.ptr(forced), _lib.ptr(masks),
-                                0, None, None)
+    def _scst_opts(self, sample_n, temperature, seed, upstream, baseline, rates, forced, masks, keep_rows, row_loss, sampler, rw):
+        return _lib.TfmScstOpts(sample_n, temperature, seed, upstream, baseline, *rates, _lib.ptr(forced), _lib.ptr(masks), keep_rows, _lib.ptr(row_loss),
+                                sampler, rw)
 
     @_on_device
     def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, dropout=None, att_masks=None,
                 keep_rows=0):
         """One cross-entropy step of the Transformer on the device (capb200_tfm_xe_step): the teacher-forced pass over every position
         (TransformerModel.py:340-348), LanguageModelCriterion / LabelSmoothing, backward through decoder and encoder.  ``drop_prob`` is
-        att_embed's dropout (drop_prob_lm), ``dropout`` the Transformer's own rate.  Result as B200UpDownModel.xe_step."""
-        lib = self._ensure_engine(att_feats.device)
-        att, region_masks = self._clip(att_feats, att_masks)
-        dev = att.device
-        B, R = att.shape[0], att.shape[1]
-        if labels.dim() == 3:
-            labels = labels.reshape(-1, labels.shape[2])
-            masks = masks.reshape(-1, masks.shape[2])
-        labels = labels.detach().to(torch.long).contiguous()
-        masks = masks.detach().to(torch.float32).contiguous()
-        N, Lc = labels.shape
-        if N % B != 0 or Lc > self.seq_length + 2 or masks.shape != labels.shape:
-            raise ValueError('labels/masks must be [B * seq_per_img, <= seq_length + 2]')
-        # self.ss_prob is ignored, as in the reference: TransformerModel._forward is one parallel pass with no scheduled-sampling branch
-        V1 = self.vocab_size + 1
-        fg, g = self._grad_table(lib, dev)
-        logprobs = torch.empty(N, Lc - 1, V1, dtype=torch.float32, device=dev)
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        p_lm = self.drop_prob_lm if drop_prob is None else drop_prob
-        p = self.dropout if dropout is None else dropout
-        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
-        xo = _lib.TfmXeOpts(N // B, seed, float(label_smoothing), float(upstream), float(p_lm), float(p), _lib.ptr(region_masks), int(keep_rows), _lib.ptr(row_loss))
-        _lib.check(lib.capb200_tfm_xe_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(xo), _lib.ptr(labels), _lib.ptr(masks), Lc, ctypes.byref(g),
-                                           _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), 'tfm_xe_step')
-        return {'loss': loss[0], 'logprobs': logprobs, 'grads': self._result_grads(fg), 'seed': seed, 'flat': fg, 'tokens_used': None, 'row_loss': row_loss}
+        att_embed's dropout (drop_prob_lm), ``dropout`` the Transformer's own rate.  self.ss_prob is ignored, as in the reference:
+        TransformerModel._forward is one parallel pass with no scheduled-sampling branch.  Result as B200UpDownModel.xe_step."""
+        return self._xe_step(fc_feats, att_feats, labels, masks, self._rates(True, drop_prob, dropout), label_smoothing, seed, upstream, att_masks,
+                             keep_rows)
 
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy', dropout=None,
@@ -1217,48 +1107,18 @@ class B200TransformerModel(B200CaptionModel):
         """One self-critical step of the Transformer on the device (capb200_tfm_scst_step): eval-mode greedy baseline (or leave-one-out),
         train-mode samples drawn position by position on the K/V tape, CIDEr-D (or weighted, ``reward_weights``) reward, RewardCriterion,
         batched backward.  ``sample_method`` / ``baseline_method`` / ``forced_baseline`` and the result as B200UpDownModel.scst_step."""
-        from .rewards import pack_references, weights_struct
-        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
-        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', att_feats.shape[0],
-                                                    self.seq_length, self.vocab_size + 1, temperature, att_feats.device)
-        lib = self._ensure_engine(att_feats.device)
-        att, masks = self._clip(att_feats, att_masks)
-        dev = att.device
-        B, R = att.shape[0], att.shape[1]
-        N, T, V1 = B * sample_n, self.seq_length, self.vocab_size + 1
-        refs, offsets, L = pack_references(gts, dev)
-        fg, g = self._grad_table(lib, dev)
-        if baseline not in ('greedy', 'leave_one_out'):
-            raise ValueError("baseline must be 'greedy' or 'leave_one_out'")
-        loo = baseline == 'leave_one_out'
-        sample_seq, greedy_seq, logprobs, reward, loss = self._step_buffers(('scst', B, sample_n), lambda: (
-            torch.zeros(N, T, dtype=torch.long, device=dev), torch.zeros(B, T, dtype=torch.long, device=dev),
-            torch.zeros(N, T, V1, dtype=torch.float32, device=dev), torch.empty(N, T, dtype=torch.float32, device=dev),
-            torch.empty(1, dtype=torch.float32, device=dev)))
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        p_lm = self.drop_prob_lm if drop_prob is None else drop_prob
-        p = self.dropout if dropout is None else dropout
-        forced = None
-        if forced_tokens is not None:
-            forced = forced_tokens.detach().to(device=dev, dtype=torch.long).contiguous()
-            assert forced.shape == (N, T)
-        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
-        so = _lib.TfmScstOpts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, float(p_lm),
-                              float(p), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss), sampler,
-                              None if rw is None else ctypes.pointer(rw))
-        _lib.check(lib.capb200_tfm_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs), _lib.ptr(offsets), L,
-                                             ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq), _lib.ptr(logprobs),
-                                             _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'tfm_scst_step')
-        return {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
-                'grads': self._result_grads(fg), 'seed': seed, 'flat': fg, 'row_loss': row_loss}
+        return self._scst_step(fc_feats, att_feats, gts, table, sample_n, self._rates(True, drop_prob, dropout), temperature, seed, upstream, baseline,
+                               forced_tokens, att_masks, keep_rows, reward_weights, sample_method, baseline_method, forced_baseline)
 
 
 class B200AoAModel(B200CaptionModel):
     """Drop-in for captioning.models.AoAModel.AoAModel in the configs/aoa.yml configuration (refine=1, refine_aoa=1, use_ff=0,
     decoder_type='AoA', use_multi_head=2, multi_head_scale=1, mean_feats=1): same state_dict keys (no fc_embed), same surfaces."""
 
+    family = _lib.FAMILY_AOA
     family_name = 'aoa'
+    _abi, _takes_fc, _entry = 'aoa', False, 'aoa'
+    _weights_struct = _grads_struct = _lib.AoaWeights
 
     def __init__(self, opt, numeric_mode=None):
         super().__init__(opt, numeric_mode)
@@ -1298,8 +1158,9 @@ class B200AoAModel(B200CaptionModel):
         self.core.attention.norm = _ln_params(H)
         self.core.attention.linears = nn.ModuleList([nn.Linear(H, H)])
 
-    def _tensors(self):
-        return [prm for _, prm in self._slots()]          # attribute access: works on nn.DataParallel replicas too (their parameters() is empty)
+    def _cfg(self):
+        return _lib.AoaCfg(self.vocab_size, self.input_encoding_size, self.rnn_size, self.num_heads, self.att_feat_size, self.seq_length,
+                           _lib.MODES[self.numeric_mode])
 
     def _slots(self):
         """(field path in capb200_aoa_weights / capb200_aoa_grads, parameter) pairs."""
@@ -1320,8 +1181,8 @@ class B200AoAModel(B200CaptionModel):
                 (('logit_w',), self.logit.weight), (('logit_b',), self.logit.bias)]
         return out
 
-    def _grad_groups(self):
-        slots = {'/'.join(str(x) for x in path): prm for path, prm in self._slots()}
+    def _grad_groups(self, named):
+        slots = dict(named)
         pick = lambda names: [(n, slots[n]) for n in names]
         groups = [pick(['logit_w', 'logit_b']),
                   pick(['att2ctx_w', 'att2ctx_b', 'attn_q_w', 'attn_q_b', 'att_lstm_w_ih', 'att_lstm_w_hh', 'att_lstm_b_ih', 'att_lstm_b_hh', 'attn_norm_a',
@@ -1334,53 +1195,20 @@ class B200AoAModel(B200CaptionModel):
         assert sum(len(g) for g in groups) == len(slots)
         return groups
 
-    def _grad_table(self, lib, device):
-        fg = self._flat_grads(device)
-        g = _lib.AoaWeights()
-        for path, _ in self._slots():
-            ptr = fg.by_name['/'.join(str(x) for x in path)].data_ptr()
-            if len(path) == 1:
-                setattr(g, path[0], ptr)
-            else:
-                setattr(g.refiner[path[1]], path[2], ptr)
-        # the engine records the group events only for a listener (B200LossWrapper.enable_gradient_sync); without one the whole step may run as a CUDA graph
-        table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
-        _lib.check(lib.capb200_aoa_set_grad_events(self._engine, table, n), 'aoa_set_grad_events')
-        return fg, g
-
-    # ---- autograd path hooks (B200CaptionModel._vjp_run); the rates xe_step / scst_step default to
-    _vjp_prefix, _grads_struct, _vjp_ss = 'aoa', _lib.AoaWeights, True
-
-    def _vjp_params(self):
-        return self._tensors()
-
-    def _vjp_feats(self, fc_feats, att_feats, att_masks):
-        att, masks = self._clip(att_feats, att_masks)
-        return None, att, masks, att.shape[0], att.shape[1]
-
-    @staticmethod
-    def _vjp_feat_args(fc, att):
-        return (_lib.ptr(att),)
-
-    def _vjp_rates(self, train):
+    def _rates(self, train, drop_prob=None, drop_attn=0.1, drop_aoa=None, drop_sublayer=0.1, ctx_drop=None):
         """drop_prob_lm, drop_attn, drop_aoa, drop_sublayer, ctx_drop"""
-        return (float(self.drop_prob_lm), 0.1, float(self.dropout_aoa), 0.1, int(self.ctx_drop)) if train else (0.0, 0.0, 0.0, 0.0, 0)
+        if not train:
+            return 0.0, 0.0, 0.0, 0.0, 0
+        return (float(self.drop_prob_lm if drop_prob is None else drop_prob), float(drop_attn), float(self.dropout_aoa if drop_aoa is None else drop_aoa),
+                float(drop_sublayer), int(self.ctx_drop if ctx_drop is None else ctx_drop))
 
-    def _vjp_xe_opts(self, spi, steps, seed, train, masks, ss_prob, tokens_used):
-        return _lib.AoaXeOpts(spi, steps, seed, 0.0, 1.0, *self._vjp_rates(train), _lib.ptr(masks), float(ss_prob), _lib.ptr(tokens_used), 0, None)
+    def _xe_opts(self, spi, steps, seed, label_smoothing, upstream, rates, masks, ss_prob, tokens_used, keep_rows, row_loss):
+        return _lib.AoaXeOpts(spi, steps, seed, label_smoothing, upstream, *rates, _lib.ptr(masks), ss_prob, _lib.ptr(tokens_used), keep_rows,
+                              _lib.ptr(row_loss))
 
-    def _vjp_scst_opts(self, sample_n, temperature, seed, train, masks, forced):
-        return _lib.AoaScstOpts(sample_n, float(temperature), seed, 1.0, _lib.BASELINE_GREEDY, *self._vjp_rates(train), _lib.ptr(forced), _lib.ptr(masks),
-                                0, None, None)
-
-    def _fill_table(self, table, tensor_of):
-        """Writes data pointers into an AoaWeights-layout ctypes struct; ``tensor_of`` maps id(parameter) -> tensor to point at."""
-        for path, prm in self._slots():
-            ptr = tensor_of[id(prm)].data_ptr()
-            if len(path) == 1:
-                setattr(table, path[0], ptr)
-            else:
-                setattr(table.refiner[path[1]], path[2], ptr)
+    def _scst_opts(self, sample_n, temperature, seed, upstream, baseline, rates, forced, masks, keep_rows, row_loss, sampler, rw):
+        return _lib.AoaScstOpts(sample_n, temperature, seed, upstream, baseline, *rates, _lib.ptr(forced), _lib.ptr(masks), keep_rows, _lib.ptr(row_loss),
+                                sampler, rw)
 
     @_on_device
     def scst_step(self, fc_feats, att_feats, gts, table, sample_n, temperature=1.0, drop_prob=None, seed=None, upstream=1.0, baseline='greedy',
@@ -1391,125 +1219,16 @@ class B200AoAModel(B200CaptionModel):
         the decoder and the six refiner layers.  ``fc_feats`` is unused (mean_feats=1).  ``reward_weights``, ``sample_method``,
         ``baseline_method`` and ``forced_baseline`` as in B200UpDownModel.scst_step.
         Returns the dict of B200UpDownModel.scst_step."""
-        from .rewards import pack_references, weights_struct
-        rw = weights_struct(reward_weights, gts)          # refuses a missing reference list before any device work
-        sampler, _keep, temperature = _scst_sampler(sample_method, baseline_method, forced_baseline, baseline == 'leave_one_out', att_feats.shape[0],
-                                                    self.seq_length, self.vocab_size + 1, temperature, att_feats.device)
-        lib = self._ensure_engine(att_feats.device)
-        att, masks = self._clip(att_feats, att_masks)
-        dev = att.device
-        B, R = att.shape[0], att.shape[1]
-        N, T, V1 = B * sample_n, self.seq_length, self.vocab_size + 1
-        refs, offsets, L = pack_references(gts, dev)
-        slots = self._slots()
-        fg, g = self._grad_table(lib, dev)
-        if baseline not in ('greedy', 'leave_one_out'):
-            raise ValueError("baseline must be 'greedy' or 'leave_one_out'")
-        loo = baseline == 'leave_one_out'
-        sample_seq, greedy_seq, logprobs, reward, loss = self._step_buffers(('scst', B, sample_n), lambda: (
-            torch.zeros(N, T, dtype=torch.long, device=dev), torch.zeros(B, T, dtype=torch.long, device=dev),
-            torch.zeros(N, T, V1, dtype=torch.float32, device=dev), torch.empty(N, T, dtype=torch.float32, device=dev),
-            torch.empty(1, dtype=torch.float32, device=dev)))
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        p = self.drop_prob_lm if drop_prob is None else drop_prob
-        forced = None
-        if forced_tokens is not None:
-            forced = forced_tokens.detach().to(device=dev, dtype=torch.long).contiguous()
-            assert forced.shape == (N, T)
-        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
-        so = _lib.AoaScstOpts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT if loo else _lib.BASELINE_GREEDY, float(p),
-                              float(drop_attn), float(self.dropout_aoa if drop_aoa is None else drop_aoa), float(drop_sublayer),
-                              int(self.ctx_drop if ctx_drop is None else ctx_drop), _lib.ptr(forced), _lib.ptr(masks), int(keep_rows), _lib.ptr(row_loss),
-                              sampler, None if rw is None else ctypes.pointer(rw))
-        _lib.check(lib.capb200_aoa_scst_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(so), table.handle_for(refs), _lib.ptr(refs), _lib.ptr(offsets), L,
-                                             ctypes.byref(g), _lib.ptr(sample_seq), None if loo else _lib.ptr(greedy_seq), _lib.ptr(logprobs),
-                                             _lib.ptr(reward), _lib.ptr(loss), _lib.current_stream()), 'aoa_scst_step')
-        return {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
-                'grads': {prm: fg.by_name['/'.join(str(x) for x in path)] for path, prm in slots}, 'seed': seed, 'flat': fg, 'row_loss': row_loss}
+        return self._scst_step(fc_feats, att_feats, gts, table, sample_n, self._rates(True, drop_prob, drop_attn, drop_aoa, drop_sublayer, ctx_drop),
+                               temperature, seed, upstream, baseline, forced_tokens, att_masks, keep_rows, reward_weights, sample_method, baseline_method,
+                               forced_baseline)
 
     @_on_device
     def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, drop_attn=0.1, drop_aoa=None,
                 drop_sublayer=0.1, ctx_drop=None, att_masks=None, keep_rows=0):
         """One cross-entropy step of AoANet on the device (capb200_aoa_xe_step); arguments and result as B200UpDownModel.xe_step."""
-        lib = self._ensure_engine(att_feats.device)
-        att, region_masks = self._clip(att_feats, att_masks)
-        dev = att.device
-        B, R = att.shape[0], att.shape[1]
-        if labels.dim() == 3:
-            labels = labels.reshape(-1, labels.shape[2])
-            masks = masks.reshape(-1, masks.shape[2])
-        labels = labels.detach().to(torch.long).contiguous()
-        masks = masks.detach().to(torch.float32).contiguous()
-        N, Lc = labels.shape
-        if N % B != 0 or Lc > self.seq_length + 2 or masks.shape != labels.shape:
-            raise ValueError('labels/masks must be [B * seq_per_img, <= seq_length + 2]')
-        steps = self._teacher_steps(labels[:, :-1])
-        V1 = self.vocab_size + 1
-        slots = self._slots()
-        fg, g = self._grad_table(lib, dev)
-        logprobs = torch.zeros(N, Lc - 1, V1, dtype=torch.float32, device=dev)
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        p = self.drop_prob_lm if drop_prob is None else drop_prob
-        tokens_used = torch.zeros(N, Lc - 1, dtype=torch.long, device=dev) if self.ss_prob > 0.0 else None
-        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
-        xo = _lib.AoaXeOpts(N // B, steps, seed, float(label_smoothing), float(upstream), float(p), float(drop_attn),
-                            float(self.dropout_aoa if drop_aoa is None else drop_aoa), float(drop_sublayer), int(self.ctx_drop if ctx_drop is None else ctx_drop),
-                            _lib.ptr(region_masks), float(self.ss_prob), _lib.ptr(tokens_used), int(keep_rows), _lib.ptr(row_loss))
-        _lib.check(lib.capb200_aoa_xe_step(self._engine, _lib.ptr(att), B, R, ctypes.byref(xo), _lib.ptr(labels), _lib.ptr(masks), Lc, ctypes.byref(g),
-                                           _lib.ptr(logprobs), _lib.ptr(loss), _lib.current_stream()), 'aoa_xe_step')
-        return {'loss': loss[0], 'logprobs': logprobs, 'grads': {prm: fg.by_name['/'.join(str(x) for x in path)] for path, prm in slots}, 'seed': seed,
-                'flat': fg, 'tokens_used': tokens_used, 'row_loss': row_loss}
-
-    def _ensure_engine(self, device):
-        lib = self._enter_device(device)
-        key = (_tls.dev, self.numeric_mode)
-        if self._engine is None or self._engine_key != key:
-            self._destroy_engine()
-            cfg = _lib.AoaCfg(self.vocab_size, self.input_encoding_size, self.rnn_size, self.num_heads, self.att_feat_size, self.seq_length,
-                              _lib.MODES[self.numeric_mode])
-            with torch.cuda.device(device):
-                eng = lib.capb200_aoa_create(ctypes.byref(cfg))
-            if not eng:
-                raise RuntimeError('capb200 aoa_create failed: %s' % lib.capb200_last_error().decode())
-            self._engine, self._engine_key, self._bound_versions = eng, key, None
-        tensors = self._tensors()
-        versions = self._bind_key(tensors)
-        if versions is None or versions != self._bound_versions:
-            for t in tensors:
-                if t.device != device or t.dtype != torch.float32 or not t.is_contiguous():
-                    raise RuntimeError('capb200: parameters must be contiguous float32 tensors on %s' % device)
-            w = _lib.AoaWeights()
-            self._fill_table(w, {id(t): t for t in tensors})
-            _lib.check(lib.capb200_aoa_bind_weights(self._engine, ctypes.byref(w), _lib.current_stream()), 'aoa_bind_weights')
-            self._keepalive = tensors
-            self._bound_versions = versions
-        return lib
-
-    def _free_engine(self, handle):
-        _lib.load().capb200_aoa_destroy(handle)
-
-    @property
-    def launch_count(self) -> int:
-        return 0 if self._engine is None else int(_lib.load().capb200_aoa_launch_count(self._engine))
-
-    def _call_sample(self, lib, fc, att, masks, B, R, so, tok, ld_tok, seq, logprobs):
-        return lib.capb200_aoa_decode_sample(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(so), _lib.ptr(tok), ld_tok,
-                                             _lib.ptr(seq), _lib.ptr(logprobs), None, _lib.current_stream())
-
-    def _call_beam(self, lib, fc, att, masks, B, R, bo, seq, logprobs, d_seq, d_len, d_p, d_raw):
-        return lib.capb200_aoa_decode_beam(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(bo), _lib.ptr(seq), _lib.ptr(logprobs),
-                                           _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw), _lib.current_stream())
-
-    def _call_beam_diverse(self, lib, fc, att, masks, B, R, do, seq, logprobs, d_seq, d_len, d_p, d_raw):
-        return lib.capb200_aoa_decode_beam_diverse(self._engine, _lib.ptr(att), _lib.ptr(masks), B, R, ctypes.byref(do), _lib.ptr(seq),
-                                                   _lib.ptr(logprobs), _lib.ptr(d_seq), _lib.ptr(d_len), _lib.ptr(d_p), _lib.ptr(d_raw),
-                                                   _lib.current_stream())
-
-    def _call_record(self, lib, image, rank, dst):
-        return lib.capb200_aoa_beam_record_logprobs(self._engine, image, rank, _lib.ptr(dst), _lib.current_stream())
+        return self._xe_step(fc_feats, att_feats, labels, masks, self._rates(True, drop_prob, drop_attn, drop_aoa, drop_sublayer, ctx_drop),
+                             label_smoothing, seed, upstream, att_masks, keep_rows)
 
 
 class B200AttEnsemble(B200CaptionModel):
@@ -1524,6 +1243,7 @@ class B200AttEnsemble(B200CaptionModel):
     Transformer members and training raise NotImplementedError."""
 
     family_name = 'AttEnsemble'
+    _abi = 'ensemble'
     _no_diverse = 'an ensemble runs group_size 1 only'
 
     def __init__(self, models, weights=None):
@@ -1566,20 +1286,13 @@ class B200AttEnsemble(B200CaptionModel):
             m._ensure_engine(device)
         members = (_lib.EnsembleMember * len(self.models))()
         for k, (m, w) in enumerate(zip(self.models, weights)):
-            members[k].family = _lib.FAMILY_AOA if isinstance(m, B200AoAModel) else m.family
+            members[k].family = m.family
             members[k].engine, members[k].weight = m._engine, w
         lib = self._enter_device(device)
         if self._engine is None:
             self._engine = lib.capb200_ensemble_create()
         self._members = members
         return lib
-
-    def _free_engine(self, handle):
-        _lib.load().capb200_ensemble_destroy(handle)
-
-    @property
-    def launch_count(self) -> int:
-        return 0 if self._engine is None else int(_lib.load().capb200_ensemble_launch_count(self._engine))
 
     def _call_sample(self, lib, fc, att, masks, B, R, so, tok, ld_tok, seq, logprobs):
         return lib.capb200_ensemble_decode_sample(self._engine, self._members, len(self._members), _lib.ptr(fc), _lib.ptr(att), _lib.ptr(masks), B, R,
