@@ -18,25 +18,11 @@
 
 using namespace capb200;
 
-namespace capb200 {
-__global__ void capb_add_vec_kernel(const float* a, const float* b, float* o, int n) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) o[i] = a[i] + b[i];
-}
-__global__ void capb_interleave_gates_kernel(const float* src, float* dst, int H) {      // dst[4*j+g] = src[g*H + j]
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < 4 * H) dst[i] = src[(i & 3) * H + (i >> 2)];
-}
-}  // namespace capb200
-
-struct capb200_aoa_engine {
+struct capb200_aoa_engine : EngineBase {
     capb200_aoa_cfg cfg{};
     capb200_aoa_weights w{};
-    int V1 = 0, E = 0, H = 0, heads = 0, dk = 0, F = 0, T = 0, mode = 0;
-    bool tc = false, bound = false;
-    long launches = 0;
+    int E = 0, H = 0, heads = 0, dk = 0, F = 0;
 
-    char* wblock = nullptr;
     float *r_qkv_w[CAPB200_AOA_REFINER_LAYERS] = {}, *r_qkv_b[CAPB200_AOA_REFINER_LAYERS] = {};
     float *bsum = nullptr, *bsum_il = nullptr;
     float* xgate = nullptr;
@@ -44,37 +30,21 @@ struct capb200_aoa_engine {
     Planes p_att, p_ctx, p_logit, p_ih_x, p_ih_c, p_hh, p_q, p_a2c_a, p_a2c_h;
     Planes pr_qkv[CAPB200_AOA_REFINER_LAYERS], pr_aoa_a[CAPB200_AOA_REFINER_LAYERS], pr_aoa_q[CAPB200_AOA_REFINER_LAYERS];
 
-    char* ws = nullptr;
-    int capB = 0, capRows = 0, capR = 0, capBeam = 0;
     Planes in_att;
     Act rx, rln, rqkv, ratt, rt, att_e, mean, p_att_kv, g_mean;     // prologue activations
     Act h0_in, h0_out, ctx_in, ctx_out, xt, gates, qln, qproj, att, t2;   // decoder activations [rows, .]
     float* c0[2] = {nullptr, nullptr};
     long ld_c = 0;
     int core_cur = 0;
-    DecodeBuffers d;
-    std::vector<GemmTcPlan*> plans;
-    char* tape = nullptr;          // SCST training tape (owned, grown on demand)
-    size_t tape_bytes = 0;
-    Tf32Context* tf32 = nullptr;   // tensor maps + transposed operands of the training GEMMs (tensor-core modes)
-    cudaEvent_t grad_events[10] = {};   // caller-owned: recorded when a gradient group is complete (capb200_aoa_set_grad_events)
-    cudaStream_t side = nullptr;        // the greedy baseline of the SCST step runs here, concurrently with the sampling forward
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    StepGraph sg;                       // CUDA graph of the whole SCST step (engine_common.cuh)
+
+    int decode_workspace(int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) override;
+    int decode_prepare(const float* fc, const float* att, const DecodeCtx& c, cudaStream_t st) override;
+    int decode_core(int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld, const DecodeCtx& c, cudaStream_t st) override;
 };
 
 namespace {
 
 enum Site { A_ATT = 0, A_CTX, A_GMEAN, A_LSTM, A_Q, A_A2C, A_LOGIT, A_REF /* + 2*l: qkv, aoa */, A_COUNT = A_REF + 2 * CAPB200_AOA_REFINER_LAYERS };
-
-void destroy_plans(capb200_aoa_engine* e) {
-    for (auto& p : e->plans) { if (p) gemm_tc_plan_destroy(p); p = nullptr; }
-}
-
-int gemm(capb200_aoa_engine* e, int site, GemmProblem& g, int plan_rows, cudaStream_t st) {
-    e->launches++;
-    return run_gemm_mode(e->mode, &e->plans[site], g, plan_rows, st);
-}
 
 void layout_weights(capb200_aoa_engine* e, Arena& a) {
     const int H = e->H, E = e->E;
@@ -130,32 +100,7 @@ void layout_workspace(capb200_aoa_engine* e, Arena& a, int B, int rows, int R, i
 }
 
 int ensure_workspace(capb200_aoa_engine* e, int B, int rows, int R, int beam, cudaStream_t st) {
-    if (B <= e->capB && rows <= e->capRows && R <= e->capR && beam <= e->capBeam && e->ws != nullptr) return 0;
-    const int nB = B > e->capB ? B : e->capB, nRows = rows > e->capRows ? rows : e->capRows;
-    const int nR = R > e->capR ? R : e->capR, nBeam = beam > e->capBeam ? beam : e->capBeam;
-    Arena dry;
-    layout_workspace(e, dry, nB, nRows, nR, nBeam);
-    const size_t need = dry.off + 256;
-    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-    destroy_plans(e);
-    if (e->ws) CAPB_CHECK_CUDA(cudaFree(e->ws));
-    e->ws = nullptr;
-    CAPB_CHECK_CUDA(cudaMalloc(&e->ws, need));
-    Arena real;
-    real.base = e->ws;
-    layout_workspace(e, real, nB, nRows, nR, nBeam);
-    e->capB = nB; e->capRows = nRows; e->capR = nR; e->capBeam = nBeam;
-    CAPB_CHECK_CUDA(cudaMemsetAsync(e->ws, 0, need, st));
-    return fill_int_launch(e->d.neg1, nRows, -1, st);
-}
-
-int pack(capb200_aoa_engine* e, const float* w, long ldw, int rows, int cols, const Planes& p, cudaStream_t st) {
-    e->launches++;
-    return split_planes_launch(w, ldw, rows, cols, p.hi, p.lo, p.ld, st);
-}
-int pack_gates(capb200_aoa_engine* e, const float* w, long ldw, int H, int cols, const Planes& p, cudaStream_t st) {
-    e->launches++;
-    return split_planes_interleave_launch(w, ldw, H, cols, p.hi, p.lo, p.ld, st);
+    return e->grow(B, rows, R, beam, st, [&](Arena& a, int nB, int nRows, int nR, int nBeam) { layout_workspace(e, a, nB, nRows, nR, nBeam); });
 }
 
 int prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, cudaStream_t st) {
@@ -175,7 +120,7 @@ int prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, i
         g.seg[0].lda_h = e->in_att.ld;
         g.epi.bias = w.att_embed_b; g.epi.relu = 1;
         g.epi.C = e->rx.v.f; g.epi.ldc = e->rx.v.ld;
-        if (gemm(e, A_ATT, g, capBR, st)) return 1;
+        if (e->gemm(A_ATT, g, capBR, st)) return 1;
     }
     if (mask != nullptr) { e->launches++; if (mask_rows_launch(e->rx.v, B, R, H, mask, R, st)) return 1; }
     for (int l = 0; l < CAPB200_AOA_REFINER_LAYERS; ++l) {
@@ -188,7 +133,7 @@ int prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, i
             g.seg[0] = seg_of(e->rln.v, e->r_qkv_w[l], H, e->pr_qkv[l], H);
             g.epi.bias = e->r_qkv_b[l];
             g.epi.C = e->rqkv.v.f; g.epi.ldc = e->rqkv.v.ld;
-            if (gemm(e, A_REF + 2 * l, g, capBR, st)) return 1;
+            if (e->gemm(A_REF + 2 * l, g, capBR, st)) return 1;
         }
         e->launches++;
         if (enc_self_attention_launch(B, R, e->heads, e->dk, e->rqkv.v.f, e->rqkv.v.f + H, e->rqkv.v.f + 2 * H, e->rqkv.v.ld, mask, R, e->ratt.v, st)) return 1;
@@ -199,7 +144,7 @@ int prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, i
             g.seg[1] = seg_of(e->rln.v, L.aoa_w + H, 2 * H, e->pr_aoa_q[l], H);
             g.epi.bias = L.aoa_b;
             g.epi.C = e->rt.v.f; g.epi.ldc = e->rt.v.ld;
-            if (gemm(e, A_REF + 2 * l + 1, g, capBR, st)) return 1;
+            if (e->gemm(A_REF + 2 * l + 1, g, capBR, st)) return 1;
         }
         e->launches++;
         ActView xo = e->rx.v;
@@ -215,7 +160,7 @@ int prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, i
         g.seg[0] = seg_of(e->att_e.v, w.ctx2att_w, H, e->p_ctx, H);
         g.epi.bias = w.ctx2att_b;
         g.epi.C = e->p_att_kv.v.f; g.epi.ldc = e->p_att_kv.v.ld;
-        if (gemm(e, A_CTX, g, capBR, st)) return 1;
+        if (e->gemm(A_CTX, g, capBR, st)) return 1;
     }
     {   // time-invariant gate term: mean_feats * W_ih[:, E:]^T + b_ih + b_hh
         GemmProblem g;
@@ -223,12 +168,12 @@ int prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, i
         g.seg[0] = seg_of(e->mean.v, w.att_lstm_w_ih + E, E + H, e->p_ih_c, H);
         g.epi.bias = e->tc ? e->bsum_il : e->bsum;
         g.epi.C = e->g_mean.v.f; g.epi.ldc = e->g_mean.v.ld;
-        if (gemm(e, A_GMEAN, g, e->capB, st)) return 1;
+        if (e->gemm(A_GMEAN, g, e->capB, st)) return 1;
     }
     return 0;
 }
 
-int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld_logits, int B, int R,
+int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld_logits, int R,
               const float* mask, cudaStream_t st) {
     const int H = e->H, E = e->E;
     const capb200_aoa_weights& w = e->w;
@@ -253,7 +198,7 @@ int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const
         } else {
             g.epi.C = e->gates.v.f; g.epi.ldc = e->gates.v.ld;
         }
-        if (gemm(e, A_LSTM, g, e->capRows, st)) return 1;
+        if (e->gemm(A_LSTM, g, e->capRows, st)) return 1;
     }
     if (!e->tc) {
         e->launches++;
@@ -270,7 +215,7 @@ int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const
         g.seg[0] = seg_of(e->qln.v, w.attn_q_w, H, e->p_q, H);
         g.epi.bias = w.attn_q_b;
         g.epi.C = e->qproj.v.f; g.epi.ldc = e->qproj.v.ld;
-        if (gemm(e, A_Q, g, e->capRows, st)) return 1;
+        if (e->gemm(A_Q, g, e->capRows, st)) return 1;
     }
     e->launches++;
     // AoAModel.py:168 passes (query, value = p_att[..., :H], key = p_att[..., H:]): the first half of ctx2att's output is V, the second K
@@ -283,7 +228,7 @@ int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const
         g.seg[1] = seg_of(e->h0_out.v, w.att2ctx_w + H, 2 * H, e->p_a2c_h, H);
         g.epi.bias = w.att2ctx_b;
         g.epi.C = e->t2.v.f; g.epi.ldc = e->t2.v.ld;
-        if (gemm(e, A_A2C, g, e->capRows, st)) return 1;
+        if (e->gemm(A_A2C, g, e->capRows, st)) return 1;
     }
     e->launches++;
     if (glu_launch(rows, H, e->t2.v.f, e->t2.v.ld, nullptr, 0, e->ctx_out.v, st)) return 1;
@@ -292,83 +237,45 @@ int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const
     g.seg[0] = seg_of(e->ctx_out.v, w.logit_w, H, e->p_logit, H);
     g.epi.bias = w.logit_b;
     g.epi.C = logits; g.epi.ldc = ld_logits;
-    (void)B;
-    return gemm(e, A_LOGIT, g, e->capRows, st);
-}
-
-int check_ready(capb200_aoa_engine* e) {
-    CAPB_REQUIRE(e != nullptr, "null engine");
-    CAPB_REQUIRE(e->bound, "capb200_aoa_bind_weights has not been called");
-    CAPB_CHECK_RANGE();
-    return 0;
+    return e->gemm(A_LOGIT, g, e->capRows, st);
 }
 
 }  // namespace
 
-// ---- the decode pieces (engine_common.cuh) ----------------------------------------------------------------------------
-namespace capb200 {
+EngineBase* capb200::engine_base(capb200_aoa_engine* e) { return e; }
 
-int aoa_member_info(capb200_aoa_engine* e, MemberInfo* m) {
-    if (check_ready(e)) return 1;
-    m->family = CAPB200_FAMILY_AOA;
-    m->V1 = e->V1; m->T = e->T;
-    m->attends = true;
-    m->graph_ok = true;
-    m->ws = e->ws; m->wblock = e->wblock;
-    m->fresh = e->d.neg1;
-    m->launches = &e->launches;
+int capb200_aoa_engine::decode_workspace(int B, int rows, int R, int beam, int /*rows_per_image*/, cudaStream_t st) {
+    return ensure_workspace(this, B, rows, R, beam, st);
+}
+
+int capb200_aoa_engine::decode_prepare(const float* /*fc*/, const float* att, const DecodeCtx& c, cudaStream_t st) {
+    if (prepare(this, att, c.mask, c.B, c.R, st)) return 1;
+    core_cur = 0;
     return 0;
 }
 
-int aoa_decode_workspace(capb200_aoa_engine* e, int B, int rows, int R, int beam, cudaStream_t st) {
-    return ensure_workspace(e, B, rows, R, beam, st);
+int capb200_aoa_engine::decode_core(int rows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld, const DecodeCtx& c,
+                                    cudaStream_t st) {
+    return core_step(this, rows, rpi, tokens, src_row, logits, ld, c.R, c.mask, st);
 }
-
-int aoa_decode_prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, cudaStream_t st) {
-    if (prepare(e, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
-    return 0;
-}
-
-int aoa_decode_core(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int R,
-                    const float* mask, cudaStream_t st) {
-    return core_step(e, rows, rpi, tokens, src_row, logits, ld, 0, R, mask, st);
-}
-
-}  // namespace capb200
 
 extern "C" {
 
 capb200_aoa_engine* capb200_aoa_create(const capb200_aoa_cfg* c) {
     if (c == nullptr) { set_error("null cfg"); return nullptr; }
     if (c->heads < 1 || c->rnn_size % c->heads != 0) { set_error("rnn_size must be divisible by the head count"); return nullptr; }
-    if (c->numeric_mode < 0 || c->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
-    if (c->seq_length < 1 || c->seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device: the capb200 engine has no CPU fallback"); return nullptr; }
-    capb200_aoa_engine* e = new capb200_aoa_engine();
+    capb200_aoa_engine* e = create_engine<capb200_aoa_engine>(c->vocab_size, c->seq_length, c->numeric_mode, A_COUNT);
+    if (e == nullptr) return nullptr;
     e->cfg = *c;
-    e->V1 = c->vocab_size + 1; e->E = c->input_encoding_size; e->H = c->rnn_size; e->heads = c->heads; e->dk = c->rnn_size / c->heads;
-    e->F = c->att_feat_size; e->T = c->seq_length; e->mode = c->numeric_mode;
-    e->tc = c->numeric_mode != CAPB200_MODE_SIMT_FP32;
-    e->plans.assign(A_COUNT, nullptr);
+    e->E = c->input_encoding_size; e->H = c->rnn_size; e->heads = c->heads; e->dk = c->rnn_size / c->heads; e->F = c->att_feat_size;
+    e->bind_name = "capb200_aoa_bind_weights";
+    e->family = CAPB200_FAMILY_AOA;
+    e->graph_family = 9;
+    e->grad_groups = 10;
     return e;
 }
 
-void capb200_aoa_destroy(capb200_aoa_engine* e) {
-    if (e == nullptr) return;
-    destroy_plans(e);
-    cudaFree(e->wblock);
-    cudaFree(e->ws);
-    e->d.release();
-    cudaFree(e->tape);
-    e->sg.destroy();
-    tf32_context_destroy(e->tf32);
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->side) cudaStreamDestroy(e->side);
-    delete e;
-}
+void capb200_aoa_destroy(capb200_aoa_engine* e) { delete e; }
 
 long capb200_aoa_launch_count(const capb200_aoa_engine* e) { return e ? e->launches : 0; }
 
@@ -379,14 +286,7 @@ int capb200_aoa_bind_weights(capb200_aoa_engine* e, const capb200_aoa_weights* w
                  "missing AoA weights");
     e->w = *w;
     const int H = e->H, E = e->E, V1 = e->V1;
-    if (e->wblock == nullptr) {
-        Arena dry;
-        layout_weights(e, dry);
-        CAPB_CHECK_CUDA(cudaMalloc(&e->wblock, dry.off + 256));
-        Arena real;
-        real.base = e->wblock;
-        layout_weights(e, real);
-    }
+    if (e->alloc_wblock(st, [&](Arena& a) { layout_weights(e, a); })) return 1;
     const long hh = (long)H * H;
     for (int l = 0; l < CAPB200_AOA_REFINER_LAYERS; ++l) {
         const capb200_aoa_refiner_layer& L = w->refiner[l];
@@ -397,126 +297,42 @@ int capb200_aoa_bind_weights(capb200_aoa_engine* e, const capb200_aoa_weights* w
         CAPB_CHECK_CUDA(cudaMemcpyAsync(e->r_qkv_b[l] + H, L.k_b, sizeof(float) * H, cudaMemcpyDeviceToDevice, st));
         CAPB_CHECK_CUDA(cudaMemcpyAsync(e->r_qkv_b[l] + 2 * H, L.v_b, sizeof(float) * H, cudaMemcpyDeviceToDevice, st));
     }
-    capb_add_vec_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(w->att_lstm_b_ih, w->att_lstm_b_hh, e->bsum, 4 * H);
-    capb_interleave_gates_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(e->bsum, e->bsum_il, H);
-    CAPB_CHECK_CUDA(cudaGetLastError());
+    if (add_vec_launch(w->att_lstm_b_ih, w->att_lstm_b_hh, e->bsum, 4 * H, st) || interleave_gates_launch(e->bsum, e->bsum_il, H, st)) return 1;
     e->launches += 2;
     if (e->tc) {
-        int rc = pack(e, w->att_embed_w, e->F, H, e->F, e->p_att, st) | pack(e, w->ctx2att_w, H, 2 * H, H, e->p_ctx, st) |
-                 pack(e, w->logit_w, H, V1, H, e->p_logit, st) | pack(e, w->attn_q_w, H, H, H, e->p_q, st) |
-                 pack(e, w->att2ctx_w, 2 * H, 2 * H, H, e->p_a2c_a, st) | pack(e, w->att2ctx_w + H, 2 * H, 2 * H, H, e->p_a2c_h, st) |
-                 pack_gates(e, w->att_lstm_w_ih, E + H, H, E, e->p_ih_x, st) | pack_gates(e, w->att_lstm_w_ih + E, E + H, H, H, e->p_ih_c, st) |
-                 pack_gates(e, w->att_lstm_w_hh, H, H, H, e->p_hh, st);
+        int rc = e->pack(w->att_embed_w, e->F, H, e->F, e->p_att, st) | e->pack(w->ctx2att_w, H, 2 * H, H, e->p_ctx, st) |
+                 e->pack(w->logit_w, H, V1, H, e->p_logit, st) | e->pack(w->attn_q_w, H, H, H, e->p_q, st) |
+                 e->pack(w->att2ctx_w, 2 * H, 2 * H, H, e->p_a2c_a, st) | e->pack(w->att2ctx_w + H, 2 * H, 2 * H, H, e->p_a2c_h, st) |
+                 e->pack_gates(w->att_lstm_w_ih, E + H, H, E, e->p_ih_x, st) | e->pack_gates(w->att_lstm_w_ih + E, E + H, H, H, e->p_ih_c, st) |
+                 e->pack_gates(w->att_lstm_w_hh, H, H, H, e->p_hh, st);
         for (int l = 0; l < CAPB200_AOA_REFINER_LAYERS; ++l) {
-            rc |= pack(e, e->r_qkv_w[l], H, 3 * H, H, e->pr_qkv[l], st) | pack(e, w->refiner[l].aoa_w, 2 * H, 2 * H, H, e->pr_aoa_a[l], st) |
-                  pack(e, w->refiner[l].aoa_w + H, 2 * H, 2 * H, H, e->pr_aoa_q[l], st);
+            rc |= e->pack(e->r_qkv_w[l], H, 3 * H, H, e->pr_qkv[l], st) | e->pack(w->refiner[l].aoa_w, 2 * H, 2 * H, H, e->pr_aoa_a[l], st) |
+                  e->pack(w->refiner[l].aoa_w + H, 2 * H, 2 * H, H, e->pr_aoa_q[l], st);
         }
         if (rc) return 1;
     }
-    {   // per-token gate table: relu(embed) * W_ih[:, 0:E]^T
-        const long ldE = round_up(E, 8);
-        char* tmp = nullptr;
-        const size_t tmp_bytes = (size_t)V1 * ldE * (sizeof(float) + (e->tc ? 2 * sizeof(__half) : 0)) + 1024;
-        CAPB_CHECK_CUDA(cudaMallocAsync(&tmp, tmp_bytes, st));
-        CAPB_CHECK_CUDA(cudaMemsetAsync(tmp, 0, tmp_bytes, st));
-        ActView ev;
-        ev.ld = ldE;
-        ev.f = reinterpret_cast<float*>(tmp);
-        if (e->tc) { ev.hi = reinterpret_cast<__half*>(tmp + (size_t)V1 * ldE * sizeof(float)); ev.lo = ev.hi + (size_t)V1 * ldE; }
-        int rc = 0;
-        if (ldE == E) rc = relu_copy_launch(w->embed, (long)V1 * E, ev, st);
-        else {
-            for (int v = 0; v < V1 && !rc; ++v) {
-                ActView rv = ev;
-                rv.f += (long)v * ldE; if (rv.hi) { rv.hi += (long)v * ldE; rv.lo += (long)v * ldE; }
-                rc = relu_copy_launch(w->embed + (long)v * E, E, rv, st);
-            }
-        }
-        GemmProblem g;
-        g.M = V1; g.N = 4 * H; g.nseg = 1;
-        g.seg[0] = seg_of(ev, w->att_lstm_w_ih, E + H, e->p_ih_x, E);
-        g.epi.C = e->xgate; g.epi.ldc = e->ld_xgate;
-        if (!rc) {
-            if (!e->tc) rc = gemm_simt_launch(g, st);
-            else {
-                GemmTcPlan* plan = gemm_tc_plan_create(g, e->mode == CAPB200_MODE_TC_F16X3 ? 3 : 1);
-                rc = plan ? gemm_tc_plan_launch(plan, nullptr, 0, st) : 1;
-                if (plan) gemm_tc_plan_destroy(plan);
-            }
-        }
-        e->launches += 2;
-        cudaFreeAsync(tmp, st);
-        if (rc) return 1;
-    }
-    if (e->tc && !e->bound) {        // first binding only: a re-binding must not stall the training loop (see capb200_engine_bind_weights)
-        CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-        CAPB_CHECK_RANGE();
-    }
-    e->bound = true;
-    return 0;
+    // per-token gate table: relu(embed) * W_ih[:, 0:E]^T
+    if (build_gate_table(*e, w->embed, E, H, w->att_lstm_w_ih, E + H, e->p_ih_x, e->xgate, e->ld_xgate, st)) return 1;
+    return e->finish_bind(st);
 }
 
 int capb200_aoa_decode_beam(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq,
                             float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && att != nullptr && seq != nullptr && B >= 1 && R >= 1, "bad argument");
-    const int beam = opts->beam_size, keep = opts->sample_n;
-    CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= e->V1, "beam_size must be in 1..16 and <= V+1");
-    CAPB_REQUIRE(keep == 1 || keep == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
-    if (aoa_decode_workspace(e, B, B * beam, R, beam, st)) return 1;
-    if (aoa_decode_prepare(e, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return aoa_decode_core(e, nrows, live, tokens, src_row, logits, ld, R, mask, st);
-    };
-    return beam_decode_driver(e->d, e->V1, e->T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
-                              done_raw, core, &e->launches, st, loop_graph_key(e->ws, e->wblock, mask, R, 9), to_edits(opts->edits), opts->temperature);
+    return decode_beam(e, nullptr, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_aoa_decode_beam_diverse(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
                                     long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && att != nullptr && seq != nullptr && B >= 1 && R >= 1, "bad argument");
-    if (opts->group_size == 1) return capb200_aoa_decode_beam(e, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream);
-    const int beam = opts->base.beam_size;
-    CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= e->V1, "beam_size must be in 2..16 and <= V+1");
-    if (aoa_decode_workspace(e, B, B * beam, R, beam, st)) return 1;
-    if (aoa_decode_prepare(e, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return aoa_decode_core(e, nrows, rpi, tokens, src_row, logits, ld, R, mask, st);
-    };
-    return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
-                                      opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
-                                      loop_graph_key(e->ws, e->wblock, mask, R, 9), to_edits(opts->base.edits), opts->base.temperature);
+    return decode_beam_diverse(e, nullptr, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_aoa_beam_record_logprobs(capb200_aoa_engine* e, int image, int rank, float* dst, void* stream) {
-    if (check_ready(e)) return 1;
-    return beam_record_logprobs(e->d, e->V1, e->T, image, rank, dst, static_cast<cudaStream_t>(stream));
+    return decode_record_logprobs(e, image, rank, dst, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_aoa_decode_sample(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_sample_opts* opts,
                               const long long* tokens_in, long ld_tok, long long* seq, float* seq_logprobs, float* picked, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && att != nullptr && seq_logprobs != nullptr && B >= 1 && R >= 1, "bad argument");
-    const int n = opts->sample_n, method = opts->method;
-    CAPB_REQUIRE(n >= 1 && method >= 0 && method <= 5, "bad sampling options");
-    if (method == CAPB200_SAMPLE_FORCED || method == CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(tokens_in != nullptr && ld_tok >= 1, "token matrix required");
-    if (method != CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(seq != nullptr, "seq output required");
-    if (method == CAPB200_SAMPLE_MULTINOMIAL) CAPB_REQUIRE(opts->temperature > 0.f, "temperature must be positive");
-    const int rows = B * n;
-    const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : e->T;
-    const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : e->T;
-    CAPB_REQUIRE(steps >= 0 && steps <= t_out, "steps out of range");
-    if (aoa_decode_workspace(e, B, rows, R, 1, st)) return 1;
-    if (aoa_decode_prepare(e, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return aoa_decode_core(e, nrows, n, tokens, src_row, logits, ld, R, mask, st);
-    };
-    return sample_decode_driver(e->d, e->V1, e->T, rows, method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked,
-                                core, &e->launches, st, to_edits(opts->edits), opts->top);
+    return decode_sample(e, nullptr, att, mask, B, R, opts, tokens_in, ld_tok, seq, seq_logprobs, picked, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
@@ -566,6 +382,24 @@ struct AoaTrainArgs : TrainArgs {
     float p_at = 0.f, p_aoa = 0.f, p_sub = 0.f;
     int ctx_drop = 0;
 };
+
+// AoANet's own rates (capb200_aoa_xe_opts / capb200_aoa_scst_opts), checked, into `ta`
+template <class Opts>
+int aoa_rates(const Opts& o, AoaTrainArgs* ta) {
+    CAPB_REQUIRE(o.drop_attn >= 0.f && o.drop_attn < 1.f && o.drop_aoa >= 0.f && o.drop_aoa < 1.f && o.drop_sublayer >= 0.f && o.drop_sublayer < 1.f,
+                 "dropout rates must be in [0, 1)");
+    ta->p_at = o.drop_attn; ta->p_aoa = o.drop_aoa; ta->p_sub = o.drop_sublayer; ta->ctx_drop = o.ctx_drop;
+    return 0;
+}
+
+// AoANet's options as the shared option structs
+capb200_scst_opts shared_opts(const capb200_aoa_scst_opts& o) {
+    return {o.sample_n, o.temperature, o.seed, o.drop_prob_lm, o.upstream, o.baseline, o.forced_tokens, o.att_masks, o.keep_rows, o.row_loss, o.sampler,
+            o.reward_weights};
+}
+capb200_xe_opts shared_opts(const capb200_aoa_xe_opts& o) {
+    return {o.seq_per_img, o.steps, o.seed, o.drop_prob_lm, o.label_smoothing, o.upstream, o.att_masks, o.ss_prob, o.tokens_used, o.keep_rows, o.row_loss};
+}
 
 int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const AoaTrainArgs& ta, const capb200_aoa_grads* grads, cudaStream_t st) {
     const int n = ta.n, N = B * n, T = ta.T, E = e->E, H = e->H, V1 = e->V1, F = e->F, heads = e->heads, dk = e->dk;
@@ -762,35 +596,22 @@ extern "C" int capb200_aoa_scst_step(capb200_aoa_engine* e, const float* att, in
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
-    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, opts->reward_weights};
     AoaTrainArgs ta;
-    if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
-    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    if (aoa_rates(*opts, &ta) ||
+        scst_train_args(B, shared_opts(*opts), table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     return run_scst_step(e, opts, grads, ta, nullptr, 0, att, sizeof(float) * (size_t)B * R * e->F, B, R, static_cast<cudaStream_t>(stream),
                          [&](const float*, const float* att_s, const AoaTrainArgs& t, cudaStream_t s) { return aoa_train_step(e, att_s, B, R, t, grads, s); });
 }
 
-extern "C" int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* events, int n) {
-    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 10, "AoANet has 10 gradient groups");
-    for (int i = 0; i < 10; ++i) e->grad_events[i] = (events != nullptr && i < n) ? static_cast<cudaEvent_t>(events[i]) : nullptr;
-    return 0;
-}
+extern "C" int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* events, int n) { return set_grad_events(e, events, n); }
 
 extern "C" int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_xe_opts* opts, const long long* labels,
                                    const float* masks, int label_cols, const capb200_aoa_grads* grads, float* logprobs, float* loss, void* stream) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
-    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_xe_opts shared = {opts->seq_per_img, opts->steps, opts->seed, opts->drop_prob_lm, opts->label_smoothing, opts->upstream,
-                                    opts->att_masks, opts->ss_prob, opts->tokens_used, opts->keep_rows, opts->row_loss};
     AoaTrainArgs ta;
-    if (xe_train_args(B, shared, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
-    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    if (aoa_rates(*opts, &ta) || xe_train_args(B, shared_opts(*opts), labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_eager_step(st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
 }
@@ -801,13 +622,8 @@ extern "C" int capb200_aoa_xe_vjp(capb200_aoa_engine* e, const float* att, int B
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && att && labels && logprobs && (grads || vjp->forward_only), "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
-    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_xe_opts shared = {opts->seq_per_img, opts->steps, opts->seed, opts->drop_prob_lm, opts->label_smoothing, opts->upstream,
-                                    opts->att_masks, opts->ss_prob, opts->tokens_used, opts->keep_rows, opts->row_loss};
     AoaTrainArgs ta;
-    if (xe_train_args(B, shared, labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
-    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    if (aoa_rates(*opts, &ta) || xe_train_args(B, shared_opts(*opts), labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_vjp_step(e, st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
 }
@@ -817,13 +633,11 @@ extern "C" int capb200_aoa_scst_vjp(capb200_aoa_engine* e, const float* att, int
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && att && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    const float p_at = opts->drop_attn, p_aoa = opts->drop_aoa, p_sub = opts->drop_sublayer;
-    CAPB_REQUIRE(p_at >= 0.f && p_at < 1.f && p_aoa >= 0.f && p_aoa < 1.f && p_sub >= 0.f && p_sub < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->drop_prob_lm, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, nullptr};
+    capb200_scst_opts shared = shared_opts(*opts);
+    shared.reward_weights = nullptr;     // no reward runs under the autograd entry points
     AoaTrainArgs ta;
-    if (scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
-    ta.p_at = p_at; ta.p_aoa = p_aoa; ta.p_sub = p_sub; ta.ctx_drop = opts->ctx_drop;
+    if (aoa_rates(*opts, &ta) ||
+        scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_vjp_step(e, st, [&] { return aoa_train_step(e, att, B, R, ta, grads, st); });
 }

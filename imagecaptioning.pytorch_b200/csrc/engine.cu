@@ -84,18 +84,12 @@ constexpr int G_REPORTED = 9;      // ids exposed through capb200_engine_read_pr
 using namespace capb200;
 
 
-struct capb200_engine {
+struct capb200_engine : EngineBase {
     capb200_model_cfg cfg{};
     capb200_weights w{};
-    int V1 = 0, E = 0, H = 0, A = 0, T = 0;
-    int mode = 0;
-    bool tc = false;
-    bool bound = false;
-    long launches = 0;
+    int E = 0, H = 0, A = 0;
 
-    // bind-time buffers (owned)
-    char* wblock = nullptr;
-    size_t wblock_bytes = 0;
+    // bind-time buffers (in the weight block)
     float *bsum_att = nullptr, *bsum_lang = nullptr, *bsum_core = nullptr;
     float *bsum_att_il = nullptr, *bsum_lang_il = nullptr;   // gate-interleaved copies for the fused LSTM epilogue (tensor-core modes)
     float* xgate = nullptr;          // [V+1, 4H] relu(embed) * W_ih[:, 2H:]^T: per-token gate contribution (eval-mode decode)
@@ -103,29 +97,14 @@ struct capb200_engine {
     bool use_xgate = true;
     Planes p_fc, p_attw, p_ctx, p_logit, p_a_ih_h, p_a_ih_fc, p_a_ih_x, p_a_hh, p_l_ih_a, p_l_ih_h, p_l_hh, p_h2att, p_i2h, p_h2h, p_a2c;
 
-    // workspace (owned)
-    char* ws = nullptr;
-    size_t ws_bytes = 0;
-    int capB = 0, capRows = 0, capR = 0, capBeam = 0;
+    // workspace
     Planes in_fc, in_att;                        // split copies of the user inputs (tensor-core modes)
     Act fc_e, att_e, p_att, g_fc, xt, h0_in, h1_in, h0_out, h1_out, att_res, att_h, gates;
     float *c0[2] = {nullptr, nullptr}, *c1[2] = {nullptr, nullptr};
     long ld_c = 0;
     int* img_of_row = nullptr;
     float* att_score = nullptr;   // [rows, R] attention scores
-    DecodeBuffers d;              // tokens / beam state / slab shared with the other families' engines
-
-    GemmTcPlan* plans[G_COUNT] = {nullptr};
     int core_cur = 0;   // which c buffer currently holds the state
-
-    // SCST training tape (owned, grown on demand)
-    char* tape = nullptr;
-    size_t tape_bytes = 0;
-    Tf32Context* tf32 = nullptr;       // tensor maps + transposed operands of the training GEMMs (tensor-core modes)
-    StepGraph sg;                                      // CUDA graph of the whole SCST step
-    cudaEvent_t grad_events[2] = {nullptr, nullptr};   // caller-owned: recorded when a gradient group is complete (capb200_engine_set_grad_events)
-    cudaStream_t side = nullptr;
-    cudaEvent_t ev_gfork = nullptr, ev_gjoin = nullptr;     // fork / join of the SCST step's concurrent greedy baseline
 
     // optional per-GEMM device timing (cudaEvent pairs on the launching stream), off by default
     bool profiling = false;
@@ -136,15 +115,16 @@ struct capb200_engine {
     double prof_ms[G_COUNT] = {0};
     double prof_flops[G_COUNT] = {0};
     long prof_calls[G_COUNT] = {0};
+
+    ~capb200_engine() override { for (cudaEvent_t ev : ev_pool) cudaEventDestroy(ev); }
+    int decode_workspace(int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) override;
+    int decode_prepare(const float* fc, const float* att, const DecodeCtx& c, cudaStream_t st) override;
+    int decode_core(int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld, const DecodeCtx& c, cudaStream_t st) override;
+    bool next_state(NextStateGather* next) override;
+    bool loop_graph_ok() const override { return !profiling; }
 };
 
 namespace {
-
-void destroy_plans(capb200_engine* e) {
-    for (int i = 0; i < G_COUNT; ++i) {
-        if (e->plans[i]) { gemm_tc_plan_destroy(e->plans[i]); e->plans[i] = nullptr; }
-    }
-}
 
 void layout_weights(capb200_engine* e, Arena& a) {
     const int H = e->H, E = e->E, A = e->A, V1 = e->V1;
@@ -183,23 +163,10 @@ void layout_weights(capb200_engine* e, Arena& a) {
     }
 }
 
-// the families that attend over the regions (UpDown, Att2in2); NewFC reads the fc features only
-bool attends(const capb200_engine* e) { return e->cfg.family != CAPB200_FAMILY_NEWFC; }
-
-int pack(capb200_engine* e, const float* w, long ldw, int rows, int cols, const Planes& p, cudaStream_t st) {
-    e->launches++;
-    return split_planes_launch(w, ldw, rows, cols, p.hi, p.lo, p.ld, st);
-}
-// LSTM weight blocks [4H, cols] are stored gate-interleaved (row 4*j+g) so the GEMM epilogue can apply the cell directly
-int pack_gates(capb200_engine* e, const float* w, long ldw, int H, int cols, const Planes& p, cudaStream_t st) {
-    e->launches++;
-    return split_planes_interleave_launch(w, ldw, H, cols, p.hi, p.lo, p.ld, st);
-}
-
 void layout_workspace(capb200_engine* e, Arena& a, int B, int rows, int R, int beam) {
     const int H = e->H, E = e->E, A = e->A, T = e->T;
     const bool updown = e->cfg.family == CAPB200_FAMILY_UPDOWN;
-    const bool attn = attends(e);
+    const bool attn = e->reads_att;
     const bool tc = e->tc;
     if (tc) {
         e->in_fc = carve_planes(a, B, e->cfg.fc_feat_size);
@@ -232,42 +199,12 @@ void layout_workspace(capb200_engine* e, Arena& a, int B, int rows, int R, int b
 }
 
 int ensure_workspace(capb200_engine* e, int B, int rows, int R, int beam, cudaStream_t st) {
-    if (B <= e->capB && rows <= e->capRows && R <= e->capR && beam <= e->capBeam && e->ws != nullptr) return 0;
-    const int nB = B > e->capB ? B : e->capB, nRows = rows > e->capRows ? rows : e->capRows;
-    const int nR = R > e->capR ? R : e->capR, nBeam = beam > e->capBeam ? beam : e->capBeam;
-    Arena dry;
-    layout_workspace(e, dry, nB, nRows, nR, nBeam);
-    const size_t need = dry.off + 256;
-    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-    destroy_plans(e);
-    if (e->ws) CAPB_CHECK_CUDA(cudaFree(e->ws));
-    e->ws = nullptr;
-    CAPB_CHECK_CUDA(cudaMalloc(&e->ws, need));
-    e->ws_bytes = need;
-    Arena real;
-    real.base = e->ws;
-    layout_workspace(e, real, nB, nRows, nR, nBeam);
-    e->capB = nB; e->capRows = nRows; e->capR = nR; e->capBeam = nBeam;
-    CAPB_CHECK_CUDA(cudaMemsetAsync(e->ws, 0, need, st));
-    return fill_int_launch(e->d.neg1, nRows, -1, st);
+    return e->grow(B, rows, R, beam, st, [&](Arena& a, int nB, int nRows, int nR, int nBeam) { layout_workspace(e, a, nB, nRows, nR, nBeam); });
 }
 
-// ---- GEMM dispatch ------------------------------------------------------------------------------------------------
-// `plan_rows` is the row capacity the tensor maps are encoded for; M the rows valid in this launch.
-int run_gemm_inner(capb200_engine* e, int id, GemmProblem& g, int plan_rows, cudaStream_t st) {
-    e->launches++;
-    if (!e->tc) return gemm_simt_launch(g, st);
-    if (e->plans[id] == nullptr) {
-        GemmProblem planned = g;
-        planned.M = plan_rows;
-        e->plans[id] = gemm_tc_plan_create(planned, e->mode == CAPB200_MODE_TC_F16X3 ? 3 : 1);
-        if (e->plans[id] == nullptr) return 1;
-    }
-    return gemm_tc_plan_launch(e->plans[id], &g.epi, g.M, st);
-}
-
+// ---- GEMM dispatch: the engine's GEMM, timed per launch while profiling ----------------------------------------------------------------------
 int run_gemm(capb200_engine* e, int id, GemmProblem& g, int plan_rows, cudaStream_t st) {
-    if (!e->profiling) return run_gemm_inner(e, id, g, plan_rows, st);
+    if (!e->profiling) return e->gemm(id, g, plan_rows, st);
     if (e->ev_used + 2 > e->ev_pool.size()) {
         for (int i = 0; i < 64; ++i) {
             cudaEvent_t ev;
@@ -278,7 +215,7 @@ int run_gemm(capb200_engine* e, int id, GemmProblem& g, int plan_rows, cudaStrea
     double k_total = 0;
     for (int s = 0; s < g.nseg; ++s) k_total += g.seg[s].K;
     CAPB_CHECK_CUDA(cudaEventRecord(e->ev_pool[e->ev_used], st));
-    const int rc = run_gemm_inner(e, id, g, plan_rows, st);
+    const int rc = e->gemm(id, g, plan_rows, st);
     CAPB_CHECK_CUDA(cudaEventRecord(e->ev_pool[e->ev_used + 1], st));
     e->ev_used += 2;
     e->ev_ids.push_back(id);
@@ -306,7 +243,7 @@ int prepare(capb200_engine* e, const float* fc, const float* att, const float* m
         g.epi.C = e->fc_e.v.f; g.epi.ldc = e->fc_e.v.ld; g.epi.C_hi = e->fc_e.v.hi; g.epi.C_lo = e->fc_e.v.lo; g.epi.ldcs = e->fc_e.v.ld;
         if (run_gemm(e, G_FC, g, e->capB, st)) return 1;
     }
-    if (!attends(e)) return 0;
+    if (!e->reads_att) return 0;
     ActView att_in; att_in.f = const_cast<float*>(att); att_in.ld = e->cfg.att_feat_size;
     if (e->tc) {
         e->launches++;
@@ -510,49 +447,95 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
     return run_gemm(e, G_LOGIT, g, e->capRows, st);
 }
 
-int check_ready(capb200_engine* e) {
-    CAPB_REQUIRE(e != nullptr, "null engine");
-    CAPB_REQUIRE(e->bound, "capb200_engine_bind_weights has not been called");
-    CAPB_CHECK_RANGE();
-    return 0;
-}
-
 }  // namespace
 
-// ---- the decode pieces (engine_common.cuh) ----------------------------------------------------------------------------
+// ---- pieces the AoA engine shares (engine_common.cuh) and the decode hooks ------------------------------------------------------------------
 namespace capb200 {
 
-int lstm_member_info(capb200_engine* e, MemberInfo* m) {
-    if (check_ready(e)) return 1;
-    m->family = e->cfg.family;
-    m->V1 = e->V1; m->T = e->T;
-    m->attends = attends(e);
-    m->graph_ok = !e->profiling;
-    m->ws = e->ws; m->wblock = e->wblock;
-    m->fresh = e->d.neg1;
-    m->launches = &e->launches;
+int add_vec_launch(const float* a, const float* b, float* o, int n, cudaStream_t st) {
+    add_vec_kernel<<<cdiv(n, 256), 256, 0, st>>>(a, b, o, n);
+    CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-// rows_per_image: the rows of one image in the first core call (NewFC feeds each row its image's embedding there)
-int lstm_decode_workspace(capb200_engine* e, int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) {
-    if (ensure_workspace(e, B, rows, R, beam, st)) return 1;
-    if (!attends(e)) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(e->img_of_row, rows, rows_per_image); e->launches++; }
+int interleave_gates_launch(const float* src, float* dst, int H, cudaStream_t st) {
+    interleave_gates_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(src, dst, H);
+    CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-int lstm_decode_prepare(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, cudaStream_t st) {
-    if (prepare(e, fc, att, mask, B, R, st)) return 1;
-    e->core_cur = 0;
-    return 0;
+int build_gate_table(EngineBase& e, const float* embed, int E, int H, const float* w_x, long ld_w, const Planes& p_x, float* xgate, long ld_xgate,
+                     cudaStream_t st) {
+    const int V1 = e.V1;
+    const long ldE = round_up(E, 8);
+    char* tmp = nullptr;
+    const size_t tmp_bytes = (size_t)V1 * ldE * (sizeof(float) + (e.tc ? 2 * sizeof(__half) : 0)) + 1024;
+    CAPB_CHECK_CUDA(cudaMallocAsync(&tmp, tmp_bytes, st));
+    CAPB_CHECK_CUDA(cudaMemsetAsync(tmp, 0, tmp_bytes, st));
+    ActView ev;
+    ev.ld = ldE;
+    ev.f = reinterpret_cast<float*>(tmp);
+    if (e.tc) {
+        ev.hi = reinterpret_cast<__half*>(tmp + (size_t)V1 * ldE * sizeof(float));
+        ev.lo = ev.hi + (size_t)V1 * ldE;
+    }
+    int rc = 0;
+    if (ldE == E) {
+        rc = relu_copy_launch(embed, (long)V1 * E, ev, st);
+    } else {
+        for (int v = 0; v < V1 && !rc; ++v) {     // ragged pitch (tiny test configs only): row by row
+            ActView rv = ev;
+            rv.f += (long)v * ldE; if (rv.hi) { rv.hi += (long)v * ldE; rv.lo += (long)v * ldE; }
+            rc = relu_copy_launch(embed + (long)v * E, E, rv, st);
+        }
+    }
+    GemmProblem g;
+    g.M = V1; g.N = 4 * H; g.nseg = 1;
+    g.seg[0] = seg_of(ev, w_x, ld_w, p_x, E);
+    g.epi.C = xgate; g.epi.ldc = ld_xgate;
+    if (!rc) {
+        if (!e.tc) {
+            rc = gemm_simt_launch(g, st);
+        } else {
+            GemmTcPlan* plan = gemm_tc_plan_create(g, e.mode == CAPB200_MODE_TC_F16X3 ? 3 : 1);
+            rc = plan ? gemm_tc_plan_launch(plan, nullptr, 0, st) : 1;
+            if (plan) gemm_tc_plan_destroy(plan);
+        }
+    }
+    e.launches += 2;
+    cudaFreeAsync(tmp, st);
+    return rc;
 }
 
-int lstm_decode_core(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int B, int R,
-                     const float* mask, cudaStream_t st) {
-    return core_step(e, rows, rpi, tokens, src_row, logits, ld, B, R, mask, st, e->d.states_gathered);
-}
+EngineBase* engine_base(capb200_engine* e) { return e; }
 
 }  // namespace capb200
+
+int capb200_engine::decode_workspace(int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) {
+    if (ensure_workspace(this, B, rows, R, beam, st)) return 1;
+    if (!reads_att) { iota_div_kernel<<<cdiv(rows, 256), 256, 0, st>>>(img_of_row, rows, rows_per_image); launches++; }
+    return 0;
+}
+
+int capb200_engine::decode_prepare(const float* fc, const float* att, const DecodeCtx& c, cudaStream_t st) {
+    if (prepare(this, fc, att, c.mask, c.B, c.R, st)) return 1;
+    core_cur = 0;
+    return 0;
+}
+
+int capb200_engine::decode_core(int rows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld, const DecodeCtx& c,
+                                cudaStream_t st) {
+    return core_step(this, rows, rpi, tokens, src_row, logits, ld, c.B, c.R, c.mask, st, d.states_gathered);
+}
+
+// UpDown's two states can be gathered by the fused beam step (the word enters through the per-token gate table, not an embedding copy)
+bool capb200_engine::next_state(NextStateGather* next) {
+    if (cfg.family != CAPB200_FAMILY_UPDOWN || !use_xgate) return false;
+    next->s0.src = h0_out.v.f; next->s0.ld_src = h0_out.v.ld; next->s0.dst = h0_in.v;
+    next->s1.src = h1_out.v.f; next->s1.ld_src = h1_out.v.ld; next->s1.dst = h1_in.v;
+    next->H = H;
+    return true;
+}
 
 // =====================================================================================================================
 // C ABI
@@ -569,40 +552,20 @@ capb200_engine* capb200_engine_create(const capb200_model_cfg* cfg) {
         set_error("unknown model family");
         return nullptr;
     }
-    if (cfg->numeric_mode < 0 || cfg->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
-    if (cfg->seq_length < 1 || cfg->seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        set_error("no CUDA device: the capb200 engine has no CPU fallback");
-        return nullptr;
-    }
-    capb200_engine* e = new capb200_engine();
+    capb200_engine* e = create_engine<capb200_engine>(cfg->vocab_size, cfg->seq_length, cfg->numeric_mode, G_COUNT);
+    if (e == nullptr) return nullptr;
     e->cfg = *cfg;
-    e->V1 = cfg->vocab_size + 1;
     e->E = cfg->input_encoding_size;
     e->H = cfg->rnn_size;
     e->A = cfg->att_hid_size;
-    e->T = cfg->seq_length;
-    e->mode = cfg->numeric_mode;
-    e->tc = cfg->numeric_mode != CAPB200_MODE_SIMT_FP32;
+    e->bind_name = "capb200_engine_bind_weights";
+    e->family = e->graph_family = cfg->family;
+    e->reads_fc = cfg->family != CAPB200_FAMILY_ATT2IN2;
+    e->reads_att = cfg->family != CAPB200_FAMILY_NEWFC;
     return e;
 }
 
-void capb200_engine_destroy(capb200_engine* e) {
-    if (e == nullptr) return;
-    destroy_plans(e);
-    for (cudaEvent_t ev : e->ev_pool) cudaEventDestroy(ev);
-    cudaFree(e->wblock);
-    cudaFree(e->ws);
-    e->d.release();
-    cudaFree(e->tape);
-    e->sg.destroy();
-    tf32_context_destroy(e->tf32);
-    if (e->ev_gfork) cudaEventDestroy(e->ev_gfork);
-    if (e->ev_gjoin) cudaEventDestroy(e->ev_gjoin);
-    if (e->side) cudaStreamDestroy(e->side);
-    delete e;
-}
+void capb200_engine_destroy(capb200_engine* e) { delete e; }
 
 long capb200_engine_launch_count(const capb200_engine* e) { return e ? e->launches : 0; }
 
@@ -655,210 +618,79 @@ int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, voi
     }
     e->w = *w;
     const int H = e->H, E = e->E, A = e->A, V1 = e->V1;
-    if (e->wblock == nullptr) {
-        Arena dry;
-        layout_weights(e, dry);
-        e->wblock_bytes = dry.off + 256;
-        CAPB_CHECK_CUDA(cudaMalloc(&e->wblock, e->wblock_bytes));
-        CAPB_CHECK_CUDA(cudaMemsetAsync(e->wblock, 0, e->wblock_bytes, st));
-        Arena real;
-        real.base = e->wblock;
-        layout_weights(e, real);
-    }
+    if (e->alloc_wblock(st, [&](Arena& a) { layout_weights(e, a); })) return 1;
+    int rc = 0;
     if (updown) {
-        add_vec_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(w->att_lstm_b_ih, w->att_lstm_b_hh, e->bsum_att, 4 * H);
-        add_vec_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(w->lang_lstm_b_ih, w->lang_lstm_b_hh, e->bsum_lang, 4 * H);
-        interleave_gates_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(e->bsum_att, e->bsum_att_il, H);
-        interleave_gates_kernel<<<cdiv(4 * H, 256), 256, 0, st>>>(e->bsum_lang, e->bsum_lang_il, H);
+        rc |= add_vec_launch(w->att_lstm_b_ih, w->att_lstm_b_hh, e->bsum_att, 4 * H, st);
+        rc |= add_vec_launch(w->lang_lstm_b_ih, w->lang_lstm_b_hh, e->bsum_lang, 4 * H, st);
+        rc |= interleave_gates_launch(e->bsum_att, e->bsum_att_il, H, st);
+        rc |= interleave_gates_launch(e->bsum_lang, e->bsum_lang_il, H, st);
         e->launches += 4;
     } else {
-        add_vec_kernel<<<cdiv(5 * H, 256), 256, 0, st>>>(w->i2h_b, w->h2h_b, e->bsum_core, 5 * H);
+        rc |= add_vec_launch(w->i2h_b, w->h2h_b, e->bsum_core, 5 * H, st);
         e->launches += 1;
         if (att2in2) {     // the a2c bias joins the candidate columns' bias: the a2c GEMM then needs no bias of its own
-            add_vec_kernel<<<cdiv(2 * H, 256), 256, 0, st>>>(e->bsum_core + 3 * H, w->a2c_b, e->bsum_core + 3 * H, 2 * H);
+            rc |= add_vec_launch(e->bsum_core + 3 * H, w->a2c_b, e->bsum_core + 3 * H, 2 * H, st);
             e->launches += 1;
         }
     }
-    CAPB_CHECK_CUDA(cudaGetLastError());
+    if (rc) return 1;
     if (e->tc) {
-        int rc = pack(e, w->logit_w, H, V1, H, e->p_logit, st);
+        rc = e->pack(w->logit_w, H, V1, H, e->p_logit, st);
         if (updown) {
-            rc |= pack(e, w->fc_embed_w, e->cfg.fc_feat_size, H, e->cfg.fc_feat_size, e->p_fc, st);
-            rc |= pack(e, w->att_embed_w, e->cfg.att_feat_size, H, e->cfg.att_feat_size, e->p_attw, st);
-            rc |= pack(e, w->ctx2att_w, H, A, H, e->p_ctx, st);
-            rc |= pack_gates(e, w->att_lstm_w_ih, E + 2 * H, H, H, e->p_a_ih_h, st);
-            rc |= pack_gates(e, w->att_lstm_w_ih + H, E + 2 * H, H, H, e->p_a_ih_fc, st);
-            rc |= pack_gates(e, w->att_lstm_w_ih + 2 * H, E + 2 * H, H, E, e->p_a_ih_x, st);
-            rc |= pack_gates(e, w->att_lstm_w_hh, H, H, H, e->p_a_hh, st);
-            rc |= pack_gates(e, w->lang_lstm_w_ih, 2 * H, H, H, e->p_l_ih_a, st);
-            rc |= pack_gates(e, w->lang_lstm_w_ih + H, 2 * H, H, H, e->p_l_ih_h, st);
-            rc |= pack_gates(e, w->lang_lstm_w_hh, H, H, H, e->p_l_hh, st);
-            rc |= pack(e, w->h2att_w, H, A, H, e->p_h2att, st);
+            rc |= e->pack(w->fc_embed_w, e->cfg.fc_feat_size, H, e->cfg.fc_feat_size, e->p_fc, st);
+            rc |= e->pack(w->att_embed_w, e->cfg.att_feat_size, H, e->cfg.att_feat_size, e->p_attw, st);
+            rc |= e->pack(w->ctx2att_w, H, A, H, e->p_ctx, st);
+            rc |= e->pack_gates(w->att_lstm_w_ih, E + 2 * H, H, H, e->p_a_ih_h, st);
+            rc |= e->pack_gates(w->att_lstm_w_ih + H, E + 2 * H, H, H, e->p_a_ih_fc, st);
+            rc |= e->pack_gates(w->att_lstm_w_ih + 2 * H, E + 2 * H, H, E, e->p_a_ih_x, st);
+            rc |= e->pack_gates(w->att_lstm_w_hh, H, H, H, e->p_a_hh, st);
+            rc |= e->pack_gates(w->lang_lstm_w_ih, 2 * H, H, H, e->p_l_ih_a, st);
+            rc |= e->pack_gates(w->lang_lstm_w_ih + H, 2 * H, H, H, e->p_l_ih_h, st);
+            rc |= e->pack_gates(w->lang_lstm_w_hh, H, H, H, e->p_l_hh, st);
+            rc |= e->pack(w->h2att_w, H, A, H, e->p_h2att, st);
         } else if (att2in2) {
-            rc |= pack(e, w->att_embed_w, e->cfg.att_feat_size, H, e->cfg.att_feat_size, e->p_attw, st);
-            rc |= pack(e, w->ctx2att_w, H, A, H, e->p_ctx, st);
-            rc |= pack(e, w->h2att_w, H, A, H, e->p_h2att, st);
-            rc |= pack(e, w->i2h_w, E, 5 * H, E, e->p_i2h, st);
-            rc |= pack(e, w->h2h_w, H, 5 * H, H, e->p_h2h, st);
-            rc |= pack(e, w->a2c_w, H, 2 * H, H, e->p_a2c, st);
+            rc |= e->pack(w->att_embed_w, e->cfg.att_feat_size, H, e->cfg.att_feat_size, e->p_attw, st);
+            rc |= e->pack(w->ctx2att_w, H, A, H, e->p_ctx, st);
+            rc |= e->pack(w->h2att_w, H, A, H, e->p_h2att, st);
+            rc |= e->pack(w->i2h_w, E, 5 * H, E, e->p_i2h, st);
+            rc |= e->pack(w->h2h_w, H, 5 * H, H, e->p_h2h, st);
+            rc |= e->pack(w->a2c_w, H, 2 * H, H, e->p_a2c, st);
         } else {
-            rc |= pack(e, w->fc_embed_w, e->cfg.fc_feat_size, E, e->cfg.fc_feat_size, e->p_fc, st);
-            rc |= pack(e, w->i2h_w, E, 5 * H, E, e->p_i2h, st);
-            rc |= pack(e, w->h2h_w, H, 5 * H, H, e->p_h2h, st);
+            rc |= e->pack(w->fc_embed_w, e->cfg.fc_feat_size, E, e->cfg.fc_feat_size, e->p_fc, st);
+            rc |= e->pack(w->i2h_w, E, 5 * H, E, e->p_i2h, st);
+            rc |= e->pack(w->h2h_w, H, 5 * H, H, e->p_h2h, st);
         }
         if (rc) return 1;
     }
-    if (updown) {
-        // per-token gate table: relu(embed)[V+1,E] * W_ih[:, 2H:2H+E]^T  (one GEMM per bind; replaces a K=E segment in every step)
-        const long n = (long)V1 * E;
-        const long ldE = round_up(E, 8);
-        char* tmp = nullptr;
-        const size_t tmp_bytes = (size_t)V1 * ldE * (sizeof(float) + (e->tc ? 2 * sizeof(__half) : 0)) + 1024;
-        CAPB_CHECK_CUDA(cudaMallocAsync(&tmp, tmp_bytes, st));
-        ActView ev;
-        ev.ld = ldE;
-        ev.f = reinterpret_cast<float*>(tmp);
-        if (e->tc) {
-            ev.hi = reinterpret_cast<__half*>(tmp + (size_t)V1 * ldE * sizeof(float));
-            ev.lo = ev.hi + (size_t)V1 * ldE;
-        }
-        int rc = 0;
-        if (ldE == E) {
-            rc = relu_copy_launch(w->embed, n, ev, st);
-        } else {
-            CAPB_CHECK_CUDA(cudaMemsetAsync(tmp, 0, tmp_bytes, st));
-            for (int v = 0; v < V1 && !rc; ++v) {     // ragged pitch (tiny test configs only): row by row
-                ActView rv = ev;
-                rv.f += (long)v * ldE; if (rv.hi) { rv.hi += (long)v * ldE; rv.lo += (long)v * ldE; }
-                rc = relu_copy_launch(w->embed + (long)v * E, E, rv, st);
-            }
-        }
-        GemmProblem g;
-        g.M = V1; g.N = 4 * H; g.nseg = 1;
-        g.seg[0] = seg_of(ev, w->att_lstm_w_ih + 2 * H, E + 2 * H, e->p_a_ih_x, E);
-        g.epi.C = e->xgate; g.epi.ldc = e->ld_xgate;
-        if (!rc) {
-            if (!e->tc) {
-                rc = gemm_simt_launch(g, st);
-            } else {
-                GemmTcPlan* plan = gemm_tc_plan_create(g, e->mode == CAPB200_MODE_TC_F16X3 ? 3 : 1);
-                rc = plan ? gemm_tc_plan_launch(plan, nullptr, 0, st) : 1;
-                if (plan) gemm_tc_plan_destroy(plan);
-            }
-        }
-        e->launches += 2;
-        cudaFreeAsync(tmp, st);
-        if (rc) return 1;
-    }
-    if (e->tc && !e->bound) {   // first binding: wait for the conversions and refuse weights outside the fp16 range of the split planes.
-        // Re-bindings (a training loop changes the weights every step) must not stall the host: the range flag is host-mapped and every later
-        // entry point checks it (check_ready), so an overflow introduced by an optimizer step is reported by the next call instead.
-        CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-        CAPB_CHECK_RANGE();
-    }
-    e->bound = true;
-    return 0;
-}
-
-static int decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
-                       long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream, int form) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq != nullptr, "null argument");
-    const int beam = opts->beam_size, keep = opts->sample_n;
-    CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= e->V1, "beam_size must be in 1..16 and <= V+1");
-    CAPB_REQUIRE(keep == 1 || keep == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
-    CAPB_REQUIRE(B >= 1, "empty batch");
-    const bool attn = attends(e);
-    if (attn) CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
-    if (!attn) R = 1;
-    const int T = e->T, V1 = e->V1;
-    const int rows = B * beam;
-    if (lstm_decode_workspace(e, B, rows, R, beam, 1, st)) return 1;
-    if (lstm_decode_prepare(e, fc, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return lstm_decode_core(e, nrows, live, tokens, src_row, logits, ld, B, R, mask, st);
-    };
-    // UpDown's two states can be gathered by the fused beam step (the word enters through the per-token gate table, not an embedding copy)
-    NextStateGather next;
-    const bool gather = e->cfg.family == CAPB200_FAMILY_UPDOWN && e->use_xgate;
-    if (gather) {
-        next.s0.src = e->h0_out.v.f; next.s0.ld_src = e->h0_out.v.ld; next.s0.dst = e->h0_in.v;
-        next.s1.src = e->h1_out.v.f; next.s1.ld_src = e->h1_out.v.ld; next.s1.dst = e->h1_in.v;
-        next.H = e->H;
-    }
-    return beam_decode_driver(e->d, V1, T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
-                              done_raw, core, &e->launches, st, e->profiling ? 0ull : loop_graph_key(e->ws, e->wblock, mask, R, (int)e->cfg.family),
-                              to_edits(opts->edits), opts->temperature, gather ? &next : nullptr, form);
+    // per-token gate table: relu(embed)[V+1,E] * W_ih[:, 2H:2H+E]^T
+    if (updown && build_gate_table(*e, w->embed, E, H, w->att_lstm_w_ih + 2 * H, E + 2 * H, e->p_a_ih_x, e->xgate, e->ld_xgate, st)) return 1;
+    return e->finish_bind(st);
 }
 
 int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
                         long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
-    return decode_beam(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream, 0);
+    return decode_beam(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_decode_beam_form(int form, capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R,
                              const capb200_beam_opts* opts, long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p,
                              float* done_raw, void* stream) {
-    return decode_beam(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream, form);
+    return decode_beam(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, static_cast<cudaStream_t>(stream), form);
 }
 
 int capb200_decode_beam_diverse(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
                                 long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq != nullptr, "null argument");
-    // NewFC picks its fresh-state pass (the image embedding step) per core call, not per row, so its groups cannot start at different steps
-    CAPB_REQUIRE(attends(e), "diverse beam search runs on UpDown and Att2in2 (NewFC's fresh-state pass is chosen per call, not per row)");
-    if (opts->group_size == 1) return capb200_decode_beam(e, fc, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, stream);
-    const int beam = opts->base.beam_size;
-    CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= e->V1, "beam_size must be in 2..16 and <= V+1");
-    CAPB_REQUIRE(B >= 1, "empty batch");
-    CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
-    const int rows = B * beam;
-    if (lstm_decode_workspace(e, B, rows, R, beam, 1, st)) return 1;      // attending families only: no NewFC row table
-    if (lstm_decode_prepare(e, fc, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int rpi, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return lstm_decode_core(e, nrows, rpi, tokens, src_row, logits, ld, B, R, mask, st);
-    };
-    return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
-                                      opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
-                                      e->profiling ? 0ull : loop_graph_key(e->ws, e->wblock, mask, R, (int)e->cfg.family), to_edits(opts->base.edits),
-                                      opts->base.temperature);
+    return decode_beam_diverse(e, fc, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_beam_record_logprobs(capb200_engine* e, int image, int rank, float* dst, void* stream) {
-    if (check_ready(e)) return 1;
-    return beam_record_logprobs(e->d, e->V1, e->T, image, rank, dst, static_cast<cudaStream_t>(stream));
+    return decode_record_logprobs(e, image, rank, dst, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_decode_sample(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_sample_opts* opts,
                           const long long* tokens_in, long ld_tok, long long* seq, float* seq_logprobs, float* picked, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && (fc != nullptr || e->cfg.family == CAPB200_FAMILY_ATT2IN2) && seq_logprobs != nullptr, "null argument");
-    const int n = opts->sample_n;
-    CAPB_REQUIRE(n >= 1 && B >= 1, "empty batch");
-    const bool attn = attends(e);
-    if (attn) CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
-    if (!attn) R = 1;
-    const int method = opts->method;
-    CAPB_REQUIRE(method >= 0 && method <= 5, "unknown sampling method");
-    if (method == CAPB200_SAMPLE_FORCED || method == CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(tokens_in != nullptr && ld_tok >= 1, "token matrix required");
-    if (method != CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(seq != nullptr, "seq output required");
-    if (method == CAPB200_SAMPLE_MULTINOMIAL || method >= CAPB200_SAMPLE_TOPK) CAPB_REQUIRE(opts->temperature > 0.f, "temperature must be positive");
-    const int T = e->T, V1 = e->V1;
-    const int rows = B * n;
-    const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : T;
-    const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : T;
-    CAPB_REQUIRE(steps >= 0 && steps <= t_out, "steps out of range");
-    if (lstm_decode_workspace(e, B, rows, R, 1, n, st)) return 1;
-    if (lstm_decode_prepare(e, fc, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return lstm_decode_core(e, nrows, n, tokens, src_row, logits, ld, B, R, mask, st);
-    };
-    return sample_decode_driver(e->d, V1, T, rows, method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked, core,
-                                &e->launches, st, to_edits(opts->edits), opts->top);
+    return decode_sample(e, fc, att, mask, B, R, opts, tokens_in, ld_tok, seq, seq_logprobs, picked, static_cast<cudaStream_t>(stream));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1197,7 +1029,7 @@ namespace {
 // (1) of an SCST step with the eval-mode baseline: fork it and enqueue it right away on this engine's decode path (NewFC: att = null, R = 0).
 int start_baseline(capb200_engine* e, const float* fc, const float* att, int B, int R, const TrainArgs& ta, const StepTape& tp, StepBaseline& gb,
                           cudaStream_t st) {
-    if (gb.fork(ta, &e->side, &e->ev_gfork, &e->ev_gjoin, st)) return 1;
+    if (gb.fork(ta, &e->side, &e->ev_fork, &e->ev_join, st)) return 1;
     return gb.enqueue(B, ta.T, e->V1, ta.greedy_seq, tp.glp, [&](const capb200_sample_opts* so, const long long* tok, long long* seq, float* lp, void* s) {
         return capb200_decode_sample(e, fc, att, ta.mask, B, R, so, tok, tok ? ta.T : 0, seq, lp, nullptr, s);
     });
@@ -1607,6 +1439,15 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
     return rc;
 }
 
+// the feature checks of a family's training steps: UpDown reads fc and att, Att2in2 att, NewFC fc (and has no regions)
+int check_train_feats(const capb200_engine* e, int family, const float* fc, const float* att, int R, const float* att_masks) {
+    CAPB_REQUIRE(e->cfg.family == family, "the entry point does not match the engine's family");
+    if (family != CAPB200_FAMILY_ATT2IN2) CAPB_REQUIRE(fc != nullptr, "null argument");
+    if (family == CAPB200_FAMILY_NEWFC) CAPB_REQUIRE(att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
+    else CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
+    return 0;
+}
+
 }  // namespace
 
 // The UpDown, Att2in2 and NewFC entry points take the shared option structs (capb200_scst_opts / capb200_xe_opts) with the same meaning.
@@ -1615,9 +1456,8 @@ extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, cons
                                         const capb200_updown_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
                                         float* reward, float* loss, void* stream) {
     if (check_ready(e)) return 1;
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_UPDOWN, "the SCST step is implemented for the UpDown family");
-    CAPB_REQUIRE(opts && fc && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
-    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
+    if (check_train_feats(e, CAPB200_FAMILY_UPDOWN, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     return run_scst_step(e, opts, grads, ta, fc, sizeof(float) * (size_t)B * e->cfg.fc_feat_size, att, sizeof(float) * (size_t)B * R * e->cfg.att_feat_size,
@@ -1630,9 +1470,8 @@ extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, con
                                          const capb200_att2in2_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
                                          float* reward, float* loss, void* stream) {
     if (check_ready(e)) return 1;
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_ATT2IN2, "capb200_att2in2_scst_step needs an Att2in2 engine");
-    CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
-    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
+    if (check_train_feats(e, CAPB200_FAMILY_ATT2IN2, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     // the fc features are not read (the greedy baseline's decode call ignores them): not staged
@@ -1644,9 +1483,8 @@ extern "C" int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const
                                        const long long* labels, const float* masks, int label_cols, const capb200_att2in2_grads* grads, float* logprobs,
                                        float* loss, void* stream) {
     if (check_ready(e)) return 1;
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_ATT2IN2, "capb200_att2in2_xe_step needs an Att2in2 engine");
-    CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
-    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts && labels && masks && grads && logprobs && loss, "null argument");
+    if (check_train_feats(e, CAPB200_FAMILY_ATT2IN2, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1658,10 +1496,9 @@ extern "C" int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const
                                        const capb200_newfc_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
                                        float* reward, float* loss, void* stream) {
     if (check_ready(e)) return 1;
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_NEWFC, "capb200_newfc_scst_step needs a NewFC engine");
-    CAPB_REQUIRE(opts && fc && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
+    CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
-    CAPB_REQUIRE(opts->att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
+    if (check_train_feats(e, CAPB200_FAMILY_NEWFC, fc, nullptr, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     return run_scst_step(e, opts, grads, ta, fc, sizeof(float) * (size_t)B * e->cfg.fc_feat_size, nullptr, 0, B, R, static_cast<cudaStream_t>(stream),
@@ -1672,29 +1509,23 @@ extern "C" int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const f
                                      const capb200_xe_opts* opts, const long long* labels, const float* masks, int label_cols,
                                      const capb200_newfc_grads* grads, float* logprobs, float* loss, void* stream) {
     if (check_ready(e)) return 1;
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_NEWFC, "capb200_newfc_xe_step needs a NewFC engine");
-    CAPB_REQUIRE(opts && fc && labels && masks && grads && logprobs && loss, "null argument");
+    CAPB_REQUIRE(opts && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
-    CAPB_REQUIRE(opts->att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
+    if (check_train_feats(e, CAPB200_FAMILY_NEWFC, fc, nullptr, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_eager_step(st, [&] { return newfc_train_step(e, fc, B, ta, grads, st); });
 }
 
-extern "C" int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n) {
-    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 2, "UpDown, Att2in2 and NewFC have 2 gradient groups");
-    for (int i = 0; i < 2; ++i) e->grad_events[i] = (events != nullptr && i < n) ? static_cast<cudaEvent_t>(events[i]) : nullptr;
-    return 0;
-}
+extern "C" int capb200_engine_set_grad_events(capb200_engine* e, void* const* events, int n) { return set_grad_events(e, events, n); }
 
 extern "C" int capb200_updown_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
                                       const long long* labels, const float* masks, int label_cols, const capb200_updown_grads* grads, float* logprobs,
                                       float* loss, void* stream) {
     if (check_ready(e)) return 1;
-    CAPB_REQUIRE(e->cfg.family == CAPB200_FAMILY_UPDOWN, "the XE step is implemented for the UpDown family");
-    CAPB_REQUIRE(opts && fc && att && labels && masks && grads && logprobs && loss, "null argument");
-    CAPB_REQUIRE(R >= 1, "attention features required");
+    CAPB_REQUIRE(opts && labels && masks && grads && logprobs && loss, "null argument");
+    if (check_train_feats(e, CAPB200_FAMILY_UPDOWN, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (xe_train_args(B, *opts, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1704,21 +1535,12 @@ extern "C" int capb200_updown_xe_step(capb200_engine* e, const float* fc, const 
 // ---- autograd entry points of UpDown, Att2in2 and NewFC (include/capb200.h: capb200_vjp_opts) ----------------------------------------------
 namespace {
 
-// the feature checks of a family: UpDown reads fc and att, Att2in2 att, NewFC fc (and has no regions)
-int check_vjp_feats(const capb200_engine* e, int family, const float* fc, const float* att, int R, const float* att_masks) {
-    CAPB_REQUIRE(e->cfg.family == family, "the entry point does not match the engine's family");
-    if (family != CAPB200_FAMILY_ATT2IN2) CAPB_REQUIRE(fc != nullptr, "null argument");
-    if (family == CAPB200_FAMILY_NEWFC) CAPB_REQUIRE(att_masks == nullptr, "NewFC has no region features: att_masks must be NULL");
-    else CAPB_REQUIRE(att != nullptr && R >= 1, "attention features required");
-    return 0;
-}
-
 template <class Grads, class Step>
 int xe_vjp(capb200_engine* e, int family, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const capb200_vjp_opts* vjp,
            const long long* labels, int label_cols, const Grads* grads, float* logprobs, void* stream, Step step) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && labels && logprobs && (grads || vjp->forward_only), "null argument");
-    if (check_vjp_feats(e, family, fc, att, R, opts->att_masks)) return 1;
+    if (check_train_feats(e, family, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (xe_train_args(B, *opts, labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1730,7 +1552,7 @@ int scst_vjp(capb200_engine* e, int family, const float* fc, const float* att, i
              const Grads* grads, long long* sample_seq, float* sample_logprobs, void* stream, Step step) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
-    if (check_vjp_feats(e, family, fc, att, R, opts->att_masks)) return 1;
+    if (check_train_feats(e, family, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
     if (scst_train_args(B, *opts, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -3,6 +3,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <string>
+#include <vector>
 
 #include "../../include/capb200.h"
 #include "common.cuh"
@@ -514,33 +516,6 @@ int sample_decode_driver(DecodeBuffers& d, int V1, int T, int rows, int method, 
     return 0;
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// The three pieces every eval-mode decode of the LSTM engine (engine.cu) and the AoA engine (aoa_engine.cu) is built from: workspace sizing
-// for `rows` rows, the prologue (_prepare_feature) for B images, and one application of the recurrent core.  The single-model entry points
-// and the test-time ensemble (ensemble.cu) run the same three.
-// ---------------------------------------------------------------------------------------------------------------------
-struct MemberInfo {
-    int family = 0;                  // CAPB200_FAMILY_*
-    int V1 = 0, T = 0;
-    bool attends = true;             // reads the region features (NewFC reads the fc features only)
-    bool graph_ok = true;            // false while the engine times its GEMMs (per-launch events are not captured)
-    const void* ws = nullptr;        // workspace and weight block: what captured launches of the core read
-    const void* wblock = nullptr;
-    const int* fresh = nullptr;      // the engine's all -1 parent-row table: src_row of a fresh zero state
-    long* launches = nullptr;        // the engine's launch counter
-};
-
-int lstm_member_info(capb200_engine* e, MemberInfo* m);
-int lstm_decode_workspace(capb200_engine* e, int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st);
-int lstm_decode_prepare(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, cudaStream_t st);
-int lstm_decode_core(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int B, int R,
-                     const float* mask, cudaStream_t st);
-int aoa_member_info(capb200_aoa_engine* e, MemberInfo* m);
-int aoa_decode_workspace(capb200_aoa_engine* e, int B, int rows, int R, int beam, cudaStream_t st);
-int aoa_decode_prepare(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, cudaStream_t st);
-int aoa_decode_core(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, int R,
-                    const float* mask, cudaStream_t st);
-
 // CUDA graph of a whole fused training step (see run_scst_step in train_common.cuh) + the engine-owned staging buffer that gives the graph stable input
 // addresses.  CAPB200_SCST_GRAPH=0 keeps the steps eager.
 struct StepGraph {
@@ -656,6 +631,292 @@ inline cudaError_t create_side_stream(cudaStream_t* s) {
     int least = 0, greatest = 0;
     if (cudaDeviceGetStreamPriorityRange(&least, &greatest) == cudaSuccess) return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, least);
     return cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The decode workspace of an engine or of the ensemble: one cudaMalloc'ed block holding the family's activations and the DecodeBuffers, and
+// the GEMM plans whose tensor maps are encoded on it.
+// ---------------------------------------------------------------------------------------------------------------------
+struct Workspace {
+    char* ws = nullptr;
+    size_t ws_bytes = 0;
+    int capB = 0, capRows = 0, capR = 0, capBeam = 0;     // extents the block is laid out for (the ensemble's third extent is the caption length)
+    DecodeBuffers d;
+    std::vector<GemmTcPlan*> plans;                       // per GEMM call site (tensor-core modes)
+
+    void destroy_plans() {
+        for (auto& p : plans) { if (p) gemm_tc_plan_destroy(p); p = nullptr; }
+    }
+    // Grows the block to the largest (B, rows, R, beam) seen so far, laid out by layout(arena, B, rows, R, beam) (a dry run sizes it).  Growing
+    // synchronises `st`, drops the plans, zero-fills the new block and sets d.neg1 to all -1.
+    template <class Layout>
+    int grow(int B, int rows, int R, int beam, cudaStream_t st, Layout layout) {
+        if (ws != nullptr && B <= capB && rows <= capRows && R <= capR && beam <= capBeam) return 0;
+        const int nB = B > capB ? B : capB, nRows = rows > capRows ? rows : capRows;
+        const int nR = R > capR ? R : capR, nBeam = beam > capBeam ? beam : capBeam;
+        Arena dry;
+        layout(dry, nB, nRows, nR, nBeam);
+        const size_t need = dry.off + 256;
+        CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
+        destroy_plans();
+        if (ws) CAPB_CHECK_CUDA(cudaFree(ws));
+        ws = nullptr;
+        CAPB_CHECK_CUDA(cudaMalloc(&ws, need));
+        ws_bytes = need;
+        Arena real;
+        real.base = ws;
+        layout(real, nB, nRows, nR, nBeam);
+        capB = nB; capRows = nRows; capR = nR; capBeam = nBeam;
+        CAPB_CHECK_CUDA(cudaMemsetAsync(ws, 0, need, st));
+        return fill_int_launch(d.neg1, nRows, -1, st);
+    }
+    void release() {
+        destroy_plans();
+        cudaFree(ws);
+        d.release();
+    }
+};
+
+// What a family's core reads besides its rows: the batch, the region count it runs with, their mask, and under teacher forcing the token
+// matrix (the Transformer masks its pad keys with it).
+struct DecodeCtx {
+    int B = 0, R = 0;
+    const float* mask = nullptr;
+    const long long* labels = nullptr;
+    long ld_labels = 0;
+};
+
+// ---------------------------------------------------------------------------------------------------------------------
+// What every engine owns -- capb200_engine (UpDown, Att2in2, NewFC: engine.cu), capb200_aoa_engine (aoa_engine.cu) and capb200_tfm_engine
+// (tfm_engine.cu) -- and the three hooks every eval-mode decode is built from: workspace sizing for `rows` rows, the prologue
+// (_prepare_feature) for B images, and one application of the recurrent core.  The single-model decodes below and the test-time ensemble
+// (ensemble.cu) run the same three.
+// ---------------------------------------------------------------------------------------------------------------------
+struct EngineBase : Workspace {
+    int V1 = 0, T = 0, mode = 0;
+    bool tc = false, bound = false;
+    long launches = 0;
+    const char* bind_name = "";      // the family's bind entry point, named when it has not been called
+    int family = -1;                 // CAPB200_FAMILY_* as an ensemble member declares it (-1: the Transformer, which is never one)
+    int graph_family = 0;            // the family's term of loop_graph_key
+    bool reads_fc = false;           // the decode reads the fc features (UpDown, NewFC)
+    bool reads_att = true;           // ... and the regions; a family without them runs with R = 1 (NewFC)
+    int max_teacher_steps = 1 << 30; // teacher-forced positions the core holds (the Transformer's cache: T + 1)
+
+    char* wblock = nullptr;          // bind-time buffers
+    size_t wblock_bytes = 0;
+    char* tape = nullptr;            // training tape, grown on demand
+    size_t tape_bytes = 0;
+    Tf32Context* tf32 = nullptr;     // tensor maps + transposed operands of the training GEMMs (tensor-core modes)
+    static constexpr int kMaxGradGroups = 10;
+    cudaEvent_t grad_events[kMaxGradGroups] = {};   // caller-owned: recorded when a gradient group is complete (*_set_grad_events)
+    int grad_groups = 2;             // the family's gradient groups: 2, AoANet 10
+    cudaStream_t side = nullptr;     // the SCST step's concurrent greedy baseline runs here
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    StepGraph sg;                    // CUDA graph of the whole SCST step
+
+    virtual ~EngineBase() {
+        release();
+        cudaFree(wblock);
+        cudaFree(tape);
+        sg.destroy();
+        tf32_context_destroy(tf32);
+        if (ev_fork) cudaEventDestroy(ev_fork);
+        if (ev_join) cudaEventDestroy(ev_join);
+        if (side) cudaStreamDestroy(side);
+    }
+    // rows_per_image: the rows of one image in the first core call (NewFC feeds each row its image's embedding there)
+    virtual int decode_workspace(int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) = 0;
+    virtual int decode_prepare(const float* fc, const float* att, const DecodeCtx& c, cudaStream_t st) = 0;
+    // src_row: parent row per row -- d.neg1 a fresh zero state, null the row itself (sampling from t = 1 on)
+    virtual int decode_core(int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld, const DecodeCtx& c,
+                            cudaStream_t st) = 0;
+    // the states the fused beam step may gather for the next core call (UpDown), after decode_workspace
+    virtual bool next_state(NextStateGather*) { return false; }
+    // whether the beam loop may be captured into a graph (not while the LSTM engine times its GEMMs: per-launch events are not captured)
+    virtual bool loop_graph_ok() const { return true; }
+
+    // one GEMM in the engine's numeric mode at call site `site`
+    int gemm(int site, GemmProblem& g, int plan_rows, cudaStream_t st) {
+        launches++;
+        return run_gemm_mode(mode, &plans[site], g, plan_rows, st);
+    }
+    // the split fp16 planes of a weight [rows, cols]
+    int pack(const float* w, long ldw, int rows, int cols, const Planes& p, cudaStream_t st) {
+        launches++;
+        return split_planes_launch(w, ldw, rows, cols, p.hi, p.lo, p.ld, st);
+    }
+    // LSTM weight blocks [4H, cols] are stored gate-interleaved (row 4*j+g) so the GEMM epilogue can apply the cell directly
+    int pack_gates(const float* w, long ldw, int H, int cols, const Planes& p, cudaStream_t st) {
+        launches++;
+        return split_planes_interleave_launch(w, ldw, H, cols, p.hi, p.lo, p.ld, st);
+    }
+    // the weight block, allocated and zero-filled on the first bind and laid out by layout(arena) (a dry run sizes it)
+    template <class Layout>
+    int alloc_wblock(cudaStream_t st, Layout layout) {
+        if (wblock != nullptr) return 0;
+        Arena dry;
+        layout(dry);
+        wblock_bytes = dry.off + 256;
+        CAPB_CHECK_CUDA(cudaMalloc(&wblock, wblock_bytes));
+        CAPB_CHECK_CUDA(cudaMemsetAsync(wblock, 0, wblock_bytes, st));
+        Arena real;
+        real.base = wblock;
+        layout(real);
+        return 0;
+    }
+    // The end of a bind.  The first one waits for the conversions and refuses weights outside the fp16 range of the split planes.  Re-bindings
+    // (a training loop changes the weights every step) must not stall the host: the range flag is host-mapped and every later entry point
+    // checks it (check_ready), so an overflow introduced by an optimizer step is reported by the next call instead.
+    int finish_bind(cudaStream_t st) {
+        if (tc && !bound) {
+            CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
+            CAPB_CHECK_RANGE();
+        }
+        bound = true;
+        return 0;
+    }
+};
+
+// The checks every engine's create makes after its family's own, and the engine with the shared fields set (`sites` GEMM call sites); null
+// after an error.
+template <class Engine>
+Engine* create_engine(int vocab_size, int seq_length, int numeric_mode, int sites) {
+    if (numeric_mode < 0 || numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
+    if (seq_length < 1 || seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device: the capb200 engine has no CPU fallback"); return nullptr; }
+    Engine* e = new Engine();
+    e->V1 = vocab_size + 1;
+    e->T = seq_length;
+    e->mode = numeric_mode;
+    e->tc = numeric_mode != CAPB200_MODE_SIMT_FP32;
+    e->plans.assign(sites, nullptr);
+    return e;
+}
+
+// The per-token gate table of an LSTM whose word enters through the W_ih columns `w_x` (planes p_x): relu(embed)[V+1, E] * w_x^T into
+// xgate [V+1, ld_xgate].  One GEMM per bind; it replaces a K = E segment in every decode step (engine.cu).
+int build_gate_table(EngineBase& e, const float* embed, int E, int H, const float* w_x, long ld_w, const Planes& p_x, float* xgate, long ld_xgate,
+                     cudaStream_t st);
+int add_vec_launch(const float* a, const float* b, float* o, int n, cudaStream_t st);
+int interleave_gates_launch(const float* src, float* dst, int H, cudaStream_t st);      // dst[4*j+g] = src[g*H + j]
+
+// The engine behind an ensemble member's handle (engine.cu, aoa_engine.cu)
+EngineBase* engine_base(capb200_engine* e);
+EngineBase* engine_base(capb200_aoa_engine* e);
+
+inline int check_ready(const EngineBase* e) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    CAPB_REQUIRE(e->bound, std::string(e->bind_name) + " has not been called");
+    CAPB_CHECK_RANGE();
+    return 0;
+}
+
+inline int set_grad_events(EngineBase* e, void* const* events, int n) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    CAPB_REQUIRE(n >= 0 && n <= e->grad_groups, "the engine has " + std::to_string(e->grad_groups) + " gradient groups");
+    for (int i = 0; i < e->grad_groups; ++i) e->grad_events[i] = (events != nullptr && i < n) ? static_cast<cudaEvent_t>(events[i]) : nullptr;
+    return 0;
+}
+
+// ---- the argument checks of the decode entry points (the engines' and the ensemble's) -------------------------------------------------------
+// beam_size and sample_n of a beam search; with group_size > 1 (`diverse`) the driver checks sample_n against beam_size / group_size
+inline int check_beam_opts(const capb200_beam_opts* o, int V1, const long long* seq, bool diverse = false) {
+    CAPB_REQUIRE(o != nullptr && seq != nullptr, "null argument");
+    const int beam = o->beam_size;
+    if (diverse) {
+        CAPB_REQUIRE(beam >= 2 && beam <= 16 && beam <= V1, "beam_size must be in 2..16 and <= V+1");
+        return 0;
+    }
+    CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= V1, "beam_size must be in 1..16 and <= V+1");
+    CAPB_REQUIRE(o->sample_n == 1 || o->sample_n == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
+    return 0;
+}
+
+// sampling / teacher forcing; *steps = the positions to run (T, or opts->steps under teacher forcing)
+inline int check_sample_opts(const capb200_sample_opts* o, int B, int T, int max_teacher_steps, const long long* tokens_in, long ld_tok,
+                             const long long* seq, const float* seq_logprobs, int* steps) {
+    CAPB_REQUIRE(o != nullptr && seq_logprobs != nullptr, "null argument");
+    const int method = o->method;
+    CAPB_REQUIRE(o->sample_n >= 1 && B >= 1, "empty batch");
+    CAPB_REQUIRE(method >= 0 && method <= 5, "unknown sampling method");
+    const bool teacher = method == CAPB200_SAMPLE_TEACHER;
+    if (method == CAPB200_SAMPLE_FORCED || teacher) CAPB_REQUIRE(tokens_in != nullptr && ld_tok >= 1, "token matrix required");
+    if (!teacher) CAPB_REQUIRE(seq != nullptr, "seq output required");
+    if (method == CAPB200_SAMPLE_MULTINOMIAL || method >= CAPB200_SAMPLE_TOPK) CAPB_REQUIRE(o->temperature > 0.f, "temperature must be positive");
+    *steps = teacher ? o->steps : T;
+    CAPB_REQUIRE(*steps >= 0 && *steps <= (teacher ? ld_tok : T) && *steps <= max_teacher_steps, "steps out of range");
+    return 0;
+}
+
+// the features an engine's decode reads
+inline int check_decode_feats(const EngineBase& e, const float* fc, const float* att, int B, int* R) {
+    CAPB_REQUIRE(B >= 1, "empty batch");
+    CAPB_REQUIRE(fc != nullptr || !e.reads_fc, "fc features required");
+    if (!e.reads_att) *R = 1;
+    else CAPB_REQUIRE(att != nullptr && *R >= 1, "attention features required");
+    return 0;
+}
+
+// ---- the decode entry points of every engine: the checks, the family's three hooks, the driver ----------------------------------------------
+inline unsigned long long engine_loop_key(EngineBase* e, const float* mask, int R) {
+    return e->loop_graph_ok() ? loop_graph_key(e->ws, e->wblock, mask, R, e->graph_family) : 0ull;
+}
+
+inline int decode_beam(EngineBase* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq,
+                       float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, cudaStream_t st, int form = 0) {
+    if (check_ready(e) || check_beam_opts(opts, e->V1, seq) || check_decode_feats(*e, fc, att, B, &R)) return 1;
+    const int beam = opts->beam_size;
+    const DecodeCtx c{B, R, mask};
+    if (e->decode_workspace(B, B * beam, R, beam, 1, st) || e->decode_prepare(fc, att, c, st)) return 1;
+    auto core = [&](int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld) {
+        return e->decode_core(rows, rpi, tokens, src_row, t, logits, ld, c, st);
+    };
+    NextStateGather next;
+    const bool gather = e->next_state(&next);
+    return beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->sample_n, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len,
+                              done_p, done_raw, core, &e->launches, st, engine_loop_key(e, mask, R), to_edits(opts->edits), opts->temperature,
+                              gather ? &next : nullptr, form);
+}
+
+inline int decode_beam_diverse(EngineBase* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_diverse_opts* opts,
+                               long long* seq, float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, cudaStream_t st) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts != nullptr, "null argument");
+    // NewFC picks its fresh-state pass (the image embedding step) per core call, not per row, so its groups cannot start at different steps
+    CAPB_REQUIRE(e->reads_att, "diverse beam search needs a family that attends over regions (NewFC's fresh-state pass is chosen per call, not per row)");
+    if (opts->group_size == 1) return decode_beam(e, fc, att, mask, B, R, &opts->base, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, st);
+    if (check_beam_opts(&opts->base, e->V1, seq, true) || check_decode_feats(*e, fc, att, B, &R)) return 1;
+    const int beam = opts->base.beam_size;
+    const DecodeCtx c{B, R, mask};
+    if (e->decode_workspace(B, B * beam, R, beam, 1, st) || e->decode_prepare(fc, att, c, st)) return 1;
+    auto core = [&](int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld) {
+        return e->decode_core(rows, rpi, tokens, src_row, t, logits, ld, c, st);
+    };
+    return diverse_beam_decode_driver(e->d, e->V1, e->T, B, beam, opts->group_size, opts->diversity_lambda, opts->base.sample_n, opts->base.penalty_kind,
+                                      opts->base.penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, core, &e->launches, st,
+                                      engine_loop_key(e, mask, R), to_edits(opts->base.edits), opts->base.temperature);
+}
+
+inline int decode_record_logprobs(EngineBase* e, int image, int rank, float* dst, cudaStream_t st) {
+    if (check_ready(e)) return 1;
+    return beam_record_logprobs(e->d, e->V1, e->T, image, rank, dst, st);
+}
+
+inline int decode_sample(EngineBase* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_sample_opts* opts,
+                         const long long* tokens_in, long ld_tok, long long* seq, float* seq_logprobs, float* picked, cudaStream_t st) {
+    int steps = 0;
+    if (check_ready(e) || check_sample_opts(opts, B, e->T, e->max_teacher_steps, tokens_in, ld_tok, seq, seq_logprobs, &steps) ||
+        check_decode_feats(*e, fc, att, B, &R)) return 1;
+    const int n = opts->sample_n, rows = B * n;
+    const DecodeCtx c{B, R, mask, opts->method == CAPB200_SAMPLE_TEACHER ? tokens_in : nullptr, ld_tok};
+    if (e->decode_workspace(B, rows, R, 1, n, st) || e->decode_prepare(fc, att, c, st)) return 1;
+    auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int t, float* logits, long ld) {
+        return e->decode_core(nrows, n, tokens, src_row, t, logits, ld, c, st);
+    };
+    return sample_decode_driver(e->d, e->V1, e->T, rows, opts->method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs,
+                                picked, core, &e->launches, st, to_edits(opts->edits), opts->top);
 }
 
 // Training-step GEMMs on the raw fp32 PyTorch weights (always current, no repack after optimizer steps).  With a Tf32Context (tensor-core

@@ -15,10 +15,7 @@
 
 using namespace capb200;
 
-struct capb200_ensemble {
-    char* ws = nullptr;          // the DecodeBuffers of the ensemble's searches
-    int capB = 0, capRows = 0, capBeam = 0, capT = 0;
-    DecodeBuffers d;
+struct capb200_ensemble : Workspace {      // the DecodeBuffers of the ensemble's searches
     float* mix = nullptr;        // [K, rows, V+1] member logits of one step
     size_t mix_bytes = 0;
     int V1 = 0, T = 0;           // of the last decode (capb200_ensemble_beam_record_logprobs)
@@ -84,10 +81,8 @@ int mix_launch(const float* z, long member_stride, int rows, int V1, const MixWe
 }
 
 struct Member {
-    int family = 0;
-    void* engine = nullptr;
+    EngineBase* e = nullptr;
     int R = 1;                 // region count the member runs with (1 for NewFC, which reads the fc features only)
-    MemberInfo info;
 };
 
 struct Members {
@@ -95,13 +90,6 @@ struct Members {
     int K = 0;
     MixWeights mw{};
 };
-
-bool is_aoa(const Member& m) { return m.family == CAPB200_FAMILY_AOA; }
-
-int member_info(Member& m) {
-    return is_aoa(m) ? aoa_member_info(static_cast<capb200_aoa_engine*>(m.engine), &m.info)
-                     : lstm_member_info(static_cast<capb200_engine*>(m.engine), &m.info);
-}
 
 // Everything the reference takes from models[0] or that would make the mixture meaningless is refused here, before any device work.
 int resolve(const capb200_ensemble_member* members, int K, const float* fc, const float* att, int R, Members& E) {
@@ -126,58 +114,39 @@ int resolve(const capb200_ensemble_member* members, int K, const float* fc, cons
     for (int k = 0; k < K; ++k) {
         const capb200_ensemble_member& c = members[k];
         Member& m = E.m[k];
-        m.family = c.family;
-        m.engine = c.engine;
-        if (member_info(m)) return 1;
-        CAPB_REQUIRE(m.info.family == c.family, "member family does not match its engine");
-        CAPB_REQUIRE(m.info.V1 == E.m[0].info.V1 && m.info.T == E.m[0].info.T,
-                     "every member needs the first member's vocab_size and seq_length (AttEnsemble.py:22-23)");
+        // the handle's type is the one its declared family names (include/capb200.h: capb200_ensemble_member)
+        m.e = c.family == CAPB200_FAMILY_AOA ? engine_base(static_cast<capb200_aoa_engine*>(c.engine)) : engine_base(static_cast<capb200_engine*>(c.engine));
+        if (check_ready(m.e)) return 1;
+        CAPB_REQUIRE(m.e->family == c.family, "member family does not match its engine");
+        CAPB_REQUIRE(m.e->V1 == E.m[0].e->V1 && m.e->T == E.m[0].e->T, "every member needs the first member's vocab_size and seq_length (AttEnsemble.py:22-23)");
         cudaPointerAttributes pa;
-        CAPB_CHECK_CUDA(cudaPointerGetAttributes(&pa, m.info.wblock));
+        CAPB_CHECK_CUDA(cudaPointerGetAttributes(&pa, m.e->wblock));
         CAPB_REQUIRE(pa.device == dev, "every member must live on the current device");
-        m.R = m.info.attends ? R : 1;
-        reads_att |= m.info.attends;
-        reads_fc |= c.family == CAPB200_FAMILY_UPDOWN || c.family == CAPB200_FAMILY_NEWFC;
+        m.R = m.e->reads_att ? R : 1;
+        reads_att |= m.e->reads_att;
+        reads_fc |= m.e->reads_fc;
     }
     CAPB_REQUIRE(!reads_fc || fc != nullptr, "fc features required");
     CAPB_REQUIRE(!reads_att || (att != nullptr && R >= 1), "attention features required");
     return 0;
 }
 
+// the third extent of the ensemble's workspace is the caption length
 int ensure_workspace(capb200_ensemble* s, int B, int rows, int beam, int T, cudaStream_t st) {
-    if (s->ws != nullptr && B <= s->capB && rows <= s->capRows && beam <= s->capBeam && T <= s->capT) return 0;
-    const int nB = B > s->capB ? B : s->capB, nRows = rows > s->capRows ? rows : s->capRows;
-    const int nBeam = beam > s->capBeam ? beam : s->capBeam, nT = T > s->capT ? T : s->capT;
-    Arena dry;
-    s->d.carve(dry, nB, nRows, nBeam, nT);
-    const size_t need = dry.off + 256;
-    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-    if (s->ws) CAPB_CHECK_CUDA(cudaFree(s->ws));
-    s->ws = nullptr;
-    CAPB_CHECK_CUDA(cudaMalloc(&s->ws, need));
-    Arena real;
-    real.base = s->ws;
-    s->d.carve(real, nB, nRows, nBeam, nT);
-    s->capB = nB; s->capRows = nRows; s->capBeam = nBeam; s->capT = nT;
-    CAPB_CHECK_CUDA(cudaMemsetAsync(s->ws, 0, need, st));
-    return fill_int_launch(s->d.neg1, nRows, -1, st);
+    return s->grow(B, rows, T, beam, st, [&](Arena& a, int nB, int nRows, int nT, int nBeam) { s->d.carve(a, nB, nRows, nBeam, nT); });
 }
 
 // Sizes every workspace for `rows` rows and runs each member's prologue; member launches are counted as the ensemble's.
 int setup(capb200_ensemble* s, Members& E, const float* fc, const float* att, const float* mask, int B, int rows, int beam, int rows_per_image,
           cudaStream_t st) {
-    const int V1 = E.m[0].info.V1, T = E.m[0].info.T;
+    const int V1 = E.m[0].e->V1, T = E.m[0].e->T;
     if (ensure_workspace(s, B, rows, beam, T, st)) return 1;
     if (grow_buffer(reinterpret_cast<void**>(&s->mix), &s->mix_bytes, sizeof(float) * E.K * rows * (size_t)V1, st)) return 1;
     for (int k = 0; k < E.K; ++k) {
-        Member& m = E.m[k];
-        const long l0 = *m.info.launches;
-        int rc = is_aoa(m) ? aoa_decode_workspace(static_cast<capb200_aoa_engine*>(m.engine), B, rows, m.R, beam, st)
-                           : lstm_decode_workspace(static_cast<capb200_engine*>(m.engine), B, rows, m.R, beam, rows_per_image, st);
-        if (!rc) rc = member_info(m);        // the workspace (and its fresh-state table) may have moved
-        if (!rc) rc = is_aoa(m) ? aoa_decode_prepare(static_cast<capb200_aoa_engine*>(m.engine), att, mask, B, m.R, st)
-                                : lstm_decode_prepare(static_cast<capb200_engine*>(m.engine), fc, att, mask, B, m.R, st);
-        s->launches += *m.info.launches - l0;
+        EngineBase* e = E.m[k].e;
+        const long l0 = e->launches;
+        const int rc = e->decode_workspace(B, rows, E.m[k].R, beam, rows_per_image, st) || e->decode_prepare(fc, att, {B, E.m[k].R, mask}, st);
+        s->launches += e->launches - l0;
         if (rc) return 1;
     }
     return 0;
@@ -185,18 +154,15 @@ int setup(capb200_ensemble* s, Members& E, const float* fc, const float* att, co
 
 // One ensemble step on `rows` rows: every member's core into its slice of s->mix, then the mixture into `logits`.  A fresh state (the
 // drivers pass their own all -1 table) is handed to each member as that member's fresh-state table: NewFC recognises it by address.
-int step(capb200_ensemble* s, Members& E, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld, long member_stride, int B,
-         const float* mask, cudaStream_t st) {
-    const int V1 = E.m[0].info.V1;
+int step(capb200_ensemble* s, Members& E, int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld, long member_stride,
+         int B, const float* mask, cudaStream_t st) {
+    const int V1 = E.m[0].e->V1;
     const bool fresh = src_row == s->d.neg1;
     for (int k = 0; k < E.K; ++k) {
-        Member& m = E.m[k];
-        const long l0 = *m.info.launches;
-        const int* src = fresh ? m.info.fresh : src_row;
-        float* zk = s->mix + k * member_stride;
-        const int rc = is_aoa(m) ? aoa_decode_core(static_cast<capb200_aoa_engine*>(m.engine), rows, rpi, tokens, src, zk, V1, m.R, mask, st)
-                                 : lstm_decode_core(static_cast<capb200_engine*>(m.engine), rows, rpi, tokens, src, zk, V1, B, m.R, mask, st);
-        s->launches += *m.info.launches - l0;
+        EngineBase* e = E.m[k].e;
+        const long l0 = e->launches;
+        const int rc = e->decode_core(rows, rpi, tokens, fresh ? e->d.neg1 : src_row, t, s->mix + k * member_stride, V1, {B, E.m[k].R, mask}, st);
+        s->launches += e->launches - l0;
         if (rc) return 1;
     }
     s->launches++;
@@ -211,10 +177,10 @@ unsigned long long graph_key(const capb200_ensemble* s, const Members& E, const 
     mix(reinterpret_cast<uintptr_t>(s->ws)); mix(reinterpret_cast<uintptr_t>(s->mix)); mix((unsigned long long)E.K);
     for (int k = 0; k < E.K; ++k) {
         const Member& m = E.m[k];
-        if (!m.info.graph_ok) return 0;
+        if (!m.e->loop_graph_ok()) return 0;
         unsigned bits = 0;
         memcpy(&bits, &E.mw.w[k], sizeof(float));
-        mix(loop_graph_key(m.info.ws, m.info.wblock, mask, m.R, m.family));
+        mix(loop_graph_key(m.e->ws, m.e->wblock, mask, m.R, m.e->family));
         mix((unsigned long long)bits);
     }
     return h | 1ull;
@@ -230,8 +196,7 @@ capb200_ensemble* capb200_ensemble_create(void) { return new capb200_ensemble();
 void capb200_ensemble_destroy(capb200_ensemble* s) {
     if (s == nullptr) return;
     if (s->ws != nullptr || s->mix != nullptr) {         // nothing to release on the device if it never decoded
-        s->d.release();
-        cudaFree(s->ws);
+        s->release();
         cudaFree(s->mix);
     }
     delete s;
@@ -242,21 +207,20 @@ long capb200_ensemble_launch_count(const capb200_ensemble* s) { return s ? s->la
 int capb200_ensemble_decode_beam(capb200_ensemble* s, const capb200_ensemble_member* members, int K, const float* fc, const float* att,
                                  const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq, float* seq_logprobs,
                                  long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
-    CAPB_REQUIRE(s != nullptr && opts != nullptr && seq != nullptr, "null argument");
+    CAPB_REQUIRE(s != nullptr, "null argument");
     Members E;
     if (resolve(members, K, fc, att, R, E)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int V1 = E.m[0].info.V1, T = E.m[0].info.T;
-    const int beam = opts->beam_size, keep = opts->sample_n;
-    CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= V1, "beam_size must be in 1..16 and <= V+1");
-    CAPB_REQUIRE(keep == 1 || keep == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
+    const int V1 = E.m[0].e->V1, T = E.m[0].e->T;
+    if (check_beam_opts(opts, V1, seq)) return 1;
     CAPB_REQUIRE(B >= 1, "empty batch");
+    const int beam = opts->beam_size, keep = opts->sample_n;
     const int rows = B * beam;
     if (setup(s, E, fc, att, mask, B, rows, beam, 1, st)) return 1;
     s->V1 = V1; s->T = T;
     const long stride = (long)rows * V1;
-    auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return step(s, E, nrows, live, tokens, src_row, logits, ld, stride, B, mask, st);
+    auto core = [&](int nrows, int live, const int* tokens, const int* src_row, int t, float* logits, long ld) {
+        return step(s, E, nrows, live, tokens, src_row, t, logits, ld, stride, B, mask, st);
     };
     return beam_decode_driver(s->d, V1, T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
                               done_raw, core, &s->launches, st, graph_key(s, E, mask), to_edits(opts->edits), opts->temperature);
@@ -270,27 +234,20 @@ int capb200_ensemble_beam_record_logprobs(capb200_ensemble* s, int image, int ra
 int capb200_ensemble_decode_sample(capb200_ensemble* s, const capb200_ensemble_member* members, int K, const float* fc, const float* att,
                                    const float* mask, int B, int R, const capb200_sample_opts* opts, const long long* tokens_in, long ld_tok,
                                    long long* seq, float* seq_logprobs, float* picked, void* stream) {
-    CAPB_REQUIRE(s != nullptr && opts != nullptr && seq_logprobs != nullptr, "null argument");
+    CAPB_REQUIRE(s != nullptr, "null argument");
     Members E;
     if (resolve(members, K, fc, att, R, E)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int V1 = E.m[0].info.V1, T = E.m[0].info.T;
-    const int n = opts->sample_n, method = opts->method;
-    CAPB_REQUIRE(n >= 1 && B >= 1, "empty batch");
-    CAPB_REQUIRE(method >= 0 && method <= 5, "unknown sampling method");
-    if (method == CAPB200_SAMPLE_FORCED || method == CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(tokens_in != nullptr && ld_tok >= 1, "token matrix required");
-    if (method != CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(seq != nullptr, "seq output required");
-    if (method == CAPB200_SAMPLE_MULTINOMIAL || method >= CAPB200_SAMPLE_TOPK) CAPB_REQUIRE(opts->temperature > 0.f, "temperature must be positive");
-    const int rows = B * n;
-    const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : T;
-    const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : T;
-    CAPB_REQUIRE(steps >= 0 && steps <= t_out, "steps out of range");
+    const int V1 = E.m[0].e->V1, T = E.m[0].e->T;
+    int steps = 0;
+    if (check_sample_opts(opts, B, T, 1 << 30, tokens_in, ld_tok, seq, seq_logprobs, &steps)) return 1;
+    const int n = opts->sample_n, rows = B * n;
     if (setup(s, E, fc, att, mask, B, rows, 1, n, st)) return 1;
     const long stride = (long)rows * V1;
-    auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int /*t*/, float* logits, long ld) {
-        return step(s, E, nrows, n, tokens, src_row, logits, ld, stride, B, mask, st);
+    auto core = [&](int nrows, int /*live*/, const int* tokens, const int* src_row, int t, float* logits, long ld) {
+        return step(s, E, nrows, n, tokens, src_row, t, logits, ld, stride, B, mask, st);
     };
-    return sample_decode_driver(s->d, V1, T, rows, method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked, core,
+    return sample_decode_driver(s->d, V1, T, rows, opts->method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked, core,
                                 &s->launches, st, to_edits(opts->edits), opts->top);
 }
 

@@ -20,15 +20,12 @@ namespace capb200 {
 const char* last_error_cstr();
 }
 
-struct capb200_tfm_engine {
+struct capb200_tfm_engine : EngineBase {
     capb200_tfm_cfg cfg{};
     capb200_tfm_weights w{};
-    int V1 = 0, D = 0, Dff = 0, H = 0, dk = 0, NE = 0, ND = 0, F = 0, T = 0, mode = 0;
-    bool tc = false, bound = false;
-    long launches = 0;
+    int D = 0, Dff = 0, H = 0, dk = 0, NE = 0, ND = 0, F = 0;
 
-    // bind-time (owned): concatenated projections and their split planes
-    char* wblock = nullptr;
+    // bind-time (in the weight block): concatenated projections and their split planes
     float *enc_qkv_w[CAPB200_TFM_MAX_LAYERS] = {}, *enc_qkv_b[CAPB200_TFM_MAX_LAYERS] = {};
     float *dec_qkv_w[CAPB200_TFM_MAX_LAYERS] = {}, *dec_qkv_b[CAPB200_TFM_MAX_LAYERS] = {};
     float *dec_skv_w[CAPB200_TFM_MAX_LAYERS] = {}, *dec_skv_b[CAPB200_TFM_MAX_LAYERS] = {};
@@ -37,41 +34,23 @@ struct capb200_tfm_engine {
     Planes pd_qkv[CAPB200_TFM_MAX_LAYERS], pd_o[CAPB200_TFM_MAX_LAYERS], pd_qs[CAPB200_TFM_MAX_LAYERS], pd_skv[CAPB200_TFM_MAX_LAYERS],
         pd_os[CAPB200_TFM_MAX_LAYERS], pd_w1[CAPB200_TFM_MAX_LAYERS], pd_w2[CAPB200_TFM_MAX_LAYERS];
 
-    // workspace (owned)
-    char* ws = nullptr;
-    int capB = 0, capRows = 0, capR = 0, capBeam = 0;
+    // workspace
     Planes in_att;
     Act ex, eln, eqkv, eatt, eh, mem;            // encoder activations [B*R, .]
     float* skv[CAPB200_TFM_MAX_LAYERS] = {};     // per decoder layer [B*R, 2D]: K | V of the memory
     Act x, ln, qkv, att, qs, hh;                 // decoder activations [rows, .]
     float *kc[CAPB200_TFM_MAX_LAYERS] = {}, *vc[CAPB200_TFM_MAX_LAYERS] = {};   // [T][rows][D]
     long cache_step_stride = 0;
-    DecodeBuffers d;
-    std::vector<GemmTcPlan*> plans;
 
-    // training steps (capb200_tfm_xe_step / capb200_tfm_scst_step)
-    char* tape = nullptr;
-    size_t tape_bytes = 0;
-    Tf32Context* tf32 = nullptr;
-    cudaEvent_t grad_events[2] = {};
-    cudaStream_t side = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    StepGraph sg;                       // CUDA graph of the whole SCST step (engine_common.cuh)
+    int decode_workspace(int B, int rows, int R, int beam, int rows_per_image, cudaStream_t st) override;
+    int decode_prepare(const float* fc, const float* att, const DecodeCtx& c, cudaStream_t st) override;
+    int decode_core(int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld, const DecodeCtx& c, cudaStream_t st) override;
 };
 
 namespace {
 
 enum Site { S_ATT = 0, S_GEN = 1, S_ENC = 2 /* + 4*l: qkv,o,w1,w2 */, S_SKV = 2 + 4 * CAPB200_TFM_MAX_LAYERS /* + l */,
             S_DEC = S_SKV + CAPB200_TFM_MAX_LAYERS /* + 6*l: qkv,o,qs,os,w1,w2 */, S_COUNT = S_DEC + 6 * CAPB200_TFM_MAX_LAYERS };
-
-void destroy_plans(capb200_tfm_engine* e) {
-    for (auto& p : e->plans) { if (p) gemm_tc_plan_destroy(p); p = nullptr; }
-}
-
-int gemm(capb200_tfm_engine* e, int site, GemmProblem& g, int plan_rows, cudaStream_t st) {
-    e->launches++;
-    return run_gemm_mode(e->mode, &e->plans[site], g, plan_rows, st);
-}
 
 // y = f32_view(x * W^T + b) (+ residual); x given as an ActView, W as fp32 pointer + planes
 int linear(capb200_tfm_engine* e, int site, const ActView& x, int M, int K, const float* w, const Planes& wp, const float* b, int N, ActView out,
@@ -82,7 +61,7 @@ int linear(capb200_tfm_engine* e, int site, const ActView& x, int M, int K, cons
     g.epi.bias = b; g.epi.relu = relu ? 1 : 0;
     g.epi.residual = residual; g.epi.ld_res = ld_res;
     g.epi.C = out.f; g.epi.ldc = out.ld; g.epi.C_hi = out.hi; g.epi.C_lo = out.lo; g.epi.ldcs = out.ld;
-    return gemm(e, site, g, plan_rows, st);
+    return e->gemm(site, g, plan_rows, st);
 }
 
 void layout_weights(capb200_tfm_engine* e, Arena& a) {
@@ -133,29 +112,11 @@ void layout_workspace(capb200_tfm_engine* e, Arena& a, int B, int rows, int R, i
 }
 
 int ensure_workspace(capb200_tfm_engine* e, int B, int rows, int R, int beam, cudaStream_t st) {
-    if (B <= e->capB && rows <= e->capRows && R <= e->capR && beam <= e->capBeam && e->ws != nullptr) return 0;
-    const int nB = B > e->capB ? B : e->capB, nRows = rows > e->capRows ? rows : e->capRows;
-    const int nR = R > e->capR ? R : e->capR, nBeam = beam > e->capBeam ? beam : e->capBeam;
-    Arena dry;
-    layout_workspace(e, dry, nB, nRows, nR, nBeam);
-    const size_t need = dry.off + 256;
-    CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-    destroy_plans(e);
-    if (e->ws) CAPB_CHECK_CUDA(cudaFree(e->ws));
-    e->ws = nullptr;
-    CAPB_CHECK_CUDA(cudaMalloc(&e->ws, need));
-    Arena real;
-    real.base = e->ws;
-    layout_workspace(e, real, nB, nRows, nR, nBeam);
-    e->capB = nB; e->capRows = nRows; e->capR = nR; e->capBeam = nBeam;
-    CAPB_CHECK_CUDA(cudaMemsetAsync(e->ws, 0, need, st));
-    return fill_int_launch(e->d.neg1, nRows, -1, st);
+    return e->grow(B, rows, R, beam, st, [&](Arena& a, int nB, int nRows, int nR, int nBeam) { layout_workspace(e, a, nB, nRows, nR, nBeam); });
 }
 
-int pack(capb200_tfm_engine* e, const float* w, int rows, int cols, const Planes& p, cudaStream_t st) {
-    e->launches++;
-    return split_planes_launch(w, cols, rows, cols, p.hi, p.lo, p.ld, st);
-}
+// the split planes of a contiguous weight [rows, cols]
+int pack(capb200_tfm_engine* e, const float* w, int rows, int cols, const Planes& p, cudaStream_t st) { return e->pack(w, cols, rows, cols, p, st); }
 
 int concat_rows(float* dst, const float* a, const float* b, const float* c, long n_each, cudaStream_t st) {
     CAPB_CHECK_CUDA(cudaMemcpyAsync(dst, a, sizeof(float) * n_each, cudaMemcpyDeviceToDevice, st));
@@ -182,7 +143,7 @@ int prepare(capb200_tfm_engine* e, const float* att, const float* mask, int B, i
         g.seg[0].lda_h = e->in_att.ld;
         g.epi.bias = w.att_embed_b; g.epi.relu = 1;
         g.epi.C = e->ex.v.f; g.epi.ldc = e->ex.v.ld;
-        if (gemm(e, S_ATT, g, capBR, st)) return 1;
+        if (e->gemm(S_ATT, g, capBR, st)) return 1;
     }
     if (mask != nullptr) { e->launches++; if (mask_rows_launch(e->ex.v, B, R, D, mask, R, st)) return 1; }
     for (int l = 0; l < e->NE; ++l) {
@@ -243,14 +204,23 @@ int core_step(capb200_tfm_engine* e, int rows, int rpi, const int* tokens, const
     return linear(e, S_GEN, e->ln.v, rows, D, w.gen_w, e->p_gen, w.gen_b, e->V1, lo, false, nullptr, 0, capRows, st);
 }
 
-int check_ready(capb200_tfm_engine* e) {
-    CAPB_REQUIRE(e != nullptr, "null engine");
-    CAPB_REQUIRE(e->bound, "capb200_tfm_bind_weights has not been called");
-    CAPB_CHECK_RANGE();
-    return 0;
+}  // namespace
+
+int capb200_tfm_engine::decode_workspace(int B, int rows, int R, int beam, int /*rows_per_image*/, cudaStream_t st) {
+    return ensure_workspace(this, B, rows, R, beam, st);
 }
 
-}  // namespace
+int capb200_tfm_engine::decode_prepare(const float* /*fc*/, const float* att, const DecodeCtx& c, cudaStream_t st) {
+    return prepare(this, att, c.mask, c.B, c.R, st);
+}
+
+// Beam search hands over parent rows from t = 1 on: a beam row then reads its ancestors' cache entries through the search history.  Sampling
+// rows read their own; teacher forcing masks the pad keys with the labels.
+int capb200_tfm_engine::decode_core(int rows, int rpi, const int* tokens, const int* src_row, int t, float* logits, long ld, const DecodeCtx& c,
+                                    cudaStream_t st) {
+    const int* anc = (t > 0 && src_row != nullptr) ? beam_ancestors(d.bs, t) : nullptr;
+    return core_step(this, rows, rpi, tokens, anc, c.labels, c.ld_labels, t, logits, ld, c.R, c.mask, st);
+}
 
 extern "C" {
 
@@ -258,33 +228,18 @@ capb200_tfm_engine* capb200_tfm_create(const capb200_tfm_cfg* c) {
     if (c == nullptr) { set_error("null cfg"); return nullptr; }
     if (c->n_enc < 0 || c->n_enc > CAPB200_TFM_MAX_LAYERS || c->n_dec < 1 || c->n_dec > CAPB200_TFM_MAX_LAYERS) { set_error("layer count must be within 1..8"); return nullptr; }
     if (c->heads < 1 || c->d_model % c->heads != 0) { set_error("d_model must be divisible by the head count"); return nullptr; }
-    if (c->numeric_mode < 0 || c->numeric_mode > 2) { set_error("unknown numeric mode"); return nullptr; }
-    if (c->seq_length < 1 || c->seq_length > CAPB200_MAX_SEQ_LENGTH) { set_error("seq_length must be in 1..256 (CAPB200_MAX_SEQ_LENGTH)"); return nullptr; }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_error("no CUDA device: the capb200 engine has no CPU fallback"); return nullptr; }
-    capb200_tfm_engine* e = new capb200_tfm_engine();
+    capb200_tfm_engine* e = create_engine<capb200_tfm_engine>(c->vocab_size, c->seq_length, c->numeric_mode, S_COUNT);
+    if (e == nullptr) return nullptr;
     e->cfg = *c;
-    e->V1 = c->vocab_size + 1; e->D = c->d_model; e->Dff = c->d_ff; e->H = c->heads; e->dk = c->d_model / c->heads;
-    e->NE = c->n_enc; e->ND = c->n_dec; e->F = c->att_feat_size; e->T = c->seq_length; e->mode = c->numeric_mode;
-    e->tc = c->numeric_mode != CAPB200_MODE_SIMT_FP32;
-    e->plans.assign(S_COUNT, nullptr);
+    e->D = c->d_model; e->Dff = c->d_ff; e->H = c->heads; e->dk = c->d_model / c->heads;
+    e->NE = c->n_enc; e->ND = c->n_dec; e->F = c->att_feat_size;
+    e->bind_name = "capb200_tfm_bind_weights";
+    e->graph_family = 7;
+    e->max_teacher_steps = e->T + 1;      // the K/V cache holds bos + T labels
     return e;
 }
 
-void capb200_tfm_destroy(capb200_tfm_engine* e) {
-    if (e == nullptr) return;
-    destroy_plans(e);
-    cudaFree(e->wblock);
-    cudaFree(e->ws);
-    cudaFree(e->tape);
-    e->sg.destroy();
-    tf32_context_destroy(e->tf32);
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->side) cudaStreamDestroy(e->side);
-    e->d.release();
-    delete e;
-}
+void capb200_tfm_destroy(capb200_tfm_engine* e) { delete e; }
 
 long capb200_tfm_launch_count(const capb200_tfm_engine* e) { return e ? e->launches : 0; }
 
@@ -294,14 +249,7 @@ int capb200_tfm_bind_weights(capb200_tfm_engine* e, const capb200_tfm_weights* w
     CAPB_REQUIRE(w->att_embed_w && w->att_embed_b && w->lut && w->pe && w->gen_w && w->gen_b && w->dec_norm_a && w->dec_norm_b, "missing weights");
     e->w = *w;
     const int D = e->D, Dff = e->Dff;
-    if (e->wblock == nullptr) {
-        Arena dry;
-        layout_weights(e, dry);
-        CAPB_CHECK_CUDA(cudaMalloc(&e->wblock, dry.off + 256));
-        Arena real;
-        real.base = e->wblock;
-        layout_weights(e, real);
-    }
+    if (e->alloc_wblock(st, [&](Arena& a) { layout_weights(e, a); })) return 1;
     const long dd = (long)D * D;
     for (int l = 0; l < e->NE; ++l) {
         const capb200_mha_weights& a = w->enc[l].self_attn;
@@ -326,60 +274,22 @@ int capb200_tfm_bind_weights(capb200_tfm_engine* e, const capb200_tfm_weights* w
             rc |= pack(e, w->dec[l].w1_w, Dff, D, e->pd_w1[l], st) | pack(e, w->dec[l].w2_w, D, Dff, e->pd_w2[l], st);
         }
         if (rc) return 1;
-        if (!e->bound) {        // first binding only: a re-binding must not stall the training loop (see capb200_engine_bind_weights)
-            CAPB_CHECK_CUDA(cudaStreamSynchronize(st));
-            CAPB_CHECK_RANGE();
-        }
     }
-    e->bound = true;
-    return 0;
+    return e->finish_bind(st);
 }
 
 int capb200_tfm_decode_beam(capb200_tfm_engine* e, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq,
                             float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && att != nullptr && seq != nullptr && B >= 1 && R >= 1, "bad argument");
-    const int beam = opts->beam_size, keep = opts->sample_n;
-    CAPB_REQUIRE(beam >= 1 && beam <= 16 && beam <= e->V1, "beam_size must be in 1..16 and <= V+1");
-    CAPB_REQUIRE(keep == 1 || keep == beam, "sample_n must be 1 or beam_size (AttModel.py:223)");
-    if (ensure_workspace(e, B, B * beam, R, beam, st)) return 1;
-    if (prepare(e, att, mask, B, R, st)) return 1;
-    auto core = [&](int nrows, int live, const int* tokens, const int* /*src_row*/, int t, float* logits, long ld) {
-        const int* anc = (t == 0) ? nullptr : beam_ancestors(e->d.bs, t);
-        return core_step(e, nrows, live, tokens, anc, nullptr, 0, t, logits, ld, R, mask, st);
-    };
-    return beam_decode_driver(e->d, e->V1, e->T, B, beam, keep, opts->penalty_kind, opts->penalty_alpha, seq, seq_logprobs, done_seq, done_len, done_p,
-                              done_raw, core, &e->launches, st, loop_graph_key(e->ws, e->wblock, mask, R, 7), to_edits(opts->edits), opts->temperature);
+    return decode_beam(e, nullptr, att, mask, B, R, opts, seq, seq_logprobs, done_seq, done_len, done_p, done_raw, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_tfm_beam_record_logprobs(capb200_tfm_engine* e, int image, int rank, float* dst, void* stream) {
-    if (check_ready(e)) return 1;
-    return beam_record_logprobs(e->d, e->V1, e->T, image, rank, dst, static_cast<cudaStream_t>(stream));
+    return decode_record_logprobs(e, image, rank, dst, static_cast<cudaStream_t>(stream));
 }
 
 int capb200_tfm_decode_sample(capb200_tfm_engine* e, const float* att, const float* mask, int B, int R, const capb200_sample_opts* opts,
                               const long long* tokens_in, long ld_tok, long long* seq, float* seq_logprobs, float* picked, void* stream) {
-    if (check_ready(e)) return 1;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CAPB_REQUIRE(opts != nullptr && att != nullptr && seq_logprobs != nullptr && B >= 1 && R >= 1, "bad argument");
-    const int n = opts->sample_n, method = opts->method;
-    CAPB_REQUIRE(n >= 1 && method >= 0 && method <= 5, "bad sampling options");
-    if (method == CAPB200_SAMPLE_FORCED || method == CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(tokens_in != nullptr && ld_tok >= 1, "token matrix required");
-    if (method != CAPB200_SAMPLE_TEACHER) CAPB_REQUIRE(seq != nullptr, "seq output required");
-    if (method == CAPB200_SAMPLE_MULTINOMIAL) CAPB_REQUIRE(opts->temperature > 0.f, "temperature must be positive");
-    const int rows = B * n;
-    const int steps = (method == CAPB200_SAMPLE_TEACHER) ? opts->steps : e->T;
-    const long t_out = (method == CAPB200_SAMPLE_TEACHER) ? ld_tok : e->T;
-    CAPB_REQUIRE(steps >= 0 && steps <= t_out && steps <= e->T + 1, "steps out of range");
-    if (ensure_workspace(e, B, rows, R, 1, st)) return 1;
-    if (prepare(e, att, mask, B, R, st)) return 1;
-    const long long* labels = (method == CAPB200_SAMPLE_TEACHER) ? tokens_in : nullptr;
-    auto core = [&](int nrows, int /*live*/, const int* tokens, const int* /*src_row*/, int t, float* logits, long ld) {
-        return core_step(e, nrows, n, tokens, nullptr, labels, ld_tok, t, logits, ld, R, mask, st);
-    };
-    return sample_decode_driver(e->d, e->V1, e->T, rows, method, opts->temperature, opts->seed, steps, tokens_in, ld_tok, seq, seq_logprobs, picked,
-                                core, &e->launches, st, to_edits(opts->edits), opts->top);
+    return decode_sample(e, nullptr, att, mask, B, R, opts, tokens_in, ld_tok, seq, seq_logprobs, picked, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
@@ -453,6 +363,24 @@ void layout_ttape(TTape& tp, Arena& a, int B, int R, int N, int T, int D, int Df
 struct TfmTrainArgs : TrainArgs {
     float p_lm = 0.f;
 };
+
+// att_embed's rate (drop_prob_lm of capb200_tfm_xe_opts / capb200_tfm_scst_opts), checked, into `ta`
+template <class Opts>
+int tfm_rates(const Opts& o, TfmTrainArgs* ta) {
+    CAPB_REQUIRE(o.drop_prob_lm >= 0.f && o.drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
+    ta->p_lm = o.drop_prob_lm;
+    return 0;
+}
+
+// the Transformer's options as the shared option structs (p = its `dropout`); XE evaluates every position (one pass over label_cols - 1
+// positions) and has no scheduled sampling
+capb200_scst_opts shared_opts(const capb200_tfm_scst_opts& o) {
+    return {o.sample_n, o.temperature, o.seed, o.dropout, o.upstream, o.baseline, o.forced_tokens, o.att_masks, o.keep_rows, o.row_loss, o.sampler,
+            o.reward_weights};
+}
+capb200_xe_opts shared_opts(const capb200_tfm_xe_opts& o, int label_cols) {
+    return {o.seq_per_img, label_cols - 1, o.seed, o.dropout, o.label_smoothing, o.upstream, o.att_masks, 0.f, nullptr, o.keep_rows, o.row_loss};
+}
 
 int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const TfmTrainArgs& ta, const capb200_tfm_grads* grads, cudaStream_t st) {
     const int n = ta.n, N = B * n, T = ta.T, D = e->D, Dff = e->Dff, V1 = e->V1, F = e->F, heads = e->H, dk = e->dk, NE = e->NE, ND = e->ND;
@@ -666,24 +594,15 @@ int tfm_train_step(capb200_tfm_engine* e, const float* att, int B, int R, const 
 
 }  // namespace
 
-extern "C" int capb200_tfm_set_grad_events(capb200_tfm_engine* e, void* const* events, int n) {
-    CAPB_REQUIRE(e != nullptr && n >= 0 && n <= 2, "the transformer has 2 gradient groups");
-    for (int i = 0; i < 2; ++i) e->grad_events[i] = (events != nullptr && i < n) ? static_cast<cudaEvent_t>(events[i]) : nullptr;
-    return 0;
-}
+extern "C" int capb200_tfm_set_grad_events(capb200_tfm_engine* e, void* const* events, int n) { return set_grad_events(e, events, n); }
 
 extern "C" int capb200_tfm_xe_step(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_xe_opts* opts, const long long* labels,
                                    const float* masks, int label_cols, const capb200_tfm_grads* grads, float* logprobs, float* loss, void* stream) {
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
-    // every position is evaluated (one pass over label_cols - 1 positions), no scheduled sampling
-    const capb200_xe_opts shared = {opts->seq_per_img, label_cols - 1, opts->seed, opts->dropout, opts->label_smoothing, opts->upstream,
-                                    opts->att_masks, 0.f, nullptr, opts->keep_rows, opts->row_loss};
     TfmTrainArgs ta;
-    if (xe_train_args(B, shared, labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
-    ta.p_lm = opts->drop_prob_lm;
+    if (tfm_rates(*opts, &ta) || xe_train_args(B, shared_opts(*opts, label_cols), labels, masks, label_cols, logprobs, loss, e->T, &ta)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_eager_step(st, [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
 }
@@ -694,12 +613,9 @@ extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, in
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, opts->reward_weights};
     TfmTrainArgs ta;
-    if (scst_train_args(B, shared, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
-    ta.p_lm = opts->drop_prob_lm;
+    if (tfm_rates(*opts, &ta) ||
+        scst_train_args(B, shared_opts(*opts), table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     return run_scst_step(e, opts, grads, ta, nullptr, 0, att, sizeof(float) * (size_t)B * R * e->F, B, R, static_cast<cudaStream_t>(stream),
                          [&](const float*, const float* att_s, const TfmTrainArgs& t, cudaStream_t s) { return tfm_train_step(e, att_s, B, R, t, grads, s); });
 }
@@ -710,12 +626,8 @@ extern "C" int capb200_tfm_xe_vjp(capb200_tfm_engine* e, const float* att, int B
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && att && labels && logprobs && (grads || vjp->forward_only), "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_xe_opts shared = {opts->seq_per_img, label_cols - 1, opts->seed, opts->dropout, opts->label_smoothing, opts->upstream,
-                                    opts->att_masks, 0.f, nullptr, opts->keep_rows, opts->row_loss};
     TfmTrainArgs ta;
-    if (xe_train_args(B, shared, labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
-    ta.p_lm = opts->drop_prob_lm;
+    if (tfm_rates(*opts, &ta) || xe_train_args(B, shared_opts(*opts, label_cols), labels, nullptr, label_cols, logprobs, nullptr, e->T, &ta, vjp)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_vjp_step(e, st, [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
 }
@@ -725,12 +637,11 @@ extern "C" int capb200_tfm_scst_vjp(capb200_tfm_engine* e, const float* att, int
     if (check_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && att && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
-    CAPB_REQUIRE(opts->drop_prob_lm >= 0.f && opts->drop_prob_lm < 1.f, "dropout rates must be in [0, 1)");
-    const capb200_scst_opts shared = {opts->sample_n, opts->temperature, opts->seed, opts->dropout, opts->upstream, opts->baseline,
-                                      opts->forced_tokens, opts->att_masks, opts->keep_rows, opts->row_loss, opts->sampler, nullptr};
+    capb200_scst_opts shared = shared_opts(*opts);
+    shared.reward_weights = nullptr;     // no reward runs under the autograd entry points
     TfmTrainArgs ta;
-    if (scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
-    ta.p_lm = opts->drop_prob_lm;
+    if (tfm_rates(*opts, &ta) ||
+        scst_train_args(B, shared, nullptr, nullptr, nullptr, 0, sample_seq, nullptr, sample_logprobs, nullptr, nullptr, e->T, &ta, vjp)) return 1;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return run_vjp_step(e, st, [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
 }

@@ -341,13 +341,12 @@ int run_eager_step(cudaStream_t st, Step step) {
 
 // A step of an autograd entry point (capb200_*_vjp): eager, and with the engine's gradient-group events unset -- its gradients go to the
 // caller's own table, which no data-parallel listener waits on.
-template <class Engine, class Step>
-int run_vjp_step(Engine* e, cudaStream_t st, Step step) {
-    constexpr int n = sizeof(e->grad_events) / sizeof(e->grad_events[0]);
-    cudaEvent_t saved[n];
-    for (int i = 0; i < n; ++i) { saved[i] = e->grad_events[i]; e->grad_events[i] = nullptr; }
+template <class Step>
+int run_vjp_step(EngineBase* e, cudaStream_t st, Step step) {
+    cudaEvent_t saved[EngineBase::kMaxGradGroups];
+    for (int i = 0; i < e->grad_groups; ++i) { saved[i] = e->grad_events[i]; e->grad_events[i] = nullptr; }
     const int rc = run_eager_step(st, step);
-    for (int i = 0; i < n; ++i) e->grad_events[i] = saved[i];
+    for (int i = 0; i < e->grad_groups; ++i) e->grad_events[i] = saved[i];
     return rc;
 }
 
@@ -390,7 +389,7 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
     StepGraph::mix(key, methods, sizeof(methods)); StepGraph::mix(key, tops, sizeof(tops)); StepGraph::mix(key, table_key, sizeof(table_key)); StepGraph::mix(key, grads, sizeof(*grads)); StepGraph::mix(key, &e->w, sizeof(e->w));
     const void* ptrs[] = {ta.table, ta.refs, ta.ref_offsets, ta.sample_seq, ta.greedy_seq, ta.logprobs, ta.reward, ta.loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
     StepGraph::mix(key, ptrs, sizeof(ptrs));
-    StepGraph::mix(key, e->grad_events, sizeof(e->grad_events));
+    StepGraph::mix(key, e->grad_events, sizeof(cudaEvent_t) * e->grad_groups);
     const int dims[] = {B, R, ta.L};
     StepGraph::mix(key, dims, sizeof(dims));
     const int rc = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return counted(staged(0), staged(1), ts, gst); });
