@@ -1,6 +1,6 @@
 """CPU oracle for the caption-decode hot path (TEST INFRASTRUCTURE ONLY).
 
-This file is a from-scratch, functional restatement (torch fp32 on CPU, no nn.Module) of the
+This file is a from-scratch, functional restatement (torch on CPU, no nn.Module; fp32, or float64 when given float64 weights and features) of the
 reference algorithm on the path BASELINE.json names.  It is the *checker*: only ``tests/``,
 ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / ``--impl reference`` leg may import it.
 The product package (``imagecaptioning.pytorch_b200``) never does.
@@ -351,7 +351,7 @@ class Family:
     def init_state(self, n: int):
         if self.name == 'transformer':
             return []
-        z = torch.zeros(self.num_layers, n, self.rnn_size)
+        z = torch.zeros(self.num_layers, n, self.rnn_size, dtype=self.W['logit.weight'].dtype)
         return (z, z.clone())
 
     def embed(self, it: Tensor) -> Tensor:
@@ -467,7 +467,7 @@ def sample_beam(fam: Family, fc: Tensor, att: Tensor, masks: Optional[Tensor] = 
     done = beam_search(fam, state, logprobs, fc_r, att_r, p_att_r, masks_r, beam_size, length_penalty, record_margin=record_margin,
                        margin_rows=margin_rows)
     seq = torch.zeros(B * sample_n, T, dtype=torch.long)
-    seq_lp = torch.zeros(B * sample_n, T, V1)
+    seq_lp = torch.zeros(B * sample_n, T, V1, dtype=fc.dtype)
     for k in range(B):
         for n in range(sample_n):
             rec = done[k][n]
@@ -493,7 +493,7 @@ def sample(fam: Family, fc: Tensor, att: Tensor, masks: Optional[Tensor] = None,
     fc_e, att_e, p_att, masks = (repeat_rows(x, sample_n) for x in (fc_e, att_e, p_att, masks))
     state = fam.init_state(N)
     seq = torch.zeros(N, T, dtype=torch.long)
-    seq_lp = torch.zeros(N, T, V1)
+    seq_lp = torch.zeros(N, T, V1, dtype=fc.dtype)
     it = torch.zeros(N, dtype=torch.long)
     unfinished = None
     for t in range(T):
@@ -549,7 +549,7 @@ def forward_teacher(fam: Family, fc: Tensor, att: Tensor, seq: Tensor, masks: Op
     fc_e, att_e, p_att, masks = fam.prepare(fc, att, masks)
     fc_e, att_e, p_att, masks = (repeat_rows(x, spi) for x in (fc_e, att_e, p_att, masks))
     state = fam.init_state(N)
-    out = torch.zeros(N, seq.shape[1], fam.vocab1)
+    out = torch.zeros(N, seq.shape[1], fam.vocab1, dtype=fc.dtype)
     for i in range(seq.shape[1]):
         if i >= 1 and int(seq[:, i].sum()) == 0:
             break

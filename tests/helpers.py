@@ -77,3 +77,88 @@ def check_decode(fam, fc, att, seq, lp, oseq, olp, margins, masks=None, sample_n
         best = np.array([d[0]['p'] for d in odone])
         assert np.abs(np.asarray(done_p)[:, 0] - best).max() < 1e-3
     return strict
+
+
+# ---- dropout masks of the fused training steps, regenerated from the engine's Philox streams (capb200.h lists the sites) -----------------
+
+def _mask_fn(b200, seed):
+    L, lib = b200._lib, b200._lib.load()
+
+    def mask(site, step, shape, p):
+        n = int(np.prod(shape))
+        m = torch.empty(n, device='cuda')
+        L.check(lib.capb200_dropout_mask(L.ptr(m), n, seed, site, step, p, L.current_stream()), 'dropout_mask')
+        return m.cpu().reshape(shape)
+    return mask
+
+
+def dropout_masks(b200, seed, p, B, R, N, T, E, H):
+    """UpDown: fc_embed [B, H], att_embed [B, R, H], the word embedding [T, N, E] and the LSTM output [T, N, H]."""
+    mask = _mask_fn(b200, seed)
+    return {'fc': mask(0, 0, (B, H), p), 'att': mask(1, 0, (B, R, H), p),
+            'xt': torch.stack([mask(2, t, (N, E), p) for t in range(T)]), 'out': torch.stack([mask(3, t, (N, H), p) for t in range(T)])}
+
+
+def att2in2_masks(b200, seed, p, B, R, N, T, E, H):
+    """Att2in2: att_embed [B, R, H], the word embedding [T, N, E] and the core output [T, N, H]."""
+    d = dropout_masks(b200, seed, p, B, R, N, T, E, H)
+    del d['fc']
+    return d
+
+
+def aoa_masks(b200, seed, B, R, N, T, E, H, heads, p_lm, p_at, p_aoa, p_sub):
+    """Every dropout mask of one AoANet training step: att_embed, the refiner's attention / AoA / sublayer sites, then per step the word,
+    ctx, decoder attention and output sites."""
+    mask = _mask_fn(b200, seed)
+    d = {'att': mask(1, 0, (B, R, H), p_lm)}
+    for l in range(6):
+        d['ref_p%d' % l] = mask(10 + l, 0, (B, heads, R, R), p_at)
+        d['ref_aoa%d' % l] = mask(20 + l, 0, (B, R, 2 * H), p_aoa)
+        d['ref_sub%d' % l] = mask(30 + l, 0, (B, R, H), p_sub)
+    d['xt'] = torch.stack([mask(2, t, (N, E), p_lm) for t in range(T)])
+    d['out'] = torch.stack([mask(3, t, (N, H), p_lm) for t in range(T)])
+    d['ctx'] = torch.stack([mask(4, t, (N, H), p_lm) for t in range(T)])
+    d['p'] = torch.stack([mask(5, t, (N, heads, 1, R), p_at) for t in range(T)])
+    return d
+
+
+# ---- gradients against a float64 reference, with a bar calibrated by the fp32 oracle's own distance from it ------------------------------
+
+def grad_bar(err32, ref_scale, largest, floor=2e-6, factor=4.0):
+    """max(factor x the calibrating oracle's error, floor x the float64 tensor's size) + 1e-7 x the step's largest gradient entry."""
+    return max(factor * err32, floor * ref_scale) + 1e-7 * largest
+
+
+def check_grads_f64(named, ref64, ref32, keep=None, zero_rel=1e-12, label='', floor=2e-6, factor=4.0):
+    """Every engine gradient (``named``: {name: tensor}) against float64 autograd ``ref64``, in max-abs and in Frobenius norm, each held to
+    grad_bar with the oracle ``ref32`` supplying the error an implementation of the same arithmetic makes (fp32, or the engine mode's).  ``keep`` {name: bool mask} leaves out
+    the entries float64 cannot decide (gradients routed through a ReLU whose input is within rounding of zero).  A tensor whose float64
+    gradient is zero (softmax shift invariance: alpha_net.bias, attention key biases) holds rounding noise only and is held to 4x the fp32
+    oracle's noise or 1e-6 of the step's largest gradient.  Prints, per tensor, the error as a fraction of its bar and the oracle's own
+    error relative to the tensor; returns the worst fraction."""
+    assert set(named) == set(ref64), set(named) ^ set(ref64)
+    largest = max(float(v.abs().max()) for v in ref64.values())
+    failures, worst = [], (0.0, '')
+    for k in sorted(named):
+        g, r64, r32 = named[k].detach().cpu().double(), ref64[k], ref32[k].double()
+        if keep is not None and k in keep:
+            g, r64, r32 = g[keep[k]], r64[keep[k]], r32[keep[k]]
+        scale = float(r64.abs().max())
+        e, e32 = (g - r64).abs(), (r32 - r64).abs()
+        if scale <= zero_rel * largest:
+            bar = max(factor * float(e32.max()), 1e-6 * largest)
+            ratio = float(e.max()) / bar
+            rel32 = float(e32.max()) / largest
+        else:
+            bar = grad_bar(float(e32.max()), scale, largest, floor, factor)
+            nbar = grad_bar(float(e32.norm()), float(r64.norm()), largest * e.numel() ** 0.5, floor, factor)
+            ratio = max(float(e.max()) / bar, float(e.norm()) / nbar)
+            rel32 = float(e32.max()) / scale
+        print('%s %-45s err/bar %.3f  oracle %.2e' % (label, k, ratio, rel32))
+        worst = max(worst, (ratio, k))
+        if ratio > 1.0:
+            failures.append((k, ratio, float(e.max()), scale))
+    print('%s worst gradient err/bar %.3f (%s)' % (label, worst[0], worst[1]))
+    assert not failures, failures
+    assert sum(float(v.abs().max()) > 1e-5 for v in ref64.values()) >= 15          # the comparison is not vacuous
+    return worst[0]

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import LOGP_TOL, PARITY_MODES, co, family_opt
+from helpers import LOGP_TOL, PARITY_MODES, att2in2_masks, co, family_opt
 import att2in2_oracle as ao
 import dbs_oracle
 
@@ -145,17 +145,6 @@ def _pair(mode, seed=31):
     return m, W
 
 
-def _masks(b200, seed, p, B, R, N, T):
-    L, lib = b200._lib, b200._lib.load()
-
-    def mask(site, step, rows, cols):
-        mm = torch.empty(rows * cols, device='cuda')
-        L.check(lib.capb200_dropout_mask(L.ptr(mm), rows * cols, seed, site, step, p, L.current_stream()), 'dropout_mask')
-        return mm.cpu().reshape(rows, cols)
-    return {'att': mask(1, 0, B * R, CFG['H']).reshape(B, R, CFG['H']), 'xt': torch.stack([mask(2, t, N, CFG['E']) for t in range(T)]),
-            'out': torch.stack([mask(3, t, N, CFG['H']) for t in range(T)])}
-
-
 def _check_grads(model, grads, ograds, rel=5e-4):
     name_of = {id(p): k for k, p in model.state_dict(keep_vars=True).items()}
     assert len(grads) == 17
@@ -209,7 +198,7 @@ def test_scst_step(mode, kind):
         assert torch.equal(res['greedy_seq'].cpu(), og)
         reward, _ = cdo.self_critical_reward(og.numpy(), gts, sseq.numpy(), df, ref_len)
         reward = torch.from_numpy(reward).float()
-    fam.drop = _masks(b200, seed, p, B, R, B * n, T)
+    fam.drop = att2in2_masks(b200, seed, p, B, R, B * n, T, CFG['E'], CFG['H'])
     _, lp = co.sample(fam, fc, att, regions, sample_method='sample', sample_n=n, forced_tokens=sseq)
     if keep:
         rows = co.reward_criterion(lp, sseq, reward, reduction='none')
@@ -246,7 +235,7 @@ def test_xe_step(mode, ss_prob):
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam = ao.Att2in2Family(Wg, T)
     if p:
-        fam.drop = _masks(b200, seed, p, B, R, B * spi, T + 1)
+        fam.drop = att2in2_masks(b200, seed, p, B, R, B * spi, T + 1, CFG['E'], CFG['H'])
     lp = co.forward_teacher(fam, fc, att, used, regions)
     loss = co.label_smoothing_loss(lp, labels[..., 1:], masks[..., 1:], 0.1)
     loss.backward()

@@ -9,11 +9,11 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import LOGP_TOL, check_decode, co, family_opt
+from helpers import LOGP_TOL, aoa_masks, check_decode, co, dropout_masks, family_opt
 import bleu_oracle as bo
 import dbs_oracle
 from test_gpu_diverse_beam import DECISIVE, P_TOL
-from test_gpu_scst import _aoa_masks, _check_grads, _dropout_masks
+from test_gpu_scst import _check_grads
 from test_gpu_tfm_train import _check_grads as _tfm_check_grads, _grad_weights, _masks as _tfm_masks
 from test_long_captions_cpu import corpus_df, load_case
 
@@ -329,7 +329,7 @@ def test_updown_scst_long():
     assert torch.equal(greedy_seq, og) and bool((sample_seq > 0).all())
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('updown', Wg, T)
-    fam_g.drop = _dropout_masks(b200, 79, 0.5, B, R, B * n, T, RNN['E'], RNN['H'])
+    fam_g.drop = dropout_masks(b200, 79, 0.5, B, R, B * n, T, RNN['E'], RNN['H'])
     _, lp = co.sample(fam_g, fc, att, sample_method='sample', sample_n=n, forced_tokens=sample_seq)
     reward, _ = cdo.self_critical_reward(greedy_seq.numpy(), gts, sample_seq.numpy(), df, ref_len)
     assert np.abs(res['reward'].cpu().numpy() - reward).max() < 1e-5 and np.abs(reward).max() > 0
@@ -360,7 +360,7 @@ def test_aoa_scst_long(baseline):
     assert bool((seq > 0).all())
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('aoa', Wg, T, heads=heads)
-    fam_g.drop = _aoa_masks(b200, 4323, B, R, B * n, T, AOA['E'], AOA['H'], heads, p_lm, p_at, p_aoa, p_sub)
+    fam_g.drop = aoa_masks(b200, 4323, B, R, B * n, T, AOA['E'], AOA['H'], heads, p_lm, p_at, p_aoa, p_sub)
     _, lp = co.sample(fam_g, fc, att, None, sample_method='sample', sample_n=n, forced_tokens=seq)
     if baseline == 'greedy':
         og, _ = co.sample(fam, fc, att)

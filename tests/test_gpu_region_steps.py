@@ -8,8 +8,8 @@ tensor's largest entry):
 import pytest
 import torch
 
-from helpers import LOGP_TOL, build_pair, check_decode, co, family_opt
-from test_gpu_scst import CFG as UD_CFG, _aoa_masks, _check_grads, _dropout_masks, _labels
+from helpers import LOGP_TOL, aoa_masks, build_pair, check_decode, co, dropout_masks, family_opt
+from test_gpu_scst import CFG as UD_CFG, _check_grads, _labels
 from test_gpu_tfm_train import _check_grads as _tfm_check_grads, _grad_weights, _labels as _tfm_labels, _masks as _tfm_masks
 
 pytestmark = pytest.mark.gpu
@@ -57,7 +57,7 @@ def test_aoa_scst_at_100_regions(baseline, clip):
     seq = res['sample_seq'].cpu()
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('aoa', Wg, T, heads=AOA_HEADS)
-    fam_g.drop = _aoa_masks(b200, 4323, B, Rc, B * n, T, AOA['E'], AOA['H'], AOA_HEADS, p_lm, p_at, p_aoa, p_sub)
+    fam_g.drop = aoa_masks(b200, 4323, B, Rc, B * n, T, AOA['E'], AOA['H'], AOA_HEADS, p_lm, p_at, p_aoa, p_sub)
     _, lp = co.sample(fam_g, fc, att, masks, sample_method='sample', sample_n=n, forced_tokens=seq)
     if baseline == 'greedy':
         og, _ = co.sample(fam, fc, att, masks)
@@ -90,7 +90,7 @@ def test_aoa_xe_at_100_regions(clip):
     torch.cuda.synchronize()
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam = co.Family('aoa', Wg, T, heads=AOA_HEADS)
-    fam.drop = _aoa_masks(b200, 556, B, Rc, B * spi, T + 1, AOA['E'], AOA['H'], AOA_HEADS, p_lm, p_at, p_aoa, p_sub)
+    fam.drop = aoa_masks(b200, 556, B, Rc, B * spi, T + 1, AOA['E'], AOA['H'], AOA_HEADS, p_lm, p_at, p_aoa, p_sub)
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1], masks)
     loss = co.language_model_criterion(lp, labels[..., 1:].reshape(B * spi, -1), lmasks[..., 1:].reshape(B * spi, -1))
     loss.backward()
@@ -225,7 +225,7 @@ def test_updown_scst_16_samples_at_300_regions():
     assert torch.equal(greedy_seq, og)
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('updown', Wg, T)
-    fam_g.drop = _dropout_masks(b200, 79, 0.5, B, R, B * n, T, UD_CFG['E'], UD_CFG['H'])
+    fam_g.drop = dropout_masks(b200, 79, 0.5, B, R, B * n, T, UD_CFG['E'], UD_CFG['H'])
     _, lp = co.sample(fam_g, fc, att, sample_method='sample', sample_n=n, forced_tokens=sample_seq)
     reward, _ = cdo.self_critical_reward(greedy_seq.numpy(), gts, sample_seq.numpy(), df, ref_len)
     loss = co.reward_criterion(lp, sample_seq, torch.from_numpy(reward).float())

@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import LOGP_TOL, build_pair, co
+from helpers import LOGP_TOL, aoa_masks, build_pair, co, dropout_masks
 
 pytestmark = pytest.mark.gpu
 
@@ -120,17 +120,6 @@ def test_loss_wrapper_backward_sets_param_grads():
     b200.rewards.reset_scorer()
 
 
-def _dropout_masks(b200, seed, p, B, R, N, T, E, H):
-    L, lib = b200._lib, b200._lib.load()
-
-    def mask(site, step, rows, cols):
-        m = torch.empty(rows * cols, device='cuda')
-        L.check(lib.capb200_dropout_mask(L.ptr(m), rows * cols, seed, site, step, p, L.current_stream()), 'dropout_mask')
-        return m.cpu().reshape(rows, cols)
-    return {'fc': mask(0, 0, B, H), 'att': mask(1, 0, B * R, H).reshape(B, R, H),
-            'xt': torch.stack([mask(2, t, N, E) for t in range(T)]), 'out': torch.stack([mask(3, t, N, H) for t in range(T)])}
-
-
 def _check_grads(model, grads, ograds, rel=5e-4):
     name_of = {id(p): k for k, p in model.state_dict(keep_vars=True).items()}
     largest = max(float(v.abs().max()) for v in ograds.values())
@@ -174,7 +163,7 @@ def test_xe_step_gradients(mode, drop_prob, short, smoothing):
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam = co.Family('updown', Wg, T)
     if drop_prob > 0:
-        fam.drop = _dropout_masks(b200, 77, drop_prob, B, R, B * spi, T + 1, CFG['E'], CFG['H'])
+        fam.drop = dropout_masks(b200, 77, drop_prob, B, R, B * spi, T + 1, CFG['E'], CFG['H'])
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1])
     if short:
         assert float(lp[:, -1].abs().max()) == 0.0
@@ -233,7 +222,7 @@ def test_new_self_critical_step(drop_prob):
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam = co.Family('updown', Wg, T)
     if drop_prob > 0:
-        fam.drop = _dropout_masks(b200, 99, drop_prob, B, R, B * n, T, CFG['E'], CFG['H'])
+        fam.drop = dropout_masks(b200, 99, drop_prob, B, R, B * n, T, CFG['E'], CFG['H'])
     _, lp = co.sample(fam, fc, att, sample_method='sample', sample_n=n, forced_tokens=seq)
     scores = torch.from_numpy(cdo.get_scores(gts, seq.numpy(), df, ref_len))
     loss = co.new_self_critical_loss(lp, seq, scores, n)
@@ -285,27 +274,6 @@ def test_loss_wrapper_xe_and_structure_branches():
 AOA_CFG = dict(V=40, E=32, H=64, A=0, F_fc=32, F_att=40, T=7)
 
 
-def _aoa_masks(b200, seed, B, R, N, T, E, H, heads, p_lm, p_at, p_aoa, p_sub):
-    """Every dropout mask of one AoANet training step, regenerated from the engine's Philox streams (capb200.h lists the sites)."""
-    L, lib = b200._lib, b200._lib.load()
-
-    def mask(site, step, shape, p):
-        n = int(np.prod(shape))
-        m = torch.empty(n, device='cuda')
-        L.check(lib.capb200_dropout_mask(L.ptr(m), n, seed, site, step, p, L.current_stream()), 'dropout_mask')
-        return m.cpu().reshape(shape)
-    d = {'att': mask(1, 0, (B, R, H), p_lm)}
-    for l in range(6):
-        d['ref_p%d' % l] = mask(10 + l, 0, (B, heads, R, R), p_at)
-        d['ref_aoa%d' % l] = mask(20 + l, 0, (B, R, 2 * H), p_aoa)
-        d['ref_sub%d' % l] = mask(30 + l, 0, (B, R, H), p_sub)
-    d['xt'] = torch.stack([mask(2, t, (N, E), p_lm) for t in range(T)])
-    d['out'] = torch.stack([mask(3, t, (N, H), p_lm) for t in range(T)])
-    d['ctx'] = torch.stack([mask(4, t, (N, H), p_lm) for t in range(T)])
-    d['p'] = torch.stack([mask(5, t, (N, heads, 1, R), p_at) for t in range(T)])
-    return d
-
-
 @pytest.mark.parametrize('mode,dropout,baseline', [('tc_f16x3', False, 'greedy'), ('tc_f16x3', True, 'greedy'), ('simt_fp32', True, 'leave_one_out')])
 def test_aoa_scst_step_gradients(mode, dropout, baseline):
     """AoANet SCST step (BASELINE configs[3]): loss, reward and every parameter gradient against torch autograd through the oracle, with
@@ -331,7 +299,7 @@ def test_aoa_scst_step_gradients(mode, dropout, baseline):
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('aoa', Wg, T, heads=heads)
     if dropout:
-        fam_g.drop = _aoa_masks(b200, 4321, B, R, B * n, T, E, H, heads, p_lm, p_at, p_aoa, p_sub)
+        fam_g.drop = aoa_masks(b200, 4321, B, R, B * n, T, E, H, heads, p_lm, p_at, p_aoa, p_sub)
     _, lp = co.sample(fam_g, fc, att, sample_method='sample', sample_n=n, forced_tokens=seq)
     if baseline == 'greedy':
         og, _ = co.sample(fam, fc, att)
@@ -372,7 +340,7 @@ def test_aoa_xe_step_gradients(dropout, smoothing):
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam = co.Family('aoa', Wg, T, heads=heads)
     if dropout:
-        fam.drop = _aoa_masks(b200, 555, B, R, B * spi, T + 1, E, H, heads, p_lm, p_at, p_aoa, p_sub)
+        fam.drop = aoa_masks(b200, 555, B, R, B * spi, T + 1, E, H, heads, p_lm, p_at, p_aoa, p_sub)
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1])
     assert float(lp[:, -1].abs().max()) == 0.0
     tl, tm = labels[..., 1:].reshape(B * spi, -1), masks[..., 1:].reshape(B * spi, -1)
@@ -430,7 +398,7 @@ def test_scst_step_gradients_with_region_masks(mode, clip):
     assert torch.equal(greedy_seq, og)
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('updown', Wg, T)
-    fam_g.drop = _dropout_masks(b200, 77, 0.5, B, Rc, B * n, T, CFG['E'], CFG['H'])
+    fam_g.drop = dropout_masks(b200, 77, 0.5, B, Rc, B * n, T, CFG['E'], CFG['H'])
     _, lp = co.sample(fam_g, fc, att, masks, sample_method='sample', sample_n=n, forced_tokens=sample_seq)
     reward, _ = cdo.self_critical_reward(greedy_seq.numpy(), gts, sample_seq.numpy(), df, ref_len)
     loss = co.reward_criterion(lp, sample_seq, torch.from_numpy(reward).float())
@@ -454,7 +422,7 @@ def test_xe_step_gradients_with_region_masks():
     torch.cuda.synchronize()
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam = co.Family('updown', Wg, T)
-    fam.drop = _dropout_masks(b200, 78, 0.5, B, Rc, B * spi, T + 1, CFG['E'], CFG['H'])
+    fam.drop = dropout_masks(b200, 78, 0.5, B, Rc, B * spi, T + 1, CFG['E'], CFG['H'])
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1], masks)
     tl, tm = labels[..., 1:].reshape(B * spi, -1), lmasks[..., 1:].reshape(B * spi, -1)
     loss = co.label_smoothing_loss(lp, tl, tm, 0.1)
@@ -491,7 +459,7 @@ def test_aoa_scst_step_gradients_with_region_masks(clip):
     assert torch.equal(res['greedy_seq'].cpu(), og)
     Wg = {k: v.clone().requires_grad_(True) for k, v in W.items()}
     fam_g = co.Family('aoa', Wg, T, heads=heads)
-    fam_g.drop = _aoa_masks(b200, 4322, B, Rc, B * n, T, E, H, heads, p_lm, p_at, p_aoa, p_sub)
+    fam_g.drop = aoa_masks(b200, 4322, B, Rc, B * n, T, E, H, heads, p_lm, p_at, p_aoa, p_sub)
     _, lp = co.sample(fam_g, fc, att, masks, sample_method='sample', sample_n=n, forced_tokens=seq)
     reward, _ = cdo.self_critical_reward(og.numpy(), gts, seq.numpy(), df, ref_len)
     loss = co.reward_criterion(lp, seq, torch.from_numpy(reward).float())

@@ -1,0 +1,603 @@
+"""The fused training steps of UpDown, Att2in2 and AoANet at the widths they train at, against float64 autograd through the oracle.
+
+UpDown runs at bench.py's CFG (V 9487, E = H = 1000, A 512, F 2048), Att2in2 at the a2i2 recipe width (E = H = A = 512) and AoANet at
+configs/aoa.yml's (E = H = 1024, 8 heads, 6 refiner layers), all with 36 regions and 20 steps.  In both modes the vocabulary-row kernels
+loop 37 times per row, the attention backward runs 16 column blocks per image and the autograd VJP takes its 4-wide form.  The training
+GEMMs differ by mode: tc_f16x3 runs them on gemm_tf32.cu's wgmma 3xTF32 kernel, whose tile follows the row count (50 rows per step: tile
+width 64, swapped; 1000 rows batched over time: the normal orientation, cluster split-K over K = 9488 for the logit layer); simt_fp32 runs
+gemm_generic.cu's CUDA-core kernels with their one tile shape.
+
+Every case compares loss, picked log-probs, reward and every parameter gradient with the same step run through the oracle in float64.  The
+bar calibrates itself: the step also runs through the oracle in float32, and each tensor's error may be at most
+    max(4 x the fp32 oracle's error, 2e-6 x max|f64|) + 1e-7 x the step's largest gradient entry,
+(the 2e-6 grows as sqrt(N * T / 1000) past 1000 reduced (step, row) pairs),
+in max-abs and in Frobenius norm.  Samples and baseline captions are replayed (forced_tokens / forced_baseline), so no near-tie in sampling
+can change what is compared.
+
+Kinks: a ReLU input or a maxout pair within rounding of the switch point can land on either side in fp32.  The float64 pass lists those
+units (margin KINK_MARGIN x the layer's RMS, several times the fp32 error of these dot products):
+* ReLU (att_embed, fc_embed): the gradient through unit j only reaches row j of the layer's weight and entry j of its bias, so those
+  entries are left out;
+* Att2in2's maxout: the routed gradient runs back through the recurrence into every core tensor, so leaving entries out would drop whole
+  tensors.  Instead the gradient change of re-routing each ambiguous unit is computed in float64 (one caption row rerun), and for each unit
+  the side that fits the engine better is taken.  Each change is hundreds of times the bar, so the choice is never close.
+The fp32 oracle follows float64's decisions at every kink, so its distance from float64 is arithmetic only.
+
+Calibration per mode: simt_fp32 is held to the fp32 oracle.  tc_f16x3 is held to the same oracle with every Linear's forward and input
+gradient computed as gemm_tf32 does (_mm_tf32x3): hi / lo tf32 split, three wgmmas per k8 step into one fp32 accumulator, and the
+accumulator truncated (rounded toward zero) by every instruction, the budget test_gpu_ops.py already gives this kernel.  Over K = 3000
+that is 1125 truncations, biased toward zero, so the mode's log-probs and gradients sit 10-40x further from float64 than fp32's; the
+emulation reproduces that (its picked log-probs sit 1-3x the engine's distance from float64) and the bar is 4x its error, as for fp32.
+It over-counts the forward's truncations (the kernel's cluster split-K gives each CTA a slice of K) and leaves the weight gradients, which
+the engine batches over time, in fp32, so it is no tighter bound than that: at 320 rows the engine's logit.weight gradient reaches 1.25x
+the emulation's error.
+
+Att2in2 runs in simt_fp32 only.  In tc_f16x3 the engine's own error in the maxout inputs is of the order of the kink margin, and the
+gradient change of re-routing a unit is no longer decisive against the mode's error, so the maxout decisions cannot be read off.
+
+The loss is a sum over every caption position, reduced in another order than torch's; its floor is the pairwise-summation bound
+2^-24 x log2(terms) x sum of |terms| rather than a fixed 1e-6.
+"""
+import contextlib
+import time
+
+import numpy as np
+import pytest
+import torch
+
+import att2in2_oracle as ao
+from helpers import aoa_masks, att2in2_masks, check_grads_f64, co, dropout_masks, family_opt
+
+pytestmark = pytest.mark.gpu
+
+R, T, SPI, HEADS = 36, 20, 5, 8
+CFGS = {'updown': dict(V=9487, E=1000, H=1000, A=512, F_fc=2048, F_att=2048, T=T),      # bench.py CFG
+        'att2in2': dict(V=9487, E=512, H=512, A=512, F_fc=2048, F_att=2048, T=T),       # a2i2 recipe
+        'aoa': dict(V=9487, E=1024, H=1024, A=0, F_fc=2048, F_att=2048, T=T)}           # configs/aoa.yml
+LOGIT_SCALE = {'updown': 12.0, 'att2in2': 12.0, 'aoa': 6.0}                               # bench.py's synthetic models
+RATES = {'updown': 0.5, 'att2in2': 0.5, 'aoa': (0.5, 0.1, 0.3, 0.1)}                      # drop_prob_lm (+ AoANet: attention, AoA, sublayer)
+KINK_MARGIN = 2e-5              # ReLU inputs and maxout a - b: x the layer's RMS, at least 5x the fp32 oracle's own error there (asserted)
+SEED = 4242
+COLLIDE = 7                     # the word that fills whole caption rows: embed_scatter's atomics all land on one row of d_emb
+
+_MODELS, _WEIGHTS = {}, {}
+_CASES = {}                     # each case's float64 / fp32 references, held until every mode has been compared with them
+
+
+def _tf32(x, nearest):
+    """x (fp32) cut to tf32's 10 explicit mantissa bits: to nearest with ties away from zero (cvt.rna.tf32), or toward zero (what the
+    tensor core keeps of the fp32 lo operand)."""
+    i = x.contiguous().view(torch.int32)
+    return ((i + 0x1000 if nearest else i) & ~0x1FFF).view(torch.float32)
+
+
+def _mm_tf32x3(a, b):
+    """a [M, K] @ b [K, N] as gemm_tf32.cu computes it, on the GPU: hi = rna(x), lo = x - hi as the tensor core keeps it, and per k8 step
+    three wgmmas (hi.lo, lo.hi, hi.hi) into one fp32 accumulator that every instruction truncates (rounds toward zero).  The products of a
+    k8 step are summed exactly (float64); each truncation is taken at the exact running sum, which leaves out only the second-order effect
+    of earlier truncations on later ones.  The whole K runs through one accumulator (the kernel's cluster split-K gives each CTA a slice
+    and sums the slices rounded to nearest, so this is the larger of the two truncation counts)."""
+    dev = torch.device('cuda')
+    a, b = a.detach().to(dev, torch.float32), b.detach().to(dev, torch.float32)
+    M, K = a.shape
+    N = b.shape[1]
+    Kp = -(-K // 8) * 8
+    a, b = torch.nn.functional.pad(a, (0, Kp - K)), torch.nn.functional.pad(b.t(), (0, Kp - K))      # [M, Kp], [N, Kp]
+    ah, bh = _tf32(a, True), _tf32(b, True)
+    al, bl = _tf32(a - ah, False), _tf32(b - bh, False)
+    J = Kp // 8
+    out = torch.empty(M, N, dtype=torch.float64, device=dev)
+    rows = max(1, int(2e8 // (N * J * 3)))
+    for m0 in range(0, M, rows):
+        sl = slice(m0, m0 + rows)
+
+        def step(x, y):
+            return torch.einsum('mjb,njb->mnj', x[sl].double().view(-1, J, 8), y.double().view(N, J, 8))
+        seq = torch.stack([step(ah, bl), step(al, bh), step(ah, bh)], -1).flatten(2)          # [m, N, 3J], in issue order
+        run = seq.cumsum(-1)
+        f = run.float()
+        f = torch.where(f.double().abs() > run.abs(), torch.nextafter(f, torch.zeros_like(f)), f)     # round toward zero
+        out[sl] = run[..., -1] + (f.double() - run).sum(-1)
+        del seq, run, f
+    return out.float().cpu()
+
+
+class _Tf32x3Linear(torch.autograd.Function):
+    """x @ w.T with the forward and the input gradient as gemm_tf32 computes them; the weight gradient in plain fp32."""
+    @staticmethod
+    def forward(ctx, x, w):
+        ctx.save_for_backward(x, w)
+        return _mm_tf32x3(x.reshape(-1, x.shape[-1]), w.t()).reshape(*x.shape[:-1], w.shape[0])
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, w = ctx.saved_tensors
+        g2 = gy.reshape(-1, gy.shape[-1])
+        return _mm_tf32x3(g2, w).reshape(x.shape), g2.t() @ x.reshape(-1, x.shape[-1])
+
+
+def _tf32x3_linear(x, w, b=None):
+    y = _Tf32x3Linear.apply(x, w)
+    return y if b is None else y + b
+
+
+@contextlib.contextmanager
+def _linear(fn):
+    orig = co.linear
+    co.linear = fn
+    try:
+        yield
+    finally:
+        co.linear = orig
+
+
+@contextlib.contextmanager
+def _routed_maxout(record, route=None, flip=None):
+    """co.maxout_lstm with its routing exposed: each call appends a - b of the two maxout halves to ``record``; ``route`` (one bool [N, H]
+    per step) fixes which half takes the gradient, and ``flip`` {step: bool [N, H]} re-routes single units.  The forward value is always
+    max(a, b)."""
+    orig, step = co.maxout_lstm, [0]
+
+    def maxout_lstm(W, x, state):
+        h, c = state
+        hs = h.shape[2]
+        s = co.linear(x, W['_core.i2h.weight'], W['_core.i2h.bias']) + co.linear(h[-1], W['_core.h2h.weight'], W['_core.h2h.bias'])
+        sig = torch.sigmoid(s[:, :3 * hs])
+        a, b = s[:, 3 * hs:4 * hs], s[:, 4 * hs:5 * hs]
+        record.append((a - b).detach())
+        t = step[0]
+        step[0] += 1
+        sel = (a > b) if route is None else route[t]
+        if flip is not None and t in flip:
+            sel = sel ^ flip[t]
+        routed = torch.where(sel, a, b)
+        g = routed + (torch.maximum(a, b) - routed).detach()
+        c_new = sig[:, hs:2 * hs] * c[-1] + sig[:, :hs] * g
+        h_new = sig[:, 2 * hs:] * torch.tanh(c_new)
+        return h_new, (h_new.unsqueeze(0), c_new.unsqueeze(0))
+    co.maxout_lstm = maxout_lstm
+    try:
+        yield
+    finally:
+        co.maxout_lstm = orig
+
+
+def _weights(family):
+    if family not in _WEIGHTS:
+        c = CFGS[family]
+        _WEIGHTS[family] = co.make_weights(family, c['V'], c['E'], c['H'], c['A'], c['F_fc'], c['F_att'], seed=1, logit_scale=LOGIT_SCALE[family])
+    return _WEIGHTS[family]
+
+
+def _model(family, mode, autograd=False):
+    import imagecaptioning.pytorch_b200 as b200
+    key = (family, mode, autograd)
+    if key not in _MODELS:
+        c = CFGS[family]
+        opt = family_opt(family, c['V'], c['E'], c['H'], c['A'], c['F_fc'], c['F_att'], T, heads=HEADS)
+        opt.b200_autograd = int(autograd)
+        m = b200.setup(opt, numeric_mode=mode)
+        m.load_state_dict(_weights(family), strict=True)
+        _MODELS[key] = m.cuda()
+    return _MODELS[key]
+
+
+def _region_masks(B):
+    """Prefix masks: image 0 keeps all 36 regions, the others 3 to 35, several of them fewer than 10."""
+    m = torch.zeros(B, R)
+    for i in range(B):
+        m[i, :R if i == 0 else [7, 20, 3, 35, 9, 28, 5, 14, 31][(i - 1) % 9]] = 1
+    return m
+
+
+def _samples(gts, B, V, seed):
+    """Forced samples [B * 5, T] built from each image's references (so CIDEr-D rewards differ from row to row) with edges: row 0 is EOS
+    at t = 0; image 1's five samples are identical; every even row of the even images runs all T steps without EOS; image 3's rows are
+    COLLIDE at every step but one, image 4's at every other step."""
+    rng = np.random.RandomState(seed)
+    tok = np.zeros((B * SPI, T), np.int64)
+    for i in range(B * SPI):
+        b, j = divmod(i, SPI)
+        ref = [w for w in gts[b][j % len(gts[b])] if w > 0]
+        words = [w if rng.rand() > 0.3 else int(rng.randint(1, V + 1)) for w in ref]
+        full = b % 2 == 0 and j % 2 == 0
+        ln = T if full else int(rng.randint(1, T))
+        while len(words) < ln:
+            words.append(int(min(rng.zipf(1.3), V)))
+        tok[i, :ln] = words[:ln]
+    tok[0] = 0
+    if B > 1:
+        tok[SPI:2 * SPI] = tok[SPI]
+    if B > 4:
+        for j in range(SPI):
+            r3, r4 = 3 * SPI + j, 4 * SPI + j
+            tok[r3] = COLLIDE
+            tok[r3, j] = tok[r4, j] if tok[r4, j] else 1
+            tok[r4, ::2] = COLLIDE
+            tok[r4, 1::2] = np.where(tok[r4, 1::2] > 0, tok[r4, 1::2], 2)
+    return torch.from_numpy(tok)
+
+
+def _labels(gts, B, V, seed):
+    """XE labels [B, 5, T + 2] of mixed lengths 1 .. T (BOS at 0, EOS after the last word) built from the references, image 3's rows
+    filled with COLLIDE, and their masks."""
+    tok = _samples(gts, B, V, seed)
+    tok[0, :3] = torch.tensor([5, 6, 7])          # the sampler's EOS-first row has no XE counterpart: a 3-word caption instead
+    labels = torch.zeros(B * SPI, T + 2, dtype=torch.long)
+    masks = torch.zeros(B * SPI, T + 2)
+    for i in range(B * SPI):
+        ln = int((tok[i] > 0).cumprod(0).sum())
+        labels[i, 1:1 + ln] = tok[i, :ln]
+        masks[i, :ln + 2] = 1
+    return labels.view(B, SPI, -1), masks.view(B, SPI, -1)
+
+
+class Case:
+    def __init__(self, family, kind, dropout, B, smoothing=0.0, regions=False):
+        from oracle import ciderd_oracle as cdo
+        self.family, self.kind, self.dropout, self.B, self.smoothing = family, kind, dropout, B, smoothing
+        c = CFGS[family]
+        self.c, self.N = c, B * SPI
+        self.fc, self.att = co.make_inputs(B, R, c['F_fc'], c['F_att'], seed=17)
+        self.regions = _region_masks(B) if regions else None
+        self.Rc = R if self.regions is None else int(self.regions.sum(1).max())
+        self.gts = cdo.make_refs(B, c['V'], seed=5)
+        self.df, self.ref_len = cdo.build_document_frequency(cdo.make_refs(1000, c['V'], seed=4))
+        self.steps = T + 1 if kind in ('xe', 'autograd') else T
+        if kind in ('greedy', 'leave_one_out'):
+            self.tok = _samples(self.gts, B, c['V'], seed=23)
+            self.base = torch.stack([torch.from_numpy(np.pad(self.gts[b][1][:9], (0, T - 9))) for b in range(B)])
+            if kind == 'greedy':
+                reward, _ = cdo.self_critical_reward(self.base.numpy(), self.gts, self.tok.numpy(), self.df, self.ref_len)
+            else:
+                sc = cdo.get_scores(self.gts, self.tok.numpy(), self.df, self.ref_len).reshape(B, SPI)
+                reward = np.repeat((sc - (sc.sum(1, keepdims=True) - sc) / (SPI - 1)).reshape(-1, 1), T, 1)
+            self.reward = torch.from_numpy(np.ascontiguousarray(reward)).double()
+            self.mask = torch.cat([torch.ones(self.N, 1), (self.tok[:, :-1] > 0).double()], 1)
+        else:
+            self.labels, self.lmasks = _labels(self.gts, B, c['V'], seed=29)
+            self.tl, self.tm = self.labels[..., 1:].reshape(self.N, -1), self.lmasks[..., 1:].reshape(self.N, -1)
+            if kind == 'autograd':
+                self.G = torch.randn(self.N, T + 1, c['V'] + 1, generator=torch.Generator().manual_seed(31))
+        self.drop = None
+
+    # ---- the step through the oracle ----------------------------------------------------------------------------------------------------
+    def _family(self, W):
+        return ao.Att2in2Family(W, T) if self.family == 'att2in2' else co.Family(self.family, W, T, heads=HEADS)
+
+    def _inputs(self, rows, dt):
+        """(fc, att, regions, drop, words) of all rows (rows None) or of one caption row."""
+        fc, att, reg, drop = self.fc, self.att, self.regions, self.drop
+        words = self.tok if self.kind in ('greedy', 'leave_one_out') else self.labels[..., :-1].reshape(self.N, -1)
+        if rows is not None:
+            # row n of image b, and a companion row of COLLIDE words that runs every step (a teacher-forced pass stops at the first
+            # column where every row is pad, and the full batch runs on past row n's end); only row n enters the objective
+            n = rows
+            b = n // SPI
+            fc, att = fc[b:b + 1], att[b:b + 1]
+            words = torch.cat([words[n:n + 1], torch.full_like(words[n:n + 1], COLLIDE)])
+            rb = R if reg is None else int(reg[b].sum())
+            if reg is not None:
+                reg = reg[b:b + 1]
+            if drop is not None:
+                drop = {'att': drop['att'][b:b + 1, :rb], 'xt': drop['xt'][:, [n, n]], 'out': drop['out'][:, [n, n]]}
+        if drop is not None:
+            drop = {k: v.to(dt) for k, v in drop.items()}
+        return fc.to(dt), att.to(dt), reg, drop, words
+
+    def _objective(self, lp, rows, dt):
+        """The step's loss (all rows), or the share of it that one caption row contributes (same normaliser)."""
+        sl = slice(None) if rows is None else slice(rows, rows + 1)
+        if self.kind in ('greedy', 'leave_one_out'):
+            reward = self.reward.to(dt)[sl]
+            if rows is None:
+                return co.reward_criterion(lp, self.tok, reward)
+            tok, mask = self.tok[sl], self.mask.to(dt)[sl]
+            return -(lp.gather(2, tok.unsqueeze(2)).squeeze(2) * reward * mask).sum() / self.mask.sum()
+        if self.kind == 'autograd':
+            return (lp * self.G.to(dt)[sl]).sum()
+        tl, tm = self.tl[sl], self.tm[sl]
+        if self.smoothing:
+            crit = lambda *a, **k: co.label_smoothing_loss(*a, self.smoothing, **k)       # noqa: E731
+        else:
+            crit = co.language_model_criterion
+        if rows is None:
+            return crit(lp, tl, tm)
+        return (crit(lp, tl, tm, reduction='none') * tm.sum(1).to(dt)).sum() / self.tm.sum()
+
+    def oracle(self, dt, rows=None, route=None, flip=None, record=None, tf32x3=False):
+        W = {k: v.detach().to(dt, copy=True).requires_grad_(True) for k, v in _weights(self.family).items()}
+        fam = self._family(W)
+        fc, att, reg, fam.drop, words = self._inputs(rows, dt)
+        maxout = _routed_maxout([] if record is None else record, route, flip) if self.family == 'att2in2' else contextlib.nullcontext()
+        with maxout, (_linear(_tf32x3_linear) if tf32x3 else contextlib.nullcontext()):
+            if self.kind in ('greedy', 'leave_one_out'):
+                _, lp = co.sample(fam, fc, att, reg, sample_method='sample', sample_n=2 if rows is not None else SPI, forced_tokens=words)
+            else:
+                lp = co.forward_teacher(fam, fc, att, words.view(fc.shape[0], -1, words.shape[1]), reg)
+        if rows is not None:
+            lp = lp[:1]
+        loss = self._objective(lp, rows, dt)
+        loss.backward()
+        return float(loss), lp.detach(), {k: v.grad for k, v in W.items()}
+
+    def picked(self, lp):
+        if self.kind in ('greedy', 'leave_one_out'):
+            return lp.gather(2, self.tok.unsqueeze(2)).squeeze(2)
+        if self.kind == 'autograd':
+            return lp
+        return lp.gather(2, self.tl[:, :lp.shape[1]].unsqueeze(2)).squeeze(2)
+
+    def relu_kinks(self):
+        """{parameter name: bool mask of the entries kept}: rows j of a ReLU layer's weight (and entry j of its bias) whose input lies within
+        KINK_MARGIN x RMS of zero for some valid region (or image), in float64.  The fp32 pre-activations must sit well inside the margin."""
+        W = _weights(self.family)
+        layers = [('att_embed.0', self.att)] + ([('fc_embed.0', self.fc.unsqueeze(1))] if self.family == 'updown' else [])
+        keep, left_out, self.kink_rows = {}, 0, {}
+        for name, x in layers:
+            pre = co.linear(x.double(), W[name + '.weight'].double(), W[name + '.bias'].double())
+            valid = torch.ones(pre.shape[:2], dtype=torch.bool)
+            if self.regions is not None and name == 'att_embed.0':
+                valid = self.regions.bool()
+            rms = float(pre[valid].pow(2).mean().sqrt())
+            pre32 = co.linear(x, W[name + '.weight'], W[name + '.bias'])
+            assert 5 * float((pre32.double() - pre).abs().max()) < KINK_MARGIN * rms
+            amb = ((pre.abs() < KINK_MARGIN * rms) & valid.unsqueeze(-1)).any(1).any(0)          # [H]
+            keep[name + '.weight'] = ~amb.unsqueeze(1).expand_as(W[name + '.weight'])
+            keep[name + '.bias'] = ~amb
+            left_out += int(amb.sum()) * (W[name + '.weight'].shape[1] + 1)
+            self.kink_rows[name] = int(amb.sum())
+        return keep, left_out
+
+    def reference(self):
+        t0 = time.time()
+        rec64, rec32 = [], []
+        loss64, lp64, g64 = self.oracle(torch.float64, record=rec64)
+        route = [d > 0 for d in rec64] if rec64 else None
+        loss32, lp32, g32 = self.oracle(torch.float32, route=route, record=rec32)
+        self.ref = dict(loss64=loss64, loss32=loss32, picked64=self.picked(lp64), picked32=self.picked(lp32).double(), g64=g64, g32=g32)
+        self.ref['l1'] = self._loss_l1(lp64)
+        self.keep, self.left_out = self.relu_kinks()
+        self.maxout = []
+        if rec64:
+            d = torch.stack(rec64)                                   # [steps, N, H]
+            rms = float(d.pow(2).mean().sqrt())
+            err32 = float((torch.stack(rec32).double() - d).abs().max())
+            assert 5 * err32 < KINK_MARGIN * rms, (err32, rms)
+            self.maxout = [tuple(int(v) for v in u) for u in (d.abs() < KINK_MARGIN * rms).nonzero()]
+            self.route = route
+        self.ref_seconds = time.time() - t0
+
+    def reference_tf32x3(self):
+        """The calibrating oracle of tc_f16x3: the fp32 oracle with every Linear's forward and input gradient as gemm_tf32 computes them,
+        following float64's maxout routing."""
+        if 'g3' not in self.ref:
+            loss3, lp3, g3 = self.oracle(torch.float32, route=getattr(self, 'route', None), tf32x3=True)
+            self.ref.update(loss3=loss3, picked3=self.picked(lp3).double(), g3=g3)
+        return self.ref['loss3'], self.ref['picked3'], self.ref['g3']
+
+    def _loss_l1(self, lp64):
+        """(number of summed terms, sum of their magnitudes) of the step's loss."""
+        if self.kind in ('greedy', 'leave_one_out'):
+            p = lp64.gather(2, self.tok.unsqueeze(2)).squeeze(2)
+            return p.numel(), float((p * self.reward * self.mask).abs().sum() / self.mask.sum())
+        if self.kind == 'autograd':
+            return lp64.numel(), float((lp64 * self.G.double()).abs().sum())
+        n = self.tm.numel() * (lp64.shape[2] if self.smoothing else 1)
+        return n, abs(self.ref['loss64'])        # NLL and KL terms are all >= 0
+
+    def maxout_delta(self, unit, bases):
+        """float64 gradient change of re-routing one maxout unit (t, n, j): only caption row n's share of the loss changes.  ``bases`` caches
+        each row's share as float64 routes it."""
+        t, n, j = unit
+        route = [r[[n, n]] for r in self.route]
+        if n not in bases:
+            bases[n] = self.oracle(torch.float64, rows=n, route=route)[2]
+        base = bases[n]
+        flip = torch.zeros(2, self.c['H'], dtype=torch.bool)
+        flip[0, j] = True
+        _, _, moved = self.oracle(torch.float64, rows=n, route=route, flip={t: flip})
+        return {k: moved[k] - base[k] for k in base}
+
+
+def _fit_maxout(case, named):
+    """The float64 gradients with each ambiguous maxout unit routed the way that fits the engine better; returns (gradients, re-routed)."""
+    g64 = {k: v.clone() for k, v in case.ref['g64'].items()}
+    largest = max(float(v.abs().max()) for v in g64.values())
+    scale = {k: float(v.abs().max()) + 1e-6 * largest for k, v in g64.items()}       # a zero-gradient tensor's noise must not decide
+    keep = {k: case.keep.get(k, torch.ones((), dtype=torch.bool)) for k in g64}          # ReLU kink entries say nothing about the maxout
+    moved, bases = 0, {}
+    for u in case.maxout:
+        delta = case.maxout_delta(u, bases)
+
+        def miss(k, d):
+            return float((((named[k].double() - g64[k] - d) / scale[k]) * keep[k]).pow(2).sum())
+        before = sum(miss(k, 0.0) for k in delta)
+        after = sum(miss(k, delta[k]) for k in delta)
+        size = sum(float(((delta[k] / scale[k]) * keep[k]).pow(2).sum()) for k in delta)
+        # after - before = size - 2 <misfit, delta>: the engine's misfit must project onto delta at ~0 (not re-routed) or ~1 (re-routed),
+        # never in between, so an engine error can never pass for a maxout decision
+        assert size < 1e-18 or abs(after - before) >= 0.8 * size, (u, before, after, size)
+        if after < before:
+            for k in delta:
+                g64[k] += delta[k]
+            moved += 1
+    return g64, moved
+
+
+def _scalar_bar(err, floor=1e-6, factor=4.0):
+    return max(factor * err, floor)
+
+
+def _reference(family, kind, dropout, B, smoothing, regions, masks_fn, modes):
+    key = (family, kind, dropout, B, smoothing, regions)
+    if key not in _CASES:
+        case = Case(family, kind, dropout, B, smoothing, regions)
+        if dropout:
+            case.drop = masks_fn(case)
+        case.reference()
+        case.uses = 0
+        _CASES[key] = case
+    case = _CASES[key]
+    case.uses += 1
+    if case.uses == modes:                # every mode this case runs in has had it
+        del _CASES[key]
+    return case
+
+
+def _masks_fn(family):
+    import imagecaptioning.pytorch_b200 as b200
+
+    def make(case):
+        c, steps = case.c, case.steps
+        if family == 'aoa':
+            return aoa_masks(b200, SEED, case.B, case.Rc, case.N, steps, c['E'], c['H'], HEADS, *RATES['aoa'])
+        fn = dropout_masks if family == 'updown' else att2in2_masks
+        return fn(b200, SEED, RATES[family], case.B, case.Rc, case.N, steps, c['E'], c['H'])
+    return make
+
+
+def _check_masks(family, drop):
+    rates = RATES[family] if family == 'aoa' else (RATES[family],) * 4
+    for k, m in drop.items():
+        p = rates[1] if k.startswith('ref_p') or k == 'p' else rates[2] if k.startswith('ref_aoa') else rates[3] if k.startswith('ref_sub') else rates[0]
+        assert abs(float((m > 0).double().mean()) - (1 - p)) < 0.02, (k, p)
+
+
+def _run_engine(family, mode, case):
+    model = _model(family, mode, autograd=case.kind == 'autograd')
+    fc, att = case.fc.cuda(), case.att.cuda()
+    reg = None if case.regions is None else case.regions.cuda()
+    if family == 'aoa':
+        p = RATES['aoa'] if case.dropout else (0.0,) * 4
+        rates = dict(drop_prob=p[0], drop_attn=p[1], drop_aoa=p[2], drop_sublayer=p[3], ctx_drop=1)
+    else:
+        rates = dict(drop_prob=RATES[family] if case.dropout else 0.0)
+    name_of = {id(p): k for k, p in model.state_dict(keep_vars=True).items()}
+    if case.kind == 'autograd':
+        model.eval()
+        for p in model.parameters():
+            p.grad = None
+        lp = model(fc, att, case.labels[..., :-1].cuda(), reg)
+        (lp * case.G.cuda()).sum().backward()
+        torch.cuda.synchronize()
+        return dict(lp=lp.detach().cpu(),
+                    grads={k: p.grad.detach().cpu() for k, p in model.state_dict(keep_vars=True).items() if isinstance(p, torch.nn.Parameter)})
+    model.train()
+    if case.kind == 'xe':
+        res = model.xe_step(fc, att, case.labels.cuda(), case.lmasks.cuda(), label_smoothing=case.smoothing, seed=SEED, att_masks=reg, **rates)
+        lp = res['logprobs']
+    else:
+        import imagecaptioning.pytorch_b200 as b200
+        table = b200.rewards.CiderDTable(case.df, case.ref_len)
+        kw = dict(forced_tokens=case.tok.cuda(), att_masks=reg, seed=SEED, **rates)
+        if case.kind == 'greedy':
+            res = model.scst_step(fc, att, case.gts, table, SPI, forced_baseline=case.base.cuda(), **kw)
+            assert torch.equal(res['greedy_seq'].cpu(), case.base)
+        else:
+            res = model.scst_step(fc, att, case.gts, table, SPI, baseline='leave_one_out', **kw)
+        assert torch.equal(res['sample_seq'].cpu(), case.tok)
+        lp = res['sample_logprobs']
+    torch.cuda.synchronize()
+    out = dict(loss=float(res['loss']), lp=lp.detach().cpu(), grads={name_of[id(p)]: g.detach().cpu() for p, g in res['grads'].items()})
+    if case.kind != 'xe':
+        out['reward'] = res['reward'].detach().cpu()
+    return out
+
+
+def _compare(family, mode, case):
+    t0 = time.time()
+    got = _run_engine(family, mode, case)
+    ref = case.ref
+    if mode == 'tc_f16x3':
+        loss_c, picked_c, g_c = case.reference_tf32x3()
+        oname, factor = '3xTF32 oracle', 4.0
+    else:
+        loss_c, picked_c, g_c = ref['loss32'], ref['picked32'], ref['g32']
+        oname, factor = 'fp32 oracle', 4.0
+    label = '[%s %s %s drop=%s N=%d%s]' % (family, mode, case.kind + ('' if case.kind != 'xe' else ' ls=%g' % case.smoothing), case.dropout,
+                                           case.N, ' regions' if case.regions is not None else '')
+    print('%s float64 reference %.1f s; ReLU units left out per layer %s, %d ambiguous maxout units' % (label, case.ref_seconds, case.kink_rows,
+                                                                                                       len(case.maxout)))
+    assert all(v <= 0.15 * case.c["H"] for v in case.kink_rows.values()), case.kink_rows        # some rows of the layer, not the layer
+    # scalars: loss (not for the autograd case, whose objective is a sum over every log-prob), picked log-probs, reward
+    if 'loss' in got:
+        n, l1 = ref['l1']
+        floor = max(1e-6, 2.0 ** -24 * np.log2(n) * l1)
+        ec = abs(loss_c - ref['loss64'])
+        e = abs(got['loss'] - ref['loss64'])
+        print('%s loss %.6f err %.2e bar %.2e (%s %.2e)' % (label, ref['loss64'], e, _scalar_bar(ec, floor, factor), oname, ec))
+        assert e <= _scalar_bar(ec, floor, factor), ('loss', e, ec, floor)
+        assert abs(ref['loss64']) > 1e-3 or case.kind == 'leave_one_out'
+    picked = case.picked(got['lp']).double()
+    ec = float((picked_c - ref['picked64']).abs().max())
+    e = float((picked - ref['picked64']).abs().max())
+    print('%s picked log-probs err %.2e bar %.2e (%s %.2e)' % (label, e, _scalar_bar(ec, 1e-6, factor), oname, ec))
+    assert e <= _scalar_bar(ec, 1e-6, factor), ('picked log-probs', e, ec)
+    if 'reward' in got:
+        ec = float((case.reward.float().double() - case.reward).abs().max())
+        e = float((got['reward'].double() - case.reward).abs().max())
+        assert e <= _scalar_bar(ec, 1e-6, factor), ('reward', e, ec)
+        assert float(case.reward.abs().max()) > 1e-2
+    # gradients; the float64 side re-routed at the ambiguous maxout units the way the engine went
+    g64, moved = (_fit_maxout(case, got['grads']) if case.maxout else (ref['g64'], 0))
+    if case.maxout:
+        print('%s maxout units re-routed to fit the engine: %d of %d' % (label, moved, len(case.maxout)))
+    # the fp32 oracle followed float64's routing: it is measured against the float64 gradients before the re-routing
+    gc = {k: g_c[k].double() + (g64[k] - ref['g64'][k]) for k in g64}
+    # a weight gradient reduces over every (step, row) pair; rounding of a sequential fp32 accumulation grows as the square root of that
+    # length (simt_fp32's gemm_wgrad_launch: core.lang_lstm.weight_ih measured at 0.43 / 0.62 / 1.03 of the fixed 2e-6 floor for 1000 / 3200
+    # / 6400 pairs), so the floor does.  In tc_f16x3 the calibrating oracle's own error is the larger term.
+    floor = 2e-6 * max(1.0, case.N * case.steps / 1000) ** 0.5
+    worst = check_grads_f64(got['grads'], g64, gc, keep=case.keep, label=label, floor=floor, factor=factor)
+    print('%s worst gradient err/bar %.3f; compared in %.1f s' % (label, worst, time.time() - t0))
+
+
+MODES = ['tc_f16x3', 'simt_fp32']
+STEPS = [('greedy', 0.0), ('leave_one_out', 0.0), ('xe', 0.0), ('xe', 0.1)]
+
+
+def _run(family, mode, kind, smoothing, dropout, B):
+    case = _reference(family, kind, dropout, B, smoothing, kind == 'leave_one_out', _masks_fn(family), 1 if family == 'att2in2' else len(MODES))
+    if dropout:
+        _check_masks(family, case.drop)
+    _compare(family, mode, case)
+
+
+@pytest.mark.parametrize('dropout', [False, True])
+@pytest.mark.parametrize('kind,smoothing', STEPS)
+@pytest.mark.parametrize('mode', MODES)
+def test_updown_step_f64(mode, kind, smoothing, dropout):
+    _run('updown', mode, kind, smoothing, dropout, 10)
+
+
+@pytest.mark.parametrize('B', [32, pytest.param(64, marks=pytest.mark.slow)])
+@pytest.mark.parametrize('kind,smoothing', [('greedy', 0.0), ('xe', 0.1)])
+@pytest.mark.parametrize('mode', MODES)
+def test_updown_step_f64_rows(mode, kind, smoothing, B):
+    """160 and 320 rows per step.  In tc_f16x3 the per-step GEMMs run gemm_tf32's swapped tile of width 256 (160 rows) and its normal
+    orientation (320 rows); in simt_fp32 the same steps at larger M through gemm_generic."""
+    _run('updown', mode, kind, smoothing, True, B)
+
+
+@pytest.mark.parametrize('dropout', [False, True])
+@pytest.mark.parametrize('kind,smoothing', STEPS)
+@pytest.mark.parametrize('mode', ['simt_fp32'])
+def test_att2in2_step_f64(mode, kind, smoothing, dropout):
+    """simt_fp32 only: see the module docstring on Att2in2's maxout in tc_f16x3."""
+    _run('att2in2', mode, kind, smoothing, dropout, 10)
+
+
+@pytest.mark.parametrize('dropout', [False, True])
+@pytest.mark.parametrize('kind,smoothing', STEPS)
+@pytest.mark.parametrize('mode', MODES)
+def test_aoa_step_f64(mode, kind, smoothing, dropout):
+    _run('aoa', mode, kind, smoothing, dropout, 10)
+
+
+@pytest.mark.parametrize('family,mode', [(f, m) for f in ('updown', 'att2in2', 'aoa') for m in MODES if (f, m) != ('att2in2', 'tc_f16x3')])
+def test_autograd_teacher_f64(family, mode):
+    """model.autograd: teacher-forced log-probs under grad and the backward of a seeded upstream gradient (logsoftmax_vjp_kernel<4>:
+    V + 1 = 9488 is a multiple of 4)."""
+    case = _reference(family, 'autograd', False, 10, 0.0, True, None, 1 if family == 'att2in2' else len(MODES))
+    _compare(family, mode, case)

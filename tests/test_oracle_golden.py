@@ -297,3 +297,33 @@ def test_transformer_training_steps_of_the_reference(golden_dir):
     loss = co.reward_criterion(lp, seq, torch.from_numpy(reward).float())
     assert abs(float(loss) - float(g['sc_loss'])) < 1e-5
     grads_of(loss, Wg, 'sc_')
+
+
+@pytest.mark.parametrize('family', ['updown', 'att2in2', 'aoa'])
+def test_oracle_runs_in_float64(family):
+    """Given float64 weights and features the oracle computes in float64 throughout (its state, sampled and teacher-forced log-prob
+    buffers follow the inputs' dtype), and agrees with its float32 self within 1e-5 of each tensor's largest entry."""
+    import att2in2_oracle as ao
+    V, E, H, A, F_fc, F_att, T, B, R, n = 30, 16, 24, 12, 20, 20, 6, 3, 5, 2
+    W = co.make_weights(family, V, E, H, A, F_fc, F_att, seed=3, logit_scale=3.0)
+    fc, att = co.make_inputs(B, R, F_fc, F_att, seed=2)
+    masks = torch.ones(B, R)
+    masks[1, 3:] = 0
+    tok = torch.randint(1, V + 1, (B * n, T), generator=torch.Generator().manual_seed(1))
+    tok[0, 2:] = 0
+    reward = torch.randn(B * n, 1, generator=torch.Generator().manual_seed(4)).expand(-1, T)
+    out = {}
+    for dt in (torch.float32, torch.float64):
+        Wg = {k: v.to(dt, copy=True).requires_grad_(True) for k, v in W.items()}
+        fam = ao.Att2in2Family(Wg, T) if family == 'att2in2' else co.Family(family, Wg, T, heads=4)
+        _, lp = co.sample(fam, fc.to(dt), att.to(dt), masks, sample_method='sample', sample_n=n, forced_tokens=tok)
+        tf = co.forward_teacher(fam, fc.to(dt), att.to(dt), torch.cat([torch.zeros(B * n, 1, dtype=torch.long), tok], 1).view(B, n, -1), masks)
+        assert lp.dtype == dt and tf.dtype == dt
+        (co.reward_criterion(lp, tok, reward.to(dt)) + tf.sum() * 1e-3).backward()
+        assert all(v.grad is not None and v.grad.dtype == dt for v in Wg.values())
+        out[dt] = (lp.detach(), {k: v.grad for k, v in Wg.items()})
+    (lp32, g32), (lp64, g64) = out[torch.float32], out[torch.float64]
+    assert float((lp64 - lp32.double()).abs().max()) <= 1e-5 * float(lp64.abs().max())
+    largest = max(float(v.abs().max()) for v in g64.values())
+    for k in g64:          # tensors whose true gradient is zero (alpha_net.bias, attention key biases) hold fp32 noise of the step's size
+        assert float((g64[k] - g32[k].double()).abs().max()) <= 1e-5 * float(g64[k].abs().max()) + 1e-7 * largest, k
