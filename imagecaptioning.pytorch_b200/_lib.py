@@ -87,6 +87,10 @@ class ScstOpts(Structure):
 BASELINE_GREEDY, BASELINE_LEAVE_ONE_OUT = 0, 1
 
 
+class PpoOpts(Structure):
+    _fields_ = [('cliprange', c_float), ('kl_coef', c_float)]
+
+
 class AoaScstOpts(Structure):
     _fields_ = [('sample_n', c_int), ('temperature', c_float), ('seed', c_ulonglong), ('upstream', c_float), ('baseline', c_int),
                 ('drop_prob_lm', c_float), ('drop_attn', c_float), ('drop_aoa', c_float), ('drop_sublayer', c_float), ('ctx_drop', c_int),
@@ -333,6 +337,18 @@ SIGNATURES = {
                                    c_void_p, c_void_p]),
     'capb200_tfm_scst_vjp': (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(TfmScstOpts), POINTER(VjpOpts), POINTER(TfmWeights), c_void_p,
                                      c_void_p, c_void_p]),
+    # PPO steps: (engine, old engine, [fc,] att, B, R, opts, ppo, table, refs, ref_offsets, L, grads, sample_seq, sample_logprobs, scores, loss,
+    #             pg_loss, kl_loss, clipfrac, stream)
+    'capb200_updown_ppo_step': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), POINTER(PpoOpts), c_void_p, c_void_p,
+                                        c_void_p, c_int, c_void_p] + [c_void_p] * 8),
+    'capb200_att2in2_ppo_step': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), POINTER(PpoOpts), c_void_p, c_void_p,
+                                         c_void_p, c_int, c_void_p] + [c_void_p] * 8),
+    'capb200_newfc_ppo_step': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(ScstOpts), POINTER(PpoOpts), c_void_p, c_void_p,
+                                       c_void_p, c_int, c_void_p] + [c_void_p] * 8),
+    'capb200_aoa_ppo_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(AoaScstOpts), POINTER(PpoOpts), c_void_p, c_void_p, c_void_p,
+                                     c_int, c_void_p] + [c_void_p] * 8),
+    'capb200_tfm_ppo_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(TfmScstOpts), POINTER(PpoOpts), c_void_p, c_void_p, c_void_p,
+                                     c_int, c_void_p] + [c_void_p] * 8),
 }
 
 _lib = None

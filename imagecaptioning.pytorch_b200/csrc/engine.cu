@@ -1448,6 +1448,26 @@ int check_train_feats(const capb200_engine* e, int family, const float* fc, cons
     return 0;
 }
 
+// The PPO entry points of UpDown, Att2in2 and NewFC: the family's sampled step `step(ta, stream)` with the PPO criterion, the old policy's
+// teacher-forced pass on `old`'s decode path.
+template <class Step>
+int ppo_entry(capb200_engine* e, capb200_engine* old, int family, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+              const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L, const void* grads,
+              long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss, float* kl_loss, float* clipfrac, cudaStream_t st,
+              Step step) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && loss, "null argument");
+    CAPB_REQUIRE(R >= 0, "R must be >= 0");
+    if (check_train_feats(e, family, fc, att, R, opts->att_masks)) return 1;
+    TrainArgs ta;
+    if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, nullptr, sample_logprobs, nullptr, loss, e->T, &ta)) return 1;
+    return run_ppo_step(e, old, ppo, ta, B, scores, pg_loss, kl_loss, clipfrac, st,
+                        [&](const capb200_sample_opts* so, const long long* tok, float* lo, void* s) {
+                            return capb200_decode_sample(old, fc, att, ta.mask, B, R, so, tok, e->T, nullptr, lo, nullptr, s);
+                        },
+                        [&] { return step(ta, st); });
+}
+
 }  // namespace
 
 // The UpDown, Att2in2 and NewFC entry points take the shared option structs (capb200_scst_opts / capb200_xe_opts) with the same meaning.
@@ -1503,6 +1523,33 @@ extern "C" int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const
     if (scst_train_args(B, *opts, table, refs, ref_offsets, L, sample_seq, greedy_seq, sample_logprobs, reward, loss, e->T, &ta)) return 1;
     return run_scst_step(e, opts, grads, ta, fc, sizeof(float) * (size_t)B * e->cfg.fc_feat_size, nullptr, 0, B, R, static_cast<cudaStream_t>(stream),
                          [&](const float* fc_s, const float*, const TrainArgs& t, cudaStream_t s) { return newfc_train_step(e, fc_s, B, t, grads, s); });
+}
+
+extern "C" int capb200_updown_ppo_step(capb200_engine* e, capb200_engine* old, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                                       const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                                       const capb200_updown_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss,
+                                       float* pg_loss, float* kl_loss, float* clipfrac, void* stream) {
+    return ppo_entry(e, old, CAPB200_FAMILY_UPDOWN, fc, att, B, R, opts, ppo, table, refs, ref_offsets, L, grads, sample_seq, sample_logprobs, scores, loss,
+                     pg_loss, kl_loss, clipfrac, static_cast<cudaStream_t>(stream),
+                     [&](const TrainArgs& ta, cudaStream_t st) { return updown_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_att2in2_ppo_step(capb200_engine* e, capb200_engine* old, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                                        const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                                        const capb200_att2in2_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss,
+                                        float* pg_loss, float* kl_loss, float* clipfrac, void* stream) {
+    return ppo_entry(e, old, CAPB200_FAMILY_ATT2IN2, fc, att, B, R, opts, ppo, table, refs, ref_offsets, L, grads, sample_seq, sample_logprobs, scores, loss,
+                     pg_loss, kl_loss, clipfrac, static_cast<cudaStream_t>(stream),
+                     [&](const TrainArgs& ta, cudaStream_t st) { return att2in2_train_step(e, fc, att, B, R, ta, grads, st); });
+}
+
+extern "C" int capb200_newfc_ppo_step(capb200_engine* e, capb200_engine* old, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B,
+                                      int R, const capb200_scst_opts* opts, const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs,
+                                      const int* ref_offsets, int L, const capb200_newfc_grads* grads, long long* sample_seq, float* sample_logprobs,
+                                      float* scores, float* loss, float* pg_loss, float* kl_loss, float* clipfrac, void* stream) {
+    return ppo_entry(e, old, CAPB200_FAMILY_NEWFC, fc, nullptr, B, R, opts, ppo, table, refs, ref_offsets, L, grads, sample_seq, sample_logprobs, scores, loss,
+                     pg_loss, kl_loss, clipfrac, static_cast<cudaStream_t>(stream),
+                     [&](const TrainArgs& ta, cudaStream_t st) { return newfc_train_step(e, fc, B, ta, grads, st); });
 }
 
 extern "C" int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,

@@ -215,6 +215,20 @@ int scst_drop_worst_launch(const long long* seq, const float* row_loss, int N, i
 int xe_loss_backward_launch(const float* logp, long ld_row, const long long* labels, long ld_l, const float* masks, long ld_m, int N, int steps, int Ls, int V1,
                             float smoothing, float upstream, float* mask_sum, float* item_loss, float* dl, float* loss, cudaStream_t st, int keep = 0,
                             float* row_loss = nullptr, float* row_msum = nullptr, float* row_coef = nullptr);
+// PPO (losses.py:267-357).  ppo_shift: the old policy's input words [0, seq[:, :-1]] [N, T].  ppo_loss_backward: from the sampled log-probs lp
+// (pitch ld_lp between sequences), the old policy's lo [N, T, V1], the per-row advantage adv [N] and the hypothesis scores [N]: d loss / d logits
+// into dl [N, T, V1], scores_out [N] (fp32), the per-row losses row_loss [N] (reduction 'none'), pg_loss / kl_loss / clipfrac, and loss: the
+// reduction 'mean' loss, or with keep > 0 the mean of the `keep` smallest row losses (drop_worst), whose rows alone get gradients.
+struct PpoScratch {
+    float* terms;       // [3, N, T]: masked pg, kl and clip terms
+    float* row_msum;    // [N]
+    float* row_coef;    // [N]
+    float* mask_sum;    // [1]
+};
+int ppo_shift_launch(const long long* seq, int N, int T, long long* tokens_in, cudaStream_t st);
+int ppo_loss_backward_launch(const float* lp, long ld_lp, const float* lo, const long long* seq, const float* adv, const double* scores, int N, int T, int V1,
+                             float cliprange, float kl_coef, float upstream, int keep, const PpoScratch& s, float* dl, float* scores_out, float* loss,
+                             float* row_loss, float* pg_loss, float* kl_loss, float* clipfrac, cudaStream_t st);
 // Backward of log_softmax for an outside gradient g = dL/dlogp over [N, T, V1] rows (pitch ld_row between sequences): dl [N, T, V1] =
 // g - exp(logp) * rowsum(g); with seq [N, T] (sampling form) the rows of sequences finished before step t get zero.
 int logsoftmax_vjp_launch(const float* logp, const float* g, long ld_row, const long long* seq, int N, int T, int V1, float* dl, cudaStream_t st);

@@ -7,6 +7,7 @@
 //   lstm_cell_backward       nn.LSTMCell (AttModel.py:628,635)
 //   maxout_cell_backward     Att2in2Core's maxout cell (AttModel.py:773-787) and NewFC's LSTMCore (FCModel.py:25-42)
 //   attention_backward       models/AttModel.py:728-748
+//   ppo                      modules/losses.py:267-357 (PPOLoss) composed with F.log_softmax
 // Dropout masks are never stored: keep(seed, site, step, element) is a pure function (Philox4x32-10), re-evaluated in the backward.
 #include <type_traits>
 
@@ -232,6 +233,134 @@ __global__ void __launch_bounds__(256) drop_worst_select_kernel(const float* __r
         __syncthreads();
     }
     if (threadIdx.x == 0) *loss = sh[0] / (float)k;
+}
+
+// ---- PPO (losses.py:267-357): the clipped policy-ratio loss against a frozen old policy plus a token-level KL penalty.
+// lp [N, T, V1] are the new policy's sampled log-probs, lo [N, T, V1] the old policy's teacher-forced ones over the same words,
+// mask[n, t] = 1 for t = 0 or seq[n, t-1] > 0.
+// The old policy's input words: [0, seq[:, :-1]] (losses.py:319)
+__global__ void ppo_shift_kernel(const long long* __restrict__ seq, int N, int T, long long* __restrict__ tokens_in) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N * T) return;
+    const int t = i % T;
+    tokens_in[i] = t == 0 ? 0 : seq[i - 1];
+}
+
+// single CTA: each row's mask count and their total
+__global__ void __launch_bounds__(256) ppo_mask_kernel(const long long* __restrict__ seq, int N, int T, float* __restrict__ row_msum,
+                                                       float* __restrict__ mask_sum) {
+    __shared__ float sh[256];
+    float acc = 0.f;
+    for (int n = threadIdx.x; n < N; n += 256) {
+        float ms = 0.f;
+        for (int t = 0; t < T; ++t) ms += (t == 0 || seq[(long)n * T + t - 1] > 0) ? 1.f : 0.f;
+        row_msum[n] = ms;
+        acc += ms;
+    }
+    sh[threadIdx.x] = acc;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+        if (threadIdx.x < w) sh[threadIdx.x] += sh[threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *mask_sum = sh[0];
+}
+
+// One CTA per (n, t).  ratio = exp(lp[seq] - lo[seq]); pg = max(-adv ratio, -adv clamp(ratio, 1 - eps, 1 + eps)); kl = sum_v exp(lo) (lo - lp)
+// (F.kl_div(lp, lo, log_target=True)); clip = |ratio - 1| > eps.  The gradient G = d loss / d lp of the row, scaled by coef:
+//   at the picked word  -adv ratio when the unclamped branch is taken (inside the clip range torch.maximum splits the gradient between two
+//                       equal branches whose sum is that), 0 when the clamped one is larger;
+//   on every word       -kl_coef exp(lo_v);
+// and the log-softmax backward folded in: dl = G - exp(lp) sum(G).  coef = mask * upstream / sum(mask) (reduction 'mean'), or mask alone for
+// drop_worst, whose per-row coefficient is applied after the selection (ppo_scale_rows_kernel).  terms [3][N*T]: masked pg, kl, clip.
+__global__ void __launch_bounds__(256) ppo_row_kernel(const float* __restrict__ lp, long ld_lp, const float* __restrict__ lo, const long long* __restrict__ seq,
+                                                      const float* __restrict__ adv, const float* __restrict__ mask_sum, float upstream, bool per_row,
+                                                      float eps, float kl_coef, int T, int V1, float* __restrict__ dl, float* __restrict__ terms) {
+    __shared__ float red[2][32];
+    const long item = blockIdx.x;                 // n * T + t
+    const long NT = (long)gridDim.x;
+    const int t = (int)(item % T);
+    const long n = item / T;
+    float* d = dl + item * V1;
+    const float m = (t == 0 || seq[n * T + t - 1] > 0) ? 1.f : 0.f;
+    if (m == 0.f) {
+        for (int v = threadIdx.x; v < V1; v += blockDim.x) d[v] = 0.f;
+        if (threadIdx.x == 0) terms[item] = terms[NT + item] = terms[2 * NT + item] = 0.f;
+        return;
+    }
+    const float* p = lp + n * ld_lp + (long)t * V1;
+    const float* q = lo + item * V1;
+    float kl = 0.f, so = 0.f;
+    for (int v = threadIdx.x; v < V1; v += blockDim.x) {
+        const float l = q[v], e = expf(l);
+        kl += e * (l - p[v]);
+        so += e;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        kl += __shfl_xor_sync(0xffffffffu, kl, o);
+        so += __shfl_xor_sync(0xffffffffu, so, o);
+    }
+    if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = kl; red[1][threadIdx.x >> 5] = so; }
+    __syncthreads();
+    kl = 0.f; so = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { kl += red[0][w]; so += red[1][w]; }
+    const long long tok = seq[item];
+    const float a = adv[n];
+    const float ratio = expf(p[tok] - q[tok]);
+    const float clamped = fminf(fmaxf(ratio, 1.f - eps), 1.f + eps);
+    const float pg1 = -a * ratio, pg2 = -a * clamped;
+    const bool unclamped = (ratio >= 1.f - eps && ratio <= 1.f + eps) || pg1 > pg2;
+    const float g_pick = unclamped ? -a * ratio : 0.f;
+    const float coef = per_row ? m : m * upstream / (*mask_sum);
+    const float gsum = coef * (g_pick - kl_coef * so);
+    for (int v = threadIdx.x; v < V1; v += blockDim.x) {
+        const float g = coef * ((v == tok ? g_pick : 0.f) - kl_coef * expf(q[v]));
+        d[v] = g - expf(p[v]) * gsum;
+    }
+    if (threadIdx.x == 0) {
+        terms[item] = fmaxf(pg1, pg2);
+        terms[NT + item] = kl;
+        terms[2 * NT + item] = fabsf(ratio - 1.f) > eps ? 1.f : 0.f;
+    }
+}
+
+// single CTA: the masked means (pg_loss, kl_loss, clipfrac, and loss = pg_loss + kl_coef kl_loss), each row's masked mean of
+// pg + kl_coef kl (reduction 'none'), and the rewarded scores in fp32 (losses.py:302: scores.type_as(input))
+__global__ void __launch_bounds__(256) ppo_reduce_kernel(const float* __restrict__ terms, const float* __restrict__ row_msum, const double* __restrict__ scores,
+                                                         int N, int T, float kl_coef, float* __restrict__ row_loss, float* __restrict__ scores_out,
+                                                         float* __restrict__ loss, float* __restrict__ pg_loss, float* __restrict__ kl_loss,
+                                                         float* __restrict__ clipfrac) {
+    __shared__ float sh[4][256];
+    const long NT = (long)N * T;
+    float a_pg = 0.f, a_kl = 0.f, a_cl = 0.f, a_m = 0.f;
+    for (int n = threadIdx.x; n < N; n += 256) {
+        float r_pg = 0.f, r_kl = 0.f, r_cl = 0.f;
+        for (int t = 0; t < T; ++t) {
+            const long i = (long)n * T + t;
+            r_pg += terms[i]; r_kl += terms[NT + i]; r_cl += terms[2 * NT + i];
+        }
+        const float ms = row_msum[n];
+        row_loss[n] = (r_pg + kl_coef * r_kl) / ms;
+        scores_out[n] = (float)scores[n];
+        a_pg += r_pg; a_kl += r_kl; a_cl += r_cl; a_m += ms;
+    }
+    sh[0][threadIdx.x] = a_pg; sh[1][threadIdx.x] = a_kl; sh[2][threadIdx.x] = a_cl; sh[3][threadIdx.x] = a_m;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+        if (threadIdx.x < w)
+            for (int k = 0; k < 4; ++k) sh[k][threadIdx.x] += sh[k][threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const float pg = sh[0][0] / sh[3][0], kl = sh[1][0] / sh[3][0];
+        *pg_loss = pg; *kl_loss = kl; *clipfrac = sh[2][0] / sh[3][0];
+        if (loss != nullptr) *loss = pg + kl_coef * kl;
+    }
+}
+
+// drop_worst: row n of d logits [N, cols] times row_coef[n] (upstream / (k * row mask count) for kept rows, 0 for dropped ones)
+__global__ void ppo_scale_rows_kernel(float* __restrict__ dl, long n, long cols, const float* __restrict__ row_coef) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) dl[i] *= row_coef[i / cols];
 }
 
 // nn.LSTMCell backward (gate pre-activations saved): dgates [rows, 4H] (i,f,g,o) and dc_prev from dh, dc
@@ -501,6 +630,28 @@ int xe_loss_backward_launch(const float* logp, long ld_row, const long long* lab
         LAUNCH_OK();
     }
     xe_loss_kernel<<<1, 256, 0, st>>>(item_loss, N, steps, Ls, masks, ld_m, smoothing, V1, mask_sum, loss);
+    LAUNCH_OK();
+}
+int ppo_shift_launch(const long long* seq, int N, int T, long long* tokens_in, cudaStream_t st) {
+    ppo_shift_kernel<<<cdiv(N * T, 256), 256, 0, st>>>(seq, N, T, tokens_in);
+    LAUNCH_OK();
+}
+int ppo_loss_backward_launch(const float* lp, long ld_lp, const float* lo, const long long* seq, const float* adv, const double* scores, int N, int T, int V1,
+                             float cliprange, float kl_coef, float upstream, int keep, const PpoScratch& s, float* dl, float* scores_out, float* loss,
+                             float* row_loss, float* pg_loss, float* kl_loss, float* clipfrac, cudaStream_t st) {
+    CAPB_REQUIRE(keep >= 0 && keep <= N, "drop_worst: the number of kept rows must be in 0..rows");
+    ppo_mask_kernel<<<1, 256, 0, st>>>(seq, N, T, s.row_msum, s.mask_sum);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    ppo_row_kernel<<<N * T, 256, 0, st>>>(lp, ld_lp, lo, seq, adv, s.mask_sum, upstream, keep > 0, cliprange, kl_coef, T, V1, dl, s.terms);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    ppo_reduce_kernel<<<1, 256, 0, st>>>(s.terms, s.row_msum, scores, N, T, kl_coef, row_loss, scores_out, keep > 0 ? nullptr : loss, pg_loss, kl_loss, clipfrac);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    if (keep > 0) {
+        drop_worst_select_kernel<<<1, 256, 0, st>>>(row_loss, s.row_msum, N, keep, upstream, s.row_coef, loss);
+        CAPB_CHECK_CUDA(cudaGetLastError());
+        const long cols = (long)T * V1;
+        ppo_scale_rows_kernel<<<nblocks(N * cols), 256, 0, st>>>(dl, N * cols, cols, s.row_coef);
+    }
     LAUNCH_OK();
 }
 int logsoftmax_vjp_launch(const float* logp, const float* g, long ld_row, const long long* seq, int N, int T, int V1, float* dl, cudaStream_t st) {

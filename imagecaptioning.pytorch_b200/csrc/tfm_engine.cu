@@ -620,6 +620,25 @@ extern "C" int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, in
                          [&](const float*, const float* att_s, const TfmTrainArgs& t, cudaStream_t s) { return tfm_train_step(e, att_s, B, R, t, grads, s); });
 }
 
+// PPO (include/capb200.h: capb200_ppo_opts): the sampled step with the PPO criterion; the old policy's teacher-forced pass runs on `old`.
+extern "C" int capb200_tfm_ppo_step(capb200_tfm_engine* e, capb200_tfm_engine* old, const float* att, int B, int R, const capb200_tfm_scst_opts* opts,
+                                    const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                                    const capb200_tfm_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
+                                    float* kl_loss, float* clipfrac, void* stream) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && loss, "null argument");
+    CAPB_REQUIRE(R >= 1, "attention features required");
+    TfmTrainArgs ta;
+    if (tfm_rates(*opts, &ta) ||
+        scst_train_args(B, shared_opts(*opts), table, refs, ref_offsets, L, sample_seq, nullptr, sample_logprobs, nullptr, loss, e->T, &ta)) return 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return run_ppo_step(e, old, ppo, ta, B, scores, pg_loss, kl_loss, clipfrac, st,
+                        [&](const capb200_sample_opts* so, const long long* tok, float* lo, void* s) {
+                            return capb200_tfm_decode_sample(old, att, ta.mask, B, R, so, tok, e->T, nullptr, lo, nullptr, s);
+                        },
+                        [&] { return tfm_train_step(e, att, B, R, ta, grads, st); });
+}
+
 // The autograd entry points (include/capb200.h: capb200_vjp_opts) on the Transformer's option structs.
 extern "C" int capb200_tfm_xe_vjp(capb200_tfm_engine* e, const float* att, int B, int R, const capb200_tfm_xe_opts* opts, const capb200_vjp_opts* vjp,
                                   const long long* labels, int label_cols, const capb200_tfm_grads* grads, float* logprobs, void* stream) {

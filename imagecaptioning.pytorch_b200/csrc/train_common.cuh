@@ -4,6 +4,8 @@
 // keeps its prologue, its core step, the backward through time and the weight gradients.
 #pragma once
 #include <cmath>
+#include <cstring>
+#include <functional>
 
 #include "engine_common.cuh"
 
@@ -11,6 +13,17 @@ namespace capb200 {
 
 // an fp32-only view (no fp16 planes) of a row-major activation
 inline ActView f32_view(float* f, long ld) { return ActView{f, nullptr, nullptr, ld}; }
+
+// The PPO criterion of a sampled step (run_ppo_step): its options, outputs, the scratch it keeps on the old policy's engine, and the old policy's
+// teacher-forced pass old_pass(tokens_in [N, T], lo [N, T, V1], stream).
+struct PpoArgs {
+    float cliprange = 0.2f, kl_coef = 0.02f;
+    float *scores = nullptr, *pg_loss = nullptr, *kl_loss = nullptr, *clipfrac = nullptr;
+    long long* tokens_in = nullptr;
+    float *lo = nullptr, *adv = nullptr;
+    PpoScratch s{};
+    std::function<int(const long long*, float*, cudaStream_t)> old_pass;
+};
 
 // One training step: SCST (sampled words, reward-weighted loss) or XE (teacher-forced words, cross-entropy).
 struct TrainArgs {
@@ -46,6 +59,8 @@ struct TrainArgs {
     int baseline_method = CAPB200_SAMPLE_GREEDY;
     float baseline_top = 0.f;
     const long long* forced_baseline = nullptr;
+    // PPO in place of RewardCriterion (leave-one-out advantage, no eval-mode baseline)
+    const PpoArgs* ppo = nullptr;
 
     // The weighted reward runs only when it can differ from CIDEr-D alone: a BLEU weight <= 0 adds weight * 0.
     bool weighted_reward() const { return !xe && (w_bleu > 0.0 || w_cider != 1.0); }
@@ -272,6 +287,20 @@ inline int train_vocab_step(const TrainArgs& ta, const StepTape& tp, int N, int 
     return vocab_step_launch(va, st);
 }
 
+// PPO's loss and d loss / d logits into tp.DL: the old policy's teacher-forced pass over [0, seq[:, :-1]], the reward with the leave-one-out
+// advantage (losses.py:300-306), then the clipped-ratio + KL criterion.
+inline int ppo_loss_backward(const TrainArgs& ta, const StepTape& tp, int B, int N, int V1, cudaStream_t st) {
+    const PpoArgs& pa = *ta.ppo;
+    const int T = ta.T;
+    if (ppo_shift_launch(ta.sample_seq, N, T, pa.tokens_in, st) || pa.old_pass(pa.tokens_in, pa.lo, st)) return 1;
+    if (!ta.weighted_reward()) {
+        if (cider_reward_launch(ta.table->t, ta.sample_seq, N, nullptr, B, T, ta.refs, ta.ref_offsets, ta.L, tp.scores, pa.adv, 1, 1, st)) return 1;
+    } else if (weighted_reward_launch(ta.table ? ta.table->t : nullptr, ta.w_cider, ta.w_bleu, ta.sample_seq, N, nullptr, B, T, ta.refs, ta.ref_offsets, ta.L,
+                                      tp.scores, tp.scores + N + B, pa.adv, 1, 1, st)) return 1;
+    return ppo_loss_backward_launch(ta.logprobs, (long)ta.Tl * V1, pa.lo, ta.sample_seq, pa.adv, tp.scores, N, T, V1, pa.cliprange, pa.kl_coef, ta.upstream,
+                                    ta.keep, pa.s, tp.DL, pa.scores, ta.loss, ta.row_loss ? ta.row_loss : tp.row_loss, pa.pg_loss, pa.kl_loss, pa.clipfrac, st);
+}
+
 // The loss and d loss / d logits into tp.DL: the XE criterion (LanguageModelCriterion / LabelSmoothing), or -- after joining the greedy
 // baseline -- the reward (CIDEr-D, or the weighted CIDEr-D + BLEU-4), RewardCriterion, drop_worst and the d logits of the SCST loss.
 inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const StepBaseline& gb, int B, int N, int V1, cudaStream_t st) {
@@ -283,6 +312,7 @@ inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const StepBase
     if (ta.xe)
         return xe_loss_backward_launch(ta.logprobs, ld_lp, ta.labels, ta.ld_labels, ta.masks, ta.ld_masks, N, T, ta.Tl, V1, ta.smoothing, ta.upstream,
                                        tp.mask_sum, tp.item_loss, tp.DL, ta.loss, st, ta.keep, row_loss, tp.row_msum, tp.row_coef);
+    if (ta.ppo != nullptr) return ppo_loss_backward(ta, tp, B, N, V1, st);
     if (gb.join(st)) return 1;     // the reward needs the baseline captions
     const long long* greedy = ta.greedy_baseline ? ta.greedy_seq : nullptr;
     if (!ta.weighted_reward()) {
@@ -395,6 +425,51 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
     const int rc = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return counted(staged(0), staged(1), ts, gst); });
     if (e->sg.leave(st, gst)) return 1;
     return rc;
+}
+
+// Runs one PPO step eagerly: `step()` is the family's sampled training step with ta.ppo set.  The old policy `old` is an engine of the same
+// family and configuration whose weights stay frozen; its teacher-forced pass, old_pass(opts, tokens_in, lo, stream) -- the family's
+// capb200_*decode_sample on `old` -- runs in eval mode on the step's stream, and the criterion's scratch (lo [N, T, V1], the shifted words, the
+// advantage and the per-position terms) lives on the old engine's training tape, which nothing else uses while it does not train.
+template <class Engine, class Args, class OldPass, class Step>
+int run_ppo_step(Engine* e, Engine* old, const capb200_ppo_opts* po, Args& ta, int B, float* scores, float* pg_loss, float* kl_loss, float* clipfrac,
+                 cudaStream_t st, OldPass old_pass, Step step) {
+    CAPB_REQUIRE(po && old && scores && pg_loss && kl_loss && clipfrac, "null argument");
+    if (check_ready(old)) return 1;
+    CAPB_REQUIRE(old != e, "the old policy needs an engine of its own");
+    CAPB_REQUIRE(memcmp(&old->cfg, &e->cfg, sizeof(e->cfg)) == 0, "the old policy's engine must have the family and configuration of the new one");
+    CAPB_REQUIRE(!ta.greedy_baseline, "PPO takes the leave-one-out advantage: baseline must be CAPB200_BASELINE_LEAVE_ONE_OUT");
+    CAPB_REQUIRE(std::isfinite(po->cliprange) && po->cliprange > 0.f && std::isfinite(po->kl_coef) && po->kl_coef >= 0.f,
+                 "PPO needs cliprange > 0 and kl_coef >= 0");
+    const int n = ta.n, N = B * n, T = ta.T;
+    const size_t NT = (size_t)N * T;
+    PpoArgs pa;
+    pa.cliprange = po->cliprange; pa.kl_coef = po->kl_coef;
+    pa.scores = scores; pa.pg_loss = pg_loss; pa.kl_loss = kl_loss; pa.clipfrac = clipfrac;
+    auto layout = [&](Arena& a) {
+        pa.lo = a.take<float>(NT * e->V1);
+        pa.tokens_in = a.take<long long>(NT);
+        pa.adv = a.take<float>(N);
+        pa.s.terms = a.take<float>(3 * NT);
+        pa.s.row_msum = a.take<float>(N); pa.s.row_coef = a.take<float>(N); pa.s.mask_sum = a.take<float>(1);
+    };
+    Arena dry;
+    layout(dry);
+    if (grow_buffer(reinterpret_cast<void**>(&old->tape), &old->tape_bytes, dry.off + 256, st)) return 1;
+    Arena ar;
+    ar.base = old->tape;
+    layout(ar);
+    capb200_sample_opts so;
+    memset(&so, 0, sizeof(so));
+    so.edits.unk_col = -1; so.sample_n = n; so.method = CAPB200_SAMPLE_TEACHER; so.temperature = 1.f; so.steps = T;
+    pa.old_pass = [&](const long long* tok, float* lo, cudaStream_t s) { return old_pass(&so, tok, lo, static_cast<void*>(s)); };
+    ta.ppo = &pa;
+    // the launches PPO adds to the sampled step's count: the word shift, and the criterion's three against RewardCriterion's two
+    return run_eager_step(st, [&] {
+        const int rc = step();
+        e->launches += ta.reward_extra_launches() + 2;
+        return rc;
+    });
 }
 
 }  // namespace capb200

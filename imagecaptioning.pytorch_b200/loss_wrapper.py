@@ -8,9 +8,12 @@ sc_flag=True follows loss_wrapper.py:56-73 exactly: the eval-mode baseline (opt.
 reward (``cider_reward_weight * CIDEr-D + bleu_reward_weight * BLEU-4``) and RewardCriterion -- every stage on the device through the C ABI.  sc_flag=False is the XE stage
 (loss_wrapper.py:54-55: teacher-forced forward + LanguageModelCriterion / LabelSmoothing) and struc_flag=True the structure-loss
 branch (loss_wrapper.py:25-53) with ``structure_loss_type='new_self_critical'`` (losses.py:168-187), the recipe of the reference's
-best models; both run as one fused device step incl. the backward pass (UpDown, Att2in2, NewFC, AoANet, Transformer).
+best models, or with ``use_ppo=1`` the PPO loss (losses.py:267-357) against a frozen old policy loaded from ``ppo_old_model_path``; each
+runs as one fused device step incl. the backward pass (UpDown, Att2in2, NewFC, AoANet, Transformer).
 """
 from __future__ import annotations
+
+import copy
 
 import torch
 import torch.nn as nn
@@ -200,11 +203,32 @@ class _DropWorstLoss(torch.autograd.Function):
         return (None, None, None, None, None) + tuple(None for _ in ctx.params)
 
 
+def ppo_old_model(model, path):
+    """The frozen old policy of PPO (losses.py:271-290): a copy of ``model`` with the state dict saved at ``path`` -- a PyTorch-Lightning
+    checkpoint is unwrapped first -- in eval mode and without gradients."""
+    assert path is not None, 'Must provide old model path for PPO'
+    old = copy.deepcopy(model)
+    dev = next(model.parameters()).device
+    # the reference's own torch.load of a trainer checkpoint, whose Lightning form also pickles the vocabulary and the options
+    state_dict = torch.load(path, map_location=dev, weights_only=False)
+    if 'pytorch-lightning_version' in state_dict:
+        state_dict = state_dict['state_dict']
+        del state_dict['_vocab']
+        del state_dict['_opt']
+    old.load_state_dict(state_dict)
+    old.eval()
+    for p_ in old.parameters():
+        p_.requires_grad = False
+    return old
+
+
 class B200LossWrapper(nn.Module):
     def __init__(self, model, opt):
         super().__init__()
         self.opt = opt
         self.model = model
+        # PPO's frozen old policy (loss_wrapper.py:15 -> losses.PPOLoss), built only with use_ppo
+        self.old_model = ppo_old_model(model, getattr(opt, 'ppo_old_model_path', None)) if getattr(opt, 'use_ppo', 0) == 1 else None
         smoothing = getattr(opt, 'label_smoothing', 0)
         self.crit = LabelSmoothing(smoothing=smoothing) if smoothing > 0 else LanguageModelCriterion()      # loss_wrapper.py:10-13
         self.rl_crit = RewardCriterion()
@@ -301,6 +325,23 @@ class B200LossWrapper(nn.Module):
         self.last_step = res
         return res
 
+    def _ppo_step(self, fc_feats, att_feats, gts, att_masks, drop_worst_flag):
+        """PPOLoss (losses.py:291-357) as one fused step: the train-mode samples, the old policy's teacher-forced pass, the reward with the
+        leave-one-out advantage, the clipped-ratio + KL criterion and the backward."""
+        opt = self.opt
+        self.model.train()
+        keep = self._keep_rows(len(gts) * opt.train_sample_n, drop_worst_flag)
+        w = self._weights()
+        extra = {} if w is None else {'reward_weights': w}
+        if opt.train_sample_method != 'sample':
+            extra['sample_method'] = opt.train_sample_method
+        res = self.model.ppo_step(self.old_model, fc_feats, att_feats, gts, self._scorer(), opt.train_sample_n,
+                                  cliprange=getattr(opt, 'ppo_cliprange', 0.2), kl_coef=getattr(opt, 'ppo_kl_coef', 0.02), att_masks=att_masks,
+                                  keep_rows=keep, **extra)
+        res['keep_rows'] = keep
+        self.last_step = res
+        return res
+
     def forward(self, fc_feats, att_feats, labels, masks, att_masks, gts, gt_indices, sc_flag, struc_flag, drop_worst_flag):
         opt = self.opt
         out = {}
@@ -311,22 +352,37 @@ class B200LossWrapper(nn.Module):
             w = opt.structure_loss_weight
             lm_loss = self._xe_loss(fc_feats, att_feats, labels, masks, att_masks, drop_worst_flag, snapshot=w > 0) if w < 1 else \
                 torch.zeros((), device=fc_feats.device)
+            use_ppo = getattr(opt, 'use_ppo', 0) == 1
             if w > 0:
-                if getattr(opt, 'use_ppo', 0) or opt.structure_loss_type != 'new_self_critical' or not can_fuse:
+                if use_ppo:
+                    # PPO reads sample_logprobs as log-probs (loss_wrapper.py:31-32): a margin loss without struc_use_logsoftmax hands it logits
+                    ltype = opt.structure_loss_type
+                    if not (getattr(opt, 'struc_use_logsoftmax', 0) or ltype == 'softmax_margin' or 'margin' not in ltype):
+                        raise NotImplementedError('PPO on logits (output_logsoftmax=0) is out of scope of the engine')
+                    if not hasattr(self.model, 'ppo_step') or not can_fuse:
+                        raise NotImplementedError('PPO runs on the fused step: train_sample_method ' + _FUSED_SAMPLERS)
+                elif opt.structure_loss_type != 'new_self_critical' or not can_fuse:
                     raise NotImplementedError("the structure-loss branch covers structure_loss_type='new_self_critical' on the fused SCST steps")
                 if getattr(opt, 'entropy_reward_weight', 0) > 0 or getattr(opt, 'self_cider_reward_weight', 0) > 0:
                     raise NotImplementedError('entropy / self-CIDEr rewards are out of scope of the engine')
                 gts = [gts[_] for _ in gt_indices.tolist()]
                 if drop_worst_flag and 0 < w < 1:
                     raise NotImplementedError('drop_worst with a mixed XE / structure loss: the two fused steps would select rows independently')
-                res = self._sampled_step(fc_feats, att_feats, gts, 'leave_one_out', att_masks, drop_worst_flag)
-                rw = self._weights()
-                # out['reward'] is the score the step rewarded, in fp32 as losses.py:61-62 casts it
-                scores = cider_scores(gts, res['sample_seq']) if rw is None else weighted_scores(gts, res['sample_seq'], rw)
-                struc = {'loss': self._bridge(res), 'reward': scores.float().view(-1, opt.train_sample_n)}
+                if use_ppo:
+                    res = self._ppo_step(fc_feats, att_feats, gts, att_masks, drop_worst_flag)
+                    struc = {'loss': self._bridge(res), 'reward': res['scores'].clone()}
+                    ppo_out = {k: res[k].clone() for k in ('pg_loss', 'kl_loss', 'clipfrac')}
+                else:
+                    res = self._sampled_step(fc_feats, att_feats, gts, 'leave_one_out', att_masks, drop_worst_flag)
+                    rw = self._weights()
+                    # out['reward'] is the score the step rewarded, in fp32 as losses.py:61-62 casts it
+                    scores = cider_scores(gts, res['sample_seq']) if rw is None else weighted_scores(gts, res['sample_seq'], rw)
+                    struc = {'loss': self._bridge(res), 'reward': scores.float().view(-1, opt.train_sample_n)}
             else:
                 struc = {'loss': torch.zeros((), device=fc_feats.device), 'reward': torch.zeros((), device=fc_feats.device)}
             out['lm_loss'], out['struc_loss'], out['reward'] = lm_loss, struc['loss'], struc['reward']
+            if use_ppo and w > 0:
+                out.update(ppo_out)
             out['loss'] = (1 - w) * lm_loss + w * struc['loss']
             return out
         if not sc_flag:

@@ -634,6 +634,59 @@ class B200CaptionModel(nn.Module):
         return {'loss': loss[0], 'reward': reward, 'sample_seq': sample_seq, 'greedy_seq': None if loo else greedy_seq, 'sample_logprobs': logprobs,
                 'grads': self._grads_of(fg, slots), 'seed': seed, 'flat': fg, 'row_loss': row_loss}
 
+    # ---- PPO step: train-mode samples + the frozen old policy's teacher-forced pass + reward + clipped-ratio / KL criterion + BPTT -------------
+    @_on_device
+    def ppo_step(self, old_model, fc_feats, att_feats, gts, table, sample_n, cliprange=0.2, kl_coef=0.02, temperature=1.0, seed=None, upstream=1.0,
+                 forced_tokens=None, att_masks=None, keep_rows=0, reward_weights=None, sample_method='sample', **rates):
+        """One PPO step on the device (capb200_<family>_ppo_step; PPOLoss, losses.py:267-357): the train-mode samples of scst_step, the
+        teacher-forced pass of ``old_model`` -- a frozen model of the same family and configuration -- in eval mode over [0, seq[:, :-1]],
+        the reward (CIDEr-D, or ``reward_weights`` = (cider, bleu)) with the leave-one-out advantage, then
+        ``pg_loss + kl_coef * kl_loss`` with the policy ratio clipped to [1 - cliprange, 1 + cliprange] and the gradients of the new policy.
+        ``rates`` are the family's dropout rates as its scst_step takes them (drop_prob; the Transformer's dropout; AoANet's drop_attn, ...).
+        ``keep_rows`` > 0 is drop_worst: the loss is the mean of the keep_rows smallest per-row losses ('row_loss' holds every row's).
+        Returns {'loss', 'pg_loss', 'kl_loss', 'clipfrac' (0-dim), 'scores' [B, n] (the rewarded scores, out['reward']), 'sample_seq',
+        'sample_logprobs', 'grads', 'flat', 'seed', 'row_loss'}."""
+        from .rewards import pack_references, weights_struct
+        if self._entry is None:
+            raise NotImplementedError('%s has no fused PPO step' % type(self).__name__)
+        if old_model is self or type(old_model) is not type(self) or bytes(old_model._cfg()) != bytes(self._cfg()):
+            raise ValueError('ppo_step needs an old model of its own with the family and configuration of this one')
+        if int(sample_n) < 2:
+            raise ValueError("PPO's leave-one-out advantage needs sample_n >= 2")
+        lead = fc_feats if self._takes_fc else att_feats
+        rw = weights_struct(reward_weights, gts)
+        sampler, _keep, temperature = _scst_sampler(sample_method, 'greedy', None, True, lead.shape[0], self.seq_length, self.vocab_size + 1,
+                                                    temperature, lead.device)
+        lib = self._ensure_engine(lead.device)
+        old_model._ensure_engine(lead.device)
+        feats, masks, B, R = self._train_feats(fc_feats, att_feats, att_masks)
+        dev = feats[0].device
+        N, T, V1 = B * sample_n, self.seq_length, self.vocab_size + 1
+        refs, offsets, L = pack_references(gts, dev)
+        slots = self._grad_slots()
+        fg, g = self._grad_table(lib, dev, slots)
+        sample_seq, logprobs, scores, stats = self._step_buffers(('ppo', B, sample_n), lambda: (
+            torch.zeros(N, T, dtype=torch.long, device=dev), torch.zeros(N, T, V1, dtype=torch.float32, device=dev),
+            torch.empty(N, dtype=torch.float32, device=dev), torch.empty(4, dtype=torch.float32, device=dev)))
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        forced = None
+        if forced_tokens is not None:
+            forced = forced_tokens.detach().to(device=dev, dtype=torch.long).contiguous()
+            assert forced.shape == (N, T)
+        row_loss = torch.empty(N, dtype=torch.float32, device=dev) if keep_rows else None
+        so = self._scst_opts(sample_n, float(temperature), seed, float(upstream), _lib.BASELINE_LEAVE_ONE_OUT, self._rates(True, **rates), forced, masks,
+                             int(keep_rows), row_loss, sampler, None if rw is None else ctypes.pointer(rw))
+        po = _lib.PpoOpts(float(cliprange), float(kl_coef))
+        entry = 'capb200_%s_ppo_step' % self._entry
+        _lib.check(getattr(lib, entry)(self._engine, old_model._engine, *map(_lib.ptr, feats), B, R, ctypes.byref(so), ctypes.byref(po),
+                                       table.handle_for(refs), _lib.ptr(refs), _lib.ptr(offsets), L, ctypes.byref(g), _lib.ptr(sample_seq),
+                                       _lib.ptr(logprobs), _lib.ptr(scores), *(_lib.ptr(stats[i:i + 1]) for i in range(4)), _lib.current_stream()),
+                   entry[len('capb200_'):])
+        return {'loss': stats[0], 'pg_loss': stats[1], 'kl_loss': stats[2], 'clipfrac': stats[3], 'scores': scores.view(B, sample_n),
+                'sample_seq': sample_seq, 'sample_logprobs': logprobs, 'grads': self._grads_of(fg, slots), 'seed': seed, 'flat': fg,
+                'row_loss': row_loss}
+
     @_on_device
     def xe_step(self, fc_feats, att_feats, labels, masks, label_smoothing=0.0, drop_prob=None, seed=None, upstream=1.0, att_masks=None, keep_rows=0):
         """One cross-entropy step on the device (capb200_updown_xe_step and its Att2in2 / NewFC counterparts): teacher-forced forward over ``labels[..., :-1]`` in train mode,

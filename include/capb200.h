@@ -745,6 +745,47 @@ int capb200_tfm_scst_step(capb200_tfm_engine* e, const float* att, int B, int R,
 int capb200_tfm_set_grad_events(capb200_tfm_engine* e, void* const* events, int n);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * PPO fine-tuning (LossWrapper with opt.use_ppo, losses.py:267-357; loss_wrapper.py:39-53) of every family: one fused step of
+ *   (1) the family's sampled forward in train mode, exactly as its *_scst_step draws it (opts: sample_n >= 2, temperature, seed, dropout
+ *       rates, forced_tokens, att_masks, keep_rows / row_loss, sampler, reward_weights; baseline must be CAPB200_BASELINE_LEAVE_ONE_OUT);
+ *   (2) the frozen old policy's teacher-forced pass over [0, seq[:, :-1]] on `old` -- an engine of the same family and configuration
+ *       holding the old weights -- in eval mode, on `stream`; its log-probs lo [N, T, V+1] stay on `old`'s training tape;
+ *   (3) the reward (cider * CIDEr-D + bleu * BLEU-4) and the leave-one-out advantage adv = s - mean of the image's other samples;
+ *   (4) the criterion, mask[n, t] = 1 for t = 0 or seq[n, t-1] > 0, ratio = exp(lp[seq] - lo[seq]), eps = ppo->cliprange:
+ *       pg = max(-adv ratio, -adv clamp(ratio, 1 - eps, 1 + eps)), kl = sum_v exp(lo_v) (lo_v - lp_v) over the full row,
+ *       pg_loss / kl_loss / clipfrac = masked means of pg, kl and |ratio - 1| > eps,
+ *       loss = pg_loss + kl_coef * kl_loss (reduction 'mean'), or with keep_rows > 0 the mean of the keep_rows smallest per-row masked
+ *       means of pg + kl_coef * kl (drop_worst; row_loss receives every row's);
+ *   (5) the backward through the new policy alone, into grads (every buffer OVERWRITTEN).
+ * Outputs: sample_seq [N, T] int64, sample_logprobs [N, T, V+1], scores [N] (the rewarded scores in fp32, out['reward']), loss, pg_loss,
+ * kl_loss, clipfrac [1].  The step runs eagerly (no CUDA graph); `old` must not be used by another call until it returns.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct {
+    float cliprange;           /* ppo_cliprange (0.2), > 0 */
+    float kl_coef;             /* ppo_kl_coef (0.02), >= 0 */
+} capb200_ppo_opts;
+int capb200_updown_ppo_step(capb200_engine* e, capb200_engine* old, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                            const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                            const capb200_updown_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
+                            float* kl_loss, float* clipfrac, void* stream);
+int capb200_att2in2_ppo_step(capb200_engine* e, capb200_engine* old, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                             const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                             const capb200_att2in2_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
+                             float* kl_loss, float* clipfrac, void* stream);
+int capb200_newfc_ppo_step(capb200_engine* e, capb200_engine* old, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts,
+                           const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                           const capb200_newfc_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
+                           float* kl_loss, float* clipfrac, void* stream);
+int capb200_aoa_ppo_step(capb200_aoa_engine* e, capb200_aoa_engine* old, const float* att, int B, int R, const capb200_aoa_scst_opts* opts,
+                         const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                         const capb200_aoa_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
+                         float* kl_loss, float* clipfrac, void* stream);
+int capb200_tfm_ppo_step(capb200_tfm_engine* e, capb200_tfm_engine* old, const float* att, int B, int R, const capb200_tfm_scst_opts* opts,
+                         const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
+                         const capb200_tfm_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
+                         float* kl_loss, float* clipfrac, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Autograd entry points of every family: the forward of the fused training steps without their criterion, and the backward of a
  * caller-given dL/dlogprobs, so that any loss written in PyTorch trains an engine model (models.py: model.autograd).
  *   *_xe_vjp    teacher form: the forward of the family's xe_step over labels[..., :label_cols-1] (scheduled sampling included; the
