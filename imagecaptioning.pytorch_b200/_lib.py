@@ -220,6 +220,10 @@ SIGNATURES = {
     'capb200_engine_create': (c_void_p, [POINTER(ModelCfg)]),
     'capb200_engine_destroy': (None, [c_void_p]),
     'capb200_engine_bind_weights': (c_int, [c_void_p, POINTER(Weights), c_void_p]),
+    'capb200_engine_set_logit_layers': (c_int, [c_void_p, c_int]),
+    'capb200_engine_bind_logit_head': (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    'capb200_engine_bind_logit_head_grads': (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p)]),
+    'capb200_engine_set_logit_dropout': (c_int, [c_void_p, c_float]),
     'capb200_decode_beam': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),
     'capb200_decode_beam_form': (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p,
@@ -244,6 +248,10 @@ SIGNATURES = {
     'capb200_aoa_create': (c_void_p, [POINTER(AoaCfg)]),
     'capb200_aoa_destroy': (None, [c_void_p]),
     'capb200_aoa_bind_weights': (c_int, [c_void_p, POINTER(AoaWeights), c_void_p]),
+    'capb200_aoa_set_logit_layers': (c_int, [c_void_p, c_int]),
+    'capb200_aoa_bind_logit_head': (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    'capb200_aoa_bind_logit_head_grads': (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_void_p)]),
+    'capb200_aoa_set_logit_dropout': (c_int, [c_void_p, c_float]),
     'capb200_aoa_decode_beam': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, POINTER(BeamOpts), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p]),
     'capb200_aoa_beam_record_logprobs': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -96,6 +96,7 @@ void layout_workspace(capb200_aoa_engine* e, Arena& a, int B, int rows, int R, i
     e->t2.carve(a, rows, 2 * H, false);
     e->ld_c = round_up(H, 8);
     for (int i = 0; i < 2; ++i) e->c0[i] = a.take<float>((long)rows * e->ld_c);
+    e->carve_head(a, rows);
     e->d.carve(a, B, rows, beam, T);
 }
 
@@ -232,9 +233,11 @@ int core_step(capb200_aoa_engine* e, int rows, int rpi, const int* tokens, const
     }
     e->launches++;
     if (glu_launch(rows, H, e->t2.v.f, e->t2.v.ld, nullptr, 0, e->ctx_out.v, st)) return 1;
+    ActView x;
+    if (e->run_logit_head(e->ctx_out.v, rows, &x, st)) return 1;
     GemmProblem g;
     g.M = rows; g.N = e->V1; g.nseg = 1;
-    g.seg[0] = seg_of(e->ctx_out.v, w.logit_w, H, e->p_logit, H);
+    g.seg[0] = seg_of(x, w.logit_w, H, e->p_logit, H);
     g.epi.bias = w.logit_b;
     g.epi.C = logits; g.epi.ldc = ld_logits;
     return e->gemm(A_LOGIT, g, e->capRows, st);
@@ -314,6 +317,26 @@ int capb200_aoa_bind_weights(capb200_aoa_engine* e, const capb200_aoa_weights* w
     // per-token gate table: relu(embed) * W_ih[:, 0:E]^T
     if (build_gate_table(*e, w->embed, E, H, w->att_lstm_w_ih, E + H, e->p_ih_x, e->xgate, e->ld_xgate, st)) return 1;
     return e->finish_bind(st);
+}
+
+int capb200_aoa_set_logit_layers(capb200_aoa_engine* e, int logit_layers) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->set_logit_layers(logit_layers, e->H);
+}
+
+int capb200_aoa_bind_logit_head(capb200_aoa_engine* e, const float* const* w, const float* const* b, void* stream) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->bind_logit_head(w, b, static_cast<cudaStream_t>(stream));
+}
+
+int capb200_aoa_bind_logit_head_grads(capb200_aoa_engine* e, float* const* gw, float* const* gb) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->bind_logit_head_grads(gw, gb);
+}
+
+int capb200_aoa_set_logit_dropout(capb200_aoa_engine* e, float p) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->set_logit_dropout(p);
 }
 
 int capb200_aoa_decode_beam(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq,
@@ -413,6 +436,7 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
 
     ATape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](ATape& t, Arena& a) { layout_atape(t, a, B, R, N, T, E, H, heads, V1); })) return 1;
+    if (head_train_tape(e, (long)T * N, st)) return 1;
     // ---- (1) greedy baseline, eval mode: the regular decode path, forked here, enqueued after the prologue
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;         // decode workspace sized before anything is in flight
     StepBaseline gb;
@@ -487,7 +511,10 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
         }
         float* outd = tp.outd + (long)t * H;                                   // [N][T][H]: batched logit backward
         if (glu_dropout_launch(N, H, t2, 2 * H, out_t, H, outd, (long)T * H, seed, t, p_lm, st)) return 1;
-        if (sk.lin(outd, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        const float* lin_in;
+        long ld_in;
+        if (head_train_forward(e, sk, outd, (long)T * H, N, T, t, seed, &lin_in, &ld_in, st)) return 1;
+        if (sk.lin(lin_in, ld_in, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
         if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 15;
     }
@@ -497,7 +524,7 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
     if (ta.forward_only) return 0;
     CAPB_NVTX("capb200 aoa train step: reward, loss, backward, weight gradients");
     const capb200_aoa_grads& G = *grads;
-    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.outd, tp.dOUTD, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
+    if (loss_and_logit_backward(e, ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.outd, tp.dOUTD, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dctx, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc, 0, sizeof(float) * NH, st));
@@ -593,7 +620,7 @@ int aoa_train_step(capb200_aoa_engine* e, const float* att, int B, int R, const 
 extern "C" int capb200_aoa_scst_step(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_scst_opts* opts,
                                      const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L, const capb200_aoa_grads* grads,
                                      long long* sample_seq, long long* greedy_seq, float* sample_logprobs, float* reward, float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     AoaTrainArgs ta;
@@ -608,7 +635,7 @@ extern "C" int capb200_aoa_ppo_step(capb200_aoa_engine* e, capb200_aoa_engine* o
                                     const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
                                     const capb200_aoa_grads* grads, long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss,
                                     float* kl_loss, float* clipfrac, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     AoaTrainArgs ta;
@@ -626,7 +653,7 @@ extern "C" int capb200_aoa_set_grad_events(capb200_aoa_engine* e, void* const* e
 
 extern "C" int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_xe_opts* opts, const long long* labels,
                                    const float* masks, int label_cols, const capb200_aoa_grads* grads, float* logprobs, float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && att && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     AoaTrainArgs ta;
@@ -638,7 +665,7 @@ extern "C" int capb200_aoa_xe_step(capb200_aoa_engine* e, const float* att, int 
 // The autograd entry points (include/capb200.h: capb200_vjp_opts) on AoANet's option structs.
 extern "C" int capb200_aoa_xe_vjp(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_xe_opts* opts, const capb200_vjp_opts* vjp,
                                   const long long* labels, int label_cols, const capb200_aoa_grads* grads, float* logprobs, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && att && labels && logprobs && (grads || vjp->forward_only), "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     AoaTrainArgs ta;
@@ -649,7 +676,7 @@ extern "C" int capb200_aoa_xe_vjp(capb200_aoa_engine* e, const float* att, int B
 
 extern "C" int capb200_aoa_scst_vjp(capb200_aoa_engine* e, const float* att, int B, int R, const capb200_aoa_scst_opts* opts, const capb200_vjp_opts* vjp,
                                     const capb200_aoa_grads* grads, long long* sample_seq, float* sample_logprobs, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && att && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
     CAPB_REQUIRE(R >= 1, "attention features required");
     capb200_scst_opts shared = shared_opts(*opts);

@@ -193,6 +193,7 @@ void layout_workspace(capb200_engine* e, Arena& a, int B, int rows, int R, int b
         e->c0[i] = a.take<float>((long)rows * e->ld_c);
         e->c1[i] = a.take<float>((long)rows * e->ld_c);
     }
+    e->carve_head(a, rows);
     e->img_of_row = a.take<int>(rows);
     e->att_score = a.take<float>((long)rows * (R > 0 ? R : 1));
     e->d.carve(a, B, rows, beam, T);
@@ -282,12 +283,24 @@ int prepare(capb200_engine* e, const float* fc, const float* att, const float* m
     return 0;
 }
 
+// ---- the vocabulary projection of the core's output `h` (through the logit head's hidden layers, if any) into the caller's log-prob storage
+int logit_gemm(capb200_engine* e, const ActView& h, int rows, float* logits, long ld_logits, cudaStream_t st) {
+    ActView x;
+    if (e->run_logit_head(h, rows, &x, st)) return 1;
+    GemmProblem g;
+    g.M = rows; g.N = e->V1; g.nseg = 1;
+    g.seg[0] = seg_of(x, e->w.logit_w, e->H, e->p_logit, e->H);
+    g.epi.bias = e->w.logit_b;
+    g.epi.C = logits; g.epi.ldc = ld_logits;
+    return run_gemm(e, G_LOGIT, g, e->capRows, st);
+}
+
 // ---- one application of the recurrent core on `rows` rows (rpi rows per image) -----------------------------------------
 // tokens: input word per row; src_row: parent row per row (nullptr = identity, e->neg1 = fresh zero state)
 // states_gathered (UpDown): h0_in / h1_in already hold the parents' states (the previous step's beam_search_step_kernel wrote them)
 int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int* src_row, float* logits, long ld_logits, int n_images, int R,
               const float* mask, cudaStream_t st, bool states_gathered = false) {
-    const int H = e->H, E = e->E, A = e->A, V1 = e->V1;
+    const int H = e->H, E = e->E, A = e->A;
     const capb200_weights& w = e->w;
     if (e->cfg.family == CAPB200_FAMILY_UPDOWN) {
         StateCopy s0, s1;
@@ -359,15 +372,7 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
                                       nullptr, 0, nullptr, st)) return 1;
         }
         e->core_cur = nxt;
-        {   // vocabulary projection straight into the caller's log-prob storage
-            GemmProblem g;
-            g.M = rows; g.N = V1; g.nseg = 1;
-            g.seg[0] = seg_of(e->h1_out.v, w.logit_w, H, e->p_logit, H);
-            g.epi.bias = w.logit_b;
-            g.epi.C = logits; g.epi.ldc = ld_logits;
-            if (run_gemm(e, G_LOGIT, g, e->capRows, st)) return 1;
-        }
-        return 0;
+        return logit_gemm(e, e->h1_out.v, rows, logits, ld_logits, st);
     }
     if (e->cfg.family == CAPB200_FAMILY_ATT2IN2) {
         // ---- Att2in2 (AttModel.py:770-790): attention on the PREVIOUS h, maxout cell whose candidate pair also gets a2c(att_res).
@@ -408,12 +413,7 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
         e->launches++;
         if (maxout_pointwise_launch(rows, H, e->gates.v.f, e->gates.v.ld, src_row, e->c0[cur], e->ld_c, e->c0[nxt], e->ld_c, e->h0_out.v, st)) return 1;
         e->core_cur = nxt;
-        GemmProblem g;
-        g.M = rows; g.N = V1; g.nseg = 1;
-        g.seg[0] = seg_of(e->h0_out.v, w.logit_w, H, e->p_logit, H);
-        g.epi.bias = w.logit_b;
-        g.epi.C = logits; g.epi.ldc = ld_logits;
-        return run_gemm(e, G_LOGIT, g, e->capRows, st);
+        return logit_gemm(e, e->h0_out.v, rows, logits, ld_logits, st);
     }
     // ---- NewFC: maxout LSTM; a fresh state first consumes the image embedding (AttModel.py:925-936)
     const bool fresh = (src_row == e->d.neg1);
@@ -439,12 +439,7 @@ int core_step(capb200_engine* e, int rows, int rpi, const int* tokens, const int
         if (maxout_pointwise_launch(rows, H, e->gates.v.f, e->gates.v.ld, srcs, e->c0[cur], e->ld_c, e->c0[nxt], e->ld_c, e->h0_out.v, st)) return 1;
         e->core_cur = nxt;
     }
-    GemmProblem g;
-    g.M = rows; g.N = V1; g.nseg = 1;
-    g.seg[0] = seg_of(e->h0_out.v, w.logit_w, H, e->p_logit, H);
-    g.epi.bias = w.logit_b;
-    g.epi.C = logits; g.epi.ldc = ld_logits;
-    return run_gemm(e, G_LOGIT, g, e->capRows, st);
+    return logit_gemm(e, e->h0_out.v, rows, logits, ld_logits, st);
 }
 
 }  // namespace
@@ -666,6 +661,26 @@ int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, voi
     // per-token gate table: relu(embed)[V+1,E] * W_ih[:, 2H:2H+E]^T
     if (updown && build_gate_table(*e, w->embed, E, H, w->att_lstm_w_ih + 2 * H, E + 2 * H, e->p_a_ih_x, e->xgate, e->ld_xgate, st)) return 1;
     return e->finish_bind(st);
+}
+
+int capb200_engine_set_logit_layers(capb200_engine* e, int logit_layers) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->set_logit_layers(logit_layers, e->H);
+}
+
+int capb200_engine_bind_logit_head(capb200_engine* e, const float* const* w, const float* const* b, void* stream) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->bind_logit_head(w, b, static_cast<cudaStream_t>(stream));
+}
+
+int capb200_engine_bind_logit_head_grads(capb200_engine* e, float* const* gw, float* const* gb) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->bind_logit_head_grads(gw, gb);
+}
+
+int capb200_engine_set_logit_dropout(capb200_engine* e, float p) {
+    CAPB_REQUIRE(e != nullptr, "null engine");
+    return e->set_logit_dropout(p);
 }
 
 int capb200_decode_beam(capb200_engine* e, const float* fc, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts,
@@ -1081,6 +1096,7 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     // ---- (1) greedy baseline, eval mode (no dropout): the regular decode path
     Tape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](Tape& t, Arena& a) { layout_tape(t, a, B, R, N, T, E, H, A, V1); })) return 1;
+    if (head_train_tape(e, (long)T * N, st)) return 1;
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;        // decode workspace sized before anything is in flight
     StepBaseline gb;
     if (start_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
@@ -1144,7 +1160,10 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
         // core output = dropout(h_lang), stored in (n, t) order for the batched logit backward
         float* out = tp.out + (long)t * H;
         if (dropout_copy_launch(h1, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
-        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        const float* lin_in;
+        long ld_in;
+        if (head_train_forward(e, sk, out, (long)T * H, N, T, t, seed, &lin_in, &ld_in, st)) return 1;
+        if (sk.lin(lin_in, ld_in, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
         if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 12;
     }
@@ -1155,7 +1174,7 @@ int updown_train_step(capb200_engine* e, const float* fc, const float* att, int 
     CAPB_NVTX("capb200 train step: reward, loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_updown_grads& G = *grads;
-    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
+    if (loss_and_logit_backward(e, ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh0, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc0, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh1, 0, sizeof(float) * NH, st));
@@ -1235,6 +1254,7 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
 
     MaxoutTape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](MaxoutTape& t, Arena& a) { layout_maxout_tape(t, a, B, R, N, T, E, H, A, V1); })) return 1;
+    if (head_train_tape(e, (long)T * N, st)) return 1;
     if (ensure_workspace(e, B, N, R, 1, st)) return 1;
     StepBaseline gb;
     if (start_baseline(e, fc, att, B, R, ta, tp, gb, st)) return 1;
@@ -1278,7 +1298,10 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
         // core output = dropout(h), stored in (n, t) order for the batched logit backward
         float* out = tp.out + (long)t * H;
         if (dropout_copy_launch(h, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
-        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        const float* lin_in;
+        long ld_in;
+        if (head_train_forward(e, sk, out, (long)T * H, N, T, t, seed, &lin_in, &ld_in, st)) return 1;
+        if (sk.lin(lin_in, ld_in, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
         if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 11;
     }
@@ -1289,7 +1312,7 @@ int att2in2_train_step(capb200_engine* e, const float* fc, const float* att, int
     CAPB_NVTX("capb200 att2in2 train step: loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_att2in2_grads& G = *grads;
-    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
+    if (loss_and_logit_backward(e, ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.d_att_e, 0, sizeof(float) * BR * H, st));
@@ -1346,6 +1369,7 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
 
     MaxoutTape tp;
     if (carve_tape(&e->tape, &e->tape_bytes, tp, st, [&](MaxoutTape& t, Arena& a) { layout_newfc_tape(t, a, B, N, T, E, H, V1); })) return 1;
+    if (head_train_tape(e, (long)T * N, st)) return 1;
     if (ensure_workspace(e, B, N, 1, 1, st)) return 1;      // R = 1: the region count the greedy baseline's decode call sizes its workspace for
     StepBaseline gb;
     if (start_baseline(e, fc, nullptr, B, 0, ta, tp, gb, st)) return 1;
@@ -1391,7 +1415,10 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
         // core output = dropout(h) (FCModel.py:40), stored in (n, t) order for the batched logit backward
         float* out = tp.out + (long)t * H;
         if (dropout_copy_launch(h, H, out, (long)T * H, N, H, seed, 3, (unsigned)t, p, st)) return 1;
-        if (sk.lin(out, (long)T * H, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
+        const float* lin_in;
+        long ld_in;
+        if (head_train_forward(e, sk, out, (long)T * H, N, T, t, seed, &lin_in, &ld_in, st)) return 1;
+        if (sk.lin(lin_in, ld_in, w.logit_w, H, w.logit_b, ta.logprobs + (long)t * V1, ld_lp, N, V1, H, 0)) return 1;
         if (train_vocab_step(ta, tp, N, V1, t, st)) return 1;
         e->launches += 7;
     }
@@ -1402,7 +1429,7 @@ int newfc_train_step(capb200_engine* e, const float* fc, int B, const TrainArgs&
     CAPB_NVTX("capb200 newfc train step: loss, backward through time, weight gradients");
     const long TN = (long)T * N;
     const capb200_newfc_grads& G = *grads;
-    if (loss_and_logit_backward(ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
+    if (loss_and_logit_backward(e, ta, tp, gb, sk, B, N, V1, H, w.logit_w, tp.out, tp.dOUT, G.logit_w, G.logit_b, e->grad_events[0], st)) return 1;
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dh, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(tp.dc, 0, sizeof(float) * NH, st));
     CAPB_CHECK_CUDA(cudaMemsetAsync(G.embed, 0, sizeof(float) * (size_t)V1 * E, st));
@@ -1455,7 +1482,7 @@ int ppo_entry(capb200_engine* e, capb200_engine* old, int family, const float* f
               const capb200_ppo_opts* ppo, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L, const void* grads,
               long long* sample_seq, float* sample_logprobs, float* scores, float* loss, float* pg_loss, float* kl_loss, float* clipfrac, cudaStream_t st,
               Step step) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
     if (check_train_feats(e, family, fc, att, R, opts->att_masks)) return 1;
@@ -1475,7 +1502,7 @@ extern "C" int capb200_updown_scst_step(capb200_engine* e, const float* fc, cons
                                         const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
                                         const capb200_updown_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
                                         float* reward, float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     if (check_train_feats(e, CAPB200_FAMILY_UPDOWN, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
@@ -1489,7 +1516,7 @@ extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, con
                                          const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
                                          const capb200_att2in2_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
                                          float* reward, float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     if (check_train_feats(e, CAPB200_FAMILY_ATT2IN2, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
@@ -1502,7 +1529,7 @@ extern "C" int capb200_att2in2_scst_step(capb200_engine* e, const float* fc, con
 extern "C" int capb200_att2in2_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
                                        const long long* labels, const float* masks, int label_cols, const capb200_att2in2_grads* grads, float* logprobs,
                                        float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && labels && masks && grads && logprobs && loss, "null argument");
     if (check_train_feats(e, CAPB200_FAMILY_ATT2IN2, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
@@ -1515,7 +1542,7 @@ extern "C" int capb200_newfc_scst_step(capb200_engine* e, const float* fc, const
                                        const capb200_scst_opts* opts, const capb200_cider_table* table, const int* refs, const int* ref_offsets, int L,
                                        const capb200_newfc_grads* grads, long long* sample_seq, long long* greedy_seq, float* sample_logprobs,
                                        float* reward, float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && table && refs && ref_offsets && grads && sample_seq && sample_logprobs && reward && loss, "null argument");
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
     if (check_train_feats(e, CAPB200_FAMILY_NEWFC, fc, nullptr, R, opts->att_masks)) return 1;
@@ -1555,7 +1582,7 @@ extern "C" int capb200_newfc_ppo_step(capb200_engine* e, capb200_engine* old, co
 extern "C" int capb200_newfc_xe_step(capb200_engine* e, const float* fc, const float* /*att: NewFC reads the fc features only*/, int B, int R,
                                      const capb200_xe_opts* opts, const long long* labels, const float* masks, int label_cols,
                                      const capb200_newfc_grads* grads, float* logprobs, float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && labels && masks && grads && logprobs && loss, "null argument");
     CAPB_REQUIRE(R >= 0, "R must be >= 0");
     if (check_train_feats(e, CAPB200_FAMILY_NEWFC, fc, nullptr, R, opts->att_masks)) return 1;
@@ -1570,7 +1597,7 @@ extern "C" int capb200_engine_set_grad_events(capb200_engine* e, void* const* ev
 extern "C" int capb200_updown_xe_step(capb200_engine* e, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts,
                                       const long long* labels, const float* masks, int label_cols, const capb200_updown_grads* grads, float* logprobs,
                                       float* loss, void* stream) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && labels && masks && grads && logprobs && loss, "null argument");
     if (check_train_feats(e, CAPB200_FAMILY_UPDOWN, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
@@ -1585,7 +1612,7 @@ namespace {
 template <class Grads, class Step>
 int xe_vjp(capb200_engine* e, int family, const float* fc, const float* att, int B, int R, const capb200_xe_opts* opts, const capb200_vjp_opts* vjp,
            const long long* labels, int label_cols, const Grads* grads, float* logprobs, void* stream, Step step) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && labels && logprobs && (grads || vjp->forward_only), "null argument");
     if (check_train_feats(e, family, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;
@@ -1597,7 +1624,7 @@ int xe_vjp(capb200_engine* e, int family, const float* fc, const float* att, int
 template <class Grads, class Step>
 int scst_vjp(capb200_engine* e, int family, const float* fc, const float* att, int B, int R, const capb200_scst_opts* opts, const capb200_vjp_opts* vjp,
              const Grads* grads, long long* sample_seq, float* sample_logprobs, void* stream, Step step) {
-    if (check_ready(e)) return 1;
+    if (check_train_ready(e)) return 1;
     CAPB_REQUIRE(opts && vjp && sample_seq && sample_logprobs && (grads || vjp->forward_only), "null argument");
     if (check_train_feats(e, family, fc, att, R, opts->att_masks)) return 1;
     TrainArgs ta;

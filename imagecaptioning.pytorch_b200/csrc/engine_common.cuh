@@ -715,8 +715,29 @@ struct EngineBase : Workspace {
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     StepGraph sg;                    // CUDA graph of the whole SCST step
 
+    // AttModel's output head with logit_layers = k > 1 (AttModel.py:87-92): k - 1 hidden Linear(H, H) + ReLU layers between the core's
+    // output and the vocabulary projection, outside the recurrence.  Their Dropout(0.5) is a train-mode op, so no decode applies it.
+    int logit_layers = 1;
+    int head_H = 0;
+    int head_site0 = 0;                          // GEMM call site of hidden layer 0; layer i runs at head_site0 + i
+    std::vector<const float*> head_w, head_b;    // [k - 1] the caller's fp32 weights [H, H] and biases [H]
+    std::vector<Planes> head_planes;             // their split fp16 planes (tensor-core modes), in head_block
+    char* head_block = nullptr;
+    bool head_bound = false;
+    Act head_act[2];                             // the hidden activations [rows, H] of the decode workspace, layer i in head_act[i & 1]
+    // training: the gradient buffers of the hidden layers (group 0, with the vocabulary Linear), the dropout rate of the next training calls
+    // (AttModel's Dropout(0.5) in train mode, 0 in eval mode), and the tape of the k - 1 post-dropout activations [N, T, H] plus two
+    // gradient scratch slabs of the same size, grown on demand
+    std::vector<float*> head_gw, head_gb;
+    bool head_grads_bound = false;
+    float head_drop = 0.5f;
+    float* head_tape = nullptr;
+    size_t head_tape_bytes = 0;
+
     virtual ~EngineBase() {
         release();
+        cudaFree(head_block);
+        cudaFree(head_tape);
         cudaFree(wblock);
         cudaFree(tape);
         sg.destroy();
@@ -776,6 +797,83 @@ struct EngineBase : Workspace {
         bound = true;
         return 0;
     }
+
+    // ---- the logit head (logit_layers > 1) ----
+    // The depth is fixed before the first decode: the workspace and the GEMM call sites are laid out for it.
+    int set_logit_layers(int k, int H) {
+        CAPB_REQUIRE(k >= 1, "logit_layers must be >= 1");
+        if (k == logit_layers) return 0;
+        CAPB_REQUIRE(logit_layers == 1 && ws == nullptr, "logit_layers is set once, before the first decode");
+        logit_layers = k;
+        head_H = H;
+        head_site0 = (int)plans.size();
+        plans.resize(plans.size() + k - 1, nullptr);
+        head_w.assign(k - 1, nullptr);
+        head_b.assign(k - 1, nullptr);
+        head_planes.assign(k - 1, Planes());
+        head_gw.assign(k - 1, nullptr);
+        head_gb.assign(k - 1, nullptr);
+        return 0;
+    }
+    // The gradient buffers gw[i] [H, H] and gb[i] [H] of hidden layer i, OVERWRITTEN by every training call that follows.
+    int bind_logit_head_grads(float* const* gw, float* const* gb) {
+        const int n = logit_layers - 1;
+        CAPB_REQUIRE(n >= 1, "the engine has no hidden head layers: set logit_layers > 1 first");
+        CAPB_REQUIRE(gw != nullptr && gb != nullptr, "null argument");
+        for (int i = 0; i < n; ++i) CAPB_REQUIRE(gw[i] != nullptr && gb[i] != nullptr, "missing logit head gradient buffers");
+        for (int i = 0; i < n; ++i) { head_gw[i] = gw[i]; head_gb[i] = gb[i]; }
+        head_grads_bound = true;
+        return 0;
+    }
+    int set_logit_dropout(float p) {
+        CAPB_REQUIRE(p >= 0.f && p < 1.f, "the logit head's dropout rate must be in [0, 1)");
+        head_drop = p;
+        return 0;
+    }
+    // (Re)binds the hidden layers' weights w[i] [H, H] and biases b[i] [H], i < k - 1; tensor-core modes repack their planes.
+    int bind_logit_head(const float* const* w, const float* const* b, cudaStream_t st) {
+        const int n = logit_layers - 1, H = head_H;
+        CAPB_REQUIRE(n >= 1, "the engine has no hidden head layers: set logit_layers > 1 first");
+        CAPB_REQUIRE(w != nullptr && b != nullptr, "null argument");
+        for (int i = 0; i < n; ++i) CAPB_REQUIRE(w[i] != nullptr && b[i] != nullptr, "missing logit head weights");
+        if (tc && head_block == nullptr) {
+            Arena dry;
+            for (int i = 0; i < n; ++i) carve_planes(dry, H, H);
+            CAPB_CHECK_CUDA(cudaMalloc(&head_block, dry.off + 256));
+            Arena real;
+            real.base = head_block;
+            for (int i = 0; i < n; ++i) head_planes[i] = carve_planes(real, H, H);
+        }
+        for (int i = 0; i < n; ++i) {
+            head_w[i] = w[i];
+            head_b[i] = b[i];
+            if (tc && pack(w[i], H, H, H, head_planes[i], st)) return 1;
+        }
+        head_bound = true;
+        return 0;
+    }
+    // the hidden activations in a decode workspace of `rows` rows
+    void carve_head(Arena& a, long rows) {
+        if (logit_layers > 1)
+            for (Act& h : head_act) h.carve(a, rows, head_H, tc);
+    }
+    // The hidden layers on `rows` rows of the core's output `x`; *out = what the vocabulary GEMM reads (x itself when k = 1).  Each layer is
+    // one GEMM whose epilogue adds the bias, applies the ReLU and stores the fp32 row with its split planes.
+    int run_logit_head(const ActView& x, int rows, ActView* out, cudaStream_t st) {
+        ActView in = x;
+        for (int i = 0; i + 1 < logit_layers; ++i) {
+            const ActView& y = head_act[i & 1].v;
+            GemmProblem g;
+            g.M = rows; g.N = head_H; g.nseg = 1;
+            g.seg[0] = seg_of(in, head_w[i], head_H, head_planes[i], head_H);
+            g.epi.bias = head_b[i]; g.epi.relu = 1;
+            g.epi.C = y.f; g.epi.ldc = y.ld; g.epi.C_hi = y.hi; g.epi.C_lo = y.lo; g.epi.ldcs = y.ld;
+            if (gemm(head_site0 + i, g, capRows, st)) return 1;
+            in = y;
+        }
+        *out = in;
+        return 0;
+    }
 };
 
 // The checks every engine's create makes after its family's own, and the engine with the shared fields set (`sites` GEMM call sites); null
@@ -809,7 +907,15 @@ EngineBase* engine_base(capb200_aoa_engine* e);
 inline int check_ready(const EngineBase* e) {
     CAPB_REQUIRE(e != nullptr, "null engine");
     CAPB_REQUIRE(e->bound, std::string(e->bind_name) + " has not been called");
+    CAPB_REQUIRE(e->logit_layers == 1 || e->head_bound, "the logit head (logit_layers > 1) has not been bound");
     CAPB_CHECK_RANGE();
+    return 0;
+}
+
+// The training steps and the autograd entry points write the head's gradients too: they need its buffers.
+inline int check_train_ready(const EngineBase* e) {
+    if (check_ready(e)) return 1;
+    CAPB_REQUIRE(e->logit_layers == 1 || e->head_grads_bound, "the logit head's gradient buffers (logit_layers > 1) have not been bound");
     return 0;
 }
 

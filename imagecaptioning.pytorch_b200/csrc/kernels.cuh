@@ -202,6 +202,8 @@ int gemm_tf32_launch(Tf32Context* ctx, int M, int N, int nseg, const float* cons
                      float* C, long ldc, const float* bias, const float* row_bias, long ld_rb, int rpg, int accumulate, cudaStream_t st);
 const float* tf32_transposed(Tf32Context* ctx, const float* src, long ld_src, int rows, int cols, bool per_step, long* ld_dst, cudaStream_t st);
 int dropout_apply_launch(float* x, int rows, int cols, long ld, unsigned long long seed, unsigned site, unsigned step, float p, cudaStream_t st);
+// x[r, c] = relu(x[r, c]) * dropmask(site, step, r*cols + c), in place (the logit head's hidden layers in the training steps)
+int relu_dropout_apply_launch(float* x, int rows, int cols, long ld, unsigned long long seed, unsigned site, unsigned step, float p, cudaStream_t st);
 int dropout_mask_launch(float* m, long n, unsigned long long seed, unsigned site, unsigned step, float p, cudaStream_t st);
 int dropout_copy_launch(const float* x, long ld_x, float* y, long ld_y, int rows, int cols, unsigned long long seed, unsigned site, unsigned step, float p,
                         cudaStream_t st);

@@ -27,6 +27,13 @@ __global__ void dropout_apply_kernel(float* x, long n, int cols, long ld, unsign
     }
 }
 
+__global__ void relu_dropout_apply_kernel(float* x, long n, int cols, long ld, unsigned long long seed, uint32_t site, uint32_t step, float p) {
+    for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+        float* v = x + (i / cols) * ld + (int)(i % cols);
+        *v = fmaxf(*v, 0.f) * drop_scale(seed, site, step, (uint32_t)i, p);
+    }
+}
+
 __global__ void dropout_mask_kernel(float* m, long n, unsigned long long seed, uint32_t site, uint32_t step, float p) {
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) m[i] = drop_scale(seed, site, step, (uint32_t)i, p);
 }
@@ -584,6 +591,10 @@ int nblocks(long n) {
 int dropout_apply_launch(float* x, int rows, int cols, long ld, unsigned long long seed, unsigned site, unsigned step, float p, cudaStream_t st) {
     if (p <= 0.f || rows <= 0) return 0;
     dropout_apply_kernel<<<nblocks((long)rows * cols), 256, 0, st>>>(x, (long)rows * cols, cols, ld, seed, site, step, p);
+    LAUNCH_OK();
+}
+int relu_dropout_apply_launch(float* x, int rows, int cols, long ld, unsigned long long seed, unsigned site, unsigned step, float p, cudaStream_t st) {
+    relu_dropout_apply_kernel<<<nblocks((long)rows * cols), 256, 0, st>>>(x, (long)rows * cols, cols, ld, seed, site, step, p);
     LAUNCH_OK();
 }
 int dropout_mask_launch(float* m, long n, unsigned long long seed, unsigned site, unsigned step, float p, cudaStream_t st) {

@@ -325,15 +325,62 @@ inline int loss_backward(const TrainArgs& ta, const StepTape& tp, const StepBase
     return scst_dlogits_launch(ta.logprobs, ld_lp, ta.sample_seq, ta.reward, tp.mask_sum, ta.upstream, N, T, V1, tp.DL, st, ta.keep > 0 ? tp.row_coef : nullptr);
 }
 
-// loss_backward, then the backward of a logit layer [V1, H] batched over all (n, t): dOUT [N, T, H] = DL W, and the logit gradients (group
-// 0, whose event `ev` is recorded here).  `out` holds the layer's inputs [N, T, H].
-inline int loss_and_logit_backward(const TrainArgs& ta, const StepTape& tp, const StepBaseline& gb, const Skinny& sk, int B, int N, int V1, int H,
-                                   const float* logit_w, const float* out, float* dOUT, float* g_logit_w, float* g_logit_b, cudaEvent_t ev, cudaStream_t st) {
+// ---- the logit head in the training steps (logit_layers = k > 1, AttModel.py:87-92) -------------------------------------------------------
+// Hidden layer i's dropout masks are keyed by (the step's seed, site kHeadDropSite + i, position t), replayable with capb200_dropout_mask.
+constexpr unsigned kHeadDropSite = 200;
+
+// The head's training tape for TN = T * N rows: the k - 1 post-dropout activations [N, T, H] (slot i = layer i), then two gradient slabs.
+inline int head_train_tape(EngineBase* e, long TN, cudaStream_t st) {
+    if (e->logit_layers == 1) return 0;
+    const size_t need = sizeof(float) * (size_t)(e->logit_layers + 1) * TN * e->head_H;
+    return grow_buffer(reinterpret_cast<void**>(&e->head_tape), &e->head_tape_bytes, need, st);
+}
+inline float* head_slot(EngineBase* e, long TN, int i) { return e->head_tape + (size_t)i * TN * e->head_H; }
+
+// Step t of the forward: x [N, H] (pitch ld) is the core's output; hidden layer i writes y_i = dropout(relu(x W_i^T + b_i)) into row (n, t)
+// of its tape slot.  *in / *ld_in: what the vocabulary Linear reads (x itself when k = 1).
+inline int head_train_forward(EngineBase* e, const Skinny& sk, const float* x, long ld, int N, int T, int t, unsigned long long seed, const float** in,
+                              long* ld_in, cudaStream_t st) {
+    const int H = e->head_H;
+    const long TN = (long)T * N;
+    for (int i = 0; i + 1 < e->logit_layers; ++i) {
+        float* y = head_slot(e, TN, i) + (long)t * H;
+        if (sk.lin(x, ld, e->head_w[i], H, e->head_b[i], y, (long)T * H, N, H, H, 0)) return 1;
+        if (relu_dropout_apply_launch(y, N, H, (long)T * H, seed, kHeadDropSite + i, (unsigned)t, e->head_drop, st)) return 1;
+        e->launches += 2;
+        x = y;
+        ld = (long)T * H;
+    }
+    *in = x;
+    *ld_in = ld;
+    return 0;
+}
+
+// loss_backward, then the backward of the output head batched over all (n, t) -- it is not recurrent: the vocabulary Linear [V1, H] (its
+// input is the last hidden activation, or `out` [N, T, H] -- the core's output -- when k = 1), then the hidden layers from the last to the
+// first (mask * relu', weight and bias gradients, input gradient), so that dOUT [N, T, H] ends up holding d loss / d core output.  All of it
+// is gradient group 0, whose event `ev` is recorded here.
+inline int loss_and_logit_backward(EngineBase* e, const TrainArgs& ta, const StepTape& tp, const StepBaseline& gb, const Skinny& sk, int B, int N, int V1,
+                                   int H, const float* logit_w, const float* out, float* dOUT, float* g_logit_w, float* g_logit_b, cudaEvent_t ev,
+                                   cudaStream_t st) {
     const int TN = ta.T * N;
+    const int L = e->logit_layers - 1;
     if (loss_backward(ta, tp, gb, B, N, V1, st)) return 1;
-    if (sk.dgrad(TN, H, V1, tp.DL, V1, logit_w, H, dOUT, H, 0)) return 1;          // dOUT = DL * W
-    if (sk.wgrad(V1, H, TN, tp.DL, V1, out, H, g_logit_w, H, 0)) return 1;         // dW = DL^T * OUT
+    float* dy = L ? head_slot(e, TN, L) : dOUT;           // d loss / d (the vocabulary Linear's input)
+    float* dz = L ? head_slot(e, TN, L + 1) : nullptr;
+    if (sk.dgrad(TN, H, V1, tp.DL, V1, logit_w, H, dy, H, 0)) return 1;            // dY = DL * W
+    if (sk.wgrad(V1, H, TN, tp.DL, V1, L ? head_slot(e, TN, L - 1) : out, H, g_logit_w, H, 0)) return 1;     // dW = DL^T * Y
     if (colsum_launch(TN, V1, tp.DL, V1, g_logit_b, 0, st)) return 1;
+    const float scale = 1.f / (1.f - e->head_drop);
+    for (int i = L - 1; i >= 0; --i) {
+        const float* y = head_slot(e, TN, i);
+        const float* x = i ? head_slot(e, TN, i - 1) : out;
+        if (relu_dropout_backward_launch((long)TN * H, y, dy, dz, scale, st)) return 1;                    // y > 0 iff kept and relu' = 1
+        if (sk.wgrad(H, H, TN, dz, H, x, H, e->head_gw[i], H, 0)) return 1;
+        if (colsum_launch(TN, H, dz, H, e->head_gb[i], 0, st)) return 1;
+        if (sk.dgrad(TN, H, H, dz, H, e->head_w[i], H, i ? dy : dOUT, H, 0)) return 1;
+        e->launches += 4;
+    }
     return record_group_event(ev, st);
 }
 
@@ -420,6 +467,13 @@ int run_scst_step(Engine* e, const Opts* opts, const Grads* grads, const Args& t
     const void* ptrs[] = {ta.table, ta.refs, ta.ref_offsets, ta.sample_seq, ta.greedy_seq, ta.logprobs, ta.reward, ta.loss, e->tape, e->ws, e->wblock, e->sg.stage, gst};
     StepGraph::mix(key, ptrs, sizeof(ptrs));
     StepGraph::mix(key, e->grad_events, sizeof(cudaEvent_t) * e->grad_groups);
+    if (e->logit_layers > 1) {                                // the logit head's weights, gradient buffers, dropout rate and tape
+        const size_t n = sizeof(void*) * (e->logit_layers - 1);
+        StepGraph::mix(key, e->head_w.data(), n); StepGraph::mix(key, e->head_b.data(), n);
+        StepGraph::mix(key, e->head_gw.data(), n); StepGraph::mix(key, e->head_gb.data(), n);
+        const void* hp[2] = {e->head_tape, e->head_block};
+        StepGraph::mix(key, hp, sizeof(hp)); StepGraph::mix(key, &e->head_drop, sizeof(float)); StepGraph::mix(key, &e->logit_layers, sizeof(int));
+    }
     const int dims[] = {B, R, ta.L};
     StepGraph::mix(key, dims, sizeof(dims));
     const int rc = run_step_graph(e->sg, key, opts->seed, &e->launches, gst, [&]() { return counted(staged(0), staged(1), ts, gst); });
@@ -437,7 +491,8 @@ int run_ppo_step(Engine* e, Engine* old, const capb200_ppo_opts* po, Args& ta, i
     CAPB_REQUIRE(po && old && scores && pg_loss && kl_loss && clipfrac, "null argument");
     if (check_ready(old)) return 1;
     CAPB_REQUIRE(old != e, "the old policy needs an engine of its own");
-    CAPB_REQUIRE(memcmp(&old->cfg, &e->cfg, sizeof(e->cfg)) == 0, "the old policy's engine must have the family and configuration of the new one");
+    CAPB_REQUIRE(memcmp(&old->cfg, &e->cfg, sizeof(e->cfg)) == 0 && old->logit_layers == e->logit_layers,
+                 "the old policy's engine must have the family and configuration of the new one");
     CAPB_REQUIRE(!ta.greedy_baseline, "PPO takes the leave-one-out advantage: baseline must be CAPB200_BASELINE_LEAVE_ONE_OUT");
     CAPB_REQUIRE(std::isfinite(po->cliprange) && po->cliprange > 0.f && std::isfinite(po->kl_coef) && po->kl_coef >= 0.f,
                  "PPO needs cliprange > 0 and kl_coef >= 0");

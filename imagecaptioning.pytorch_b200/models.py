@@ -193,8 +193,10 @@ class B200CaptionModel(nn.Module):
             raise NotImplementedError('capb200 engine assumes bos = eos = pad = 0 (AttModel.py:65-67 defaults)')
         if getattr(opt, 'use_bn', 0):
             raise NotImplementedError('use_bn is not on the engine decode path')
-        if getattr(opt, 'logit_layers', 1) != 1:
-            raise NotImplementedError('logit_layers > 1 is not on the engine decode path')
+        # AttModel.py:87-92; k <= 0 makes the reference's reduce fail on an empty list
+        self.logit_layers = int(getattr(opt, 'logit_layers', 1))
+        if self.logit_layers < 1:
+            raise ValueError('logit_layers must be >= 1 (got %d)' % self.logit_layers)
         self.ss_prob = 0.0
         self.vocab = opt.vocab
         self.bad_endings_ix = [int(k) for k, v in self.vocab.items() if v in BAD_ENDINGS]
@@ -206,6 +208,41 @@ class B200CaptionModel(nn.Module):
         # differentiable _forward / _sample (the autograd entry points, include/capb200.h: capb200_vjp_opts); off = the calls as before
         self.autograd = bool(getattr(opt, 'b200_autograd', 0))
 
+    # ---- the output head (AttModel.py:87-92) -------------------------------------------------------------------------
+    def _make_logit(self):
+        """self.logit as AttModel builds it: the vocabulary Linear, or for logit_layers = k > 1 k - 1 [Linear(H, H), ReLU, Dropout(0.5)]
+        blocks ahead of it (state_dict keys logit.0, logit.3, ..., logit.{3(k-1)}).  The engine runs the hidden layers outside the recurrence,
+        in every decode and every training call (their gradients are group 0, with the vocabulary Linear's)."""
+        H, V1 = self.rnn_size, self.vocab_size + 1
+        if self.logit_layers == 1:
+            return nn.Linear(H, V1)
+        hidden = [m for _ in range(self.logit_layers - 1) for m in (nn.Linear(H, H), nn.ReLU(), nn.Dropout(0.5))]
+        return nn.Sequential(*hidden, nn.Linear(H, V1))
+
+    @property
+    def _vocab_logit(self):
+        """The vocabulary Linear of self.logit (its last layer)."""
+        return self.logit if isinstance(self.logit, nn.Linear) else self.logit[-1]
+
+    def _head_named(self):
+        """[(state_dict name, tensor)] of the logit head's hidden layers, weight then bias per layer; empty for logit_layers = 1 and for the
+        Transformer (which has no self.logit)."""
+        head = getattr(self, 'logit', None)
+        if not isinstance(head, nn.Sequential):
+            return []
+        return [('logit.%d.%s' % (3 * i, f), getattr(head[3 * i], f)) for i in range(len(head) // 3) for f in ('weight', 'bias')]
+
+    def _bind_head_grads(self, lib, grads, train):
+        """Registers the gradient buffers of the head's hidden layers (``grads``: [w_0, b_0, w_1, ...] as _head_named) and its dropout rate
+        (Dropout(0.5) in train mode, off in eval mode) with the engine for the training calls that follow."""
+        if not grads:
+            return
+        n = len(grads) // 2
+        gw = (ctypes.c_void_p * n)(*[t.data_ptr() for t in grads[0::2]])
+        gb = (ctypes.c_void_p * n)(*[t.data_ptr() for t in grads[1::2]])
+        _lib.check(getattr(lib, 'capb200_%s_bind_logit_head_grads' % self._abi)(self._engine, gw, gb), '%s_bind_logit_head_grads' % self._abi)
+        _lib.check(getattr(lib, 'capb200_%s_set_logit_dropout' % self._abi)(self._engine, 0.5 if train else 0.0), '%s_set_logit_dropout' % self._abi)
+
     # ---- engine plumbing --------------------------------------------------------------------------------------------
     _engine = _slot_property('engine')
     _engine_key = _slot_property('key')
@@ -216,16 +253,16 @@ class B200CaptionModel(nn.Module):
 
     def _grad_groups(self, named):
         """The [(slot name, parameter)] of _grad_slots split into lists in the order the engine completes the gradients (include/capb200.h:
-        *_set_grad_events): the logit layer first."""
+        *_set_grad_events): the logit layer and the head's hidden layers first."""
         slots = dict(named)
-        first = ('logit_w', 'logit_b')
+        first = ('logit_w', 'logit_b') + tuple(n for n, _ in self._head_named())
         return [[(k, slots[k]) for k in first], [(k, v) for k, v in named if k not in first]]
 
     def _flat_grads(self, device, slots):
         """The persistent flat gradient buffer of this device, its {name: view} table and the engine-recorded group events.  Keyed by name:
         nn.DataParallel replicas carry different Parameter objects every forward but the same names and shapes."""
         from .grad_sync import FlatGrads
-        groups = self._grad_groups([(_slot_name(path), p) for path, p in slots])
+        groups = self._grad_groups([(_slot_name(path), p) for path, p in slots] + self._head_named())
         sig = tuple((n, tuple(p.shape)) for g in groups for n, p in g)
         fg = self._flat
         if fg is None or fg.sig != sig:
@@ -274,6 +311,7 @@ class B200CaptionModel(nn.Module):
         fg = self._flat_grads(device, slots)
         g = self._grads_struct()
         self._fill_struct(g, [(path, fg.by_name[_slot_name(path)]) for path, _ in slots])
+        self._bind_head_grads(lib, [fg.by_name[n] for n, _ in self._head_named()], True)      # the fused steps run in train mode
         # the engine records the group events only for a listener (B200LossWrapper.enable_gradient_sync); without one the whole step may run as a CUDA graph
         table, n = fg.event_table() if getattr(self, '_grad_sync_on', False) else (None, 0)
         _lib.check(getattr(lib, 'capb200_%s_set_grad_events' % self._abi)(self._engine, table, n), '%s_set_grad_events' % self._abi)
@@ -299,18 +337,27 @@ class B200CaptionModel(nn.Module):
             if not eng:
                 raise RuntimeError('capb200 %s_create failed: %s' % (self._abi, lib.capb200_last_error().decode()))
             self._engine, self._engine_key, self._bound_versions = eng, key, None
+            if self._head_named():
+                _lib.check(getattr(lib, 'capb200_%s_set_logit_layers' % self._abi)(eng, self.logit_layers), '%s_set_logit_layers' % self._abi)
         slots = self._slots()
-        versions = self._bind_key([t for _, t in slots])
+        head = self._head_named()
+        versions = self._bind_key([t for _, t in slots] + [t for _, t in head])
         if versions is None or versions != self._bound_versions:
             keep = []
-            for path, t in slots:
+            for name, t in [(_slot_name(path), t) for path, t in slots] + head:
                 if t.device != device or t.dtype != torch.float32:
-                    raise RuntimeError('capb200: parameter %s must be a float32 tensor on %s' % (_slot_name(path), device))
+                    raise RuntimeError('capb200: parameter %s must be a float32 tensor on %s' % (name, device))
                 keep.append(t.detach().contiguous())
             w = self._weights_struct()
             self._fill_struct(w, [(path, t) for (path, _), t in zip(slots, keep)])
             _lib.check(getattr(lib, 'capb200_%s_bind_weights' % self._abi)(self._engine, ctypes.byref(w), _lib.current_stream()),
                        '%s_bind_weights' % self._abi)
+            if head:
+                hk = keep[len(slots):]
+                ws = (ctypes.c_void_p * (len(hk) // 2))(*[t.data_ptr() for t in hk[0::2]])
+                bs = (ctypes.c_void_p * (len(hk) // 2))(*[t.data_ptr() for t in hk[1::2]])
+                _lib.check(getattr(lib, 'capb200_%s_bind_logit_head' % self._abi)(self._engine, ws, bs, _lib.current_stream()),
+                           '%s_bind_logit_head' % self._abi)
             self._keepalive = keep
             self._bound_versions = versions
         return lib
@@ -575,9 +622,10 @@ class B200CaptionModel(nn.Module):
     def _scst_opts(self, sample_n, temperature, seed, upstream, baseline, rates, forced, masks, keep_rows, row_loss, sampler, rw):
         return _lib.ScstOpts(sample_n, temperature, seed, *rates, upstream, baseline, _lib.ptr(forced), _lib.ptr(masks), keep_rows, _lib.ptr(row_loss), sampler, rw)
 
-    @staticmethod
-    def _grads_of(fg, slots):
-        return {prm: fg.by_name[_slot_name(path)] for path, prm in slots}
+    def _grads_of(self, fg, slots):
+        out = {prm: fg.by_name[_slot_name(path)] for path, prm in slots}
+        out.update((prm, fg.by_name[n]) for n, prm in self._head_named())
+        return out
 
     # ---- SCST training step: greedy baseline + sampling with dropout + CIDEr-D reward + RewardCriterion + BPTT -----------------
     @_on_device
@@ -649,7 +697,8 @@ class B200CaptionModel(nn.Module):
         from .rewards import pack_references, weights_struct
         if self._entry is None:
             raise NotImplementedError('%s has no fused PPO step' % type(self).__name__)
-        if old_model is self or type(old_model) is not type(self) or bytes(old_model._cfg()) != bytes(self._cfg()):
+        if (old_model is self or type(old_model) is not type(self) or bytes(old_model._cfg()) != bytes(self._cfg())
+                or getattr(old_model, 'logit_layers', 1) != getattr(self, 'logit_layers', 1)):
             raise ValueError('ppo_step needs an old model of its own with the family and configuration of this one')
         if int(sample_n) < 2:
             raise ValueError("PPO's leave-one-out advantage needs sample_n >= 2")
@@ -740,12 +789,13 @@ class B200CaptionModel(nn.Module):
         if any(f is not None and f.requires_grad for f in feats):
             raise NotImplementedError('capb200 autograd: gradients with respect to the features are out of scope (detach them)')
 
-    def _vjp_run(self, form, feats, B, R, make_opts, words, logprobs_shape, dev, greedy=False, out_seq=None):
+    def _vjp_run(self, form, feats, B, R, make_opts, words, logprobs_shape, dev, greedy=False, out_seq=None, train=True):
         """The closure _EngineVjp calls: run(None) is the forward (log-probs), run(G) the backward of G = dL/dlogprobs (one fresh gradient
         tensor per parameter).  make_opts(replay) builds the option struct: replay=False for the forward, True for the backward, which
-        feeds the same words (words()) with the same seed."""
+        feeds the same words (words()) with the same seed.  ``train``: the logit head's dropout is on."""
         slots = self._grad_slots()
-        params = [p for _, p in slots]
+        head = [p for _, p in self._head_named()]
+        params = [p for _, p in slots] + head
         entry = 'capb200_%s_%s_vjp' % (self._entry, form)
 
         def run(G):
@@ -753,11 +803,13 @@ class B200CaptionModel(nn.Module):
             lp = torch.zeros(logprobs_shape, dtype=torch.float32, device=dev)
             if G is None:
                 opts, vo, g, grads = make_opts(False), _lib.VjpOpts(1, None, int(greedy)), None, None
+                self._bind_head_grads(lib, [torch.empty_like(p) for p in head], train)     # not written by a forward-only call
             else:
                 G = G.detach().to(torch.float32).contiguous()
                 grads = [torch.empty_like(p) for p in params]
                 g = self._grads_struct()
                 self._fill_struct(g, [(path, t) for (path, _), t in zip(slots, grads)])
+                self._bind_head_grads(lib, grads[len(slots):], train)
                 opts, vo = make_opts(True), _lib.VjpOpts(0, G.data_ptr(), 0)
             tail = (words(G is not None), logprobs_shape[1] + 1) if form == 'xe' else ()
             seq = out_seq if G is None or out_seq is None else torch.empty_like(out_seq)
@@ -797,7 +849,7 @@ class B200CaptionModel(nn.Module):
         def make_opts(replay):
             return self._xe_opts(N // B, steps, seed, 0.0, 1.0, self._rates(train), masks, 0.0 if replay else ss, None if replay else tokens_used, 0,
                                  None)
-        run, params = self._vjp_run('xe', feats, B, R, make_opts, words, (N, L, self.vocab_size + 1), dev)
+        run, params = self._vjp_run('xe', feats, B, R, make_opts, words, (N, L, self.vocab_size + 1), dev, train=train)
         return _EngineVjp.apply(run, *params)
 
     def _sample_autograd(self, fc_feats, att_feats, att_masks, opt, forced_tokens):
@@ -837,7 +889,7 @@ class B200CaptionModel(nn.Module):
             return self._scst_opts(sample_n, temperature, seed, 1.0, _lib.BASELINE_GREEDY, self._rates(train), seq if replay else forced, masks, 0, None,
                                    None, None)
         run, params = self._vjp_run('scst', feats, B, R, make_opts, None, (N, T, self.vocab_size + 1), dev,
-                                    greedy=forced is None and method == 'greedy', out_seq=seq)
+                                    greedy=forced is None and method == 'greedy', out_seq=seq, train=train)
         logprobs = _EngineVjp.apply(run, *params)
         return seq, logprobs
 
@@ -915,7 +967,7 @@ class B200UpDownModel(B200CaptionModel):
         self.embed = nn.Sequential(nn.Embedding(V1, self.input_encoding_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
         self.fc_embed = nn.Sequential(nn.Linear(self.fc_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
         self.att_embed = nn.Sequential(nn.Linear(self.att_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
-        self.logit = nn.Linear(self.rnn_size, V1)
+        self.logit = self._make_logit()
         self.ctx2att = nn.Linear(self.rnn_size, self.att_hid_size)
         self.core = _UpDownCoreParams(opt)
 
@@ -924,7 +976,7 @@ class B200UpDownModel(B200CaptionModel):
         return {
             'embed': self.embed[0].weight, 'fc_embed_w': self.fc_embed[0].weight, 'fc_embed_b': self.fc_embed[0].bias,
             'att_embed_w': self.att_embed[0].weight, 'att_embed_b': self.att_embed[0].bias,
-            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
+            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self._vocab_logit.weight, 'logit_b': self._vocab_logit.bias,
             'att_lstm_w_ih': c.att_lstm.weight_ih, 'att_lstm_w_hh': c.att_lstm.weight_hh, 'att_lstm_b_ih': c.att_lstm.bias_ih,
             'att_lstm_b_hh': c.att_lstm.bias_hh, 'lang_lstm_w_ih': c.lang_lstm.weight_ih, 'lang_lstm_w_hh': c.lang_lstm.weight_hh,
             'lang_lstm_b_ih': c.lang_lstm.bias_ih, 'lang_lstm_b_hh': c.lang_lstm.bias_hh,
@@ -961,7 +1013,7 @@ class B200Att2in2Model(B200UpDownModel):
         V1 = self.vocab_size + 1
         self.embed = nn.Sequential(nn.Embedding(V1, self.input_encoding_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
         self.att_embed = nn.Sequential(nn.Linear(self.att_feat_size, self.rnn_size), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
-        self.logit = nn.Linear(self.rnn_size, V1)
+        self.logit = self._make_logit()
         self.ctx2att = nn.Linear(self.rnn_size, self.att_hid_size)
         self.core = _Att2in2CoreParams(opt)
 
@@ -969,7 +1021,7 @@ class B200Att2in2Model(B200UpDownModel):
         c = self.core
         return {
             'embed': self.embed[0].weight, 'att_embed_w': self.att_embed[0].weight, 'att_embed_b': self.att_embed[0].bias,
-            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
+            'ctx2att_w': self.ctx2att.weight, 'ctx2att_b': self.ctx2att.bias, 'logit_w': self._vocab_logit.weight, 'logit_b': self._vocab_logit.bias,
             'h2att_w': c.attention.h2att.weight, 'h2att_b': c.attention.h2att.bias,
             'alpha_w': c.attention.alpha_net.weight, 'alpha_b': c.attention.alpha_net.bias,
             'i2h_w': c.i2h.weight, 'i2h_b': c.i2h.bias, 'h2h_w': c.h2h.weight, 'h2h_b': c.h2h.bias, 'a2c_w': c.a2c.weight, 'a2c_b': c.a2c.bias,
@@ -1001,13 +1053,13 @@ class B200NewFCModel(B200CaptionModel):
         V1 = self.vocab_size + 1
         self.embed = nn.Embedding(V1, self.input_encoding_size)
         self.fc_embed = nn.Linear(self.fc_feat_size, self.input_encoding_size)
-        self.logit = nn.Linear(self.rnn_size, V1)
+        self.logit = self._make_logit()
         self._core = _MaxoutCoreParams(opt)
 
     def _weight_table(self):
         return {
             'embed': self.embed.weight, 'fc_embed_w': self.fc_embed.weight, 'fc_embed_b': self.fc_embed.bias,
-            'logit_w': self.logit.weight, 'logit_b': self.logit.bias,
+            'logit_w': self._vocab_logit.weight, 'logit_b': self._vocab_logit.bias,
             'i2h_w': self._core.i2h.weight, 'i2h_b': self._core.i2h.bias, 'h2h_w': self._core.h2h.weight, 'h2h_b': self._core.h2h.bias,
         }
 
@@ -1190,7 +1242,7 @@ class B200AoAModel(B200CaptionModel):
         H, E, V1 = self.rnn_size, self.input_encoding_size, self.vocab_size + 1
         self.embed = nn.Sequential(nn.Embedding(V1, E), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
         self.att_embed = nn.Sequential(nn.Linear(self.att_feat_size, H), nn.ReLU(), nn.Dropout(self.drop_prob_lm))
-        self.logit = nn.Linear(H, V1)
+        self.logit = self._make_logit()
         self.ctx2att = nn.Linear(H, 2 * H)
         self.refiner = nn.Module()
         self.refiner.layers = nn.ModuleList()
@@ -1231,13 +1283,13 @@ class B200AoAModel(B200CaptionModel):
                 (('attn_norm_a',), c.attention.norm.a_2), (('attn_norm_b',), c.attention.norm.b_2),
                 (('attn_q_w',), c.attention.linears[0].weight), (('attn_q_b',), c.attention.linears[0].bias),
                 (('att2ctx_w',), c.att2ctx[0].weight), (('att2ctx_b',), c.att2ctx[0].bias),
-                (('logit_w',), self.logit.weight), (('logit_b',), self.logit.bias)]
+                (('logit_w',), self._vocab_logit.weight), (('logit_b',), self._vocab_logit.bias)]
         return out
 
     def _grad_groups(self, named):
         slots = dict(named)
         pick = lambda names: [(n, slots[n]) for n in names]
-        groups = [pick(['logit_w', 'logit_b']),
+        groups = [pick(['logit_w', 'logit_b'] + [n for n, _ in self._head_named()]),
                   pick(['att2ctx_w', 'att2ctx_b', 'attn_q_w', 'attn_q_b', 'att_lstm_w_ih', 'att_lstm_w_hh', 'att_lstm_b_ih', 'att_lstm_b_hh', 'attn_norm_a',
                         'attn_norm_b', 'embed']),
                   pick(['ctx2att_w', 'ctx2att_b', 'refiner_norm_a', 'refiner_norm_b'])]

@@ -21,9 +21,10 @@ def _uniform(gen, shape, bound):
 
 
 def make_weights(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int, seed: int = 1234,
-                 logit_scale: float = 12.0) -> Weights:
+                 logit_scale: float = 12.0, logit_layers: int = 1) -> Weights:
     """Deterministic synthetic weights with torch-default-like ranges; ``logit.weight`` is scaled so the
-    next-word distribution is peaked (top-1/top-2 margins far above the 1e-4 log-prob tolerance)."""
+    next-word distribution is peaked (top-1/top-2 margins far above the 1e-4 log-prob tolerance).  ``logit_layers`` > 1 adds the
+    output head of AttModel (add_logit_head); every other tensor is drawn as with the default."""
     g = torch.Generator().manual_seed(seed)
     V1 = V + 1
     W: Weights = {}
@@ -122,6 +123,24 @@ def make_weights(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: 
         lin('_core.h2h', 5 * H, H)
     else:
         raise ValueError(family)
+    if logit_layers > 1 and family != 'transformer':      # the Transformer has no self.logit (TransformerModel.py:285)
+        add_logit_head(W, H, logit_layers, seed)
+    return W
+
+
+def add_logit_head(W: Weights, H: int, logit_layers: int, seed: int) -> Weights:
+    """Turns W's vocabulary Linear into AttModel's head for logit_layers = k > 1 (AttModel.py:87-92): k - 1 hidden Linear(H, H) layers
+    logit.0, logit.3, ... (each followed by ReLU and Dropout in the reference) ahead of the vocabulary Linear, renamed logit.{3(k-1)}.
+    The hidden layers come from a generator of their own, with a gain of sqrt(6) that keeps the ReLU outputs at the scale of their
+    inputs, so the vocabulary rows stay as peaked as without a head."""
+    g = torch.Generator().manual_seed(seed + 7919)
+    b = 1.0 / math.sqrt(H)
+    for i in range(logit_layers - 1):
+        W['logit.%d.weight' % (3 * i)] = _uniform(g, (H, H), b) * math.sqrt(6.0)
+        W['logit.%d.bias' % (3 * i)] = _uniform(g, (H,), b)
+    last = 3 * (logit_layers - 1)
+    W['logit.%d.weight' % last] = W.pop('logit.weight')
+    W['logit.%d.bias' % last] = W.pop('logit.bias')
     return W
 
 
@@ -168,12 +187,12 @@ def document_frequency(ref_rows_per_image: Sequence[Sequence[Sequence[int]]], ma
     return dict(df), len(ref_rows_per_image)
 
 
-def model_opt(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int, T: int, heads: int = 8):
+def model_opt(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int, T: int, heads: int = 8, logit_layers: int = 1):
     """argparse-style ``opt`` of the reference for one family (for 'transformer': E = d_model, H = d_ff, A = layers per stack)."""
     import argparse
     opt = argparse.Namespace(vocab_size=V, input_encoding_size=E, rnn_size=H, num_layers=1, drop_prob_lm=0.5, max_length=T, seq_length=T,
                              fc_feat_size=F_fc, att_feat_size=F_att, att_hid_size=A, vocab={str(i): 'w%d' % i for i in range(1, V + 1)},
-                             caption_model=family, use_bn=0, logit_layers=1)
+                             caption_model=family, use_bn=0, logit_layers=logit_layers)
     if family == 'transformer':
         opt.num_layers, opt.N_enc, opt.N_dec, opt.d_model, opt.d_ff, opt.num_att_heads = A, A, A, E, H, heads
     if family == 'aoa':
@@ -183,10 +202,10 @@ def model_opt(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int
 
 
 def build_model(family: str, V: int, E: int, H: int, A: int, F_fc: int, F_att: int, T: int, seed: int, logit_scale: float, mode: str,
-                device='cuda', heads: int = 8):
+                device='cuda', heads: int = 8, logit_layers: int = 1):
     """Engine model of ``family`` with the seeded synthetic weights loaded, on ``device``, in eval mode."""
     from . import setup
-    W = make_weights(family, V, E, H, A, F_fc, F_att, seed=seed, logit_scale=logit_scale)
-    model = setup(model_opt(family, V, E, H, A, F_fc, F_att, T, heads), numeric_mode=mode)
+    W = make_weights(family, V, E, H, A, F_fc, F_att, seed=seed, logit_scale=logit_scale, logit_layers=logit_layers)
+    model = setup(model_opt(family, V, E, H, A, F_fc, F_att, T, heads, logit_layers), numeric_mode=mode)
     model.load_state_dict(W, strict=True)
     return model.to(device).eval()

@@ -144,6 +144,25 @@ void capb200_engine_destroy(capb200_engine* e);
 /* (Re)binds the parameter tensors; call again after every optimizer step.  Tensor-core modes repack the fp16 planes here. */
 int capb200_engine_bind_weights(capb200_engine* e, const capb200_weights* w, void* stream);
 
+/* AttModel's output head for logit_layers = k > 1 (AttModel.py:87-92): the state_dict's logit.0, logit.3, ..., logit.{3(k-2)} are k - 1
+ * hidden Linear(H, H) + ReLU + Dropout(0.5) layers ahead of logit.{3(k-1)}, the vocabulary projection (capb200_weights.logit_w / logit_b).
+ * The head sits outside the recurrence: the state fed to the next step is the core's output (AttModel.py:166-176).  Every decode (greedy,
+ * sampling, teacher forcing, beam and diverse beam search, ensemble members, PPO's old policy) runs the hidden layers before the vocabulary
+ * GEMM without dropout (eval mode).  Every training entry point (the fused XE / SCST / PPO steps and the *_vjp autograd entry points) runs
+ * them too: hidden layer i's dropout mask at position t is site 200 + i, step t of capb200_dropout_mask under the step's seed, with the rate
+ * of set_logit_dropout, and the head's backward runs batched over all positions ahead of backpropagation through time, in gradient group 0.
+ * set_logit_layers: k >= 1, once, before the first decode (k = 1, the default, runs exactly the single Linear).
+ * bind_logit_head: w[i] [H, H] and b[i] [H] of hidden layer i < k - 1 (logit.{3i}.weight / .bias, fp32, device); call it after every
+ * bind_weights (tensor-core modes repack the fp16 planes here).  A decode of an engine with k > 1 and no bound head is refused.
+ * bind_logit_head_grads: gw[i] [H, H] and gb[i] [H], OVERWRITTEN by every training call that follows; a training call of an engine with
+ * k > 1 and no bound gradient buffers is refused.
+ * set_logit_dropout: the hidden layers' dropout rate p in [0, 1) of the training calls that follow: 0.5 (the default; Dropout(0.5) in
+ * train mode), 0 for an eval-mode autograd pass. */
+int capb200_engine_set_logit_layers(capb200_engine* e, int logit_layers);
+int capb200_engine_bind_logit_head(capb200_engine* e, const float* const* w, const float* const* b, void* stream);
+int capb200_engine_bind_logit_head_grads(capb200_engine* e, float* const* gw, float* const* gb);
+int capb200_engine_set_logit_dropout(capb200_engine* e, float p);
+
 /* Per-step edits of the log-prob rows before the next word is chosen (the reference's decode options; the edited row is also what the
  * reference stores in seqLogprobs / done_beams[...]['logps'], and so do we).  All zero / -1 / NULL = none. */
 typedef struct {
@@ -303,6 +322,11 @@ typedef struct {
 capb200_aoa_engine* capb200_aoa_create(const capb200_aoa_cfg* cfg);
 void capb200_aoa_destroy(capb200_aoa_engine* e);
 int capb200_aoa_bind_weights(capb200_aoa_engine* e, const capb200_aoa_weights* w, void* stream);
+/* AoANet's logit head (AoAModel inherits AttModel's self.logit): as capb200_engine_set_logit_layers and the three after it */
+int capb200_aoa_set_logit_layers(capb200_aoa_engine* e, int logit_layers);
+int capb200_aoa_bind_logit_head(capb200_aoa_engine* e, const float* const* w, const float* const* b, void* stream);
+int capb200_aoa_bind_logit_head_grads(capb200_aoa_engine* e, float* const* gw, float* const* gb);
+int capb200_aoa_set_logit_dropout(capb200_aoa_engine* e, float p);
 int capb200_aoa_decode_beam(capb200_aoa_engine* e, const float* att, const float* mask, int B, int R, const capb200_beam_opts* opts, long long* seq,
                             float* seq_logprobs, long long* done_seq, int* done_len, float* done_p, float* done_raw, void* stream);
 int capb200_aoa_beam_record_logprobs(capb200_aoa_engine* e, int image, int rank, float* dst, void* stream);
