@@ -1,5 +1,6 @@
 """Shared helpers for the parity tests."""
 import argparse
+import contextlib
 import os
 import sys
 
@@ -120,6 +121,128 @@ def aoa_masks(b200, seed, B, R, N, T, E, H, heads, p_lm, p_at, p_aoa, p_sub):
     d['ctx'] = torch.stack([mask(4, t, (N, H), p_lm) for t in range(T)])
     d['p'] = torch.stack([mask(5, t, (N, heads, 1, R), p_at) for t in range(T)])
     return d
+
+
+def tfm_masks(b200, seed, B, R, N, L, T, D, Dff, heads, layers, p_lm, p):
+    """Every dropout mask of one Transformer training step over L decoder positions (T = the model's seq_length): att_embed, per encoder
+    layer the attention / sublayer / feed-forward sites, the positional embedding and per decoder layer its sites, one stream per
+    position (element index n * cols + c)."""
+    mask = _mask_fn(b200, seed)
+
+    def per_t(site, shape):            # decoder tensors  ->  [N, L, ...]
+        return torch.stack([mask(site, t, shape, p) for t in range(L)], 1)
+    idxL = T + 2
+    d = {'att_embed': mask(1, 0, (B, R, D), p_lm), 'emb': per_t(2, (N, D))}
+    for l in range(layers):
+        d['enc_p%d' % l] = mask(10 + l, 0, (B, heads, R, R), p)
+        d['enc_sub0_%d' % l] = mask(20 + l, 0, (B, R, D), p)
+        d['enc_ffn%d' % l] = mask(30 + l, 0, (B, R, Dff), p)
+        d['enc_sub1_%d' % l] = mask(40 + l, 0, (B, R, D), p)
+        d['dec_p%d' % l] = mask(50 + l, 0, (N, heads, idxL, idxL), p)[:, :, :L, :L]
+        d['dec_sub0_%d' % l] = per_t(60 + l, (N, D))
+        d['dec_src%d' % l] = per_t(70 + l, (N, heads, R)).permute(0, 2, 1, 3)          # [N, L, heads, R] -> [N, heads, L, R]
+        d['dec_sub1_%d' % l] = per_t(80 + l, (N, D))
+        d['dec_ffn%d' % l] = per_t(90 + l, (N, Dff))
+        d['dec_sub2_%d' % l] = per_t(100 + l, (N, D))
+    return d
+
+
+# ---- Transformer ReLUs: feed-forward pre-activations, and biases that keep them clear of the kink ------------------------------------
+
+@contextlib.contextmanager
+def ffn_relu_inputs(on_input):
+    """Runs the oracle's feed-forward layers (caption_oracle._ffn) through ``on_input(prefix, W, a)``, called with each layer's w_1
+    pre-activations ``a`` before the ReLU, in the order the layers run; it returns the pre-activations the layer goes on with (and may
+    change W[prefix + 'w_1.bias'] to match).  The layer's GEMMs resolve co.linear at call time, as the oracle's own do."""
+    orig = co._ffn
+
+    def ffn(W, pre, x, h_drop=None):
+        hdn = torch.relu(on_input(pre, W, co.linear(x, W[pre + 'w_1.weight'], W[pre + 'w_1.bias'])))
+        if h_drop is not None:
+            hdn = hdn * h_drop
+        return co.linear(hdn, W[pre + 'w_2.weight'], W[pre + 'w_2.bias'])
+    co._ffn = ffn
+    try:
+        yield
+    finally:
+        co._ffn = orig
+
+
+def _clear_units(a, b, margin, max_steps):
+    """New fp32 bias b' (float64 [H]) for the pre-activations a [rows, H] (computed with bias b) such that every |a - b + b'| is at least
+    margin x RMS(a): each unit with a row inside the band moves by the smallest +-k x margin x RMS (k = 1, 2, ...; + before -) that
+    clears all its rows, rounded to fp32 as the engine holds it.  Returns (b', RMS)."""
+    rms = float(a.pow(2).mean().sqrt())
+    band = margin * rms
+    amb = (a.abs() < band).any(0).nonzero().flatten()
+    b_new = b.clone()
+    if len(amb):
+        z = a[:, amb] - b[amb]                                 # the bias-free part of each ambiguous unit
+        todo = torch.ones(len(amb), dtype=torch.bool)
+        for k in range(1, max_steps + 1):
+            for sign in (1.0, -1.0):
+                cand = (b[amb] + sign * k * band).float().double()
+                # 0.1 % over the band: the RMS moves slightly once the units are shifted, and the check that follows recomputes it
+                ok = todo & ((z + cand).abs() >= 1.001 * band).all(0)
+                b_new[amb[ok]] = cand[ok]
+                todo &= ~ok
+            if not bool(todo.any()):
+                break
+        assert not bool(todo.any()), ('units with no clearing shift within %d margins' % max_steps, amb[todo].tolist())
+    return b_new, rms
+
+
+def clear_relu_kinks(W, att, forward, margin, max_steps=200):
+    """The Transformer's weights with every ReLU decisive: W {name: fp32 tensor} with att_embed's and each feed-forward w_1's bias shifted
+    so that no float64 pre-activation of the step lies within ``margin`` x the layer's RMS of zero.  A unit within rounding of its kink can
+    be on in one fp32 implementation and off in another, and its flip moves the gradient of every tensor upstream of it; moving the model
+    off the kinks lets every gradient tensor be compared in full.
+
+    ``att`` holds the region features (every region counts, masked or not); ``forward(W64)`` runs the step's float64 forward through the
+    oracle (its tokens, region masks and replayed dropout masks), which calls the encoder's and then the decoder's feed-forward layers in
+    order, so each layer is cleared on the inputs the already-shifted earlier layers give it.  Every row counts, including rows whose
+    gradient is zero (padding, finished samples, masked regions).  Returns (shifted fp32 weights, {layer: units shifted}, largest shift
+    as a fraction of its layer's RMS)."""
+    W64 = {k: v.detach().double().clone() for k, v in W.items()}
+    shifted, largest = {}, [0.0]
+
+    def clear(name, a, b):
+        b_new, rms = _clear_units(a, b, margin, max_steps)
+        moved = b_new != b
+        shifted[name] = int(moved.sum())
+        largest[0] = max(largest[0], float((b_new - b).abs().max()) / rms)
+        return b_new
+
+    x = att.double().reshape(-1, att.shape[-1])
+    b = W64['att_embed.0.bias']
+    W64['att_embed.0.bias'] = clear('att_embed', co.linear(x, W64['att_embed.0.weight'], b), b)
+
+    def on_input(pre, Wd, a):
+        b = Wd[pre + 'w_1.bias']
+        b_new = clear(pre[len('model.'):-len('.feed_forward.')], a.reshape(-1, a.shape[-1]), b)
+        Wd[pre + 'w_1.bias'] = b_new
+        return a + (b_new - b)
+    with torch.no_grad(), ffn_relu_inputs(on_input):
+        forward(W64)
+    out = {k: v.clone() for k, v in W.items()}
+    for k in out:
+        if k == 'att_embed.0.bias' or k.endswith('w_1.bias'):
+            out[k] = W64[k].float()
+    return out, shifted, largest[0]
+
+
+def relu_inputs(W, att, forward, linear=None):
+    """[(layer, pre-activations [rows, H])] of the Transformer's ReLUs (att_embed, then every feed-forward layer in order) for the step
+    ``forward(W)`` runs, in W's dtype; ``linear`` (default co.linear) computes att_embed's."""
+    out = [('att_embed', (linear or co.linear)(att.to(W['att_embed.0.weight']).reshape(-1, att.shape[-1]), W['att_embed.0.weight'],
+                                               W['att_embed.0.bias']).detach())]
+
+    def on_input(pre, Wd, a):
+        out.append((pre[len('model.'):-len('.feed_forward.')], a.detach().reshape(-1, a.shape[-1])))
+        return a
+    with torch.no_grad(), ffn_relu_inputs(on_input):
+        forward(W)
+    return out
 
 
 # ---- gradients against a float64 reference, with a bar calibrated by the fp32 oracle's own distance from it ------------------------------

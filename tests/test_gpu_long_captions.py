@@ -9,12 +9,12 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import LOGP_TOL, aoa_masks, check_decode, co, dropout_masks, family_opt
+from helpers import LOGP_TOL, aoa_masks, check_decode, co, dropout_masks, family_opt, tfm_masks
 import bleu_oracle as bo
 import dbs_oracle
 from test_gpu_diverse_beam import DECISIVE, P_TOL
 from test_gpu_scst import _check_grads
-from test_gpu_tfm_train import _check_grads as _tfm_check_grads, _grad_weights, _masks as _tfm_masks
+from test_gpu_tfm_train import _check_grads as _tfm_check_grads, _grad_weights
 from test_long_captions_cpu import corpus_df, load_case
 
 pytestmark = pytest.mark.gpu
@@ -243,7 +243,7 @@ def test_tfm_xe_long(T, cfg, heads):
     N, L = B * spi, T + 1
     Wg = _grad_weights(W)
     fam = co.Family('transformer', Wg, T, heads=heads)
-    fam.drop = _tfm_masks(b200, 98, B, R, N, L, T, cfg['E'], cfg['H'], heads, cfg['A'], p_lm, p)
+    fam.drop = tfm_masks(b200, 98, B, R, N, L, T, cfg['E'], cfg['H'], heads, cfg['A'], p_lm, p)
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1], None)
     loss = co.language_model_criterion(lp, labels.reshape(N, -1)[:, 1:], masks.reshape(N, -1)[:, 1:])
     loss.backward()
@@ -272,7 +272,7 @@ def test_tfm_new_self_critical_long(T, cfg, heads):
     N = B * n
     Wg = _grad_weights(W)
     fam_g = co.Family('transformer', Wg, T, heads=heads)
-    fam_g.drop = _tfm_masks(b200, 4324, B, R, N, T, T, cfg['E'], cfg['H'], heads, cfg['A'], p_lm, p)
+    fam_g.drop = tfm_masks(b200, 4324, B, R, N, T, T, cfg['E'], cfg['H'], heads, cfg['A'], p_lm, p)
     seq_in = torch.cat([torch.zeros(N, 1, dtype=torch.long), seq[:, :-1]], 1)
     lp = co.forward_teacher(fam_g, fc, att, seq_in, None, pad_keys_masked=False)
     scores = torch.from_numpy(cdo.get_scores(gts, seq.numpy(), df, ref_len))

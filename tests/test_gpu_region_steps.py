@@ -8,9 +8,9 @@ tensor's largest entry):
 import pytest
 import torch
 
-from helpers import LOGP_TOL, aoa_masks, build_pair, check_decode, co, dropout_masks, family_opt
+from helpers import LOGP_TOL, aoa_masks, build_pair, check_decode, co, dropout_masks, family_opt, tfm_masks
 from test_gpu_scst import CFG as UD_CFG, _check_grads, _labels
-from test_gpu_tfm_train import _check_grads as _tfm_check_grads, _grad_weights, _labels as _tfm_labels, _masks as _tfm_masks
+from test_gpu_tfm_train import _check_grads as _tfm_check_grads, _grad_weights, _labels as _tfm_labels
 
 pytestmark = pytest.mark.gpu
 
@@ -158,7 +158,7 @@ def test_tfm_xe_at_196_regions():
     N, L = B * spi, T + 1
     Wg = _grad_weights(W)
     fam = co.Family('transformer', Wg, T, heads=TFM_HEADS)
-    fam.drop = _tfm_masks(b200, 98, B, R, N, L, T, TFM['E'], TFM['H'], TFM_HEADS, TFM['A'], p_lm, p)
+    fam.drop = tfm_masks(b200, 98, B, R, N, L, T, TFM['E'], TFM['H'], TFM_HEADS, TFM['A'], p_lm, p)
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1], None)
     flat_l, flat_m = labels.reshape(N, -1), masks.reshape(N, -1)
     loss = co.language_model_criterion(lp, flat_l[:, 1:], flat_m[:, 1:])
@@ -184,7 +184,7 @@ def _tfm_scst(cfg, heads, B, R, n, seed):
     N = B * n
     Wg = _grad_weights(W)
     fam_g = co.Family('transformer', Wg, T, heads=heads)
-    fam_g.drop = _tfm_masks(b200, seed, B, R, N, T, T, cfg['E'], cfg['H'], heads, cfg['A'], p_lm, p)
+    fam_g.drop = tfm_masks(b200, seed, B, R, N, T, T, cfg['E'], cfg['H'], heads, cfg['A'], p_lm, p)
     seq_in = torch.cat([torch.zeros(N, 1, dtype=torch.long), seq[:, :-1]], 1)
     lp = co.forward_teacher(fam_g, fc, att, seq_in, None, pad_keys_masked=False)
     live = torch.cat([torch.ones(N, 1, dtype=torch.bool), seq[:, :-1] > 0], 1)

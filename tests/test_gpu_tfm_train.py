@@ -9,41 +9,13 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import LOGP_TOL, build_pair, co
+from helpers import LOGP_TOL, build_pair, co, tfm_masks
 
 pytestmark = pytest.mark.gpu
 
 # make_weights('transformer'): E = d_model, H = d_ff, A = layers per stack
 CFG = dict(V=40, E=32, H=64, A=2, F_fc=32, F_att=40, T=7)
 HEADS = 4
-
-
-def _masks(b200, seed, B, R, N, L, T, D, Dff, heads, layers, p_lm, p):
-    """Every dropout mask of one Transformer training step, regenerated from the engine's Philox streams (capb200.h lists the sites)."""
-    lb, lib = b200._lib, b200._lib.load()
-
-    def mask(site, step, shape, pr):
-        n = int(np.prod(shape))
-        m = torch.empty(n, device='cuda')
-        lb.check(lib.capb200_dropout_mask(lb.ptr(m), n, seed, site, step, pr, lb.current_stream()), 'dropout_mask')
-        return m.cpu().reshape(shape)
-
-    def per_t(site, shape):            # decoder tensors: one stream per position, element index n * cols + c  ->  [N, L, ...]
-        return torch.stack([mask(site, t, shape, p) for t in range(L)], 1)
-    idxL = T + 2
-    d = {'att_embed': mask(1, 0, (B, R, D), p_lm), 'emb': per_t(2, (N, D))}
-    for l in range(layers):
-        d['enc_p%d' % l] = mask(10 + l, 0, (B, heads, R, R), p)
-        d['enc_sub0_%d' % l] = mask(20 + l, 0, (B, R, D), p)
-        d['enc_ffn%d' % l] = mask(30 + l, 0, (B, R, Dff), p)
-        d['enc_sub1_%d' % l] = mask(40 + l, 0, (B, R, D), p)
-        d['dec_p%d' % l] = mask(50 + l, 0, (N, heads, idxL, idxL), p)[:, :, :L, :L]
-        d['dec_sub0_%d' % l] = per_t(60 + l, (N, D))
-        d['dec_src%d' % l] = per_t(70 + l, (N, heads, R)).permute(0, 2, 1, 3)          # [N, L, heads, R] -> [N, heads, L, R]
-        d['dec_sub1_%d' % l] = per_t(80 + l, (N, D))
-        d['dec_ffn%d' % l] = per_t(90 + l, (N, Dff))
-        d['dec_sub2_%d' % l] = per_t(100 + l, (N, D))
-    return d
 
 
 def _check_grads(model, grads, ograds, rel=5e-4):
@@ -103,7 +75,7 @@ def test_tfm_xe_step_gradients(mode, dropout, smoothing, region_masks):
     fam = co.Family('transformer', Wg, T, heads=HEADS)
     Rc = R if rm is None else int(rm.sum(1).max())                   # clip_att cuts the region axis to the longest valid length
     if dropout:
-        fam.drop = _masks(b200, 99, B, Rc, N, L, T, D, Dff, HEADS, layers, p_lm, p)
+        fam.drop = tfm_masks(b200, 99, B, Rc, N, L, T, D, Dff, HEADS, layers, p_lm, p)
     lp = co.forward_teacher(fam, fc, att, labels[..., :-1], rm)
     flat_l, flat_m = labels.reshape(N, -1), masks.reshape(N, -1)
     loss = co.label_smoothing_loss(lp, flat_l[:, 1:], flat_m[:, 1:], smoothing) if smoothing > 0 else co.language_model_criterion(lp, flat_l[:, 1:], flat_m[:, 1:])
@@ -138,7 +110,7 @@ def test_tfm_scst_step_gradients(mode, dropout, baseline):
     Wg = _grad_weights(W)
     fam_g = co.Family('transformer', Wg, T, heads=HEADS)
     if dropout:
-        fam_g.drop = _masks(b200, 4321, B, R, N, T, T, D, Dff, HEADS, layers, p_lm, p)
+        fam_g.drop = tfm_masks(b200, 4321, B, R, N, T, T, D, Dff, HEADS, layers, p_lm, p)
         seq_in = torch.cat([torch.zeros(N, 1, dtype=torch.long), seq[:, :-1]], 1)
         lp = co.forward_teacher(fam_g, fc, att, seq_in, None, pad_keys_masked=False)
         live = torch.cat([torch.ones(N, 1, dtype=torch.bool), seq[:, :-1] > 0], 1)         # finished rows: the reference stores zero rows

@@ -1,7 +1,9 @@
-"""The fused training steps of UpDown, Att2in2 and AoANet at the widths they train at, against float64 autograd through the oracle.
+"""The fused training steps of UpDown, Att2in2, AoANet and the Transformer at the widths they train at, against float64 autograd through
+the oracle.
 
-UpDown runs at bench.py's CFG (V 9487, E = H = 1000, A 512, F 2048), Att2in2 at the a2i2 recipe width (E = H = A = 512) and AoANet at
-configs/aoa.yml's (E = H = 1024, 8 heads, 6 refiner layers), all with 36 regions and 20 steps.  In both modes the vocabulary-row kernels
+UpDown runs at bench.py's CFG (V 9487, E = H = 1000, A 512, F 2048), Att2in2 at the a2i2 recipe width (E = H = A = 512), AoANet at
+configs/aoa.yml's (E = H = 1024, 8 heads, 6 refiner layers) and the Transformer at bench.py's transformer_scst (6 + 6 layers, d_model 512,
+d_ff 2048, 8 heads), all with 36 regions and 20 steps.  In both modes the vocabulary-row kernels
 loop 37 times per row, the attention backward runs 16 column blocks per image and the autograd VJP takes its 4-wide form.  The training
 GEMMs differ by mode: tc_f16x3 runs them on gemm_tf32.cu's wgmma 3xTF32 kernel, whose tile follows the row count (50 rows per step: tile
 width 64, swapped; 1000 rows batched over time: the normal orientation, cluster split-K over K = 9488 for the logit layer); simt_fp32 runs
@@ -23,6 +25,19 @@ units (margin KINK_MARGIN x the layer's RMS, several times the fp32 error of the
   the side that fits the engine better is taken.  Each change is hundreds of times the bar, so the choice is never close.
 The fp32 oracle follows float64's decisions at every kink, so its distance from float64 is arithmetic only.
 
+The Transformer's feed-forward ReLUs feed the residual stream, so a flipped unit moves the gradient of every tensor upstream of it, and
+they are too many to re-route one by one (about 250 units per encoder layer and 650 per decoder layer lie within 5e-4 x RMS of zero).
+Instead each case moves its model off the kinks before anything runs (helpers.clear_relu_kinks): in layer order, every att_embed or w_1
+unit with a float64 input within TFM_MARGIN x the layer's RMS of zero gets its bias shifted by the smallest +-k x margin x RMS that clears
+all its rows, and the engine and all oracles then use those fp32 weights.  Every float64 ReLU input is asserted to clear the margin, and
+5x the calibrating oracle's largest error there to stay below it, so no tensor is left out.  Measured on an H100 at 50 rows per step: the
+fp32 oracle's error there is 3.7-4.5e-6 x RMS and the 3xTF32 emulation's 0.95-1.12e-4 x RMS (5x = 0.59-0.70 of the 8e-4 margin); 100 att_embed
+units and 200-970 per feed-forward layer move, by at most 1.4e-2 x RMS.  At 160 rows per step (3360 decoder rows) 1000-1750 units per
+layer move, by at most 9.8e-2 x RMS: the rows crowd each unit's band, so the clearing shift is larger, but every unit clears within 200
+margins.  The engine fuses the q | k | v and the memory k | v projections into one GEMM each; an output column of a GEMM depends only on
+its weight row and the K loop, so the emulation's separate Linears bound them column by column (split-K follows the tile count, and the
+emulation's single accumulator is the larger truncation count either way).
+
 Calibration per mode: simt_fp32 is held to the fp32 oracle.  tc_f16x3 is held to the same oracle with every Linear's forward and input
 gradient computed as gemm_tf32 does (_mm_tf32x3): hi / lo tf32 split, three wgmmas per k8 step into one fp32 accumulator, and the
 accumulator truncated (rounded toward zero) by every instruction, the budget test_gpu_ops.py already gives this kernel.  Over K = 3000
@@ -30,7 +45,9 @@ that is 1125 truncations, biased toward zero, so the mode's log-probs and gradie
 emulation reproduces that (its picked log-probs sit 1-3x the engine's distance from float64) and the bar is 4x its error, as for fp32.
 It over-counts the forward's truncations (the kernel's cluster split-K gives each CTA a slice of K) and leaves the weight gradients, which
 the engine batches over time, in fp32, so it is no tighter bound than that: at 320 rows the engine's logit.weight gradient reaches 1.25x
-the emulation's error.
+the emulation's error.  That slack limits what tc_f16x3 can see in the weight gradients: with one of the three products (hi(dY) x lo(X))
+dropped from every Transformer weight gradient, the worst err/bar rose from 0.11 to 0.85 (src_attn.linears.1.weight) and the case still
+passed.  simt_fp32, held to the fp32 oracle, is the mode that catches errors of 1e-4 of a tensor.
 
 Att2in2 runs in simt_fp32 only.  In tc_f16x3 the engine's own error in the maxout inputs is of the order of the kink margin, and the
 gradient change of re-routing a unit is no longer decisive against the mode's error, so the maxout decisions cannot be read off.
@@ -46,17 +63,21 @@ import pytest
 import torch
 
 import att2in2_oracle as ao
-from helpers import aoa_masks, att2in2_masks, check_grads_f64, co, dropout_masks, family_opt
+from helpers import aoa_masks, att2in2_masks, check_grads_f64, clear_relu_kinks, co, dropout_masks, family_opt, ffn_relu_inputs, tfm_masks
 
 pytestmark = pytest.mark.gpu
 
 R, T, SPI, HEADS = 36, 20, 5, 8
 CFGS = {'updown': dict(V=9487, E=1000, H=1000, A=512, F_fc=2048, F_att=2048, T=T),      # bench.py CFG
         'att2in2': dict(V=9487, E=512, H=512, A=512, F_fc=2048, F_att=2048, T=T),       # a2i2 recipe
-        'aoa': dict(V=9487, E=1024, H=1024, A=0, F_fc=2048, F_att=2048, T=T)}           # configs/aoa.yml
-LOGIT_SCALE = {'updown': 12.0, 'att2in2': 12.0, 'aoa': 6.0}                               # bench.py's synthetic models
-RATES = {'updown': 0.5, 'att2in2': 0.5, 'aoa': (0.5, 0.1, 0.3, 0.1)}                      # drop_prob_lm (+ AoANet: attention, AoA, sublayer)
+        'aoa': dict(V=9487, E=1024, H=1024, A=0, F_fc=2048, F_att=2048, T=T),           # configs/aoa.yml
+        'transformer': dict(V=9487, E=512, H=2048, A=6, F_fc=2048, F_att=2048, T=T)}    # bench.py transformer_scst: d_model, d_ff, layers
+LOGIT_SCALE = {'updown': 12.0, 'att2in2': 12.0, 'aoa': 6.0, 'transformer': 3.0}           # bench.py's synthetic models
+RATES = {'updown': 0.5, 'att2in2': 0.5, 'aoa': (0.5, 0.1, 0.3, 0.1),                      # drop_prob_lm (+ AoANet: attention, AoA, sublayer)
+         'transformer': (0.5, 0.1)}                                                       # drop_prob_lm, dropout (transformer.yml, opts)
 KINK_MARGIN = 2e-5              # ReLU inputs and maxout a - b: x the layer's RMS, at least 5x the fp32 oracle's own error there (asserted)
+TFM_MARGIN = 8e-4               # the Transformer's ReLU inputs are moved this far (x the layer's RMS) from zero; 5x the calibrating oracle's
+                                # error there must stay below it (asserted; the 3xTF32 emulation's is the larger, 1e-4)
 SEED = 4242
 COLLIDE = 7                     # the word that fills whole caption rows: embed_scatter's atomics all land on one row of d_emb
 
@@ -260,6 +281,7 @@ class Case:
             if kind == 'autograd':
                 self.G = torch.randn(self.N, T + 1, c['V'] + 1, generator=torch.Generator().manual_seed(31))
         self.drop = None
+        self.W = _weights(family)             # the Transformer's are moved off its ReLU kinks for each case (reference())
 
     # ---- the step through the oracle ----------------------------------------------------------------------------------------------------
     def _family(self, W):
@@ -305,21 +327,39 @@ class Case:
             return crit(lp, tl, tm)
         return (crit(lp, tl, tm, reduction='none') * tm.sum(1).to(dt)).sum() / self.tm.sum()
 
-    def oracle(self, dt, rows=None, route=None, flip=None, record=None, tf32x3=False):
-        W = {k: v.detach().to(dt, copy=True).requires_grad_(True) for k, v in _weights(self.family).items()}
+    def _forward(self, W, dt, rows=None):
+        """The step's log-probs through the oracle with weights W.  The Transformer's is always one causal teacher-forced pass: XE masks
+        pad keys; the sampled steps feed [0, samples[:, :-1]] under the causal mask alone (what the sampler's cached K/V sees) and zero
+        the rows of finished samples, as the sampler stores them."""
         fam = self._family(W)
         fc, att, reg, fam.drop, words = self._inputs(rows, dt)
-        maxout = _routed_maxout([] if record is None else record, route, flip) if self.family == 'att2in2' else contextlib.nullcontext()
-        with maxout, (_linear(_tf32x3_linear) if tf32x3 else contextlib.nullcontext()):
-            if self.kind in ('greedy', 'leave_one_out'):
-                _, lp = co.sample(fam, fc, att, reg, sample_method='sample', sample_n=2 if rows is not None else SPI, forced_tokens=words)
-            else:
-                lp = co.forward_teacher(fam, fc, att, words.view(fc.shape[0], -1, words.shape[1]), reg)
+        sampled = self.kind in ('greedy', 'leave_one_out')
+        if self.family == 'transformer' and sampled:
+            lp = co.forward_teacher(fam, fc, att, torch.cat([torch.zeros_like(words[:, :1]), words[:, :-1]], 1), reg, pad_keys_masked=False)
+            return lp * torch.cat([torch.ones_like(words[:, :1]), (words[:, :-1] > 0).long()], 1).unsqueeze(2).to(dt)
+        if sampled:
+            return co.sample(fam, fc, att, reg, sample_method='sample', sample_n=2 if rows is not None else SPI, forced_tokens=words)[1]
+        return co.forward_teacher(fam, fc, att, words.view(fc.shape[0], -1, words.shape[1]), reg)
+
+    def oracle(self, dt, rows=None, route=None, flip=None, record=None, tf32x3=False):
+        """(loss, log-probs, gradients) of the step in dtype dt.  ``record`` collects Att2in2's maxout a - b, or the Transformer's ReLU
+        inputs (att_embed's, then each feed-forward layer's)."""
+        W = {k: v.detach().to(dt, copy=True).requires_grad_(not k.endswith('.pe')) for k, v in self.W.items()}       # pe: a buffer
+        record = [] if record is None else record
+        hooks = contextlib.nullcontext()
+        if self.family == 'att2in2':
+            hooks = _routed_maxout(record, route, flip)
+        elif self.family == 'transformer':
+            hooks = ffn_relu_inputs(lambda pre, Wd, a: record.append(a.detach().reshape(-1, a.shape[-1])) or a)
+        with hooks, (_linear(_tf32x3_linear) if tf32x3 else contextlib.nullcontext()):
+            if self.family == 'transformer':
+                record.append(co.linear(self.att.to(dt).reshape(-1, self.att.shape[-1]), W['att_embed.0.weight'], W['att_embed.0.bias']).detach())
+            lp = self._forward(W, dt, rows)
         if rows is not None:
             lp = lp[:1]
         loss = self._objective(lp, rows, dt)
         loss.backward()
-        return float(loss), lp.detach(), {k: v.grad for k, v in W.items()}
+        return float(loss), lp.detach(), {k: v.grad for k, v in W.items() if v.requires_grad}
 
     def picked(self, lp):
         if self.kind in ('greedy', 'leave_one_out'):
@@ -331,6 +371,9 @@ class Case:
     def relu_kinks(self):
         """{parameter name: bool mask of the entries kept}: rows j of a ReLU layer's weight (and entry j of its bias) whose input lies within
         KINK_MARGIN x RMS of zero for some valid region (or image), in float64.  The fp32 pre-activations must sit well inside the margin."""
+        if self.family == 'transformer':            # its ReLUs are cleared by construction (reference())
+            self.kink_rows = {}
+            return {}, 0
         W = _weights(self.family)
         layers = [('att_embed.0', self.att)] + ([('fc_embed.0', self.fc.unsqueeze(1))] if self.family == 'updown' else [])
         keep, left_out, self.kink_rows = {}, 0, {}
@@ -351,15 +394,24 @@ class Case:
 
     def reference(self):
         t0 = time.time()
+        if self.family == 'transformer':
+            self.W, self.shifted, self.largest_shift = clear_relu_kinks(_weights(self.family), self.att, lambda W: self._forward(W, torch.float64),
+                                                                        TFM_MARGIN)
         rec64, rec32 = [], []
         loss64, lp64, g64 = self.oracle(torch.float64, record=rec64)
-        route = [d > 0 for d in rec64] if rec64 else None
+        route = [d > 0 for d in rec64] if rec64 and self.family == 'att2in2' else None
         loss32, lp32, g32 = self.oracle(torch.float32, route=route, record=rec32)
         self.ref = dict(loss64=loss64, loss32=loss32, picked64=self.picked(lp64), picked32=self.picked(lp32).double(), g64=g64, g32=g32)
         self.ref['l1'] = self._loss_l1(lp64)
         self.keep, self.left_out = self.relu_kinks()
         self.maxout = []
-        if rec64:
+        if self.family == 'transformer':
+            self.relu64 = rec64
+            rms = [float(a.pow(2).mean().sqrt()) for a in rec64]
+            clear = min(float(a.abs().min()) / r for a, r in zip(rec64, rms))
+            assert clear >= TFM_MARGIN, clear                  # every float64 ReLU input lies at least the margin from its kink
+            self.relu_err = {'fp32 oracle': self._relu_err(rec32)}
+        elif rec64:
             d = torch.stack(rec64)                                   # [steps, N, H]
             rms = float(d.pow(2).mean().sqrt())
             err32 = float((torch.stack(rec32).double() - d).abs().max())
@@ -372,9 +424,16 @@ class Case:
         """The calibrating oracle of tc_f16x3: the fp32 oracle with every Linear's forward and input gradient as gemm_tf32 computes them,
         following float64's maxout routing."""
         if 'g3' not in self.ref:
-            loss3, lp3, g3 = self.oracle(torch.float32, route=getattr(self, 'route', None), tf32x3=True)
+            rec3 = []
+            loss3, lp3, g3 = self.oracle(torch.float32, route=getattr(self, 'route', None), record=rec3, tf32x3=True)
             self.ref.update(loss3=loss3, picked3=self.picked(lp3).double(), g3=g3)
+            if self.family == 'transformer':
+                self.relu_err['3xTF32 oracle'] = self._relu_err(rec3)
         return self.ref['loss3'], self.ref['picked3'], self.ref['g3']
+
+    def _relu_err(self, rec):
+        """The largest distance of an oracle's ReLU inputs from float64's, as a fraction of each layer's RMS."""
+        return max(float((a.double() - a64).abs().max() / a64.pow(2).mean().sqrt()) for a, a64 in zip(rec, self.relu64))
 
     def _loss_l1(self, lp64):
         """(number of summed terms, sum of their magnitudes) of the step's loss."""
@@ -452,25 +511,37 @@ def _masks_fn(family):
         c, steps = case.c, case.steps
         if family == 'aoa':
             return aoa_masks(b200, SEED, case.B, case.Rc, case.N, steps, c['E'], c['H'], HEADS, *RATES['aoa'])
+        if family == 'transformer':
+            return tfm_masks(b200, SEED, case.B, case.Rc, case.N, steps, T, c['E'], c['H'], HEADS, c['A'], *RATES['transformer'])
         fn = dropout_masks if family == 'updown' else att2in2_masks
         return fn(b200, SEED, RATES[family], case.B, case.Rc, case.N, steps, c['E'], c['H'])
     return make
 
 
 def _check_masks(family, drop):
-    rates = RATES[family] if family == 'aoa' else (RATES[family],) * 4
+    if family == 'transformer':         # drop_prob_lm at att_embed, the Transformer's own rate at every other site
+        rates = {k: RATES[family][0] if k == 'att_embed' else RATES[family][1] for k in drop}
+    else:
+        rates = RATES[family] if family == 'aoa' else (RATES[family],) * 4
+        rates = {k: rates[1] if k.startswith('ref_p') or k == 'p' else rates[2] if k.startswith('ref_aoa') else rates[3] if k.startswith('ref_sub')
+                 else rates[0] for k in drop}
     for k, m in drop.items():
-        p = rates[1] if k.startswith('ref_p') or k == 'p' else rates[2] if k.startswith('ref_aoa') else rates[3] if k.startswith('ref_sub') else rates[0]
+        p = rates[k]
         assert abs(float((m > 0).double().mean()) - (1 - p)) < 0.02, (k, p)
 
 
 def _run_engine(family, mode, case):
     model = _model(family, mode, autograd=case.kind == 'autograd')
+    if family == 'transformer':
+        model.load_state_dict(case.W, strict=True)            # this case's weights, off the ReLU kinks
     fc, att = case.fc.cuda(), case.att.cuda()
     reg = None if case.regions is None else case.regions.cuda()
     if family == 'aoa':
         p = RATES['aoa'] if case.dropout else (0.0,) * 4
         rates = dict(drop_prob=p[0], drop_attn=p[1], drop_aoa=p[2], drop_sublayer=p[3], ctx_drop=1)
+    elif family == 'transformer':
+        p = RATES['transformer'] if case.dropout else (0.0, 0.0)
+        rates = dict(drop_prob=p[0], dropout=p[1])
     else:
         rates = dict(drop_prob=RATES[family] if case.dropout else 0.0)
     name_of = {id(p): k for k, p in model.state_dict(keep_vars=True).items()}
@@ -520,6 +591,13 @@ def _compare(family, mode, case):
     print('%s float64 reference %.1f s; ReLU units left out per layer %s, %d ambiguous maxout units' % (label, case.ref_seconds, case.kink_rows,
                                                                                                        len(case.maxout)))
     assert all(v <= 0.15 * case.c["H"] for v in case.kink_rows.values()), case.kink_rows        # some rows of the layer, not the layer
+    if family == 'transformer':
+        print('%s ReLU units shifted per layer %s; largest shift %.2e x RMS' % (label, case.shifted, case.largest_shift))
+        err = case.relu_err[oname]
+        print('%s ReLU inputs clear of their kinks by %.1e x RMS; %s error there %.2e x RMS (5x = %.2f of the margin)' % (
+            label, TFM_MARGIN, oname, err, 5 * err / TFM_MARGIN))
+        assert 5 * err < TFM_MARGIN, (oname, err)
+        assert len(got['grads']) == 261, len(got['grads'])             # every parameter (pe is a buffer)
     # scalars: loss (not for the autograd case, whose objective is a sum over every log-prob), picked log-probs, reward
     if 'loss' in got:
         n, l1 = ref['l1']
@@ -595,7 +673,24 @@ def test_aoa_step_f64(mode, kind, smoothing, dropout):
     _run('aoa', mode, kind, smoothing, dropout, 10)
 
 
-@pytest.mark.parametrize('family,mode', [(f, m) for f in ('updown', 'att2in2', 'aoa') for m in MODES if (f, m) != ('att2in2', 'tc_f16x3')])
+@pytest.mark.parametrize('dropout', [False, True])
+@pytest.mark.parametrize('kind,smoothing', STEPS)
+@pytest.mark.parametrize('mode', MODES)
+def test_transformer_step_f64(mode, kind, smoothing, dropout):
+    _run('transformer', mode, kind, smoothing, dropout, 10)
+
+
+@pytest.mark.slow
+@pytest.mark.parametrize('kind,smoothing', [('greedy', 0.0), ('xe', 0.1)])
+@pytest.mark.parametrize('mode', MODES)
+def test_transformer_step_f64_rows(mode, kind, smoothing):
+    """160 rows per step: in tc_f16x3 the per-position GEMMs of the sampled pass run gemm_tf32's swapped tile of width 256, and the
+    batched backward runs over 160 x 21 = 3360 rows."""
+    _run('transformer', mode, kind, smoothing, True, 32)
+
+
+@pytest.mark.parametrize('family,mode', [(f, m) for f in ('updown', 'att2in2', 'aoa', 'transformer') for m in MODES
+                                         if (f, m) != ('att2in2', 'tc_f16x3')])
 def test_autograd_teacher_f64(family, mode):
     """model.autograd: teacher-forced log-probs under grad and the backward of a seeded upstream gradient (logsoftmax_vjp_kernel<4>:
     V + 1 = 9488 is a multiple of 4)."""
