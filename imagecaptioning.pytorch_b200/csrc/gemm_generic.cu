@@ -45,6 +45,13 @@ __global__ void __launch_bounds__(256) gemm_generic_kernel(int M, int N, int K, 
             Bs[kb][nn] = w;
         }
         __syncthreads();
+        // each K-tile is summed on its own and then added to the running total: a weight gradient's K ~ 1000 rows would otherwise run
+        // through one fp32 accumulator whose rounding grows with the running sum at every step (K / GK additions to it instead of K)
+        float part[4][4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) part[i][j] = 0.f;
 #pragma unroll
         for (int k = 0; k < GK; ++k) {
             float a[4], b[4];
@@ -55,8 +62,12 @@ __global__ void __launch_bounds__(256) gemm_generic_kernel(int M, int N, int K, 
 #pragma unroll
             for (int i = 0; i < 4; ++i)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+                for (int j = 0; j < 4; ++j) part[i][j] = fmaf(a[i], b[j], part[i][j]);
         }
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] += part[i][j];
         __syncthreads();
     }
 #pragma unroll

@@ -283,5 +283,6 @@ def check_grads_f64(named, ref64, ref32, keep=None, zero_rel=1e-12, label='', fl
             failures.append((k, ratio, float(e.max()), scale))
     print('%s worst gradient err/bar %.3f (%s)' % (label, worst[0], worst[1]))
     assert not failures, failures
-    assert sum(float(v.abs().max()) > 1e-5 for v in ref64.values()) >= 15          # the comparison is not vacuous
+    # the comparison is not vacuous (NewFC has 9 tensors in all: every one of them)
+    assert sum(float(v.abs().max()) > 1e-5 for v in ref64.values()) >= min(15, len(ref64))
     return worst[0]

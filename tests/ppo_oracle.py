@@ -22,10 +22,16 @@ def old_policy_input(seq):
     return torch.cat([torch.zeros_like(seq[:, :1]), seq[:, :-1]], 1)
 
 
-def ppo_loss(lp, lo, seq, scores, n, cliprange=0.2, kl_coef=0.02, reduction='mean'):
+def ppo_loss(lp, lo, seq, scores, n, cliprange=0.2, kl_coef=0.02, reduction='mean', adv=None):
+    """``adv`` [N], when given, replaces the leave-one-out advantage of ``scores`` (which may then be None): the rows of a step taken apart
+    from their image's other samples."""
     mask = token_mask(seq).to(lp.dtype)
-    reward = scores.to(lp.dtype).reshape(-1, n)
-    adv = (reward - (reward.sum(1, keepdim=True) - reward) / (n - 1)).reshape(-1, 1)
+    if adv is None:
+        reward = scores.to(lp.dtype).reshape(-1, n)
+        adv = (reward - (reward.sum(1, keepdim=True) - reward) / (n - 1)).reshape(-1, 1)
+    else:
+        reward = None
+        adv = adv.to(lp.dtype).reshape(-1, 1)
     idx = seq.unsqueeze(2)
     ratio = torch.exp(lp.gather(2, idx).squeeze(2) - lo.gather(2, idx).squeeze(2))
     clamped = ratio.clamp(1.0 - cliprange, 1.0 + cliprange)
