@@ -322,6 +322,8 @@ SIGNATURES = {
     'capb200_self_cider': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'capb200_self_cider_div': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     'capb200_div_stats': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'capb200_coco_scores': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
     'capb200_decode_gemm': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(GemmEpilogue), c_void_p, c_int, c_void_p]),
     # autograd entry points: (engine, [fc,] att, B, R, opts, vjp, labels, label_cols, grads, logprobs, stream) /
     #                        (engine, [fc,] att, B, R, opts, vjp, grads, sample_seq, sample_logprobs, stream)

@@ -16,7 +16,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(PKG, 'build')
 LIB = os.path.join(PKG, 'libcapb200.so')
-SOURCES = ['gemm_tc.cu', 'gemm_simt.cu', 'pointwise.cu', 'vocab.cu', 'beam.cu', 'reward.cu', 'diversity.cu', 'transformer.cu', 'attn_tiled.cu', 'gemm_generic.cu', 'gemm_tf32.cu', 'scst_kernels.cu', 'aoa_train_kernels.cu', 'tfm_train_kernels.cu', 'optim.cu', 'engine.cu', 'tfm_engine.cu', 'aoa_engine.cu', 'ensemble.cu']
+SOURCES = ['gemm_tc.cu', 'gemm_simt.cu', 'pointwise.cu', 'vocab.cu', 'beam.cu', 'reward.cu', 'diversity.cu', 'coco_eval.cu', 'transformer.cu', 'attn_tiled.cu', 'gemm_generic.cu', 'gemm_tf32.cu', 'scst_kernels.cu', 'aoa_train_kernels.cu', 'tfm_train_kernels.cu', 'optim.cu', 'engine.cu', 'tfm_engine.cu', 'aoa_engine.cu', 'ensemble.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC']
 
 

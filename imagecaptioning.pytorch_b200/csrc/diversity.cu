@@ -366,7 +366,11 @@ int div_stats_launch(const long long* seqs, int n_images, int n, int T, int V1, 
     CAPB_CHECK_CUDA(cudaGetLastError());
     div_stats_kernel<<<n_images, DIV_THREADS, 0, stream>>>(seqs, n, T, out_div1, out_div2, out_bleu2, out_stats);
     CAPB_CHECK_CUDA(cudaGetLastError());
-    mutual_bleu_kernel<<<n, DIV_THREADS, 0, stream>>>(out_stats, n_images, n, out_mbleu);
+    return corpus_bleu_launch(out_stats, n_images, n, out_mbleu, stream);
+}
+
+int corpus_bleu_launch(const int* stats, int n_images, int n, double* out_bleu, cudaStream_t stream) {
+    mutual_bleu_kernel<<<n, DIV_THREADS, 0, stream>>>(stats, n_images, n, out_bleu);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

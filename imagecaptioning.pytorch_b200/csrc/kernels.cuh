@@ -341,6 +341,14 @@ int weighted_reward_launch(const CiderTable* t, double w_cider, double w_bleu, c
                            const int* refs, const int* ref_offsets, int L, double* scores, double* bleu, float* reward, long ld_reward, int reward_cols,
                            cudaStream_t stream);
 int weighted_reward_launches(double w_cider, double w_bleu, bool with_reward);     // kernels weighted_reward_launch issues
+// coco-caption's Cider() [S] and the per-caption Bleu(4) statistics [S, 6] (correct 1..4-grams, length, closest reference length) over the
+// words before each first 0; S / n_images captions per image, each image counted once in the document frequencies of the corpus table t
+int coco_cider_bleu_launch(const CiderTable* t, const long long* seqs, int S, int n_images, int T, const int* refs, const int* ref_offsets, int L,
+                           double* cider, int* bleu_stats, cudaStream_t stream);
+
+// ---- diversity.cu
+// corpus BLEU-1..4 of each round j < n (caption j of every image) from per-caption statistics [n_images, n, 6]: out_bleu[n, 4]
+int corpus_bleu_launch(const int* stats, int n_images, int n, double* out_bleu, cudaStream_t stream);
 int reward_criterion_fwd_launch(const float* logprobs, long ld_row, long ld_t, const long long* seq, const float* reward, int N, int T,
                                 float* loss_mean, float* loss_rows, float* mask_sum, cudaStream_t stream);
 int reward_criterion_bwd_launch(const long long* seq, const float* reward, int N, int T, const float* mask_sum, float upstream,

@@ -116,21 +116,25 @@ __global__ void corpus_clear_kernel(CiderSlot* __restrict__ slots, unsigned long
     slots[i].idf = 0.0;
 }
 
-// the tokens of reference row r up to and including its first 0, at most min(L, 256)
-__device__ __forceinline__ int ref_len(const int* __restrict__ refs, long r, int L) {
+// the tokens of reference row r up to and including its first 0 (`with_eos`) or before it, at most min(L, 256)
+__device__ __forceinline__ int ref_len(const int* __restrict__ refs, long r, int L, bool with_eos) {
     const int cols = L < CIDER_MAXL_LONG ? L : CIDER_MAXL_LONG;
     int len = 0;
-    for (int j = 0; j < cols; ++j) { ++len; if (refs[r * L + j] == 0) break; }
+    for (int j = 0; j < cols; ++j) {
+        if (refs[r * L + j] == 0) return with_eos ? len + 1 : len;
+        ++len;
+    }
     return len;
 }
 
 // One CTA per image: every distinct n-gram of the image's references (set() over all of them, ciderD_scorer.py:143-147) adds `mult` -- the
-// number of scored hypotheses (crefs entries) of the image -- to its document frequency.  Thread items are (reference, order, position); an
+// number of scored hypotheses (crefs entries) of the image -- to its document frequency.  References end as ref_len cuts them.  Thread items are (reference, order, position); an
 // item inserts when no earlier item of the image holds the same n-gram.  A slot is claimed by swapping its key[0] from -2 (empty) to -3
 // (being written); readers that meet -3 wait for the writer to publish key[0].  The occupied slots stay at most half the capacity (`used`),
 // so every probe sequence, here and in the scoring kernels' lookups, reaches an empty slot.
 __global__ void __launch_bounds__(256) corpus_insert_kernel(CiderSlot* __restrict__ slots, unsigned long long mask, unsigned int* used,
-                                                            const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L, double mult) {
+                                                            const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L, double mult,
+                                                            int with_eos) {
     const int img = blockIdx.x;
     const int r0 = ref_offsets[img], r1 = ref_offsets[img + 1];
     const int cols = L < CIDER_MAXL_LONG ? L : CIDER_MAXL_LONG;
@@ -138,12 +142,12 @@ __global__ void __launch_bounds__(256) corpus_insert_kernel(CiderSlot* __restric
     for (long it = threadIdx.x; it < items; it += blockDim.x) {
         const long r = r0 + it / (CIDER_N * cols);
         const int n = (int)((it / cols) % CIDER_N) + 1, p = (int)(it % cols);
-        const int len = ref_len(refs, r, L);
+        const int len = ref_len(refs, r, L, with_eos != 0);
         if (p + n > len) continue;
         const int* g = refs + r * L + p;
         bool first = true;
         for (long q = r0; q <= r && first; ++q) {
-            const int lq = q == r ? p + n - 1 : ref_len(refs, q, L);          // earlier positions of this row, every position of earlier rows
+            const int lq = q == r ? p + n - 1 : ref_len(refs, q, L, with_eos != 0);          // earlier positions of this row, every position of earlier rows
             for (int j = 0; j + n <= lq && first; ++j) first = !same_gram(g, refs + q * L + j, n);
         }
         if (!first) continue;
@@ -177,9 +181,10 @@ __global__ void corpus_finalise_kernel(CiderSlot* __restrict__ slots, unsigned l
 }
 
 // Builds the corpus table for one reward call over `hyps` scored hypotheses, `per_image` of them per image, and returns its log(ref_len) =
-// log(hyps) (ciderD_scorer.py:182-186); a pickle table is left alone and returns its own.
+// log(hyps) (ciderD_scorer.py:182-186); a pickle table is left alone and returns its own.  The reward keeps each reference's closing 0
+// (`with_eos`); coco-caption's Cider scores the words before it.
 int corpus_build_launch(const CiderTable* t, int B, int hyps, int per_image, const int* refs, const int* ref_offsets, int L, double* log_ref_len,
-                        cudaStream_t stream) {
+                        cudaStream_t stream, bool with_eos = true) {
     if (!t->corpus) { *log_ref_len = t->log_ref_len; return 0; }
     CAPB_REQUIRE(t->slots != nullptr, "corpus CIDEr-D table without reserved slots (capb200_cider_table_reserve)");
     *log_ref_len = log((double)hyps);
@@ -187,7 +192,7 @@ int corpus_build_launch(const CiderTable* t, int B, int hyps, int per_image, con
     const unsigned int grid = (unsigned int)((cap + 255) / 256);
     corpus_clear_kernel<<<grid, 256, 0, stream>>>(t->slots, cap, t->used);
     CAPB_CHECK_CUDA(cudaGetLastError());
-    corpus_insert_kernel<<<B, 256, 0, stream>>>(t->slots, t->mask, t->used, refs, ref_offsets, L, (double)per_image);
+    corpus_insert_kernel<<<B, 256, 0, stream>>>(t->slots, t->mask, t->used, refs, ref_offsets, L, (double)per_image, with_eos ? 1 : 0);
     CAPB_CHECK_CUDA(cudaGetLastError());
     corpus_finalise_kernel<<<grid, 256, 0, stream>>>(t->slots, cap, *log_ref_len);
     CAPB_CHECK_CUDA(cudaGetLastError());
@@ -234,12 +239,13 @@ __device__ void cider_vectorise(const CiderSlot* slots, unsigned long long mask,
     __syncthreads();
 }
 
-// one CTA per hypothesis: hyps 0..S-1 are the samples (image i / n), S..S+B-1 the greedy captions (image i - S)
+// one CTA per hypothesis: hyps 0..S-1 are the samples (image i / n), S..S+B-1 the greedy captions (image i - S).  Captions and references
+// keep their closing 0 when `with_eos` (array_to_str, the reward form), else stop before it (the words coco-caption's Cider scores).
 template <int MAXL>
 __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __restrict__ slots, unsigned long long mask, double log_ref_len,
                                                           const long long* __restrict__ sampled, int S, const long long* __restrict__ greedy, int B,
                                                           int T, const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L,
-                                                          double* __restrict__ scores) {
+                                                          double* __restrict__ scores, int with_eos) {
     __shared__ int h_tok[MAXL], r_tok[MAXL];
     __shared__ double h_w[CIDER_N * MAXL], r_w[CIDER_N * MAXL], contrib[CIDER_N * MAXL];
     __shared__ unsigned char h_valid[CIDER_N * MAXL], r_valid[CIDER_N * MAXL];
@@ -251,7 +257,12 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
     const long long* src = hyp < S ? sampled + (long)hyp * T : greedy + (long)(hyp - S) * T;
     if (threadIdx.x == 0) {
         int len = 0;
-        for (int i = 0; i < T && i < MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
+        for (int i = 0; i < T && i < MAXL; ++i) {
+            const int v = (int)src[i];
+            if (v == 0 && !with_eos) break;
+            h_tok[len++] = v;
+            if (v == 0) break;
+        }
         h_len = len;
     }
     __syncthreads();
@@ -262,7 +273,12 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
     for (int r = r0; r < r1; ++r) {
         if (threadIdx.x == 0) {
             int len = 0;
-            for (int i = 0; i < L && i < MAXL; ++i) { const int v = refs[(long)r * L + i]; r_tok[len++] = v; if (v == 0) break; }
+            for (int i = 0; i < L && i < MAXL; ++i) {
+                const int v = refs[(long)r * L + i];
+                if (v == 0 && !with_eos) break;
+                r_tok[len++] = v;
+                if (v == 0) break;
+            }
             r_len = len;
         }
         __syncthreads();
@@ -305,12 +321,14 @@ __global__ void __launch_bounds__(256) cider_score_kernel(const CiderSlot* __res
 // One CTA per hypothesis, laid out as cider_score_kernel; thread g owns the n-gram of order g / MAXL + 1 starting at position g % MAXL (4 x 256 =
 // 1024 threads in the long form: the CTA limit sets CAPB200_MAX_SEQ_LENGTH).  The image's
 // references are staged in shared memory BLEU_REF_CHUNK at a time.  An image without references scores 0 (the Python layer refuses it).
+// `with_eos` = 0 stops captions and references before their first 0 (the words coco-caption scores).  `scores` and `stats` may each be null;
+// stats[hyp] gets correct 1..4-grams, the hypothesis length and the closest reference length (the layout of diversity.cu's BLEU statistics).
 constexpr int BLEU_REF_CHUNK = 32;
 
 template <int MAXL>
 __global__ void __launch_bounds__(CIDER_N * MAXL) bleu_score_kernel(const long long* __restrict__ sampled, int S, const long long* __restrict__ greedy,
                                                                           int B, int T, const int* __restrict__ refs, const int* __restrict__ ref_offsets, int L,
-                                                                          double* __restrict__ scores) {
+                                                                          double* __restrict__ scores, int with_eos, int* __restrict__ stats) {
     __shared__ int h_tok[MAXL];
     __shared__ int r_tok[BLEU_REF_CHUNK][MAXL];
     __shared__ int r_len[BLEU_REF_CHUNK];
@@ -322,7 +340,12 @@ __global__ void __launch_bounds__(CIDER_N * MAXL) bleu_score_kernel(const long l
     const long long* src = hyp < S ? sampled + (long)hyp * T : greedy + (long)(hyp - S) * T;
     if (threadIdx.x == 0) {
         int len = 0;
-        for (int i = 0; i < T && i < MAXL; ++i) { const int v = (int)src[i]; h_tok[len++] = v; if (v == 0) break; }
+        for (int i = 0; i < T && i < MAXL; ++i) {
+            const int v = (int)src[i];
+            if (v == 0 && !with_eos) break;
+            h_tok[len++] = v;
+            if (v == 0) break;
+        }
         h_len = len;
     }
     if (threadIdx.x < CIDER_N) correct[threadIdx.x] = 0;
@@ -352,7 +375,10 @@ __global__ void __launch_bounds__(CIDER_N * MAXL) bleu_score_kernel(const long l
         __syncthreads();
         if (threadIdx.x < cnt) {
             int len = 0;
-            for (int j = 0; j < cols; ++j) { ++len; if (r_tok[threadIdx.x][j] == 0) break; }
+            for (int j = 0; j < cols; ++j) {
+                if (r_tok[threadIdx.x][j] == 0) { len += with_eos ? 1 : 0; break; }
+                ++len;
+            }
             r_len[threadIdx.x] = len;
         }
         __syncthreads();
@@ -384,7 +410,13 @@ __global__ void __launch_bounds__(CIDER_N * MAXL) bleu_score_kernel(const long l
             const double ratio = ((double)hl + 1e-15) / ((double)best_len + 1e-9);
             if (ratio < 1.0) s *= exp(1.0 - 1.0 / ratio);
         }
-        scores[hyp] = s;
+        if (scores) scores[hyp] = s;
+        if (stats) {
+            int* st = stats + (long)hyp * 6;
+            for (int k = 0; k < CIDER_N; ++k) st[k] = correct[k];
+            st[4] = hl;
+            st[5] = best_len;
+        }
     }
 }
 
@@ -482,11 +514,21 @@ int check_reward_shapes(int S, int B, int T, int L) {
 bool long_form(int T, int L) { return T > CIDER_MAXL || L > CIDER_MAXL; }
 
 void cider_score_launch(const CiderTable* t, double log_ref_len, const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs,
-                        const int* ref_offsets, int L, double* scores, int hyps, cudaStream_t stream) {
+                        const int* ref_offsets, int L, double* scores, int hyps, cudaStream_t stream, bool with_eos = true) {
+    const int eos = with_eos ? 1 : 0;
     if (long_form(T, L))
-        cider_score_kernel<CIDER_MAXL_LONG><<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+        cider_score_kernel<CIDER_MAXL_LONG><<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores, eos);
     else
-        cider_score_kernel<CIDER_MAXL><<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+        cider_score_kernel<CIDER_MAXL><<<hyps, 256, 0, stream>>>(t->slots, t->mask, log_ref_len, sampled, S, greedy, B, T, refs, ref_offsets, L, scores, eos);
+}
+
+void bleu_score_launch(const long long* sampled, int S, const long long* greedy, int B, int T, const int* refs, const int* ref_offsets, int L, double* scores,
+                       int hyps, cudaStream_t stream, bool with_eos = true, int* stats = nullptr) {
+    const int eos = with_eos ? 1 : 0;
+    if (long_form(T, L))
+        bleu_score_kernel<CIDER_MAXL_LONG><<<hyps, CIDER_N * CIDER_MAXL_LONG, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores, eos, stats);
+    else
+        bleu_score_kernel<CIDER_MAXL><<<hyps, CIDER_N * CIDER_MAXL, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores, eos, stats);
 }
 
 }  // namespace
@@ -510,10 +552,24 @@ int bleu_scores_launch(const long long* sampled, int S, const long long* greedy,
     if (check_reward_shapes(S, B, T, L)) return 1;
     const int hyps = greedy != nullptr ? S + B : S;
     if (hyps == 0) return 0;
-    if (long_form(T, L))
-        bleu_score_kernel<CIDER_MAXL_LONG><<<hyps, CIDER_N * CIDER_MAXL_LONG, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
-    else
-        bleu_score_kernel<CIDER_MAXL><<<hyps, CIDER_N * CIDER_MAXL, 0, stream>>>(sampled, S, greedy, B, T, refs, ref_offsets, L, scores);
+    bleu_score_launch(sampled, S, greedy, B, T, refs, ref_offsets, L, scores, hyps, stream);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// coco-caption's Cider() and the Bleu(4) statistics over the words of seqs[S, T] (the ids before the first 0), per_image = S / n_images
+// consecutive captions per image, against references cut the same way.  Cider's document frequencies count each image once whatever
+// per_image is, with ref_len = log(n_images) (cider_scorer.py:96-107,165: one Cider call scores one caption per image).  `t` is a corpus
+// table reserved for the references.
+int coco_cider_bleu_launch(const CiderTable* t, const long long* seqs, int S, int n_images, int T, const int* refs, const int* ref_offsets, int L,
+                           double* cider, int* bleu_stats, cudaStream_t stream) {
+    CAPB_REQUIRE(t != nullptr && t->corpus, "the caption metrics build their document frequencies in a corpus CIDEr table");
+    if (check_reward_shapes(S, n_images, T, L)) return 1;
+    double log_ref_len = 0.0;
+    if (corpus_build_launch(t, n_images, n_images, 1, refs, ref_offsets, L, &log_ref_len, stream, false)) return 1;
+    cider_score_launch(t, log_ref_len, seqs, S, nullptr, n_images, T, refs, ref_offsets, L, cider, S, stream, false);
+    CAPB_CHECK_CUDA(cudaGetLastError());
+    bleu_score_launch(seqs, S, nullptr, n_images, T, refs, ref_offsets, L, nullptr, S, stream, false, bleu_stats);
     CAPB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -1,8 +1,10 @@
-"""Device-side mirror of the diversity half of captioning/utils/eval_multi.py: the scores the reference's projects/Diversity
-``only_eval_test_n_*.sh`` scripts compute for the caption sets ``eval_split_n`` generates.
+"""Device-side mirror of captioning/utils/eval_multi.py: the scores the reference's projects/Diversity ``only_eval_test_n_*.sh`` scripts
+compute for the caption sets ``eval_split_n`` generates, and coco-caption's language metrics that eval_utils.language_eval reports.
 
     div_stats(seqs, n)           eval_div_stats      eval_multi.py:121-175   Div-1, Div-2, gDiv-1, mutual BLEU-1..4
     self_cider(seqs, n, table)   eval_self_cider     eval_multi.py:177-217   self-CIDEr matrices and their eigenvalue diversity
+    coco_scores(seq, gts)        COCOEvalCap         eval_utils.py:84-90     BLEU-1..4, ROUGE-L and CIDEr (no METEOR, SPICE or WMD)
+    eval_oracle(seqs, gts, n)    eval_oracle         eval_multi.py:71-119    oracle_ / avg_ BLEU-1..4, ROUGE-L and CIDEr of caption sets
 
 ``seqs`` are id rows, n consecutive rows per image (2 <= n <= 32, at most 64 tokens), on a CUDA device -- what ``eval_split_n`` returns.
 A caption is its ids before the first 0, the words ``decode_sequence`` would print.  The reference runs coco-caption's PTB tokenizer over
@@ -17,6 +19,11 @@ once per image whose references contain it) and ref_len = the number of images:
 
 where ``refs_per_image[i]`` is image i's reference id rows.  Any other CiderDTable (a pickle's, through ``rewards.init_scorer``) works too;
 a corpus table has no ref_len and is refused.
+
+``coco_scores`` and ``eval_oracle`` (csrc/coco_eval.cu) return exactly what coco-caption's Bleu(4), Rouge() and Cider() return when each
+caption is the string of its ids before the first 0 joined by single spaces, against its image's references -- the loader's ``gts`` rows,
+cut the same way.  These are NOT the official COCO numbers: coco-caption's PTB tokenizer never sees the annotation text, and the
+references are the dataset's label rows, which prepro truncated at max_length and where rare words are UNK.
 """
 from __future__ import annotations
 
@@ -65,6 +72,104 @@ def _device_ids(seqs) -> torch.Tensor:
     if seqs.device.type != 'cuda':
         raise RuntimeError('capb200: the diversity kernels run on CUDA tensors only')
     return seqs.detach().to(torch.long).contiguous()
+
+
+COCO_METRICS = ('Bleu_1', 'Bleu_2', 'Bleu_3', 'Bleu_4', 'ROUGE_L', 'CIDEr')
+_coco_table: Optional[rewards.CorpusCiderDTable] = None
+
+
+def _coco_device(seq: torch.Tensor, gts: Sequence, per_image: int):
+    """(bleu [S, 4], corpus bleu [per_image, 4], rouge [S], cider [S]) as host float64 arrays from one capb200_coco_scores call and one
+    device-to-host transfer."""
+    global _coco_table
+    if not isinstance(seq, torch.Tensor) or seq.dim() != 2:
+        raise ValueError('seq must be a 2-D tensor of caption ids')
+    if seq.device.type != 'cuda':
+        raise RuntimeError('capb200: the caption metrics run on CUDA tensors only')
+    rows, T = (int(x) for x in seq.shape)
+    n = int(per_image)
+    if n < 1 or rows % n:
+        raise ValueError('%d captions do not split into %s per image' % (rows, per_image))
+    B = rows // n
+    if len(gts) != B:
+        raise ValueError('%d reference sets for %d images' % (len(gts), B))
+    if B == 0:
+        raise ValueError('no images to score')
+    if any(int(np.asarray(g).shape[0]) == 0 for g in gts):
+        raise ValueError('every image needs at least one reference (coco-caption asserts it)')
+    ids = seq.detach().to(torch.long).contiguous()
+    if _coco_table is None:
+        _coco_table = rewards.CorpusCiderDTable()
+    refs, offsets, L = rewards.pack_references(gts, ids.device)
+    # one float64 buffer: bleu [S, 4], corpus bleu [n, 4], rouge [S], cider [S], then the int32 BLEU statistics [S, 6]
+    o_cb, o_r = 4 * rows, 4 * rows + 4 * n
+    o_c, o_st = o_r + rows, o_r + 2 * rows
+    buf = torch.empty(o_st + 3 * rows, dtype=torch.float64, device=ids.device)
+    p = _lib.ptr(buf)
+    _lib.check(_lib.load().capb200_coco_scores(_coco_table._h, _lib.ptr(ids), B, n, T, _lib.ptr(refs), _lib.ptr(offsets), L, p, p + 8 * o_cb,
+                                               p + 8 * o_r, p + 8 * o_c, p + 8 * o_st, _lib.current_stream()), 'coco_scores')
+    host = buf[:o_st].cpu().numpy()
+    return host[:o_cb].reshape(rows, 4), host[o_cb:o_r].reshape(n, 4), host[o_r:o_c], host[o_c:o_st]
+
+
+def _image_keys(B: int, image_ids: Optional[Sequence]):
+    if image_ids is None:
+        return list(range(B))
+    if len(image_ids) != B:
+        raise ValueError('%d image ids for %d images' % (len(image_ids), B))
+    return list(image_ids)
+
+
+def coco_scores(seq: torch.Tensor, gts: Sequence, per_image: int = 1, image_ids: Optional[Sequence] = None):
+    """COCOEvalCap's ``eval`` and ``imgToEval`` for BLEU-1..4, ROUGE-L and CIDEr (see the module docstring for what is scored):
+        {'overall': {'Bleu_1', .., 'Bleu_4', 'ROUGE_L', 'CIDEr'}, 'imgToEval': {image_id: {'image_id', 'Bleu_1', .., 'CIDEr'}}}
+    ``seq`` [n_images * per_image, T] on a CUDA device (RuntimeError otherwise), ``gts[i]`` image i's 0-padded reference rows [n_refs, L]
+    (the loader's data['gts']); an image without references raises ValueError.  T and L are at most 256.  With per_image > 1 each of
+    the per_image rounds (caption j of every image) is scored as its own COCOEvalCap run, as eval_oracle does: 'overall' is then the list
+    of the rounds' dicts and every imgToEval entry the list of its captions' dicts.  Image ids default to 0..B-1."""
+    bleu, corpus, rouge, cider = _coco_device(seq, gts, per_image)
+    n = int(per_image)
+    B = bleu.shape[0] // n
+    keys = _image_keys(B, image_ids)
+    rounds = []
+    for j in range(n):
+        overall = {'Bleu_%d' % (k + 1): float(corpus[j, k]) for k in range(4)}
+        overall['ROUGE_L'] = float(np.mean(rouge[j::n]))
+        overall['CIDEr'] = float(np.mean(cider[j::n]))
+        rounds.append(overall)
+    per_cap = []
+    for i in range(B * n):
+        d = {'image_id': keys[i // n]}
+        d.update({'Bleu_%d' % (k + 1): float(bleu[i, k]) for k in range(4)})
+        d.update({'ROUGE_L': float(rouge[i]), 'CIDEr': float(cider[i])})
+        per_cap.append(d)
+    if n == 1:
+        return {'overall': rounds[0], 'imgToEval': {keys[i]: per_cap[i] for i in range(B)}}
+    return {'overall': rounds, 'imgToEval': {keys[i]: per_cap[i * n:(i + 1) * n] for i in range(B)}}
+
+
+def eval_oracle(seqs: torch.Tensor, gts: Sequence, n: int, image_ids: Optional[Sequence] = None):
+    """eval_oracle (eval_multi.py:71-119) for BLEU-1..4, ROUGE-L and CIDEr, as its ``out`` dict:
+        {'overall': {'oracle_Bleu_1', 'avg_Bleu_1', .., 'oracle_CIDEr', 'avg_CIDEr'}, 'ImgToEval': {image_id: {same keys}}}
+    Round j scores caption j of every image against the image's references (coco_scores with per_image = n); oracle_<m> is an image's best
+    caption under metric m, avg_<m> the mean over its captions, and 'overall' the mean of both over the images.  ``seqs`` holds n
+    consecutive rows per image, in image order (what eval_split_n returns)."""
+    bleu, _, rouge, cider = _coco_device(seqs, gts, n)
+    n = int(n)
+    B = bleu.shape[0] // n
+    keys = _image_keys(B, image_ids)
+    per_metric = [bleu[:, k] for k in range(4)] + [rouge, cider]
+    img = {}
+    for i, key in enumerate(keys):
+        d = {}
+        for name, vals in zip(COCO_METRICS, per_metric):
+            caps = vals[i * n:(i + 1) * n].tolist()
+            d['oracle_' + name] = max(caps)
+            d['avg_' + name] = sum(caps) / len(caps)
+        img[key] = d
+    first = next(iter(img.values()))
+    overall = {m: np.array([v[m] for v in img.values()]).mean() for m in first}
+    return {'overall': overall, 'ImgToEval': img}
 
 
 def div_stats(seqs: torch.Tensor, n: int, vocab_size: Optional[int] = None, image_ids: Optional[Sequence] = None):

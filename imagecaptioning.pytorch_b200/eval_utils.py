@@ -13,9 +13,16 @@ and its ``predictions`` entries (``image_id``, ``caption``, ``perplexity``, ``en
   * perplexity / entropy are reduced on the device for the whole batch and fetched with ONE device -> host copy,
   * captions are detokenised by ``utils.decode_sequence`` (one copy per batch).
 
-Language evaluation (``lang_eval=1``: the Java METEOR / SPICE tool chain of coco-caption) is outside the hot path (SURVEY.md section 2);
-pass ``eval_kwargs['language_eval']`` = a callable ``(dataset, predictions, n_predictions, eval_kwargs, split) -> stats`` to plug the
-reference's ``eval_utils.language_eval`` in.
+Language evaluation:
+  * ``eval_kwargs['language_eval'] = 'device'`` scores the split on the GPU after the loop (eval_multi.coco_scores, csrc/coco_eval.cu):
+    BLEU-1..4, ROUGE-L and CIDEr of every kept caption against its image's ``data['gts']`` rows, plus perplexity, entropy and
+    bad_count_rate, under the key names of the reference's language_eval (eval_utils.py:89-121).  With sample_n > 1 the caption sets add
+    eval_multi.div_stats' and eval_multi.self_cider's statistics and, with ``eval_kwargs['eval_oracle']``, eval_multi.eval_oracle's.  The
+    scores are coco-caption's Bleu(4) / Rouge() / Cider() over the ids joined by spaces, not the official COCO numbers: there is no PTB
+    tokenization of the annotation text and the references are the label rows (truncated at max_length, rare words UNK).  METEOR, SPICE,
+    WMD, AllSPICE, novel_sentences and vocab_size are absent.
+  * ``language_eval = 1`` means the reference's Java tool chain (METEOR / SPICE), which is not run here and raises; pass a callable
+    ``(dataset, predictions, n_predictions, eval_kwargs, split) -> stats`` to plug the reference's ``eval_utils.language_eval`` in.
 """
 from __future__ import annotations
 
@@ -141,6 +148,36 @@ def eval_split_n(model, n_predictions, input_data, eval_kwargs: Dict[str, Any] =
     return seq
 
 
+def _pad_cat(chunks):
+    T = max(int(c.shape[1]) for c in chunks)
+    return torch.cat([torch.nn.functional.pad(c, (0, T - int(c.shape[1]))) for c in chunks])
+
+
+def count_bad(sen: str) -> int:
+    """eval_utils.py:31-36: 1 when the caption's last word is a bad ending."""
+    from .models import BAD_ENDINGS
+    return 1 if sen.split(' ')[-1] in BAD_ENDINGS else 0
+
+
+def device_language_eval(predictions, seqs, gts, n_seqs, n_gts, sample_n: int, eval_kwargs: Dict[str, Any]):
+    """lang_stats of ``language_eval = 'device'``: the key names of eval_utils.py:89-121 (language_eval) for the metrics computed on the
+    device.  ``seqs`` / ``gts``: the id chunks and reference sets of ``predictions``, in their order; ``n_seqs`` / ``n_gts``: the caption
+    sets eval_split_n returned and their images' references, in image order."""
+    from . import eval_multi, rewards
+    out = dict(eval_multi.coco_scores(_pad_cat(seqs), gts, image_ids=[p['image_id'] for p in predictions])['overall'])
+    out['perplexity'] = sum([p['perplexity'] for p in predictions]) / len(predictions)
+    out['entropy'] = sum([p['entropy'] for p in predictions]) / len(predictions)
+    if n_seqs:
+        seq_n = _pad_cat(n_seqs)
+        out.update(eval_multi.div_stats(seq_n, sample_n)['overall'])
+        if eval_kwargs.get('eval_oracle', 0):
+            out.update(eval_multi.eval_oracle(seq_n, n_gts, sample_n)['overall'])
+        table = rewards.CiderDTable(*eval_multi.document_frequency(n_gts))
+        out.update(eval_multi.self_cider(seq_n, sample_n, table)['overall'])
+    out['bad_count_rate'] = sum([count_bad(p['caption']) for p in predictions]) / float(len(predictions))
+    return out
+
+
 def eval_split(model, crit, loader, eval_kwargs: Dict[str, Any] = {}):
     """Contract of captioning/utils/eval_utils.py:129-213.  ``crit`` is the XE criterion (LanguageModelCriterion / LabelSmoothing)."""
     verbose = eval_kwargs.get('verbose', True)
@@ -159,6 +196,8 @@ def eval_split(model, crit, loader, eval_kwargs: Dict[str, Any] = {}):
     loader.reset_iterator(split)
     n, loss, loss_sum, loss_evals = 0, 0.0, 0.0, 1e-8
     predictions, n_predictions = [], []
+    on_device = isinstance(lang_eval, str) and lang_eval == 'device'
+    lang_seqs, lang_gts, lang_n_seqs, lang_n_gts = [], [], [], []      # what language_eval = 'device' scores after the loop
     for data in PrefetchLoader(loader, split, device):
         n += len(data['infos'])
         fc_feats, att_feats, labels, masks, att_masks = (data[k] for k in _TENSOR_KEYS)
@@ -196,7 +235,10 @@ def eval_split(model, crit, loader, eval_kwargs: Dict[str, Any] = {}):
             if verbose:
                 print('image %s: %s' % (entry['image_id'], entry['caption']))
         if sample_n > 1:
-            eval_split_n(model, n_predictions, [fc_feats, att_feats, att_masks, data], eval_kwargs)
+            seq_n = eval_split_n(model, n_predictions, [fc_feats, att_feats, att_masks, data], eval_kwargs)
+            if on_device:
+                lang_n_seqs.append(seq_n)
+                lang_n_gts.extend(data['gts'])
         ix1 = data['bounds']['it_max']
         if num_images != -1:
             ix1 = min(ix1, num_images)
@@ -204,6 +246,16 @@ def eval_split(model, crit, loader, eval_kwargs: Dict[str, Any] = {}):
             num_images = ix1
         for _ in range(n - ix1):
             predictions.pop()
+        if on_device:                   # the captions and references of the predictions kept, trimmed as predictions was
+            lang_seqs.append(seq)
+            lang_gts.extend(data['gts'])
+            del lang_gts[len(predictions):]
+            extra = sum(int(c.shape[0]) for c in lang_seqs) - len(predictions)
+            while extra > 0:
+                last = lang_seqs.pop()
+                if int(last.shape[0]) > extra:
+                    lang_seqs.append(last[:int(last.shape[0]) - extra])
+                extra -= min(extra, int(last.shape[0]))
         if verbose:
             print('evaluating validation preformance... %d/%d (%f)' % (n, ix1, loss))
         if num_images >= 0 and n >= num_images:
@@ -217,7 +269,10 @@ def eval_split(model, crit, loader, eval_kwargs: Dict[str, Any] = {}):
         torch.save((predictions, n_predictions), os.path.join('eval_results/', '.saved_pred_' + eval_kwargs['id'] + '_' + split + '.pth'))
     if callable(lang_eval):
         lang_stats = lang_eval(dataset, predictions, n_predictions, eval_kwargs, split)
+    elif on_device:
+        lang_stats = device_language_eval(predictions, lang_seqs, lang_gts, lang_n_seqs, lang_n_gts, sample_n, eval_kwargs)
     elif lang_eval == 1:
-        raise NotImplementedError("language evaluation runs the reference's Java tool chain: pass eval_kwargs['language_eval'] = eval_utils.language_eval")
+        raise NotImplementedError("language_eval = 1 runs the reference's Java tool chain (METEOR, SPICE): pass eval_kwargs['language_eval'] = "
+                                  "'device' for BLEU, ROUGE-L and CIDEr on the GPU, or eval_utils.language_eval")
     model.train()
     return loss_sum / loss_evals, predictions, lang_stats

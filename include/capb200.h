@@ -454,6 +454,24 @@ int capb200_div_stats(const long long* seqs, int n_images, int n, int T, int V1,
                       double* out_mbleu, double* out_bleu2, int* out_bleu_stats, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Language evaluation: coco-caption's Bleu(4), Rouge() and Cider() (coco-caption/pycocoevalcap) over token ids
+ * seqs[n_images * per_image, T] int64 device: per_image consecutive captions per image; a caption is its ids before the first 0, scored
+ * as the string of those ids joined by single spaces.  refs / ref_offsets / L as in capb200_self_critical_reward, each reference cut before
+ * its first 0.  T and L between 1 and CAPB200_MAX_SEQ_LENGTH.  These are not the official COCO numbers: there is no PTB tokenization of the
+ * annotation text, and the references are the dataset's label rows (truncated at max_length, rare words UNK).
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* Outputs, float64 device memory:
+ *   out_bleu[S, 4]                  each caption's per-sentence BLEU-1..4 (Bleu(4) bleu_list, closest reference length)
+ *   out_corpus_bleu[per_image, 4]   corpus BLEU-1..4 of round j: caption j of every image (Bleu(4)'s overall score of that round)
+ *   out_rouge[S]                    ROUGE-L (beta = 1.2; an empty caption is one empty word, as str.split(" ") makes it)
+ *   out_cider[S]                    CIDEr: document frequencies count each image once, ref_len = log(n_images), whatever per_image is
+ * ws_stats[S, 6] int32 device: scratch (correct 1..4-grams, length and closest reference length of each caption).  `t` is a corpus table
+ * (capb200_cider_corpus_table_create), reserved here for the references; only its first call at a given size allocates.  The B + 1 offsets
+ * are read back (the stream is synchronised) and an image without references is refused before any launch. */
+int capb200_coco_scores(capb200_cider_table* t, const long long* seqs, int n_images, int per_image, int T, const int* refs, const int* ref_offsets,
+                        int L, double* out_bleu, double* out_corpus_bleu, double* out_rouge, double* out_cider, int* ws_stats, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * One self-critical training step of the UpDown model (LossWrapper.forward with sc_flag, loss_wrapper.py:56-73, plus the
  * loss.backward() of tools/train.py:189): eval-mode greedy baseline, train-mode multinomial samples (dropout on, AttModel.py:74-88,
  * :637), self-critical reward (CIDEr-D, or weighted CIDEr-D + BLEU-4 with opts->reward_weights), RewardCriterion, then back-propagation
